@@ -62,6 +62,18 @@ void rb_launch_count_reset(void);
 /* Profiling aid: when buf != NULL, rb_update_step records 8 globaltimer timestamps per CTA of each of its
  * tensor-core convs into buf (int64[n_convs][4096][8], launch order); NULL switches it off. */
 int rb_debug_set_buffer(void* buf);
+/* Test hook: every later tensor-core conv on this thread uses the given configuration; 0 = automatic.
+ * block_n in {16,32,64,96,128} (not applied to convs whose automatic width is 16, i.e. the split-K flow-head conv),
+ * bw_log2 in [3,7] (pixel box 2^bw_log2 x 2^(7-bw_log2)), max_ctas >= 1 caps the persistent grid (on top of any
+ * internal cta_limit), stages in [2, ring maximum of that width] (5/5/4/3/3 for 16/32/64/96/128; with block_n = 0 the
+ * request is clamped to the ring of the width each conv picks).  Anything else -> RB_ERR_BAD_ARG, before any CUDA call.
+ * Workspace sizes that depend on the pixel box (rb_encoder_workspace_bytes) must be queried under the same override. */
+int rb_debug_conv_override(int block_n, int bw_log2, int max_ctas, int stages);
+/* Configuration of the last tensor-core conv launched on this thread (for tests to assert coverage): tile width, pixel
+ * box, CTAs launched, ring depth, 128-pixel x block_n tiles.  Returns the number of tensor-core convs since the last
+ * rb_debug_conv_override() call that produced fused instance-norm statistics in their epilogue (an encoder conv whose
+ * statistics fall back to the stand-alone pass is not counted), or RB_ERR_BAD_ARG if no conv has been launched. */
+int rb_debug_conv_last(int* block_n, int* bw_log2, int* grid, int* stages, int* total_tiles);
 
 /* ---- A4: coords_grid(batch, ht, wd)  networks/utils.py:4-11 ----------------------------------
  * coords[b,y,x,0] = x, coords[b,y,x,1] = y. */

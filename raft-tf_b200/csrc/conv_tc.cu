@@ -407,8 +407,36 @@ int cached_tmap(CUtensorMap* out, const void* base, int rank, const uint64_t* di
   return RB_OK;
 }
 
+// Test hook (rb_debug_conv_override / rb_debug_conv_last): a forced configuration and the record of the last launch, per
+// thread.  0 = automatic.
+struct ConvOverride {
+  int block_n, bw_log2, max_ctas, stages;
+};
+struct ConvRecord {
+  int block_n, bw_log2, grid, stages, total_tiles;
+  int launched;     // a tensor-core conv has been launched on this thread
+  int fused_stats;  // convs since the last rb_debug_conv_override() call that wrote fused instance-norm statistics
+};
+static thread_local ConvOverride g_override = {0, 0, 0, 0};
+static thread_local ConvRecord g_record = {0, 0, 0, 0, 0, 0, 0};
+
+// Ring depth of a launch: RAFT_B200_TC_STAGES / the test hook may lower it, but never below 2 -- a consumer hands a stage
+// back only after it has issued the next one (wgmma_wait<1>), so a one-stage ring deadlocks any conv with two k-iterations.
+static int ring_stages(int max_stages) {
+  static const int env_stages = getenv("RAFT_B200_TC_STAGES") ? atoi(getenv("RAFT_B200_TC_STAGES")) : 0;  // tuning knob
+  const int req = g_override.stages > 0 ? g_override.stages : env_stages;
+  if (req <= 0) return max_stages;
+  return req < 2 ? 2 : req > max_stages ? max_stages : req;
+}
+
 static TileGeom choose_geom(int h, int w) {
   TileGeom best{};
+  if (g_override.bw_log2 > 0) {
+    const int bwl = g_override.bw_log2, bw = 1 << bwl, bh = kTileM >> bwl;
+    best.bw_log2 = bwl; best.bh_log2 = 7 - bwl;
+    best.tiles_x = (w + bw - 1) / bw; best.tiles_y = (h + bh - 1) / bh;
+    return best;
+  }
   long best_tiles = -1;
   for (int bwl = 7; bwl >= 3; --bwl) {
     int bw = 1 << bwl, bh = kTileM >> bwl;
@@ -482,12 +510,14 @@ static int launch_cfg(const ConvParams& p_in, TileGeom g, const CUtensorMap* map
   static const bool no_cluster = getenv("RAFT_B200_NO_SPLITK_CLUSTER") != nullptr;  // test knob: same sums on one CTA
   static const bool close_barrier = getenv("RAFT_B200_SPLITK_CLOSING_BARRIER") != nullptr;  // for compute-sanitizer runs
   p.split_close = close_barrier ? 1 : 0;
-  p.split_cluster = (p.split_k && 2 * g.total_tiles <= num_sms && p.cta_limit <= 0 && !no_cluster) ? 1 : 0;
+  const int max_ctas = g_override.max_ctas;  // test hook: a capped grid walks more tiles per CTA (no CTA pairs then)
+  p.split_cluster = (p.split_k && 2 * g.total_tiles <= num_sms && p.cta_limit <= 0 && max_ctas <= 0 && !no_cluster) ? 1 : 0;
   const bool cluster2 = p.split_cluster;
   cudaLaunchConfig_t cfg;
   memset(&cfg, 0, sizeof(cfg));
   int units = cluster2 ? num_sms / 2 : num_sms;  // persistent: at most one CTA (pair) per SM (pair)
   if (!cluster2 && p.cta_limit > 0 && p.cta_limit < units) units = p.cta_limit;  // leave SMs to a concurrent conv (update.cu)
+  if (max_ctas > 0 && max_ctas < units) units = max_ctas;
   cfg.gridDim = dim3((g.total_tiles < units ? g.total_tiles : units) * (cluster2 ? 2 : 1));
   cfg.blockDim = dim3(kTcThreads);
   cfg.dynamicSmemBytes = Cfg::kSmemBytes;
@@ -504,14 +534,15 @@ static int launch_cfg(const ConvParams& p_in, TileGeom g, const CUtensorMap* map
   // weight tiles overlap the tail of this one.
   static const int pdl = getenv("RAFT_B200_NO_PDL") ? 0 : 1;
   cfg.numAttrs = 1 + pdl;
-  int stages = Cfg::kStages;
-  static const int env_stages = getenv("RAFT_B200_TC_STAGES") ? atoi(getenv("RAFT_B200_TC_STAGES")) : 0;  // tuning knob
-  if (env_stages > 0 && env_stages < stages) stages = env_stages;
+  const int stages = ring_stages(Cfg::kStages);
   if (p.dbg || p.stat_part)
     RB_CHECK_CUDA(cudaLaunchKernelEx(&cfg, conv_tc_kernel<BLOCK_N, true>, maps[0], maps[1], maps[2], maps[3], p, g, stages));
   else
     RB_CHECK_CUDA(cudaLaunchKernelEx(&cfg, conv_tc_kernel<BLOCK_N, false>, maps[0], maps[1], maps[2], maps[3], p, g, stages));
   RB_CHECK_LAUNCH("conv_tc_kernel");
+  g_record.block_n = BLOCK_N; g_record.bw_log2 = g.bw_log2; g_record.grid = (int)cfg.gridDim.x; g_record.stages = stages;
+  g_record.total_tiles = g.total_tiles; g_record.launched = 1;
+  if (p.stat_part) ++g_record.fused_stats;
   return RB_OK;
 }
 
@@ -523,7 +554,8 @@ int launch_conv_tc(const ConvParams& p, cudaStream_t s) {
   int dev = 0, rc_dev;
   if ((rc_dev = current_device(&dev))) return rc_dev;
   const int num_sms = device_sm_count(dev);
-  const int bn = choose_block_n(p.cout, m_tiles, p.cta_limit > 0 && p.cta_limit < num_sms ? p.cta_limit : num_sms);
+  int bn = choose_block_n(p.cout, m_tiles, p.cta_limit > 0 && p.cta_limit < num_sms ? p.cta_limit : num_sms);
+  if (g_override.block_n > 0 && bn != 16) bn = g_override.block_n;  // the 16-wide (split-K) convs keep theirs
   CUtensorMap maps[4];
   {
     // the input view (common.cuh): strided convs traverse it with TMA element strides -- a box of bw*sx x bh*sy input
@@ -559,3 +591,36 @@ int launch_conv_tc(const ConvParams& p, cudaStream_t s) {
 }
 
 }  // namespace rb
+
+extern "C" int rb_debug_conv_override(int block_n, int bw_log2, int max_ctas, int stages) {
+  using namespace rb;
+  int ring_max = 0;  // ring depth of the forced width, or the deepest ring of any width
+  switch (block_n) {
+    case 0: ring_max = TcCfg<16>::kStages > TcCfg<32>::kStages ? TcCfg<16>::kStages : TcCfg<32>::kStages; break;
+    case 16: ring_max = TcCfg<16>::kStages; break;
+    case 32: ring_max = TcCfg<32>::kStages; break;
+    case 64: ring_max = TcCfg<64>::kStages; break;
+    case 96: ring_max = TcCfg<96>::kStages; break;
+    case 128: ring_max = TcCfg<128>::kStages; break;
+    default: RB_REQUIRE(false, RB_ERR_BAD_ARG, "rb_debug_conv_override: block_n %d not in {0,16,32,64,96,128}", block_n);
+  }
+  RB_REQUIRE(bw_log2 == 0 || (bw_log2 >= 3 && bw_log2 <= 7), RB_ERR_BAD_ARG, "rb_debug_conv_override: bw_log2 %d not 0 or in [3,7]",
+             bw_log2);
+  RB_REQUIRE(max_ctas >= 0, RB_ERR_BAD_ARG, "rb_debug_conv_override: max_ctas %d < 0", max_ctas);
+  RB_REQUIRE(stages == 0 || (stages >= 2 && stages <= ring_max), RB_ERR_BAD_ARG,
+             "rb_debug_conv_override: stages %d not 0 or in [2,%d]", stages, ring_max);
+  g_override = {block_n, bw_log2, max_ctas, stages};
+  g_record.fused_stats = 0;
+  return RB_OK;
+}
+
+extern "C" int rb_debug_conv_last(int* block_n, int* bw_log2, int* grid, int* stages, int* total_tiles) {
+  using namespace rb;
+  RB_REQUIRE(g_record.launched, RB_ERR_BAD_ARG, "rb_debug_conv_last: no tensor-core conv has been launched on this thread");
+  if (block_n) *block_n = g_record.block_n;
+  if (bw_log2) *bw_log2 = g_record.bw_log2;
+  if (grid) *grid = g_record.grid;
+  if (stages) *stages = g_record.stages;
+  if (total_tiles) *total_tiles = g_record.total_tiles;
+  return g_record.fused_stats;
+}

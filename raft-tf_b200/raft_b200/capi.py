@@ -28,6 +28,8 @@ SIGNATURES = {
     "rb_launch_count": (C.c_longlong, []),
     "rb_launch_count_reset": (None, []),
     "rb_debug_set_buffer": (_i, [_vp]),
+    "rb_debug_conv_override": (_i, [_i, _i, _i, _i]),
+    "rb_debug_conv_last": (_i, [_pi, _pi, _pi, _pi, _pi]),
     "rb_coords_grid": (_i, [_vp, _i, _i, _i, _vp]),
     "rb_corr_pyramid_bytes": (_i, [_i, _i, _i, _psz]),
     "rb_corr_level_offset": (_i, [_i, _i, _i, _i, _psz, _pi, _pi]),

@@ -44,3 +44,23 @@ def test_host_only_queries():
     assert lib.rb_conv2d_strided(p, p, None, p, 1, 8, 8, 4, 4, 2, 2, 1, 0, p, 64, None) == -3
     assert lib.rb_update_packed_conv(0, 12, None, None, None, None, None, None, None, None) == -2
 
+
+def test_conv_override_argument_checks():
+    """The tensor-core conv test hook refuses configurations the kernel cannot run, without touching CUDA."""
+    from raft_b200 import capi
+    lib = capi.lib
+    bad = [(48, 0, 0, 0), (8, 0, 0, 0), (256, 0, 0, 0), (-32, 0, 0, 0),  # tile widths
+           (0, 8, 0, 0), (0, 2, 0, 0), (0, -1, 0, 0),                    # pixel boxes
+           (0, 0, -1, 0),                                                 # CTA cap
+           (0, 0, 0, 1), (0, 0, 0, -2), (0, 0, 0, 6),                    # a 1-stage ring deadlocks; no width has 6 stages
+           (96, 0, 0, 4), (128, 0, 0, 4), (64, 0, 0, 5), (16, 0, 0, 6)]  # ring depth beyond that width's smem ring
+    try:
+        for args in bad:
+            assert lib.rb_debug_conv_override(*args) == -2, args
+            assert b"rb_debug_conv_override" in lib.rb_last_error()
+        good = [(0, 0, 0, 0), (16, 3, 1, 2), (32, 7, 5, 5), (64, 4, 2, 4), (96, 5, 0, 3), (128, 6, 1, 3), (0, 0, 0, 5)]
+        for args in good:
+            assert lib.rb_debug_conv_override(*args) == 0, args
+    finally:
+        assert lib.rb_debug_conv_override(0, 0, 0, 0) == 0
+

@@ -18,9 +18,11 @@ def _kernel_parity(env):
 
 
 @pytest.mark.parametrize("knob", ["RAFT_B200_NO_HOIST", "RAFT_B200_FH2_SIMT", "RAFT_B200_NO_PDL",
-                                  "RAFT_B200_STEM_WINDOWS", "RAFT_B200_NO_SPLITK", "RAFT_B200_NO_SPLITK_CLUSTER", "RAFT_B200_CONVF1_SIMT"])
+                                  "RAFT_B200_STEM_WINDOWS", "RAFT_B200_NO_SPLITK", "RAFT_B200_NO_SPLITK_CLUSTER", "RAFT_B200_CONVF1_SIMT",
+                                  "RAFT_B200_TC_STAGES=2"])
 def test_variant_passes_conv_and_update_parity(cuda, knob):
-    _kernel_parity(dict(os.environ, **{knob: "1"}))
+    name, _, value = knob.partition("=")
+    _kernel_parity(dict(os.environ, **{name: value or "1"}))
 
 
 def test_warp_per_pixel_lookup_kernel_bit_exact(cuda):
