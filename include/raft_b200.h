@@ -191,6 +191,19 @@ int rb_upsample_convex_crop(const float* coords1, const float* mask, float* out,
 int rb_upflow8_crop(const float* coords1, float* out, int B, int h, int w, float scale, int top, int left,
                     int out_h, int out_w, void* stream);
 
+/* ---- F5: forward-backward consistency of a pair of full-resolution flows (Sundaram et al. 2010; UnFlow) -------
+ * Both directions in one launch.  flow_fw, flow_bw: [B,H,W,2] fp32; occ_fw, occ_bw: [B,H,W] uint8:
+ * 0 = consistent, 1 = inconsistent (occluded), 2 = the flow leaves the frame.  Per pixel p = (x,y) of fw (bw alike,
+ * with the flows swapped): f = s*fw(p) (s = flow_scale: 8.0 for raft-small, whose upflow8 flow is in 1/8-resolution
+ * units, 1.0 for raft-things), q = p + f; 2 unless 0 <= q.x <= W-1 and 0 <= q.y <= H-1 (a NaN gives 2); b = s times
+ * the bilinear sample of bw at q (x0 = floor(q.x), x1 = min(x0+1, W-1), ax = q.x - x0, rows likewise,
+ * ((1-ax)b00 + ax b01)(1-ay) + ((1-ax)b10 + ax b11)ay); 1 if |f+b|^2 > alpha1 (|f|^2 + |b|^2) + alpha2, else 0.  Every
+ * operation is rounded on its own, left to right, without FMA contraction (bit-reproducible by an fp32 restatement).
+ * Null pointers, B/H/W <= 0, flow_scale <= 0 or non-finite, negative or non-finite alphas -> RB_ERR_* before any CUDA
+ * call.  UnFlow's constants are alpha1 = 0.01, alpha2 = 0.5. */
+int rb_flow_fb_check(const float* flow_fw, const float* flow_bw, uint8_t* occ_fw, uint8_t* occ_bw,
+                     int B, int H, int W, float flow_scale, float alpha1, float alpha2, void* stream);
+
 /* ---- F3 (input edge): dataflow/test_dataflow.py:56-61,96-97 + the SURVEY 8(d) shape policy ------------------
  * src: [B,H,W,3] device frames, BGR like cv2.imdecode -- fp32 in [0,1] (src_is_u8 = 0) or uint8 in [0,255]
  * (src_is_u8 = 1: x/255.0f, the reference's np.float32(x)/255.0, bit for bit).  dst: [B,H+pt+pb,W+pl+pr,3] fp32

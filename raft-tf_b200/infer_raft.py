@@ -8,7 +8,10 @@ Like the reference it decodes BGR with OpenCV, resizes both frames to 432x1024 (
 dataflow/test_dataflow.py:85-87), scales to [0,1], runs 20 iterations and writes the colour-coded flow
 to ``raft_flow_raft-things.png`` in the working directory (regardless of --small, infer_raft.py:44).
 Flags the reference parses but ignores (--gpu, --data, --out, -o) are accepted; ``--batch`` stays 1.
-Extensions: --iters, --keep-size (replicate-pad to a multiple of 8 instead of resizing), --npy.
+Extensions: --iters, --keep-size (replicate-pad to a multiple of 8 instead of resizing), --npy, --flo, and
+--bidirectional: also the flow im2 -> im1 (``raft_flow_raft-things_bw.png``, ``<npy>_bw.npy``, ``<flo>_bw.flo``) and the
+forward-backward occlusion masks ``raft_occ_fw.png`` / ``raft_occ_bw.png`` (0 consistent, 128 occluded, 255 leaves the
+frame), from one pass that encodes each frame once.
 """
 import argparse
 import os
@@ -49,6 +52,8 @@ def main(argv=None):
     p.add_argument('--keep-size', action='store_true', help='extension: pad to a multiple of 8 instead of resizing to 432x1024')
     p.add_argument('--npy', default=None, help='extension: also save the raw [H,W,2] flow')
     p.add_argument('--flo', default=None, help='extension: also save the flow as a Middlebury .flo file')
+    p.add_argument('--bidirectional', action='store_true',
+                   help='extension: also the backward flow and the forward-backward occlusion masks')
     args = p.parse_args(argv)
     if args.mode != 'test':
         print(f"mode '{args.mode}' has no implementation in the reference either (infer_raft.py:71-95); nothing to do")
@@ -58,14 +63,31 @@ def main(argv=None):
     from flow_utils import flow_to_color, write_flo
     left, right = read_pair(args.im1, args.im2, None if args.keep_size else (432, 1024))
     model = RAFT.RAFT(left.shape[1:], args, iters=args.iters).load(args.load)
-    flow = model.forward(left, right).cpu().numpy()
+    if args.bidirectional:
+        flow, flow_bw, occ_fw, occ_bw = (t.cpu().numpy() for t in model.forward_bidirectional(left, right))
+    else:
+        flow = model.forward(left, right).cpu().numpy()
     print(0, flow.shape)
     cv2.imwrite("raft_flow_raft-things.png", flow_to_color(flow[0], convert_to_bgr=True))
     if args.npy:
         np.save(args.npy, flow[0])
     if args.flo:
         write_flo(args.flo, flow[0])
+    if args.bidirectional:
+        cv2.imwrite("raft_flow_raft-things_bw.png", flow_to_color(flow_bw[0], convert_to_bgr=True))
+        grey = np.array([0, 128, 255], dtype=np.uint8)  # consistent / occluded / leaves the frame
+        cv2.imwrite("raft_occ_fw.png", grey[occ_fw[0]])
+        cv2.imwrite("raft_occ_bw.png", grey[occ_bw[0]])
+        if args.npy:
+            np.save(_bw_path(args.npy), flow_bw[0])
+        if args.flo:
+            write_flo(_bw_path(args.flo), flow_bw[0])
     return 0
+
+
+def _bw_path(path):
+    stem, ext = os.path.splitext(path)
+    return stem + "_bw" + ext
 
 
 if __name__ == '__main__':

@@ -90,8 +90,22 @@ class RAFT(object):
         uint8 in [0,255] (extension: the /255 of test_dataflow.py:96-97 then runs on the GPU); numpy or torch, host or
         CUDA -> [B,H,W,2] torch CUDA flow (a fresh tensor per call, like a session.run result).  H, W that are not
         multiples of 8 are replicate-padded and the flow cropped back, both inside the engine's own kernels."""
-        def as_tensor(x):
-            t = torch.as_tensor(x)
-            return t if t.dtype == torch.uint8 else t.to(torch.float32)
-        flow = self.engine().forward(as_tensor(input_left), as_tensor(input_right))
+        flow = self.engine().forward(_as_tensor(input_left), _as_tensor(input_right))
         return flow.clone()
+
+    @torch.no_grad()
+    def forward_bidirectional(self, input_left, input_right, check=True):
+        """Extension (frame interpolation needs flow both ways): the flows left -> right and right -> left of the same
+        frames, each frame encoded once and both directions run as one batch.  Inputs as for ``forward``.  Returns fresh
+        tensors ``(flow_fw, flow_bw, occ_fw, occ_bw)``: flow_fw equals ``forward(left, right)`` and flow_bw equals
+        ``forward(right, left)`` bit for bit; the [B,H,W] uint8 masks are the forward-backward consistency check
+        (networks.utils.fb_consistency with UnFlow's alpha1 = 0.01, alpha2 = 0.5; flow_scale 8 for raft-small, whose
+        flow is in 1/8-resolution units): 0 consistent, 1 occluded, 2 the flow leaves the frame.  check=False skips the
+        check and returns None for both masks."""
+        out = self.engine().forward_bidirectional(_as_tensor(input_left), _as_tensor(input_right), check=check)
+        return tuple(None if t is None else t.clone() for t in out)
+
+
+def _as_tensor(x):
+    t = torch.as_tensor(x)
+    return t if t.dtype == torch.uint8 else t.to(torch.float32)

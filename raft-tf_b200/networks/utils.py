@@ -36,3 +36,20 @@ def upflow8(flow):
     with torch.cuda.device(out.device):
         capi.check(capi.lib.rb_upflow8(capi.ptr(coords1), capi.ptr(out), b, h, w, 1.0, capi.stream()))
     return out
+
+
+def fb_consistency(flow_fw, flow_bw, alpha1=0.01, alpha2=0.5, flow_scale=1.0):
+    """Extension (no counterpart in the reference): forward-backward consistency of two [B,H,W,2] flows on the GPU
+    (rb_flow_fb_check; Sundaram et al. 2010, UnFlow's alpha1 / alpha2 as defaults).  flow_scale multiplies both flows
+    first: 8.0 for raft-small, whose upflow8 output is in 1/8-resolution units.  Returns (occ_fw, occ_bw), [B,H,W]
+    uint8: 0 consistent, 1 inconsistent (occluded), 2 the flow leaves the frame."""
+    assert flow_fw.shape == flow_bw.shape and flow_fw.dim() == 4 and flow_fw.shape[-1] == 2, (flow_fw.shape, flow_bw.shape)
+    assert flow_fw.device == flow_bw.device, (flow_fw.device, flow_bw.device)
+    b, H, W, _ = flow_fw.shape
+    fw, bw = flow_fw.contiguous().float(), flow_bw.contiguous().float()
+    occ_fw = torch.empty(b, H, W, dtype=torch.uint8, device=fw.device)
+    occ_bw = torch.empty_like(occ_fw)
+    with torch.cuda.device(fw.device):
+        capi.check(capi.lib.rb_flow_fb_check(capi.ptr(fw), capi.ptr(bw), capi.ptr(occ_fw), capi.ptr(occ_bw), b, H, W,
+                                             float(flow_scale), float(alpha1), float(alpha2), capi.stream()))
+    return occ_fw, occ_bw

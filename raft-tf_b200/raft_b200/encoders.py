@@ -9,6 +9,7 @@ reference.
 """
 from __future__ import annotations
 
+import copy
 from typing import Dict
 
 import numpy as np
@@ -121,6 +122,13 @@ class CudaEncoder:
             capi.check(lib.rb_encoder_weights_pack(self.small, self.norm, self.out_dim, Ws, bs, bns, capi.ptr(self.blob), nbytes,
                                                    capi.stream()))
         self._ws, self._ws_key = None, None
+
+    def with_own_workspace(self) -> "CudaEncoder":
+        """The same packed weights with a workspace of its own.  The workspace is reallocated when the frame batch
+        changes, so a caller that alternates two batch sizes, each captured in a CUDA graph, needs one encoder per size."""
+        twin = copy.copy(self)
+        twin._ws, twin._ws_key = None, None
+        return twin
 
     def __call__(self, img01_nhwc: torch.Tensor, out: torch.Tensor = None) -> torch.Tensor:
         """[B,H,W,3] fp32 in [0,1] (NOT yet 2x-1) -> [B,H/8,W/8,out_dim] fp32."""

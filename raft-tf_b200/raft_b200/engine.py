@@ -3,6 +3,8 @@
 rb_encoder_forward x2 (fnet on both frames, cnet on a forked stream; csrc/encoder.cu) -> rb_corr_build ->
 rb_update_set_state_cnet -> rb_raft_iterate (lookup + update block per iteration) -> rb_upsample_convex /
 rb_upflow8, all replayed from ONE CUDA graph.  Mirrors RAFT.network_graph (networks/RAFT.py:78-109).
+forward_bidirectional runs both directions of B frame pairs as 2B pairs through the same path (each frame encoded once)
+and adds the forward-backward consistency check (rb_flow_fb_check, csrc/consistency.cu) to the same graph.
 The torch/cuDNN restatement of the encoders (encoders.Encoder) is a cross-check behind RAFT_B200_TORCH_ENCODERS=1.
 """
 from __future__ import annotations
@@ -17,8 +19,18 @@ from . import capi
 from .encoders import CudaEncoder, Encoder
 from .weights import pack_update_block
 
+# what one pass computes: L->R only (forward), both directions (forward_bidirectional), both plus the occlusion check
+FORWARD, BIDIRECTIONAL, BIDIRECTIONAL_CHECK = 0, 1, 2
+# forward-backward consistency thresholds of UnFlow (Meister et al. 2018): |f+b|^2 > a1 (|f|^2 + |b|^2) + a2
+FB_ALPHA1, FB_ALPHA2 = 0.01, 0.5
+
 
 class RaftEngine:
+    # everything _ensure allocates for one (B, H, W, u8, mode); parked per mode so alternating modes re-captures nothing
+    _STATE = ("pad", "h", "w", "Hp", "Wp", "pairs", "pyr_bytes", "pyramid", "cws_bytes", "corr_ws", "ws_bytes", "ws",
+              "coords1", "mask", "flow_up", "occ", "fmaps", "fmap1", "fmap2", "cmap", "images", "staged", "raw", "_shape",
+              "_graph")
+
     def __init__(self, params: Dict[str, np.ndarray], small: bool = False, iters: int = 20,
                  device: Optional[torch.device] = None, use_graph: bool = True, math_mode: int = capi.RB_MATH_TC,
                  volume_free: Optional[bool] = None):
@@ -46,49 +58,67 @@ class RaftEngine:
                 self.fnet = CudaEncoder(params, "fnet", small, "instance", self.fdim, self.device)
                 self.cnet = CudaEncoder(params, "cnet", small, cnorm, self.hidden + self.ctx, self.device)
             self.blob = pack_update_block(params, small, self.device)
+        # the bidirectional pass runs the context encoder on 2B frames, forward on B: a twin with its own workspace keeps
+        # the workspace each mode's CUDA graph was captured with (the feature encoder sees 2B frames in both modes)
+        self.cnet_bidir = self.cnet if self.torch_encoders else self.cnet.with_own_workspace()
         self._shape = None
         self._graph = None
+        self._parked = {}  # (B, H, W, u8, mode) -> buffers and graph of the other modes at the current frame size
         self._enc_stream = None   # forked stream of the context encoder (encode())
         self._capture_stream = None  # CUDA-graph capture stream on this engine's device (run())
         self._cnet_pending = False
         self._range_checked = False  # first forward of this weight set: fp16-range check of the split path's inputs
 
     # ---- buffers -------------------------------------------------------------------------------
-    def _ensure(self, B: int, H: int, W: int, u8: bool = False):
+    def _ensure(self, B: int, H: int, W: int, u8: bool = False, mode: int = FORWARD):
         """Buffers for B frame pairs of H x W pixels.  H, W need not be multiples of 8: frames are replicate-padded
         to (Hp, Wp) by rb_frames_prepare (upstream InputPadder 'sintel' split, SURVEY 8(d)) and the flow is cropped
-        back by the upsampling kernel -- the reference itself cannot run such shapes (SURVEY fact 6)."""
-        if self._shape == (B, H, W, u8):
+        back by the upsampling kernel -- the reference itself cannot run such shapes (SURVEY fact 6).
+
+        In the bidirectional modes the hot path runs 2B pairs, (L_i -> R_i) then (R_i -> L_i): fmaps holds 3B feature
+        maps [fL | fR | fL], so fmap1 = fmaps[:2B] and fmap2 = fmaps[B:] are both contiguous views."""
+        key = (B, H, W, u8, mode)
+        if self._shape == key:
             return
+        # alternating modes on one frame size keeps every mode's buffers and CUDA graph; a new frame size drops them
+        if self._shape is not None:
+            self._parked[self._shape] = {k: getattr(self, k) for k in self._STATE}
+        self._parked = {k: v for k, v in self._parked.items() if k[:4] == key[:4]}
+        if key in self._parked:
+            self.__dict__.update(self._parked.pop(key))
+            return
+        bidir = mode != FORWARD
+        NB = 2 * B if bidir else B  # frame pairs through the hot path
         ph, pw = (-H) % 8, (-W) % 8
         self.pad = (ph // 2, ph - ph // 2, pw // 2, pw - pw // 2)  # top, bottom, left, right
         Hp, Wp = H + ph, W + pw
         h, w, s = Hp // 8, Wp // 8, int(self.small)
         d = self.device
         lib = capi.lib
-        self.h, self.w, self.Hp, self.Wp = h, w, Hp, Wp
+        self.h, self.w, self.Hp, self.Wp, self.pairs = h, w, Hp, Wp, NB
         if self.volume_free:
             self.pyr_bytes, self.pyramid = 0, None
-            self.cws_bytes = capi.size_query(lib.rb_corr_otf_workspace_bytes, B, h, w, self.fdim)  # pooled fmap2, levels 1..3
+            self.cws_bytes = capi.size_query(lib.rb_corr_otf_workspace_bytes, NB, h, w, self.fdim)  # pooled fmap2, levels 1..3
         else:
-            self.pyr_bytes = capi.size_query(lib.rb_corr_pyramid_bytes, B, h, w)
+            self.pyr_bytes = capi.size_query(lib.rb_corr_pyramid_bytes, NB, h, w)
             self.pyramid = torch.empty(self.pyr_bytes // 4, dtype=torch.float32, device=d)
-            self.cws_bytes = capi.size_query(lib.rb_corr_workspace_bytes, B, h, w, self.fdim)
+            self.cws_bytes = capi.size_query(lib.rb_corr_workspace_bytes, NB, h, w, self.fdim)
         self.corr_ws = torch.zeros(self.cws_bytes, dtype=torch.uint8, device=d)
-        self.ws_bytes = capi.size_query(lib.rb_update_workspace_bytes, s, B, h, w)
+        self.ws_bytes = capi.size_query(lib.rb_update_workspace_bytes, s, NB, h, w)
         self.ws = torch.zeros(self.ws_bytes, dtype=torch.uint8, device=d)  # zero fill = channel padding
-        self.coords1 = torch.empty(B, h, w, 2, dtype=torch.float32, device=d)
-        self.mask = None if self.small else torch.empty(B, h, w, 576, dtype=torch.float32, device=d)
-        self.flow_up = torch.empty(B, H, W, 2, dtype=torch.float32, device=d)
-        self.fmaps = torch.empty(2 * B, h, w, self.fdim, dtype=torch.float32, device=d)
-        self.fmap1, self.fmap2 = self.fmaps[:B], self.fmaps[B:]
-        self.cmap = torch.empty(B, h, w, self.hidden + self.ctx, dtype=torch.float32, device=d)
+        self.coords1 = torch.empty(NB, h, w, 2, dtype=torch.float32, device=d)
+        self.mask = None if self.small else torch.empty(NB, h, w, 576, dtype=torch.float32, device=d)
+        self.flow_up = torch.empty(NB, H, W, 2, dtype=torch.float32, device=d)  # bidirectional: [L->R | R->L]
+        self.occ = torch.empty(2 * B, H, W, dtype=torch.uint8, device=d) if mode == BIDIRECTIONAL_CHECK else None
+        self.fmaps = torch.empty(NB + B, h, w, self.fdim, dtype=torch.float32, device=d)
+        self.fmap1, self.fmap2 = self.fmaps[:NB], self.fmaps[B:]
+        self.cmap = torch.empty(NB, h, w, self.hidden + self.ctx, dtype=torch.float32, device=d)
         self.images = torch.empty(2 * B, Hp, Wp, 3, dtype=torch.float32, device=d)  # [left | right], [0,1], padded
         # staging buffer of the raw frames (uint8 or unpadded fp32); fp32 frames that need no padding go straight
         # into self.images
         self.staged = bool(u8 or ph or pw)
         self.raw = torch.empty(2 * B, H, W, 3, dtype=torch.uint8 if u8 else torch.float32, device=d) if self.staged else None
-        self._shape = (B, H, W, u8)
+        self._shape = key
         self._graph = None
 
     # ---- stages --------------------------------------------------------------------------------
@@ -98,19 +128,25 @@ class RaftEngine:
         The context encoder is independent of the feature encoder (RAFT.py:79-87) and both are chains of ~50 small
         kernels at 1/4 and 1/8 resolution: cnet runs on a forked stream beside fnet (a fork/join that is captured into
         the CUDA graph like the flow branch of the update block).  With defer_join the caller joins (`_join_cnet`)
-        where cmap is first needed -- after the correlation volume, which only needs the feature maps."""
-        B, H, W, u8 = self._shape
+        where cmap is first needed -- after the correlation volume, which only needs the feature maps.
+
+        Bidirectional modes: cnet runs on all 2B frames (the R->L pairs need the context of R), and the last B feature
+        maps are a device-to-device copy of the first B (a copy-engine transfer, no kernel)."""
+        B, H, W, u8, mode = self._shape
+        bidir = mode != FORWARD
+        cnet, cframes = (self.cnet_bidir, self.images) if bidir else (self.cnet, self.images[:B])
+        fout = self.fmaps[:2 * B]  # [fL | fR]
         capi.check(capi.lib.rb_set_math_mode(self.math_mode))  # per-thread library state: set before ANY kernel of ours
         if self.staged:  # F3: u8 -> fp32 /255 and replicate padding in one pass (csrc/frames.cu)
             capi.check(capi.lib.rb_frames_prepare(capi.ptr(self.raw), int(u8), capi.ptr(self.images), 2 * B, H, W,
                                                   *self.pad, capi.stream()))
         if self.torch_encoders:
             both = self.images * 2.0 - 1.0
-            self.fmaps.copy_(self.fnet(both))  # instance norm is per sample, so batching left|right is exact
-            self.cmap.copy_(self.cnet(both[:B]))
+            fout.copy_(self.fnet(both))  # instance norm is per sample, so batching left|right is exact
+            self.cmap.copy_(cnet(both if bidir else both[:B]))
         elif os.environ.get("RAFT_B200_SERIAL_ENCODERS"):
-            self.fnet(self.images, out=self.fmaps)
-            self.cnet(self.images[:B], out=self.cmap)
+            self.fnet(self.images, out=fout)
+            cnet(cframes, out=self.cmap)
         else:
             main = torch.cuda.current_stream(self.device)
             if self._enc_stream is None:
@@ -118,11 +154,13 @@ class RaftEngine:
             side = self._enc_stream
             side.wait_stream(main)  # fork: the frames are in place
             with torch.cuda.stream(side):
-                self.cnet(self.images[:B], out=self.cmap)
-            self.fnet(self.images, out=self.fmaps)
+                cnet(cframes, out=self.cmap)
+            self.fnet(self.images, out=fout)
             self._cnet_pending = True
-            if not defer_join:
-                self._join_cnet()
+        if bidir:
+            self.fmaps[2 * B:].copy_(self.fmaps[:B])  # contiguous, same dtype: cudaMemcpyAsync on the current stream
+        if self._cnet_pending and not defer_join:
+            self._join_cnet()
 
     def _join_cnet(self):
         if self._cnet_pending:
@@ -130,8 +168,9 @@ class RaftEngine:
             self._cnet_pending = False
 
     def _hot_path(self):
-        """corr build + iterations + upsampling: hand-written kernels only (graph-capturable)."""
-        B, H, W, _ = self._shape
+        """corr build + iterations + upsampling (+ the consistency check): hand-written kernels only (graph-capturable)."""
+        B0, H, W, _, mode = self._shape
+        B = self.pairs
         h, w, s, lib, st = self.h, self.w, int(self.small), capi.lib, capi.stream()
         capi.check(lib.rb_set_math_mode(self.math_mode))
         if self.volume_free:
@@ -158,6 +197,10 @@ class RaftEngine:
         else:
             capi.check(lib.rb_upsample_convex_crop(capi.ptr(self.coords1), capi.ptr(self.mask), capi.ptr(self.flow_up),
                                                    B, h, w, top, left, H, W, st))
+        if mode == BIDIRECTIONAL_CHECK:  # raft-small's flow is in 1/8-resolution units (upflow8 does not scale it)
+            capi.check(lib.rb_flow_fb_check(capi.ptr(self.flow_up[:B0]), capi.ptr(self.flow_up[B0:]), capi.ptr(self.occ[:B0]),
+                                            capi.ptr(self.occ[B0:]), B0, H, W, 8.0 if self.small else 1.0, FB_ALPHA1,
+                                            FB_ALPHA2, st))
 
     def _all(self):
         self.encode(defer_join=True)
@@ -202,19 +245,37 @@ class RaftEngine:
         uint8 in [0,255] (what cv2.imdecode yields, test_dataflow.py:56-61; the /255 then happens on the GPU).  Host
         (ideally pinned) or CUDA tensors; any H, W >= 8.  Returns the [B,H,W,2] flow -- the engine-owned buffer itself,
         overwritten by the next call (networks.RAFT.RAFT.forward hands out a copy)."""
+        self._run_frames(left, right, FORWARD)
+        return self.flow_up
+
+    @torch.no_grad()
+    def forward_bidirectional(self, left: torch.Tensor, right: torch.Tensor, check: bool = True):
+        """Both directions of B frame pairs in one pass: fnet once on the 2B frames, cnet on all 2B, the hot path on 2B
+        pairs (L_i -> R_i, then R_i -> L_i).  Frames as for forward(); per pair the flows are bit-identical to
+        forward(L, R) and forward(R, L) (every kernel is batch-invariant, DESIGN §4).  Returns (flow_fw, flow_bw, occ_fw,
+        occ_bw): [B,H,W,2] fp32 flows and [B,H,W] uint8 masks of rb_flow_fb_check (0 consistent, 1 occluded, 2 leaves
+        the frame; None when check is False) -- views of engine-owned buffers, overwritten by the next call.
+        Alternating with forward() at one frame size keeps the buffers and CUDA graph of each mode (the memory of
+        both); a call at another frame size releases them."""
+        mode = BIDIRECTIONAL_CHECK if check else BIDIRECTIONAL
+        self._run_frames(left, right, mode)
+        B = left.shape[0]
+        occ = (self.occ[:B], self.occ[B:]) if check else (None, None)
+        return (self.flow_up[:B], self.flow_up[B:]) + occ
+
+    def _run_frames(self, left: torch.Tensor, right: torch.Tensor, mode: int):
         assert left.shape == right.shape and left.dim() == 4 and left.shape[-1] == 3 and left.dtype == right.dtype
         u8 = left.dtype == torch.uint8
         assert u8 or left.dtype == torch.float32, left.dtype
         with torch.cuda.device(self.device):
             B = left.shape[0]
-            self._ensure(B, left.shape[1], left.shape[2], u8)
+            self._ensure(B, left.shape[1], left.shape[2], u8, mode)
             dst = self.raw if self.staged else self.images
             dst[:B].copy_(left, non_blocking=True)  # H2D when the caller hands pinned host tensors
             dst[B:].copy_(right, non_blocking=True)
             self.run()
             if not self._range_checked:
                 self._check_range()
-        return self.flow_up
 
     def _check_range(self):
         """Once per engine: the split-operand format (fp16 hi/lo planes) saturates beyond 65504.  The fp32 tensors at
