@@ -350,7 +350,9 @@ __device__ __forceinline__ void epilogue_store(const ConvParams& p, int pix, int
         y[i] = (p.div != 0.f) ? div_rn(y[i], p) : p.scale * y[i];
       }
       float* dst = p.f0 + (size_t)pix * p.cout + c;
-      if (full && (p.cout & 3) == 0 && NV % 4 == 0) {
+      // 16-byte stores only at 16-byte aligned addresses: f0 may start anywhere (correlation-pyramid level l starts at
+      // B*N*sum(h_k*w_k, k<l) floats, e.g. 70227 for a 9x17 grid at B = 3, whose level 1 has 32-float rows)
+      if (full && NV % 4 == 0 && (reinterpret_cast<uintptr_t>(dst) & 15) == 0) {
 #pragma unroll
         for (int i = 0; i < NV; i += 4) *reinterpret_cast<float4*>(dst + i) = make_float4(y[i], y[i + 1], y[i + 2], y[i + 3]);
       } else {

@@ -23,6 +23,9 @@ from .weights import pack_update_block
 FORWARD, BIDIRECTIONAL, BIDIRECTIONAL_CHECK = 0, 1, 2
 # forward-backward consistency thresholds of UnFlow (Meister et al. 2018): |f+b|^2 > a1 (|f|^2 + |b|^2) + a2
 FB_ALPHA1, FB_ALPHA2 = 0.01, 0.5
+# smallest frame side: the 4-level correlation pyramid needs a 1/8-resolution grid of at least 8 (level 3 is grid >> 3),
+# and ceil(H / 8) >= 8 means H >= 57
+MIN_FRAME = 57
 
 
 class RaftEngine:
@@ -80,6 +83,9 @@ class RaftEngine:
         key = (B, H, W, u8, mode)
         if self._shape == key:
             return
+        if H < MIN_FRAME or W < MIN_FRAME:  # refused here, before the encoders run or any buffer is allocated
+            raise ValueError(f"raft_b200: {H}x{W} frames are too small: frames must be at least {MIN_FRAME} pixels on each "
+                             "side (a 1/8-resolution grid of at least 8x8 for the 4-level correlation pyramid)")
         # alternating modes on one frame size keeps every mode's buffers and CUDA graph; a new frame size drops them
         if self._shape is not None:
             self._parked[self._shape] = {k: getattr(self, k) for k in self._STATE}
@@ -243,8 +249,9 @@ class RaftEngine:
     def forward(self, left: torch.Tensor, right: torch.Tensor) -> torch.Tensor:
         """left/right: [B,H,W,3] frames, BGR like the reference: fp32 in [0,1] (RAFT.inputs(), RAFT.py:45-51) or
         uint8 in [0,255] (what cv2.imdecode yields, test_dataflow.py:56-61; the /255 then happens on the GPU).  Host
-        (ideally pinned) or CUDA tensors; any H, W >= 8.  Returns the [B,H,W,2] flow -- the engine-owned buffer itself,
-        overwritten by the next call (networks.RAFT.RAFT.forward hands out a copy)."""
+        (ideally pinned) or CUDA tensors; any H, W >= 57 (MIN_FRAME; smaller frames raise ValueError).  Returns the
+        [B,H,W,2] flow -- the engine-owned buffer itself, overwritten by the next call (networks.RAFT.RAFT.forward hands
+        out a copy)."""
         self._run_frames(left, right, FORWARD)
         return self.flow_up
 

@@ -45,6 +45,44 @@ def test_host_only_queries():
     assert lib.rb_update_packed_conv(0, 12, None, None, None, None, None, None, None, None) == -2
 
 
+def test_pipeline_argument_checks():
+    """Bad arguments of the frame, upsampling, loop and volume-free entry points return RB_ERR_* with a message before any
+    CUDA call (every pointer below is a host address: a launch would fail, not return these codes)."""
+    from raft_b200 import capi
+    lib = capi.lib
+    BAD_SHAPE, BAD_ARG = -1, -2
+    buf = (ctypes.c_float * 16)()
+    p = ctypes.cast(buf, ctypes.c_void_p)
+
+    def refused(rc, code, *words):
+        assert rc == code, (rc, code)
+        msg = lib.rb_last_error()
+        assert all(w in msg for w in words), msg
+
+    # rb_frames_prepare(src, u8, dst, B, H, W, top, bottom, left, right)
+    refused(lib.rb_frames_prepare(None, 1, p, 2, 37, 53, 0, 0, 0, 0, None), BAD_ARG, b"rb_frames_prepare", b"null")
+    refused(lib.rb_frames_prepare(p, 0, None, 2, 37, 53, 0, 0, 0, 0, None), BAD_ARG, b"rb_frames_prepare", b"null")
+    for pads in ((-1, 0, 0, 0), (0, -1, 0, 0), (0, 0, -1, 0), (0, 0, 0, -3)):
+        refused(lib.rb_frames_prepare(p, 1, p, 2, 37, 53, *pads, None), BAD_SHAPE, b"rb_frames_prepare", b"pad")
+    # crops of the 8h x 8w = 56 x 72 field: (top, left, out_h, out_w)
+    for top, left, oh, ow in ((0, 0, 57, 72), (0, 0, 56, 73), (50, 0, 7, 8), (0, 70, 8, 3), (-1, 0, 8, 8), (0, -2, 8, 8),
+                              (0, 0, 0, 8), (0, 0, 8, 0), (4, 4, -1, 8)):
+        refused(lib.rb_upsample_convex_crop(p, p, p, 2, 7, 9, top, left, oh, ow, None), BAD_SHAPE,
+                b"rb_upsample_convex_crop", b"outside")
+        refused(lib.rb_upflow8_crop(p, p, 2, 7, 9, ctypes.c_float(1.0), top, left, oh, ow, None), BAD_SHAPE,
+                b"rb_upflow8_crop", b"outside")
+    # rb_raft_iterate(small, weights, workspace, pyramid, coords1, mask_out, B, h, w, iters)
+    for small in (0, 1):
+        refused(lib.rb_raft_iterate(small, p, p, p, p, p, 1, 8, 8, 0, None), BAD_ARG, b"rb_raft_iterate", b"iters")
+    refused(lib.rb_raft_iterate(0, p, p, p, p, None, 1, 8, 8, 4, None), BAD_ARG, b"rb_raft_iterate", b"mask_out")
+    # volume-free lookups: C must be 128 or 256, the grid at least 8 x 8
+    for B, h, w, C in ((1, 8, 8, 64), (1, 7, 8, 256), (1, 8, 7, 128)):
+        refused(lib.rb_corr_otf_lookup(p, p, p, p, p, B, h, w, C, 4, None), BAD_SHAPE, b"volume-free")
+        for small in (0, 1):
+            refused(lib.rb_update_lookup_otf(small, p, p, p, p, p, B, h, w, C, None), BAD_SHAPE, b"volume-free")
+    refused(lib.rb_corr_otf_prepare(p, p, 1 << 20, 1, 7, 8, 256, None), BAD_SHAPE, b"rb_corr_otf_prepare")
+
+
 def test_conv_override_argument_checks():
     """The tensor-core conv test hook refuses configurations the kernel cannot run, without touching CUDA."""
     from raft_b200 import capi

@@ -145,9 +145,11 @@ def test_bilinear_sampler_general(cuda):
 
 
 @pytest.mark.parametrize("mode", ["tc", "simt"])
-@pytest.mark.parametrize("B,h,w,C", [(1, 16, 32, 128), (2, 13, 27, 256), (1, 24, 40, 256)])
+@pytest.mark.parametrize("B,h,w,C", [(1, 16, 32, 128), (2, 13, 27, 256), (1, 24, 40, 256), (3, 9, 17, 256), (1, 9, 17, 128)])
 def test_corr_pyramid(cuda, mode, B, h, w, C):
-    """GetCorrPyramid (model_utils.py:199-221): GEMM + /sqrt(C) + 3x VALID 2x2 average pooling."""
+    """GetCorrPyramid (model_utils.py:199-221): GEMM + /sqrt(C) + 3x VALID 2x2 average pooling.  At 9 x 17 levels 1 and 2
+    (4 x 8, 2 x 4) start at float offsets that are not multiples of 4 while their rows are: the epilogue must not use
+    16-byte stores there."""
     from raft_b200 import capi
     from networks.model_utils import GetCorrPyramid
     g = torch.Generator().manual_seed(11)
