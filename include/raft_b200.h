@@ -204,6 +204,39 @@ int rb_upflow8_crop(const float* coords1, float* out, int B, int h, int w, float
 int rb_flow_fb_check(const float* flow_fw, const float* flow_bw, uint8_t* occ_fw, uint8_t* occ_bw,
                      int B, int H, int W, float flow_scale, float alpha1, float alpha2, void* stream);
 
+/* ---- F6: frame interpolation -- flow_utils.py:166-274 reverse_flow_avg_skip_static, batched, and the frame blend -----
+ * rb_flow_reverse: per sample of flow01 [B,H,W,2] fp32, bit for bit with the reference under numpy >= 2:
+ *  1. static(p) = every channel c has d_c < 10, d_c = uint8(bg - im0) (img_u8 = 1: wraps, like numpy's uint8) or
+ *     |fl32(bg - im0)| (img_u8 = 0); bg, im0: [B,H,W,img_channels], both or neither (neither: nothing is static);
+ *  2. f = fl32((static ? +inf : flow01) * time_step);
+ *  3. (px, py) = (double)f + (x, y); a source with an infinite or NaN coordinate is skipped (NaN: the reference raises);
+ *  4. target = (clamp(rint(px), 0, W-1), clamp(rint(py), 0, H-1)), rint rounding half to even like np.round;
+ *  5. each target sums -f over its sources in fp32 from +0.0, in source raster order, and counts them;
+ *  6. flow_t = fl32(sum / (double)count) where count > 0; multi = count > 1; empty = count == 0;
+ *  7. each empty pixel gets the fp32 mean, summed in the order up, down, left, right from +0.0, of the nearest
+ *     non-empty pixels above / below in its column and left / right in its row (+0.0 if there are none);
+ *  8. empty_eroded = 5x5 minimum of empty over the window clipped to the image (cv2.erode's default border).
+ * flow_t [B,H,W,2] fp32; empty, multi, empty_eroded, static_mask [B,H,W] uint8 (empty_eroded, static_mask nullable).
+ * Deterministic (no float atomics): a stable radix sort orders every target's sources; a target that every source of
+ * its frame hits is summed by one thread in O(H W).  The workspace (rb_flow_reverse_workspace_bytes) holds CUB's
+ * temporary storage too, so the call allocates nothing and is CUDA-graph capturable.  Null pointers, only one of bg /
+ * im0, non-finite time_step, B/H/W <= 0, B*H*W + 1 >= 2^32 and a workspace smaller than its fixed part -> RB_ERR_*
+ * before any CUDA call (the rest of the size check queries the device). */
+int rb_flow_reverse_workspace_bytes(int B, int H, int W, size_t* bytes);
+int rb_flow_reverse(const float* flow01, const void* bg, const void* im0, int img_u8, int img_channels, float time_step,
+                    float* flow_t, uint8_t* empty, uint8_t* multi, uint8_t* empty_eroded, uint8_t* static_mask,
+                    int B, int H, int W, void* workspace, size_t workspace_bytes, void* stream);
+/* rb_frame_synthesize: frames [2B,Hp,Wp,3] fp32 = [I0 | I1], read at rows [top, top+H) x cols [left, left+W);
+ * flow_t0, flow_t1 [B,H,W,2] (time t -> frame 0 / frame 1, pixels), empty0, empty1 [B,H,W] uint8 (rb_flow_reverse);
+ * out [B,H,W,3] fp32.  Per pixel p and frame k: q = (min(max(x + F.x, 0), W-1), likewise y; NaN -> 0), v_k = the
+ * bilinear sample of I_k at q per channel (the arithmetic of rb_flow_fb_check); w0 = empty0 ? 0 : 1-t,
+ * w1 = empty1 ? 0 : t, both 0 -> (1-t, t); out = (w0 v_0 + w1 v_1) / (w0 + w1).  Every operation is rounded on its own,
+ * left to right, so t = 0 gives I0 and t = 1 gives I1 exactly.  t outside [0, 1], null pointers, bad shapes or a crop
+ * outside the frames -> RB_ERR_* before any CUDA call. */
+int rb_frame_synthesize(const float* frames, int Hp, int Wp, int top, int left, const float* flow_t0,
+                        const float* flow_t1, const uint8_t* empty0, const uint8_t* empty1, float t, float* out,
+                        int B, int H, int W, void* stream);
+
 /* ---- F3 (input edge): dataflow/test_dataflow.py:56-61,96-97 + the SURVEY 8(d) shape policy ------------------
  * src: [B,H,W,3] device frames, BGR like cv2.imdecode -- fp32 in [0,1] (src_is_u8 = 0) or uint8 in [0,255]
  * (src_is_u8 = 1: x/255.0f, the reference's np.float32(x)/255.0, bit for bit).  dst: [B,H+pt+pb,W+pl+pr,3] fp32

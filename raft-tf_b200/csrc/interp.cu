@@ -1,0 +1,367 @@
+// F6: frame interpolation.  rb_flow_reverse is the reference's flow reversal (flow_utils.py:166-274,
+// reverse_flow_avg_skip_static) batched and bit for bit; rb_frame_synthesize warps both frames to time t and blends them.
+//
+// Reversal: every source pixel of frame 0 is moved by time_step * flow to its nearest target pixel, and each target
+// averages -time_step * flow over its sources in source raster order (the reference's loop order).  The fixed order
+// rules out float atomics: keys (target index) are radix-sorted with the source index as value -- a stable sort, so
+// every target's segment lists its sources in raster order -- and one thread per target sums its segment.  A target hit
+// by every source of its frame therefore costs one thread O(H W): inherent to the order the result is defined by.
+#define CCCL_DISABLE_NVTX
+#include <cub/device/device_radix_sort.cuh>
+#include <cub/device/device_scan.cuh>
+#include <math.h>
+
+#include "common.cuh"
+
+namespace rb {
+namespace {
+
+constexpr size_t kAlign = 256;
+
+inline size_t align_up(size_t n) { return (n + kAlign - 1) / kAlign * kAlign; }
+
+// workspace: per-target counts and segment offsets, keys and values before / after the sort, the scaled flow of every
+// source, the up/down neighbour count of the hole fill, then CUB's temporary storage
+struct ReverseWs {
+  size_t counts, offsets, keys_in, keys_out, vals_in, vals_out, fs, nfound, temp, fixed;
+};
+
+ReverseWs reverse_layout(size_t n) {
+  ReverseWs l;
+  size_t o = 0;
+  const size_t u32 = align_up(n * sizeof(uint32_t));
+  l.counts = o, o += u32;
+  l.offsets = o, o += u32;
+  l.keys_in = o, o += u32;
+  l.keys_out = o, o += u32;
+  l.vals_in = o, o += u32;
+  l.vals_out = o, o += u32;
+  l.fs = o, o += align_up(n * sizeof(float2));
+  l.nfound = o, o += align_up(n);
+  l.temp = o;
+  l.fixed = o;
+  return l;
+}
+
+int key_bits(size_t n) {  // keys are 0..n (n = skipped source)
+  int b = 1;
+  while (b < 32 && (size_t(1) << b) <= n) ++b;
+  return b;
+}
+
+// CUB's temporary storage for the sort and the scan (they run one after the other and share it)
+cudaError_t cub_temp_bytes(size_t n, size_t* bytes) {
+  size_t sort_b = 0, scan_b = 0;
+  const uint32_t* ci = nullptr;
+  uint32_t* o = nullptr;
+  cudaError_t e = cub::DeviceRadixSort::SortPairs(nullptr, sort_b, ci, o, ci, o, (uint32_t)n, 0, key_bits(n));
+  if (e != cudaSuccess) return e;
+  e = cub::DeviceScan::ExclusiveSum(nullptr, scan_b, ci, o, (uint32_t)n);
+  *bytes = align_up(sort_b > scan_b ? sort_b : scan_b);
+  return e;
+}
+
+// One thread per source pixel: static mask, scaled flow, target key; counts by integer atomics (order-free).
+__global__ void __launch_bounds__(256) reverse_keys_kernel(const float2* __restrict__ flow, const void* __restrict__ bg,
+                                                           const void* __restrict__ im0, int u8, int C, int H, int W,
+                                                           uint32_t n, float ts, uint32_t* __restrict__ counts,
+                                                           uint32_t* __restrict__ keys, uint32_t* __restrict__ vals,
+                                                           float2* __restrict__ fs, uint8_t* __restrict__ static_out) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const uint32_t hw = (uint32_t)H * W;
+  const int x = (int)(i % W), y = (int)((i / W) % H);
+  const uint32_t base = i - (i % hw);
+  bool st = false;
+  if (bg != nullptr) {  // static: every channel differs by < 10 (uint8: the wrapped difference, as numpy computes it)
+    st = true;
+    for (int c = 0; c < C; ++c) {
+      const size_t k = (size_t)i * C + c;
+      if (u8) {
+        const uint8_t d = (uint8_t)(static_cast<const uint8_t*>(bg)[k] - static_cast<const uint8_t*>(im0)[k]);
+        st = st && d < 10;
+      } else {
+        const float d = fabsf(__fsub_rn(static_cast<const float*>(bg)[k], static_cast<const float*>(im0)[k]));
+        st = st && d < 10.f;
+      }
+    }
+  }
+  if (static_out != nullptr) static_out[i] = st ? 1 : 0;
+  float2 f = st ? make_float2(INFINITY, INFINITY) : flow[i];
+  f.x = __fmul_rn(f.x, ts);
+  f.y = __fmul_rn(f.y, ts);
+  fs[i] = f;
+  // float32 + int64 arange promotes to float64 in the reference; +-inf is skipped there, NaN (where the reference
+  // raises) is skipped here
+  const double px = (double)f.x + x, py = (double)f.y + y;
+  uint32_t key = n;
+  if (isfinite(px) && isfinite(py)) {
+    const int rx = (int)fmin(fmax(rint(px), 0.0), (double)(W - 1));  // rint: half to even, like np.round
+    const int ry = (int)fmin(fmax(rint(py), 0.0), (double)(H - 1));
+    key = base + (uint32_t)ry * W + rx;
+    atomicAdd(&counts[key], 1u);
+  }
+  keys[i] = key;
+  vals[i] = i;
+}
+
+// One thread per target: its sources in raster order, -f summed in fp32 from +0.0, divided as the reference does
+// (fp32 sum / float64 count, rounded to fp32).
+__global__ void __launch_bounds__(256) reverse_average_kernel(const uint32_t* __restrict__ counts,
+                                                              const uint32_t* __restrict__ offsets,
+                                                              const uint32_t* __restrict__ src,
+                                                              const float2* __restrict__ fs, uint32_t n,
+                                                              float2* __restrict__ flow_t, uint8_t* __restrict__ empty,
+                                                              uint8_t* __restrict__ multi) {
+  const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= n) return;
+  const uint32_t c = counts[k], o = offsets[k];
+  float ax = 0.f, ay = 0.f;
+  constexpr uint32_t kBatch = 8;  // loads of a batch in flight together; the adds stay in order
+  uint32_t j = 0;
+  for (; j + kBatch <= c; j += kBatch) {
+    float2 f[kBatch];
+#pragma unroll
+    for (uint32_t u = 0; u < kBatch; ++u) f[u] = fs[src[o + j + u]];
+#pragma unroll
+    for (uint32_t u = 0; u < kBatch; ++u) {
+      ax = __fadd_rn(ax, -f[u].x);
+      ay = __fadd_rn(ay, -f[u].y);
+    }
+  }
+  for (; j < c; ++j) {
+    const float2 f = fs[src[o + j]];
+    ax = __fadd_rn(ax, -f.x);
+    ay = __fadd_rn(ay, -f.y);
+  }
+  if (c > 0) {
+    ax = __double2float_rn(__ddiv_rn((double)ax, (double)c));
+    ay = __double2float_rn(__ddiv_rn((double)ay, (double)c));
+  }
+  flow_t[k] = make_float2(ax, ay);
+  empty[k] = c == 0 ? 1 : 0;
+  multi[k] = c > 1 ? 1 : 0;
+}
+
+// Hole fill, pass 1: one thread per (sample, column) walks down (nearest non-empty above) and up (below).  An empty
+// pixel's flow_t holds the running sum (+0.0 + up) + down and nfound the neighbours found so far.  Only non-empty
+// pixels are read as neighbours, so the sums never see each other.
+__global__ void __launch_bounds__(128) fill_columns_kernel(float2* __restrict__ ft, const uint8_t* __restrict__ empty,
+                                                           uint8_t* __restrict__ nfound, int B, int H, int W) {
+  const int t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= B * W) return;
+  const int b = t / W, x = t % W;
+  const size_t col = (size_t)b * H * W + x;
+  bool have = false;
+  float2 last = make_float2(0.f, 0.f);
+  for (int y = 0; y < H; ++y) {
+    const size_t p = col + (size_t)y * W;
+    if (!empty[p]) {
+      have = true;
+      last = ft[p];
+    } else {
+      ft[p] = have ? make_float2(__fadd_rn(0.f, last.x), __fadd_rn(0.f, last.y)) : make_float2(0.f, 0.f);
+      nfound[p] = have ? 1 : 0;
+    }
+  }
+  have = false;
+  for (int y = H - 1; y >= 0; --y) {
+    const size_t p = col + (size_t)y * W;
+    if (!empty[p]) {
+      have = true;
+      last = ft[p];
+    } else if (have) {
+      const float2 s = ft[p];
+      ft[p] = make_float2(__fadd_rn(s.x, last.x), __fadd_rn(s.y, last.y));
+      nfound[p] += 1;
+    }
+  }
+}
+
+// Pass 2: one thread per (sample, row) adds the nearest non-empty pixel on the left, then the right, and divides by the
+// number found (fp32, correctly rounded); none found gives +0.0.
+__global__ void __launch_bounds__(128) fill_rows_kernel(float2* __restrict__ ft, const uint8_t* __restrict__ empty,
+                                                        uint8_t* __restrict__ nfound, int B, int H, int W) {
+  const int t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= B * H) return;
+  const size_t row = (size_t)t * W;
+  bool have = false;
+  float2 last = make_float2(0.f, 0.f);
+  for (int x = 0; x < W; ++x) {
+    const size_t p = row + x;
+    if (!empty[p]) {
+      have = true;
+      last = ft[p];
+    } else if (have) {
+      const float2 s = ft[p];
+      ft[p] = make_float2(__fadd_rn(s.x, last.x), __fadd_rn(s.y, last.y));
+      nfound[p] += 1;
+    }
+  }
+  have = false;
+  for (int x = W - 1; x >= 0; --x) {
+    const size_t p = row + x;
+    if (!empty[p]) {
+      have = true;
+      last = ft[p];
+      continue;
+    }
+    float2 s = ft[p];
+    int m = nfound[p];
+    if (have) {
+      s = make_float2(__fadd_rn(s.x, last.x), __fadd_rn(s.y, last.y));
+      ++m;
+    }
+    // the fp32 quotient through fp64 (double rounding is innocuous for division: 53 >= 2*24 + 2); __fdiv_rn's slow-path
+    // call would put this loop's state on the stack
+    ft[p] = m > 0 ? make_float2(__double2float_rn(__ddiv_rn((double)s.x, (double)m)),
+                                __double2float_rn(__ddiv_rn((double)s.y, (double)m)))
+                  : make_float2(0.f, 0.f);
+  }
+}
+
+// 5x5 minimum of `empty` over the window clipped to the image (cv2.erode's default border)
+__global__ void __launch_bounds__(256) erode5_kernel(const uint8_t* __restrict__ empty, uint8_t* __restrict__ out,
+                                                     int H, int W, uint32_t n) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const int x = (int)(i % W), y = (int)((i / W) % H);
+  const uint8_t* img = empty + (i - ((size_t)y * W + x));
+  uint8_t m = 1;
+  for (int yy = max(y - 2, 0); yy <= min(y + 2, H - 1); ++yy)
+    for (int xx = max(x - 2, 0); xx <= min(x + 2, W - 1); ++xx) m &= img[(size_t)yy * W + xx];
+  out[i] = m;
+}
+
+// One thread per output pixel: both frames sampled at p + F_tk(p) (clamped to the frame; NaN -> 0) with the bilinear
+// arithmetic of rb_flow_fb_check, blended by (1-t, t) with empty targets weighted 0.
+__global__ void __launch_bounds__(256) frame_synthesize_kernel(const float* __restrict__ frames, int Hp, int Wp, int top,
+                                                               int left, const float2* __restrict__ f0,
+                                                               const float2* __restrict__ f1,
+                                                               const uint8_t* __restrict__ e0,
+                                                               const uint8_t* __restrict__ e1, float t,
+                                                               float* __restrict__ out, int B, int H, int W) {
+  const size_t p = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  const size_t npix = (size_t)B * H * W;
+  if (p >= npix) return;
+  const int x = (int)(p % W), y = (int)((p / W) % H), b = (int)(p / ((size_t)H * W));
+  const float s = __fsub_rn(1.f, t);
+  float w0 = e0[p] ? 0.f : s, w1 = e1[p] ? 0.f : t;
+  if (w0 == 0.f && w1 == 0.f) w0 = s, w1 = t;
+  float v[2][3];
+  for (int k = 0; k < 2; ++k) {
+    const float2 F = (k == 0 ? f0 : f1)[p];
+    const float qx = fminf(fmaxf(__fadd_rn((float)x, F.x), 0.f), (float)(W - 1));
+    const float qy = fminf(fmaxf(__fadd_rn((float)y, F.y), 0.f), (float)(H - 1));
+    const int x0 = (int)floorf(qx), y0 = (int)floorf(qy);
+    const int x1 = min(x0 + 1, W - 1), y1 = min(y0 + 1, H - 1);
+    const float ax = __fsub_rn(qx, (float)x0), ay = __fsub_rn(qy, (float)y0);
+    const float cx = __fsub_rn(1.f, ax), cy = __fsub_rn(1.f, ay);
+    const float* img = frames + ((size_t)(k * B + b) * Hp + top) * Wp * 3 + (size_t)left * 3;
+    const float* r0 = img + (size_t)y0 * Wp * 3;
+    const float* r1 = img + (size_t)y1 * Wp * 3;
+    for (int c = 0; c < 3; ++c) {
+      const float t0 = __fadd_rn(__fmul_rn(cx, r0[x0 * 3 + c]), __fmul_rn(ax, r0[x1 * 3 + c]));
+      const float t1 = __fadd_rn(__fmul_rn(cx, r1[x0 * 3 + c]), __fmul_rn(ax, r1[x1 * 3 + c]));
+      v[k][c] = __fadd_rn(__fmul_rn(t0, cy), __fmul_rn(t1, ay));
+    }
+  }
+  const float den = __fadd_rn(w0, w1);
+  for (int c = 0; c < 3; ++c)
+    out[p * 3 + c] = __fdiv_rn(__fadd_rn(__fmul_rn(w0, v[0][c]), __fmul_rn(w1, v[1][c])), den);
+}
+
+}  // namespace
+}  // namespace rb
+
+using namespace rb;
+
+extern "C" int rb_flow_reverse_workspace_bytes(int B, int H, int W, size_t* bytes) {
+  RB_REQUIRE(bytes, RB_ERR_BAD_ARG, "rb_flow_reverse_workspace_bytes: null pointer");
+  RB_REQUIRE(B > 0 && H > 0 && W > 0, RB_ERR_BAD_SHAPE, "rb_flow_reverse_workspace_bytes: bad shape B=%d H=%d W=%d", B,
+             H, W);
+  const size_t n = (size_t)B * H * W;
+  RB_REQUIRE(n + 1 < (size_t(1) << 32), RB_ERR_BAD_SHAPE,
+             "rb_flow_reverse_workspace_bytes: B*H*W = %zu pixels: keys need B*H*W + 1 < 2^32", n);
+  size_t temp = 0;
+  RB_CHECK_CUDA(cub_temp_bytes(n, &temp));
+  *bytes = reverse_layout(n).fixed + temp;
+  return RB_OK;
+}
+
+extern "C" int rb_flow_reverse(const float* flow01, const void* bg, const void* im0, int img_u8, int img_channels,
+                               float time_step, float* flow_t, uint8_t* empty, uint8_t* multi, uint8_t* empty_eroded,
+                               uint8_t* static_mask, int B, int H, int W, void* workspace, size_t workspace_bytes,
+                               void* stream) {
+  RB_REQUIRE(flow01 && flow_t && empty && multi && workspace, RB_ERR_BAD_ARG, "rb_flow_reverse: null pointer");
+  RB_REQUIRE((bg == nullptr) == (im0 == nullptr), RB_ERR_BAD_ARG, "rb_flow_reverse: pass both bg and im0, or neither");
+  RB_REQUIRE(bg == nullptr || img_channels > 0, RB_ERR_BAD_SHAPE, "rb_flow_reverse: img_channels must be > 0 (got %d)",
+             img_channels);
+  RB_REQUIRE(isfinite(time_step), RB_ERR_BAD_ARG, "rb_flow_reverse: time_step must be finite (got %g)",
+             (double)time_step);
+  RB_REQUIRE(B > 0 && H > 0 && W > 0, RB_ERR_BAD_SHAPE, "rb_flow_reverse: bad shape B=%d H=%d W=%d", B, H, W);
+  const size_t n = (size_t)B * H * W;
+  RB_REQUIRE(n + 1 < (size_t(1) << 32), RB_ERR_BAD_SHAPE,
+             "rb_flow_reverse: B*H*W = %zu pixels: keys need B*H*W + 1 < 2^32", n);
+  const ReverseWs l = reverse_layout(n);
+  // the fixed part is known without CUDA; CUB's share needs a device query
+  RB_REQUIRE(workspace_bytes >= l.fixed, RB_ERR_WORKSPACE, "rb_flow_reverse: workspace of %zu bytes is too small",
+             workspace_bytes);
+  size_t temp = 0;
+  RB_CHECK_CUDA(cub_temp_bytes(n, &temp));
+  RB_REQUIRE(workspace_bytes >= l.fixed + temp, RB_ERR_WORKSPACE,
+             "rb_flow_reverse: workspace of %zu bytes is too small (need %zu)", workspace_bytes, l.fixed + temp);
+  char* ws = static_cast<char*>(workspace);
+  uint32_t* counts = reinterpret_cast<uint32_t*>(ws + l.counts);
+  uint32_t* offsets = reinterpret_cast<uint32_t*>(ws + l.offsets);
+  uint32_t* keys_in = reinterpret_cast<uint32_t*>(ws + l.keys_in);
+  uint32_t* keys_out = reinterpret_cast<uint32_t*>(ws + l.keys_out);
+  uint32_t* vals_in = reinterpret_cast<uint32_t*>(ws + l.vals_in);
+  uint32_t* vals_out = reinterpret_cast<uint32_t*>(ws + l.vals_out);
+  float2* fs = reinterpret_cast<float2*>(ws + l.fs);
+  uint8_t* nfound = reinterpret_cast<uint8_t*>(ws + l.nfound);
+  const cudaStream_t st = (cudaStream_t)stream;
+  const uint32_t n32 = (uint32_t)n;
+  const unsigned blocks = (unsigned)((n + 255) / 256);
+
+  RB_CHECK_CUDA(cudaMemsetAsync(counts, 0, n * sizeof(uint32_t), st));
+  reverse_keys_kernel<<<blocks, 256, 0, st>>>(reinterpret_cast<const float2*>(flow01), bg, im0, img_u8, img_channels, H,
+                                              W, n32, time_step, counts, keys_in, vals_in, fs, static_mask);
+  RB_CHECK_LAUNCH("reverse_keys_kernel");
+  size_t tb = temp;
+  RB_CHECK_CUDA(cub::DeviceScan::ExclusiveSum(ws + l.temp, tb, counts, offsets, n32, st));
+  tb = temp;
+  RB_CHECK_CUDA(cub::DeviceRadixSort::SortPairs(ws + l.temp, tb, keys_in, keys_out, vals_in, vals_out, n32, 0,
+                                                key_bits(n), st));
+  reverse_average_kernel<<<blocks, 256, 0, st>>>(counts, offsets, vals_out, fs, n32, reinterpret_cast<float2*>(flow_t),
+                                                 empty, multi);
+  RB_CHECK_LAUNCH("reverse_average_kernel");
+  fill_columns_kernel<<<(B * W + 127) / 128, 128, 0, st>>>(reinterpret_cast<float2*>(flow_t), empty, nfound, B, H, W);
+  RB_CHECK_LAUNCH("fill_columns_kernel");
+  fill_rows_kernel<<<(B * H + 127) / 128, 128, 0, st>>>(reinterpret_cast<float2*>(flow_t), empty, nfound, B, H, W);
+  RB_CHECK_LAUNCH("fill_rows_kernel");
+  if (empty_eroded != nullptr) {
+    erode5_kernel<<<blocks, 256, 0, st>>>(empty, empty_eroded, H, W, n32);
+    RB_CHECK_LAUNCH("erode5_kernel");
+  }
+  return RB_OK;
+}
+
+extern "C" int rb_frame_synthesize(const float* frames, int Hp, int Wp, int top, int left, const float* flow_t0,
+                                   const float* flow_t1, const uint8_t* empty0, const uint8_t* empty1, float t,
+                                   float* out, int B, int H, int W, void* stream) {
+  RB_REQUIRE(frames && flow_t0 && flow_t1 && empty0 && empty1 && out, RB_ERR_BAD_ARG,
+             "rb_frame_synthesize: null pointer");
+  RB_REQUIRE(t >= 0.f && t <= 1.f, RB_ERR_BAD_ARG, "rb_frame_synthesize: t must be in [0, 1] (got %g)", (double)t);
+  RB_REQUIRE(B > 0 && H > 0 && W > 0, RB_ERR_BAD_SHAPE, "rb_frame_synthesize: bad shape B=%d H=%d W=%d", B, H, W);
+  RB_REQUIRE(top >= 0 && left >= 0 && top + H <= Hp && left + W <= Wp, RB_ERR_BAD_SHAPE,
+             "rb_frame_synthesize: crop (%d, %d) + %dx%d outside the %dx%d frames", top, left, H, W, Hp, Wp);
+  const size_t npix = (size_t)B * H * W;
+  const size_t blocks = (npix + 255) / 256;
+  RB_REQUIRE(blocks <= 0x7fffffffu, RB_ERR_BAD_SHAPE, "rb_frame_synthesize: %zu pixels exceed one grid", npix);
+  frame_synthesize_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(
+      frames, Hp, Wp, top, left, reinterpret_cast<const float2*>(flow_t0), reinterpret_cast<const float2*>(flow_t1),
+      empty0, empty1, t, out, B, H, W);
+  RB_CHECK_LAUNCH("frame_synthesize_kernel");
+  return RB_OK;
+}

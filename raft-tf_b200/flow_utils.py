@@ -1,7 +1,8 @@
 """Flow colour coding used by the CLI (the reference's infer_raft.py:25,43 calls
 flow_utils.flow_to_color(flow, convert_to_bgr=True)).  Independent numpy implementation of the
 Middlebury colour wheel (Baker et al., ICCV 2007): same normalisation by the maximum radius
-(+1e-5) and floor(255*col) quantisation as the reference's flow_utils.py:95-121."""
+(+1e-5) and floor(255*col) quantisation as the reference's flow_utils.py:95-121.  reverse_flow_avg_skip_static is the
+reference's flow reversal (flow_utils.py:166-274) computed on the GPU; it imports torch only when called."""
 import numpy as np
 
 _SEGMENTS = (("RY", 15), ("YG", 6), ("GC", 4), ("CB", 11), ("BM", 13), ("MR", 6))
@@ -50,6 +51,37 @@ def flow_to_color(flow_uv, clip_flow=None, convert_to_bgr=False):
         col = np.where(inside, 1 - rad * (1 - col), col * 0.75)
         img[..., 2 - ch if convert_to_bgr else ch] = np.floor(255 * col)
     return img
+
+
+def reverse_flow_avg_skip_static(flow01_origin, bg, im0, time_step=1.0):
+    """The reference's flow_utils.py:166-274 on cuda:0, same name, arguments and 5-tuple: the flow 0 -> 1 projected to
+    time `time_step`, giving the flow from there back to frame 0 (rb_flow_reverse, bit for bit with the reference under
+    numpy >= 2).  flow01_origin: [H,W,2] float32; bg, im0: [H,W,C] uint8 or float32 (None for both: nothing static).
+    Returns numpy (flow10 float32 [H,W,2], empty uint8, uint8(count > 1), static_mask int64 [H,W,1], empty eroded by
+    5x5 uint8).  Differences: a NaN flow is skipped (the reference raises), and nothing is printed."""
+    import torch
+    from networks.utils import reverse_flow
+
+    flow = np.asarray(flow01_origin)
+    if flow.dtype != np.float32:
+        raise TypeError(f"reverse_flow_avg_skip_static: flow must be float32, got {flow.dtype}")
+    if flow.ndim != 3 or flow.shape[2] != 2:
+        raise ValueError(f"reverse_flow_avg_skip_static: flow must be [H,W,2], got {flow.shape}")
+    imgs = []
+    for im in (bg, im0):
+        if im is None:
+            imgs.append(None)
+            continue
+        im = np.asarray(im)
+        if im.dtype not in (np.uint8, np.float32):
+            raise TypeError(f"reverse_flow_avg_skip_static: images must be uint8 or float32, got {im.dtype}")
+        if im.ndim != 3 or im.shape[:2] != flow.shape[:2]:
+            raise ValueError(f"reverse_flow_avg_skip_static: images must be [H,W,C] with the flow's H, W, got {im.shape}")
+        imgs.append(torch.from_numpy(np.ascontiguousarray(im))[None].to("cuda:0"))
+    f = torch.from_numpy(np.ascontiguousarray(flow))[None].to("cuda:0")
+    out = reverse_flow(f, float(time_step), *imgs)
+    flow10, empty, multi, static, eroded = (t[0].cpu().numpy() for t in out)
+    return flow10, empty, multi, static.astype(np.int64)[..., None], eroded
 
 
 def write_flo(path, flow_uv):

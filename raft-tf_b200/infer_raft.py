@@ -11,7 +11,8 @@ Flags the reference parses but ignores (--gpu, --data, --out, -o) are accepted; 
 Extensions: --iters, --keep-size (replicate-pad to a multiple of 8 instead of resizing), --npy, --flo, and
 --bidirectional: also the flow im2 -> im1 (``raft_flow_raft-things_bw.png``, ``<npy>_bw.npy``, ``<flo>_bw.flo``) and the
 forward-backward occlusion masks ``raft_occ_fw.png`` / ``raft_occ_bw.png`` (0 consistent, 128 occluded, 255 leaves the
-frame), from one pass that encodes each frame once.
+frame), from one pass that encodes each frame once, and --interpolate T [T ...]: the frames at times T in [0, 1] between
+im1 (0) and im2 (1), written as ``raft_interp_<k>.png`` (k = position in the list).
 """
 import argparse
 import os
@@ -54,7 +55,11 @@ def main(argv=None):
     p.add_argument('--flo', default=None, help='extension: also save the flow as a Middlebury .flo file')
     p.add_argument('--bidirectional', action='store_true',
                    help='extension: also the backward flow and the forward-backward occlusion masks')
+    p.add_argument('--interpolate', type=float, nargs='+', default=None, metavar='T',
+                   help='extension: also write the frames at times T in [0, 1] between im1 and im2 (raft_interp_<k>.png)')
     args = p.parse_args(argv)
+    if args.interpolate and not all(0.0 <= t <= 1.0 for t in args.interpolate):
+        p.error('--interpolate: every T must be in [0, 1]')
     if args.mode != 'test':
         print(f"mode '{args.mode}' has no implementation in the reference either (infer_raft.py:71-95); nothing to do")
         return 0
@@ -82,6 +87,10 @@ def main(argv=None):
             np.save(_bw_path(args.npy), flow_bw[0])
         if args.flo:
             write_flo(_bw_path(args.flo), flow_bw[0])
+    if args.interpolate:
+        frames = model.interpolate(left, right, args.interpolate).cpu().numpy()
+        for k, frame in enumerate(frames):
+            cv2.imwrite(f"raft_interp_{k}.png", np.clip(np.rint(255.0 * frame[0]), 0, 255).astype(np.uint8))
     return 0
 
 

@@ -105,6 +105,19 @@ class RAFT(object):
         out = self.engine().forward_bidirectional(_as_tensor(input_left), _as_tensor(input_right), check=check)
         return tuple(None if t is None else t.clone() for t in out)
 
+    @torch.no_grad()
+    def interpolate(self, input_left, input_right, t=0.5):
+        """Extension (the reference computes the flow for frame interpolation and projects it to time t with
+        flow_utils.py:166 on the CPU): the frames at time t between left (t = 0) and right (t = 1).  One bidirectional
+        pass, then per t the flows from time t to both frames by the reference's flow reversal (rb_flow_reverse, bit for
+        bit) and a blend of both frames warped by them (rb_frame_synthesize; a frame whose reversed flow is empty at a
+        pixel gets weight 0 there).  Inputs as for ``forward``.  A float t in [0, 1] gives a fresh [B,H,W,3] fp32 tensor,
+        BGR in [0,1] (uint8 frames are divided by 255); a sequence of T times gives [T,B,H,W,3] from one pass.  t = 0
+        and t = 1 return the frames themselves exactly.  A t outside [0, 1] raises ValueError."""
+        scalar = np.ndim(t) == 0
+        out = self.engine().interpolate(_as_tensor(input_left), _as_tensor(input_right), [t] if scalar else list(t))
+        return out[0] if scalar else out
+
 
 def _as_tensor(x):
     t = torch.as_tensor(x)

@@ -53,3 +53,56 @@ def fb_consistency(flow_fw, flow_bw, alpha1=0.01, alpha2=0.5, flow_scale=1.0):
         capi.check(capi.lib.rb_flow_fb_check(capi.ptr(fw), capi.ptr(bw), capi.ptr(occ_fw), capi.ptr(occ_bw), b, H, W,
                                              float(flow_scale), float(alpha1), float(alpha2), capi.stream()))
     return occ_fw, occ_bw
+
+
+def reverse_flow(flow, time_step=1.0, bg=None, im0=None):
+    """The reference's flow_utils.py:166 reverse_flow_avg_skip_static on a batch of CUDA flows (rb_flow_reverse, bit for
+    bit): projects the [B,H,W,2] flow 0 -> 1 to time `time_step` and returns the flow from there back to frame 0.
+    bg, im0: optional [B,H,W,C] images (both or neither); pixels where every channel differs by < 10 are static and
+    skipped (uint8 pairs compare the wrapped uint8 difference, as numpy does; any other pair is compared in fp32).
+    Returns (flow_t [B,H,W,2] fp32, empty, multi, static, empty_eroded), the last four [B,H,W] uint8: no source
+    landed, more than one landed, the static mask, and empty eroded by a 5x5 window.  Empty pixels hold the mean of their
+    nearest non-empty neighbours up, down, left and right.  A NaN flow is skipped (the reference raises on it)."""
+    assert flow.dim() == 4 and flow.shape[-1] == 2, flow.shape
+    if (bg is None) != (im0 is None):
+        raise ValueError("reverse_flow: pass both bg and im0, or neither")
+    B, H, W, _ = flow.shape
+    f = flow.contiguous().float()
+    u8, C = 0, 0
+    if bg is not None:
+        assert bg.shape == im0.shape and bg.dim() == 4 and tuple(bg.shape[:3]) == (B, H, W), (bg.shape, im0.shape)
+        if bg.dtype == torch.uint8 and im0.dtype == torch.uint8:
+            u8 = 1
+        else:  # numpy promotes a uint8 / float32 pair to float32; the values are exact
+            bg, im0 = bg.float(), im0.float()
+        bg, im0, C = bg.contiguous(), im0.contiguous(), bg.shape[-1]
+    out = torch.empty_like(f)
+    empty, multi, static, eroded = (torch.empty(B, H, W, dtype=torch.uint8, device=f.device) for _ in range(4))
+    with torch.cuda.device(f.device):
+        nbytes = capi.size_query(capi.lib.rb_flow_reverse_workspace_bytes, B, H, W)
+        ws = torch.empty(nbytes, dtype=torch.uint8, device=f.device)
+        capi.check(capi.lib.rb_flow_reverse(capi.ptr(f), capi.ptr(bg), capi.ptr(im0), u8, C, float(time_step),
+                                            capi.ptr(out), capi.ptr(empty), capi.ptr(multi), capi.ptr(eroded),
+                                            capi.ptr(static), B, H, W, capi.ptr(ws), nbytes, capi.stream()))
+    return out, empty, multi, static, eroded
+
+
+def synthesize(frame0, frame1, flow_t0, flow_t1, empty0, empty1, t):
+    """Extension: the frame at time t in [0, 1] between [B,H,W,3] frames frame0 and frame1 (rb_frame_synthesize):
+    each frame sampled bilinearly at p + flow_tk(p) (the flows from time t to frame k, e.g. reverse_flow(flow_01, t) and
+    reverse_flow(flow_10, 1 - t)) and blended with weights 1 - t and t, a frame whose flow is empty at p weighted 0
+    (unless both are).  t = 0 gives frame0 and t = 1 gives frame1 exactly.  -> [B,H,W,3] fp32."""
+    t = float(t)
+    if not 0.0 <= t <= 1.0:
+        raise ValueError(f"synthesize: t must be in [0, 1] (got {t})")
+    assert frame0.shape == frame1.shape and frame0.dim() == 4 and frame0.shape[-1] == 3, (frame0.shape, frame1.shape)
+    B, H, W, _ = frame0.shape
+    assert flow_t0.shape == flow_t1.shape == (B, H, W, 2) and empty0.shape == empty1.shape == (B, H, W)
+    frames = torch.cat([frame0, frame1]).float().contiguous()
+    f0, f1 = flow_t0.contiguous().float(), flow_t1.contiguous().float()
+    e0, e1 = empty0.contiguous().to(torch.uint8), empty1.contiguous().to(torch.uint8)
+    out = torch.empty(B, H, W, 3, dtype=torch.float32, device=frames.device)
+    with torch.cuda.device(out.device):
+        capi.check(capi.lib.rb_frame_synthesize(capi.ptr(frames), H, W, 0, 0, capi.ptr(f0), capi.ptr(f1), capi.ptr(e0),
+                                                capi.ptr(e1), t, capi.ptr(out), B, H, W, capi.stream()))
+    return out

@@ -5,6 +5,8 @@ rb_update_set_state_cnet -> rb_raft_iterate (lookup + update block per iteration
 rb_upflow8, all replayed from ONE CUDA graph.  Mirrors RAFT.network_graph (networks/RAFT.py:78-109).
 forward_bidirectional runs both directions of B frame pairs as 2B pairs through the same path (each frame encoded once)
 and adds the forward-backward consistency check (rb_flow_fb_check, csrc/consistency.cu) to the same graph.
+interpolate runs the same bidirectional pass (without the check) from its own graph, then per time t two flow reversals
+and the frame blend (rb_flow_reverse, rb_frame_synthesize, csrc/interp.cu) eagerly on the same stream.
 The torch/cuDNN restatement of the encoders (encoders.Encoder) is a cross-check behind RAFT_B200_TORCH_ENCODERS=1.
 """
 from __future__ import annotations
@@ -19,8 +21,9 @@ from . import capi
 from .encoders import CudaEncoder, Encoder
 from .weights import pack_update_block
 
-# what one pass computes: L->R only (forward), both directions (forward_bidirectional), both plus the occlusion check
-FORWARD, BIDIRECTIONAL, BIDIRECTIONAL_CHECK = 0, 1, 2
+# what one pass computes: L->R only (forward), both directions (forward_bidirectional), both plus the occlusion check,
+# both directions for interpolate (which also holds the buffers of the per-t calls)
+FORWARD, BIDIRECTIONAL, BIDIRECTIONAL_CHECK, INTERPOLATE = 0, 1, 2, 3
 # forward-backward consistency thresholds of UnFlow (Meister et al. 2018): |f+b|^2 > a1 (|f|^2 + |b|^2) + a2
 FB_ALPHA1, FB_ALPHA2 = 0.01, 0.5
 # smallest frame side: the 4-level correlation pyramid needs a 1/8-resolution grid of at least 8 (level 3 is grid >> 3),
@@ -31,7 +34,7 @@ MIN_FRAME = 57
 class RaftEngine:
     # everything _ensure allocates for one (B, H, W, u8, mode); parked per mode so alternating modes re-captures nothing
     _STATE = ("pad", "h", "w", "Hp", "Wp", "pairs", "pyr_bytes", "pyramid", "cws_bytes", "corr_ws", "ws_bytes", "ws",
-              "coords1", "mask", "flow_up", "occ", "fmaps", "fmap1", "fmap2", "cmap", "images", "staged", "raw", "_shape",
+              "coords1", "mask", "flow_up", "occ", "rev_ws_bytes", "rev_ws", "flow_t", "empty_t", "fmaps", "fmap1", "fmap2", "cmap", "images", "staged", "raw", "_shape",
               "_graph")
 
     def __init__(self, params: Dict[str, np.ndarray], small: bool = False, iters: int = 20,
@@ -116,6 +119,13 @@ class RaftEngine:
         self.mask = None if self.small else torch.empty(NB, h, w, 576, dtype=torch.float32, device=d)
         self.flow_up = torch.empty(NB, H, W, 2, dtype=torch.float32, device=d)  # bidirectional: [L->R | R->L]
         self.occ = torch.empty(2 * B, H, W, dtype=torch.uint8, device=d) if mode == BIDIRECTIONAL_CHECK else None
+        if mode == INTERPOLATE:  # per t: flow and empty mask from time t to frame 0 ([0]) and to frame 1 ([1])
+            self.rev_ws_bytes = capi.size_query(lib.rb_flow_reverse_workspace_bytes, B, H, W)
+            self.rev_ws = torch.empty(self.rev_ws_bytes, dtype=torch.uint8, device=d)
+            self.flow_t = torch.empty(2, B, H, W, 2, dtype=torch.float32, device=d)
+            self.empty_t = torch.empty(2, 2, B, H, W, dtype=torch.uint8, device=d)  # [empty | multi]
+        else:
+            self.rev_ws_bytes, self.rev_ws, self.flow_t, self.empty_t = 0, None, None, None
         self.fmaps = torch.empty(NB + B, h, w, self.fdim, dtype=torch.float32, device=d)
         self.fmap1, self.fmap2 = self.fmaps[:NB], self.fmaps[B:]
         self.cmap = torch.empty(NB, h, w, self.hidden + self.ctx, dtype=torch.float32, device=d)
@@ -269,6 +279,39 @@ class RaftEngine:
         B = left.shape[0]
         occ = (self.occ[:B], self.occ[B:]) if check else (None, None)
         return (self.flow_up[:B], self.flow_up[B:]) + occ
+
+    @torch.no_grad()
+    def interpolate(self, left: torch.Tensor, right: torch.Tensor, ts) -> torch.Tensor:
+        """Frames at times ts (each in [0, 1]; 0 = left, 1 = right) between B frame pairs: one bidirectional pass (as
+        forward_bidirectional(check=False), from a graph of its own), then per t, eagerly on the same stream,
+        rb_flow_reverse(flow_fw, t) -> flow and empty mask from t to left, rb_flow_reverse(flow_bw, 1 - t) -> from t to
+        right, and rb_frame_synthesize on the padded frames the pass used.  raft-small's flow is in 1/8-resolution units,
+        so its time steps are 8t and 8(1 - t) (exact: scaling by 8 commutes with fp32 rounding).  Frames as for
+        forward().  Returns a fresh [T,B,H,W,3] fp32 tensor, BGR in [0,1] (uint8 frames are divided by 255 first)."""
+        ts = [float(t) for t in ts]
+        if not ts or not all(0.0 <= t <= 1.0 for t in ts):
+            raise ValueError(f"raft_b200: interpolation times must be a non-empty list in [0, 1] (got {ts})")
+        self._run_frames(left, right, INTERPOLATE)
+        B, H, W = left.shape[0], left.shape[1], left.shape[2]
+        out = torch.empty(len(ts), B, H, W, 3, dtype=torch.float32, device=self.device)
+        with torch.cuda.device(self.device):
+            for k, t in enumerate(ts):
+                self._interpolate_at(t, out[k])
+        return out
+
+    def _interpolate_at(self, t: float, out: torch.Tensor):
+        """The per-t work of interpolate on the flows of the last INTERPOLATE pass: two reversals and the blend into
+        out [B,H,W,3]."""
+        B, H, W = self._shape[:3]
+        s = 8.0 if self.small else 1.0
+        lib, st, ptr = capi.lib, capi.stream(), capi.ptr
+        for d, (flow, step) in enumerate(((self.flow_up[:B], s * t), (self.flow_up[B:], s * (1.0 - t)))):
+            capi.check(lib.rb_flow_reverse(ptr(flow), None, None, 0, 0, step, ptr(self.flow_t[d]), ptr(self.empty_t[0, d]),
+                                           ptr(self.empty_t[1, d]), None, None, B, H, W, ptr(self.rev_ws),
+                                           self.rev_ws_bytes, st))
+        capi.check(lib.rb_frame_synthesize(ptr(self.images), self.Hp, self.Wp, self.pad[0], self.pad[2],
+                                           ptr(self.flow_t[0]), ptr(self.flow_t[1]), ptr(self.empty_t[0, 0]),
+                                           ptr(self.empty_t[0, 1]), t, ptr(out), B, H, W, st))
 
     def _run_frames(self, left: torch.Tensor, right: torch.Tensor, mode: int):
         assert left.shape == right.shape and left.dim() == 4 and left.shape[-1] == 3 and left.dtype == right.dtype
