@@ -244,6 +244,17 @@ int rb_frame_synthesize(const float* frames, int Hp, int Wp, int top, int left, 
  * RAFT.input_preprocess (RAFT.py:53-59) is applied inside rb_encoder_forward. */
 int rb_frames_prepare(const void* src, int src_is_u8, float* dst, int B, int H, int W, int pad_top,
                       int pad_bottom, int pad_left, int pad_right, void* stream);
+/* rb_frames_resize: the reference's cv2.resize of every frame to the network size (test_dataflow.py:85-87), bit for
+ * bit with OpenCV 4.13's bilinear resize, then (uint8) the /255 of rb_frames_prepare and the replicate pad.
+ * src [B,H,W,3] uint8 or fp32, any H, W >= 1; dst [B,Ho+pad_top+pad_bottom,Wo+pad_left+pad_right,3] fp32.  One thread
+ * per output pixel, coefficients computed in-kernel (tests/resize_oracle.py restates both of cv2's algorithms).
+ * Null pointers, B/H/W/Ho/Wo <= 0, negative pads -> RB_ERR_* before any CUDA call; no allocation, no synchronisation. */
+int rb_frames_resize(const void* src, int src_is_u8, float* dst, int B, int H, int W, int Ho, int Wo, int pad_top,
+                     int pad_bottom, int pad_left, int pad_right, void* stream);
+/* rb_flow_resize: flow_utils.py:277-284 resize_flow for a batch: flow [B,H,W,2] fp32 -> dst [B,Ho,Wo,2], each channel
+ * resized like cv2's float bilinear resize, then u *= fl32(Wo / W) and v *= fl32(Ho / H) (numpy >= 2 float32 multiply).
+ * Argument errors as rb_frames_resize. */
+int rb_flow_resize(const float* flow, float* dst, int B, int H, int W, int Ho, int Wo, void* stream);
 
 /* ---- F1: BasicEncoder / SmallEncoder  networks/model_utils.py:61-105 (+ input_preprocess RAFT.py:53-59) --
  * norm: 0 = 'none', 1 = 'instance' (fnet), 2 = 'batch' (cnet of raft-things; folded into the convs at pack

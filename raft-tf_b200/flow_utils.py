@@ -2,7 +2,8 @@
 flow_utils.flow_to_color(flow, convert_to_bgr=True)).  Independent numpy implementation of the
 Middlebury colour wheel (Baker et al., ICCV 2007): same normalisation by the maximum radius
 (+1e-5) and floor(255*col) quantisation as the reference's flow_utils.py:95-121.  reverse_flow_avg_skip_static is the
-reference's flow reversal (flow_utils.py:166-274) computed on the GPU; it imports torch only when called."""
+reference's flow reversal (flow_utils.py:166-274) and resize_flow (flow_utils.py:277-284) its flow resize, both computed on
+the GPU; they import torch only when called."""
 import numpy as np
 
 _SEGMENTS = (("RY", 15), ("YG", 6), ("GC", 4), ("CB", 11), ("BM", 13), ("MR", 6))
@@ -82,6 +83,22 @@ def reverse_flow_avg_skip_static(flow01_origin, bg, im0, time_step=1.0):
     out = reverse_flow(f, float(time_step), *imgs)
     flow10, empty, multi, static, eroded = (t[0].cpu().numpy() for t in out)
     return flow10, empty, multi, static.astype(np.int64)[..., None], eroded
+
+
+def resize_flow(flow, dW, dH):
+    """The reference's flow_utils.py:277-284 on cuda:0, same name, arguments and return value: [H,W,2] float32 numpy
+    flow -> [dH,dW,2] float32, each channel resized like cv2.resize and u, v scaled by dW / W and dH / H
+    (rb_flow_resize, bit for bit with the reference under numpy >= 2)."""
+    import torch
+    from networks.utils import resize_flow as _resize_flow
+
+    flow = np.asarray(flow)
+    if flow.dtype != np.float32:
+        raise TypeError(f"resize_flow: flow must be float32, got {flow.dtype}")
+    if flow.ndim != 3 or flow.shape[2] != 2:
+        raise ValueError(f"resize_flow: flow must be [H,W,2], got {flow.shape}")
+    f = torch.from_numpy(np.ascontiguousarray(flow))[None].to("cuda:0")
+    return _resize_flow(f, (int(dH), int(dW)))[0].cpu().numpy()
 
 
 def write_flo(path, flow_uv):

@@ -5,14 +5,15 @@ raft_b200 CUDA engine -- no TensorFlow, no tensorpack.
     python infer_raft.py --im1 frame_0016.png --im2 frame_0017.png --load release_weight/raft-things.npz [--small]
 
 Like the reference it decodes BGR with OpenCV, resizes both frames to 432x1024 (bilinear cv2.resize,
-dataflow/test_dataflow.py:85-87), scales to [0,1], runs 20 iterations and writes the colour-coded flow
+dataflow/test_dataflow.py:85-87; here on the GPU from the uint8 frames, bit for bit), scales to [0,1], runs 20 iterations and writes the colour-coded flow
 to ``raft_flow_raft-things.png`` in the working directory (regardless of --small, infer_raft.py:44).
 Flags the reference parses but ignores (--gpu, --data, --out, -o) are accepted; ``--batch`` stays 1.
 Extensions: --iters, --keep-size (replicate-pad to a multiple of 8 instead of resizing), --npy, --flo, and
 --bidirectional: also the flow im2 -> im1 (``raft_flow_raft-things_bw.png``, ``<npy>_bw.npy``, ``<flo>_bw.flo``) and the
 forward-backward occlusion masks ``raft_occ_fw.png`` / ``raft_occ_bw.png`` (0 consistent, 128 occluded, 255 leaves the
 frame), from one pass that encodes each frame once, and --interpolate T [T ...]: the frames at times T in [0, 1] between
-im1 (0) and im2 (1), written as ``raft_interp_<k>.png`` (k = position in the list).
+im1 (0) and im2 (1), written as ``raft_interp_<k>.png`` (k = position in the list), and --native-flow: the written
+flow(s) resized back to im1's size with the reference's flow_utils.resize_flow (no effect with --keep-size).
 """
 import argparse
 import os
@@ -23,18 +24,29 @@ import numpy as np
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 
 
+def _decode(path):
+    import cv2
+    with open(path, "rb") as f:
+        img = cv2.imdecode(np.asarray(bytearray(f.read()), dtype="uint8"), cv2.IMREAD_COLOR)  # BGR
+    if img is None:
+        raise FileNotFoundError(path)
+    return img
+
+
 def read_pair(im1, im2, size):
     import cv2
     out = []
     for path in (im1, im2):
-        with open(path, "rb") as f:
-            img = cv2.imdecode(np.asarray(bytearray(f.read()), dtype="uint8"), cv2.IMREAD_COLOR)  # BGR
-        if img is None:
-            raise FileNotFoundError(path)
+        img = _decode(path)
         if size is not None:
             img = cv2.resize(img, dsize=(size[1], size[0]))
         out.append(np.float32(img) / 255.0)
     return out[0][None], out[1][None]
+
+
+def decode_pair(im1, im2):
+    """Both frames as decoded (BGR uint8, their own size), [1,H,W,3] each: the engine resizes and scales them."""
+    return tuple(_decode(path)[None] for path in (im1, im2))
 
 
 def main(argv=None):
@@ -57,6 +69,8 @@ def main(argv=None):
                    help='extension: also the backward flow and the forward-backward occlusion masks')
     p.add_argument('--interpolate', type=float, nargs='+', default=None, metavar='T',
                    help='extension: also write the frames at times T in [0, 1] between im1 and im2 (raft_interp_<k>.png)')
+    p.add_argument('--native-flow', action='store_true',
+                   help="extension: resize the written flow(s) back to im1's size (flow_utils.resize_flow)")
     args = p.parse_args(argv)
     if args.interpolate and not all(0.0 <= t <= 1.0 for t in args.interpolate):
         p.error('--interpolate: every T must be in [0, 1]')
@@ -65,13 +79,25 @@ def main(argv=None):
         return 0
     from networks import RAFT
     import cv2
-    from flow_utils import flow_to_color, write_flo
-    left, right = read_pair(args.im1, args.im2, None if args.keep_size else (432, 1024))
-    model = RAFT.RAFT(left.shape[1:], args, iters=args.iters).load(args.load)
+    from flow_utils import flow_to_color, resize_flow, write_flo
+    if args.keep_size:
+        left, right = read_pair(args.im1, args.im2, None)
+        model = RAFT.RAFT(left.shape[1:], args, iters=args.iters).load(args.load)
+    else:  # the reference's 432x1024 (infer_raft.py:69,76), resized and scaled on the GPU
+        left, right = decode_pair(args.im1, args.im2)
+        native = left.shape[1:3]
+        if left.shape != right.shape:  # one engine pass takes one frame size: resize such a pair on the host, as before
+            left, right = read_pair(args.im1, args.im2, (432, 1024))
+        model = RAFT.RAFT((432, 1024, 3), args, iters=args.iters, input_size=(432, 1024)).load(args.load)
     if args.bidirectional:
         flow, flow_bw, occ_fw, occ_bw = (t.cpu().numpy() for t in model.forward_bidirectional(left, right))
     else:
         flow = model.forward(left, right).cpu().numpy()
+    if args.native_flow and not args.keep_size:
+        H, W = native
+        flow = resize_flow(flow[0], W, H)[None]
+        if args.bidirectional:
+            flow_bw = resize_flow(flow_bw[0], W, H)[None]
     print(0, flow.shape)
     cv2.imwrite("raft_flow_raft-things.png", flow_to_color(flow[0], convert_to_bgr=True))
     if args.npy:

@@ -5,7 +5,8 @@ contract (returns 0.0 and publishes the result under the name ``flow_result``, R
 ``forward`` is the direct call.  Extensions over the reference (which hard-codes them, SURVEY fact
 5): ``iters``, ``batch`` and the image shape are honoured as parameters; inputs whose H/W are not
 multiples of 8 are replicate-padded and the flow cropped back (the reference itself cannot run such
-shapes, SURVEY fact 6)."""
+shapes, SURVEY fact 6).  ``input_size=(Ho, Wo)`` gives the reference's input semantics instead: frames of any
+size are resized to Ho x Wo on the GPU, bit for bit like the cv2.resize of its test dataflow."""
 import numpy as np
 import torch
 
@@ -21,7 +22,7 @@ class RAFT(object):
     weight_decay = 1e-5          # vestigial in the reference too (RAFT.py:14)
     data_format = 'NHWC'
 
-    def __init__(self, image_shape, args, iters=20, batch=1, device=None, volume_free=None):
+    def __init__(self, image_shape, args, iters=20, batch=1, device=None, volume_free=None, input_size=None):
         self.dropout = 0.0
         self.corr_radius = 4
         self.hidden_dim = 128
@@ -37,6 +38,8 @@ class RAFT(object):
             self.corr_radius = 3
         self.device = torch.device(device if device is not None else 'cuda:0')
         self.volume_free = volume_free  # extension (SURVEY 8(f) F2): None = RAFT_B200_VOLUME_FREE env, default off
+        # extension: (Ho, Wo) the frames are resized to on the GPU (test_dataflow.py:85-87), None = their own size
+        self.input_size = None if input_size is None else (int(input_size[0]), int(input_size[1]))
         self.flow_result = None
         self._engine = None
         self._params = None
@@ -80,7 +83,7 @@ class RAFT(object):
             if self._params is None:
                 raise RuntimeError("RAFT.load(<npz>) must be called before inference")
             self._engine = RaftEngine(self._params, small=self.small, iters=self.iters, device=self.device,
-                                      volume_free=self.volume_free)
+                                      volume_free=self.volume_free, input_size=self.input_size)
         return self._engine
 
     # -- inference ---------------------------------------------------------------------------------
@@ -89,7 +92,9 @@ class RAFT(object):
         """[B,H,W,3] frames, BGR like the reference -- fp32 in [0,1] (the reference's placeholders, RAFT.py:45-51) or
         uint8 in [0,255] (extension: the /255 of test_dataflow.py:96-97 then runs on the GPU); numpy or torch, host or
         CUDA -> [B,H,W,2] torch CUDA flow (a fresh tensor per call, like a session.run result).  H, W that are not
-        multiples of 8 are replicate-padded and the flow cropped back, both inside the engine's own kernels."""
+        multiples of 8 are replicate-padded and the flow cropped back, both inside the engine's own kernels.  With
+        input_size the frames may have any size: they are resized to input_size first (rb_frames_resize, in the same
+        CUDA graph) and the flow is at input_size, as in the reference; flow_utils.resize_flow takes it back."""
         flow = self.engine().forward(_as_tensor(input_left), _as_tensor(input_right))
         return flow.clone()
 

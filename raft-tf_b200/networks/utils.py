@@ -106,3 +106,32 @@ def synthesize(frame0, frame1, flow_t0, flow_t1, empty0, empty1, t):
         capi.check(capi.lib.rb_frame_synthesize(capi.ptr(frames), H, W, 0, 0, capi.ptr(f0), capi.ptr(f1), capi.ptr(e0),
                                                 capi.ptr(e1), t, capi.ptr(out), B, H, W, capi.stream()))
     return out
+
+
+def resize_frames(frames, size, pad=(0, 0, 0, 0)):
+    """The reference's cv2.resize of frames to size = (Ho, Wo) (test_dataflow.py:85-87), bit for bit, on [B,H,W,3]
+    CUDA frames: uint8 (then divided by 255 like test_dataflow.py:96-97) or fp32 -> [B,Ho,Wo,3] fp32, replicate-padded
+    by pad = (top, bottom, left, right) (rb_frames_resize)."""
+    assert frames.dim() == 4 and frames.shape[-1] == 3 and frames.dtype in (torch.uint8, torch.float32), frames.shape
+    frames = frames.contiguous()
+    B, H, W, _ = frames.shape
+    Ho, Wo = int(size[0]), int(size[1])
+    t, b, l, r = (int(p) for p in pad)
+    out = torch.empty(B, Ho + t + b, Wo + l + r, 3, dtype=torch.float32, device=frames.device)
+    with torch.cuda.device(frames.device):
+        capi.check(capi.lib.rb_frames_resize(capi.ptr(frames), int(frames.dtype == torch.uint8), capi.ptr(out), B, H, W,
+                                             Ho, Wo, t, b, l, r, capi.stream()))
+    return out
+
+
+def resize_flow(flow, size):
+    """The reference's flow_utils.resize_flow (flow_utils.py:277-284) on [B,H,W,2] fp32 CUDA flows: both channels
+    resized to size = (Ho, Wo) like cv2.resize, u scaled by Wo / W and v by Ho / H -> [B,Ho,Wo,2] (rb_flow_resize)."""
+    assert flow.dim() == 4 and flow.shape[-1] == 2 and flow.dtype == torch.float32, (flow.shape, flow.dtype)
+    flow = flow.contiguous()
+    B, H, W, _ = flow.shape
+    Ho, Wo = int(size[0]), int(size[1])
+    out = torch.empty(B, Ho, Wo, 2, dtype=torch.float32, device=flow.device)
+    with torch.cuda.device(flow.device):
+        capi.check(capi.lib.rb_flow_resize(capi.ptr(flow), capi.ptr(out), B, H, W, Ho, Wo, capi.stream()))
+    return out

@@ -68,6 +68,8 @@ SIGNATURES = {
     "rb_flow_reverse": (_i, [_vp, _vp, _vp, _i, _i, _f, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _vp, _sz, _vp]),
     "rb_frame_synthesize": (_i, [_vp, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _f, _vp, _i, _i, _i, _vp]),
     "rb_frames_prepare": (_i, [_vp, _i, _vp, _i, _i, _i, _i, _i, _i, _i, _vp]),
+    "rb_frames_resize": (_i, [_vp, _i, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp]),
+    "rb_flow_resize": (_i, [_vp, _vp, _i, _i, _i, _i, _i, _vp]),
     "rb_encoder_num_convs": (_i, [_i]),
     "rb_encoder_conv_name": (C.c_char_p, [_i, _i]),
     "rb_encoder_norm_name": (C.c_char_p, [_i, _i]),

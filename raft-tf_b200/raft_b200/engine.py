@@ -7,12 +7,14 @@ forward_bidirectional runs both directions of B frame pairs as 2B pairs through 
 and adds the forward-backward consistency check (rb_flow_fb_check, csrc/consistency.cu) to the same graph.
 interpolate runs the same bidirectional pass (without the check) from its own graph, then per time t two flow reversals
 and the frame blend (rb_flow_reverse, rb_frame_synthesize, csrc/interp.cu) eagerly on the same stream.
+With input_size set, every mode first resizes the frames to that size like the reference's cv2.resize (rb_frames_resize,
+csrc/resize.cu, in the graph in place of rb_frames_prepare), and its outputs come back at that size.
 The torch/cuDNN restatement of the encoders (encoders.Encoder) is a cross-check behind RAFT_B200_TORCH_ENCODERS=1.
 """
 from __future__ import annotations
 
 import os
-from typing import Dict, Optional
+from typing import Dict, Optional, Tuple
 
 import numpy as np
 import torch
@@ -33,15 +35,23 @@ MIN_FRAME = 57
 
 class RaftEngine:
     # everything _ensure allocates for one (B, H, W, u8, mode); parked per mode so alternating modes re-captures nothing
-    _STATE = ("pad", "h", "w", "Hp", "Wp", "pairs", "pyr_bytes", "pyramid", "cws_bytes", "corr_ws", "ws_bytes", "ws",
-              "coords1", "mask", "flow_up", "occ", "rev_ws_bytes", "rev_ws", "flow_t", "empty_t", "fmaps", "fmap1", "fmap2", "cmap", "images", "staged", "raw", "_shape",
+    _STATE = ("_key", "src_hw", "pad", "h", "w", "Hp", "Wp", "pairs", "pyr_bytes", "pyramid", "cws_bytes", "corr_ws",
+              "ws_bytes", "ws", "coords1", "mask", "flow_up", "occ", "rev_ws_bytes", "rev_ws", "flow_t", "empty_t", "fmaps", "fmap1", "fmap2", "cmap", "images", "staged", "raw", "_shape",
               "_graph")
 
     def __init__(self, params: Dict[str, np.ndarray], small: bool = False, iters: int = 20,
                  device: Optional[torch.device] = None, use_graph: bool = True, math_mode: int = capi.RB_MATH_TC,
-                 volume_free: Optional[bool] = None):
+                 volume_free: Optional[bool] = None, input_size: Optional[Tuple[int, int]] = None):
+        if input_size is not None:
+            input_size = (int(input_size[0]), int(input_size[1]))
+            if min(input_size) < MIN_FRAME:
+                raise ValueError(f"raft_b200: input_size {input_size[0]}x{input_size[1]} is too small: frames must be at "
+                                 f"least {MIN_FRAME} pixels on each side")
         if not torch.cuda.is_available():
             raise RuntimeError("raft_b200 needs a CUDA device (no CPU fallback)")
+        # network size (Ho, Wo): frames of any size are resized to it on the GPU like the reference's test dataflow
+        # (cv2.resize, test_dataflow.py:85-87); None runs frames at their own size (padded to a multiple of 8)
+        self.input_size = input_size
         self.device = torch.device(device if device is not None else "cuda:0")
         self.small, self.iters = bool(small), int(iters)
         self.hidden, self.ctx, self.radius, self.fdim = (96, 64, 3, 128) if small else (128, 128, 4, 256)
@@ -67,9 +77,10 @@ class RaftEngine:
         # the bidirectional pass runs the context encoder on 2B frames, forward on B: a twin with its own workspace keeps
         # the workspace each mode's CUDA graph was captured with (the feature encoder sees 2B frames in both modes)
         self.cnet_bidir = self.cnet if self.torch_encoders else self.cnet.with_own_workspace()
-        self._shape = None
+        self._shape = None  # (B, H, W, u8, mode) at the size the network runs (input_size when set)
+        self._key = None    # (B, H, W, u8, mode) at the frames' own size
         self._graph = None
-        self._parked = {}  # (B, H, W, u8, mode) -> buffers and graph of the other modes at the current frame size
+        self._parked = {}  # _key -> buffers and graph of the other modes at the current frame size
         self._enc_stream = None   # forked stream of the context encoder (encode())
         self._capture_stream = None  # CUDA-graph capture stream on this engine's device (run())
         self._cnet_pending = False
@@ -82,16 +93,25 @@ class RaftEngine:
         back by the upsampling kernel -- the reference itself cannot run such shapes (SURVEY fact 6).
 
         In the bidirectional modes the hot path runs 2B pairs, (L_i -> R_i) then (R_i -> L_i): fmaps holds 3B feature
-        maps [fL | fR | fL], so fmap1 = fmaps[:2B] and fmap2 = fmaps[B:] are both contiguous views."""
+        maps [fL | fR | fL], so fmap1 = fmaps[:2B] and fmap2 = fmaps[B:] are both contiguous views.
+
+        With input_size the frames' H x W (any size >= 1) only sizes the staging buffer; everything else is allocated
+        for input_size, and the parking key keeps the frames' own size, so a new source size never finds a graph
+        captured for another one."""
         key = (B, H, W, u8, mode)
-        if self._shape == key:
+        if self._key == key:
             return
+        src_hw = (H, W)
+        if self.input_size is not None:
+            if H < 1 or W < 1:
+                raise ValueError(f"raft_b200: empty {H}x{W} frames")
+            H, W = self.input_size
         if H < MIN_FRAME or W < MIN_FRAME:  # refused here, before the encoders run or any buffer is allocated
             raise ValueError(f"raft_b200: {H}x{W} frames are too small: frames must be at least {MIN_FRAME} pixels on each "
                              "side (a 1/8-resolution grid of at least 8x8 for the 4-level correlation pyramid)")
         # alternating modes on one frame size keeps every mode's buffers and CUDA graph; a new frame size drops them
-        if self._shape is not None:
-            self._parked[self._shape] = {k: getattr(self, k) for k in self._STATE}
+        if self._key is not None:
+            self._parked[self._key] = {k: getattr(self, k) for k in self._STATE}
         self._parked = {k: v for k, v in self._parked.items() if k[:4] == key[:4]}
         if key in self._parked:
             self.__dict__.update(self._parked.pop(key))
@@ -130,11 +150,13 @@ class RaftEngine:
         self.fmap1, self.fmap2 = self.fmaps[:NB], self.fmaps[B:]
         self.cmap = torch.empty(NB, h, w, self.hidden + self.ctx, dtype=torch.float32, device=d)
         self.images = torch.empty(2 * B, Hp, Wp, 3, dtype=torch.float32, device=d)  # [left | right], [0,1], padded
-        # staging buffer of the raw frames (uint8 or unpadded fp32); fp32 frames that need no padding go straight
-        # into self.images
-        self.staged = bool(u8 or ph or pw)
-        self.raw = torch.empty(2 * B, H, W, 3, dtype=torch.uint8 if u8 else torch.float32, device=d) if self.staged else None
-        self._shape = key
+        # staging buffer of the raw frames (uint8 or unpadded fp32, at the frames' own size); fp32 frames that need no
+        # resize and no padding go straight into self.images
+        self.staged = bool(u8 or ph or pw or self.input_size is not None)
+        self.raw = torch.empty(2 * B, *src_hw, 3, dtype=torch.uint8 if u8 else torch.float32, device=d) if self.staged else None
+        self.src_hw = src_hw
+        self._key = key
+        self._shape = (B, H, W, u8, mode)
         self._graph = None
 
     # ---- stages --------------------------------------------------------------------------------
@@ -153,7 +175,10 @@ class RaftEngine:
         cnet, cframes = (self.cnet_bidir, self.images) if bidir else (self.cnet, self.images[:B])
         fout = self.fmaps[:2 * B]  # [fL | fR]
         capi.check(capi.lib.rb_set_math_mode(self.math_mode))  # per-thread library state: set before ANY kernel of ours
-        if self.staged:  # F3: u8 -> fp32 /255 and replicate padding in one pass (csrc/frames.cu)
+        if self.input_size is not None:  # F3: cv2 resize, u8 -> fp32 /255 and replicate padding in one pass (csrc/resize.cu)
+            capi.check(capi.lib.rb_frames_resize(capi.ptr(self.raw), int(u8), capi.ptr(self.images), 2 * B, *self.src_hw,
+                                                 H, W, *self.pad, capi.stream()))
+        elif self.staged:  # F3: u8 -> fp32 /255 and replicate padding in one pass (csrc/frames.cu)
             capi.check(capi.lib.rb_frames_prepare(capi.ptr(self.raw), int(u8), capi.ptr(self.images), 2 * B, H, W,
                                                   *self.pad, capi.stream()))
         if self.torch_encoders:
@@ -259,8 +284,9 @@ class RaftEngine:
     def forward(self, left: torch.Tensor, right: torch.Tensor) -> torch.Tensor:
         """left/right: [B,H,W,3] frames, BGR like the reference: fp32 in [0,1] (RAFT.inputs(), RAFT.py:45-51) or
         uint8 in [0,255] (what cv2.imdecode yields, test_dataflow.py:56-61; the /255 then happens on the GPU).  Host
-        (ideally pinned) or CUDA tensors; any H, W >= 57 (MIN_FRAME; smaller frames raise ValueError).  Returns the
-        [B,H,W,2] flow -- the engine-owned buffer itself, overwritten by the next call (networks.RAFT.RAFT.forward hands
+        (ideally pinned) or CUDA tensors; any H, W >= 57 (MIN_FRAME; smaller frames raise ValueError), or any size
+        with input_size set, which resizes them to input_size first.  Returns the [B,H,W,2] flow (at input_size when
+        set) -- the engine-owned buffer itself, overwritten by the next call (networks.RAFT.RAFT.forward hands
         out a copy)."""
         self._run_frames(left, right, FORWARD)
         return self.flow_up
@@ -292,7 +318,7 @@ class RaftEngine:
         if not ts or not all(0.0 <= t <= 1.0 for t in ts):
             raise ValueError(f"raft_b200: interpolation times must be a non-empty list in [0, 1] (got {ts})")
         self._run_frames(left, right, INTERPOLATE)
-        B, H, W = left.shape[0], left.shape[1], left.shape[2]
+        B, H, W = self._shape[:3]
         out = torch.empty(len(ts), B, H, W, 3, dtype=torch.float32, device=self.device)
         with torch.cuda.device(self.device):
             for k, t in enumerate(ts):
