@@ -109,7 +109,6 @@ struct ConvParams {
   // (The iteration-invariant `inp` slice of the GRU inputs is convolved once per pair and skipped afterwards.)
   int ck_begin, ck_count, ck_skip_at, ck_skip;
   const float* addend;  // optional fp32 [pixel][cout] added to the accumulator before bias/activation
-  int pdl_early;
   const float* flow_tail;  // EPI_ACT, 16-channel epilogue: coords1; the last two channels are written as flow = coords1 - grid
   double* stat_part;  // EPI_F32 + tensor-core wide epilogue: per-(sample, strip, channel) sum / sum of squares of the
   int stat_strips;    // stored values, [B][strips][2][cout] (strip = 4 * tile-in-image + lane quarter); encoder.cu

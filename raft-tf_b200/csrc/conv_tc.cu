@@ -95,7 +95,6 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
   const int first = splitk ? (int)(blockIdx.x >> 1) : (int)blockIdx.x;  // first work item of this CTA (pair)
   const int stride = splitk ? (int)(gridDim.x >> 1) : (int)gridDim.x;
   if (dbg && threadIdx.x == 0) dbg[1] = gtime_ns();
-  if (p.pdl_early) asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
   // Programmatic dependent launch: this kernel may have been started while its predecessor is still running.  Everything
   // up to here and the WEIGHT tiles of the first ring stages are independent of it; `griddepcontrol.wait` (no-op without
   // the launch attribute) is executed by the producer before its first activation load and by the consumers before
@@ -349,16 +348,8 @@ int make_tmap(CUtensorMap* out, const void* base, int rank, const uint64_t* dims
   for (int i = 0; i + 1 < rank; ++i) gstr[i] = strides_bytes[i];
   const CUtensorMapDataType dt = kind == TMAP_F16_SW128 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
   const CUtensorMapSwizzle sw = kind == TMAP_F16_SW128 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B;
-  // L2 promotion: 256-byte requests suit the dense 128-byte operand rows of the GEMM tiles; the lookup's 64-byte patch
-  // rows are a gather (r01: 1.86x the algorithmic DRAM bytes) -> none.  RAFT_B200_LOOKUP_L2PROMO = 0/64/128/256: A/B knob.
-  CUtensorMapL2promotion promo = CU_TENSOR_MAP_L2_PROMOTION_L2_256B;
-  if (kind == TMAP_F32_SW64_GATHER) {
-    static const int env = getenv("RAFT_B200_LOOKUP_L2PROMO") ? atoi(getenv("RAFT_B200_LOOKUP_L2PROMO")) : 0;
-    promo = env == 256 ? CU_TENSOR_MAP_L2_PROMOTION_L2_256B : env == 128 ? CU_TENSOR_MAP_L2_PROMOTION_L2_128B
-            : env == 64 ? CU_TENSOR_MAP_L2_PROMOTION_L2_64B : CU_TENSOR_MAP_L2_PROMOTION_NONE;
-  }
   CUresult r = fn(out, dt, (cuuint32_t)rank, const_cast<void*>(base), gdim, gstr, bx, es, CU_TENSOR_MAP_INTERLEAVE_NONE, sw,
-                  promo, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+                  CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   RB_REQUIRE(r == CUDA_SUCCESS, RB_ERR_CUDA,
              "cuTensorMapEncodeTiled failed (%d): rank %d dims [%llu,%llu,%llu,%llu] box [%u,%u,%u,%u]", (int)r, rank,
              (unsigned long long)dims[0], (unsigned long long)(rank > 1 ? dims[1] : 0),
@@ -420,11 +411,10 @@ struct ConvRecord {
 static thread_local ConvOverride g_override = {0, 0, 0, 0};
 static thread_local ConvRecord g_record = {0, 0, 0, 0, 0, 0, 0};
 
-// Ring depth of a launch: RAFT_B200_TC_STAGES / the test hook may lower it, but never below 2 -- a consumer hands a stage
-// back only after it has issued the next one (wgmma_wait<1>), so a one-stage ring deadlocks any conv with two k-iterations.
+// Ring depth of a launch: the test hook may lower it, but never below 2 -- a consumer hands a stage back only after it has
+// issued the next one (wgmma_wait<1>), so a one-stage ring deadlocks any conv with two k-iterations.
 static int ring_stages(int max_stages) {
-  static const int env_stages = getenv("RAFT_B200_TC_STAGES") ? atoi(getenv("RAFT_B200_TC_STAGES")) : 0;  // tuning knob
-  const int req = g_override.stages > 0 ? g_override.stages : env_stages;
+  const int req = g_override.stages;
   if (req <= 0) return max_stages;
   return req < 2 ? 2 : req > max_stages ? max_stages : req;
 }
@@ -458,9 +448,8 @@ int conv_tc_tiles_per_image(int h, int w) {
 }
 // The conv can produce the statistics itself: tensor-core back end, 16-channel epilogue (see epilogue_wide_ok()).
 bool conv_tc_fused_stats_ok(const ConvParams& p) {
-  static const bool off = getenv("RAFT_B200_NO_FUSED_STATS") != nullptr;  // A/B knob
   auto al = [](const void* q) { return (reinterpret_cast<uintptr_t>(q) & 31) == 0; };
-  return !off && math_mode() == RB_MATH_TC && p.epi == EPI_F32 && (p.cout & 15) == 0 && al(p.bias) && al(p.addend) && al(p.f0) &&
+  return math_mode() == RB_MATH_TC && p.epi == EPI_F32 && (p.cout & 15) == 0 && al(p.bias) && al(p.addend) && al(p.f0) &&
          p.cin_pad % kChunkK == 0;
 }
 
@@ -507,11 +496,10 @@ static int launch_cfg(const ConvParams& p_in, TileGeom g, const CUtensorMap* map
   // split-K: only when every pixel tile gets its own CTA pair in one wave (batch 1), else the plain persistent grid
   if (p.split_k && !(BLOCK_N == 16 && p.cout <= 2 && p.epi == EPI_DELTA && !p.w_per_batch && conv_chunks(p) % 2 == 0))
     p.split_k = 0;
-  static const bool no_cluster = getenv("RAFT_B200_NO_SPLITK_CLUSTER") != nullptr;  // test knob: same sums on one CTA
   static const bool close_barrier = getenv("RAFT_B200_SPLITK_CLOSING_BARRIER") != nullptr;  // for compute-sanitizer runs
   p.split_close = close_barrier ? 1 : 0;
   const int max_ctas = g_override.max_ctas;  // test hook: a capped grid walks more tiles per CTA (no CTA pairs then)
-  p.split_cluster = (p.split_k && 2 * g.total_tiles <= num_sms && p.cta_limit <= 0 && max_ctas <= 0 && !no_cluster) ? 1 : 0;
+  p.split_cluster = (p.split_k && 2 * g.total_tiles <= num_sms && p.cta_limit <= 0 && max_ctas <= 0) ? 1 : 0;
   const bool cluster2 = p.split_cluster;
   cudaLaunchConfig_t cfg;
   memset(&cfg, 0, sizeof(cfg));

@@ -304,86 +304,57 @@ corr_lookup_kernel(const __grid_constant__ PyramidView pv, const __grid_constant
 }
 
 // ---------------------------------------------------------------------------------------------
-// A2/A3 lookup, warp-per-pixel form ("v5", round 2): the kernel of the VOLUME-FREE path (OTF = true) and an opt-in
-// alternative for the materialised volume (RAFT_B200_LOOKUP_V5=1).  What the r01 profile said about the round-1 kernel: 75 SASS instructions per tap (swizzle /
-// index arithmetic), 1.86x more DRAM bytes than the algorithmic count (16-column, (2r+3)-row boxes promoted to 256-byte
-// L2 requests).  v5:
+// A2/A3 lookup, warp-per-pixel form ("v5"): the kernel of the VOLUME-FREE path (SURVEY 8(f) F2).  Level l of the pyramid
+// is fmap1 . pool^l(fmap2)^T / sqrt(C) (exact by linearity, gemm_tc.cu); the (2r+3) x 11 entries a unit can touch are
+// evaluated on the fly instead of being read from a materialised volume.
 //   * one WARP per query pixel, its 4 pyramid levels = 4 units; lane = tap (t = i*D + j, ceil(K/32) rounds), so the
 //     results of a unit are 32 consecutive words of the staging row (conflict-free) and a unit's patch is read by
 //     lanes whose rows land in 8 distinct bank groups under the 64-byte swizzle (conflict-free up to j = 0 / D-1);
-//   * the patch of a unit is ONE TMA box of 16 columns x (2r+2) rows fp32 (64-byte swizzle, L2 promotion off) whose origin
-//     is (x0 & ~3, y0), (x0, y0) = clamp(trunc(centroid - r)): one row less than v4.  (A 12-column box at the unaligned x0
-//     was tried first: the TMA unit raises "illegal instruction" when the innermost box coordinate is not a
-//     multiple of 16 bytes.)  The (2r+2)^2 footprint plus the
-//     fp32-rounding slack column fits; a unit whose rounding slack falls outside the box (trunc(fl(c+d)) ==
-//     trunc(c-r)+d+1 in the last row) is detected while its index tables are built and takes a per-tap global-load
-//     path (warp-uniform branch, ~never taken);
+//   * the patch of a unit is 16 columns x (2r+3) rows fp32 whose origin is (x0, y0) = clamp(trunc(centroid - r)): the
+//     (2r+2)^2 footprint plus the fp32-rounding slack row and column;
 //   * separable index math once per unit: x table {qx, 1-qx, 4*col of x0, of x1} and y table {qy, 1-qy, swizzled row address
 //     of y0, of y1} in shared memory (two 128-bit broadcast loads per tap; texel address = row address XOR 4*col, one
 //     LOP3), tap arithmetic exactly as the reference
 //     (trunc toward zero, clamp, weights from the CLAMPED x1/y1, add_n order, no FMA contraction) => bit-identical;
-//   * every warp is self-contained (own mbarrier, own staging row, __syncwarp only): no block-wide barrier after the
-//     prologue; the fp16 hi/lo split happens in the output pass on 8 consecutive channels per lane (128-bit stores).
+//   * every warp is self-contained (own patch slots, own tables, own staging row, __syncwarp only): no block-wide barrier;
+//     the fp16 hi/lo split happens in the output pass on 8 consecutive channels per lane (128-bit stores).
 // ---------------------------------------------------------------------------------------------
-template <int R, bool OTF = false>
+template <int R>
 struct LookupV5 {
-  // OTF (volume-free, SURVEY 8(f) F2): the patch is COMPUTED (dot products against pooled fmap2), with the slack row included
-  static constexpr int D = 2 * R + 1, K = D * D, COLS = 16, ROWS = OTF ? D + 2 : D + 1, PITCH = COLS * 4;
-  static constexpr int SLOT = (ROWS * PITCH + 127) / 128 * 128;  // TMA destinations are 128-byte aligned
+  static constexpr int D = 2 * R + 1, K = D * D, COLS = 16, ROWS = D + 2, PITCH = COLS * 4;
+  static constexpr int SLOT = (ROWS * PITCH + 127) / 128 * 128;  // 128-byte aligned slots: the swizzle phase is known
   static constexpr int PB = 16, WARPS = PB, NT = WARPS * 32, ROUNDS = (K + 31) / 32;
   static constexpr int OUTP = (4 * K + 7) / 8 * 8;  // staged channels per pixel (324 -> 328, 196 -> 200)
   static constexpr int TABN = 2 * D;                // table entries per unit: D x-entries, D y-entries (float4 each)
   static constexpr int kTabOff = PB * 4 * SLOT;
   static constexpr int kStageOff = kTabOff + PB * 4 * TABN * 16;
-  static constexpr int kBarOff = kStageOff + PB * OUTP * 4;
-  static constexpr int kBytes = kBarOff + 128;
+  static constexpr int kBytes = kStageOff + PB * OUTP * 4;
 };
-// volume-free mode: level l of the pyramid is fmap1 . pool^l(fmap2)^T / sqrt(C) (exact by linearity, gemm_tc.cu); here the
-// (2r+3) x 11 entries a unit can touch are evaluated on the fly instead of being read from a materialised volume.
 struct OtfView {
   const float* f1;                 // [B,h,w,C]
   const float* f2[RB_NUM_LEVELS];  // pooled fmap2, level l: [B, h>>l, w>>l, C] fp32
   int C, N;                        // channels (<= 256, multiple of 4), pixels per sample (h*w)
 };
-struct PyramidMapsV5 {
-  CUtensorMap m[RB_NUM_LEVELS];  // (W_l, H_l, B*N) fp32, box (16, 2r+2, 1), 64-byte swizzle, no L2 promotion
-};
 // Byte offset of patch element (row, col) inside a unit whose slot starts `unit_off` bytes after the 1024-byte aligned
-// start of shared memory: rows are 64 bytes; CU_TENSOR_MAP_SWIZZLE_64B XORs the 16-byte chunk index with bits [7,9) of the
-// shared-memory byte address, i.e. with s(row) = (unit_off / 128 + row / 2) & 3.
+// start of shared memory: rows are 64 bytes, and the 16-byte chunk index is XORed with s(row) = (unit_off / 128 + row / 2) & 3
+// (the layout of CU_TENSOR_MAP_SWIZZLE_64B).
 __device__ __forceinline__ int v5_row_off(int unit_off, int row) { return row * 64 + ((((unit_off >> 7) + (row >> 1)) & 3) << 4); }
 
-template <int R, bool SPLIT, bool OTF = false>
-__global__ void __launch_bounds__(LookupV5<R, OTF>::NT, OTF ? 2 : 3)
-corr_lookup_v5_kernel(const __grid_constant__ PyramidView pv, const __grid_constant__ PyramidMapsV5 maps,
-                      const float2* __restrict__ coords, float* __restrict__ out_f32, __half* __restrict__ out_hi,
-                      __half* __restrict__ out_lo, int out_stride, int npix, const OtfView otf) {
-  using L = LookupV5<R, OTF>;
+template <int R, bool SPLIT>
+__global__ void __launch_bounds__(LookupV5<R>::NT, 2)
+corr_lookup_v5_kernel(const __grid_constant__ PyramidView pv, const float2* __restrict__ coords, float* __restrict__ out_f32,
+                      __half* __restrict__ out_hi, __half* __restrict__ out_lo, int out_stride, int npix, const OtfView otf) {
+  using L = LookupV5<R>;
   constexpr int D = L::D, K = L::K;
   extern __shared__ __align__(1024) uint8_t lk5_smem[];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int pix = blockIdx.x * L::PB + warp;
   float4* tab = reinterpret_cast<float4*>(lk5_smem + L::kTabOff) + warp * 4 * L::TABN;
   float* stage = reinterpret_cast<float*>(lk5_smem + L::kStageOff) + warp * L::OUTP;
-  // ONE mbarrier per block at a block-uniform address (the v4 pattern).  A per-warp barrier has a warp-dependent address:
-  // ptxas then emulates mbarrier.init with STS.64 + SYNCS.CCTL.IVALL instead of SYNCS.EXCH, and a build of this kernel
-  // with per-warp barriers died with "illegal instruction" -- not worth the ~1 us of decoupling.
-  uint64_t* bar = reinterpret_cast<uint64_t*>(lk5_smem + L::kBarOff);
-  uint8_t* patch = lk5_smem + warp * 4 * L::SLOT;
   const uint32_t patch0_u32 = tc::smem_u32(lk5_smem);  // 1024-byte aligned (checked below): slot offsets decide the swizzle
   if (threadIdx.x == 0 && (patch0_u32 & 1023u)) __trap();
   const bool live = pix < npix;
 
-  int n_tma = 0;
-#pragma unroll
-  for (int l = 0; l < 4; ++l) n_tma += (!OTF && pv.tma_ok[l]) ? 1 : 0;
-  if (threadIdx.x == 0) {
-    tc::mbar_init(bar, 1);
-    tc::fence_barrier_init();
-    tc::fence_proxy_async();
-    const int live_px = min(L::PB, npix - (int)blockIdx.x * L::PB);  // >= 1: the grid covers npix
-    if (n_tma) tc::mbar_arrive_expect_tx(bar, (uint32_t)(live_px * n_tma * L::ROWS * L::PITCH));
-  }
   if (lane < L::OUTP - 4 * K) stage[4 * K + lane] = 0.f;  // channel padding of the staged row
   // taps of this lane: t = lane + 32*round = i*D + j   (i walks x, j walks y: model_utils.py:235-237)
   int ti[L::ROUNDS], tj[L::ROUNDS];
@@ -393,7 +364,6 @@ corr_lookup_v5_kernel(const __grid_constant__ PyramidView pv, const __grid_const
     ti[rd] = t / D;
     tj[rd] = t - ti[rd] * D;
   }
-  __syncthreads();  // barrier initialised before any warp can issue a TMA that signals it (the only block-wide barrier)
   // PDL: dependents may be scheduled from here on (their own griddepcontrol.wait still waits for this grid to finish);
   // nothing above touched global memory, everything below comes after the predecessor kernel.
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
@@ -401,7 +371,7 @@ corr_lookup_v5_kernel(const __grid_constant__ PyramidView pv, const __grid_const
   if (!live) return;  // warp-uniform; no block-wide barrier below
 
   const float2 c = __ldg(coords + pix);
-  // ---- unit origins (lanes 0..3 hold the values of unit k = lane) and TMA issue ----------------------------------------
+  // ---- unit origins (lanes 0..3 hold the values of unit k = lane) ----------------------------------------------------------
   int bx, by;
   {
     const int k = lane & 3;
@@ -409,11 +379,8 @@ corr_lookup_v5_kernel(const __grid_constant__ PyramidView pv, const __grid_const
     const int H = pv.hl[k], W = pv.wl[k];
     bx = min(max((int)__fadd_rn(c.x * inv, (float)(-R)), 0), W - 1);
     by = min(max((int)__fadd_rn(c.y * inv, (float)(-R)), 0), H - 1);
-    if (!OTF) bx &= ~3;  // TMA: the innermost box coordinate must be a multiple of 16 bytes
-    if (!OTF && lane < 4 && pv.tma_ok[k]) tc::tma_load_3d(&maps.m[k], bar, patch + k * L::SLOT, bx, by, pix);
   }
   // ---- index tables: lane -> (unit k = lane >> 3, entry e = lane & 7); entry 8 (r = 4) by the lanes with e = 0 / 1 ------
-  unsigned bad = 0;
   {
     const int k = lane >> 3, e = lane & 7;
     const int bxk = __shfl_sync(0xffffffffu, bx, k), byk = __shfl_sync(0xffffffffu, by, k);
@@ -428,7 +395,6 @@ corr_lookup_v5_kernel(const __grid_constant__ PyramidView pv, const __grid_const
       x1 = min(max(x1, 0), W - 1);
       const float qx = __fsub_rn((float)x1, x);  // utils.py:84 (clamped x1)
       const int a0 = x0 - bxk, a1 = x1 - bxk;
-      if ((unsigned)a0 >= (unsigned)L::COLS || (unsigned)a1 >= (unsigned)L::COLS) bad = 1;
       tab[k * L::TABN + i] = make_float4(qx, __fsub_rn(1.0f, qx), __int_as_float(a0 * 4), __int_as_float(a1 * 4));
     };
     auto y_entry = [&](int j) {
@@ -439,7 +405,6 @@ corr_lookup_v5_kernel(const __grid_constant__ PyramidView pv, const __grid_const
       y1 = min(max(y1, 0), H - 1);
       const float qy = __fsub_rn((float)y1, y);  // utils.py:85
       const int r0 = y0 - byk, r1 = y1 - byk;
-      if ((unsigned)r0 >= (unsigned)L::ROWS || (unsigned)r1 >= (unsigned)L::ROWS) bad = 1;
       const int uoff = (warp * 4 + k) * L::SLOT;  // slot offset from the 1024-byte aligned start of shared memory
       tab[k * L::TABN + D + j] = make_float4(qy, __fsub_rn(1.0f, qy), __int_as_float((int)patch0_u32 + uoff + v5_row_off(uoff, r0)),
                                              __int_as_float((int)patch0_u32 + uoff + v5_row_off(uoff, r1)));
@@ -450,13 +415,12 @@ corr_lookup_v5_kernel(const __grid_constant__ PyramidView pv, const __grid_const
       if (e == 1) y_entry(8);
     }
   }
-  const unsigned badmask = __ballot_sync(0xffffffffu, bad != 0);  // bits 8k..8k+7 belong to unit k
-  // ---- volume-free mode: evaluate the patch entries ----------------------------------------------------------------------
+  // ---- evaluate the patch entries -------------------------------------------------------------------------------------------
   // The warp reads each target feature row COALESCED (lane = 4 channels per 128-channel half; fmap1[pix] stays in 8
   // registers), 8 entries at a time, and reduces the 8 x 32 partial sums with a recursive-halving exchange (9 shuffles per 8
   // entries).  First version (lane = entry, each lane streaming its own 1 KB row): 32 L1 lines per load instruction, 2x
   // sector waste, 1.3 ms per lookup at 55x128 -- L2-bound; neighbouring pixels share most rows, which this form lets L1 see.
-  if constexpr (OTF) {
+  {
     const int C = otf.C;
     const bool two = C > 128;  // C is 128 or 256 (launch_lookup_otf)
     const float4 fa = __ldg(reinterpret_cast<const float4*>(otf.f1 + (size_t)pix * C + 4 * lane));
@@ -517,34 +481,12 @@ corr_lookup_v5_kernel(const __grid_constant__ PyramidView pv, const __grid_const
       }
     }
   }
-  // ---- levels TMA cannot address (W % 4 != 0): plain loads into the same layout ------------------------------------------
-  if (!OTF && n_tma < 4) {
-#pragma unroll
-    for (int k = 0; k < 4; ++k) {
-      if (pv.tma_ok[k]) continue;
-      const int bxk = __shfl_sync(0xffffffffu, bx, k), byk = __shfl_sync(0xffffffffu, by, k);
-      const int H = pv.hl[k], W = pv.wl[k];
-      const int uoff = (warp * 4 + k) * L::SLOT;
-      for (int e = lane; e < L::ROWS * 4; e += 32) {
-        const int row = e >> 2, ch = e & 3;
-        const float* src = pv.base[k] + ((size_t)pix * H + min(byk + row, H - 1)) * W;
-        const int col = bxk + ch * 4;
-        float4 v;
-        v.x = __ldg(src + min(col + 0, W - 1)); v.y = __ldg(src + min(col + 1, W - 1));
-        v.z = __ldg(src + min(col + 2, W - 1)); v.w = __ldg(src + min(col + 3, W - 1));
-        *reinterpret_cast<float4*>(lk5_smem + uoff + (v5_row_off(uoff, row) ^ (ch * 16))) = v;
-      }
-    }
-  }
-  __syncwarp();  // tables and fallback patches visible to the warp
-  if (n_tma) tc::mbar_wait(bar, 0);  // all patches of the block have landed
+  __syncwarp();  // tables and patches visible to the warp
   // ---- taps -----------------------------------------------------------------------------------------------------------------
 #pragma unroll
   for (int k = 0; k < 4; ++k) {
-    const int bxk = __shfl_sync(0xffffffffu, bx, k), byk = __shfl_sync(0xffffffffu, by, k);  // converged here (slow path only)
     const float4* xt = tab + k * L::TABN;
     const float4* yt = xt + D;
-    const bool slow = ((badmask >> (8 * k)) & 0xffu) != 0;  // warp-uniform
 #pragma unroll
     for (int rd = 0; rd < L::ROUNDS; ++rd) {
       const int t = lane + 32 * rd;
@@ -552,19 +494,9 @@ corr_lookup_v5_kernel(const __grid_constant__ PyramidView pv, const __grid_const
         const float4 X = xt[ti[rd]], Y = yt[tj[rd]];
         const float wa = __fmul_rn(X.x, Y.x), wb = __fmul_rn(X.x, Y.y);  // utils.py:86-89
         const float wc = __fmul_rn(X.y, Y.x), wd = __fmul_rn(X.y, Y.y);
+        // Y.z / Y.w: swizzled row addresses (64-byte aligned + chunk phase), X.z / X.w: 4 * column
         const int a0 = __float_as_int(X.z), a1 = __float_as_int(X.w), r0 = __float_as_int(Y.z), r1 = __float_as_int(Y.w);
-        float Ia, Ib, Ic, Id;
-        if (OTF || !slow) {  // r0 / r1: swizzled row addresses (64-byte aligned + chunk phase), a0 / a1: 4 * column
-          Ia = lds_f32(r0 ^ a0); Ib = lds_f32(r1 ^ a0);
-          Ic = lds_f32(r0 ^ a1); Id = lds_f32(r1 ^ a1);
-        } else {  // rounding slack outside the box: read the four texels from the volume itself
-          const int H = pv.hl[k], W = pv.wl[k];
-          const float* img = pv.base[k] + (size_t)pix * H * W;
-          const int ubase = (int)patch0_u32 + (warp * 4 + k) * L::SLOT;
-          const int x0 = bxk + (a0 >> 2), x1 = bxk + (a1 >> 2), y0 = byk + ((r0 - ubase) >> 6), y1 = byk + ((r1 - ubase) >> 6);
-          Ia = __ldg(img + (size_t)y0 * W + x0); Ib = __ldg(img + (size_t)y1 * W + x0);
-          Ic = __ldg(img + (size_t)y0 * W + x1); Id = __ldg(img + (size_t)y1 * W + x1);
-        }
+        const float Ia = lds_f32(r0 ^ a0), Ib = lds_f32(r1 ^ a0), Ic = lds_f32(r0 ^ a1), Id = lds_f32(r1 ^ a1);
         stage[k * K + t] = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(wa, Ia), __fmul_rn(wb, Ib)), __fmul_rn(wc, Ic)),
                                      __fmul_rn(wd, Id));  // tf.add_n order (utils.py:98)
       }
@@ -664,15 +596,15 @@ static int launch_lookup_cfg(const PyramidView& pv, const PyramidMaps& maps, con
   return RB_OK;
 }
 
-template <int R, bool SPLIT, bool OTF = false>
-static int launch_lookup_v5(const PyramidView& pv, const PyramidMapsV5& maps, const float2* c2, float* out_f32, __half* out_hi,
-                            __half* out_lo, int out_stride, int npix, cudaStream_t s, const OtfView& otf = OtfView{}) {
-  using L = LookupV5<R, OTF>;
+template <int R, bool SPLIT>
+static int launch_lookup_v5(const PyramidView& pv, const float2* c2, float* out_f32, __half* out_hi, __half* out_lo,
+                            int out_stride, int npix, cudaStream_t s, const OtfView& otf) {
+  using L = LookupV5<R>;
   static PerDeviceOnce attr_set;
   int dev = 0, rc_dev;
   if ((rc_dev = current_device(&dev))) return rc_dev;
   if (!attr_set.test(dev)) {
-    RB_CHECK_CUDA(cudaFuncSetAttribute(corr_lookup_v5_kernel<R, SPLIT, OTF>, cudaFuncAttributeMaxDynamicSharedMemorySize, L::kBytes));
+    RB_CHECK_CUDA(cudaFuncSetAttribute(corr_lookup_v5_kernel<R, SPLIT>, cudaFuncAttributeMaxDynamicSharedMemorySize, L::kBytes));
     attr_set.set(dev);
   }
   static const int pdl = getenv("RAFT_B200_NO_PDL") ? 0 : 1;
@@ -687,7 +619,7 @@ static int launch_lookup_v5(const PyramidView& pv, const PyramidMapsV5& maps, co
   attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
   cfg.numAttrs = pdl;
-  RB_CHECK_CUDA(cudaLaunchKernelEx(&cfg, corr_lookup_v5_kernel<R, SPLIT, OTF>, pv, maps, c2, out_f32, out_hi, out_lo, out_stride, npix, otf));
+  RB_CHECK_CUDA(cudaLaunchKernelEx(&cfg, corr_lookup_v5_kernel<R, SPLIT>, pv, c2, out_f32, out_hi, out_lo, out_stride, npix, otf));
   RB_CHECK_LAUNCH("corr_lookup_v5_kernel");
   return RB_OK;
 }
@@ -703,31 +635,6 @@ int launch_lookup(const float* pyramid, const float* coords, float* out_f32, __h
   const int npix = B * h * w;
   const float2* c2 = reinterpret_cast<const float2*>(coords);
   const bool split = out_hi != nullptr;
-  // Default: corr_lookup_kernel (block = 16 px x 4 levels, thread = window row).  RAFT_B200_LOOKUP_V5=1 selects the
-  // warp-per-pixel kernel (lane = tap) that the volume-free path is built on: same DRAM traffic, 29 % shared-memory bank
-  // conflicts (nine window rows of one column can never sit in nine distinct bank groups) -- slower at batch 8, kept
-  // selectable because it shares every line with the volume-free instantiation.
-  static const bool v5 = getenv("RAFT_B200_LOOKUP_V5") != nullptr;
-  const bool f32_rows_ok = split || (out_stride % 4 == 0 && reinterpret_cast<uintptr_t>(out_f32) % 16 == 0);
-  if (v5 && f32_rows_ok) {
-    PyramidMapsV5 maps;
-    memset(&maps, 0, sizeof(maps));
-    for (int l = 0; l < RB_NUM_LEVELS; ++l) {
-      if (!pv.tma_ok[l]) continue;
-      uint64_t dims[3] = {(uint64_t)pv.wl[l], (uint64_t)pv.hl[l], (uint64_t)npix};
-      uint64_t str[2] = {(uint64_t)pv.wl[l] * 4, (uint64_t)pv.wl[l] * pv.hl[l] * 4};
-      uint32_t box[3] = {16u, (uint32_t)(2 * radius + 2), 1};
-      if (cached_tmap(&maps.m[l], pv.base[l], 3, dims, str, box, tc::TMAP_F32_SW64_GATHER) != RB_OK) pv.tma_ok[l] = 0;  // plain loads
-    }
-    static const bool no_tma = getenv("RAFT_B200_LOOKUP_NOTMA") != nullptr;  // diagnostic: stage every level with plain loads
-    if (no_tma)
-      for (int l = 0; l < RB_NUM_LEVELS; ++l) pv.tma_ok[l] = 0;
-    if (radius == 4)
-      return split ? launch_lookup_v5<4, true>(pv, maps, c2, nullptr, out_hi, out_lo, out_stride, npix, s)
-                   : launch_lookup_v5<4, false>(pv, maps, c2, out_f32, nullptr, nullptr, out_stride, npix, s);
-    return split ? launch_lookup_v5<3, true>(pv, maps, c2, nullptr, out_hi, out_lo, out_stride, npix, s)
-                 : launch_lookup_v5<3, false>(pv, maps, c2, out_f32, nullptr, nullptr, out_stride, npix, s);
-  }
   PyramidMaps maps;
   memset(&maps, 0, sizeof(maps));
   for (int l = 0; l < RB_NUM_LEVELS; ++l) {
@@ -776,16 +683,14 @@ int launch_lookup_otf(const float* fmap1, const float* fmap2, const float* poole
     pv.hl[l] = level_dim(h, l); pv.wl[l] = level_dim(w, l);
     otf.f2[l] = l == 0 ? fmap2 : pooled + otf_level_offset(B, h, w, C, l);
   }
-  PyramidMapsV5 maps;
-  memset(&maps, 0, sizeof(maps));
   const float2* c2 = reinterpret_cast<const float2*>(coords);
   const int npix = B * h * w;
   const bool split = out_hi != nullptr;
   if (radius == 4)
-    return split ? launch_lookup_v5<4, true, true>(pv, maps, c2, nullptr, out_hi, out_lo, out_stride, npix, s, otf)
-                 : launch_lookup_v5<4, false, true>(pv, maps, c2, out_f32, nullptr, nullptr, out_stride, npix, s, otf);
-  return split ? launch_lookup_v5<3, true, true>(pv, maps, c2, nullptr, out_hi, out_lo, out_stride, npix, s, otf)
-               : launch_lookup_v5<3, false, true>(pv, maps, c2, out_f32, nullptr, nullptr, out_stride, npix, s, otf);
+    return split ? launch_lookup_v5<4, true>(pv, c2, nullptr, out_hi, out_lo, out_stride, npix, s, otf)
+                 : launch_lookup_v5<4, false>(pv, c2, out_f32, nullptr, nullptr, out_stride, npix, s, otf);
+  return split ? launch_lookup_v5<3, true>(pv, c2, nullptr, out_hi, out_lo, out_stride, npix, s, otf)
+               : launch_lookup_v5<3, false>(pv, c2, out_f32, nullptr, nullptr, out_stride, npix, s, otf);
 }
 
 int corr_build_tc(const float* fmap1, const float* fmap2, float* pyramid, int B, int h, int w, int C,

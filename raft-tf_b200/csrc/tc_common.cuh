@@ -153,7 +153,7 @@ __device__ __forceinline__ void wgmma_f16<128>(float* d, uint64_t a, uint64_t b)
 
 // ---- host: tensor maps --------------------------------------------------------------------------------
 // up to 4 dims (innermost first), zero fill for out-of-bounds boxes; kind selects element type and swizzle
-enum { TMAP_F16_SW128 = 0, TMAP_F32_SW64 = 1, TMAP_F32_SW64_GATHER = 2 };  // GATHER: as SW64 but without L2 promotion (lookup v5)
+enum { TMAP_F16_SW128 = 0, TMAP_F32_SW64 = 1 };
 int make_tmap(CUtensorMap* out, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
               const uint32_t* box, int kind, const uint32_t* elem_strides = nullptr);
 

@@ -234,7 +234,7 @@ __global__ void copy_f32_kernel(const float* __restrict__ src, float* __restrict
 }
 
 // encoder/convf1: 7x7 conv over the 2-channel flow + ReLU (model_utils.py:114,124), CUDA-core form: the cross-check back end
-// (RB_MATH_SIMT) and RAFT_B200_CONVF1_SIMT=1; the default is the tensor-core form (flow_prep_kernel below + conv_tc)
+// (RB_MATH_SIMT) and the shapes the tensor-core form rejects; the default is the tensor-core form (flow_prep_kernel below + conv_tc)
 // (K = 98 is no tensor-core shape).  flow = coords1 - coords_grid (RAFT.py:95) is formed while
 // staging; SAME padding zero-pads the FLOW.  One thread per output channel, SEG-pixel row segment
 // per block (SEG = 16 at batch 1: 440 blocks instead of 220 -- the kernel is latency-bound, and with the convf2 that
@@ -345,10 +345,7 @@ static ConvParams base_params(const Variant& v, const PackedLayout& L, const voi
 // convolutions is computed once in rb_update_set_state* and added in the epilogue: the per-iteration K loop
 // skips those channels (-1/3 of the GRU MMA work and operand traffic; identical up to fp32 summation order).
 // Only when the slice is aligned to the 64-channel chunks (raft-things: [128,256)).
-static inline bool can_hoist(const Variant& v) {
-  static const bool off = getenv("RAFT_B200_NO_HOIST") != nullptr;  // A/B knob
-  return !off && !v.small && v.hidden % 64 == 0 && v.ctx % 64 == 0;
-}
+static inline bool can_hoist(const Variant& v) { return !v.small && v.hidden % 64 == 0 && v.ctx % 64 == 0; }
 static void hoist_inp(const Variant& v, const Workspace& W, int idx, ConvParams& p) {
   if (!can_hoist(v)) return;
   const int total = v.hx / 64, inp0 = v.hidden / 64, ninp = v.ctx / 64;
@@ -357,150 +354,11 @@ static void hoist_inp(const Variant& v, const Workspace& W, int idx, ConvParams&
   p.bias = nullptr;  // folded into the addend
 }
 
-// flow_head/conv2 (3x3, fh -> 2 channels, model_utils.py:134) + coords1 += delta (RAFT.py:102) on CUDA cores.
-// As an implicit GEMM this conv uses 2 of the 16 columns of the narrowest MMA tile and still streams a 32 KB
-// activation tile per (tap, 64-channel chunk) through every CTA;
-// here the split planes are joined to fp32 once per 8x8-pixel halo tile in shared memory and 112 blocks (batch 1) do
-// 2 x 9 x CIN FMAs per pixel.  256 threads = 64 pixels x 4 channel quarters of every 64-channel chunk; fixed
-// summation order (bit-reproducible, batched == per-sample).  The weights are staged before griddepcontrol.wait.
-template <int CIN>
-__global__ void __launch_bounds__(256) flow_head2_kernel(const __half* __restrict__ in_hi, const __half* __restrict__ in_lo,
-                                                         int in_stride, const __half* __restrict__ w_hi,
-                                                         const __half* __restrict__ w_lo, const float* __restrict__ bias,
-                                                         float* coords1, float* delta_out, int h, int w, int trigger) {
-  constexpr int kPitch = 68;  // floats per halo pixel (64 + 4: conflict-free 128-bit reads across pixels)
-  __shared__ __align__(16) float2 wsm[9 * CIN];
-  __shared__ __align__(16) float act[100 * kPitch];
-  __shared__ float2 red[4][64];
-  const int tid = threadIdx.x, px = tid & 63, q = tid >> 6;
-  const int b = blockIdx.z, y0 = blockIdx.y * 8, x0 = blockIdx.x * 8;
-  for (int i = tid * 8; i < 9 * CIN; i += 256 * 8) {  // packed [cout_pad][9][CIN] split planes -> fp32 (w[.., 0], w[.., 1])
-    const uint4 h0 = *reinterpret_cast<const uint4*>(w_hi + i), l0 = *reinterpret_cast<const uint4*>(w_lo + i);
-    const uint4 h1 = *reinterpret_cast<const uint4*>(w_hi + 9 * CIN + i), l1 = *reinterpret_cast<const uint4*>(w_lo + 9 * CIN + i);
-    const __half* a0 = reinterpret_cast<const __half*>(&h0);
-    const __half* b0 = reinterpret_cast<const __half*>(&l0);
-    const __half* a1 = reinterpret_cast<const __half*>(&h1);
-    const __half* b1 = reinterpret_cast<const __half*>(&l1);
-#pragma unroll
-    for (int k = 0; k < 8; ++k) wsm[i + k] = make_float2(join_f32(a0[k], b0[k]), join_f32(a1[k], b1[k]));
-  }
-  if (trigger == 0) asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-  asm volatile("griddepcontrol.wait;" ::: "memory");
-  const int ly = px >> 3, lx = px & 7;
-  float acc0 = 0.f, acc1 = 0.f;
-  // halo staging: 100 pixels x 8 vectors of 8 channels = 800 vectors, up to 4 per thread; the vectors of chunk c+1 are
-  // requested before the FMAs of chunk c (the kernel has 8 warps per SM: un-overlapped L2 latency would dominate it)
-  uint4 vh[4], vl[4];
-  size_t voff[4];
-  bool vin[4];
-#pragma unroll
-  for (int k = 0; k < 4; ++k) {
-    const int v = tid + k * 256;
-    const int hp = v >> 3, c8 = (v & 7) * 8;
-    const int hy = hp / 10, hx = hp - hy * 10;
-    const int y = y0 - 1 + hy, x = x0 - 1 + hx;
-    vin[k] = v < 800 && y >= 0 && y < h && x >= 0 && x < w;  // SAME padding: zeros outside the image
-    voff[k] = vin[k] ? ((size_t)(b * h + y) * w + x) * in_stride + c8 : 0;
-  }
-  auto fetch = [&](int chunk) {
-#pragma unroll
-    for (int k = 0; k < 4; ++k) {
-      if (vin[k]) {
-        vh[k] = *reinterpret_cast<const uint4*>(in_hi + voff[k] + chunk * 64);
-        vl[k] = *reinterpret_cast<const uint4*>(in_lo + voff[k] + chunk * 64);
-      } else {
-        vh[k] = make_uint4(0, 0, 0, 0);
-        vl[k] = make_uint4(0, 0, 0, 0);
-      }
-    }
-  };
-  fetch(0);
-  for (int chunk = 0; chunk < CIN / 64; ++chunk) {
-    __syncthreads();  // the previous chunk has been consumed (first pass: the weights are in place)
-#pragma unroll
-    for (int k = 0; k < 4; ++k) {
-      const int v = tid + k * 256;
-      if (v < 800) {
-        const int hp = v >> 3, c8 = (v & 7) * 8;
-        const __half* hh = reinterpret_cast<const __half*>(&vh[k]);
-        const __half* ll = reinterpret_cast<const __half*>(&vl[k]);
-        float f[8];
-#pragma unroll
-        for (int i = 0; i < 8; ++i) f[i] = join_f32(hh[i], ll[i]);
-        float4* dst = reinterpret_cast<float4*>(&act[hp * kPitch + c8]);
-        dst[0] = make_float4(f[0], f[1], f[2], f[3]);
-        dst[1] = make_float4(f[4], f[5], f[6], f[7]);
-      }
-    }
-    __syncthreads();
-    if (chunk + 1 < CIN / 64) fetch(chunk + 1);
-#pragma unroll
-    for (int t = 0; t < 9; ++t) {
-      const int ky = t / 3, kx = t - ky * 3;
-      const float4* a = reinterpret_cast<const float4*>(&act[((ly + ky) * 10 + lx + kx) * kPitch + q * 16]);
-      const float2* ww = &wsm[t * CIN + chunk * 64 + q * 16];
-#pragma unroll
-      for (int c4 = 0; c4 < 4; ++c4) {
-        const float4 av = a[c4];
-        const float2 u0 = ww[c4 * 4 + 0], u1 = ww[c4 * 4 + 1], u2 = ww[c4 * 4 + 2], u3 = ww[c4 * 4 + 3];
-        acc0 = fmaf(av.x, u0.x, acc0); acc1 = fmaf(av.x, u0.y, acc1);
-        acc0 = fmaf(av.y, u1.x, acc0); acc1 = fmaf(av.y, u1.y, acc1);
-        acc0 = fmaf(av.z, u2.x, acc0); acc1 = fmaf(av.z, u2.y, acc1);
-        acc0 = fmaf(av.w, u3.x, acc0); acc1 = fmaf(av.w, u3.y, acc1);
-      }
-    }
-  }
-  if (trigger == 1) asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-  red[q][px] = make_float2(acc0, acc1);
-  __syncthreads();
-  if (tid < 64) {
-    const int y = y0 + ly, x = x0 + lx;
-    if (y < h && x < w) {
-      const float2 r0 = red[0][px], r1 = red[1][px], r2 = red[2][px], r3 = red[3][px];
-      const float d0 = ((r0.x + r1.x) + (r2.x + r3.x)) + bias[0];
-      const float d1 = ((r0.y + r1.y) + (r2.y + r3.y)) + bias[1];
-      const size_t o = ((size_t)(b * h + y) * w + x) * 2;
-      float2 c = *reinterpret_cast<float2*>(coords1 + o);
-      c.x += d0; c.y += d1;
-      *reinterpret_cast<float2*>(coords1 + o) = c;
-      if (delta_out) *reinterpret_cast<float2*>(delta_out + o) = make_float2(d0, d1);
-    }
-  }
-}
-
-static int launch_flow_head2(const ConvParams& p, cudaStream_t s) {
-  static const int pdl = getenv("RAFT_B200_NO_PDL") ? 0 : 1;
-  cudaLaunchConfig_t cfg;
-  memset(&cfg, 0, sizeof(cfg));
-  cfg.gridDim = dim3((p.w + 7) / 8, (p.h + 7) / 8, p.B);
-  cfg.blockDim = dim3(256);
-  cfg.stream = s;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = pdl;
-  // when the dependents (next iteration's lookup / convc1) may be scheduled: 0 = kernel start, 1 = after the FMA loop,
-  // 2 = at completion (tuning knob)
-  static const int trigger = getenv("RAFT_B200_FH2_TRIGGER") ? atoi(getenv("RAFT_B200_FH2_TRIGGER")) : 1;
-  if (p.cin_pad == 256) {
-    RB_CHECK_CUDA(cudaLaunchKernelEx(&cfg, flow_head2_kernel<256>, p.in_hi, p.in_lo, p.in_stride, p.w_hi, p.w_lo, p.bias, p.f1,
-                                     p.f2, p.h, p.w, trigger));
-  } else {
-    RB_CHECK_CUDA(cudaLaunchKernelEx(&cfg, flow_head2_kernel<128>, p.in_hi, p.in_lo, p.in_stride, p.w_hi, p.w_lo, p.bias, p.f1,
-                                     p.f2, p.h, p.w, trigger));
-  }
-  RB_CHECK_LAUNCH("flow_head2_kernel");
-  return RB_OK;
-}
-
 // Phase-timestamp debug buffer (tools/phase_times.py): rb_debug_set_buffer(ptr, convs) makes the next update
 // step record 8 timestamps per CTA for each of its convs, in launch order, 4096 CTAs per conv.
 static thread_local long long* g_dbg = nullptr;
 static thread_local int g_dbg_idx = 0;
 static int launch_conv_dbg(ConvParams& p, cudaStream_t s) {
-  static const int early = getenv("RAFT_B200_PDL_EARLY") ? 1 : 0;
-  p.pdl_early = early;
   if (g_dbg) p.dbg = g_dbg + (size_t)(g_dbg_idx++) * 4096 * 8;
   return launch_conv(p, s);
 }
@@ -552,19 +410,16 @@ static int update_step(const Variant& v, const void* blob, void* wsp, float* coo
   RB_CHECK_CUDA(cudaEventRecord(ss->fork, s));
   RB_CHECK_CUDA(cudaStreamWaitEvent(ss->stream, ss->fork, 0));
   {  // flow branch (side stream): convf1 (7x7) -> convf2
-    static const int seg_env = getenv("RAFT_B200_CONV7_SEG") ? atoi(getenv("RAFT_B200_CONV7_SEG")) : 0;  // tuning knob
-    // pixels per block of the CUDA-core flow_conv7 (RB_MATH_SIMT / RAFT_B200_CONVF1_SIMT only): carried over from the B200
-    // version of this kernel, not re-measured on H100
-    const int seg = seg_env ? seg_env : ((long)B * h * w <= 16384 ? 16 : 32);
+    // pixels per block of the CUDA-core flow_conv7: carried over from the B200 version of this kernel, not re-measured on H100
+    const int seg = (long)B * h * w <= 16384 ? 16 : 32;
     const float* Wf = reinterpret_cast<const float*>(bb + L.f1_w);
     const float* bf = reinterpret_cast<const float*>(bb + L.f1_b);
     const float2* c1 = reinterpret_cast<const float2*>(coords1);
 #define RB_LAUNCH_CONV7(COUT, SEG) \
     flow_conv7_kernel<COUT, SEG><<<dim3((w + SEG - 1) / SEG, h, B), COUT, 0, ss->stream>>>(c1, Wf, bf, W.f1, v.f1, W.hx, W.qx, v.hx, foff, h, w)
-    // default: convf1 on the tensor cores (flow_prep_kernel + 7x1 conv over the window view); RAFT_B200_CONVF1_SIMT=1 and the
-    // CUDA-core math mode keep the CUDA-core kernel
-    static const bool f1_simt = getenv("RAFT_B200_CONVF1_SIMT") != nullptr;
-    const bool f1_tc = !f1_simt && math_mode() == RB_MATH_TC && (foff & 1) == 0 && (v.hx & 1) == 0 && w >= 8;
+    // default: convf1 on the tensor cores (flow_prep_kernel + 7x1 conv over the window view); the CUDA-core math mode and
+    // the shapes the window view cannot take keep the CUDA-core kernel
+    const bool f1_tc = math_mode() == RB_MATH_TC && (foff & 1) == 0 && (v.hx & 1) == 0 && w >= 8;
     if (f1_tc) {
       const size_t cells = (size_t)B * h * (w + 8);
       flow_prep_kernel<<<(unsigned)((cells + 255) / 256), 256, 0, ss->stream>>>(c1, W.fl, W.hx, W.qx, v.hx, foff, B, h, w);
@@ -581,17 +436,16 @@ static int update_step(const Variant& v, const void* blob, void* wsp, float* coo
       p.cout = L.f1t_cout; p.cout_pad = L.f1t_cout_pad;
       p.B = B; p.h = h; p.w = w; p.hidden = v.hidden; p.scale = 1.f;
       set_act(p, ACT_RELU, W.f1, v.f1, 0);
-      static const int lim1 = getenv("RAFT_B200_CONVF1_CTAS") ? atoi(getenv("RAFT_B200_CONVF1_CTAS")) : -1;  // tuning knob
       // batch 1: 28 CTAs = the 55 128-wide tiles in two full rounds, leaving the SMs to the lookup and convc1 / convc2.
       // Re-swept on H100 (132 SMs, 700 W, forward pass at 440x1024, L2 flushed, 3 interleaved runs each): 28/38 13.03 ms,
       // 38/38 13.00, no limit 12.94, 19/28 13.20 ms, against a spread of about 0.09 ms between runs of one setting --
       // no setting is clearly better, so 28 / 38 stay.
-      p.cta_limit = lim1 >= 0 ? lim1 : ((long)B * h * w <= 16384 ? 28 : 0);
+      p.cta_limit = (long)B * h * w <= 16384 ? 28 : 0;
       if ((rc = launch_conv_dbg(p, ss->stream))) return rc;
     } else if (v.small) {
-      if (seg == 8) RB_LAUNCH_CONV7(64, 8); else if (seg == 16) RB_LAUNCH_CONV7(64, 16); else RB_LAUNCH_CONV7(64, 32);
+      if (seg == 16) RB_LAUNCH_CONV7(64, 16); else RB_LAUNCH_CONV7(64, 32);
     } else {
-      if (seg == 8) RB_LAUNCH_CONV7(128, 8); else if (seg == 16) RB_LAUNCH_CONV7(128, 16); else RB_LAUNCH_CONV7(128, 32);
+      if (seg == 16) RB_LAUNCH_CONV7(128, 16); else RB_LAUNCH_CONV7(128, 32);
     }
 #undef RB_LAUNCH_CONV7
     RB_CHECK_LAUNCH("flow_conv7_kernel");
@@ -600,8 +454,7 @@ static int update_step(const Variant& v, const void* blob, void* wsp, float* coo
       set_act(p, ACT_RELU, W.cf, v.cf, v.cor);
       // convf2 runs beside convc1 / convc2 of the main stream: a small CTA budget keeps it off the SMs they need
       // (batch 1: the other convs use 55-110 of the 132 SMs)
-      static const int lim = getenv("RAFT_B200_CONVF2_CTAS") ? atoi(getenv("RAFT_B200_CONVF2_CTAS")) : -1;  // tuning knob
-      p.cta_limit = lim >= 0 ? lim : ((long)B * h * w <= 16384 ? 38 : 0);
+      p.cta_limit = (long)B * h * w <= 16384 ? 38 : 0;
       if ((rc = launch_conv_dbg(p, ss->stream))) return rc;
     }
     RB_CHECK_CUDA(cudaEventRecord(ss->join, ss->stream));
@@ -662,18 +515,9 @@ static int update_step(const Variant& v, const void* blob, void* wsp, float* coo
     p.epi = EPI_DELTA; p.f1 = coords1; p.f2 = delta_out;
     // 36 k-iterations on 55 CTAs at batch 1 while 77 SMs idle: two CTAs per pixel tile, half of the channel chunks each
     // (conv_tc.cu, split-K over a cluster when the tiles fit one wave of CTA pairs; the same two-halves sum on one CTA
-    // otherwise, so batched and per-sample runs stay bit-identical).  RAFT_B200_NO_SPLITK=1: one accumulator.
-    static const bool no_splitk = getenv("RAFT_B200_NO_SPLITK") != nullptr;
-    p.split_k = no_splitk ? 0 : 1;
-    // RAFT_B200_FH2_SIMT=1: CUDA-core kernel instead of the N=16 implicit GEMM -> opt-in.
-    static const bool fh2_simt = getenv("RAFT_B200_FH2_SIMT") != nullptr;
-    const bool direct = fh2_simt && p.kh == 3 && p.kw == 3 && p.in_choff == 0 && p.in_stride % 8 == 0 &&
-                        (p.cin_pad == 256 || p.cin_pad == 128) && p.cout == 2;
-    if (direct) {
-      if ((rc = launch_flow_head2(p, s))) return rc;
-    } else if ((rc = launch_conv_dbg(p, s))) {
-      return rc;
-    }
+    // otherwise, so batched and per-sample runs stay bit-identical).
+    p.split_k = 1;
+    if ((rc = launch_conv_dbg(p, s))) return rc;
   }
   // ---- mask head (model_utils.py:180-183); only the last iteration's mask is ever consumed ----
   if (mask_out) {

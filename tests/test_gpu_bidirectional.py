@@ -108,12 +108,6 @@ def test_eager_equals_graph(cuda):
     assert all(torch.equal(x, y) for x, y in zip(a, b))
 
 
-@pytest.mark.parametrize("knob", ["RAFT_B200_TORCH_ENCODERS", "RAFT_B200_SERIAL_ENCODERS"])
-def test_encoder_paths(cuda, monkeypatch, knob):
-    monkeypatch.setenv(knob, "1")
-    _check_bidirectional(cuda, False, 2, 64, 96)
-
-
 def test_full_size(cuda):
     """436x1024 (padded to 440): the full-size pyramid at 2B pairs."""
     _check_bidirectional(cuda, False, 1, 436, 1024)

@@ -13,7 +13,6 @@ Configurations recorded by rb_debug_conv_last are printed at the end of the modu
 import contextlib
 import ctypes as C
 import math
-import os
 
 import numpy as np
 import pytest
@@ -78,9 +77,7 @@ def _auto_block_n(cout, m_tiles, ctas):
 
 
 def _ring(block_n, stages):
-    env = int(os.environ.get("RAFT_B200_TC_STAGES", "0") or 0)
-    req = stages if stages > 0 else env
-    return RING[block_n] if req <= 0 else min(max(req, 2), RING[block_n])
+    return RING[block_n] if stages <= 0 else min(max(stages, 2), RING[block_n])
 
 
 def _expected(cfg, B, h, w, cout):

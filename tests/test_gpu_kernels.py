@@ -57,8 +57,9 @@ def test_lookup_bit_exact(cuda, B, h, w, r):
 
 def test_lookup_rounding_slack_outside_the_box(cuda):
     """fl(c + d) can round UP across an integer (c = 15.999999, d = +4 -> 20.0 while trunc(c - 4) + 8 = 19): the window then
-    reaches one row / column beyond the (2r+2)^2 footprint.  Lookup v5 stages (2r+2) rows and takes a per-tap global-load
-    path for such units; columns have the slack inside the 12-column box.  Must stay bit-exact."""
+    reaches one row / column beyond the (2r+2)^2 footprint.  The lookup stages (2r+2) rows per unit and reads a window row
+    that falls outside them with per-tap global loads; the slack column lies inside the 16 staged columns.  Must stay
+    bit-exact."""
     from networks.model_utils import SampleCorr
     B, h, w, r = 1, 48, 64, 4
     pyr = _rand_pyramid(B, h, w, 77)
