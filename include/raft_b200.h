@@ -50,6 +50,22 @@ const char* rb_last_error(void);
 /* Select the back end for subsequent calls on this thread (default RB_MATH_TC). */
 int rb_set_math_mode(int mode);
 int rb_get_math_mode(void);
+/* Numerics of the network for subsequent calls on this thread (default RB_SEMANTICS_REFERENCE); like the math mode it is
+ * read when a kernel is launched, so it may be set inside CUDA-graph capture.  Unknown values -> RB_ERR_BAD_ARG.
+ *   RB_SEMANTICS_REFERENCE  the TF port: truncating / clamping lookup, TF 'SAME' pads on stride-2 convs;
+ *   RB_SEMANTICS_UPSTREAM   princeton-vl RAFT (PyTorch): the lookup is bilinear_sampler + F.grid_sample(align_corners=True,
+ *                           padding_mode="zeros"), stride-2 convs pad k / 2 before.  It applies to rb_corr_lookup,
+ *                           rb_update_lookup, rb_raft_iterate, rb_corr_otf_lookup, rb_update_lookup_otf, rb_encoder_forward and
+ *                           rb_conv2d_strided.  The lookups need every pyramid level to be at least 2 x 2 (grid h, w >= 16)
+ *                           and return RB_ERR_BAD_SHAPE before any CUDA call otherwise.
+ * Upstream lookup, per tap at level l (W_l x H_l), each step rounded to fp32 on its own:
+ *   x = c.x / 2^l + dx;  g = 2x / (W_l - 1) - 1;  ix = ((g + 1) * 0.5) * (W_l - 1);  ix = -100 unless |ix| <= 2^24 (NaN too);
+ *   x0 = floor(ix), x1 = x0 + 1 (unclamped), the same for y;  nw = (x1 - ix)(y1 - iy), ne = (ix - x0)(y1 - iy),
+ *   sw = (x1 - ix)(iy - y0), se = (ix - x0)(iy - y0);  a corner outside the level reads 0;
+ *   out = fma(I_se, se, fma(I_sw, sw, fma(I_ne, ne, I_nw * nw))). */
+enum { RB_SEMANTICS_REFERENCE = 0, RB_SEMANTICS_UPSTREAM = 1 };
+int rb_set_semantics(int semantics);
+int rb_get_semantics(void);
 /* Device selection.  The library carries its own CUDA runtime instance; its per-thread current device does not follow the
  * host framework's (torch.cuda.device(...), cudaSetDevice in another runtime).  Call this when the calling thread switches
  * GPUs, before the calls that enqueue work (their stream argument 0 = "default stream of the current device").
@@ -109,7 +125,8 @@ int rb_conv2d(const float* x, const float* W_host, const float* b_host, float* y
               int cin, int cout, int kh, int kw, int relu, void* workspace, size_t workspace_bytes,
               void* stream);
 /* Same with tensorpack's `strides` argument (1 or 2; the encoders' stride-2 layers, model_utils.py:21,39,68,92):
- * y [B, ceil(h/stride), ceil(w/stride), cout], TensorFlow 'SAME' padding (pad before = total / 2, the odd one after).
+ * y [B, ceil(h/stride), ceil(w/stride), cout], TensorFlow 'SAME' padding (pad before = total / 2, the odd one after), or
+ * PyTorch's pad before = k / 2 under RB_SEMANTICS_UPSTREAM.
  * The strided taps are read through TMA element strides -- no gathered copy of the input.  Same workspace query. */
 int rb_conv2d_strided(const float* x, const float* W_host, const float* b_host, float* y, int B, int h, int w,
                       int cin, int cout, int kh, int kw, int stride, int relu, void* workspace,

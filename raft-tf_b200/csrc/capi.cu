@@ -6,6 +6,7 @@
 namespace rb {
 static thread_local char g_err[512] = "";
 static thread_local int g_mode = RB_MATH_TC;
+static thread_local int g_semantics = RB_SEMANTICS_REFERENCE;
 static thread_local long long g_launches = 0;
 
 void set_error(const char* fmt, ...) {
@@ -16,6 +17,7 @@ void set_error(const char* fmt, ...) {
 }
 void count_launch() { ++g_launches; }
 int math_mode() { return g_mode; }
+int semantics() { return g_semantics; }
 
 int current_device(int* dev) {
   RB_CHECK_CUDA(cudaGetDevice(dev));
@@ -45,6 +47,15 @@ extern "C" int rb_set_math_mode(int mode) {
   return RB_OK;
 }
 extern "C" int rb_get_math_mode(void) { return rb::g_mode; }
+extern "C" int rb_set_semantics(int semantics) {
+  if (semantics != RB_SEMANTICS_REFERENCE && semantics != RB_SEMANTICS_UPSTREAM) {
+    rb::set_error("rb_set_semantics: unknown semantics %d", semantics);
+    return RB_ERR_BAD_ARG;
+  }
+  rb::g_semantics = semantics;
+  return RB_OK;
+}
+extern "C" int rb_get_semantics(void) { return rb::g_semantics; }
 // The library links its own (static) CUDA runtime, whose per-thread "current device" is independent of the host
 // framework's: a caller that drives several GPUs from one thread tells the library which one the following calls (and their
 // stream handles -- stream 0 means "the current device's default stream") belong to.  raft_b200/capi.py does this in stream().

@@ -14,6 +14,18 @@ namespace rb {
 void set_error(const char* fmt, ...);
 void count_launch();
 int math_mode();
+int semantics();  // RB_SEMANTICS_* of the calling thread (rb_set_semantics), read when a kernel is launched
+
+// Pad before the first tap of a stride-s conv with an odd k x k kernel over an extent n; the output extent is ceil(n / s)
+// in both conventions.  RB_SEMANTICS_REFERENCE: TensorFlow 'SAME', total = max((out - 1) * s + k - n, 0), before = total / 2
+// (the odd one after).  RB_SEMANTICS_UPSTREAM: PyTorch's symmetric padding = k / 2.  They differ on even n only.
+inline void conv_pad_before(int n, int k, int s, int sem, int* before, int* out) {
+  const int o = (n + s - 1) / s;
+  int total = (o - 1) * s + k - n;
+  if (total < 0) total = 0;
+  *before = sem == RB_SEMANTICS_UPSTREAM ? k / 2 : total / 2;
+  *out = o;
+}
 
 // Function attributes (cudaFuncAttributeMaxDynamicSharedMemorySize) and the SM count are PER DEVICE: a process may
 // drive several GPUs (RaftEngine(device=...)), so "already set" is tracked per (call site, device ordinal).

@@ -62,15 +62,6 @@ extern "C" int rb_conv2d_workspace_bytes(int B, int h, int w, int cin, int cout,
   return RB_OK;
 }
 
-// TF 'SAME': out = ceil(n / s), total pad = max((out - 1) * s + k - n, 0), before = total / 2 (the rest after)
-static inline void same_pad_tf(int n, int k, int s, int* before, int* out) {
-  const int o = (n + s - 1) / s;
-  int total = (o - 1) * s + k - n;
-  if (total < 0) total = 0;
-  *before = total / 2;
-  *out = o;
-}
-
 extern "C" int rb_conv2d(const float* x, const float* W_host, const float* b_host, float* y, int B, int h, int w,
                          int cin, int cout, int kh, int kw, int relu, void* workspace, size_t workspace_bytes,
                          void* stream) {
@@ -117,8 +108,8 @@ extern "C" int rb_conv2d_strided(const float* x, const float* W_host, const floa
   p.B = B; p.h = h; p.w = w;
   if (stride != 1) {  // strided input view (ConvParams, common.cuh): y is [B, ceil(h/s), ceil(w/s), cout]
     int pt, pl, oh, ow;
-    same_pad_tf(h, kh, stride, &pt, &oh);
-    same_pad_tf(w, kw, stride, &pl, &ow);
+    conv_pad_before(h, kh, stride, semantics(), &pt, &oh);
+    conv_pad_before(w, kw, stride, semantics(), &pl, &ow);
     p.in_h = h; p.in_w = w; p.h = oh; p.w = ow;
     p.sx = p.sy = stride;
     p.pad_explicit = 1; p.pad_x = pl; p.pad_y = pt;

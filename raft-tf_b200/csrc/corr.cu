@@ -103,7 +103,31 @@ __global__ void avgpool2_kernel(const float* __restrict__ src, float* __restrict
 //            for 324 useful bytes).  fp32 mode (rb_corr_lookup) stores directly.
 // r01 history: v1 one warp per unit, 391 warp instructions per unit, issue-bound; v2 block-cooperative with LDG
 // staging, LSU-wavefront-bound (108 wavefronts per unit); v3 = this.
+//
+// UP = true is the sampler of RB_SEMANTICS_UPSTREAM (include/raft_b200.h): x is normalised and unnormalised as upstream's
+// bilinear_sampler + F.grid_sample(align_corners=True) do (up_unnorm), x0 = floor(ix) and x1 = x0 + 1 are not clamped, corners
+// outside the level read 0 and the four products are summed nw, ne, sw, se with FMA contraction.  Footprint: the round trip
+// moves ix a few ulp away from x (|ix - x| <= ~4 (W_l - 1) 2^-24, far below one pixel for any level up to 2^16 columns), so
+// floor(ix) is floor(x) - 1, floor(x) or floor(x) + 1 -- only within those ulp of an integer.  The origin is therefore taken
+// from the round-tripped coordinate of window column / row 0 itself (not from x): with x_i = fl(x_0 + i) every column has
+// floor(ix_0) + i - 1 <= x0_i <= floor(ix_0) + i + 1, so x0 >= origin and x1 <= origin + 2r + 2 -- the same one column / row of
+// slack as the reference sampler (the `far` row, 3 alignment columns + 2r + 3 <= 16).  The origin is clamped to [-16, W_l]
+// (no int overflow for far-away or NaN coordinates); a clamped origin only occurs when every tap of the unit lies outside the
+// level, and the tap indices, clamped into the staged box, then read zeros.  The TMA box's out-of-bounds fill supplies the
+// zero padding; the plain-load fallback and the `far` loads check the level bounds themselves.
 // ---------------------------------------------------------------------------------------------
+// RB_SEMANTICS_UPSTREAM coordinate of a tap: upstream's bilinear_sampler normalises (g = 2x / (n - 1) - 1), PyTorch's CUDA
+// grid sampler unnormalises (GridSampler.cuh: ((g + 1) / 2) * (n - 1)), every step rounded on its own; coordinates PyTorch
+// replaces by -100 (non-finite or beyond the int range) and those beyond 2^24 (outside every level either way) become -100.
+__device__ __forceinline__ float up_unnorm(float x, int n) {
+  const float nm1 = (float)(n - 1);
+  const float g = __fsub_rn(__fdiv_rn(__fmul_rn(2.0f, x), nm1), 1.0f);
+  const float ix = __fmul_rn(__fmul_rn(__fadd_rn(g, 1.0f), 0.5f), nm1);
+  return fabsf(ix) <= 16777216.0f ? ix : -100.0f;
+}
+// footprint origin of a unit under RB_SEMANTICS_UPSTREAM from the coordinate of window column / row 0 (see above)
+__device__ __forceinline__ int up_origin(float x0, int n) { return min(max((int)floorf(up_unnorm(x0, n)), -16), n); }
+
 struct PyramidView {
   const float* base[RB_NUM_LEVELS];
   int hl[RB_NUM_LEVELS], wl[RB_NUM_LEVELS];
@@ -129,25 +153,26 @@ __device__ __forceinline__ float lds_f32(uint32_t addr) {
   return v;
 }
 
-template <int R>
+template <int R, bool UP = false>
 struct LookupSmem {
   static constexpr int D = 2 * R + 1, K = D * D, UNITS = kLookupPB * 4;
   static constexpr int OUTP = (4 * K + 7) / 8 * 8;  // staged channels per pixel and plane (324 -> 328, 196 -> 200)
   static constexpr int kPatchOff = 0;
   static constexpr int kXtabOff = UNITS * kUnitBytes;              // float2 [UNITS][D]: (qx, 4*col of x0 | 4*col of x1 << 8)
-  static constexpr int kOutOff = kXtabOff + UNITS * D * 8;         // float [PB][OUTP]: results before the hi/lo split
+  static constexpr int kX1Off = kXtabOff + UNITS * D * 8;          // UP: float [UNITS][D]: weight of x1 (ix - x0)
+  static constexpr int kOutOff = kX1Off + (UP ? UNITS * D * 4 : 0);  // float [PB][OUTP]: results before the hi/lo split
   static_assert(3 * (kOutOff + kLookupPB * OUTP * 4 + UNITS * 8 + 16 + kLookupPB * 8 + 1024) <= 228 * 1024, "three blocks per SM");
   static constexpr int kBaseOff = kOutOff + kLookupPB * OUTP * 4;  // int [UNITS][2]: bx4, by
   static constexpr int kBarOff = kBaseOff + UNITS * 8;
   static constexpr int kBytes = kBarOff + 16 + kLookupPB * 8;  // + float2 [PB]: the block's coordinates
 };
 
-template <int R, bool SPLIT>
+template <int R, bool SPLIT, bool UP>
 __global__ void __launch_bounds__(kLookupPB * 4 * (2 * R + 1), 3)
 corr_lookup_kernel(const __grid_constant__ PyramidView pv, const __grid_constant__ PyramidMaps maps,
                    const float2* __restrict__ coords, float* __restrict__ out_f32, __half* __restrict__ out_hi,
                    __half* __restrict__ out_lo, int out_stride, int npix) {
-  using L = LookupSmem<R>;
+  using L = LookupSmem<R, UP>;
   // P = rows staged per unit: the (2r+2)-row footprint.  The row the fp32 rounding of cy + dy can add (r01 staged it for
   // every unit: +9 % DRAM bytes in a kernel that runs at 80 % of the HBM copy peak at batch 8) is handled by the threads
   // that actually need it with four global loads per tap (`far`, below) -- about one window row in a million.
@@ -155,6 +180,7 @@ corr_lookup_kernel(const __grid_constant__ PyramidView pv, const __grid_constant
   extern __shared__ __align__(1024) uint8_t lk_smem[];  // no static shared memory in this kernel: the slots start at 0
   float* patch = reinterpret_cast<float*>(lk_smem + L::kPatchOff);
   float2* xtab = reinterpret_cast<float2*>(lk_smem + L::kXtabOff);
+  float* x1tab = reinterpret_cast<float*>(lk_smem + L::kX1Off);
   float* ostage = reinterpret_cast<float*>(lk_smem + L::kOutOff);
   int* ubase = reinterpret_cast<int*>(lk_smem + L::kBaseOff);
   uint64_t* bar = reinterpret_cast<uint64_t*>(lk_smem + L::kBarOff);
@@ -196,8 +222,8 @@ corr_lookup_kernel(const __grid_constant__ PyramidView pv, const __grid_constant
     const float inv = 1.0f / (float)(1 << lvl);  // centroid / 2**i (model_utils.py:239), exact
     const int H = pv.hl[lvl], W = pv.wl[lvl];
     const float xf0 = __fadd_rn(c.x * inv, (float)(-R)), yf0 = __fadd_rn(c.y * inv, (float)(-R));
-    const int bx4 = min(max((int)xf0, 0), W - 1) & ~3;
-    const int by = min(max((int)yf0, 0), H - 1);
+    const int bx4 = (UP ? up_origin(xf0, W) : min(max((int)xf0, 0), W - 1)) & ~3;
+    const int by = UP ? up_origin(yf0, H) : min(max((int)yf0, 0), H - 1);
     ubase[2 * u] = bx4;
     ubase[2 * u + 1] = by;
     if (pv.tma_ok[lvl]) tc::tma_load_3d(&maps.m[lvl], bar, lk_smem + u * kUnitBytes, bx4, by, pix);
@@ -211,11 +237,19 @@ corr_lookup_kernel(const __grid_constant__ PyramidView pv, const __grid_constant
       if (pv.tma_ok[lvl]) continue;
       const int pix = min(pix0 + (u >> 2), npix - 1);
       const int H = pv.hl[lvl], W = pv.wl[lvl];
-      const int yy = min(ubase[2 * u + 1] + py, H - 1), col = ubase[2 * u] + ch * 4;
-      const float* row = pv.base[lvl] + ((size_t)pix * H + yy) * W;
       float4 v;
-      v.x = __ldg(row + min(col + 0, W - 1)); v.y = __ldg(row + min(col + 1, W - 1));
-      v.z = __ldg(row + min(col + 2, W - 1)); v.w = __ldg(row + min(col + 3, W - 1));
+      if constexpr (UP) {  // zero outside the level
+        const int yy = ubase[2 * u + 1] + py, col = ubase[2 * u] + ch * 4;
+        const bool rin = yy >= 0 && yy < H;
+        const float* row = pv.base[lvl] + ((size_t)pix * H + (rin ? yy : 0)) * W;
+        auto ld = [&](int x) { return rin && x >= 0 && x < W ? __ldg(row + x) : 0.0f; };
+        v = make_float4(ld(col), ld(col + 1), ld(col + 2), ld(col + 3));
+      } else {
+        const int yy = min(ubase[2 * u + 1] + py, H - 1), col = ubase[2 * u] + ch * 4;
+        const float* row = pv.base[lvl] + ((size_t)pix * H + yy) * W;
+        v.x = __ldg(row + min(col + 0, W - 1)); v.y = __ldg(row + min(col + 1, W - 1));
+        v.z = __ldg(row + min(col + 2, W - 1)); v.w = __ldg(row + min(col + 3, W - 1));
+      }
       *reinterpret_cast<float4*>(&patch[u * (kUnitBytes / 4) + patch_idx(py, ch * 4, (u * (kUnitBytes / 128)) & 3)]) = v;
     }
   }
@@ -227,7 +261,14 @@ corr_lookup_kernel(const __grid_constant__ PyramidView pv, const __grid_constant
   const float2 c = cnew[pl];
   const float inv = 1.0f / (float)(1 << lvl);
   const float cx = c.x * inv, cy = c.y * inv;
-  {
+  if constexpr (UP) {
+    const float ix = up_unnorm(__fadd_rn(cx, (float)(j - R)), W);
+    const int x0 = (int)floorf(ix);
+    const int bx4 = ubase[2 * u];
+    const int ax0 = min(max(x0 - bx4, 0), kPatchCols - 1), ax1 = min(max(x0 + 1 - bx4, 0), kPatchCols - 1);
+    xtab[u * D + j] = make_float2(__fsub_rn((float)(x0 + 1), ix), __int_as_float((ax0 * 4) | (ax1 * 4 << 8)));
+    x1tab[u * D + j] = __fsub_rn(ix, (float)x0);
+  } else {
     // x side of window column i = j (i walks x: model_utils.py:235-237)
     const float x = __fadd_rn(cx, (float)(j - R));
     int x0 = (int)x;  // tf.cast truncates toward zero (utils.py:54-57)
@@ -239,12 +280,23 @@ corr_lookup_kernel(const __grid_constant__ PyramidView pv, const __grid_constant
     const int ax0 = min(max(x0 - bx4, 0), kPatchCols - 1), ax1 = min(max(x1 - bx4, 0), kPatchCols - 1);
     xtab[u * D + j] = make_float2(qx, __int_as_float((ax0 * 4) | (ax1 * 4 << 8)));
   }
-  const float y = __fadd_rn(cy, (float)(j - R));
-  int y0 = (int)y;
-  int y1 = y0 + 1;
-  y0 = min(max(y0, 0), H - 1);
-  y1 = min(max(y1, 0), H - 1);
-  const float qy = __fsub_rn((float)y1, y), pyw = __fsub_rn(1.0f, qy);  // utils.py:85
+  int y0, y1;
+  float qy, pyw;  // weights of rows y0 and y1
+  if constexpr (UP) {
+    const float iy = up_unnorm(__fadd_rn(cy, (float)(j - R)), H);
+    y0 = (int)floorf(iy);
+    y1 = y0 + 1;
+    qy = __fsub_rn((float)y1, iy);
+    pyw = __fsub_rn(iy, (float)y0);
+  } else {
+    const float y = __fadd_rn(cy, (float)(j - R));
+    y0 = (int)y;
+    y1 = y0 + 1;
+    y0 = min(max(y0, 0), H - 1);
+    y1 = min(max(y1, 0), H - 1);
+    qy = __fsub_rn((float)y1, y);  // utils.py:85
+    pyw = __fsub_rn(1.0f, qy);
+  }
   const int by = ubase[2 * u + 1];
   const bool far = (y1 - by) > P - 1 || (y0 - by) > P - 1;  // rounding slack row outside the staged box
   const int r0 = min(max(y0 - by, 0), P - 1), r1 = min(max(y1 - by, 0), P - 1);
@@ -260,12 +312,13 @@ corr_lookup_kernel(const __grid_constant__ PyramidView pv, const __grid_constant
   if (n_tma) tc::mbar_wait(bar, 0);    // TMA patches landed
   // ---- phase 2: taps of window row j ------------------------------------------------------------------------------
   const bool live = pix < npix;
+  const bool ry0 = (unsigned)y0 < (unsigned)H, ry1 = (unsigned)y1 < (unsigned)H;  // UP: rows inside the level (`far` loads)
 #pragma unroll
   for (int i = 0; i < D; ++i) {
     const float2 xt = xtab[u * D + i];
     const uint32_t pk = (uint32_t)__float_as_int(xt.y), c0 = pk & 0xffu, c1 = pk >> 8;
-    const float pxw = __fsub_rn(1.0f, xt.x);
-    const float wa = __fmul_rn(xt.x, qy), wb = __fmul_rn(xt.x, pyw);  // utils.py:86-89
+    const float pxw = UP ? x1tab[u * D + i] : __fsub_rn(1.0f, xt.x);
+    const float wa = __fmul_rn(xt.x, qy), wb = __fmul_rn(xt.x, pyw);  // utils.py:86-89 (UP: nw, sw, ne, se)
     const float wc = __fmul_rn(pxw, qy), wd = __fmul_rn(pxw, pyw);
     float Ia, Ib, Ic, Id;
     if (!far) {
@@ -273,11 +326,24 @@ corr_lookup_kernel(const __grid_constant__ PyramidView pv, const __grid_constant
     } else {
       const float* img = pv.base[lvl] + (size_t)min(pix, npix - 1) * H * W;
       const int bx4 = ubase[2 * u], xa = bx4 + (int)(c0 >> 2), xb = bx4 + (int)(c1 >> 2);
-      Ia = __ldg(img + (size_t)y0 * W + xa); Ib = __ldg(img + (size_t)y1 * W + xa);
-      Ic = __ldg(img + (size_t)y0 * W + xb); Id = __ldg(img + (size_t)y1 * W + xb);
+      if constexpr (UP) {  // zero outside the level
+        const bool ca = (unsigned)xa < (unsigned)W, cb = (unsigned)xb < (unsigned)W;
+        const float* p0 = img + (size_t)max(y0, 0) * W;
+        const float* p1 = img + (size_t)max(y1, 0) * W;
+        Ia = (ry0 && ca) ? __ldg(p0 + xa) : 0.0f; Ib = (ry1 && ca) ? __ldg(p1 + xa) : 0.0f;
+        Ic = (ry0 && cb) ? __ldg(p0 + xb) : 0.0f; Id = (ry1 && cb) ? __ldg(p1 + xb) : 0.0f;
+      } else {
+        Ia = __ldg(img + (size_t)y0 * W + xa); Ib = __ldg(img + (size_t)y1 * W + xa);
+        Ic = __ldg(img + (size_t)y0 * W + xb); Id = __ldg(img + (size_t)y1 * W + xb);
+      }
     }
-    const float v = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(wa, Ia), __fmul_rn(wb, Ib)), __fmul_rn(wc, Ic)),
-                              __fmul_rn(wd, Id));  // tf.add_n order (utils.py:98)
+    float v;
+    if constexpr (UP) {  // nw, ne, sw, se with FMA contraction (include/raft_b200.h)
+      v = fmaf(Id, wd, fmaf(Ib, wb, fmaf(Ic, wc, __fmul_rn(Ia, wa))));
+    } else {
+      v = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(wa, Ia), __fmul_rn(wb, Ib)), __fmul_rn(wc, Ic)),
+                    __fmul_rn(wd, Id));  // tf.add_n order (utils.py:98)
+    }
     const int ch = lvl * K + i * D + j;
     if constexpr (SPLIT) {
       ostage[pl * OUTP + ch] = v;
@@ -340,7 +406,7 @@ struct OtfView {
 // (the layout of CU_TENSOR_MAP_SWIZZLE_64B).
 __device__ __forceinline__ int v5_row_off(int unit_off, int row) { return row * 64 + ((((unit_off >> 7) + (row >> 1)) & 3) << 4); }
 
-template <int R, bool SPLIT>
+template <int R, bool SPLIT, bool UP>
 __global__ void __launch_bounds__(LookupV5<R>::NT, 2)
 corr_lookup_v5_kernel(const __grid_constant__ PyramidView pv, const float2* __restrict__ coords, float* __restrict__ out_f32,
                       __half* __restrict__ out_hi, __half* __restrict__ out_lo, int out_stride, int npix, const OtfView otf) {
@@ -377,8 +443,13 @@ corr_lookup_v5_kernel(const __grid_constant__ PyramidView pv, const float2* __re
     const int k = lane & 3;
     const float inv = 1.0f / (float)(1 << k);  // centroid / 2**i (model_utils.py:239), exact
     const int H = pv.hl[k], W = pv.wl[k];
-    bx = min(max((int)__fadd_rn(c.x * inv, (float)(-R)), 0), W - 1);
-    by = min(max((int)__fadd_rn(c.y * inv, (float)(-R)), 0), H - 1);
+    if constexpr (UP) {  // round-tripped coordinate of window column / row 0 (footprint argument above corr_lookup_kernel)
+      bx = up_origin(__fadd_rn(c.x * inv, (float)(-R)), W);
+      by = up_origin(__fadd_rn(c.y * inv, (float)(-R)), H);
+    } else {
+      bx = min(max((int)__fadd_rn(c.x * inv, (float)(-R)), 0), W - 1);
+      by = min(max((int)__fadd_rn(c.y * inv, (float)(-R)), 0), H - 1);
+    }
   }
   // ---- index tables: lane -> (unit k = lane >> 3, entry e = lane & 7); entry 8 (r = 4) by the lanes with e = 0 / 1 ------
   {
@@ -388,6 +459,14 @@ corr_lookup_v5_kernel(const __grid_constant__ PyramidView pv, const float2* __re
     const float cx = c.x * inv, cy = c.y * inv;
     const int H = pv.hl[k], W = pv.wl[k];
     auto x_entry = [&](int i) {
+      if constexpr (UP) {  // weights of x0 and x1, patch columns clamped into the 11 evaluated ones
+        const float ix = up_unnorm(__fadd_rn(cx, (float)(i - R)), W);
+        const int x0 = (int)floorf(ix);
+        const int a0 = min(max(x0 - bxk, 0), 10), a1 = min(max(x0 + 1 - bxk, 0), 10);
+        tab[k * L::TABN + i] = make_float4(__fsub_rn((float)(x0 + 1), ix), __fsub_rn(ix, (float)x0), __int_as_float(a0 * 4),
+                                           __int_as_float(a1 * 4));
+        return;
+      }
       const float x = __fadd_rn(cx, (float)(i - R));
       int x0 = (int)x;  // tf.cast truncates toward zero (utils.py:54-57)
       int x1 = x0 + 1;
@@ -398,6 +477,16 @@ corr_lookup_v5_kernel(const __grid_constant__ PyramidView pv, const float2* __re
       tab[k * L::TABN + i] = make_float4(qx, __fsub_rn(1.0f, qx), __int_as_float(a0 * 4), __int_as_float(a1 * 4));
     };
     auto y_entry = [&](int j) {
+      if constexpr (UP) {
+        const int uoff = (warp * 4 + k) * L::SLOT;
+        const float iy = up_unnorm(__fadd_rn(cy, (float)(j - R)), H);
+        const int y0 = (int)floorf(iy);
+        const int r0 = min(max(y0 - byk, 0), L::ROWS - 1), r1 = min(max(y0 + 1 - byk, 0), L::ROWS - 1);
+        tab[k * L::TABN + D + j] = make_float4(__fsub_rn((float)(y0 + 1), iy), __fsub_rn(iy, (float)y0),
+                                               __int_as_float((int)patch0_u32 + uoff + v5_row_off(uoff, r0)),
+                                               __int_as_float((int)patch0_u32 + uoff + v5_row_off(uoff, r1)));
+        return;
+      }
       const float y = __fadd_rn(cy, (float)(j - R));
       int y0 = (int)y;
       int y1 = y0 + 1;
@@ -440,6 +529,10 @@ corr_lookup_v5_kernel(const __grid_constant__ PyramidView pv, const float2* __re
         for (int u = 0; u < 8; ++u) {
           const int e = min(e0 + u, NE - 1);
           const int row = e / 11, col = e - row * 11;
+          if (UP && (byk + row < 0 || byk + row >= H || bxk + col < 0 || bxk + col >= W)) {  // zero outside the level
+            p[u] = 0.0f;
+            continue;
+          }
           const float* src = f2b + ((size_t)min(byk + row, H - 1) * W + min(bxk + col, W - 1)) * C;
           const float4 v = __ldg(reinterpret_cast<const float4*>(src));
           float acc = fmaf(fa.w, v.w, fmaf(fa.z, v.z, fmaf(fa.y, v.y, fa.x * v.x)));
@@ -497,8 +590,12 @@ corr_lookup_v5_kernel(const __grid_constant__ PyramidView pv, const float2* __re
         // Y.z / Y.w: swizzled row addresses (64-byte aligned + chunk phase), X.z / X.w: 4 * column
         const int a0 = __float_as_int(X.z), a1 = __float_as_int(X.w), r0 = __float_as_int(Y.z), r1 = __float_as_int(Y.w);
         const float Ia = lds_f32(r0 ^ a0), Ib = lds_f32(r1 ^ a0), Ic = lds_f32(r0 ^ a1), Id = lds_f32(r1 ^ a1);
-        stage[k * K + t] = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(wa, Ia), __fmul_rn(wb, Ib)), __fmul_rn(wc, Ic)),
-                                     __fmul_rn(wd, Id));  // tf.add_n order (utils.py:98)
+        if constexpr (UP) {  // nw, ne, sw, se with FMA contraction (include/raft_b200.h)
+          stage[k * K + t] = fmaf(Id, wd, fmaf(Ib, wb, fmaf(Ic, wc, __fmul_rn(Ia, wa))));
+        } else {
+          stage[k * K + t] = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(wa, Ia), __fmul_rn(wb, Ib)), __fmul_rn(wc, Ic)),
+                                       __fmul_rn(wd, Id));  // tf.add_n order (utils.py:98)
+        }
       }
     }
   }
@@ -559,20 +656,15 @@ int pyramid_view(const float* pyramid, int B, int h, int w, PyramidView* pv) {
   return RB_OK;
 }
 
-template <int R>
-static size_t lookup_smem_bytes() {
-  return (size_t)LookupSmem<R>::kBytes;
-}
-
-template <int R, bool SPLIT>
+template <int R, bool SPLIT, bool UP>
 static int launch_lookup_cfg(const PyramidView& pv, const PyramidMaps& maps, const float2* c2, float* out_f32, __half* out_hi,
                              __half* out_lo, int out_stride, int npix, cudaStream_t s) {
   static PerDeviceOnce attr_set;
-  const size_t smem = lookup_smem_bytes<R>();
+  const size_t smem = (size_t)LookupSmem<R, UP>::kBytes;
   int dev = 0, rc_dev;
   if ((rc_dev = current_device(&dev))) return rc_dev;
   if (!attr_set.test(dev)) {
-    RB_CHECK_CUDA(cudaFuncSetAttribute(corr_lookup_kernel<R, SPLIT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    RB_CHECK_CUDA(cudaFuncSetAttribute(corr_lookup_kernel<R, SPLIT, UP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     attr_set.set(dev);
   }
   dim3 grid((npix + kLookupPB - 1) / kLookupPB), block(kLookupPB * 4 * (2 * R + 1));
@@ -591,12 +683,12 @@ static int launch_lookup_cfg(const PyramidView& pv, const PyramidMaps& maps, con
   attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
   cfg.numAttrs = pdl;
-  RB_CHECK_CUDA(cudaLaunchKernelEx(&cfg, corr_lookup_kernel<R, SPLIT>, pv, maps, c2, out_f32, out_hi, out_lo, out_stride, npix));
+  RB_CHECK_CUDA(cudaLaunchKernelEx(&cfg, corr_lookup_kernel<R, SPLIT, UP>, pv, maps, c2, out_f32, out_hi, out_lo, out_stride, npix));
   RB_CHECK_LAUNCH("corr_lookup_kernel");
   return RB_OK;
 }
 
-template <int R, bool SPLIT>
+template <int R, bool SPLIT, bool UP>
 static int launch_lookup_v5(const PyramidView& pv, const float2* c2, float* out_f32, __half* out_hi, __half* out_lo,
                             int out_stride, int npix, cudaStream_t s, const OtfView& otf) {
   using L = LookupV5<R>;
@@ -604,7 +696,7 @@ static int launch_lookup_v5(const PyramidView& pv, const float2* c2, float* out_
   int dev = 0, rc_dev;
   if ((rc_dev = current_device(&dev))) return rc_dev;
   if (!attr_set.test(dev)) {
-    RB_CHECK_CUDA(cudaFuncSetAttribute(corr_lookup_v5_kernel<R, SPLIT>, cudaFuncAttributeMaxDynamicSharedMemorySize, L::kBytes));
+    RB_CHECK_CUDA(cudaFuncSetAttribute(corr_lookup_v5_kernel<R, SPLIT, UP>, cudaFuncAttributeMaxDynamicSharedMemorySize, L::kBytes));
     attr_set.set(dev);
   }
   static const int pdl = getenv("RAFT_B200_NO_PDL") ? 0 : 1;
@@ -619,13 +711,29 @@ static int launch_lookup_v5(const PyramidView& pv, const float2* c2, float* out_
   attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
   cfg.numAttrs = pdl;
-  RB_CHECK_CUDA(cudaLaunchKernelEx(&cfg, corr_lookup_v5_kernel<R, SPLIT>, pv, c2, out_f32, out_hi, out_lo, out_stride, npix, otf));
+  RB_CHECK_CUDA(cudaLaunchKernelEx(&cfg, corr_lookup_v5_kernel<R, SPLIT, UP>, pv, c2, out_f32, out_hi, out_lo, out_stride, npix, otf));
   RB_CHECK_LAUNCH("corr_lookup_v5_kernel");
   return RB_OK;
 }
 
+// RB_SEMANTICS_UPSTREAM divides by W_l - 1 and H_l - 1: every level must be at least 2 x 2 (checked before any CUDA call)
+int check_lookup_size(const char* fn, int h, int w) {
+  RB_REQUIRE(semantics() != RB_SEMANTICS_UPSTREAM || ((h >> 3) >= 2 && (w >> 3) >= 2), RB_ERR_BAD_SHAPE,
+             "%s: grid %dx%d too small for the upstream lookup (every pyramid level must be at least 2x2: h, w >= 16)", fn, h, w);
+  return RB_OK;
+}
+
+template <int R, bool UP>
+static int launch_lookup_r(const PyramidView& pv, const PyramidMaps& maps, const float2* c2, float* out_f32, __half* out_hi,
+                           __half* out_lo, int out_stride, int npix, cudaStream_t s) {
+  return out_hi ? launch_lookup_cfg<R, true, UP>(pv, maps, c2, nullptr, out_hi, out_lo, out_stride, npix, s)
+                : launch_lookup_cfg<R, false, UP>(pv, maps, c2, out_f32, nullptr, nullptr, out_stride, npix, s);
+}
+
 int launch_lookup(const float* pyramid, const float* coords, float* out_f32, __half* out_hi,
                   __half* out_lo, int out_stride, int B, int h, int w, int radius, cudaStream_t s) {
+  int rc_sz = check_lookup_size("lookup", h, w);
+  if (rc_sz) return rc_sz;
   PyramidView pv;
   int rc = pyramid_view(pyramid, B, h, w, &pv);
   if (rc) return rc;
@@ -634,7 +742,6 @@ int launch_lookup(const float* pyramid, const float* coords, float* out_f32, __h
              out_stride);
   const int npix = B * h * w;
   const float2* c2 = reinterpret_cast<const float2*>(coords);
-  const bool split = out_hi != nullptr;
   PyramidMaps maps;
   memset(&maps, 0, sizeof(maps));
   for (int l = 0; l < RB_NUM_LEVELS; ++l) {
@@ -644,11 +751,12 @@ int launch_lookup(const float* pyramid, const float* coords, float* out_f32, __h
     uint32_t box[3] = {(uint32_t)kPatchCols, (uint32_t)(2 * radius + 2), 1};
     if (cached_tmap(&maps.m[l], pv.base[l], 3, dims, str, box, tc::TMAP_F32_SW64) != RB_OK) pv.tma_ok[l] = 0;  // plain loads instead
   }
+  const bool up = semantics() == RB_SEMANTICS_UPSTREAM;
   if (radius == 4)
-    return split ? launch_lookup_cfg<4, true>(pv, maps, c2, nullptr, out_hi, out_lo, out_stride, npix, s)
-                 : launch_lookup_cfg<4, false>(pv, maps, c2, out_f32, nullptr, nullptr, out_stride, npix, s);
-  return split ? launch_lookup_cfg<3, true>(pv, maps, c2, nullptr, out_hi, out_lo, out_stride, npix, s)
-               : launch_lookup_cfg<3, false>(pv, maps, c2, out_f32, nullptr, nullptr, out_stride, npix, s);
+    return up ? launch_lookup_r<4, true>(pv, maps, c2, out_f32, out_hi, out_lo, out_stride, npix, s)
+              : launch_lookup_r<4, false>(pv, maps, c2, out_f32, out_hi, out_lo, out_stride, npix, s);
+  return up ? launch_lookup_r<3, true>(pv, maps, c2, out_f32, out_hi, out_lo, out_stride, npix, s)
+            : launch_lookup_r<3, false>(pv, maps, c2, out_f32, out_hi, out_lo, out_stride, npix, s);
 }
 
 // ---- F2: volume-free correlation ---------------------------------------------------------------------------------------------
@@ -669,12 +777,21 @@ __global__ void otf_pool_kernel(const float* __restrict__ src, float* __restrict
   const float* p = src + (((size_t)b * hs + 2 * y) * ws + 2 * x) * C + c;
   dst[i] = (p[0] + p[C] + p[(size_t)ws * C] + p[(size_t)ws * C + C]) * 0.25f;
 }
+template <int R, bool UP>
+static int launch_lookup_v5_r(const PyramidView& pv, const float2* c2, float* out_f32, __half* out_hi, __half* out_lo,
+                              int out_stride, int npix, cudaStream_t s, const OtfView& otf) {
+  return out_hi ? launch_lookup_v5<R, true, UP>(pv, c2, nullptr, out_hi, out_lo, out_stride, npix, s, otf)
+                : launch_lookup_v5<R, false, UP>(pv, c2, out_f32, nullptr, nullptr, out_stride, npix, s, otf);
+}
+
 int launch_lookup_otf(const float* fmap1, const float* fmap2, const float* pooled, const float* coords, float* out_f32,
                       __half* out_hi, __half* out_lo, int out_stride, int B, int h, int w, int C, int radius, cudaStream_t s) {
   RB_REQUIRE(radius == 3 || radius == 4, RB_ERR_UNSUPPORTED, "radius %d unsupported", radius);
   RB_REQUIRE(C == 128 || C == 256, RB_ERR_BAD_SHAPE, "volume-free lookup: C=%d (128 = raft-small, 256 = raft-things)", C);
   RB_REQUIRE((h >> 3) >= 1 && (w >> 3) >= 1, RB_ERR_BAD_SHAPE, "volume-free lookup: grid %dx%d too small for 4 levels", h, w);
   RB_REQUIRE(out_hi == nullptr || out_stride % 8 == 0, RB_ERR_BAD_SHAPE, "lookup: split output stride %d", out_stride);
+  int rc_sz = check_lookup_size("volume-free lookup", h, w);
+  if (rc_sz) return rc_sz;
   PyramidView pv;
   memset(&pv, 0, sizeof(pv));
   OtfView otf;
@@ -685,12 +802,12 @@ int launch_lookup_otf(const float* fmap1, const float* fmap2, const float* poole
   }
   const float2* c2 = reinterpret_cast<const float2*>(coords);
   const int npix = B * h * w;
-  const bool split = out_hi != nullptr;
+  const bool up = semantics() == RB_SEMANTICS_UPSTREAM;
   if (radius == 4)
-    return split ? launch_lookup_v5<4, true>(pv, c2, nullptr, out_hi, out_lo, out_stride, npix, s, otf)
-                 : launch_lookup_v5<4, false>(pv, c2, out_f32, nullptr, nullptr, out_stride, npix, s, otf);
-  return split ? launch_lookup_v5<3, true>(pv, c2, nullptr, out_hi, out_lo, out_stride, npix, s, otf)
-               : launch_lookup_v5<3, false>(pv, c2, out_f32, nullptr, nullptr, out_stride, npix, s, otf);
+    return up ? launch_lookup_v5_r<4, true>(pv, c2, out_f32, out_hi, out_lo, out_stride, npix, s, otf)
+              : launch_lookup_v5_r<4, false>(pv, c2, out_f32, out_hi, out_lo, out_stride, npix, s, otf);
+  return up ? launch_lookup_v5_r<3, true>(pv, c2, out_f32, out_hi, out_lo, out_stride, npix, s, otf)
+            : launch_lookup_v5_r<3, false>(pv, c2, out_f32, out_hi, out_lo, out_stride, npix, s, otf);
 }
 
 int corr_build_tc(const float* fmap1, const float* fmap2, float* pyramid, int B, int h, int w, int C,

@@ -7,7 +7,8 @@
 //   stride-1 convs  -> conv_tc implicit GEMM directly on the activation (TMA zero fill = TF SAME);
 //   strided convs   -> (3x3 s2, 1x1 s2) the same kernel over a strided input VIEW (ConvParams, common.cuh): TMA element
 //                      strides deliver every second pixel of the box, TF's asymmetric SAME offsets
-//                      (pad_before = total/2) are the tile's start coordinates -- no gather pass;
+//                      (pad_before = total/2; PyTorch's k/2 under RB_SEMANTICS_UPSTREAM) are the tile's start
+//                      coordinates -- no gather pass;
 //   7x7 s2 stem     -> one pass writes the 2x-1 image as a zero-padded space-to-depth tensor (2x2 pixels x 3 channels =
 //                      12 of 16 channels per cell); a 7x7 stride-2 window is 4x4 such cells, and the 4 cells of one
 //                      window row are 64 CONTIGUOUS channels, so the stem is a 4x1 conv (K = 4 x 64) over a view whose
@@ -104,7 +105,7 @@ static void enc_packed_layout(int small, int out_dim, std::vector<EncPacked>& P,
 
 // ---- kernels ----------------------------------------------------------------------------------------
 // Stem input: the 2x-1 image (RAFT.py:53-59) as a zero-padded space-to-depth tensor.  Padded image row r' = r + pt
-// (TF SAME: pt = total/2 rows of zeros before), cell (Y, X) holds rows 2Y, 2Y+1 and columns 2X, 2X+1: channel
+// (conv_pad_before: TF SAME's total/2 rows of zeros before, or PyTorch's 3), cell (Y, X) holds rows 2Y, 2Y+1 and columns 2X, 2X+1: channel
 // (dy*2 + dx)*3 + c of 16 (12..15 = 0).  Output pixel (oy, ox) of the 7x7 stride-2 conv reads cells (oy..oy+3, ox..ox+3).
 // One thread per cell; each cell is written once, [B][Hp][Wp][16] (the conv's view overlaps them).
 __global__ void enc_stem_s2d_kernel(const float* __restrict__ img, __half* __restrict__ out_hi, __half* __restrict__ out_lo, int B,
@@ -249,16 +250,8 @@ static EncWs enc_ws_layout(int small, int B, int H, int W, void* base) {
   return w;
 }
 
-static inline void same_pad(int n, int k, int s, int* before, int* out) {
-  const int o = (n + s - 1) / s;
-  int total = (o - 1) * s + k - n;
-  if (total < 0) total = 0;
-  *before = total / 2;
-  *out = o;
-}
-
 struct EncRun {
-  int small, norm, B;
+  int small, norm, B, sem;  // sem: RB_SEMANTICS_* (conv_pad_before)
   const char* blob;
   const std::vector<EncPacked>* P;
   EncWs ws;
@@ -276,8 +269,8 @@ static int enc_conv(const EncRun& R, int i, const float* img, SplitPtr in, int i
   p.in_hi = in.hi; p.in_lo = in.lo; p.in_stride = in_stride; p.in_choff = 0; p.cin_pad = pk.cin_pad;
   if (c.k == 7) {  // stem: 4x1 conv over the space-to-depth view of the image
     int pt, pl;
-    same_pad(h, c.k, c.stride, &pt, &oh);
-    same_pad(w, c.k, c.stride, &pl, &ow);
+    conv_pad_before(h, c.k, c.stride, R.sem, &pt, &oh);
+    conv_pad_before(w, c.k, c.stride, R.sem, &pl, &ow);
     const int Hp = oh + 3, Wp = ow + 3;
     const size_t cells = (size_t)R.B * Hp * Wp;
     enc_stem_s2d_kernel<<<(unsigned)((cells + 255) / 256), 256, 0, R.s>>>(img, R.ws.col.hi, R.ws.col.lo, R.B, h, w, pt, pl, Hp, Wp);
@@ -288,10 +281,10 @@ static int enc_conv(const EncRun& R, int i, const float* img, SplitPtr in, int i
     p.in_w = ow; p.in_h = Hp;
     p.in_rowpitch = Wp * 16;
     p.pad_explicit = 1; p.pad_x = 0; p.pad_y = 0;
-  } else if (c.stride != 1) {  // strided view of the activation, TF SAME offsets
+  } else if (c.stride != 1) {  // strided view of the activation, pad offsets of conv_pad_before
     int pt, pl;
-    same_pad(h, c.k, c.stride, &pt, &oh);
-    same_pad(w, c.k, c.stride, &pl, &ow);
+    conv_pad_before(h, c.k, c.stride, R.sem, &pt, &oh);
+    conv_pad_before(w, c.k, c.stride, R.sem, &pl, &ow);
     p.in_w = w; p.in_h = h;
     p.sx = p.sy = c.stride;
     p.pad_explicit = 1; p.pad_x = pl; p.pad_y = pt;
@@ -523,7 +516,7 @@ extern "C" int rb_encoder_forward(int small, int norm, const void* weights, cons
   RB_REQUIRE(B > 0 && H >= 8 && W >= 8 && out_dim > 0 && out_dim <= 256, RB_ERR_BAD_SHAPE, "rb_encoder_forward: bad shape");
   RB_REQUIRE(norm >= 0 && norm <= 2, RB_ERR_BAD_ARG, "rb_encoder_forward: norm %d", norm);
   EncRun R;
-  R.small = small; R.norm = norm; R.B = B;
+  R.small = small; R.norm = norm; R.B = B; R.sem = semantics();
   R.blob = reinterpret_cast<const char*>(weights);
   std::vector<EncPacked> P;
   size_t total;

@@ -22,6 +22,7 @@
 
 namespace rb {
 
+int check_lookup_size(const char* fn, int h, int w);
 int launch_lookup(const float* pyramid, const float* coords, float* out_f32, __half* out_hi,
                   __half* out_lo, int out_stride, int B, int h, int w, int radius, cudaStream_t s);
 int launch_lookup_otf(const float* fmap1, const float* fmap2, const float* pooled, const float* coords, float* out_f32,
@@ -787,6 +788,7 @@ extern "C" int rb_raft_iterate(int small, const void* weights, void* workspace, 
   RB_REQUIRE(small || mask_out, RB_ERR_BAD_ARG, "rb_raft_iterate: raft-things needs mask_out");
   int rc = check_shape("rb_raft_iterate", B, h, w);
   if (rc) return rc;
+  if ((rc = check_lookup_size("rb_raft_iterate", h, w))) return rc;  // before the first iteration's kernels
   const Variant& v = variant(small);
   for (int it = 0; it < iters; ++it) {
     float* m = (it == iters - 1 && !small) ? mask_out : nullptr;

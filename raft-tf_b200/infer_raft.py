@@ -24,29 +24,30 @@ import numpy as np
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 
 
-def _decode(path):
+def _decode(path, rgb=False):
     import cv2
     with open(path, "rb") as f:
         img = cv2.imdecode(np.asarray(bytearray(f.read()), dtype="uint8"), cv2.IMREAD_COLOR)  # BGR
     if img is None:
         raise FileNotFoundError(path)
-    return img
+    return cv2.cvtColor(img, cv2.COLOR_BGR2RGB) if rgb else img
 
 
-def read_pair(im1, im2, size):
+def read_pair(im1, im2, size, rgb=False):
     import cv2
     out = []
     for path in (im1, im2):
-        img = _decode(path)
+        img = _decode(path, rgb)
         if size is not None:
             img = cv2.resize(img, dsize=(size[1], size[0]))
         out.append(np.float32(img) / 255.0)
     return out[0][None], out[1][None]
 
 
-def decode_pair(im1, im2):
-    """Both frames as decoded (BGR uint8, their own size), [1,H,W,3] each: the engine resizes and scales them."""
-    return tuple(_decode(path)[None] for path in (im1, im2))
+def decode_pair(im1, im2, rgb=False):
+    """Both frames as decoded (BGR uint8, or RGB with rgb, their own size), [1,H,W,3] each: the engine resizes and scales
+    them."""
+    return tuple(_decode(path, rgb)[None] for path in (im1, im2))
 
 
 def main(argv=None):
@@ -71,6 +72,9 @@ def main(argv=None):
                    help='extension: also write the frames at times T in [0, 1] between im1 and im2 (raft_interp_<k>.png)')
     p.add_argument('--native-flow', action='store_true',
                    help="extension: resize the written flow(s) back to im1's size (flow_utils.resize_flow)")
+    p.add_argument('--upstream', action='store_true',
+                   help='extension: weights converted from an official princeton-vl RAFT .pth (raft_b200.convert): RGB '
+                        'frames and the upstream numerics (RAFT(..., upstream=True))')
     args = p.parse_args(argv)
     if args.interpolate and not all(0.0 <= t <= 1.0 for t in args.interpolate):
         p.error('--interpolate: every T must be in [0, 1]')
@@ -80,15 +84,17 @@ def main(argv=None):
     from networks import RAFT
     import cv2
     from flow_utils import flow_to_color, resize_flow, write_flo
+    rgb = args.upstream  # the official checkpoints expect RGB frames; the reference's expect BGR
     if args.keep_size:
-        left, right = read_pair(args.im1, args.im2, None)
-        model = RAFT.RAFT(left.shape[1:], args, iters=args.iters).load(args.load)
+        left, right = read_pair(args.im1, args.im2, None, rgb)
+        model = RAFT.RAFT(left.shape[1:], args, iters=args.iters, upstream=args.upstream).load(args.load)
     else:  # the reference's 432x1024 (infer_raft.py:69,76), resized and scaled on the GPU
-        left, right = decode_pair(args.im1, args.im2)
+        left, right = decode_pair(args.im1, args.im2, rgb)
         native = left.shape[1:3]
         if left.shape != right.shape:  # one engine pass takes one frame size: resize such a pair on the host, as before
-            left, right = read_pair(args.im1, args.im2, (432, 1024))
-        model = RAFT.RAFT((432, 1024, 3), args, iters=args.iters, input_size=(432, 1024)).load(args.load)
+            left, right = read_pair(args.im1, args.im2, (432, 1024), rgb)
+        model = RAFT.RAFT((432, 1024, 3), args, iters=args.iters, input_size=(432, 1024),
+                          upstream=args.upstream).load(args.load)
     if args.bidirectional:
         flow, flow_bw, occ_fw, occ_bw = (t.cpu().numpy() for t in model.forward_bidirectional(left, right))
     else:
@@ -116,7 +122,8 @@ def main(argv=None):
     if args.interpolate:
         frames = model.interpolate(left, right, args.interpolate).cpu().numpy()
         for k, frame in enumerate(frames):
-            cv2.imwrite(f"raft_interp_{k}.png", np.clip(np.rint(255.0 * frame[0]), 0, 255).astype(np.uint8))
+            img = np.clip(np.rint(255.0 * frame[0]), 0, 255).astype(np.uint8)
+            cv2.imwrite(f"raft_interp_{k}.png", cv2.cvtColor(img, cv2.COLOR_RGB2BGR) if rgb else img)
     return 0
 
 

@@ -22,7 +22,7 @@ class RAFT(object):
     weight_decay = 1e-5          # vestigial in the reference too (RAFT.py:14)
     data_format = 'NHWC'
 
-    def __init__(self, image_shape, args, iters=20, batch=1, device=None, volume_free=None, input_size=None):
+    def __init__(self, image_shape, args, iters=20, batch=1, device=None, volume_free=None, input_size=None, upstream=False):
         self.dropout = 0.0
         self.corr_radius = 4
         self.hidden_dim = 128
@@ -40,6 +40,8 @@ class RAFT(object):
         self.volume_free = volume_free  # extension (SURVEY 8(f) F2): None = RAFT_B200_VOLUME_FREE env, default off
         # extension: (Ho, Wo) the frames are resized to on the GPU (test_dataflow.py:85-87), None = their own size
         self.input_size = None if input_size is None else (int(input_size[0]), int(input_size[1]))
+        # extension: the numerics of princeton-vl RAFT for weights converted from its .pth checkpoints (RaftEngine upstream)
+        self.upstream = bool(upstream)
         self.flow_result = None
         self._engine = None
         self._params = None
@@ -83,7 +85,7 @@ class RAFT(object):
             if self._params is None:
                 raise RuntimeError("RAFT.load(<npz>) must be called before inference")
             self._engine = RaftEngine(self._params, small=self.small, iters=self.iters, device=self.device,
-                                      volume_free=self.volume_free, input_size=self.input_size)
+                                      volume_free=self.volume_free, input_size=self.input_size, upstream=self.upstream)
         return self._engine
 
     # -- inference ---------------------------------------------------------------------------------

@@ -9,6 +9,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("RAFT_B200_LIB") or os.path.join(_HERE, "..", "lib", "libraft_b200.so")  # env override: A/B of builds
 
 RB_MATH_TC, RB_MATH_SIMT = 0, 1
+RB_SEMANTICS_REFERENCE, RB_SEMANTICS_UPSTREAM = 0, 1
 
 if not os.path.exists(LIB_PATH):
     raise ImportError(f"raft_b200: {LIB_PATH} not found -- the CUDA extension is required (no CPU fallback); "
@@ -24,6 +25,8 @@ SIGNATURES = {
     "rb_last_error": (C.c_char_p, []),
     "rb_set_math_mode": (_i, [_i]),
     "rb_get_math_mode": (_i, []),
+    "rb_set_semantics": (_i, [_i]),
+    "rb_get_semantics": (_i, []),
     "rb_set_device": (_i, [_i]),
     "rb_launch_count": (C.c_longlong, []),
     "rb_launch_count_reset": (None, []),

@@ -30,6 +30,8 @@ FB_ALPHA1, FB_ALPHA2 = 0.01, 0.5
 # smallest frame side: the 4-level correlation pyramid needs a 1/8-resolution grid of at least 8 (level 3 is grid >> 3),
 # and ceil(H / 8) >= 8 means H >= 57
 MIN_FRAME = 57
+# upstream mode divides by W_l - 1 at every pyramid level: level 3 must be at least 2 wide, a grid of 16, H >= 121
+MIN_FRAME_UPSTREAM = 121
 
 
 class RaftEngine:
@@ -40,12 +42,21 @@ class RaftEngine:
 
     def __init__(self, params: Dict[str, np.ndarray], small: bool = False, iters: int = 20,
                  device: Optional[torch.device] = None, use_graph: bool = True, math_mode: int = capi.RB_MATH_TC,
-                 volume_free: Optional[bool] = None, input_size: Optional[Tuple[int, int]] = None):
+                 volume_free: Optional[bool] = None, input_size: Optional[Tuple[int, int]] = None,
+                 upstream: bool = False):
+        # upstream: the numerics of princeton-vl RAFT (PyTorch), for checkpoints converted from its .pth files
+        # (raft_b200.convert): grid_sample lookup, PyTorch's stride-2 padding, raft-small's flow scaled by 8
+        # (RB_SEMANTICS_UPSTREAM, include/raft_b200.h)
+        self.upstream = bool(upstream)
+        self.semantics = capi.RB_SEMANTICS_UPSTREAM if self.upstream else capi.RB_SEMANTICS_REFERENCE
+        self.min_frame = MIN_FRAME_UPSTREAM if self.upstream else MIN_FRAME
+        # raft-small's flow: in 1/8-resolution units in the reference (upflow8 does not scale it), in pixels upstream
+        self.flow_scale = 8.0 if small and not self.upstream else 1.0
         if input_size is not None:
             input_size = (int(input_size[0]), int(input_size[1]))
-            if min(input_size) < MIN_FRAME:
+            if min(input_size) < self.min_frame:
                 raise ValueError(f"raft_b200: input_size {input_size[0]}x{input_size[1]} is too small: frames must be at "
-                                 f"least {MIN_FRAME} pixels on each side")
+                                 f"least {self.min_frame} pixels on each side")
         if not torch.cuda.is_available():
             raise RuntimeError("raft_b200 needs a CUDA device (no CPU fallback)")
         # network size (Ho, Wo): frames of any size are resized to it on the GPU like the reference's test dataflow
@@ -97,9 +108,10 @@ class RaftEngine:
             if H < 1 or W < 1:
                 raise ValueError(f"raft_b200: empty {H}x{W} frames")
             H, W = self.input_size
-        if H < MIN_FRAME or W < MIN_FRAME:  # refused here, before the encoders run or any buffer is allocated
-            raise ValueError(f"raft_b200: {H}x{W} frames are too small: frames must be at least {MIN_FRAME} pixels on each "
-                             "side (a 1/8-resolution grid of at least 8x8 for the 4-level correlation pyramid)")
+        if H < self.min_frame or W < self.min_frame:  # refused here, before the encoders run or any buffer is allocated
+            raise ValueError(f"raft_b200: {H}x{W} frames are too small: frames must be at least {self.min_frame} pixels on "
+                             f"each side (a 1/8-resolution grid of at least {(self.min_frame + 7) // 8}x"
+                             f"{(self.min_frame + 7) // 8} for the 4-level correlation pyramid)")
         # alternating modes on one frame size keeps every mode's buffers and CUDA graph; a new frame size drops them
         if self._key is not None:
             self._parked[self._key] = {k: getattr(self, k) for k in self._STATE}
@@ -166,6 +178,7 @@ class RaftEngine:
         cnet, cframes = (self.cnet_bidir, self.images) if bidir else (self.cnet, self.images[:B])
         fout = self.fmaps[:2 * B]  # [fL | fR]
         capi.check(capi.lib.rb_set_math_mode(self.math_mode))  # per-thread library state: set before ANY kernel of ours
+        capi.check(capi.lib.rb_set_semantics(self.semantics))
         if self.input_size is not None:  # F3: cv2 resize, u8 -> fp32 /255 and replicate padding in one pass (csrc/resize.cu)
             capi.check(capi.lib.rb_frames_resize(capi.ptr(self.raw), int(u8), capi.ptr(self.images), 2 * B, *self.src_hw,
                                                  H, W, *self.pad, capi.stream()))
@@ -197,6 +210,7 @@ class RaftEngine:
         B = self.pairs
         h, w, s, lib, st = self.h, self.w, int(self.small), capi.lib, capi.stream()
         capi.check(lib.rb_set_math_mode(self.math_mode))
+        capi.check(lib.rb_set_semantics(self.semantics))
         if self.volume_free:
             capi.check(lib.rb_corr_otf_prepare(capi.ptr(self.fmap2), capi.ptr(self.corr_ws), self.cws_bytes, B, h, w, self.fdim, st))
         else:
@@ -217,13 +231,14 @@ class RaftEngine:
                                            capi.ptr(self.coords1), capi.ptr(self.mask), B, h, w, self.iters, st))
         top, left = self.pad[0], self.pad[2]  # crop the padding away while upsampling
         if self.small:
-            capi.check(lib.rb_upflow8_crop(capi.ptr(self.coords1), capi.ptr(self.flow_up), B, h, w, 1.0, top, left, H, W, st))
+            capi.check(lib.rb_upflow8_crop(capi.ptr(self.coords1), capi.ptr(self.flow_up), B, h, w, 8.0 / self.flow_scale,
+                                           top, left, H, W, st))
         else:
             capi.check(lib.rb_upsample_convex_crop(capi.ptr(self.coords1), capi.ptr(self.mask), capi.ptr(self.flow_up),
                                                    B, h, w, top, left, H, W, st))
-        if mode == BIDIRECTIONAL_CHECK:  # raft-small's flow is in 1/8-resolution units (upflow8 does not scale it)
+        if mode == BIDIRECTIONAL_CHECK:  # flow_scale: raft-small's reference flow is in 1/8-resolution units
             capi.check(lib.rb_flow_fb_check(capi.ptr(self.flow_up[:B0]), capi.ptr(self.flow_up[B0:]), capi.ptr(self.occ[:B0]),
-                                            capi.ptr(self.occ[B0:]), B0, H, W, 8.0 if self.small else 1.0, FB_ALPHA1,
+                                            capi.ptr(self.occ[B0:]), B0, H, W, self.flow_scale, FB_ALPHA1,
                                             FB_ALPHA2, st))
 
     def _all(self):
@@ -261,7 +276,8 @@ class RaftEngine:
     def forward(self, left: torch.Tensor, right: torch.Tensor) -> torch.Tensor:
         """left/right: [B,H,W,3] frames, BGR like the reference: fp32 in [0,1] (RAFT.inputs(), RAFT.py:45-51) or
         uint8 in [0,255] (what cv2.imdecode yields, test_dataflow.py:56-61; the /255 then happens on the GPU).  Host
-        (ideally pinned) or CUDA tensors; any H, W >= 57 (MIN_FRAME; smaller frames raise ValueError), or any size
+        (ideally pinned) or CUDA tensors; any H, W >= 57 (MIN_FRAME; 121 with upstream=True, whose weights expect RGB
+        frames; smaller frames raise ValueError), or any size
         with input_size set, which resizes them to input_size first.  Returns the [B,H,W,2] flow (at input_size when
         set) -- the engine-owned buffer itself, overwritten by the next call (networks.RAFT.RAFT.forward hands
         out a copy)."""
@@ -288,8 +304,8 @@ class RaftEngine:
         """Frames at times ts (each in [0, 1]; 0 = left, 1 = right) between B frame pairs: one bidirectional pass (as
         forward_bidirectional(check=False), from a graph of its own), then per t, eagerly on the same stream,
         rb_flow_reverse(flow_fw, t) -> flow and empty mask from t to left, rb_flow_reverse(flow_bw, 1 - t) -> from t to
-        right, and rb_frame_synthesize on the padded frames the pass used.  raft-small's flow is in 1/8-resolution units,
-        so its time steps are 8t and 8(1 - t) (exact: scaling by 8 commutes with fp32 rounding).  Frames as for
+        right, and rb_frame_synthesize on the padded frames the pass used.  raft-small's reference flow is in 1/8-resolution
+        units, so its time steps are 8t and 8(1 - t) (exact: scaling by 8 commutes with fp32 rounding); upstream, t.  Frames as for
         forward().  Returns a fresh [T,B,H,W,3] fp32 tensor, BGR in [0,1] (uint8 frames are divided by 255 first)."""
         ts = [float(t) for t in ts]
         if not ts or not all(0.0 <= t <= 1.0 for t in ts):
@@ -306,7 +322,7 @@ class RaftEngine:
         """The per-t work of interpolate on the flows of the last INTERPOLATE pass: two reversals and the blend into
         out [B,H,W,3]."""
         B, H, W = self._shape[:3]
-        s = 8.0 if self.small else 1.0
+        s = self.flow_scale
         lib, st, ptr = capi.lib, capi.stream(), capi.ptr
         for d, (flow, step) in enumerate(((self.flow_up[:B], s * t), (self.flow_up[B:], s * (1.0 - t)))):
             capi.check(lib.rb_flow_reverse(ptr(flow), None, None, 0, 0, step, ptr(self.flow_t[d]), ptr(self.empty_t[0, d]),
