@@ -37,17 +37,36 @@ enum {
 };
 
 /* Arithmetic back end for the GEMM-shaped ops (corr build, update-block convs).
- *   RB_MATH_TC    wgmma tensor cores, fp16 hi/lo split operands, 3 MMAs per product,
- *                 fp32 accumulation in registers (error ~2^-22 relative per product);
- *   RB_MATH_SIMT  the same split operands multiplied on the fp32 CUDA cores (bring-up /
- *                 cross-check path; identical buffers and epilogues). */
-enum { RB_MATH_TC = 0, RB_MATH_SIMT = 1 };
+ *   RB_MATH_TC       wgmma tensor cores, fp16 hi/lo split operands, 3 MMAs per product,
+ *                    fp32 accumulation in registers (error ~2^-22 relative per product);
+ *   RB_MATH_SIMT     the same split operands multiplied on the fp32 CUDA cores (bring-up /
+ *                    cross-check path; identical buffers and epilogues);
+ *   RB_MATH_TC_FP16  mixed precision at the boundary of upstream RAFT's --mixed_precision (torch autocast around fnet,
+ *                    cnet and the update block; fp32 correlation and coords1 += delta):
+ *                    - every conv (update block, convf1's window form, the hoisted `inp` convs, all encoder convs with
+ *                      the stem and the stride-2 views, rb_conv2d / rb_conv2d_strided) is ONE wgmma per product:
+ *                      fp16(a) * fp16(w), both the round-to-nearest hi plane (what autocast's cast gives), accumulated
+ *                      in fp32 registers; the lo planes are not read;
+ *                    - as in RB_MATH_TC: the correlation build (3 products), the lookups and the volume-free path, every
+ *                      epilogue and elementwise op in fp32 (GRU gates, instance-norm statistics and apply, residuals,
+ *                      coords1 += delta, mask softmax, upsampling), every buffer layout -- epilogues still write both
+ *                      planes, so a workspace stays valid when the mode changes between calls;
+ *                    - combines with either semantics, the volume-free lookup and rb_frames_resize;
+ *                    - deterministic like RB_MATH_TC: the same K order and split-K halves, so batched runs equal
+ *                      per-sample runs and every tile configuration gives the same bits;
+ *                    - not bit-identical to upstream under autocast, which keeps activations and elementwise ops in fp16
+ *                      (here fp32), rounds the batch-norm conv's weights before the norm (here batch norm is folded
+ *                      into the weights first) and sums in cuDNN's order.
+ *                    The flow misses the 1e-3 bar of RB_MATH_TC by design: about 1e-2 max-abs against fp64 at 64x96 and
+ *                    8 iterations, 1e-1 at 128x256 and 32 (DESIGN section 2).
+ * Like the semantics, the mode is per thread and read when a kernel is launched (it may be set inside graph capture). */
+enum { RB_MATH_TC = 0, RB_MATH_SIMT = 1, RB_MATH_TC_FP16 = 2 };
 
 #define RB_NUM_LEVELS 4
 
 int rb_version(void);
 const char* rb_last_error(void);
-/* Select the back end for subsequent calls on this thread (default RB_MATH_TC). */
+/* Select the back end for subsequent calls on this thread (default RB_MATH_TC); other values -> RB_ERR_BAD_ARG. */
 int rb_set_math_mode(int mode);
 int rb_get_math_mode(void);
 /* Numerics of the network for subsequent calls on this thread (default RB_SEMANTICS_REFERENCE); like the math mode it is
@@ -81,8 +100,9 @@ int rb_debug_set_buffer(void* buf);
 /* Test hook: every later tensor-core conv on this thread uses the given configuration; 0 = automatic.
  * block_n in {16,32,64,96,128} (not applied to convs whose automatic width is 16, i.e. the split-K flow-head conv),
  * bw_log2 in [3,7] (pixel box 2^bw_log2 x 2^(7-bw_log2)), max_ctas >= 1 caps the persistent grid (on top of any
- * internal cta_limit), stages in [2, ring maximum of that width] (5/5/4/3/3 for 16/32/64/96/128; with block_n = 0 the
- * request is clamped to the ring of the width each conv picks).  Anything else -> RB_ERR_BAD_ARG, before any CUDA call.
+ * internal cta_limit), stages in [2, ring maximum of that width] (5/5/4/3/3 for 16/32/64/96/128; 6 for every width of the
+ * single-pass kernel when the thread's math mode is RB_MATH_TC_FP16 at the time of this call; with block_n = 0 the request
+ * is clamped to the ring of the width each conv picks).  Anything else -> RB_ERR_BAD_ARG, before any CUDA call.
  * Workspace sizes that depend on the pixel box (rb_encoder_workspace_bytes) must be queried under the same override. */
 int rb_debug_conv_override(int block_n, int bw_log2, int max_ctas, int stages);
 /* Configuration of the last tensor-core conv launched on this thread (for tests to assert coverage): tile width, pixel
@@ -90,6 +110,9 @@ int rb_debug_conv_override(int block_n, int bw_log2, int max_ctas, int stages);
  * rb_debug_conv_override() call that produced fused instance-norm statistics in their epilogue (an encoder conv whose
  * statistics fall back to the stand-alone pass is not counted), or RB_ERR_BAD_ARG if no conv has been launched. */
 int rb_debug_conv_last(int* block_n, int* bw_log2, int* grid, int* stages, int* total_tiles);
+/* wgmma per product of that conv: 3 (split operands) or 1 (the single-pass kernel of RB_MATH_TC_FP16); RB_ERR_BAD_ARG if
+ * no conv has been launched on this thread. */
+int rb_debug_conv_last_passes(void);
 
 /* ---- A4: coords_grid(batch, ht, wd)  networks/utils.py:4-11 ----------------------------------
  * coords[b,y,x,0] = x, coords[b,y,x,1] = y. */

@@ -39,7 +39,7 @@ int device_sm_count(int dev) {
 extern "C" int rb_version(void) { return 100; }
 extern "C" const char* rb_last_error(void) { return rb::g_err; }
 extern "C" int rb_set_math_mode(int mode) {
-  if (mode != RB_MATH_TC && mode != RB_MATH_SIMT) {
+  if (mode != RB_MATH_TC && mode != RB_MATH_SIMT && mode != RB_MATH_TC_FP16) {
     rb::set_error("rb_set_math_mode: unknown mode %d", mode);
     return RB_ERR_BAD_ARG;
   }

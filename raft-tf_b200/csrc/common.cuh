@@ -14,6 +14,9 @@ namespace rb {
 void set_error(const char* fmt, ...);
 void count_launch();
 int math_mode();
+// the conv runs on the wgmma kernel: RB_MATH_TC or RB_MATH_TC_FP16 (the correlation build and the tensor-core forms of
+// convf1 / the motion encoder's flow slot / the fused instance-norm statistics follow this, not the single-pass flag)
+inline bool math_mode_tc() { const int m = math_mode(); return m == RB_MATH_TC || m == RB_MATH_TC_FP16; }
 int semantics();  // RB_SEMANTICS_* of the calling thread (rb_set_semantics), read when a kernel is launched
 
 // Pad before the first tap of a stride-s conv with an odd k x k kernel over an extent n; the output extent is ceil(n / s)
@@ -154,6 +157,9 @@ struct ConvParams {
   const __half* res_hi;
   const __half* res_lo;
   int res_stride;
+  // tensor-core back end: 1 = single pass, fp16(a) * fp16(b) from the hi planes only (RB_MATH_TC_FP16; set by launch_conv,
+  // never by the correlation build).  Read on the host only; last, so the kernels' view of the fields above is unchanged.
+  int single_pass;
 };
 __host__ __device__ inline int conv_sx(const ConvParams& p) { return p.sx > 0 ? p.sx : 1; }
 __host__ __device__ inline int conv_sy(const ConvParams& p) { return p.sy > 0 ? p.sy : 1; }
@@ -525,7 +531,14 @@ int launch_conv_tc(const ConvParams& p, cudaStream_t s);
 int conv_tc_tiles_per_image(int h, int w);
 bool conv_tc_fused_stats_ok(const ConvParams& p);
 inline int launch_conv(const ConvParams& p, cudaStream_t s) {
-  return math_mode() == RB_MATH_SIMT ? launch_conv_simt(p, s) : launch_conv_tc(p, s);
+  const int m = math_mode();
+  if (m == RB_MATH_SIMT) return launch_conv_simt(p, s);
+  if (m == RB_MATH_TC_FP16) {
+    ConvParams q = p;
+    q.single_pass = 1;
+    return launch_conv_tc(q, s);
+  }
+  return launch_conv_tc(p, s);
 }
 
 __device__ __forceinline__ long long gtime_ns() {

@@ -1,4 +1,5 @@
-// wgmma implicit-GEMM convolution / GEMM over split fp16 operands (the RB_MATH_TC back end).
+// wgmma implicit-GEMM convolution / GEMM over split fp16 operands (the RB_MATH_TC back end), and its single-pass variant
+// over the hi planes only (RB_MATH_TC_FP16).
 //
 // One CTA computes a 128-pixel x BLOCK_N-channel output tile.  The 128 pixels are a BH x BW box of
 // one image, so for every filter tap the A operand is ONE TMA box load from the NHWC activation
@@ -9,6 +10,8 @@
 //     HH += A_hi x B_hi^T,   X += A_hi x B_lo^T,   X += A_lo x B_hi^T
 // (m64nBLOCK_Nk16, fp32 accumulators in registers); the epilogue forms HH + 2^-11 * X in fp32 and applies the fused
 // epilogue of common.cuh.
+// SINGLE (RB_MATH_TC_FP16, ConvParams::single_pass): a stage holds A_hi and B_hi only, each k-slice issues HH += A_hi x B_hi^T
+// alone, and the epilogue consumes HH -- fp16(a) * fp16(b) with fp32 accumulation, in the same K order.
 // Warpgroup roles: 0 = TMA producer (one elected thread), 1 and 2 = consumers: wgmma on tile rows [0,64) / [64,128),
 // then the epilogue of those rows.  The accumulator fragments are staged through shared memory in slabs of 32 columns
 // so that every epilogue thread owns one pixel and 16 consecutive channels (the layout the epilogues and the fused
@@ -36,10 +39,12 @@ constexpr int kMaxSmem = 227 * 1024;       // opt-in shared memory per block on 
 // PERSISTENT kernel: each CTA walks tiles t = blockIdx.x, blockIdx.x + gridDim.x, ... (n-tile fastest, so CTAs that
 // run side by side share the same activation tile in L2).  The smem ring and its mbarrier phases simply continue across
 // tiles, so the producer streams the next tile's operands while the consumers run the epilogue of the current one.
-template <int BLOCK_N>
+template <int BLOCK_N, bool SINGLE = false>
 struct TcCfg {
   static constexpr int kBTileBytes = BLOCK_N * 128;
-  static constexpr int kStageBytes = 2 * kATileBytes + 2 * kBTileBytes;
+  static constexpr int kPlanes = SINGLE ? 1 : 2;          // hi (| lo) per operand
+  static constexpr int kBOff = kPlanes * kATileBytes;      // B_hi inside a stage: A_hi | A_lo | B_hi | B_lo, or A_hi | B_hi
+  static constexpr int kStageBytes = kPlanes * (kATileBytes + kBTileBytes);
   static constexpr int kRingBytes = kMaxSmem - 1024 /*align slack*/ - kStagingBytes - 256 /*barriers*/ - 1024 /*split-K partials*/;
   static constexpr int kStages = kRingBytes / kStageBytes > 6 ? 6 : kRingBytes / kStageBytes;
   static constexpr int kSmemBytes = kStages * kStageBytes + 1024 + kStagingBytes + 256 + 1024;
@@ -51,12 +56,13 @@ __device__ __forceinline__ void consumer_bar_sync(int id) { asm volatile("bar.sy
 
 // EXTRAS: phase timestamps (p.dbg) and fused instance-norm statistics (p.stat_part) -- a separate instantiation, so that
 // the kernel the update block runs carries none of their registers.
-template <int BLOCK_N, bool EXTRAS>
+// SINGLE: the single-pass variant (tmA_lo / tmB_lo are not read).
+template <int BLOCK_N, bool EXTRAS, bool SINGLE>
 __global__ void __launch_bounds__(kTcThreads, 1)
 conv_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant__ CUtensorMap tmA_lo,
                const __grid_constant__ CUtensorMap tmB_hi, const __grid_constant__ CUtensorMap tmB_lo,
                const ConvParams p, const TileGeom g, const int STAGES) {
-  using Cfg = TcCfg<BLOCK_N>;
+  using Cfg = TcCfg<BLOCK_N, SINGLE>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   float* staging = reinterpret_cast<float*>(smem + STAGES * Cfg::kStageBytes);
@@ -83,7 +89,11 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
   const int tiles_per_img = g.tiles_x * g.tiles_y;
 
   if (threadIdx.x == 0) {
-    prefetch_tmap(&tmA_hi); prefetch_tmap(&tmA_lo); prefetch_tmap(&tmB_hi); prefetch_tmap(&tmB_lo);
+    if constexpr (SINGLE) {
+      prefetch_tmap(&tmA_hi); prefetch_tmap(&tmB_hi);
+    } else {
+      prefetch_tmap(&tmA_hi); prefetch_tmap(&tmA_lo); prefetch_tmap(&tmB_hi); prefetch_tmap(&tmB_lo);
+    }
     for (int s = 0; s < STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 2); }  // one arrival per consumer warpgroup
     mbar_init(red_bar, 128);
     fence_barrier_init();
@@ -128,13 +138,13 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
           uint8_t* st = smem + slot * Cfg::kStageBytes;
           const int c0 = p.in_choff + k.ck * kChunkK;
           tma_load_4d(&tmA_hi, &full_bar[slot], st, c0, xs + k.kx, ys + k.ky, b);
-          tma_load_4d(&tmA_lo, &full_bar[slot], st + kATileBytes, c0, xs + k.kx, ys + k.ky, b);
+          if constexpr (!SINGLE) tma_load_4d(&tmA_lo, &full_bar[slot], st + kATileBytes, c0, xs + k.kx, ys + k.ky, b);
         };
         auto load_b = [&](const KIter& k, int slot) {
           uint8_t* st = smem + slot * Cfg::kStageBytes;
           const int kcol = (k.ky * p.kw + k.kx) * p.cin_pad + k.ck * kChunkK;
-          tma_load_3d(&tmB_hi, &full_bar[slot], st + 2 * kATileBytes, kcol, n0, wb);
-          tma_load_3d(&tmB_lo, &full_bar[slot], st + 2 * kATileBytes + Cfg::kBTileBytes, kcol, n0, wb);
+          tma_load_3d(&tmB_hi, &full_bar[slot], st + Cfg::kBOff, kcol, n0, wb);
+          if constexpr (!SINGLE) tma_load_3d(&tmB_lo, &full_bar[slot], st + Cfg::kBOff + Cfg::kBTileBytes, kcol, n0, wb);
         };
         KIter k = {krank * chunks, 0, 0, conv_chunk(p, krank * chunks)};
         int it0 = 0;
@@ -180,7 +190,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
     float* stg = staging + cw * 64 * kSlabPitch;
     asm volatile("griddepcontrol.wait;" ::: "memory");  // addend / z / h reads and all stores come after the predecessor
     constexpr int kNumAcc = BLOCK_N == 16 ? 2 : 1;  // the split-K halves of a 16-wide tile on one CTA
-    float hh[kNumAcc][Cfg::kAcc], xx[kNumAcc][Cfg::kAcc];
+    float hh[kNumAcc][Cfg::kAcc], xx[kNumAcc][SINGLE ? 1 : Cfg::kAcc];  // SINGLE: no cross-term accumulators
     int s = 0, pend = -1, li = 0;
     uint32_t phase = 0;
     // k-iterations [it0, it1) into (H, X); the wgmma group of a stage stays in flight while the next stage is issued, the
@@ -192,15 +202,17 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
         const uint32_t st = smem_u32(smem + s * Cfg::kStageBytes);
         const uint64_t a_hi = wgmma_desc_sw128(st + cw * 64 * 128);
         const uint64_t a_lo = wgmma_desc_sw128(st + kATileBytes + cw * 64 * 128);
-        const uint64_t b_hi = wgmma_desc_sw128(st + 2 * kATileBytes);
-        const uint64_t b_lo = wgmma_desc_sw128(st + 2 * kATileBytes + Cfg::kBTileBytes);
+        const uint64_t b_hi = wgmma_desc_sw128(st + Cfg::kBOff);
+        const uint64_t b_lo = wgmma_desc_sw128(st + Cfg::kBOff + Cfg::kBTileBytes);
         wgmma_fence();
 #pragma unroll
         for (int k = 0; k < kChunkK / 16; ++k) {
           const uint64_t koff = (uint64_t)(k * 2);  // 32 bytes per k-slice, in 16-byte units
           wgmma_f16<BLOCK_N>(H, a_hi + koff, b_hi + koff);
-          wgmma_f16<BLOCK_N>(X, a_hi + koff, b_lo + koff);
-          wgmma_f16<BLOCK_N>(X, a_lo + koff, b_hi + koff);
+          if constexpr (!SINGLE) {
+            wgmma_f16<BLOCK_N>(X, a_hi + koff, b_lo + koff);
+            wgmma_f16<BLOCK_N>(X, a_lo + koff, b_hi + koff);
+          }
         }
         wgmma_commit();
         wgmma_wait<1>();
@@ -221,8 +233,9 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
       for (int a = 0; a < kNumAcc; ++a)
 #pragma unroll
         for (int i = 0; i < Cfg::kAcc; ++i) {
-          hh[a][i] = 0.f; xx[a][i] = 0.f;
-          fence_operand(hh[a][i]); fence_operand(xx[a][i]);  // zeroed before the first wgmma, not between stages
+          hh[a][i] = 0.f;
+          fence_operand(hh[a][i]);  // zeroed before the first wgmma, not between stages
+          if constexpr (!SINGLE) { xx[a][i] = 0.f; fence_operand(xx[a][i]); }
         }
       const int it_half = (halves && !splitk) ? kiters / 2 : kiters;  // first k-iteration of the second accumulator
       mma_range(hh[0], xx[0], 0, it_half);
@@ -231,7 +244,10 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
 #pragma unroll
       for (int a = 0; a < kNumAcc; ++a)
 #pragma unroll
-        for (int i = 0; i < Cfg::kAcc; ++i) { fence_operand(hh[a][i]); fence_operand(xx[a][i]); }
+        for (int i = 0; i < Cfg::kAcc; ++i) {
+          fence_operand(hh[a][i]);
+          if constexpr (!SINGLE) fence_operand(xx[a][i]);
+        }
       if (t == 0) mbar_arrive(&empty_bar[pend]);
       pend = -1;
       if (li == 0) {
@@ -241,9 +257,15 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
       if (dbg && li == 0 && t == 0 && cw == 0) dbg[5] = gtime_ns();  // epilogue of the first tile begins
 #pragma unroll
       for (int i = 0; i < Cfg::kAcc; ++i) {
-        hh[0][i] = hh[0][i] + xx[0][i] * kLoInv;
-        if constexpr (BLOCK_N == 16) {
-          if (halves && !splitk) hh[0][i] += hh[1][i] + xx[1][i] * kLoInv;  // second accumulator of the same CTA
+        if constexpr (SINGLE) {
+          if constexpr (BLOCK_N == 16) {
+            if (halves && !splitk) hh[0][i] += hh[1][i];  // second accumulator of the same CTA
+          }
+        } else {
+          hh[0][i] = hh[0][i] + xx[0][i] * kLoInv;
+          if constexpr (BLOCK_N == 16) {
+            if (halves && !splitk) hh[0][i] += hh[1][i] + xx[1][i] * kLoInv;  // second accumulator of the same CTA
+          }
         }
       }
 #pragma unroll
@@ -407,9 +429,10 @@ struct ConvRecord {
   int block_n, bw_log2, grid, stages, total_tiles;
   int launched;     // a tensor-core conv has been launched on this thread
   int fused_stats;  // convs since the last rb_debug_conv_override() call that wrote fused instance-norm statistics
+  int passes;       // wgmma per product: 3 (split operands) or 1 (single pass)
 };
 static thread_local ConvOverride g_override = {0, 0, 0, 0};
-static thread_local ConvRecord g_record = {0, 0, 0, 0, 0, 0, 0};
+static thread_local ConvRecord g_record = {0, 0, 0, 0, 0, 0, 0, 0};
 
 // Ring depth of a launch: the test hook may lower it, but never below 2 -- a consumer hands a stage back only after it has
 // issued the next one (wgmma_wait<1>), so a one-stage ring deadlocks any conv with two k-iterations.
@@ -449,7 +472,7 @@ int conv_tc_tiles_per_image(int h, int w) {
 // The conv can produce the statistics itself: tensor-core back end, 16-channel epilogue (see epilogue_wide_ok()).
 bool conv_tc_fused_stats_ok(const ConvParams& p) {
   auto al = [](const void* q) { return (reinterpret_cast<uintptr_t>(q) & 31) == 0; };
-  return math_mode() == RB_MATH_TC && p.epi == EPI_F32 && (p.cout & 15) == 0 && al(p.bias) && al(p.addend) && al(p.f0) &&
+  return math_mode_tc() && p.epi == EPI_F32 && (p.cout & 15) == 0 && al(p.bias) && al(p.addend) && al(p.f0) &&
          p.cin_pad % kChunkK == 0;
 }
 
@@ -477,15 +500,15 @@ static int choose_block_n(int cout, long m_tiles, int ctas) {  // ctas: persiste
   return best;
 }
 
-template <int BLOCK_N>
+template <int BLOCK_N, bool SINGLE>
 static int launch_cfg(const ConvParams& p_in, TileGeom g, const CUtensorMap* maps, cudaStream_t s) {
-  using Cfg = TcCfg<BLOCK_N>;
+  using Cfg = TcCfg<BLOCK_N, SINGLE>;
   static PerDeviceOnce attr_set;
   int dev = 0, rc_dev;
   if ((rc_dev = current_device(&dev))) return rc_dev;
   if (!attr_set.test(dev)) {
-    RB_CHECK_CUDA(cudaFuncSetAttribute(conv_tc_kernel<BLOCK_N, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
-    RB_CHECK_CUDA(cudaFuncSetAttribute(conv_tc_kernel<BLOCK_N, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
+    RB_CHECK_CUDA(cudaFuncSetAttribute(conv_tc_kernel<BLOCK_N, false, SINGLE>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
+    RB_CHECK_CUDA(cudaFuncSetAttribute(conv_tc_kernel<BLOCK_N, true, SINGLE>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
     attr_set.set(dev);
   }
   const int num_sms = device_sm_count(dev);
@@ -524,12 +547,12 @@ static int launch_cfg(const ConvParams& p_in, TileGeom g, const CUtensorMap* map
   cfg.numAttrs = 1 + pdl;
   const int stages = ring_stages(Cfg::kStages);
   if (p.dbg || p.stat_part)
-    RB_CHECK_CUDA(cudaLaunchKernelEx(&cfg, conv_tc_kernel<BLOCK_N, true>, maps[0], maps[1], maps[2], maps[3], p, g, stages));
+    RB_CHECK_CUDA(cudaLaunchKernelEx(&cfg, conv_tc_kernel<BLOCK_N, true, SINGLE>, maps[0], maps[1], maps[2], maps[3], p, g, stages));
   else
-    RB_CHECK_CUDA(cudaLaunchKernelEx(&cfg, conv_tc_kernel<BLOCK_N, false>, maps[0], maps[1], maps[2], maps[3], p, g, stages));
+    RB_CHECK_CUDA(cudaLaunchKernelEx(&cfg, conv_tc_kernel<BLOCK_N, false, SINGLE>, maps[0], maps[1], maps[2], maps[3], p, g, stages));
   RB_CHECK_LAUNCH("conv_tc_kernel");
   g_record.block_n = BLOCK_N; g_record.bw_log2 = g.bw_log2; g_record.grid = (int)cfg.gridDim.x; g_record.stages = stages;
-  g_record.total_tiles = g.total_tiles; g_record.launched = 1;
+  g_record.total_tiles = g.total_tiles; g_record.launched = 1; g_record.passes = SINGLE ? 1 : 3;
   if (p.stat_part) ++g_record.fused_stats;
   return RB_OK;
 }
@@ -544,6 +567,7 @@ int launch_conv_tc(const ConvParams& p, cudaStream_t s) {
   const int num_sms = device_sm_count(dev);
   int bn = choose_block_n(p.cout, m_tiles, p.cta_limit > 0 && p.cta_limit < num_sms ? p.cta_limit : num_sms);
   if (g_override.block_n > 0 && bn != 16) bn = g_override.block_n;  // the 16-wide (split-K) convs keep theirs
+  const bool single = p.single_pass != 0;
   CUtensorMap maps[4];
   {
     // the input view (common.cuh): strided convs traverse it with TMA element strides -- a box of bw*sx x bh*sy input
@@ -558,7 +582,8 @@ int launch_conv_tc(const ConvParams& p, cudaStream_t s) {
     uint32_t es[4] = {1, (uint32_t)sx, (uint32_t)sy, 1};
     int rc;
     if ((rc = cached_tmap(&maps[0], p.in_hi, 4, dims, str, box, tc::TMAP_F16_SW128, es))) return rc;
-    if ((rc = cached_tmap(&maps[1], p.in_lo, 4, dims, str, box, tc::TMAP_F16_SW128, es))) return rc;
+    if (single) maps[1] = maps[0];  // not read by the single-pass kernel
+    else if ((rc = cached_tmap(&maps[1], p.in_lo, 4, dims, str, box, tc::TMAP_F16_SW128, es))) return rc;
   }
   {
     const uint64_t ktot = (uint64_t)p.kh * p.kw * p.cin_pad;
@@ -567,31 +592,50 @@ int launch_conv_tc(const ConvParams& p, cudaStream_t s) {
     uint32_t box[3] = {(uint32_t)kChunkK, (uint32_t)bn, 1};
     int rc;
     if ((rc = cached_tmap(&maps[2], p.w_hi, 3, dims, str, box))) return rc;
-    if ((rc = cached_tmap(&maps[3], p.w_lo, 3, dims, str, box))) return rc;
+    if (single) maps[3] = maps[2];
+    else if ((rc = cached_tmap(&maps[3], p.w_lo, 3, dims, str, box))) return rc;
+  }
+  if (single) {
+    switch (bn) {
+      case 16: return launch_cfg<16, true>(p, g, maps, s);
+      case 32: return launch_cfg<32, true>(p, g, maps, s);
+      case 64: return launch_cfg<64, true>(p, g, maps, s);
+      case 96: return launch_cfg<96, true>(p, g, maps, s);
+      default: return launch_cfg<128, true>(p, g, maps, s);
+    }
   }
   switch (bn) {
-    case 16: return launch_cfg<16>(p, g, maps, s);
-    case 32: return launch_cfg<32>(p, g, maps, s);
-    case 64: return launch_cfg<64>(p, g, maps, s);
-    case 96: return launch_cfg<96>(p, g, maps, s);
-    default: return launch_cfg<128>(p, g, maps, s);
+    case 16: return launch_cfg<16, false>(p, g, maps, s);
+    case 32: return launch_cfg<32, false>(p, g, maps, s);
+    case 64: return launch_cfg<64, false>(p, g, maps, s);
+    case 96: return launch_cfg<96, false>(p, g, maps, s);
+    default: return launch_cfg<128, false>(p, g, maps, s);
   }
 }
 
 }  // namespace rb
 
+namespace rb {
+// ring depth of the forced width, or the deepest ring of any width (0: block_n is not a width)
+template <bool SINGLE>
+static int ring_max_of(int block_n) {
+  switch (block_n) {
+    case 0: return TcCfg<16, SINGLE>::kStages > TcCfg<32, SINGLE>::kStages ? TcCfg<16, SINGLE>::kStages : TcCfg<32, SINGLE>::kStages;
+    case 16: return TcCfg<16, SINGLE>::kStages;
+    case 32: return TcCfg<32, SINGLE>::kStages;
+    case 64: return TcCfg<64, SINGLE>::kStages;
+    case 96: return TcCfg<96, SINGLE>::kStages;
+    case 128: return TcCfg<128, SINGLE>::kStages;
+    default: return 0;
+  }
+}
+}  // namespace rb
+
 extern "C" int rb_debug_conv_override(int block_n, int bw_log2, int max_ctas, int stages) {
   using namespace rb;
-  int ring_max = 0;  // ring depth of the forced width, or the deepest ring of any width
-  switch (block_n) {
-    case 0: ring_max = TcCfg<16>::kStages > TcCfg<32>::kStages ? TcCfg<16>::kStages : TcCfg<32>::kStages; break;
-    case 16: ring_max = TcCfg<16>::kStages; break;
-    case 32: ring_max = TcCfg<32>::kStages; break;
-    case 64: ring_max = TcCfg<64>::kStages; break;
-    case 96: ring_max = TcCfg<96>::kStages; break;
-    case 128: ring_max = TcCfg<128>::kStages; break;
-    default: RB_REQUIRE(false, RB_ERR_BAD_ARG, "rb_debug_conv_override: block_n %d not in {0,16,32,64,96,128}", block_n);
-  }
+  // the ring of the kernel the thread's math mode launches
+  const int ring_max = math_mode() == RB_MATH_TC_FP16 ? ring_max_of<true>(block_n) : ring_max_of<false>(block_n);
+  RB_REQUIRE(ring_max > 0, RB_ERR_BAD_ARG, "rb_debug_conv_override: block_n %d not in {0,16,32,64,96,128}", block_n);
   RB_REQUIRE(bw_log2 == 0 || (bw_log2 >= 3 && bw_log2 <= 7), RB_ERR_BAD_ARG, "rb_debug_conv_override: bw_log2 %d not 0 or in [3,7]",
              bw_log2);
   RB_REQUIRE(max_ctas >= 0, RB_ERR_BAD_ARG, "rb_debug_conv_override: max_ctas %d < 0", max_ctas);
@@ -611,4 +655,11 @@ extern "C" int rb_debug_conv_last(int* block_n, int* bw_log2, int* grid, int* st
   if (stages) *stages = g_record.stages;
   if (total_tiles) *total_tiles = g_record.total_tiles;
   return g_record.fused_stats;
+}
+
+extern "C" int rb_debug_conv_last_passes(void) {
+  using namespace rb;
+  RB_REQUIRE(g_record.launched, RB_ERR_BAD_ARG,
+             "rb_debug_conv_last_passes: no tensor-core conv has been launched on this thread");
+  return g_record.passes;
 }

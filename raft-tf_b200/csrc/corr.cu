@@ -859,7 +859,8 @@ extern "C" int rb_corr_build(const float* fmap1, const float* fmap2, float* pyra
   RB_REQUIRE(B > 0 && (h >> 3) >= 1 && (w >> 3) >= 1, RB_ERR_BAD_SHAPE, "rb_corr_build: grid %dx%d too small", h, w);
   RB_REQUIRE(C > 0 && C % 16 == 0, RB_ERR_BAD_SHAPE, "rb_corr_build: C=%d must be a multiple of 16", C);
   cudaStream_t s = (cudaStream_t)stream;
-  if (math_mode() == RB_MATH_TC) return corr_build_tc(fmap1, fmap2, pyramid, B, h, w, C, workspace, workspace_bytes, s);
+  // RB_MATH_TC_FP16 too: the correlation keeps its three products (launch_conv_tc with single_pass = 0)
+  if (math_mode_tc()) return corr_build_tc(fmap1, fmap2, pyramid, B, h, w, C, workspace, workspace_bytes, s);
   const int N = h * w;
   dim3 grid((N + 63) / 64, (N + 63) / 64, B);
   corr_gemm_simt_kernel<<<grid, 256, 0, s>>>(fmap1, fmap2, pyramid, N, C, 0.f);

@@ -420,7 +420,7 @@ static int update_step(const Variant& v, const void* blob, void* wsp, float* coo
     flow_conv7_kernel<COUT, SEG><<<dim3((w + SEG - 1) / SEG, h, B), COUT, 0, ss->stream>>>(c1, Wf, bf, W.f1, v.f1, W.hx, W.qx, v.hx, foff, h, w)
     // default: convf1 on the tensor cores (flow_prep_kernel + 7x1 conv over the window view); the CUDA-core math mode and
     // the shapes the window view cannot take keep the CUDA-core kernel
-    const bool f1_tc = math_mode() == RB_MATH_TC && (foff & 1) == 0 && (v.hx & 1) == 0 && w >= 8;
+    const bool f1_tc = math_mode_tc() && (foff & 1) == 0 && (v.hx & 1) == 0 && w >= 8;
     if (f1_tc) {
       const size_t cells = (size_t)B * h * (w + 8);
       flow_prep_kernel<<<(unsigned)((cells + 255) / 256), 256, 0, ss->stream>>>(c1, W.fl, W.hx, W.qx, v.hx, foff, B, h, w);
@@ -481,7 +481,7 @@ static int update_step(const Variant& v, const void* blob, void* wsp, float* coo
     ConvParams p = base_params(v, L, blob, P_MOTION, W.cf, v.cf, 0, B, h, w);
     set_act(p, ACT_RELU, W.hx, v.hx, xoff);
     p.d1_hi = W.qx.hi; p.d1_lo = W.qx.lo; p.d1_stride = v.hx; p.d1_choff = xoff;
-    if (math_mode() == RB_MATH_TC && (p.cout & 15) == 14 && p.cout + 2 <= p.cout_pad && foff == xoff + p.cout) {
+    if (math_mode_tc() && (p.cout & 15) == 14 && p.cout + 2 <= p.cout_pad && foff == xoff + p.cout) {
       // things: 126 channels + the 2 flow channels right behind them = one full 16-channel group -> the tensor-core
       // epilogue writes the flow slot too and takes its 256-bit path (the weight rows / biases 126,127 are zero)
       p.cout += 2;

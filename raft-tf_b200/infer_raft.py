@@ -13,7 +13,8 @@ Extensions: --iters, --keep-size (replicate-pad to a multiple of 8 instead of re
 forward-backward occlusion masks ``raft_occ_fw.png`` / ``raft_occ_bw.png`` (0 consistent, 128 occluded, 255 leaves the
 frame), from one pass that encodes each frame once, and --interpolate T [T ...]: the frames at times T in [0, 1] between
 im1 (0) and im2 (1), written as ``raft_interp_<k>.png`` (k = position in the list), and --native-flow: the written
-flow(s) resized back to im1's size with the reference's flow_utils.resize_flow (no effect with --keep-size).
+flow(s) resized back to im1's size with the reference's flow_utils.resize_flow (no effect with --keep-size), and
+--mixed_precision (upstream RAFT's spelling): every conv with fp16 operands and fp32 accumulation, the correlation in fp32.
 """
 import argparse
 import os
@@ -50,7 +51,7 @@ def decode_pair(im1, im2, rgb=False):
     return tuple(_decode(path, rgb)[None] for path in (im1, im2))
 
 
-def main(argv=None):
+def parser():
     p = argparse.ArgumentParser()
     p.add_argument('--gpu', default='1', help='comma separated list of GPU(s) to use (ignored, as in the reference)')
     p.add_argument('--data', default='', help='unused (reference flag)')
@@ -75,6 +76,14 @@ def main(argv=None):
     p.add_argument('--upstream', action='store_true',
                    help='extension: weights converted from an official princeton-vl RAFT .pth (raft_b200.convert): RGB '
                         'frames and the upstream numerics (RAFT(..., upstream=True))')
+    p.add_argument('--mixed_precision', action='store_true',
+                   help="extension: upstream RAFT's mixed precision -- fp16 conv operands, fp32 accumulation and "
+                        "correlation (RAFT(..., mixed_precision=True)); the flow differs from the default by ~1e-2 px")
+    return p
+
+
+def main(argv=None):
+    p = parser()
     args = p.parse_args(argv)
     if args.interpolate and not all(0.0 <= t <= 1.0 for t in args.interpolate):
         p.error('--interpolate: every T must be in [0, 1]')
@@ -87,14 +96,15 @@ def main(argv=None):
     rgb = args.upstream  # the official checkpoints expect RGB frames; the reference's expect BGR
     if args.keep_size:
         left, right = read_pair(args.im1, args.im2, None, rgb)
-        model = RAFT.RAFT(left.shape[1:], args, iters=args.iters, upstream=args.upstream).load(args.load)
+        model = RAFT.RAFT(left.shape[1:], args, iters=args.iters, upstream=args.upstream,
+                          mixed_precision=args.mixed_precision).load(args.load)
     else:  # the reference's 432x1024 (infer_raft.py:69,76), resized and scaled on the GPU
         left, right = decode_pair(args.im1, args.im2, rgb)
         native = left.shape[1:3]
         if left.shape != right.shape:  # one engine pass takes one frame size: resize such a pair on the host, as before
             left, right = read_pair(args.im1, args.im2, (432, 1024), rgb)
         model = RAFT.RAFT((432, 1024, 3), args, iters=args.iters, input_size=(432, 1024),
-                          upstream=args.upstream).load(args.load)
+                          upstream=args.upstream, mixed_precision=args.mixed_precision).load(args.load)
     if args.bidirectional:
         flow, flow_bw, occ_fw, occ_bw = (t.cpu().numpy() for t in model.forward_bidirectional(left, right))
     else:

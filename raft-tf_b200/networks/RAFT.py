@@ -6,7 +6,8 @@ contract (returns 0.0 and publishes the result under the name ``flow_result``, R
 5): ``iters``, ``batch`` and the image shape are honoured as parameters; inputs whose H/W are not
 multiples of 8 are replicate-padded and the flow cropped back (the reference itself cannot run such
 shapes, SURVEY fact 6).  ``input_size=(Ho, Wo)`` gives the reference's input semantics instead: frames of any
-size are resized to Ho x Wo on the GPU, bit for bit like the cv2.resize of its test dataflow."""
+size are resized to Ho x Wo on the GPU, bit for bit like the cv2.resize of its test dataflow.  ``mixed_precision=True``
+runs every conv with fp16 operands and fp32 accumulation, like upstream RAFT's --mixed_precision (RB_MATH_TC_FP16)."""
 import numpy as np
 import torch
 
@@ -22,7 +23,8 @@ class RAFT(object):
     weight_decay = 1e-5          # vestigial in the reference too (RAFT.py:14)
     data_format = 'NHWC'
 
-    def __init__(self, image_shape, args, iters=20, batch=1, device=None, volume_free=None, input_size=None, upstream=False):
+    def __init__(self, image_shape, args, iters=20, batch=1, device=None, volume_free=None, input_size=None, upstream=False,
+                 mixed_precision=False):
         self.dropout = 0.0
         self.corr_radius = 4
         self.hidden_dim = 128
@@ -42,6 +44,8 @@ class RAFT(object):
         self.input_size = None if input_size is None else (int(input_size[0]), int(input_size[1]))
         # extension: the numerics of princeton-vl RAFT for weights converted from its .pth checkpoints (RaftEngine upstream)
         self.upstream = bool(upstream)
+        # extension: fp16 conv operands with fp32 accumulation, upstream's --mixed_precision (RaftEngine mixed_precision)
+        self.mixed_precision = bool(mixed_precision)
         self.flow_result = None
         self._engine = None
         self._params = None
@@ -85,7 +89,8 @@ class RAFT(object):
             if self._params is None:
                 raise RuntimeError("RAFT.load(<npz>) must be called before inference")
             self._engine = RaftEngine(self._params, small=self.small, iters=self.iters, device=self.device,
-                                      volume_free=self.volume_free, input_size=self.input_size, upstream=self.upstream)
+                                      volume_free=self.volume_free, input_size=self.input_size, upstream=self.upstream,
+                                      mixed_precision=self.mixed_precision)
         return self._engine
 
     # -- inference ---------------------------------------------------------------------------------

@@ -8,7 +8,7 @@ import os
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("RAFT_B200_LIB") or os.path.join(_HERE, "..", "lib", "libraft_b200.so")  # env override: A/B of builds
 
-RB_MATH_TC, RB_MATH_SIMT = 0, 1
+RB_MATH_TC, RB_MATH_SIMT, RB_MATH_TC_FP16 = 0, 1, 2
 RB_SEMANTICS_REFERENCE, RB_SEMANTICS_UPSTREAM = 0, 1
 
 if not os.path.exists(LIB_PATH):
@@ -33,6 +33,7 @@ SIGNATURES = {
     "rb_debug_set_buffer": (_i, [_vp]),
     "rb_debug_conv_override": (_i, [_i, _i, _i, _i]),
     "rb_debug_conv_last": (_i, [_pi, _pi, _pi, _pi, _pi]),
+    "rb_debug_conv_last_passes": (_i, []),
     "rb_coords_grid": (_i, [_vp, _i, _i, _i, _vp]),
     "rb_corr_pyramid_bytes": (_i, [_i, _i, _i, _psz]),
     "rb_corr_level_offset": (_i, [_i, _i, _i, _i, _psz, _pi, _pi]),

@@ -43,7 +43,15 @@ class RaftEngine:
     def __init__(self, params: Dict[str, np.ndarray], small: bool = False, iters: int = 20,
                  device: Optional[torch.device] = None, use_graph: bool = True, math_mode: int = capi.RB_MATH_TC,
                  volume_free: Optional[bool] = None, input_size: Optional[Tuple[int, int]] = None,
-                 upstream: bool = False):
+                 upstream: bool = False, mixed_precision: bool = False):
+        # mixed_precision: upstream RAFT's --mixed_precision boundary -- every conv as one fp16 x fp16 wgmma per product with
+        # fp32 accumulation, the correlation and all elementwise work as in RB_MATH_TC (RB_MATH_TC_FP16, include/raft_b200.h)
+        if mixed_precision:
+            if math_mode == capi.RB_MATH_SIMT:
+                raise ValueError("raft_b200: mixed_precision runs the convs on the tensor cores; it cannot be combined with "
+                                 "math_mode=RB_MATH_SIMT")
+            math_mode = capi.RB_MATH_TC_FP16
+        self.mixed_precision = math_mode == capi.RB_MATH_TC_FP16
         # upstream: the numerics of princeton-vl RAFT (PyTorch), for checkpoints converted from its .pth files
         # (raft_b200.convert): grid_sample lookup, PyTorch's stride-2 padding, raft-small's flow scaled by 8
         # (RB_SEMANTICS_UPSTREAM, include/raft_b200.h)
