@@ -277,6 +277,24 @@ int rb_frame_synthesize(const float* frames, int Hp, int Wp, int top, int left, 
                         const float* flow_t1, const uint8_t* empty0, const uint8_t* empty1, float t, float* out,
                         int B, int H, int W, void* stream);
 
+/* ---- F9: end-point-error metrics (upstream RAFT's evaluate.py validate_sintel / validate_kitti) ---------------------
+ * flow, gt: [B,H,W,2] fp32; valid: [B,H,W] uint8, nonzero = the pixel counts (NULL: every pixel counts).  Per pixel,
+ * every operation rounded on its own (no FMA contraction), so the values equal upstream's torch expressions bit for bit:
+ *   d = flow_scale * flow - gt,  e = sqrt(d.x*d.x + d.y*d.y),  m = sqrt(gt.x*gt.x + gt.y*gt.y),
+ *   outlier = e > 3.0f && e / m > 0.05f  (KITTI's F1 rule; IEEE semantics for m = 0).
+ * flow_scale as in rb_flow_fb_check: 8.0 for raft-small's reference-semantics flow (1/8-resolution units; x8 is exact),
+ * 1.0 otherwise.  epe (nullable): [B,H,W] fp32, written for every pixel, counted or not.  stats: [B][RB_FLOW_STATS] fp64,
+ * over the counted pixels of sample b: {n, sum e, #(e < 1), #(e < 3), #(e < 5), #outliers}; the counts are exact and a NaN
+ * flow propagates into the sum.  The reduction is deterministic and independent of B: each sample's pixels are split
+ * into fixed chunks, each reduced by one block in a fixed tree into the workspace (rb_flow_metrics_workspace_bytes), and a
+ * second launch adds each sample's partials in a fixed order -- a batch gives the per-sample bits, no allocation, no
+ * float atomics, graph-capturable.  Null pointers, B/H/W <= 0, flow_scale <= 0 or non-finite, B > 65535 and a workspace
+ * that is too small -> RB_ERR_* before any CUDA call. */
+#define RB_FLOW_STATS 6
+int rb_flow_metrics_workspace_bytes(int B, int H, int W, size_t* bytes);
+int rb_flow_metrics(const float* flow, float flow_scale, const float* gt, const uint8_t* valid, int B, int H, int W,
+                    float* epe, double* stats, void* workspace, size_t workspace_bytes, void* stream);
+
 /* ---- F3 (input edge): dataflow/test_dataflow.py:56-61,96-97 + the SURVEY 8(d) shape policy ------------------
  * src: [B,H,W,3] device frames, BGR like cv2.imdecode -- fp32 in [0,1] (src_is_u8 = 0) or uint8 in [0,255]
  * (src_is_u8 = 1: x/255.0f, the reference's np.float32(x)/255.0, bit for bit).  dst: [B,H+pt+pb,W+pl+pr,3] fp32

@@ -112,6 +112,20 @@ def write_flo(path, flow_uv):
         f.tofile(fh)
 
 
+def read_kitti_flow(path):
+    """KITTI's 16-bit flow PNG -> (flow [H,W,2] float32, valid [H,W] uint8), like upstream RAFT's readFlowKITTI and the
+    mask of validate_kitti: in OpenCV's BGR order channel 2 is u, channel 1 is v and channel 0 the valid flag; flow =
+    (x - 2**15) / 64 (exact in float32), valid = flag >= 0.5."""
+    import cv2
+    raw = cv2.imread(str(path), cv2.IMREAD_ANYDEPTH | cv2.IMREAD_COLOR)
+    if raw is None:
+        raise FileNotFoundError(f"cannot read KITTI flow {path}")
+    if raw.dtype != np.uint16 or raw.ndim != 3 or raw.shape[2] != 3:
+        raise ValueError(f"{path}: a KITTI flow is a 3-channel 16-bit PNG, got {raw.dtype} {raw.shape}")
+    flow = (raw[..., 2:0:-1].astype(np.float32) - np.float32(2 ** 15)) / np.float32(64.0)
+    return np.ascontiguousarray(flow), (raw[..., 0] >= 0.5).astype(np.uint8)
+
+
 def read_flo(path):
     with open(path, "rb") as fh:
         magic = np.fromfile(fh, np.float32, 1)[0]

@@ -7,7 +7,7 @@ raft_b200 CUDA engine -- no TensorFlow, no tensorpack.
 Like the reference it decodes BGR with OpenCV, resizes both frames to 432x1024 (bilinear cv2.resize,
 dataflow/test_dataflow.py:85-87; here on the GPU from the uint8 frames, bit for bit), scales to [0,1], runs 20 iterations and writes the colour-coded flow
 to ``raft_flow_raft-things.png`` in the working directory (regardless of --small, infer_raft.py:44).
-Flags the reference parses but ignores (--gpu, --data, --out, -o) are accepted; ``--batch`` stays 1.
+Flags the reference parses but ignores (--gpu, -o) are accepted; --data, --out and --batch are read by -m val only.
 Extensions: --iters, --keep-size (replicate-pad to a multiple of 8 instead of resizing), --npy, --flo, and
 --bidirectional: also the flow im2 -> im1 (``raft_flow_raft-things_bw.png``, ``<npy>_bw.npy``, ``<flo>_bw.flo``) and the
 forward-backward occlusion masks ``raft_occ_fw.png`` / ``raft_occ_bw.png`` (0 consistent, 128 occluded, 255 leaves the
@@ -15,6 +15,13 @@ frame), from one pass that encodes each frame once, and --interpolate T [T ...]:
 im1 (0) and im2 (1), written as ``raft_interp_<k>.png`` (k = position in the list), and --native-flow: the written
 flow(s) resized back to im1's size with the reference's flow_utils.resize_flow (no effect with --keep-size), and
 --mixed_precision (upstream RAFT's spelling): every conv with fp16 operands and fp32 accumulation, the correlation in fp32.
+
+-m val (declared by the reference, implemented here): upstream RAFT's validation on a Sintel or KITTI-2015 training tree,
+
+    python infer_raft.py -m val --dataset sintel --data datasets/Sintel --load raft-things.npz --upstream [--batch 8]
+
+prints upstream's lines (``Validation (clean) EPE: ...``, ``Validation KITTI: <epe>, <f1>``) and writes the aggregates and
+per-pair records to ``<--out>/val_<dataset>.json`` (raft_b200.evaluate).
 """
 import argparse
 import os
@@ -54,16 +61,21 @@ def decode_pair(im1, im2, rgb=False):
 def parser():
     p = argparse.ArgumentParser()
     p.add_argument('--gpu', default='1', help='comma separated list of GPU(s) to use (ignored, as in the reference)')
-    p.add_argument('--data', default='', help='unused (reference flag)')
+    p.add_argument('--data', default='', help='-m val: dataset root (reference flag)')
     p.add_argument('--load', default='release_weight/raft-things.npz', help='npz checkpoint keyed by TF variable names')
     p.add_argument('-m', '--mode', default='test', choices=['train', 'val', 'test', 'export', 'flops'])
-    p.add_argument('--out', default='./log')
-    p.add_argument('--batch', default=1, type=int)
+    p.add_argument('--out', default='./log', help='-m val: where val_<dataset>.json is written')
+    p.add_argument('--batch', default=1, type=int, help='-m val: frame pairs per engine pass (test mode runs one pair)')
     p.add_argument('-o', '--optimizer', default='adam', choices=['adam', 'adamw', 'sgd', 'sgd_cyclic', 'sgd_1cycle'])
     p.add_argument('--im1', default='frame_0010.png')
     p.add_argument('--im2', default='frame_0011.png')
     p.add_argument('--small', action='store_true')
-    p.add_argument('--iters', type=int, default=20, help='extension: GRU iterations (reference: 20)')
+    p.add_argument('--iters', type=int, default=None,
+                   help='extension: GRU iterations (test mode: 20 like the reference; -m val: the protocol\'s 32 / 24)')
+    p.add_argument('--dataset', default=None, choices=['sintel', 'kitti'], help='-m val: which training set --data holds')
+    p.add_argument('--dstype', nargs='+', default=['clean', 'final'], choices=['clean', 'final'],
+                   help='-m val, Sintel: the passes to evaluate')
+    p.add_argument('--workers', type=int, default=4, help='-m val: frame-decoding threads')
     p.add_argument('--keep-size', action='store_true', help='extension: pad to a multiple of 8 instead of resizing to 432x1024')
     p.add_argument('--npy', default=None, help='extension: also save the raw [H,W,2] flow')
     p.add_argument('--flo', default=None, help='extension: also save the flow as a Middlebury .flo file')
@@ -87,6 +99,10 @@ def main(argv=None):
     args = p.parse_args(argv)
     if args.interpolate and not all(0.0 <= t <= 1.0 for t in args.interpolate):
         p.error('--interpolate: every T must be in [0, 1]')
+    if args.mode == 'val':
+        if not args.data or not args.dataset:
+            p.error('-m val needs --data <dataset root> and --dataset {sintel,kitti}')
+        return validate(args)
     if args.mode != 'test':
         print(f"mode '{args.mode}' has no implementation in the reference either (infer_raft.py:71-95); nothing to do")
         return 0
@@ -94,6 +110,7 @@ def main(argv=None):
     import cv2
     from flow_utils import flow_to_color, resize_flow, write_flo
     rgb = args.upstream  # the official checkpoints expect RGB frames; the reference's expect BGR
+    args.iters = 20 if args.iters is None else args.iters
     if args.keep_size:
         left, right = read_pair(args.im1, args.im2, None, rgb)
         model = RAFT.RAFT(left.shape[1:], args, iters=args.iters, upstream=args.upstream,
@@ -134,6 +151,22 @@ def main(argv=None):
         for k, frame in enumerate(frames):
             img = np.clip(np.rint(255.0 * frame[0]), 0, 255).astype(np.uint8)
             cv2.imwrite(f"raft_interp_{k}.png", cv2.cvtColor(img, cv2.COLOR_RGB2BGR) if rgb else img)
+    return 0
+
+
+def validate(args):
+    """-m val: raft_b200.evaluate on --data, upstream's summary lines on stdout, everything in <--out>/val_<dataset>.json."""
+    import json
+    from networks import RAFT
+    from raft_b200.evaluate import evaluate, summary_lines
+    model = RAFT.RAFT(None, args, upstream=args.upstream, mixed_precision=args.mixed_precision).load(args.load)
+    res = evaluate(model, args.data, args.dataset, dstypes=tuple(args.dstype), batch=args.batch, workers=args.workers,
+                   iters=args.iters)
+    for line in summary_lines(res):
+        print(line)
+    os.makedirs(args.out, exist_ok=True)
+    with open(os.path.join(args.out, f"val_{args.dataset}.json"), "w") as f:
+        json.dump(res, f, indent=1)
     return 0
 
 

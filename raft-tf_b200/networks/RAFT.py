@@ -15,7 +15,7 @@ from networks import model_utils
 from networks.model_utils import GetCorrPyramid, SampleCorr, BasicUpdateBlock, SmallUpdateBlock  # noqa: F401
 from networks.utils import coords_grid, upflow8  # noqa: F401
 from raft_b200 import capi
-from raft_b200.engine import RaftEngine
+from raft_b200.engine import PAD_MODES, RaftEngine
 from raft_b200.weights import load_npz
 
 
@@ -24,7 +24,7 @@ class RAFT(object):
     data_format = 'NHWC'
 
     def __init__(self, image_shape, args, iters=20, batch=1, device=None, volume_free=None, input_size=None, upstream=False,
-                 mixed_precision=False):
+                 mixed_precision=False, pad_mode='sintel'):
         self.dropout = 0.0
         self.corr_radius = 4
         self.hidden_dim = 128
@@ -46,6 +46,10 @@ class RAFT(object):
         self.upstream = bool(upstream)
         # extension: fp16 conv operands with fp32 accumulation, upstream's --mixed_precision (RaftEngine mixed_precision)
         self.mixed_precision = bool(mixed_precision)
+        # extension: upstream InputPadder's padding to a multiple of 8, 'sintel' (split) or 'kitti' (bottom only)
+        if pad_mode not in PAD_MODES:
+            raise ValueError(f"pad_mode must be one of {PAD_MODES} (got {pad_mode!r})")
+        self.pad_mode = pad_mode
         self.flow_result = None
         self._engine = None
         self._params = None
@@ -90,7 +94,7 @@ class RAFT(object):
                 raise RuntimeError("RAFT.load(<npz>) must be called before inference")
             self._engine = RaftEngine(self._params, small=self.small, iters=self.iters, device=self.device,
                                       volume_free=self.volume_free, input_size=self.input_size, upstream=self.upstream,
-                                      mixed_precision=self.mixed_precision)
+                                      mixed_precision=self.mixed_precision, pad_mode=self.pad_mode)
         return self._engine
 
     # -- inference ---------------------------------------------------------------------------------

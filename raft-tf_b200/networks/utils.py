@@ -55,6 +55,32 @@ def fb_consistency(flow_fw, flow_bw, alpha1=0.01, alpha2=0.5, flow_scale=1.0):
     return occ_fw, occ_bw
 
 
+FLOW_STATS = ("n", "sum_epe", "lt1", "lt3", "lt5", "outliers")  # the columns of flow_metrics' stats (RB_FLOW_STATS)
+
+
+def flow_metrics(flow, gt, valid=None, flow_scale=1.0, return_epe=False):
+    """Extension (upstream RAFT's evaluate.py): end-point-error statistics of [B,H,W,2] CUDA flows against ground truth gt
+    (rb_flow_metrics).  valid: optional [B,H,W] mask, nonzero = the pixel counts.  flow_scale multiplies the flow first: 8.0
+    for raft-small in the reference semantics, whose upflow8 output is in 1/8-resolution units.  Returns the [B,6] fp64
+    stats {n, sum of EPE, #(EPE < 1), #(EPE < 3), #(EPE < 5), #KITTI outliers (EPE > 3 and EPE / |gt| > 0.05)} over the
+    counted pixels (FLOW_STATS), and with return_epe also the [B,H,W] fp32 per-pixel EPE (every pixel)."""
+    assert flow.shape == gt.shape and flow.dim() == 4 and flow.shape[-1] == 2, (flow.shape, gt.shape)
+    assert flow.device == gt.device, (flow.device, gt.device)
+    B, H, W, _ = flow.shape
+    f, g = flow.contiguous().float(), gt.contiguous().float()
+    if valid is not None:
+        assert tuple(valid.shape) == (B, H, W) and valid.device == f.device, (valid.shape, valid.device)
+        valid = valid.contiguous().to(torch.uint8)
+    stats = torch.empty(B, len(FLOW_STATS), dtype=torch.float64, device=f.device)
+    epe = torch.empty(B, H, W, dtype=torch.float32, device=f.device) if return_epe else None
+    with torch.cuda.device(f.device):
+        nbytes = capi.size_query(capi.lib.rb_flow_metrics_workspace_bytes, B, H, W)
+        ws = torch.empty(nbytes, dtype=torch.uint8, device=f.device)
+        capi.check(capi.lib.rb_flow_metrics(capi.ptr(f), float(flow_scale), capi.ptr(g), capi.ptr(valid), B, H, W,
+                                            capi.ptr(epe), capi.ptr(stats), capi.ptr(ws), nbytes, capi.stream()))
+    return (stats, epe) if return_epe else stats
+
+
 def reverse_flow(flow, time_step=1.0, bg=None, im0=None):
     """The reference's flow_utils.py:166 reverse_flow_avg_skip_static on a batch of CUDA flows (rb_flow_reverse, bit for
     bit): projects the [B,H,W,2] flow 0 -> 1 to time `time_step` and returns the flow from there back to frame 0.

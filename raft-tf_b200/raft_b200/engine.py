@@ -32,6 +32,8 @@ FB_ALPHA1, FB_ALPHA2 = 0.01, 0.5
 MIN_FRAME = 57
 # upstream mode divides by W_l - 1 at every pyramid level: level 3 must be at least 2 wide, a grid of 16, H >= 121
 MIN_FRAME_UPSTREAM = 121
+# upstream InputPadder's modes (pad_mode)
+PAD_MODES = ("sintel", "kitti")
 
 
 class RaftEngine:
@@ -43,7 +45,12 @@ class RaftEngine:
     def __init__(self, params: Dict[str, np.ndarray], small: bool = False, iters: int = 20,
                  device: Optional[torch.device] = None, use_graph: bool = True, math_mode: int = capi.RB_MATH_TC,
                  volume_free: Optional[bool] = None, input_size: Optional[Tuple[int, int]] = None,
-                 upstream: bool = False, mixed_precision: bool = False):
+                 upstream: bool = False, mixed_precision: bool = False, pad_mode: str = "sintel"):
+        # pad_mode: how frames are replicate-padded to a multiple of 8, like upstream's InputPadder -- 'sintel' splits the
+        # padding top / bottom and left / right, 'kitti' pads the bottom only (and splits left / right)
+        if pad_mode not in PAD_MODES:
+            raise ValueError(f"raft_b200: pad_mode must be one of {PAD_MODES} (got {pad_mode!r})")
+        self.pad_mode = pad_mode
         # mixed_precision: upstream RAFT's --mixed_precision boundary -- every conv as one fp16 x fp16 wgmma per product with
         # fp32 accumulation, the correlation and all elementwise work as in RB_MATH_TC (RB_MATH_TC_FP16, include/raft_b200.h)
         if mixed_precision:
@@ -99,7 +106,7 @@ class RaftEngine:
     # ---- buffers -------------------------------------------------------------------------------
     def _ensure(self, B: int, H: int, W: int, u8: bool = False, mode: int = FORWARD):
         """Buffers for B frame pairs of H x W pixels.  H, W need not be multiples of 8: frames are replicate-padded
-        to (Hp, Wp) by rb_frames_prepare (upstream InputPadder 'sintel' split, SURVEY 8(d)) and the flow is cropped
+        to (Hp, Wp) by rb_frames_prepare (upstream InputPadder's split of pad_mode, SURVEY 8(d)) and the flow is cropped
         back by the upsampling kernel -- the reference itself cannot run such shapes (SURVEY fact 6).
 
         In the bidirectional modes the hot path runs 2B pairs, (L_i -> R_i) then (R_i -> L_i): fmaps holds 3B feature
@@ -130,7 +137,8 @@ class RaftEngine:
         bidir = mode != FORWARD
         NB = 2 * B if bidir else B  # frame pairs through the hot path
         ph, pw = (-H) % 8, (-W) % 8
-        self.pad = (ph // 2, ph - ph // 2, pw // 2, pw - pw // 2)  # top, bottom, left, right
+        top = 0 if self.pad_mode == "kitti" else ph // 2
+        self.pad = (top, ph - top, pw // 2, pw - pw // 2)  # top, bottom, left, right
         Hp, Wp = H + ph, W + pw
         h, w, s = Hp // 8, Wp // 8, int(self.small)
         d = self.device

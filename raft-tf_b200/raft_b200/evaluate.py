@@ -1,0 +1,271 @@
+"""F9: upstream RAFT's validation protocol (evaluate.py: validate_sintel, validate_kitti) with the metrics on the GPU.
+
+    from raft_b200.evaluate import evaluate
+    res = evaluate(RAFT(None, args, upstream=True).load("raft-things.npz"), "datasets/Sintel", "sintel")
+
+Sintel: every frame of <root>/training/{clean,final}/<scene>/ paired with the next one, ground truth
+<root>/training/flow/<scene>/frame_NNNN.flo, 32 iterations, InputPadder 'sintel' padding, every pixel counted.  KITTI-2015:
+<root>/training/image_2/<id>_10.png and <id>_11.png, ground truth <root>/training/flow_occ/<id>_10.png (16-bit PNG with a
+valid flag), 24 iterations, 'kitti' padding (bottom only), valid pixels counted.  Frames run at their own size.
+
+Pipeline: pairs are grouped by frame size (one CUDA graph per size) and run in batches through RaftEngine.forward, whose
+flow stays on the GPU: rb_flow_metrics scores it against the uploaded ground truth on the same stream and writes per-pair
+stats into one device buffer, read back once per split.  Worker threads decode the next batches (cv2 releases the GIL)
+while the GPU runs the current one, into two pinned staging slots used in turn; a slot is refilled only after the event
+recorded behind its batch's work has completed.  Every kernel is batch-invariant, so the results are the same bits for
+every batch size and worker count.  Aggregates are computed on the host in fp64 from the per-pair stats.
+"""
+from __future__ import annotations
+
+import os
+import re
+import struct
+from collections import namedtuple
+from concurrent.futures import ThreadPoolExecutor
+
+import numpy as np
+import torch
+
+from . import capi
+from .engine import RaftEngine
+
+# dataset -> (iterations, pad_mode): upstream's validate_sintel / validate_kitti
+PROTOCOLS = {"sintel": (32, "sintel"), "kitti": (24, "kitti")}
+DSTYPES = ("clean", "final")
+STATS = 6  # RB_FLOW_STATS: n, sum of EPE, #(EPE < 1), #(EPE < 3), #(EPE < 5), #outliers
+
+Pair = namedtuple("Pair", "image1 image2 gt")
+
+
+# ---- dataset enumeration ----------------------------------------------------------------------------
+def _listdir(path, what):
+    if not os.path.isdir(path):
+        raise FileNotFoundError(f"{what}: no directory {path}")
+    return sorted(os.listdir(path))
+
+
+def sintel_pairs(root, dstype="clean"):
+    """MPI-Sintel training pairs of one pass (dstype 'clean' or 'final'), scene by scene in sorted order: frame k with
+    frame k + 1 of the same scene and the ground truth of frame k.  Frame numbers must be consecutive within a scene, and
+    every frame but the last needs its .flo and every .flo its frame: otherwise FileNotFoundError names the file."""
+    if dstype not in DSTYPES:
+        raise ValueError(f"Sintel dstype must be one of {DSTYPES} (got {dstype!r})")
+    img_root, flow_root = os.path.join(root, "training", dstype), os.path.join(root, "training", "flow")
+    pairs = []
+    for scene in _listdir(img_root, "Sintel"):
+        sdir = os.path.join(img_root, scene)
+        if not os.path.isdir(sdir):
+            continue
+        frames = [f for f in sorted(os.listdir(sdir)) if f.endswith(".png")]
+        fdir = os.path.join(flow_root, scene)
+        flos = set(f for f in _listdir(fdir, "Sintel ground truth") if f.endswith(".flo"))
+        for a, b in zip(frames[:-1], frames[1:]):
+            ma, mb = re.fullmatch(r"frame_(\d+)\.png", a), re.fullmatch(r"frame_(\d+)\.png", b)
+            if not (ma and mb and int(mb.group(1)) == int(ma.group(1)) + 1):
+                raise FileNotFoundError(f"Sintel: {os.path.join(sdir, b)} does not follow {os.path.join(sdir, a)} "
+                                        "(frames must be frame_NNNN.png, numbered consecutively)")
+            flo = a[:-4] + ".flo"
+            if flo not in flos:
+                raise FileNotFoundError(f"Sintel: ground truth {os.path.join(fdir, flo)} of {os.path.join(sdir, a)} is "
+                                        "missing")
+            flos.discard(flo)
+            pairs.append(Pair(os.path.join(sdir, a), os.path.join(sdir, b), os.path.join(fdir, flo)))
+        if flos:
+            raise FileNotFoundError(f"Sintel: ground truth {os.path.join(fdir, sorted(flos)[0])} has no frame pair")
+    if not pairs:
+        raise FileNotFoundError(f"Sintel: no frame pairs under {img_root}")
+    return pairs
+
+
+def kitti_pairs(root):
+    """KITTI-2015 training pairs in sorted id order: image_2/<id>_10.png, image_2/<id>_11.png, flow_occ/<id>_10.png.  A
+    missing second frame or ground truth, or a ground truth without frames, raises FileNotFoundError naming the file."""
+    img_root, flow_root = os.path.join(root, "training", "image_2"), os.path.join(root, "training", "flow_occ")
+    images = set(_listdir(img_root, "KITTI"))
+    gts = set(f for f in _listdir(flow_root, "KITTI ground truth") if f.endswith("_10.png"))
+    pairs = []
+    for f in sorted(images):
+        if not f.endswith("_10.png"):
+            continue
+        second = f[:-len("_10.png")] + "_11.png"
+        if second not in images:
+            raise FileNotFoundError(f"KITTI: second frame {os.path.join(img_root, second)} is missing")
+        if f not in gts:
+            raise FileNotFoundError(f"KITTI: ground truth {os.path.join(flow_root, f)} is missing")
+        gts.discard(f)
+        pairs.append(Pair(os.path.join(img_root, f), os.path.join(img_root, second), os.path.join(flow_root, f)))
+    if gts:
+        raise FileNotFoundError(f"KITTI: ground truth {os.path.join(flow_root, sorted(gts)[0])} has no frame pair")
+    if not pairs:
+        raise FileNotFoundError(f"KITTI: no frame pairs under {img_root}")
+    return pairs
+
+
+# ---- decoding (worker threads) ------------------------------------------------------------------------
+def _png_size(path):
+    """(H, W) from the PNG header, without decoding the image."""
+    with open(path, "rb") as f:
+        head = f.read(24)
+    if len(head) < 24 or head[:8] != b"\x89PNG\r\n\x1a\n" or head[12:16] != b"IHDR":
+        raise ValueError(f"{path}: not a PNG file")
+    w, h = struct.unpack(">II", head[16:24])
+    return int(h), int(w)
+
+
+def _imread(path, rgb):
+    import cv2
+    img = cv2.imread(path, cv2.IMREAD_COLOR)  # BGR uint8
+    if img is None:
+        raise FileNotFoundError(f"cannot read {path}")
+    return cv2.cvtColor(img, cv2.COLOR_BGR2RGB) if rgb else img
+
+
+def _decode(pair, kitti, rgb):
+    from flow_utils import read_flo, read_kitti_flow
+    left, right = _imread(pair.image1, rgb), _imread(pair.image2, rgb)
+    if right.shape != left.shape:
+        raise ValueError(f"{pair.image2}: {right.shape[:2]} frame, {pair.image1} is {left.shape[:2]}")
+    gt, valid = read_kitti_flow(pair.gt) if kitti else (read_flo(pair.gt), None)
+    if gt.shape[:2] != left.shape[:2]:
+        raise ValueError(f"{pair.gt}: {gt.shape[:2]} ground truth for {left.shape[:2]} frames ({pair.image1})")
+    return left, right, gt, valid
+
+
+class _Slot:
+    """Pinned host staging of one batch (frames, ground truth, mask) and the event behind the last batch that used it."""
+
+    def __init__(self, B, H, W, kitti):
+        self.left = torch.zeros(B, H, W, 3, dtype=torch.uint8).pin_memory()
+        self.right = torch.zeros_like(self.left).pin_memory()
+        self.gt = torch.zeros(B, H, W, 2, dtype=torch.float32).pin_memory()
+        self.valid = torch.zeros(B, H, W, dtype=torch.uint8).pin_memory() if kitti else None
+        self.event = None
+
+
+# ---- the run ------------------------------------------------------------------------------------------
+def _run(engine, pairs, kitti, batch, workers, rgb):
+    """Per-pair stats [N, STATS] fp64 (host, dataset order) of engine.forward on every pair."""
+    groups = {}  # (H, W) -> pair indices in dataset order; sizes in the order they first appear
+    for i, p in enumerate(pairs):
+        groups.setdefault(_png_size(p.image1), []).append(i)
+    batches = []
+    for hw, idx in groups.items():
+        B = min(batch, len(idx))
+        batches += [(hw, B, idx[k:k + B]) for k in range(0, len(idx), B)]
+    order = [i for _, _, idx in batches for i in idx]  # processing order
+    dev = engine.device
+    pool = ThreadPoolExecutor(workers) if workers > 0 else None
+    # decode this many batches ahead of the one the GPU is given (workers=0: the main thread decodes batch j + 1 while the
+    # GPU runs batch j)
+    depth = max(1, -(-workers // batch))
+
+    def submit(j):
+        idx = batches[j][2]
+        if pool is None:
+            return [lambda i=i: _decode(pairs[i], kitti, rgb) for i in idx]
+        return [pool.submit(_decode, pairs[i], kitti, rgb).result for i in idx]
+
+    try:
+        with torch.cuda.device(dev):
+            stats = torch.empty(len(pairs), STATS, dtype=torch.float64, device=dev)
+            stream = torch.cuda.current_stream(dev)
+            ahead = [submit(j) for j in range(min(depth, len(batches)))]
+            shape, pos = None, 0
+            for j, ((H, W), B, idx) in enumerate(batches):
+                loads = ahead.pop(0)
+                if j + depth < len(batches):
+                    ahead.append(submit(j + depth))  # workers start on it now
+                if shape != (B, H, W):
+                    shape = (B, H, W)
+                    slots = [_Slot(B, H, W, kitti), _Slot(B, H, W, kitti)]
+                    gt = torch.empty(B, H, W, 2, dtype=torch.float32, device=dev)
+                    valid = torch.empty(B, H, W, dtype=torch.uint8, device=dev) if kitti else None
+                    ws_bytes = capi.size_query(capi.lib.rb_flow_metrics_workspace_bytes, B, H, W)
+                    ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
+                slot = slots[j % 2]
+                if slot.event is not None:
+                    slot.event.synchronize()  # its last batch's copies (and work) are done
+                lft, rgt, g, v = slot.left.numpy(), slot.right.numpy(), slot.gt.numpy(), None
+                if kitti:
+                    v = slot.valid.numpy()
+                for k, load in enumerate(loads):
+                    lft[k], rgt[k], g[k], vk = load()
+                    if kitti:
+                        v[k] = vk
+                nb = len(idx)  # a short last batch keeps B: the rows past nb are run but not scored
+                flow = engine.forward(slot.left, slot.right)
+                gt.copy_(slot.gt, non_blocking=True)
+                if kitti:
+                    valid.copy_(slot.valid, non_blocking=True)
+                capi.check(capi.lib.rb_flow_metrics(capi.ptr(flow), float(engine.flow_scale), capi.ptr(gt),
+                                                    capi.ptr(valid), nb, H, W, None, capi.ptr(stats[pos:pos + nb]),
+                                                    capi.ptr(ws), ws_bytes, capi.stream()))
+                slot.event = torch.cuda.Event()
+                slot.event.record(stream)
+                pos += nb
+            host = stats.cpu().numpy()
+    finally:
+        if pool is not None:
+            pool.shutdown(wait=True, cancel_futures=True)
+    out = np.empty_like(host)
+    out[order] = host
+    return out
+
+
+def aggregate(pairs, stats, kitti):
+    """fp64 aggregates of the per-pair stats [N, STATS]: epe pooled over all counted pixels (Sintel) or the mean of the
+    per-pair means (KITTI, as upstream's validate_kitti); 1px / 3px / 5px pooled fractions; f1 = 100 * outliers / pixels;
+    and one record per pair in dataset order."""
+    s = np.asarray(stats, dtype=np.float64).reshape(-1, STATS)
+    n, se, c1, c3, c5, out = s.T
+    tot = n.sum()
+    with np.errstate(divide="ignore", invalid="ignore"):
+        mean = se / n
+        res = {"epe": float(mean.mean() if kitti else se.sum() / tot), "1px": float(c1.sum() / tot),
+               "3px": float(c3.sum() / tot), "5px": float(c5.sum() / tot), "f1": float(100.0 * out.sum() / tot),
+               "pixels": int(tot), "n_pairs": len(s)}
+        res["pairs"] = [{"image1": p.image1, "image2": p.image2, "gt": p.gt, "n": int(r[0]), "epe": float(r[1] / r[0]),
+                         "1px": float(r[2] / r[0]), "3px": float(r[3] / r[0]), "5px": float(r[4] / r[0]),
+                         "f1": float(100.0 * r[5] / r[0])} for p, r in zip(pairs, np.asarray(s))]
+    return res
+
+
+def evaluate(model, root, dataset="sintel", dstypes=DSTYPES, batch=1, workers=4, iters=None):
+    """Upstream RAFT's validation of a loaded networks.RAFT.RAFT model on a Sintel or KITTI-2015 training tree.
+
+    The engine is built from the model's configuration (small, upstream, mixed_precision, volume_free, device, weights)
+    with the protocol's iterations (iters overrides them) and padding.  Frames go in RGB with upstream=True and BGR
+    otherwise, like the CLI.  A model with input_size is refused: validation runs frames at their own size.  Returns
+    {"dataset", "iters", "pad_mode", "splits": {name: aggregate(...)}} with the splits 'clean' / 'final' (Sintel, those in
+    dstypes) or 'kitti'; the same for every batch and workers."""
+    if dataset not in PROTOCOLS:
+        raise ValueError(f"dataset must be one of {tuple(PROTOCOLS)} (got {dataset!r})")
+    if getattr(model, "input_size", None) is not None:
+        raise ValueError("evaluate: validation runs frames at their own size; build the model without input_size")
+    if int(batch) < 1 or int(workers) < 0:
+        raise ValueError(f"evaluate: batch must be >= 1 and workers >= 0 (got {batch}, {workers})")
+    if model._params is None:
+        raise RuntimeError("RAFT.load(<npz>) must be called before evaluate")
+    kitti = dataset == "kitti"
+    splits = ("kitti",) if kitti else tuple(dstypes)
+    if not kitti and (not splits or any(d not in DSTYPES for d in splits)):
+        raise ValueError(f"Sintel dstypes must be a non-empty subset of {DSTYPES} (got {dstypes!r})")
+    n_iters, pad_mode = PROTOCOLS[dataset]
+    n_iters = n_iters if iters is None else int(iters)
+    lists = {s: kitti_pairs(root) if kitti else sintel_pairs(root, s) for s in splits}  # every file checked up front
+    engine = RaftEngine(model._params, small=model.small, iters=n_iters, device=model.device, volume_free=model.volume_free,
+                        upstream=model.upstream, mixed_precision=model.mixed_precision, pad_mode=pad_mode)
+    res = {"dataset": dataset, "iters": n_iters, "pad_mode": pad_mode, "splits": {}}
+    for s, pairs in lists.items():
+        res["splits"][s] = aggregate(pairs, _run(engine, pairs, kitti, int(batch), int(workers), model.upstream), kitti)
+    return res
+
+
+def summary_lines(res):
+    """upstream evaluate.py's lines: 'Validation (clean) EPE: ..., 1px: ..., 3px: ..., 5px: ...' per Sintel pass,
+    'Validation KITTI: <epe>, <f1>'."""
+    if res["dataset"] == "kitti":
+        r = res["splits"]["kitti"]
+        return ["Validation KITTI: %f, %f" % (r["epe"], r["f1"])]
+    return ["Validation (%s) EPE: %f, 1px: %f, 3px: %f, 5px: %f" % (s, r["epe"], r["1px"], r["3px"], r["5px"])
+            for s, r in res["splits"].items()]

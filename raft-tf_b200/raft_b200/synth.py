@@ -18,8 +18,9 @@ def _blur(a: np.ndarray, sigma: float) -> np.ndarray:
     return gaussian_filter(a, sigma=(sigma, sigma, 0), mode="wrap")
 
 
-def make_pair(H: int, W: int, seed: int = 1000, amp: float = 12.0) -> Tuple[np.ndarray, np.ndarray]:
-    """One synthetic frame pair, float32 [H,W,3] in [0,1]."""
+def make_pair(H: int, W: int, seed: int = 1000, amp: float = 12.0, return_flow: bool = False):
+    """One synthetic frame pair, float32 [H,W,3] in [0,1]; with return_flow also the [H,W,2] float32 flow (u, v) that
+    warped the first frame into the second (frame 2 at p samples frame 1 at p - flow(p))."""
     from scipy.ndimage import map_coordinates
     rng = np.random.default_rng(seed)
     base = rng.random((H + 64, W + 64, 3), dtype=np.float32)
@@ -36,7 +37,38 @@ def make_pair(H: int, W: int, seed: int = 1000, amp: float = 12.0) -> Tuple[np.n
     f2 = np.stack([map_coordinates(base[..., c], [ys + 32 - v, xs + 32 - u], order=1, mode="nearest")
                    for c in range(3)], axis=-1)
     f2 = f2 + rng.normal(0, 0.01, f2.shape).astype(np.float32)
-    return f1.astype(np.float32), np.clip(f2, 0, 1).astype(np.float32)
+    frames = (f1.astype(np.float32), np.clip(f2, 0, 1).astype(np.float32))
+    return frames + (np.stack([u, v], -1).astype(np.float32),) if return_flow else frames
+
+
+def write_sintel_tree(root: str, scenes: int, frames: int, H: int, W: int, seed: int = 2000,
+                      dstypes: Tuple[str, ...] = ("clean", "final")) -> int:
+    """A dataset in MPI-Sintel's training layout under root (training/<dstype>/scene_<i>/frame_NNNN.png as 8-bit PNG,
+    training/flow/scene_<i>/frame_NNNN.flo) from make_pair: frames 2j+1 and 2j+2 of a scene are one synthetic pair and the
+    ground truth of frame 2j+1 is the flow that made it; frame 2j+2 and the next pair's first frame are unrelated and get a
+    zero ground truth.  'final' holds the 'clean' frames at lower contrast, so both share the ground truth, as in Sintel.
+    Returns the number of pairs per dstype."""
+    import os
+
+    import cv2
+    from flow_utils import write_flo
+    for i in range(scenes):
+        fdir = os.path.join(root, "training", "flow", f"scene_{i}")
+        os.makedirs(fdir, exist_ok=True)
+        for j in range(0, frames, 2):
+            f1, f2, flow = make_pair(H, W, seed + 100 * i + j, return_flow=True)
+            gts = ((j, flow), (j + 1, np.zeros_like(flow)))
+            for k, g in gts:
+                if k < frames - 1:
+                    write_flo(os.path.join(fdir, f"frame_{k + 1:04d}.flo"), g)
+            for dstype in dstypes:
+                sdir = os.path.join(root, "training", dstype, f"scene_{i}")
+                os.makedirs(sdir, exist_ok=True)
+                for k, f in ((j, f1), (j + 1, f2)):
+                    if k < frames:
+                        f = f if dstype == "clean" else 0.8 * f + 0.1
+                        cv2.imwrite(os.path.join(sdir, f"frame_{k + 1:04d}.png"), np.round(255 * f).astype(np.uint8))
+    return scenes * (frames - 1)
 
 
 def make_batch(B: int, H: int, W: int, seed0: int = 1000):
