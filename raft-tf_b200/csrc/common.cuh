@@ -391,91 +391,105 @@ __device__ __forceinline__ void split2(float a, float b, uint32_t& hi, uint32_t&
   hi = *reinterpret_cast<const uint32_t*>(&h);
   lo = *reinterpret_cast<const uint32_t*>(&l);
 }
-__device__ __forceinline__ void store_split16(__half* dhi, __half* dlo, size_t off, const float* y) {
-  uint32_t h[8], l[8];
+// 8 channels = 16 bytes per fp16 plane
+__device__ __forceinline__ void st128_b32(void* dst, const uint32_t* v) {
+  asm volatile("st.global.v4.b32 [%0], {%1,%2,%3,%4};" :: "l"(dst), "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]) : "memory");
+}
+__device__ __forceinline__ void ld128_nc(const void* src, uint32_t* d) {
+  asm volatile("ld.global.nc.v4.b32 {%0,%1,%2,%3}, [%4];" : "=r"(d[0]), "=r"(d[1]), "=r"(d[2]), "=r"(d[3]) : "l"(src));
+}
+__device__ __forceinline__ void store_split8(__half* dhi, __half* dlo, size_t off, const float* y) {
+  uint32_t h[4], l[4];
 #pragma unroll
-  for (int i = 0; i < 8; ++i) split2(y[2 * i], y[2 * i + 1], h[i], l[i]);
-  st256_b32(dhi + off, h);
-  st256_b32(dlo + off, l);
-}
-__device__ __forceinline__ void load16(const float* src, float* d) {
-  ld256(src, d);
-  ld256(src + 8, d + 8);
-}
-__device__ __forceinline__ void store16(float* dst, const float* v) {
-  st256(dst, v);
-  st256(dst + 8, v + 8);
+  for (int i = 0; i < 4; ++i) split2(y[2 * i], y[2 * i + 1], h[i], l[i]);
+  st128_b32(dhi + off, h);
+  st128_b32(dlo + off, l);
 }
 
-__device__ __forceinline__ void epilogue_wide16(const ConvParams& p, int pix, int c, float* y) {
+// A thread's 16 values are two groups of 8 consecutive channels: y[0..8) = channels [ca, ca+8), y[8..16) = [cb, cb+8).
+// cb = ca + 8 is one 16-channel group.  The tensor-core kernel may instead give lanes 2i and 2i+1 the groups (ca, ca+16)
+// and (ca+8, ca+24) of the same pixel, so that each of their 16-byte fp16 stores fills one 32-byte sector
+// (conv_tc.cu: paired epilogue lanes).  ca, cb are multiples of 8; a group never straddles `hidden` or `cout`.
+__device__ __forceinline__ void epilogue_wide16(const ConvParams& p, int pix, int ca, int cb, float* y) {
   if (p.bias) {
     float t[16];
-    ld256_nc(p.bias + c, t);
-    ld256_nc(p.bias + c + 8, t + 8);
+    ld256_nc(p.bias + ca, t);
+    ld256_nc(p.bias + cb, t + 8);
 #pragma unroll
     for (int i = 0; i < 16; ++i) y[i] += t[i];
   }
   if (p.addend) {
     float t[16];
-    const float* ad = p.addend + (size_t)pix * p.cout + c;
-    ld256_nc(ad, t);
-    ld256_nc(ad + 8, t + 8);
+    const float* ad = p.addend + (size_t)pix * p.cout;
+    ld256_nc(ad + ca, t);
+    ld256_nc(ad + cb, t + 8);
 #pragma unroll
     for (int i = 0; i < 16; ++i) y[i] += t[i];
   }
+  auto store_split = [&](__half* dhi, __half* dlo, size_t base, int off) {  // both groups, channel `off` below ca / cb
+    store_split8(dhi, dlo, base + ca - off, y);
+    store_split8(dhi, dlo, base + cb - off, y + 8);
+  };
+  auto load_f32 = [&](const float* row, int off, float* d) {
+    ld256(row + ca - off, d);
+    ld256(row + cb - off, d + 8);
+  };
+  auto store_f32 = [&](float* row, int off) {
+    st256(row + ca - off, y);
+    st256(row + cb - off, y + 8);
+  };
   switch (p.epi) {
     case EPI_ACT: {
       if (p.act == ACT_RELU) {
 #pragma unroll
         for (int i = 0; i < 16; ++i) y[i] = fmaxf(y[i], 0.f);
       }
-      if (p.res_hi) {  // block output: relu(x + y), x as split planes (16 channels = 32 bytes per plane)
-        __align__(32) __half rh[16], rl[16];
-        const size_t ro = (size_t)pix * p.res_stride + c;
-        ld256_nc(reinterpret_cast<const float*>(p.res_hi + ro), reinterpret_cast<float*>(rh));
-        ld256_nc(reinterpret_cast<const float*>(p.res_lo + ro), reinterpret_cast<float*>(rl));
+      if (p.res_hi) {  // block output: relu(x + y), x as split planes (8 channels = 16 bytes per plane and group)
+        __align__(16) __half rh[16], rl[16];
+        const size_t ro = (size_t)pix * p.res_stride;
+        ld128_nc(p.res_hi + ro + ca, reinterpret_cast<uint32_t*>(rh));
+        ld128_nc(p.res_hi + ro + cb, reinterpret_cast<uint32_t*>(rh + 8));
+        ld128_nc(p.res_lo + ro + ca, reinterpret_cast<uint32_t*>(rl));
+        ld128_nc(p.res_lo + ro + cb, reinterpret_cast<uint32_t*>(rl + 8));
 #pragma unroll
         for (int i = 0; i < 16; ++i) y[i] = fmaxf(join_f32(rh[i], rl[i]) + y[i], 0.f);
       }
-      if (p.flow_tail && c + 16 == p.cout) {
-        // motion encoder: [126 conv channels | flow] (model_utils.py:119) -- the flow slot completes the 16-channel group,
-        // same arithmetic as flow_conv7_kernel (coords1 - coords_grid, RAFT.py:95)
+      if (p.flow_tail && cb + 8 == p.cout) {
+        // motion encoder: [126 conv channels | flow] (model_utils.py:119) -- the flow slot completes the last 8-channel
+        // group, same arithmetic as flow_conv7_kernel (coords1 - coords_grid, RAFT.py:95)
         const int x = pix % p.w, yy = (pix / p.w) % p.h;
         const float2 cc = *reinterpret_cast<const float2*>(p.flow_tail + (size_t)pix * 2);
         y[14] = cc.x - (float)x;
         y[15] = cc.y - (float)yy;
       }
-      store_split16(p.d0_hi, p.d0_lo, (size_t)pix * p.d0_stride + p.d0_choff + c, y);
-      if (p.d1_hi) store_split16(p.d1_hi, p.d1_lo, (size_t)pix * p.d1_stride + p.d1_choff + c, y);
+      store_split(p.d0_hi, p.d0_lo, (size_t)pix * p.d0_stride + p.d0_choff, 0);
+      if (p.d1_hi) store_split(p.d1_hi, p.d1_lo, (size_t)pix * p.d1_stride + p.d1_choff, 0);
     } break;
     case EPI_ZR: {
-      if (c < p.hidden) {
+      if (ca < p.hidden) {
 #pragma unroll
         for (int i = 0; i < 16; ++i) y[i] = sigmoid_f(y[i]);
-        store16(p.f0 + (size_t)pix * p.hidden + c, y);
+        store_f32(p.f0 + (size_t)pix * p.hidden, 0);
       } else {
-        const int ch = c - p.hidden;
         float hprev[16];
-        load16(p.f1 + (size_t)pix * p.hidden + ch, hprev);
+        load_f32(p.f1 + (size_t)pix * p.hidden, p.hidden, hprev);
 #pragma unroll
         for (int i = 0; i < 16; ++i) y[i] = sigmoid_f(y[i]) * hprev[i];
-        store_split16(p.d0_hi, p.d0_lo, (size_t)pix * p.d0_stride + p.d0_choff + ch, y);
+        store_split(p.d0_hi, p.d0_lo, (size_t)pix * p.d0_stride + p.d0_choff, p.hidden);
       }
     } break;
     case EPI_Q: {
       float z[16], hprev[16];
-      float* hp = p.f1 + (size_t)pix * p.hidden + c;
-      load16(p.f0 + (size_t)pix * p.hidden + c, z);
-      load16(hp, hprev);
+      float* hp = p.f1 + (size_t)pix * p.hidden;
+      load_f32(p.f0 + (size_t)pix * p.hidden, 0, z);
+      load_f32(hp, 0, hprev);
 #pragma unroll
       for (int i = 0; i < 16; ++i) {
         const float q = tanh_f(y[i]);
         y[i] = (1.0f - z[i]) * hprev[i] + z[i] * q;  // model_utils.py:147,155,168
       }
-      {
-        store16(hp, y);
-        store_split16(p.d0_hi, p.d0_lo, (size_t)pix * p.d0_stride + p.d0_choff + c, y);
-      }
+      store_f32(hp, 0);
+      store_split(p.d0_hi, p.d0_lo, (size_t)pix * p.d0_stride + p.d0_choff, 0);
     } break;
     default: {  // EPI_F32
       if (p.act == ACT_RELU) {
@@ -489,7 +503,7 @@ __device__ __forceinline__ void epilogue_wide16(const ConvParams& p, int pix, in
 #pragma unroll
         for (int i = 0; i < 16; ++i) y[i] = p.scale * y[i];
       }
-      store16(p.f0 + (size_t)pix * p.cout + c, y);
+      store_f32(p.f0 + (size_t)pix * p.cout, 0);
     } break;
   }
 }

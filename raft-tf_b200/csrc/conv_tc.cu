@@ -185,8 +185,19 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
     const int cw = (threadIdx.x >> 7) - 1;
     const int t = threadIdx.x & 127;
     const int wi = t >> 5;                   // warp inside the warpgroup: fragment rows 16 wi + lane/4 + {0, 8}
-    const int r = 64 * cw + (t & 63);        // epilogue: tile row = pixel index inside the box
-    const int half = t >> 6;                 // epilogue: 16-column half of a staged slab
+    // Epilogue lanes.  Default: thread t owns pixel t % 64 and the 16 columns [16 h, 16 h + 16) of a 32-column slab,
+    // h = t / 64 -- one pixel per lane, the layout of the fused instance-norm statistics (32 pixels per warp).
+    // PAIRED (every other 16-channel epilogue): lanes 2i, 2i + 1 own pixel i of the warpgroup's 64 and the 8-column groups
+    // {8 h, 16 + 8 h} of the slab, h = t % 2, so that each 16-byte fp16 store of a lane pair fills a whole 32-byte sector
+    // instead of half of one (the split-plane stores are most of the epilogue's memory traffic).  Same arithmetic per
+    // element.  Needs whole 32-channel slabs: cout, and hidden of the GRU epilogues, multiples of 32.
+    const bool paired = BLOCK_N >= 32 && wide && (p.cout & 31) == 0 && !(EXTRAS && p.stat_part) &&
+                        ((p.epi != EPI_ZR && p.epi != EPI_Q) || (p.hidden & 31) == 0);
+    const int prow = paired ? (t >> 1) : (t & 63);  // pixel of this lane among the warpgroup's 64 tile rows
+    const int r = 64 * cw + prow;            // epilogue: tile row = pixel index inside the box
+    const int half = paired ? (t & 1) : (t >> 6);  // epilogue: 16-column half (paired: 8-column groups) of a staged slab
+    const int gofs = paired ? 8 : 16;        // column of this lane's first group inside the slab: gofs * half
+    const int gsep = paired ? 16 : 8;        // columns between its two 8-column groups
     float* stg = staging + cw * 64 * kSlabPitch;
     asm volatile("griddepcontrol.wait;" ::: "memory");  // addend / z / h reads and all stores come after the predecessor
     constexpr int kNumAcc = BLOCK_N == 16 ? 2 : 1;  // the split-K halves of a 16-wide tile on one CTA
@@ -280,12 +291,12 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
         }
         consumer_bar_sync(1 + cw);
         if (Cfg::kSlab == 32 || half == 0) {  // warp-uniform
-          const int c = c0 + 16 * half;
+          const int c = c0 + gofs * half;  // first column of this lane (multiple of 8; 16 when not paired)
           float v[16];
-          const float4* src = reinterpret_cast<const float4*>(stg + (t & 63) * kSlabPitch + 16 * half);
+          const float* srow = stg + prow * kSlabPitch + c - c0;
 #pragma unroll
           for (int q4 = 0; q4 < 4; ++q4) {
-            const float4 f = src[q4];
+            const float4 f = *reinterpret_cast<const float4*>(srow + (q4 >> 1) * gsep + 4 * (q4 & 1));
             v[4 * q4] = f.x; v[4 * q4 + 1] = f.y; v[4 * q4 + 2] = f.z; v[4 * q4 + 3] = f.w;
           }
           bool store = valid && n0 + c < p.cout;
@@ -305,7 +316,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
           }
           if (store) {
             if (wide) {
-              epilogue_wide16(p, pix, n0 + c, v);
+              epilogue_wide16(p, pix, n0 + c, n0 + c + gsep, v);
             } else {
               epilogue_store<8>(p, pix, n0 + c, v);
               epilogue_store<8>(p, pix, n0 + c + 8, v + 8);
