@@ -5,6 +5,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
+#include <stdlib.h>
 
 #include "../../include/raft_b200.h"
 
@@ -37,6 +38,10 @@ struct PerDeviceOnce {
   bool test(int dev) const { return (__atomic_load_n(&done[(dev >> 6) & 3], __ATOMIC_ACQUIRE) >> (dev & 63)) & 1ull; }
   void set(int dev) { __atomic_fetch_or(&done[(dev >> 6) & 3], 1ull << (dev & 63), __ATOMIC_RELEASE); }
 };
+// v rounded up to a multiple of a (v >= 0)
+template <typename T>
+constexpr T round_up(T v, size_t a) { return (T)((v + a - 1) / a * a); }
+
 int current_device(int* dev);   // cudaGetDevice with error plumbing
 int device_sm_count(int dev);   // cached cudaDevAttrMultiProcessorCount (132 on H100 SXM)
 
@@ -66,6 +71,55 @@ int device_sm_count(int dev);   // cached cudaDevAttrMultiProcessorCount (132 on
       return code;                    \
     }                                 \
   } while (0)
+
+// ---- launches with programmatic dependent launch (PDL) ------------------------------------------
+// A PDL launch lets the kernel's blocks be scheduled while its predecessor in the stream drains; they wait in
+// griddepcontrol.wait before they read what it wrote.  RAFT_B200_NO_PDL=1 turns it off for every such launch.
+inline bool pdl_enabled() {
+  static const bool on = getenv("RAFT_B200_NO_PDL") == nullptr;
+  return on;
+}
+// The dynamic shared-memory limit of Kernel on device `dev`, raised once per (kernel, device).
+template <auto Kernel>
+int set_max_dyn_smem(int dev, int bytes) {
+  static PerDeviceOnce done;
+  if (!done.test(dev)) {
+    RB_CHECK_CUDA(cudaFuncSetAttribute(Kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
+    done.set(dev);
+  }
+  return RB_OK;
+}
+// Launches Kernel with `smem` bytes of dynamic shared memory as a PDL launch, after setting that limit on Kernel and on
+// the kernels in Also (instantiations launched interchangeably).  cluster > 0: clusters of that many CTAs along x.
+template <auto Kernel, auto... Also, typename... Args>
+int launch_pdl(dim3 grid, dim3 block, int smem, int cluster, cudaStream_t s, Args&&... args) {
+  int dev = 0, rc;
+  if ((rc = current_device(&dev))) return rc;
+  if ((rc = set_max_dyn_smem<Kernel>(dev, smem)) || ((rc = set_max_dyn_smem<Also>(dev, smem)) || ...)) return rc;
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = grid;
+  cfg.blockDim = block;
+  cfg.dynamicSmemBytes = smem;
+  cfg.stream = s;
+  cudaLaunchAttribute attr[2];
+  int n = 0;
+  if (cluster > 0) {
+    attr[n].id = cudaLaunchAttributeClusterDimension;
+    attr[n].val.clusterDim.x = cluster;
+    attr[n].val.clusterDim.y = 1;
+    attr[n].val.clusterDim.z = 1;
+    ++n;
+  }
+  if (pdl_enabled()) {
+    attr[n].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[n].val.programmaticStreamSerializationAllowed = 1;
+    ++n;
+  }
+  cfg.attrs = attr;
+  cfg.numAttrs = n;
+  RB_CHECK_CUDA(cudaLaunchKernelEx(&cfg, Kernel, static_cast<Args&&>(args)...));
+  return RB_OK;
+}
 
 // ---- split operand format ---------------------------------------------------------------------
 // An fp32 value a is carried as two fp16 numbers: hi = fp16(a) and lo = fp16((a - hi) * 2^11).

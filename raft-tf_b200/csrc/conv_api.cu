@@ -3,38 +3,26 @@
 // model_utils.py:21,39,68,92), on fp32 NHWC tensors.  Same kernels as the fused update block: the input is split to fp16 hi/lo planes, the
 // HWIO kernel is packed K-major, and the selected back end (wgmma or CUDA-core) runs the implicit
 // GEMM.  Used by the parity tests to exercise every filter shape / tile geometry in isolation.
-#include <string.h>
-
-#include <vector>
-
-#include "common.cuh"
+#include "packed.cuh"
 
 namespace rb {
 
-static inline size_t align_up_(size_t v, size_t a) { return (v + a - 1) / a * a; }
-
+// the split input, then the packed conv (a blob of one conv)
 struct ConvWs {
-  __half *in_hi, *in_lo, *w_hi, *w_lo;
-  float* bias;
-  int cin_pad, cout_pad;
-  size_t total;
+  SplitPtr in;
+  PackedConv wt;  // offsets inside `blob`
+  char* blob;
+  size_t blob_bytes, total;
 };
 
 static ConvWs conv_ws_layout(int B, int h, int w, int cin, int cout, int kh, int kw, void* base) {
   ConvWs W;
-  char* b = reinterpret_cast<char*>(base);
-  W.cin_pad = (cin + 63) / 64 * 64;
-  W.cout_pad = (cout + 15) / 16 * 16;
-  size_t off = 0;
-  auto take = [&](size_t bytes) { char* p = b + off; off += align_up_(bytes, 1024); return p; };
-  size_t act = (size_t)B * h * w * W.cin_pad * sizeof(__half);
-  size_t wt = (size_t)W.cout_pad * kh * kw * W.cin_pad * sizeof(__half);
-  W.in_hi = reinterpret_cast<__half*>(take(act));
-  W.in_lo = reinterpret_cast<__half*>(take(act));
-  W.w_hi = reinterpret_cast<__half*>(take(wt));
-  W.w_lo = reinterpret_cast<__half*>(take(wt));
-  W.bias = reinterpret_cast<float*>(take((size_t)W.cout_pad * sizeof(float)));
-  W.total = off;
+  Arena a(base), blob;
+  W.wt = reserve_conv(blob, kh, kw, round_up(cin, 64), cout);
+  W.blob_bytes = blob.size;
+  W.in = a.split((size_t)B * h * w * W.wt.cin_pad);
+  W.blob = a.take<char>(W.blob_bytes);
+  W.total = a.size;
   return W;
 }
 
@@ -80,32 +68,18 @@ extern "C" int rb_conv2d_strided(const float* x, const float* W_host, const floa
   RB_REQUIRE(workspace_bytes >= L.total, RB_ERR_WORKSPACE, "rb_conv2d: workspace has %zu bytes, need %zu", workspace_bytes,
              L.total);
   cudaStream_t s = (cudaStream_t)stream;
-  const int taps = kh * kw;
-  // pack weights on the host: HWIO -> [cout_pad][tap][cin_pad] split planes
-  size_t welems = (size_t)L.cout_pad * taps * L.cin_pad;
-  std::vector<__half> hi(welems, __float2half_rn(0.f)), lo(welems, __float2half_rn(0.f));
-  std::vector<float> bias(L.cout_pad, 0.f);
-  for (int t = 0; t < taps; ++t)
-    for (int ci = 0; ci < cin; ++ci)
-      for (int co = 0; co < cout; ++co) {
-        size_t o = ((size_t)co * taps + t) * L.cin_pad + ci;
-        split_f32(W_host[((size_t)t * cin + ci) * cout + co], hi[o], lo[o]);
-      }
-  if (b_host) memcpy(bias.data(), b_host, (size_t)cout * sizeof(float));
-  RB_CHECK_CUDA(cudaMemcpyAsync(L.w_hi, hi.data(), welems * sizeof(__half), cudaMemcpyHostToDevice, s));
-  RB_CHECK_CUDA(cudaMemcpyAsync(L.w_lo, lo.data(), welems * sizeof(__half), cudaMemcpyHostToDevice, s));
-  RB_CHECK_CUDA(cudaMemcpyAsync(L.bias, bias.data(), (size_t)L.cout_pad * sizeof(float), cudaMemcpyHostToDevice, s));
-  RB_CHECK_CUDA(cudaStreamSynchronize(s));
+  const PackedConv& wt = L.wt;
+  int rc = upload_packed(L.blob, L.blob_bytes, s, [&](void* host) {
+    pack_hwio(wt, host, W_host, cin, cout);
+    for (int co = 0; b_host && co < cout; ++co) put_bias(wt, host, co, b_host[co]);
+    return RB_OK;
+  });
+  if (rc) return rc;
   size_t npix = (size_t)B * h * w;
-  size_t n = npix * L.cin_pad;
-  split_pad_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(x, L.in_hi, L.in_lo, npix, cin, L.cin_pad);
+  size_t n = npix * wt.cin_pad;
+  split_pad_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(x, L.in.hi, L.in.lo, npix, cin, wt.cin_pad);
   RB_CHECK_LAUNCH("split_pad_kernel");
-  ConvParams p;
-  memset(&p, 0, sizeof(p));
-  p.in_hi = L.in_hi; p.in_lo = L.in_lo; p.in_stride = L.cin_pad; p.in_choff = 0; p.cin_pad = L.cin_pad;
-  p.w_hi = L.w_hi; p.w_lo = L.w_lo; p.bias = L.bias;
-  p.cout = cout; p.cout_pad = L.cout_pad; p.kh = kh; p.kw = kw;
-  p.B = B; p.h = h; p.w = w;
+  ConvParams p = conv_params(conv_weights(wt, L.blob), L.in, wt.cin_pad, 0, B, h, w);
   if (stride != 1) {  // strided input view (ConvParams, common.cuh): y is [B, ceil(h/s), ceil(w/s), cout]
     int pt, pl, oh, ow;
     conv_pad_before(h, kh, stride, semantics(), &pt, &oh);
@@ -114,6 +88,6 @@ extern "C" int rb_conv2d_strided(const float* x, const float* W_host, const floa
     p.sx = p.sy = stride;
     p.pad_explicit = 1; p.pad_x = pl; p.pad_y = pt;
   }
-  p.epi = EPI_F32; p.act = relu ? ACT_RELU : ACT_NONE; p.scale = 1.f; p.f0 = y;
+  p.epi = EPI_F32; p.act = relu ? ACT_RELU : ACT_NONE; p.f0 = y;
   return launch_conv(p, s);
 }

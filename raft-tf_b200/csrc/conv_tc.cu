@@ -514,14 +514,8 @@ static int choose_block_n(int cout, long m_tiles, int ctas) {  // ctas: persiste
 template <int BLOCK_N, bool SINGLE>
 static int launch_cfg(const ConvParams& p_in, TileGeom g, const CUtensorMap* maps, cudaStream_t s) {
   using Cfg = TcCfg<BLOCK_N, SINGLE>;
-  static PerDeviceOnce attr_set;
-  int dev = 0, rc_dev;
-  if ((rc_dev = current_device(&dev))) return rc_dev;
-  if (!attr_set.test(dev)) {
-    RB_CHECK_CUDA(cudaFuncSetAttribute(conv_tc_kernel<BLOCK_N, false, SINGLE>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
-    RB_CHECK_CUDA(cudaFuncSetAttribute(conv_tc_kernel<BLOCK_N, true, SINGLE>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
-    attr_set.set(dev);
-  }
+  int dev = 0, rc;
+  if ((rc = current_device(&dev))) return rc;
   const int num_sms = device_sm_count(dev);
   ConvParams p = p_in;
   g.n_tiles = (p.cout + BLOCK_N - 1) / BLOCK_N;
@@ -535,34 +529,25 @@ static int launch_cfg(const ConvParams& p_in, TileGeom g, const CUtensorMap* map
   const int max_ctas = g_override.max_ctas;  // test hook: a capped grid walks more tiles per CTA (no CTA pairs then)
   p.split_cluster = (p.split_k && 2 * g.total_tiles <= num_sms && p.cta_limit <= 0 && max_ctas <= 0) ? 1 : 0;
   const bool cluster2 = p.split_cluster;
-  cudaLaunchConfig_t cfg;
-  memset(&cfg, 0, sizeof(cfg));
   int units = cluster2 ? num_sms / 2 : num_sms;  // persistent: at most one CTA (pair) per SM (pair)
   if (!cluster2 && p.cta_limit > 0 && p.cta_limit < units) units = p.cta_limit;  // leave SMs to a concurrent conv (update.cu)
   if (max_ctas > 0 && max_ctas < units) units = max_ctas;
-  cfg.gridDim = dim3((g.total_tiles < units ? g.total_tiles : units) * (cluster2 ? 2 : 1));
-  cfg.blockDim = dim3(kTcThreads);
-  cfg.dynamicSmemBytes = Cfg::kSmemBytes;
-  cfg.stream = s;
-  cudaLaunchAttribute attr[2];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = cluster2 ? 2 : 1;
-  attr[0].val.clusterDim.y = 1;
-  attr[0].val.clusterDim.z = 1;
-  attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[1].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr;
-  // Programmatic dependent launch (RAFT_B200_NO_PDL=1 turns it off): the dependent conv's prologue and its first
-  // weight tiles overlap the tail of this one.
-  static const int pdl = getenv("RAFT_B200_NO_PDL") ? 0 : 1;
-  cfg.numAttrs = 1 + pdl;
+  const dim3 grid((g.total_tiles < units ? g.total_tiles : units) * (cluster2 ? 2 : 1));
   const int stages = ring_stages(Cfg::kStages);
+  // Programmatic dependent launch: the dependent conv's prologue and its first weight tiles overlap the tail of this one.
+  // Both EXTRAS instantiations get their shared-memory limit at the first launch of either.
+  constexpr auto plain = conv_tc_kernel<BLOCK_N, false, SINGLE>;
+  constexpr auto extras = conv_tc_kernel<BLOCK_N, true, SINGLE>;
+  const int cluster = cluster2 ? 2 : 1;
   if (p.dbg || p.stat_part)
-    RB_CHECK_CUDA(cudaLaunchKernelEx(&cfg, conv_tc_kernel<BLOCK_N, true, SINGLE>, maps[0], maps[1], maps[2], maps[3], p, g, stages));
+    rc = launch_pdl<extras, plain>(grid, dim3(kTcThreads), Cfg::kSmemBytes, cluster, s, maps[0], maps[1], maps[2], maps[3], p, g,
+                                   stages);
   else
-    RB_CHECK_CUDA(cudaLaunchKernelEx(&cfg, conv_tc_kernel<BLOCK_N, false, SINGLE>, maps[0], maps[1], maps[2], maps[3], p, g, stages));
+    rc = launch_pdl<plain, extras>(grid, dim3(kTcThreads), Cfg::kSmemBytes, cluster, s, maps[0], maps[1], maps[2], maps[3], p, g,
+                                   stages);
+  if (rc) return rc;
   RB_CHECK_LAUNCH("conv_tc_kernel");
-  g_record.block_n = BLOCK_N; g_record.bw_log2 = g.bw_log2; g_record.grid = (int)cfg.gridDim.x; g_record.stages = stages;
+  g_record.block_n = BLOCK_N; g_record.bw_log2 = g.bw_log2; g_record.grid = (int)grid.x; g_record.stages = stages;
   g_record.total_tiles = g.total_tiles; g_record.launched = 1; g_record.passes = SINGLE ? 1 : 3;
   if (p.stat_part) ++g_record.fused_stats;
   return RB_OK;

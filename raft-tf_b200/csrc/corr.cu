@@ -656,34 +656,16 @@ int pyramid_view(const float* pyramid, int B, int h, int w, PyramidView* pv) {
   return RB_OK;
 }
 
+// Programmatic dependent launch (as the convs, conv_tc.cu): inside the iteration loop the lookup follows the flow-head conv
+// and precedes convc1; its blocks are scheduled while the predecessor drains and wait in griddepcontrol.wait before they
+// read the coordinates.
 template <int R, bool SPLIT, bool UP>
 static int launch_lookup_cfg(const PyramidView& pv, const PyramidMaps& maps, const float2* c2, float* out_f32, __half* out_hi,
                              __half* out_lo, int out_stride, int npix, cudaStream_t s) {
-  static PerDeviceOnce attr_set;
-  const size_t smem = (size_t)LookupSmem<R, UP>::kBytes;
-  int dev = 0, rc_dev;
-  if ((rc_dev = current_device(&dev))) return rc_dev;
-  if (!attr_set.test(dev)) {
-    RB_CHECK_CUDA(cudaFuncSetAttribute(corr_lookup_kernel<R, SPLIT, UP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    attr_set.set(dev);
-  }
   dim3 grid((npix + kLookupPB - 1) / kLookupPB), block(kLookupPB * 4 * (2 * R + 1));
-  // Programmatic dependent launch (as the convs, conv_tc.cu): inside the iteration loop the lookup follows the flow-head
-  // conv and precedes convc1; its blocks are scheduled while the predecessor drains and wait in griddepcontrol.wait
-  // before they read the coordinates.
-  static const int pdl = getenv("RAFT_B200_NO_PDL") ? 0 : 1;
-  cudaLaunchConfig_t cfg;
-  memset(&cfg, 0, sizeof(cfg));
-  cfg.gridDim = grid;
-  cfg.blockDim = block;
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = s;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = pdl;
-  RB_CHECK_CUDA(cudaLaunchKernelEx(&cfg, corr_lookup_kernel<R, SPLIT, UP>, pv, maps, c2, out_f32, out_hi, out_lo, out_stride, npix));
+  int rc = launch_pdl<corr_lookup_kernel<R, SPLIT, UP>>(grid, block, LookupSmem<R, UP>::kBytes, 0, s, pv, maps, c2, out_f32,
+                                                          out_hi, out_lo, out_stride, npix);
+  if (rc) return rc;
   RB_CHECK_LAUNCH("corr_lookup_kernel");
   return RB_OK;
 }
@@ -692,26 +674,9 @@ template <int R, bool SPLIT, bool UP>
 static int launch_lookup_v5(const PyramidView& pv, const float2* c2, float* out_f32, __half* out_hi, __half* out_lo,
                             int out_stride, int npix, cudaStream_t s, const OtfView& otf) {
   using L = LookupV5<R>;
-  static PerDeviceOnce attr_set;
-  int dev = 0, rc_dev;
-  if ((rc_dev = current_device(&dev))) return rc_dev;
-  if (!attr_set.test(dev)) {
-    RB_CHECK_CUDA(cudaFuncSetAttribute(corr_lookup_v5_kernel<R, SPLIT, UP>, cudaFuncAttributeMaxDynamicSharedMemorySize, L::kBytes));
-    attr_set.set(dev);
-  }
-  static const int pdl = getenv("RAFT_B200_NO_PDL") ? 0 : 1;
-  cudaLaunchConfig_t cfg;
-  memset(&cfg, 0, sizeof(cfg));
-  cfg.gridDim = dim3((npix + L::PB - 1) / L::PB);
-  cfg.blockDim = dim3(L::NT);
-  cfg.dynamicSmemBytes = L::kBytes;
-  cfg.stream = s;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = pdl;
-  RB_CHECK_CUDA(cudaLaunchKernelEx(&cfg, corr_lookup_v5_kernel<R, SPLIT, UP>, pv, c2, out_f32, out_hi, out_lo, out_stride, npix, otf));
+  int rc = launch_pdl<corr_lookup_v5_kernel<R, SPLIT, UP>>(dim3((npix + L::PB - 1) / L::PB), dim3(L::NT), L::kBytes, 0, s, pv,
+                                                             c2, out_f32, out_hi, out_lo, out_stride, npix, otf);
+  if (rc) return rc;
   RB_CHECK_LAUNCH("corr_lookup_v5_kernel");
   return RB_OK;
 }

@@ -24,12 +24,9 @@
 
 #include <vector>
 
-#include "common.cuh"
+#include "packed.cuh"
 
 namespace rb {
-
-static inline size_t al(size_t v, size_t a = 1024) { return (v + a - 1) / a * a; }
-static inline int pad64(int c) { return (c + 63) / 64 * 64; }
 
 enum { NORM_NONE = 0, NORM_INSTANCE = 1, NORM_BATCH = 2 };
 
@@ -76,31 +73,17 @@ static inline EncDesc enc_desc(int small) {
                : EncDesc{kBasicConvs, (int)(sizeof(kBasicConvs) / sizeof(EncConv))};
 }
 
-// packed form of one conv: [cout_pad][kh*kw][cin_pad]; the stem as [cout_pad][4 cell rows][4 cells x 16]
-struct EncPacked {
-  int kh, kw, cin_pad, cout, cout_pad;
-  size_t hi, lo, bias;
-};
-static void enc_packed_layout(int small, int out_dim, std::vector<EncPacked>& P, size_t* total) {
+// packed convs in execution order; the stem as a 4x1 conv over the space-to-depth view: [cout_pad][4 cell rows][4 cells x 16]
+static size_t enc_packed_layout(int small, int out_dim, std::vector<PackedConv>& P) {
   EncDesc d = enc_desc(small);
   P.resize(d.n);
-  size_t off = 0;
+  Arena blob;
   for (int i = 0; i < d.n; ++i) {
     const EncConv& c = d.convs[i];
-    EncPacked& p = P[i];
     const int cout = c.cout < 0 ? out_dim : c.cout;
-    const bool stem = c.k == 7;  // 4x1 conv over the space-to-depth view
-    p.kh = stem ? 4 : c.k;
-    p.kw = stem ? 1 : c.k;
-    p.cin_pad = stem ? 64 : pad64(c.cin);
-    p.cout = cout;
-    p.cout_pad = (cout + 15) / 16 * 16;
-    size_t plane = (size_t)p.cout_pad * p.kh * p.kw * p.cin_pad * sizeof(__half);
-    p.hi = off; off = al(off + plane, 256);
-    p.lo = off; off = al(off + plane, 256);
-    p.bias = off; off = al(off + (size_t)p.cout_pad * sizeof(float), 256);
+    P[i] = c.k == 7 ? reserve_conv(blob, 4, 1, 64, cout) : reserve_conv(blob, c.k, c.k, round_up(c.cin, 64), cout);
   }
-  *total = off;
+  return blob.size;
 }
 
 // ---- kernels ----------------------------------------------------------------------------------------
@@ -225,35 +208,26 @@ constexpr int kStrips = 256;
 
 static EncWs enc_ws_layout(int small, int B, int H, int W, void* base) {
   EncWs w;
-  char* b = reinterpret_cast<char*>(base);
-  size_t off = 0;
+  Arena a(base);
   const size_t px2 = (size_t)B * ((H + 1) / 2) * ((W + 1) / 2);
-  const int c0 = small ? 32 : 64;
-  // the widest activation is at 1/2 resolution (pad64(c0) channels); 1/4 and 1/8 tensors are smaller
-  const size_t act_plane = al(px2 * pad64(small ? 64 : 128) * sizeof(__half) / 1);  // generous: covers px4*128, px8*128
-  for (int i = 0; i < 4; ++i) {
-    w.act[i].hi = reinterpret_cast<__half*>(b + off); off += act_plane;
-    w.act[i].lo = reinterpret_cast<__half*>(b + off); off += act_plane;
-  }
+  // the widest activation is at 1/2 resolution; 1/4 and 1/8 tensors are smaller
+  for (int i = 0; i < 4; ++i) w.act[i] = a.split(px2 * (small ? 64 : 128));  // generous: covers px4*128, px8*128
   // stem input cells: (Ho+3) x (Wo+3) x 16
-  const size_t col_plane = al((size_t)B * ((H + 1) / 2 + 3) * ((W + 1) / 2 + 3) * 16 * sizeof(__half));
-  w.col.hi = reinterpret_cast<__half*>(b + off); off += col_plane;
-  w.col.lo = reinterpret_cast<__half*>(b + off); off += col_plane;
-  w.f32 = reinterpret_cast<float*>(b + off); off += al(px2 * (size_t)(small ? 64 : 128) * sizeof(float));
+  w.col = a.split((size_t)B * ((H + 1) / 2 + 3) * ((W + 1) / 2 + 3) * 16);
+  w.f32 = a.take<float>(px2 * (size_t)(small ? 64 : 128));
   // strips: kStrips for the stand-alone statistics pass, 4 per pixel tile when the conv epilogue produces them
   const size_t fused_cap = (size_t)4 * conv_tc_tiles_per_image((H + 1) / 2, (W + 1) / 2) * 128;
   w.part_cap = fused_cap > (size_t)kStrips * 256 ? fused_cap : (size_t)kStrips * 256;
-  w.part = reinterpret_cast<double*>(b + off); off += al((size_t)B * w.part_cap * 2 * sizeof(double));
-  w.stat = reinterpret_cast<float2*>(b + off); off += al((size_t)B * 256 * sizeof(float2));
-  (void)c0;
-  w.total = off;
+  w.part = a.take<double>((size_t)B * w.part_cap * 2);
+  w.stat = a.take<float2>((size_t)B * 256);
+  w.total = a.size;
   return w;
 }
 
 struct EncRun {
   int small, norm, B, sem;  // sem: RB_SEMANTICS_* (conv_pad_before)
   const char* blob;
-  const std::vector<EncPacked>* P;
+  const std::vector<PackedConv>* P;
   EncWs ws;
   cudaStream_t s;
 };
@@ -262,11 +236,9 @@ struct EncRun {
 static int enc_conv(const EncRun& R, int i, const float* img, SplitPtr in, int in_stride, int h, int w, int relu,
                     SplitPtr res, int res_stride, SplitPtr dst, int dst_stride, float* f32_out, int* oh_, int* ow_) {
   const EncConv& c = enc_desc(R.small).convs[i];
-  const EncPacked& pk = (*R.P)[i];
+  const PackedConv& pk = (*R.P)[i];
   int oh = h, ow = w;
-  ConvParams p;
-  memset(&p, 0, sizeof(p));
-  p.in_hi = in.hi; p.in_lo = in.lo; p.in_stride = in_stride; p.in_choff = 0; p.cin_pad = pk.cin_pad;
+  ConvParams p = conv_params(conv_weights(pk, R.blob), in, in_stride, 0, R.B, h, w);
   if (c.k == 7) {  // stem: 4x1 conv over the space-to-depth view of the image
     int pt, pl;
     conv_pad_before(h, c.k, c.stride, R.sem, &pt, &oh);
@@ -289,12 +261,7 @@ static int enc_conv(const EncRun& R, int i, const float* img, SplitPtr in, int i
     p.sx = p.sy = c.stride;
     p.pad_explicit = 1; p.pad_x = pl; p.pad_y = pt;
   }
-  p.w_hi = reinterpret_cast<const __half*>(R.blob + pk.hi);
-  p.w_lo = reinterpret_cast<const __half*>(R.blob + pk.lo);
-  p.bias = reinterpret_cast<const float*>(R.blob + pk.bias);
-  p.cout = pk.cout; p.cout_pad = pk.cout_pad; p.kh = pk.kh; p.kw = pk.kw;
-  p.B = R.B; p.h = oh; p.w = ow;
-  p.scale = 1.f;
+  p.h = oh; p.w = ow;
   const bool has_norm = c.norm[0] != 0;
   const bool inorm = has_norm && R.norm == NORM_INSTANCE;
   int rc;
@@ -343,43 +310,43 @@ static int enc_forward(const EncRun& R, const float* image, float* out, int H, i
   const EncConv* C = enc_desc(R.small).convs;
   // stem: conv1 7x7 s2 + norm + relu  (model_utils.py:68-70 / 92-94)
   int c_cur = C[0].cout;
-  if ((rc = enc_conv(R, ci++, image, none, 0, H, W, 1, none, 0, A[0], pad64(c_cur), nullptr, &h, &w))) return rc;
+  if ((rc = enc_conv(R, ci++, image, none, 0, H, W, 1, none, 0, A[0], round_up(c_cur, 64), nullptr, &h, &w))) return rc;
   int cur = 0;  // index of the buffer holding the block input
   for (int layer = 0; layer < 3; ++layer) {
     for (int blk = 0; blk < 2; ++blk) {
       const int stride = (blk == 0 && layer > 0) ? 2 : 1;
       const int t1 = (cur + 1) & 3, t2 = (cur + 2) & 3, t3 = (cur + 3) & 3;
-      const int cin = c_cur;
+      const int s_in = round_up(c_cur, 64);  // activations: channels padded to 64
       int oh, ow;
       if (!R.small) {  // ResidualBlock (model_utils.py:19-35)
-        const int cout = C[ci].cout;
-        if ((rc = enc_conv(R, ci, nullptr, A[cur], pad64(cin), h, w, 1, none, 0, A[t1], pad64(cout), nullptr, &oh, &ow))) return rc;
+        const int cout = C[ci].cout, s_out = round_up(cout, 64);
+        if ((rc = enc_conv(R, ci, nullptr, A[cur], s_in, h, w, 1, none, 0, A[t1], s_out, nullptr, &oh, &ow))) return rc;
         SplitPtr res = A[cur];
-        int res_stride = pad64(cin);
+        int res_stride = s_in;
         if (stride != 1) {  // downsample.0 + downsample.1 (no ReLU) on the block input
           int dh, dw;
-          if ((rc = enc_conv(R, ci + 2, nullptr, A[cur], pad64(cin), h, w, 0, none, 0, A[t3], pad64(cout), nullptr, &dh, &dw))) return rc;
+          if ((rc = enc_conv(R, ci + 2, nullptr, A[cur], s_in, h, w, 0, none, 0, A[t3], s_out, nullptr, &dh, &dw))) return rc;
           res = A[t3];
-          res_stride = pad64(cout);
+          res_stride = s_out;
         }
-        if ((rc = enc_conv(R, ci + 1, nullptr, A[t1], pad64(cout), oh, ow, 1, res, res_stride, A[t2], pad64(cout), nullptr, &oh, &ow)))
+        if ((rc = enc_conv(R, ci + 1, nullptr, A[t1], s_out, oh, ow, 1, res, res_stride, A[t2], s_out, nullptr, &oh, &ow)))
           return rc;
         ci += (stride != 1) ? 3 : 2;
         cur = t2; c_cur = cout; h = oh; w = ow;
       } else {  // BottleneckBlock (model_utils.py:37-57)
-        const int cmid = C[ci].cout, cout = C[ci + 2].cout;
-        if ((rc = enc_conv(R, ci, nullptr, A[cur], pad64(cin), h, w, 1, none, 0, A[t1], pad64(cmid), nullptr, &oh, &ow))) return rc;
-        if ((rc = enc_conv(R, ci + 1, nullptr, A[t1], pad64(cmid), h, w, 1, none, 0, A[t2], pad64(cmid), nullptr, &oh, &ow))) return rc;
+        const int cmid = C[ci].cout, cout = C[ci + 2].cout, s_mid = round_up(cmid, 64), s_out = round_up(cout, 64);
+        if ((rc = enc_conv(R, ci, nullptr, A[cur], s_in, h, w, 1, none, 0, A[t1], s_mid, nullptr, &oh, &ow))) return rc;
+        if ((rc = enc_conv(R, ci + 1, nullptr, A[t1], s_mid, h, w, 1, none, 0, A[t2], s_mid, nullptr, &oh, &ow))) return rc;
         SplitPtr res = A[cur];
-        int res_stride = pad64(cin);
+        int res_stride = s_in;
         if (stride != 1) {
           int dh, dw;
-          if ((rc = enc_conv(R, ci + 3, nullptr, A[cur], pad64(cin), h, w, 0, none, 0, A[t3], pad64(cout), nullptr, &dh, &dw))) return rc;
+          if ((rc = enc_conv(R, ci + 3, nullptr, A[cur], s_in, h, w, 0, none, 0, A[t3], s_out, nullptr, &dh, &dw))) return rc;
           res = A[t3];
-          res_stride = pad64(cout);
+          res_stride = s_out;
         }
         // conv3 reads t2 and writes t1 (free again) with the residual fused
-        if ((rc = enc_conv(R, ci + 2, nullptr, A[t2], pad64(cmid), oh, ow, 1, res, res_stride, A[t1], pad64(cout), nullptr, &oh, &ow)))
+        if ((rc = enc_conv(R, ci + 2, nullptr, A[t2], s_mid, oh, ow, 1, res, res_stride, A[t1], s_out, nullptr, &oh, &ow)))
           return rc;
         ci += (stride != 1) ? 4 : 3;
         cur = t1; c_cur = cout; h = oh; w = ow;
@@ -388,7 +355,7 @@ static int enc_forward(const EncRun& R, const float* image, float* out, int H, i
   }
   // conv2: 1x1 to out_dim, no norm / activation (model_utils.py:76 / 100)
   int oh, ow;
-  return enc_conv(R, ci, nullptr, A[cur], pad64(c_cur), h, w, 0, none, 0, none, 0, out, &oh, &ow);
+  return enc_conv(R, ci, nullptr, A[cur], round_up(c_cur, 64), h, w, 0, none, 0, none, 0, out, &oh, &ow);
 }
 
 }  // namespace rb
@@ -415,17 +382,16 @@ extern "C" int rb_encoder_conv_shape(int small, int i, int out_dim, int* k, int*
 }
 extern "C" int rb_encoder_weights_bytes(int small, int out_dim, size_t* bytes) {
   RB_REQUIRE(bytes && out_dim > 0, RB_ERR_BAD_ARG, "rb_encoder_weights_bytes: bad argument");
-  std::vector<EncPacked> P;
-  enc_packed_layout(small, out_dim, P, bytes);
+  std::vector<PackedConv> P;
+  *bytes = enc_packed_layout(small, out_dim, P);
   return RB_OK;
 }
 
 // Layout of conv i inside the packed blob (byte offsets of the hi / lo / bias planes and the packed geometry).
 extern "C" int rb_encoder_packed_conv(int small, int out_dim, int i, size_t* hi_off, size_t* lo_off, size_t* bias_off, int* kh,
                                       int* kw, int* cin_pad, int* cout_pad) {
-  std::vector<EncPacked> P;
-  size_t total;
-  enc_packed_layout(small, out_dim, P, &total);
+  std::vector<PackedConv> P;
+  enc_packed_layout(small, out_dim, P);
   RB_REQUIRE(i >= 0 && i < (int)P.size() && out_dim > 0, RB_ERR_BAD_ARG, "rb_encoder_packed_conv: index %d out of range", i);
   if (hi_off) *hi_off = P[i].hi;
   if (lo_off) *lo_off = P[i].lo;
@@ -444,46 +410,36 @@ extern "C" int rb_encoder_weights_pack_host(int small, int norm, int out_dim, co
                                             size_t blob_bytes) {
   RB_REQUIRE(W_host && b_host && host_blob, RB_ERR_BAD_ARG, "rb_encoder_weights_pack: null pointer");
   RB_REQUIRE(norm >= 0 && norm <= 2, RB_ERR_BAD_ARG, "rb_encoder_weights_pack: norm %d", norm);
-  std::vector<EncPacked> P;
-  size_t total;
-  enc_packed_layout(small, out_dim, P, &total);
+  std::vector<PackedConv> P;
+  const size_t total = enc_packed_layout(small, out_dim, P);
   RB_REQUIRE(blob_bytes >= total, RB_ERR_WORKSPACE, "rb_encoder_weights_pack: blob has %zu bytes, need %zu", blob_bytes, total);
   EncDesc d = enc_desc(small);
-  struct HostBlob {  // same interface as the std::vector<char> the loop below was written for
-    char* p;
-    char* data() { return p; }
-  } host{reinterpret_cast<char*>(host_blob)};
   memset(host_blob, 0, total);
   for (int i = 0; i < d.n; ++i) {
     const EncConv& c = d.convs[i];
-    const EncPacked& p = P[i];
+    const PackedConv& p = P[i];
     RB_REQUIRE(W_host[i] && b_host[i], RB_ERR_BAD_ARG, "rb_encoder_weights_pack: missing weights for %s", c.name);
-    __half* hi = reinterpret_cast<__half*>(host.data() + p.hi);
-    __half* lo = reinterpret_cast<__half*>(host.data() + p.lo);
-    float* bias = reinterpret_cast<float*>(host.data() + p.bias);
-    const int cout = p.cout, taps_ref = c.k * c.k;
-    const bool stem = c.k == 7;
+    const int cout = p.cout;
     const bool fold = norm == NORM_BATCH && c.norm[0] != 0;
     RB_REQUIRE(!fold || (bn_host && bn_host[i]), RB_ERR_BAD_ARG, "rb_encoder_weights_pack: missing BN statistics for %s", c.norm);
-    for (int co = 0; co < cout; ++co) {
-      double scale = 1.0, shift = 0.0;
-      if (fold) {  // y = (conv + b - mean) / sqrt(var + eps) * gamma + beta
-        const float* bn = bn_host[i];
-        scale = (double)bn[co] / sqrt((double)bn[3 * cout + co] + 1e-5);
-        shift = (double)bn[cout + co] - (double)bn[2 * cout + co] * scale;
-      }
-      for (int t = 0; t < taps_ref; ++t)
-        for (int ci = 0; ci < c.cin; ++ci) {
-          const float val = (float)(W_host[i][((size_t)t * c.cin + ci) * cout + co] * scale);
-          size_t o = ((size_t)co * taps_ref + t) * p.cin_pad + ci;
-          if (stem) {  // tap (ky, kx) = cell (ky/2, kx/2), sub-pixel (ky%2, kx%2): [co][cell row][cell x 16 + sub*3 + ci]
-            const int ky = t / c.k, kx = t % c.k;
-            o = ((size_t)co * 4 + ky / 2) * 64 + (kx / 2) * 16 + ((ky & 1) * 2 + (kx & 1)) * 3 + ci;
-          }
-          split_f32(val, hi[o], lo[o]);
-        }
-      bias[co] = (float)(b_host[i][co] * scale + shift);
+    std::vector<double> scale(cout, 1.0), shift(cout, 0.0);
+    for (int co = 0; fold && co < cout; ++co) {  // y = (conv + b - mean) / sqrt(var + eps) * gamma + beta
+      const float* bn = bn_host[i];
+      scale[co] = (double)bn[co] / sqrt((double)bn[3 * cout + co] + 1e-5);
+      shift[co] = (double)bn[cout + co] - (double)bn[2 * cout + co] * scale[co];
     }
+    if (c.k == 7) {  // stem: tap (ky, kx) = cell (ky/2, kx/2), sub-pixel (ky%2, kx%2) -> row ky/2, k = cell x 16 + sub*3 + ci
+      for (int t = 0; t < c.k * c.k; ++t)
+        for (int ci = 0; ci < c.cin; ++ci)
+          for (int co = 0; co < cout; ++co) {
+            const int ky = t / c.k, kx = t % c.k;
+            put_weight(p, host_blob, co, ky / 2, (kx / 2) * 16 + ((ky & 1) * 2 + (kx & 1)) * 3 + ci,
+                       (float)(W_host[i][((size_t)t * c.cin + ci) * cout + co] * scale[co]));
+          }
+    } else {
+      pack_hwio(p, host_blob, W_host[i], c.cin, cout, 0, scale.data());
+    }
+    for (int co = 0; co < cout; ++co) put_bias(p, host_blob, co, (float)(b_host[i][co] * scale[co] + shift[co]));
   }
   return RB_OK;
 }
@@ -496,12 +452,9 @@ extern "C" int rb_encoder_weights_pack(int small, int norm, int out_dim, const f
   int rc = rb_encoder_weights_bytes(small, out_dim, &total);
   if (rc) return rc;
   RB_REQUIRE(blob_bytes >= total, RB_ERR_WORKSPACE, "rb_encoder_weights_pack: blob has %zu bytes, need %zu", blob_bytes, total);
-  std::vector<char> host(total, 0);
-  if ((rc = rb_encoder_weights_pack_host(small, norm, out_dim, W_host, b_host, bn_host, host.data(), total))) return rc;
-  cudaStream_t s = (cudaStream_t)stream;
-  RB_CHECK_CUDA(cudaMemcpyAsync(blob, host.data(), total, cudaMemcpyHostToDevice, s));
-  RB_CHECK_CUDA(cudaStreamSynchronize(s));
-  return RB_OK;
+  return upload_packed(blob, total, (cudaStream_t)stream, [&](void* host) {
+    return rb_encoder_weights_pack_host(small, norm, out_dim, W_host, b_host, bn_host, host, total);
+  });
 }
 
 extern "C" int rb_encoder_workspace_bytes(int small, int B, int H, int W, size_t* bytes) {
@@ -518,9 +471,8 @@ extern "C" int rb_encoder_forward(int small, int norm, const void* weights, cons
   EncRun R;
   R.small = small; R.norm = norm; R.B = B; R.sem = semantics();
   R.blob = reinterpret_cast<const char*>(weights);
-  std::vector<EncPacked> P;
-  size_t total;
-  enc_packed_layout(small, out_dim, P, &total);
+  std::vector<PackedConv> P;
+  enc_packed_layout(small, out_dim, P);
   R.P = &P;
   R.ws = enc_ws_layout(small, B, H, W, workspace);
   RB_REQUIRE(workspace_bytes >= R.ws.total, RB_ERR_WORKSPACE, "rb_encoder_forward: workspace has %zu bytes, need %zu",

@@ -13,36 +13,26 @@
 #include <math.h>
 #include <string.h>
 
-#include "common.cuh"
+#include "packed.cuh"
 
 namespace rb {
 
-static inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
-
 struct CorrWs {
-  __half* f1_hi;
-  __half* f1_lo;
-  __half* f2_hi[RB_NUM_LEVELS];
-  __half* f2_lo[RB_NUM_LEVELS];
+  SplitPtr f1;
+  SplitPtr f2[RB_NUM_LEVELS];
   size_t total;
 };
 
+// rows of pyramid level l, padded to a multiple of 16 so the "weight" operand has a legal cout_pad
+static int level_rows(int h, int w, int l) { return level_dim(h, l) * level_dim(w, l); }
+static int level_rows_pad(int h, int w, int l) { return round_up(level_rows(h, w, l), 16); }
+
 static CorrWs corr_ws_layout(int B, int h, int w, int C, void* base) {
   CorrWs W;
-  char* b = reinterpret_cast<char*>(base);
-  size_t off = 0;
-  auto take = [&](size_t bytes) { char* p = b + off; off += align_up(bytes, 1024); return p; };
-  size_t n0 = (size_t)B * h * w * C;
-  W.f1_hi = reinterpret_cast<__half*>(take(n0 * 2));
-  W.f1_lo = reinterpret_cast<__half*>(take(n0 * 2));
-  for (int l = 0; l < RB_NUM_LEVELS; ++l) {
-    // rows padded to a multiple of 16 so the packed "weight" operand has a legal cout_pad
-    size_t rows = (size_t)((level_dim(h, l) * level_dim(w, l) + 15) / 16 * 16);
-    size_t nl = (size_t)B * rows * C;
-    W.f2_hi[l] = reinterpret_cast<__half*>(take(nl * 2));
-    W.f2_lo[l] = reinterpret_cast<__half*>(take(nl * 2));
-  }
-  W.total = off;
+  Arena a(base);
+  W.f1 = a.split((size_t)B * h * w * C);
+  for (int l = 0; l < RB_NUM_LEVELS; ++l) W.f2[l] = a.split((size_t)B * level_rows_pad(h, w, l) * C);
+  W.total = a.size;
   return W;
 }
 
@@ -115,12 +105,11 @@ int corr_build_tc(const float* fmap1, const float* fmap2, float* pyramid, int B,
     CorrPrep P;
     memset(&P, 0, sizeof(P));
     P.f1 = fmap1; P.f2 = fmap2; P.B = B; P.h = h; P.w = w; P.C = C;
-    P.hi[0] = W.f1_hi; P.lo[0] = W.f1_lo; P.rows[0] = N; P.rows_pad[0] = N; P.wl[0] = w;
+    P.hi[0] = W.f1.hi; P.lo[0] = W.f1.lo; P.rows[0] = N; P.rows_pad[0] = N; P.wl[0] = w;
     size_t max_items = (size_t)B * N * (C / 4);
     for (int l = 0; l < RB_NUM_LEVELS; ++l) {
-      const int rows = level_dim(h, l) * level_dim(w, l);
-      P.hi[l + 1] = W.f2_hi[l]; P.lo[l + 1] = W.f2_lo[l];
-      P.rows[l + 1] = rows; P.rows_pad[l + 1] = (rows + 15) / 16 * 16; P.wl[l + 1] = level_dim(w, l);
+      P.hi[l + 1] = W.f2[l].hi; P.lo[l + 1] = W.f2[l].lo;
+      P.rows[l + 1] = level_rows(h, w, l); P.rows_pad[l + 1] = level_rows_pad(h, w, l); P.wl[l + 1] = level_dim(w, l);
       const size_t items = (size_t)B * P.rows_pad[l + 1] * (C / 4);
       if (items > max_items) max_items = items;
     }
@@ -130,13 +119,11 @@ int corr_build_tc(const float* fmap1, const float* fmap2, float* pyramid, int B,
   }
   size_t lvl_off = 0;
   for (int l = 0; l < RB_NUM_LEVELS; ++l) {
-    const int rows = level_dim(h, l) * level_dim(w, l), rows_pad = (rows + 15) / 16 * 16;
-    ConvParams p;
-    memset(&p, 0, sizeof(p));
-    p.in_hi = W.f1_hi; p.in_lo = W.f1_lo; p.in_stride = C; p.in_choff = 0; p.cin_pad = C;
-    p.w_hi = W.f2_hi[l]; p.w_lo = W.f2_lo[l]; p.bias = nullptr;
-    p.cout = rows; p.cout_pad = rows_pad; p.kh = 1; p.kw = 1; p.w_per_batch = 1;
-    p.B = B; p.h = h; p.w = w;
+    const int rows = level_rows(h, w, l);
+    // the (pooled) fmap2 of each batch element as the 1x1 "filter": rows = output channels, C = input channels
+    const ConvWeights f2 = {W.f2[l].hi, W.f2[l].lo, nullptr, 1, 1, C, rows, level_rows_pad(h, w, l)};
+    ConvParams p = conv_params(f2, W.f1, C, 0, B, h, w);
+    p.w_per_batch = 1;
     p.epi = EPI_F32;
     {  // divide after the matmul (:213).  sqrt(256) = 16: the division is an exact scaling, a multiply gives the same bits
       const float sq = sqrtf((float)C);

@@ -18,8 +18,6 @@ namespace {
 
 constexpr size_t kAlign = 256;
 
-inline size_t align_up(size_t n) { return (n + kAlign - 1) / kAlign * kAlign; }
-
 // workspace: per-target counts and segment offsets, keys and values before / after the sort, the scaled flow of every
 // source, the up/down neighbour count of the hole fill, then CUB's temporary storage
 struct ReverseWs {
@@ -29,15 +27,15 @@ struct ReverseWs {
 ReverseWs reverse_layout(size_t n) {
   ReverseWs l;
   size_t o = 0;
-  const size_t u32 = align_up(n * sizeof(uint32_t));
+  const size_t u32 = round_up(n * sizeof(uint32_t), kAlign);
   l.counts = o, o += u32;
   l.offsets = o, o += u32;
   l.keys_in = o, o += u32;
   l.keys_out = o, o += u32;
   l.vals_in = o, o += u32;
   l.vals_out = o, o += u32;
-  l.fs = o, o += align_up(n * sizeof(float2));
-  l.nfound = o, o += align_up(n);
+  l.fs = o, o += round_up(n * sizeof(float2), kAlign);
+  l.nfound = o, o += round_up(n, kAlign);
   l.temp = o;
   l.fixed = o;
   return l;
@@ -57,7 +55,7 @@ cudaError_t cub_temp_bytes(size_t n, size_t* bytes) {
   cudaError_t e = cub::DeviceRadixSort::SortPairs(nullptr, sort_b, ci, o, ci, o, (uint32_t)n, 0, key_bits(n));
   if (e != cudaSuccess) return e;
   e = cub::DeviceScan::ExclusiveSum(nullptr, scan_b, ci, o, (uint32_t)n);
-  *bytes = align_up(sort_b > scan_b ? sort_b : scan_b);
+  *bytes = round_up(sort_b > scan_b ? sort_b : scan_b, kAlign);
   return e;
 }
 

@@ -16,8 +16,7 @@
 #include <stdlib.h>
 #include <string.h>
 
-#include <vector>
-
+#include "packed.cuh"
 #include "tc_common.cuh"
 
 namespace rb {
@@ -56,7 +55,7 @@ static const RefConv kSmallConvs[] = {
 enum PackedId {
   P_CONVC1 = 0, P_CONVC2, P_CONVF2, P_MOTION, P_ZR1, P_Q1, P_ZR2, P_Q2, P_FH1, P_FH2, P_MASK0, P_MASK2, P_COUNT
 };
-struct PackedConv {
+struct PackedSrc {
   int src0, src1;  // reference conv indices (-1 = none)
   int cin_pad;
 };
@@ -65,7 +64,7 @@ struct Variant {
   int small, hidden, ctx, radius, corr_ch, corr_pad, c1, cf, cor, f1, hx, fh, mo_out, nref;
   const RefConv* ref;
   int convf1_ref;
-  PackedConv pk[P_COUNT];
+  PackedSrc pk[P_COUNT];
 };
 
 static const Variant kThings = {
@@ -78,48 +77,30 @@ static const Variant kSmall = {
      {-1, -1, 0}, {7, -1, 128}, {8, -1, 128}, {-1, -1, 0}, {-1, -1, 0}}};
 
 static inline const Variant& variant(int small) { return small ? kSmall : kThings; }
-static inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
-static inline int pad16(int c) { return (c + 15) / 16 * 16; }
 
 // ---- packed weight blob -------------------------------------------------------------------------
 struct PackedLayout {
-  size_t hi[P_COUNT], lo[P_COUNT], bias[P_COUNT];  // byte offsets
-  int cout[P_COUNT], cout_pad[P_COUNT], kh[P_COUNT], kw[P_COUNT];
-  size_t f1_w, f1_b;  // convf1: fp32 [49*2][cout] and bias (CUDA-core kernel)
-  size_t f1t_hi, f1t_lo, f1t_bias;  // convf1 for the tensor-core path: 7x1 conv over the 8-pixel window view, [cout_pad][7][64]
-  int f1t_cout, f1t_cout_pad;
+  PackedConv conv[P_COUNT];  // cout == 0: the variant does not have this conv
+  size_t f1_w, f1_b;         // convf1: fp32 [49*2][cout] and bias (CUDA-core kernel)
+  PackedConv f1t;            // convf1 for the tensor-core path: 7x1 conv over the 8-pixel window view, [cout_pad][7][64]
   size_t total;
 };
 
 static PackedLayout packed_layout(const Variant& v) {
   PackedLayout L;
   memset(&L, 0, sizeof(L));
-  size_t off = 0;
+  Arena blob;
   for (int i = 0; i < P_COUNT; ++i) {
-    const PackedConv& pc = v.pk[i];
+    const PackedSrc& pc = v.pk[i];
     if (pc.src0 < 0) continue;
     const RefConv& r0 = v.ref[pc.src0];
-    int cout = r0.cout + (pc.src1 >= 0 ? v.ref[pc.src1].cout : 0);
-    L.cout[i] = cout;
-    L.cout_pad[i] = pad16(cout);
-    L.kh[i] = r0.kh;
-    L.kw[i] = r0.kw;
-    size_t plane = (size_t)L.cout_pad[i] * r0.kh * r0.kw * pc.cin_pad * sizeof(__half);
-    L.hi[i] = off; off = align_up(off + plane, 256);
-    L.lo[i] = off; off = align_up(off + plane, 256);
-    L.bias[i] = off; off = align_up(off + (size_t)L.cout_pad[i] * sizeof(float), 256);
+    L.conv[i] = reserve_conv(blob, r0.kh, r0.kw, pc.cin_pad, r0.cout + (pc.src1 >= 0 ? v.ref[pc.src1].cout : 0));
   }
   const RefConv& f = v.ref[v.convf1_ref];
-  L.f1_w = off; off = align_up(off + (size_t)f.kh * f.kw * f.cin * f.cout * sizeof(float), 256);
-  L.f1_b = off; off = align_up(off + (size_t)f.cout * sizeof(float), 256);
-  L.f1t_cout = f.cout; L.f1t_cout_pad = pad16(f.cout);
-  {
-    const size_t plane = (size_t)L.f1t_cout_pad * 7 * 64 * sizeof(__half);
-    L.f1t_hi = off; off = align_up(off + plane, 256);
-    L.f1t_lo = off; off = align_up(off + plane, 256);
-    L.f1t_bias = off; off = align_up(off + (size_t)L.f1t_cout_pad * sizeof(float), 256);
-  }
-  L.total = off;
+  L.f1_w = blob.reserve((size_t)f.kh * f.kw * f.cin * f.cout * sizeof(float), 256);
+  L.f1_b = blob.reserve((size_t)f.cout * sizeof(float), 256);
+  L.f1t = reserve_conv(blob, 7, 1, 64, f.cout);
+  L.total = blob.size;
   return L;
 }
 
@@ -135,40 +116,20 @@ struct Workspace {
 
 static Workspace workspace_layout(const Variant& v, size_t npix, void* base) {
   Workspace W;
-  char* b = reinterpret_cast<char*>(base);
-  size_t off = 0;
-  auto split = [&](int C) {
-    SplitPtr sp;
-    size_t plane = align_up(npix * (size_t)C * sizeof(__half), 1024);
-    sp.hi = reinterpret_cast<__half*>(b + off);
-    sp.lo = reinterpret_cast<__half*>(b + off + plane);
-    off += 2 * plane;
-    return sp;
-  };
-  W.corr = split(v.corr_pad);
-  W.c1 = split(v.c1 > 0 ? v.c1 : 64);
-  W.cf = split(v.cf);
-  W.f1 = split(v.f1);
-  W.hx = split(v.hx);
-  W.qx = split(v.hx);
-  W.fh = split(v.fh);
-  {  // (w + 8) <= 2 w for every admissible grid (w >= 8): 2 * npix pixels of 8 channels bound the padded flow image
-    const size_t plane = align_up(2 * npix * 8 * sizeof(__half), 1024);
-    W.fl.hi = reinterpret_cast<__half*>(b + off);
-    W.fl.lo = reinterpret_cast<__half*>(b + off + plane);
-    off += 2 * plane;
-  }
-  size_t fsz = align_up(npix * (size_t)v.hidden * sizeof(float), 1024);
-  W.H = reinterpret_cast<float*>(b + off); off += fsz;
-  W.Z = reinterpret_cast<float*>(b + off); off += fsz;
-  for (int i = 0; i < 4; ++i) {
-    W.pre[i] = nullptr;
-    if (!v.small) {
-      W.pre[i] = reinterpret_cast<float*>(b + off);
-      off += align_up(npix * (size_t)((i & 1) ? v.hidden : 2 * v.hidden) * sizeof(float), 1024);
-    }
-  }
-  W.total = off;
+  Arena a(base);
+  W.corr = a.split(npix * v.corr_pad);
+  W.c1 = a.split(npix * (v.c1 > 0 ? v.c1 : 64));
+  W.cf = a.split(npix * v.cf);
+  W.f1 = a.split(npix * v.f1);
+  W.hx = a.split(npix * v.hx);
+  W.qx = a.split(npix * v.hx);
+  W.fh = a.split(npix * v.fh);
+  // (w + 8) <= 2 w for every admissible grid (w >= 8): 2 * npix pixels of 8 channels bound the padded flow image
+  W.fl = a.split(2 * npix * 8);
+  W.H = a.take<float>(npix * v.hidden);
+  W.Z = a.take<float>(npix * v.hidden);
+  for (int i = 0; i < 4; ++i) W.pre[i] = v.small ? nullptr : a.take<float>(npix * ((i & 1) ? v.hidden : 2 * v.hidden));
+  W.total = a.size;
   return W;
 }
 
@@ -325,19 +286,10 @@ __global__ void flow_prep_kernel(const float2* __restrict__ coords1, SplitPtr fl
 // ---------------------------------------------------------------------------------------------
 // one update-block application
 // ---------------------------------------------------------------------------------------------
-static ConvParams base_params(const Variant& v, const PackedLayout& L, const void* blob, int id, SplitPtr in,
-                              int in_stride, int in_choff, int B, int h, int w) {
-  ConvParams p;
-  memset(&p, 0, sizeof(p));
-  const char* bb = reinterpret_cast<const char*>(blob);
-  p.in_hi = in.hi; p.in_lo = in.lo; p.in_stride = in_stride; p.in_choff = in_choff;
-  p.cin_pad = v.pk[id].cin_pad;
-  p.w_hi = reinterpret_cast<const __half*>(bb + L.hi[id]);
-  p.w_lo = reinterpret_cast<const __half*>(bb + L.lo[id]);
-  p.bias = reinterpret_cast<const float*>(bb + L.bias[id]);
-  p.cout = L.cout[id]; p.cout_pad = L.cout_pad[id]; p.kh = L.kh[id]; p.kw = L.kw[id];
-  p.B = B; p.h = h; p.w = w;
-  p.hidden = v.hidden; p.scale = 1.f;
+static ConvParams base_params(const Variant& v, const PackedConv& c, const void* blob, SplitPtr in, int in_stride, int B, int h,
+                              int w) {
+  ConvParams p = conv_params(conv_weights(c, blob), in, in_stride, 0, B, h, w);
+  p.hidden = v.hidden;
   return p;
 }
 
@@ -425,17 +377,9 @@ static int update_step(const Variant& v, const void* blob, void* wsp, float* coo
       const size_t cells = (size_t)B * h * (w + 8);
       flow_prep_kernel<<<(unsigned)((cells + 255) / 256), 256, 0, ss->stream>>>(c1, W.fl, W.hx, W.qx, v.hx, foff, B, h, w);
       RB_CHECK_LAUNCH("flow_prep_kernel");
-      ConvParams p;
-      memset(&p, 0, sizeof(p));
-      p.in_hi = W.fl.hi; p.in_lo = W.fl.lo;
-      p.in_stride = 8; p.in_cext = 64; p.in_w = w; p.in_h = h; p.in_rowpitch = (w + 8) * 8;
-      p.cin_pad = 64; p.kh = 7; p.kw = 1;
+      ConvParams p = base_params(v, L.f1t, blob, W.fl, 8, B, h, w);
+      p.in_cext = 64; p.in_w = w; p.in_h = h; p.in_rowpitch = (w + 8) * 8;
       p.pad_explicit = 1; p.pad_x = 0; p.pad_y = 3;
-      p.w_hi = reinterpret_cast<const __half*>(bb + L.f1t_hi);
-      p.w_lo = reinterpret_cast<const __half*>(bb + L.f1t_lo);
-      p.bias = reinterpret_cast<const float*>(bb + L.f1t_bias);
-      p.cout = L.f1t_cout; p.cout_pad = L.f1t_cout_pad;
-      p.B = B; p.h = h; p.w = w; p.hidden = v.hidden; p.scale = 1.f;
       set_act(p, ACT_RELU, W.f1, v.f1, 0);
       // batch 1: 28 CTAs = the 55 128-wide tiles in two full rounds, leaving the SMs to the lookup and convc1 / convc2.
       // Re-swept on H100 (132 SMs, 700 W, forward pass at 440x1024, L2 flushed, 3 interleaved runs each): 28/38 13.03 ms,
@@ -451,7 +395,7 @@ static int update_step(const Variant& v, const void* blob, void* wsp, float* coo
 #undef RB_LAUNCH_CONV7
     RB_CHECK_LAUNCH("flow_conv7_kernel");
     {
-      ConvParams p = base_params(v, L, blob, P_CONVF2, W.f1, v.f1, 0, B, h, w);
+      ConvParams p = base_params(v, L.conv[P_CONVF2], blob, W.f1, v.f1, B, h, w);
       set_act(p, ACT_RELU, W.cf, v.cf, v.cor);
       // convf2 runs beside convc1 / convc2 of the main stream: a small CTA budget keeps it off the SMs they need
       // (batch 1: the other convs use 55-110 of the 132 SMs)
@@ -465,20 +409,20 @@ static int update_step(const Variant& v, const void* blob, void* wsp, float* coo
     if ((rc = launch_lookup(pyramid, coords1, nullptr, W.corr.hi, W.corr.lo, v.corr_pad, B, h, w, v.radius, s))) return rc;
   }
   if (!v.small) {
-    ConvParams p = base_params(v, L, blob, P_CONVC1, W.corr, v.corr_pad, 0, B, h, w);
+    ConvParams p = base_params(v, L.conv[P_CONVC1], blob, W.corr, v.corr_pad, B, h, w);
     set_act(p, ACT_RELU, W.c1, v.c1, 0);
     if ((rc = launch_conv_dbg(p, s))) return rc;
-    p = base_params(v, L, blob, P_CONVC2, W.c1, v.c1, 0, B, h, w);
+    p = base_params(v, L.conv[P_CONVC2], blob, W.c1, v.c1, B, h, w);
     set_act(p, ACT_RELU, W.cf, v.cf, 0);
     if ((rc = launch_conv_dbg(p, s))) return rc;
   } else {
-    ConvParams p = base_params(v, L, blob, P_CONVC1, W.corr, v.corr_pad, 0, B, h, w);
+    ConvParams p = base_params(v, L.conv[P_CONVC1], blob, W.corr, v.corr_pad, B, h, w);
     set_act(p, ACT_RELU, W.cf, v.cf, 0);
     if ((rc = launch_conv_dbg(p, s))) return rc;
   }
   RB_CHECK_CUDA(cudaStreamWaitEvent(s, ss->join, 0));
   {
-    ConvParams p = base_params(v, L, blob, P_MOTION, W.cf, v.cf, 0, B, h, w);
+    ConvParams p = base_params(v, L.conv[P_MOTION], blob, W.cf, v.cf, B, h, w);
     set_act(p, ACT_RELU, W.hx, v.hx, xoff);
     p.d1_hi = W.qx.hi; p.d1_lo = W.qx.lo; p.d1_stride = v.hx; p.d1_choff = xoff;
     if (math_mode_tc() && (p.cout & 15) == 14 && p.cout + 2 <= p.cout_pad && foff == xoff + p.cout) {
@@ -493,12 +437,12 @@ static int update_step(const Variant& v, const void* blob, void* wsp, float* coo
   const int passes = v.small ? 1 : 2;
   for (int pass = 0; pass < passes; ++pass) {
     int zr = pass == 0 ? P_ZR1 : P_ZR2, q = pass == 0 ? P_Q1 : P_Q2;
-    ConvParams p = base_params(v, L, blob, zr, W.hx, v.hx, 0, B, h, w);
+    ConvParams p = base_params(v, L.conv[zr], blob, W.hx, v.hx, B, h, w);
     hoist_inp(v, W, pass * 2 + 0, p);
     p.epi = EPI_ZR; p.f0 = W.Z; p.f1 = W.H;
     p.d0_hi = W.qx.hi; p.d0_lo = W.qx.lo; p.d0_stride = v.hx; p.d0_choff = 0;
     if ((rc = launch_conv_dbg(p, s))) return rc;
-    p = base_params(v, L, blob, q, W.qx, v.hx, 0, B, h, w);
+    p = base_params(v, L.conv[q], blob, W.qx, v.hx, B, h, w);
     hoist_inp(v, W, pass * 2 + 1, p);
     p.epi = EPI_Q; p.f0 = W.Z; p.f1 = W.H;
     p.d0_hi = W.hx.hi; p.d0_lo = W.hx.lo; p.d0_stride = v.hx; p.d0_choff = 0;
@@ -509,10 +453,10 @@ static int update_step(const Variant& v, const void* blob, void* wsp, float* coo
   // (18 per-pixel dot products per 16-channel group + a gather kernel, no FH store) was parity-green and slower at batch 1
   // and batch 8 -- removed again.
   {
-    ConvParams p = base_params(v, L, blob, P_FH1, W.hx, v.hx, 0, B, h, w);
+    ConvParams p = base_params(v, L.conv[P_FH1], blob, W.hx, v.hx, B, h, w);
     set_act(p, ACT_RELU, W.fh, v.fh, 0);
     if ((rc = launch_conv_dbg(p, s))) return rc;
-    p = base_params(v, L, blob, P_FH2, W.fh, v.fh, 0, B, h, w);
+    p = base_params(v, L.conv[P_FH2], blob, W.fh, v.fh, B, h, w);
     p.epi = EPI_DELTA; p.f1 = coords1; p.f2 = delta_out;
     // 36 k-iterations on 55 CTAs at batch 1 while 77 SMs idle: two CTAs per pixel tile, half of the channel chunks each
     // (conv_tc.cu, split-K over a cluster when the tiles fit one wave of CTA pairs; the same two-halves sum on one CTA
@@ -523,10 +467,10 @@ static int update_step(const Variant& v, const void* blob, void* wsp, float* coo
   // ---- mask head (model_utils.py:180-183); only the last iteration's mask is ever consumed ----
   if (mask_out) {
     RB_REQUIRE(!v.small, RB_ERR_UNSUPPORTED, "raft-small has no mask head (model_utils.py:194)");
-    ConvParams p = base_params(v, L, blob, P_MASK0, W.hx, v.hx, 0, B, h, w);
+    ConvParams p = base_params(v, L.conv[P_MASK0], blob, W.hx, v.hx, B, h, w);
     set_act(p, ACT_RELU, W.fh, v.fh, 0);
     if ((rc = launch_conv_dbg(p, s))) return rc;
-    p = base_params(v, L, blob, P_MASK2, W.fh, v.fh, 0, B, h, w);
+    p = base_params(v, L.conv[P_MASK2], blob, W.fh, v.fh, B, h, w);
     p.epi = EPI_F32; p.f0 = mask_out; p.scale = 0.25f;
     if ((rc = launch_conv_dbg(p, s))) return rc;
   }
@@ -541,7 +485,7 @@ static int precompute_inp(const Variant& v, const void* blob, void* wsp, int B, 
   const Workspace W = workspace_layout(v, npix, wsp);
   const int ids[4] = {P_ZR1, P_Q1, P_ZR2, P_Q2};
   for (int i = 0; i < 4; ++i) {
-    ConvParams p = base_params(v, L, blob, ids[i], W.hx, v.hx, 0, B, h, w);  // inp lives in HX and QX alike
+    ConvParams p = base_params(v, L.conv[ids[i]], blob, W.hx, v.hx, B, h, w);  // inp lives in HX and QX alike
     p.ck_begin = v.hidden / 64; p.ck_count = v.ctx / 64; p.ck_skip_at = 1 << 20; p.ck_skip = 0;
     p.epi = EPI_F32; p.f0 = W.pre[i]; p.scale = 1.f;
     int rc = launch_conv(p, s);
@@ -597,15 +541,15 @@ extern "C" int rb_update_packed_conv(int small, int id, size_t* hi_off, size_t* 
   const Variant& v = variant(small);
   const PackedLayout L = packed_layout(v);
   RB_REQUIRE((id >= 0 && id < P_COUNT) || id == 100, RB_ERR_BAD_ARG, "rb_update_packed_conv: id %d", id);
-  const bool f1 = id == 100;
-  if (hi_off) *hi_off = f1 ? L.f1t_hi : L.hi[id];
-  if (lo_off) *lo_off = f1 ? L.f1t_lo : L.lo[id];
-  if (bias_off) *bias_off = f1 ? L.f1t_bias : L.bias[id];
-  if (kh) *kh = f1 ? 7 : L.kh[id];
-  if (kw) *kw = f1 ? 1 : L.kw[id];
-  if (cin_pad) *cin_pad = f1 ? 64 : v.pk[id].cin_pad;
-  if (cout) *cout = f1 ? L.f1t_cout : L.cout[id];
-  if (cout_pad) *cout_pad = f1 ? L.f1t_cout_pad : L.cout_pad[id];
+  const PackedConv& c = id == 100 ? L.f1t : L.conv[id];
+  if (hi_off) *hi_off = c.hi;
+  if (lo_off) *lo_off = c.lo;
+  if (bias_off) *bias_off = c.bias;
+  if (kh) *kh = c.kh;
+  if (kw) *kw = c.kw;
+  if (cin_pad) *cin_pad = c.cin_pad;
+  if (cout) *cout = c.cout;
+  if (cout_pad) *cout_pad = c.cout_pad;
   return RB_OK;
 }
 
@@ -619,54 +563,34 @@ extern "C" int rb_update_weights_pack_host(int small, const float* const* W_host
              blob_bytes, L.total);
   for (int i = 0; i < v.nref; ++i)
     RB_REQUIRE(W_host[i] && b_host[i], RB_ERR_BAD_ARG, "rb_update_weights_pack: missing weights for %s", v.ref[i].name);
-  struct HostBlob {
-    char* p;
-    char* data() { return p; }
-  } host{reinterpret_cast<char*>(host_blob)};
   memset(host_blob, 0, L.total);
   for (int id = 0; id < P_COUNT; ++id) {
-    const PackedConv& pc = v.pk[id];
+    const PackedSrc& pc = v.pk[id];
     if (pc.src0 < 0) continue;
-    __half* hi = reinterpret_cast<__half*>(host.data() + L.hi[id]);
-    __half* lo = reinterpret_cast<__half*>(host.data() + L.lo[id]);
-    float* bias = reinterpret_cast<float*>(host.data() + L.bias[id]);
-    const int taps = L.kh[id] * L.kw[id];
     int co_base = 0;
-    for (int sidx = 0; sidx < 2; ++sidx) {
-      int src = sidx == 0 ? pc.src0 : pc.src1;
+    for (int src : {pc.src0, pc.src1}) {
       if (src < 0) continue;
       const RefConv& r = v.ref[src];
       RB_REQUIRE(r.cin <= pc.cin_pad, RB_ERR_BAD_SHAPE, "internal: cin_pad too small for %s", r.name);
-      const float* Wsrc = W_host[src];  // HWIO
-      for (int t = 0; t < taps; ++t)
-        for (int ci = 0; ci < r.cin; ++ci)
-          for (int co = 0; co < r.cout; ++co) {
-            float val = Wsrc[((size_t)t * r.cin + ci) * r.cout + co];
-            size_t o = ((size_t)(co_base + co) * taps + t) * pc.cin_pad + ci;
-            split_f32(val, hi[o], lo[o]);
-          }
-      for (int co = 0; co < r.cout; ++co) bias[co_base + co] = b_host[src][co];
+      pack_hwio(L.conv[id], host_blob, W_host[src], r.cin, r.cout, co_base);
+      for (int co = 0; co < r.cout; ++co) put_bias(L.conv[id], host_blob, co_base + co, b_host[src][co]);
       co_base += r.cout;
     }
   }
   {
     const RefConv& f = v.ref[v.convf1_ref];
-    memcpy(host.data() + L.f1_w, W_host[v.convf1_ref], (size_t)f.kh * f.kw * f.cin * f.cout * sizeof(float));
-    memcpy(host.data() + L.f1_b, b_host[v.convf1_ref], (size_t)f.cout * sizeof(float));
-    // tensor-core form: tap (ky, kx), flow channel c -> [co][ky][kx * 8 + c] (window pixel kx of 8, 8 channels per pixel)
+    char* host = reinterpret_cast<char*>(host_blob);
+    memcpy(host + L.f1_w, W_host[v.convf1_ref], (size_t)f.kh * f.kw * f.cin * f.cout * sizeof(float));
+    memcpy(host + L.f1_b, b_host[v.convf1_ref], (size_t)f.cout * sizeof(float));
+    // tensor-core form: tap (ky, kx), flow channel c -> row ky, k = kx * 8 + c (window pixel kx of 8, 8 channels per pixel)
     RB_REQUIRE(f.kh == 7 && f.kw == 7 && f.cin == 2, RB_ERR_BAD_SHAPE, "internal: convf1 is expected to be 7x7x2");
-    __half* hi = reinterpret_cast<__half*>(host.data() + L.f1t_hi);
-    __half* lo = reinterpret_cast<__half*>(host.data() + L.f1t_lo);
-    float* bias = reinterpret_cast<float*>(host.data() + L.f1t_bias);
     const float* Wsrc = W_host[v.convf1_ref];
     for (int ky = 0; ky < 7; ++ky)
       for (int kx = 0; kx < 7; ++kx)
         for (int c = 0; c < 2; ++c)
-          for (int co = 0; co < f.cout; ++co) {
-            const size_t o = ((size_t)co * 7 + ky) * 64 + kx * 8 + c;
-            split_f32(Wsrc[((size_t)(ky * 7 + kx) * 2 + c) * f.cout + co], hi[o], lo[o]);
-          }
-    for (int co = 0; co < f.cout; ++co) bias[co] = b_host[v.convf1_ref][co];
+          for (int co = 0; co < f.cout; ++co)
+            put_weight(L.f1t, host_blob, co, ky, kx * 8 + c, Wsrc[((size_t)(ky * 7 + kx) * 2 + c) * f.cout + co]);
+    for (int co = 0; co < f.cout; ++co) put_bias(L.f1t, host_blob, co, b_host[v.convf1_ref][co]);
   }
   return RB_OK;
 }
@@ -676,13 +600,8 @@ extern "C" int rb_update_weights_pack(int small, const float* const* W_host, con
   RB_REQUIRE(blob, RB_ERR_BAD_ARG, "rb_update_weights_pack: null pointer");
   const size_t total = packed_layout(variant(small)).total;
   RB_REQUIRE(blob_bytes >= total, RB_ERR_WORKSPACE, "rb_update_weights_pack: blob has %zu bytes, need %zu", blob_bytes, total);
-  std::vector<char> host(total, 0);
-  int rc = rb_update_weights_pack_host(small, W_host, b_host, host.data(), total);
-  if (rc) return rc;
-  cudaStream_t s = (cudaStream_t)stream;
-  RB_CHECK_CUDA(cudaMemcpyAsync(blob, host.data(), total, cudaMemcpyHostToDevice, s));
-  RB_CHECK_CUDA(cudaStreamSynchronize(s));  // `host` dies at return; packing is an init-time call
-  return RB_OK;
+  return upload_packed(blob, total, (cudaStream_t)stream,
+                       [&](void* host) { return rb_update_weights_pack_host(small, W_host, b_host, host, total); });
 }
 
 extern "C" int rb_update_workspace_bytes(int small, int B, int h, int w, size_t* bytes) {
