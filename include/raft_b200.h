@@ -117,6 +117,12 @@ int rb_debug_conv_last_passes(void);
 /* ---- A4: coords_grid(batch, ht, wd)  networks/utils.py:4-11 ----------------------------------
  * coords[b,y,x,0] = x, coords[b,y,x,1] = y. */
 int rb_coords_grid(float* coords, int B, int h, int w, void* stream);
+/* F10 warm start (upstream RAFT.forward's flow_init): coords1 [B,h,w,2] = coords_grid + flow_init, one fp32 add per
+ * element (upstream's coords1 = coords1 + flow_init); a NULL flow_init gives the bits of rb_coords_grid.
+ * rb_coords_to_flow: flow_low [B,h,w,2] = coords1 - coords_grid in fp32 (upstream's coords1 - coords0).  Null pointers
+ * (coords1, flow_low), B/h/w <= 0 and B*h*w >= 2^31 -> RB_ERR_* before any CUDA call. */
+int rb_coords_init(float* coords1, const float* flow_init, int B, int h, int w, void* stream);
+int rb_coords_to_flow(const float* coords1, float* flow_low, int B, int h, int w, void* stream);
 
 /* ---- A1: GetCorrPyramid(fmap1, fmap2, num_levels=4)  networks/model_utils.py:199-221 ----------
  * pyramid layout: level l (dims h_l = h >> l, w_l = w >> l, floor) is a dense fp32 array
@@ -294,6 +300,23 @@ int rb_frame_synthesize(const float* frames, int Hp, int Wp, int top, int left, 
 int rb_flow_metrics_workspace_bytes(int B, int H, int W, size_t* bytes);
 int rb_flow_metrics(const float* flow, float flow_scale, const float* gt, const uint8_t* valid, int B, int H, int W,
                     float* epe, double* stats, void* workspace, size_t workspace_bytes, void* stream);
+
+/* ---- F10: warm start -- upstream RAFT's forward_interpolate (core/utils/utils.py), batched, on the GPU -------------
+ * flow, out: [B,h,w,2] fp32 NHWC; each sample on its own.  Source pixel (x, y) with (dx, dy) = flow[b,y,x] lands at
+ * x1 = (double)x + dx, y1 = (double)y + dy (exact, like numpy's int64 + float32); it is valid iff 0 < x1 < w and
+ * 0 < y1 < h (strict; a NaN is invalid).  out[b,qy,qx] = the (dx, dy) of the valid source of sample b with the smallest
+ * d = fl64(fl64((qx - x1)^2) + fl64((qy - y1)^2)) (no FMA contraction: cKDTree's float64 squared distance), copied bit for
+ * bit; equal d -> the lower source index y*w + x.  scipy breaks such ties in kd-tree order, so the result equals upstream's
+ * griddata(method='nearest') wherever the nearest source is unique.  A sample without a valid source gives zeros
+ * (upstream's griddata raises on the empty point set).
+ * Valid sources are bucketed by integer cell (floor(x1), floor(y1)) with integer atomics, a per-sample scan and a placement
+ * pass; one thread per grid point scans rings of cells outward until no closer source can exist: O(B h w) for a flow
+ * whose sources land near the grid points (a few valid sources far from most grid points degrade to every cell).  No float
+ * atomics, the same bits for every B, no allocation (workspace: rb_flow_forward_interpolate_workspace_bytes), CUDA-graph
+ * capturable.  Null pointers, B/h/w <= 0, B*h*w >= 2^31 and a workspace that is too small -> RB_ERR_* before any CUDA call. */
+int rb_flow_forward_interpolate_workspace_bytes(int B, int h, int w, size_t* bytes);
+int rb_flow_forward_interpolate(const float* flow, float* out, int B, int h, int w, void* workspace,
+                                size_t workspace_bytes, void* stream);
 
 /* ---- F3 (input edge): dataflow/test_dataflow.py:56-61,96-97 + the SURVEY 8(d) shape policy ------------------
  * src: [B,H,W,3] device frames, BGR like cv2.imdecode -- fp32 in [0,1] (src_is_u8 = 0) or uint8 in [0,255]

@@ -18,6 +18,29 @@ __global__ void coords_grid_kernel(float2* __restrict__ coords, int B, int h, in
   coords[i] = make_float2((float)x, (float)y);
 }
 
+// F10 warm start: coords1 = grid + flow_init (upstream RAFT.forward's coords1 + flow_init), one fp32 add per element;
+// a null init writes the grid itself
+__global__ void coords_init_kernel(float2* __restrict__ coords, const float2* __restrict__ init, int B, int h, int w) {
+  int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= B * h * w) return;
+  int x = i % w, y = (i / w) % h;
+  float2 c = make_float2((float)x, (float)y);
+  if (init != nullptr) {
+    const float2 f = init[i];
+    c = make_float2(__fadd_rn(c.x, f.x), __fadd_rn(c.y, f.y));
+  }
+  coords[i] = c;
+}
+
+// flow_low = coords1 - grid in fp32 (upstream's coords1 - coords0)
+__global__ void coords_to_flow_kernel(const float2* __restrict__ coords, float2* __restrict__ flow, int B, int h, int w) {
+  int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= B * h * w) return;
+  int x = i % w, y = (i / w) % h;
+  const float2 c = coords[i];
+  flow[i] = make_float2(__fsub_rn(c.x, (float)x), __fsub_rn(c.y, (float)y));
+}
+
 // ---------------------------------------------------------------------------------------------
 // A1  SIMT fp32 correlation GEMM: vol[b, n, m] = <f1[b,n,:], f2[b,m,:]> / sqrt(C)
 //     (model_utils.py:206-215).  64x64 tile, 16-deep k slices, 4x4 micro-tile per thread.
@@ -788,6 +811,28 @@ extern "C" int rb_coords_grid(float* coords, int B, int h, int w, void* stream) 
   int n = B * h * w;
   coords_grid_kernel<<<(n + 255) / 256, 256, 0, (cudaStream_t)stream>>>(reinterpret_cast<float2*>(coords), B, h, w);
   RB_CHECK_LAUNCH("coords_grid_kernel");
+  return RB_OK;
+}
+
+extern "C" int rb_coords_init(float* coords1, const float* flow_init, int B, int h, int w, void* stream) {
+  RB_REQUIRE(coords1, RB_ERR_BAD_ARG, "rb_coords_init: null pointer");
+  RB_REQUIRE(B > 0 && h > 0 && w > 0 && (size_t)B * h * w < (size_t(1) << 31), RB_ERR_BAD_SHAPE,
+             "rb_coords_init: bad shape B=%d h=%d w=%d", B, h, w);
+  int n = B * h * w;
+  coords_init_kernel<<<(n + 255) / 256, 256, 0, (cudaStream_t)stream>>>(
+      reinterpret_cast<float2*>(coords1), reinterpret_cast<const float2*>(flow_init), B, h, w);
+  RB_CHECK_LAUNCH("coords_init_kernel");
+  return RB_OK;
+}
+
+extern "C" int rb_coords_to_flow(const float* coords1, float* flow_low, int B, int h, int w, void* stream) {
+  RB_REQUIRE(coords1 && flow_low, RB_ERR_BAD_ARG, "rb_coords_to_flow: null pointer");
+  RB_REQUIRE(B > 0 && h > 0 && w > 0 && (size_t)B * h * w < (size_t(1) << 31), RB_ERR_BAD_SHAPE,
+             "rb_coords_to_flow: bad shape B=%d h=%d w=%d", B, h, w);
+  int n = B * h * w;
+  coords_to_flow_kernel<<<(n + 255) / 256, 256, 0, (cudaStream_t)stream>>>(
+      reinterpret_cast<const float2*>(coords1), reinterpret_cast<float2*>(flow_low), B, h, w);
+  RB_CHECK_LAUNCH("coords_to_flow_kernel");
   return RB_OK;
 }
 

@@ -126,6 +126,21 @@ def read_kitti_flow(path):
     return np.ascontiguousarray(flow), (raw[..., 0] >= 0.5).astype(np.uint8)
 
 
+def write_kitti_flow(path, flow):
+    """[H,W,2] flow -> KITTI's 16-bit flow PNG, the inverse of read_kitti_flow and the bytes of upstream RAFT's
+    writeFlowKITTI: u, v as uint16(64 * flow + 2**15) in float32 (truncated), the valid flag 1 everywhere, channels in
+    OpenCV's BGR order (flag, v, u)."""
+    import cv2
+    uv = np.asarray(flow, dtype=np.float32)
+    if uv.ndim != 3 or uv.shape[2] != 2:
+        raise ValueError(f"write_kitti_flow: flow must be [H,W,2], got {uv.shape}")
+    uv = np.float32(64.0) * uv + np.float32(2 ** 15)
+    valid = np.ones([uv.shape[0], uv.shape[1], 1])
+    raw = np.concatenate([uv, valid], axis=-1).astype(np.uint16)
+    if not cv2.imwrite(str(path), raw[..., ::-1]):
+        raise OSError(f"cannot write {path}")
+
+
 def read_flo(path):
     with open(path, "rb") as fh:
         magic = np.fromfile(fh, np.float32, 1)[0]

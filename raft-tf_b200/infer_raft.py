@@ -21,7 +21,14 @@ flow(s) resized back to im1's size with the reference's flow_utils.resize_flow (
     python infer_raft.py -m val --dataset sintel --data datasets/Sintel --load raft-things.npz --upstream [--batch 8]
 
 prints upstream's lines (``Validation (clean) EPE: ...``, ``Validation KITTI: <epe>, <f1>``) and writes the aggregates and
-per-pair records to ``<--out>/val_<dataset>.json`` (raft_b200.evaluate).
+per-pair records to ``<--out>/val_<dataset>.json`` (raft_b200.evaluate).  --warm-start runs each Sintel scene as a chain,
+every pair after the first warm-started from the previous pair's flow (upstream's forward_interpolate; an extension of
+the validation, which upstream runs cold).  --split test writes upstream's test-split submission under --out instead:
+
+    python infer_raft.py -m val --split test --dataset sintel --data datasets/Sintel --out submission --load ... [--warm-start]
+
+Sintel: ``<out>/<dstype>/<scene>/frameNNNN.flo``; KITTI (no --warm-start): ``<out>/<id>_10.png``, 16-bit PNGs
+(raft_b200.evaluate.submit).
 """
 import argparse
 import os
@@ -76,6 +83,11 @@ def parser():
     p.add_argument('--dstype', nargs='+', default=['clean', 'final'], choices=['clean', 'final'],
                    help='-m val, Sintel: the passes to evaluate')
     p.add_argument('--workers', type=int, default=4, help='-m val: frame-decoding threads')
+    p.add_argument('--split', default='training', choices=['training', 'test'],
+                   help='-m val: validate on the training split, or write the test-split submission under --out')
+    p.add_argument('--warm-start', action='store_true',
+                   help="-m val, Sintel: warm-start each pair from the previous pair's flow in its scene (upstream's "
+                        "warm_start=True)")
     p.add_argument('--keep-size', action='store_true', help='extension: pad to a multiple of 8 instead of resizing to 432x1024')
     p.add_argument('--npy', default=None, help='extension: also save the raw [H,W,2] flow')
     p.add_argument('--flo', default=None, help='extension: also save the flow as a Middlebury .flo file')
@@ -102,6 +114,8 @@ def main(argv=None):
     if args.mode == 'val':
         if not args.data or not args.dataset:
             p.error('-m val needs --data <dataset root> and --dataset {sintel,kitti}')
+        if args.warm_start and args.dataset == 'kitti':
+            p.error("--warm-start needs frame sequences: KITTI's pairs are not sequences")
         return validate(args)
     if args.mode != 'test':
         print(f"mode '{args.mode}' has no implementation in the reference either (infer_raft.py:71-95); nothing to do")
@@ -155,13 +169,19 @@ def main(argv=None):
 
 
 def validate(args):
-    """-m val: raft_b200.evaluate on --data, upstream's summary lines on stdout, everything in <--out>/val_<dataset>.json."""
+    """-m val: raft_b200.evaluate on --data, upstream's summary lines on stdout, everything in <--out>/val_<dataset>.json;
+    with --split test, raft_b200.evaluate.submit's files under --out."""
     import json
     from networks import RAFT
-    from raft_b200.evaluate import evaluate, summary_lines
+    from raft_b200.evaluate import evaluate, submit, summary_lines
     model = RAFT.RAFT(None, args, upstream=args.upstream, mixed_precision=args.mixed_precision).load(args.load)
+    if args.split == 'test':
+        files = submit(model, args.data, args.dataset, args.out, dstypes=tuple(args.dstype), batch=args.batch,
+                       workers=args.workers, iters=args.iters, warm_start=args.warm_start)
+        print(f"{len(files)} flows written under {args.out}")
+        return 0
     res = evaluate(model, args.data, args.dataset, dstypes=tuple(args.dstype), batch=args.batch, workers=args.workers,
-                   iters=args.iters)
+                   iters=args.iters, warm_start=args.warm_start)
     for line in summary_lines(res):
         print(line)
     os.makedirs(args.out, exist_ok=True)

@@ -99,15 +99,23 @@ class RAFT(object):
 
     # -- inference ---------------------------------------------------------------------------------
     @torch.no_grad()
-    def forward(self, input_left, input_right):
+    def forward(self, input_left, input_right, flow_init=None, return_low=False):
         """[B,H,W,3] frames, BGR like the reference -- fp32 in [0,1] (the reference's placeholders, RAFT.py:45-51) or
         uint8 in [0,255] (extension: the /255 of test_dataflow.py:96-97 then runs on the GPU); numpy or torch, host or
         CUDA -> [B,H,W,2] torch CUDA flow (a fresh tensor per call, like a session.run result).  H, W that are not
         multiples of 8 are replicate-padded and the flow cropped back, both inside the engine's own kernels.  With
         input_size the frames may have any size: they are resized to input_size first (rb_frames_resize, in the same
-        CUDA graph) and the flow is at input_size, as in the reference; flow_utils.resize_flow takes it back."""
-        flow = self.engine().forward(_as_tensor(input_left), _as_tensor(input_right))
-        return flow.clone()
+        CUDA graph) and the flow is at input_size, as in the reference; flow_utils.resize_flow takes it back.
+
+        Extension (upstream RAFT's warm start): flow_init, a [B,h,w,2] float32 flow on the padded 1/8-resolution grid
+        (numpy or torch, host or CUDA), starts the loop from coords_grid + flow_init; return_low=True returns fresh
+        tensors (flow_low, flow_up) like upstream's test_mode, flow_low being that grid's flow after the last iteration.
+        networks.utils.forward_interpolate(flow_low) is the next frame pair's flow_init."""
+        if flow_init is not None and not isinstance(flow_init, torch.Tensor):
+            flow_init = torch.as_tensor(np.asarray(flow_init))
+        out = self.engine().forward(_as_tensor(input_left), _as_tensor(input_right), flow_init=flow_init,
+                                    return_low=return_low)
+        return tuple(t.clone() for t in out) if return_low else out.clone()
 
     @torch.no_grad()
     def forward_bidirectional(self, input_left, input_right, check=True):

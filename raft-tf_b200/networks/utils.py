@@ -81,6 +81,26 @@ def flow_metrics(flow, gt, valid=None, flow_scale=1.0, return_epe=False):
     return (stats, epe) if return_epe else stats
 
 
+def forward_interpolate(flow):
+    """Extension (upstream RAFT's core/utils/utils.py forward_interpolate, on the GPU): every grid point of the [B,h,w,2]
+    fp32 CUDA flow takes the flow of the nearest source pixel x + flow(x) that lands strictly inside the grid, per
+    sample (rb_flow_forward_interpolate; equal distances go to the lower source index, a sample without such a source
+    gives zeros).  Returns a fresh [B,h,w,2] tensor: the flow_init of the next frame pair from this pair's flow_low."""
+    if not (isinstance(flow, torch.Tensor) and flow.is_cuda and flow.dim() == 4 and flow.shape[-1] == 2
+            and flow.dtype == torch.float32):
+        raise ValueError(f"forward_interpolate: flow must be a [B,h,w,2] float32 CUDA tensor (got "
+                         f"{getattr(flow, 'shape', None)} {getattr(flow, 'dtype', type(flow))})")
+    f = flow.contiguous()
+    B, h, w, _ = f.shape
+    out = torch.empty_like(f)
+    with torch.cuda.device(f.device):
+        nbytes = capi.size_query(capi.lib.rb_flow_forward_interpolate_workspace_bytes, B, h, w)
+        ws = torch.empty(nbytes, dtype=torch.uint8, device=f.device)
+        capi.check(capi.lib.rb_flow_forward_interpolate(capi.ptr(f), capi.ptr(out), B, h, w, capi.ptr(ws), nbytes,
+                                                        capi.stream()))
+    return out
+
+
 def reverse_flow(flow, time_step=1.0, bg=None, im0=None):
     """The reference's flow_utils.py:166 reverse_flow_avg_skip_static on a batch of CUDA flows (rb_flow_reverse, bit for
     bit): projects the [B,H,W,2] flow 0 -> 1 to time `time_step` and returns the flow from there back to frame 0.

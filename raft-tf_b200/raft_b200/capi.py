@@ -35,6 +35,8 @@ SIGNATURES = {
     "rb_debug_conv_last": (_i, [_pi, _pi, _pi, _pi, _pi]),
     "rb_debug_conv_last_passes": (_i, []),
     "rb_coords_grid": (_i, [_vp, _i, _i, _i, _vp]),
+    "rb_coords_init": (_i, [_vp, _vp, _i, _i, _i, _vp]),
+    "rb_coords_to_flow": (_i, [_vp, _vp, _i, _i, _i, _vp]),
     "rb_corr_pyramid_bytes": (_i, [_i, _i, _i, _psz]),
     "rb_corr_level_offset": (_i, [_i, _i, _i, _i, _psz, _pi, _pi]),
     "rb_corr_workspace_bytes": (_i, [_i, _i, _i, _i, _psz]),
@@ -73,6 +75,8 @@ SIGNATURES = {
     "rb_frame_synthesize": (_i, [_vp, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _f, _vp, _i, _i, _i, _vp]),
     "rb_flow_metrics_workspace_bytes": (_i, [_i, _i, _i, _psz]),
     "rb_flow_metrics": (_i, [_vp, _f, _vp, _vp, _i, _i, _i, _vp, _vp, _vp, _sz, _vp]),
+    "rb_flow_forward_interpolate_workspace_bytes": (_i, [_i, _i, _i, _psz]),
+    "rb_flow_forward_interpolate": (_i, [_vp, _vp, _i, _i, _i, _vp, _sz, _vp]),
     "rb_frames_prepare": (_i, [_vp, _i, _vp, _i, _i, _i, _i, _i, _i, _i, _vp]),
     "rb_frames_resize": (_i, [_vp, _i, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp]),
     "rb_flow_resize": (_i, [_vp, _vp, _i, _i, _i, _i, _i, _vp]),

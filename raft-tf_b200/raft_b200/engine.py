@@ -7,6 +7,8 @@ forward_bidirectional runs both directions of B frame pairs as 2B pairs through 
 and adds the forward-backward consistency check (rb_flow_fb_check, csrc/consistency.cu) to the same graph.
 interpolate runs the same bidirectional pass (without the check) from its own graph, then per time t two flow reversals
 and the frame blend (rb_flow_reverse, rb_frame_synthesize, csrc/interp.cu) eagerly on the same stream.
+forward(flow_init=..., return_low=True) is upstream's warm start: the same graph with rb_coords_init in place of
+rb_coords_grid and rb_coords_to_flow (flow_low) after the loop, captured as a mode of its own (FORWARD_WARM).
 With input_size set, every mode first resizes the frames to that size like the reference's cv2.resize (rb_frames_resize,
 csrc/resize.cu, in the graph in place of rb_frames_prepare), and its outputs come back at that size.
 """
@@ -23,8 +25,9 @@ from .encoders import CudaEncoder
 from .weights import pack_update_block
 
 # what one pass computes: L->R only (forward), both directions (forward_bidirectional), both plus the occlusion check,
-# both directions for interpolate (which also holds the buffers of the per-t calls)
-FORWARD, BIDIRECTIONAL, BIDIRECTIONAL_CHECK, INTERPOLATE = 0, 1, 2, 3
+# both directions for interpolate (which also holds the buffers of the per-t calls), L->R warm-started from flow_init with
+# the 1/8-resolution flow kept (forward(flow_init=..., return_low=True))
+FORWARD, BIDIRECTIONAL, BIDIRECTIONAL_CHECK, INTERPOLATE, FORWARD_WARM = 0, 1, 2, 3, 4
 # forward-backward consistency thresholds of UnFlow (Meister et al. 2018): |f+b|^2 > a1 (|f|^2 + |b|^2) + a2
 FB_ALPHA1, FB_ALPHA2 = 0.01, 0.5
 # smallest frame side: the 4-level correlation pyramid needs a 1/8-resolution grid of at least 8 (level 3 is grid >> 3),
@@ -39,8 +42,8 @@ PAD_MODES = ("sintel", "kitti")
 class RaftEngine:
     # everything _ensure allocates for one (B, H, W, u8, mode); parked per mode so alternating modes re-captures nothing
     _STATE = ("_key", "src_hw", "pad", "h", "w", "Hp", "Wp", "pairs", "pyr_bytes", "pyramid", "cws_bytes", "corr_ws",
-              "ws_bytes", "ws", "coords1", "mask", "flow_up", "occ", "rev_ws_bytes", "rev_ws", "flow_t", "empty_t", "fmaps", "fmap1", "fmap2", "cmap", "images", "staged", "raw", "_shape",
-              "_graph")
+              "ws_bytes", "ws", "coords1", "mask", "flow_up", "occ", "rev_ws_bytes", "rev_ws", "flow_t", "empty_t", "flow_init", "flow_low", "fmaps", "fmap1", "fmap2", "cmap", "images", "staged", "raw",
+              "_shape", "_graph")
 
     def __init__(self, params: Dict[str, np.ndarray], small: bool = False, iters: int = 20,
                  device: Optional[torch.device] = None, use_graph: bool = True, math_mode: int = capi.RB_MATH_TC,
@@ -134,7 +137,7 @@ class RaftEngine:
         if key in self._parked:
             self.__dict__.update(self._parked.pop(key))
             return
-        bidir = mode != FORWARD
+        bidir = mode not in (FORWARD, FORWARD_WARM)
         NB = 2 * B if bidir else B  # frame pairs through the hot path
         ph, pw = (-H) % 8, (-W) % 8
         top = 0 if self.pad_mode == "kitti" else ph // 2
@@ -165,6 +168,11 @@ class RaftEngine:
             self.empty_t = torch.empty(2, 2, B, H, W, dtype=torch.uint8, device=d)  # [empty | multi]
         else:
             self.rev_ws_bytes, self.rev_ws, self.flow_t, self.empty_t = 0, None, None, None
+        if mode == FORWARD_WARM:  # the caller's initial flow (copied in before each replay) and the final 1/8-res flow
+            self.flow_init = torch.zeros(B, h, w, 2, dtype=torch.float32, device=d)
+            self.flow_low = torch.empty(B, h, w, 2, dtype=torch.float32, device=d)
+        else:
+            self.flow_init, self.flow_low = None, None
         self.fmaps = torch.empty(NB + B, h, w, self.fdim, dtype=torch.float32, device=d)
         self.fmap1, self.fmap2 = self.fmaps[:NB], self.fmaps[B:]
         self.cmap = torch.empty(NB, h, w, self.hidden + self.ctx, dtype=torch.float32, device=d)
@@ -190,7 +198,7 @@ class RaftEngine:
         Bidirectional modes: cnet runs on all 2B frames (the R->L pairs need the context of R), and the last B feature
         maps are a device-to-device copy of the first B (a copy-engine transfer, no kernel)."""
         B, H, W, u8, mode = self._shape
-        bidir = mode != FORWARD
+        bidir = mode not in (FORWARD, FORWARD_WARM)
         cnet, cframes = (self.cnet_bidir, self.images) if bidir else (self.cnet, self.images[:B])
         fout = self.fmaps[:2 * B]  # [fL | fR]
         capi.check(capi.lib.rb_set_math_mode(self.math_mode))  # per-thread library state: set before ANY kernel of ours
@@ -234,7 +242,10 @@ class RaftEngine:
                                          self.fdim, capi.ptr(self.corr_ws), self.cws_bytes, st))
         self._join_cnet()  # cmap (context encoder, forked stream) is first needed here
         capi.check(lib.rb_update_set_state_cnet(s, capi.ptr(self.blob), capi.ptr(self.ws), capi.ptr(self.cmap), B, h, w, st))
-        capi.check(lib.rb_coords_grid(capi.ptr(self.coords1), B, h, w, st))
+        if mode == FORWARD_WARM:  # coords1 = grid + flow_init (upstream RAFT.forward)
+            capi.check(lib.rb_coords_init(capi.ptr(self.coords1), capi.ptr(self.flow_init), B, h, w, st))
+        else:
+            capi.check(lib.rb_coords_grid(capi.ptr(self.coords1), B, h, w, st))
         if self.volume_free:  # RAFT.py:91-102 with the lookup evaluated on the fly
             for it in range(self.iters):
                 capi.check(lib.rb_update_lookup_otf(s, capi.ptr(self.ws), capi.ptr(self.fmap1), capi.ptr(self.fmap2),
@@ -245,6 +256,8 @@ class RaftEngine:
         else:
             capi.check(lib.rb_raft_iterate(s, capi.ptr(self.blob), capi.ptr(self.ws), capi.ptr(self.pyramid),
                                            capi.ptr(self.coords1), capi.ptr(self.mask), B, h, w, self.iters, st))
+        if mode == FORWARD_WARM:
+            capi.check(lib.rb_coords_to_flow(capi.ptr(self.coords1), capi.ptr(self.flow_low), B, h, w, st))
         top, left = self.pad[0], self.pad[2]  # crop the padding away while upsampling
         if self.small:
             capi.check(lib.rb_upflow8_crop(capi.ptr(self.coords1), capi.ptr(self.flow_up), B, h, w, 8.0 / self.flow_scale,
@@ -289,16 +302,30 @@ class RaftEngine:
         self._graph.replay()
 
     @torch.no_grad()
-    def forward(self, left: torch.Tensor, right: torch.Tensor) -> torch.Tensor:
+    def forward(self, left: torch.Tensor, right: torch.Tensor, flow_init: Optional[torch.Tensor] = None,
+                return_low: bool = False):
         """left/right: [B,H,W,3] frames, BGR like the reference: fp32 in [0,1] (RAFT.inputs(), RAFT.py:45-51) or
         uint8 in [0,255] (what cv2.imdecode yields, test_dataflow.py:56-61; the /255 then happens on the GPU).  Host
         (ideally pinned) or CUDA tensors; any H, W >= 57 (MIN_FRAME; 121 with upstream=True, whose weights expect RGB
         frames; smaller frames raise ValueError), or any size
         with input_size set, which resizes them to input_size first.  Returns the [B,H,W,2] flow (at input_size when
         set) -- the engine-owned buffer itself, overwritten by the next call (networks.RAFT.RAFT.forward hands
-        out a copy)."""
-        self._run_frames(left, right, FORWARD)
-        return self.flow_up
+        out a copy).
+
+        Warm start (upstream RAFT's flow_init): flow_init is a [B,h,w,2] fp32 host or CUDA tensor on the padded grid
+        h, w = Hp / 8, Wp / 8 (of input_size when set), and the loop starts from coords1 = grid + flow_init.  With
+        return_low the call returns (flow_low, flow_up), flow_low = coords1 - grid [B,h,w,2] after the last iteration,
+        in the order of upstream's test_mode tuple; forward_interpolate(flow_low) is the next frame's flow_init.  Either
+        argument runs a graph of its own (FORWARD_WARM, a zero init when flow_init is None); without them the call is the
+        plain forward above.  A wrong shape or dtype raises ValueError."""
+        if flow_init is None and not return_low:
+            self._run_frames(left, right, FORWARD)
+            return self.flow_up
+        if flow_init is not None and (not isinstance(flow_init, torch.Tensor) or flow_init.dtype != torch.float32):
+            raise ValueError(f"raft_b200: flow_init must be a float32 torch tensor (got "
+                             f"{getattr(flow_init, 'dtype', type(flow_init))})")
+        self._run_frames(left, right, FORWARD_WARM, flow_init)
+        return (self.flow_low, self.flow_up) if return_low else self.flow_up
 
     @torch.no_grad()
     def forward_bidirectional(self, left: torch.Tensor, right: torch.Tensor, check: bool = True):
@@ -348,13 +375,21 @@ class RaftEngine:
                                            ptr(self.flow_t[0]), ptr(self.flow_t[1]), ptr(self.empty_t[0, 0]),
                                            ptr(self.empty_t[0, 1]), t, ptr(out), B, H, W, st))
 
-    def _run_frames(self, left: torch.Tensor, right: torch.Tensor, mode: int):
+    def _run_frames(self, left: torch.Tensor, right: torch.Tensor, mode: int, flow_init: Optional[torch.Tensor] = None):
         assert left.shape == right.shape and left.dim() == 4 and left.shape[-1] == 3 and left.dtype == right.dtype
         u8 = left.dtype == torch.uint8
         assert u8 or left.dtype == torch.float32, left.dtype
         with torch.cuda.device(self.device):
             B = left.shape[0]
             self._ensure(B, left.shape[1], left.shape[2], u8, mode)
+            if mode == FORWARD_WARM:
+                if flow_init is None:
+                    self.flow_init.zero_()
+                elif tuple(flow_init.shape) != tuple(self.flow_init.shape):
+                    raise ValueError(f"raft_b200: flow_init must be [B,h,w,2] = {list(self.flow_init.shape)} on the padded "
+                                     f"1/8-resolution grid (got {list(flow_init.shape)})")
+                else:
+                    self.flow_init.copy_(flow_init, non_blocking=True)
             dst = self.raw if self.staged else self.images
             dst[:B].copy_(left, non_blocking=True)  # H2D when the caller hands pinned host tensors
             dst[B:].copy_(right, non_blocking=True)

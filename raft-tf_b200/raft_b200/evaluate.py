@@ -8,6 +8,9 @@ Sintel: every frame of <root>/training/{clean,final}/<scene>/ paired with the ne
 <root>/training/image_2/<id>_10.png and <id>_11.png, ground truth <root>/training/flow_occ/<id>_10.png (16-bit PNG with a
 valid flag), 24 iterations, 'kitti' padding (bottom only), valid pixels counted.  Frames run at their own size.
 
+submit writes upstream's test-split submissions (create_sintel_submission, create_kitti_submission) the same way, and
+warm_start runs each Sintel scene as a chain warm-started by forward_interpolate (upstream's warm_start=True).
+
 Pipeline: pairs are grouped by frame size (one CUDA graph per size) and run in batches through RaftEngine.forward, whose
 flow stays on the GPU: rb_flow_metrics scores it against the uploaded ground truth on the same stream and writes per-pair
 stats into one device buffer, read back once per split.  Worker threads decode the next batches (cv2 releases the GIL)
@@ -120,11 +123,16 @@ def _imread(path, rgb):
     return cv2.cvtColor(img, cv2.COLOR_BGR2RGB) if rgb else img
 
 
-def _decode(pair, kitti, rgb):
-    from flow_utils import read_flo, read_kitti_flow
+def _decode_frames(pair, rgb):
     left, right = _imread(pair.image1, rgb), _imread(pair.image2, rgb)
     if right.shape != left.shape:
         raise ValueError(f"{pair.image2}: {right.shape[:2]} frame, {pair.image1} is {left.shape[:2]}")
+    return left, right
+
+
+def _decode(pair, kitti, rgb):
+    from flow_utils import read_flo, read_kitti_flow
+    left, right = _decode_frames(pair, rgb)
     gt, valid = read_kitti_flow(pair.gt) if kitti else (read_flo(pair.gt), None)
     if gt.shape[:2] != left.shape[:2]:
         raise ValueError(f"{pair.gt}: {gt.shape[:2]} ground truth for {left.shape[:2]} frames ({pair.image1})")
@@ -132,27 +140,75 @@ def _decode(pair, kitti, rgb):
 
 
 class _Slot:
-    """Pinned host staging of one batch (frames, ground truth, mask) and the event behind the last batch that used it."""
+    """Pinned host staging of one batch (frames, and ground truth and mask when scored) and the event behind the last
+    batch that used it."""
 
-    def __init__(self, B, H, W, kitti):
+    def __init__(self, B, H, W, kitti, scored=True):
         self.left = torch.zeros(B, H, W, 3, dtype=torch.uint8).pin_memory()
         self.right = torch.zeros_like(self.left).pin_memory()
-        self.gt = torch.zeros(B, H, W, 2, dtype=torch.float32).pin_memory()
-        self.valid = torch.zeros(B, H, W, dtype=torch.uint8).pin_memory() if kitti else None
+        self.gt = torch.zeros(B, H, W, 2, dtype=torch.float32).pin_memory() if scored else None
+        self.valid = torch.zeros(B, H, W, dtype=torch.uint8).pin_memory() if kitti and scored else None
         self.event = None
 
 
-# ---- the run ------------------------------------------------------------------------------------------
-def _run(engine, pairs, kitti, batch, workers, rgb):
-    """Per-pair stats [N, STATS] fp64 (host, dataset order) of engine.forward on every pair."""
-    groups = {}  # (H, W) -> pair indices in dataset order; sizes in the order they first appear
+# ---- scheduling ---------------------------------------------------------------------------------------
+def chains_of(pairs, warm):
+    """The chains _steps runs: with warm, the pairs of each scene (consecutive pairs whose first frames share a
+    directory) as one chain of pair indices; otherwise every pair on its own."""
+    if not warm:
+        return [[i] for i in range(len(pairs))]
+    chains, last = [], None
     for i, p in enumerate(pairs):
-        groups.setdefault(_png_size(p.image1), []).append(i)
-    batches = []
-    for hw, idx in groups.items():
-        B = min(batch, len(idx))
-        batches += [(hw, B, idx[k:k + B]) for k in range(0, len(idx), B)]
-    order = [i for _, _, idx in batches for i in idx]  # processing order
+        d = os.path.dirname(p.image1)
+        if d != last:
+            chains.append([])
+            last = d
+        chains[-1].append(i)
+    return chains
+
+
+def warm_schedule(lengths, batch):
+    """Lockstep steps of chains with the given lengths on B = min(batch, len(lengths)) slots: each step is a list of B
+    entries, (chain, k) = pair k of that chain, or None for an idle slot.  A slot runs its chain's pairs in order, one per
+    step, then takes the first pair of the next chain not yet started (chains start in index order), so (chain, k > 0)
+    always runs in the slot that ran (chain, k - 1) one step before -- the pair whose flow warm-starts it."""
+    B = min(int(batch), len(lengths))
+    cur, nxt, steps = [None] * B, 0, []
+    while True:
+        for i in range(B):
+            c = cur[i]
+            if c is not None and c[1] + 1 < lengths[c[0]]:
+                cur[i] = (c[0], c[1] + 1)
+                continue
+            while nxt < len(lengths) and lengths[nxt] == 0:
+                nxt += 1
+            cur[i] = (nxt, 0) if nxt < len(lengths) else None
+            nxt += cur[i] is not None
+        if all(c is None for c in cur):
+            return steps
+        steps.append(list(cur))
+
+
+# ---- the run ------------------------------------------------------------------------------------------
+def _steps(engine, pairs, chains, decode, batch, workers, warm, scored, kitti=False):
+    """Runs every pair of chains (lists of indices into pairs) through engine.forward and yields (row, flow, slot) per
+    batch: row[i] = the pair index in batch row i (None: idle, its flow is not meaningful), flow = the engine's flow
+    buffer, slot = the pinned staging that holds the batch's decoded frames (and ground truth when scored).
+
+    Chains are grouped by frame size (one CUDA graph per size), each group run by warm_schedule.  With warm, pair k > 0
+    of a chain starts from forward_interpolate of the flow_low of pair k - 1 (computed on the device from the engine's
+    buffer, in the same row of the previous batch) and pair 0 from a zero init: grid + 0.0 is the cold start, bit for bit.
+    Worker threads decode the next batches (cv2 releases the GIL) into two pinned slots used in turn; a slot is refilled
+    only after the event recorded behind its batch's work (the consumer's included) has completed."""
+    from networks.utils import forward_interpolate
+    groups = {}  # (H, W) -> chain indices; sizes in the order they first appear
+    for c, chain in enumerate(chains):
+        groups.setdefault(_png_size(pairs[chain[0]].image1), []).append(c)
+    steps = []
+    for hw, cidx in groups.items():
+        for row in warm_schedule([len(chains[c]) for c in cidx], batch):
+            steps.append((hw, len(row), [None if e is None else chains[cidx[e[0]]][e[1]] for e in row],
+                          [e is not None and e[1] > 0 for e in row]))
     dev = engine.device
     pool = ThreadPoolExecutor(workers) if workers > 0 else None
     # decode this many batches ahead of the one the GPU is given (workers=0: the main thread decodes batch j + 1 while the
@@ -160,56 +216,78 @@ def _run(engine, pairs, kitti, batch, workers, rgb):
     depth = max(1, -(-workers // batch))
 
     def submit(j):
-        idx = batches[j][2]
+        ents = [(k, pairs[i]) for k, i in enumerate(steps[j][2]) if i is not None]
         if pool is None:
-            return [lambda i=i: _decode(pairs[i], kitti, rgb) for i in idx]
-        return [pool.submit(_decode, pairs[i], kitti, rgb).result for i in idx]
+            return [(k, lambda p=p: decode(p)) for k, p in ents]
+        return [(k, pool.submit(decode, p).result) for k, p in ents]
 
     try:
         with torch.cuda.device(dev):
-            stats = torch.empty(len(pairs), STATS, dtype=torch.float64, device=dev)
             stream = torch.cuda.current_stream(dev)
-            ahead = [submit(j) for j in range(min(depth, len(batches)))]
-            shape, pos = None, 0
-            for j, ((H, W), B, idx) in enumerate(batches):
+            ahead = [submit(j) for j in range(min(depth, len(steps)))]
+            shape, init = None, None
+            for j, ((H, W), B, row, cont) in enumerate(steps):
                 loads = ahead.pop(0)
-                if j + depth < len(batches):
+                if j + depth < len(steps):
                     ahead.append(submit(j + depth))  # workers start on it now
                 if shape != (B, H, W):
-                    shape = (B, H, W)
-                    slots = [_Slot(B, H, W, kitti), _Slot(B, H, W, kitti)]
-                    gt = torch.empty(B, H, W, 2, dtype=torch.float32, device=dev)
-                    valid = torch.empty(B, H, W, dtype=torch.uint8, device=dev) if kitti else None
-                    ws_bytes = capi.size_query(capi.lib.rb_flow_metrics_workspace_bytes, B, H, W)
-                    ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
+                    shape, init = (B, H, W), None
+                    slots = [_Slot(B, H, W, kitti, scored), _Slot(B, H, W, kitti, scored)]
                 slot = slots[j % 2]
                 if slot.event is not None:
                     slot.event.synchronize()  # its last batch's copies (and work) are done
-                lft, rgt, g, v = slot.left.numpy(), slot.right.numpy(), slot.gt.numpy(), None
-                if kitti:
-                    v = slot.valid.numpy()
-                for k, load in enumerate(loads):
-                    lft[k], rgt[k], g[k], vk = load()
-                    if kitti:
-                        v[k] = vk
-                nb = len(idx)  # a short last batch keeps B: the rows past nb are run but not scored
-                flow = engine.forward(slot.left, slot.right)
-                gt.copy_(slot.gt, non_blocking=True)
-                if kitti:
-                    valid.copy_(slot.valid, non_blocking=True)
-                capi.check(capi.lib.rb_flow_metrics(capi.ptr(flow), float(engine.flow_scale), capi.ptr(gt),
-                                                    capi.ptr(valid), nb, H, W, None, capi.ptr(stats[pos:pos + nb]),
-                                                    capi.ptr(ws), ws_bytes, capi.stream()))
+                lft, rgt = slot.left.numpy(), slot.right.numpy()
+                for k, load in loads:
+                    got = load()
+                    lft[k], rgt[k] = got[0], got[1]
+                    if scored:
+                        slot.gt.numpy()[k] = got[2]
+                        if kitti:
+                            slot.valid.numpy()[k] = got[3]
+                if warm:
+                    if init is not None:
+                        for k, c in enumerate(cont):
+                            if not c:
+                                init[k].zero_()  # a chain starts (or the row is idle): cold
+                    low, flow = engine.forward(slot.left, slot.right, flow_init=init, return_low=True)
+                else:
+                    flow = engine.forward(slot.left, slot.right)
+                yield row, flow, slot
+                if warm:
+                    init = forward_interpolate(low)  # before the next batch overwrites flow_low
                 slot.event = torch.cuda.Event()
                 slot.event.record(stream)
-                pos += nb
-            host = stats.cpu().numpy()
     finally:
         if pool is not None:
             pool.shutdown(wait=True, cancel_futures=True)
-    out = np.empty_like(host)
-    out[order] = host
-    return out
+
+
+def _run(engine, pairs, kitti, batch, workers, rgb, warm=False):
+    """Per-pair stats [N, STATS] fp64 (host, dataset order) of engine.forward on every pair (warm: scene by scene,
+    warm-started as in _steps), scored by rb_flow_metrics against the uploaded ground truth on the same stream."""
+    dev = engine.device
+    with torch.cuda.device(dev):
+        stats = torch.empty(len(pairs), STATS, dtype=torch.float64, device=dev)
+        shape = None
+        for row, flow, slot in _steps(engine, pairs, chains_of(pairs, warm), lambda p: _decode(p, kitti, rgb), batch,
+                                      workers, warm, True, kitti):
+            B, H, W = flow.shape[:3]
+            if shape != (B, H, W):
+                shape = (B, H, W)
+                gt = torch.empty(B, H, W, 2, dtype=torch.float32, device=dev)
+                valid = torch.empty(B, H, W, dtype=torch.uint8, device=dev) if kitti else None
+                ws_bytes = capi.size_query(capi.lib.rb_flow_metrics_workspace_bytes, B, H, W)
+                ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
+                part = torch.empty(B, STATS, dtype=torch.float64, device=dev)
+            gt.copy_(slot.gt, non_blocking=True)
+            if kitti:
+                valid.copy_(slot.valid, non_blocking=True)
+            # every row is scored (idle rows too: the kernel is batch-invariant), the pairs' rows are kept
+            capi.check(capi.lib.rb_flow_metrics(capi.ptr(flow), float(engine.flow_scale), capi.ptr(gt), capi.ptr(valid),
+                                                B, H, W, None, capi.ptr(part), capi.ptr(ws), ws_bytes, capi.stream()))
+            rows = [k for k, i in enumerate(row) if i is not None]
+            stats.index_copy_(0, torch.tensor([row[k] for k in rows], device=dev), part[rows])
+        return stats.cpu().numpy()
 
 
 def aggregate(pairs, stats, kitti):
@@ -230,35 +308,120 @@ def aggregate(pairs, stats, kitti):
     return res
 
 
-def evaluate(model, root, dataset="sintel", dstypes=DSTYPES, batch=1, workers=4, iters=None):
+def _setup(model, dataset, dstypes, batch, workers, iters, warm_start, what):
+    """Argument checks shared by evaluate and submit -> (kitti, splits, iterations, pad_mode)."""
+    if dataset not in PROTOCOLS:
+        raise ValueError(f"dataset must be one of {tuple(PROTOCOLS)} (got {dataset!r})")
+    if getattr(model, "input_size", None) is not None:
+        raise ValueError(f"{what}: frames run at their own size; build the model without input_size")
+    if int(batch) < 1 or int(workers) < 0:
+        raise ValueError(f"{what}: batch must be >= 1 and workers >= 0 (got {batch}, {workers})")
+    kitti = dataset == "kitti"
+    if kitti and warm_start:
+        raise ValueError(f"{what}: warm_start needs frame sequences; KITTI's pairs are not sequences")
+    if model._params is None:
+        raise RuntimeError(f"RAFT.load(<npz>) must be called before {what}")
+    splits = ("kitti",) if kitti else tuple(dstypes)
+    if not kitti and (not splits or any(d not in DSTYPES for d in splits)):
+        raise ValueError(f"Sintel dstypes must be a non-empty subset of {DSTYPES} (got {dstypes!r})")
+    n_iters, pad_mode = PROTOCOLS[dataset]
+    return kitti, splits, n_iters if iters is None else int(iters), pad_mode
+
+
+def _engine(model, n_iters, pad_mode):
+    return RaftEngine(model._params, small=model.small, iters=n_iters, device=model.device, volume_free=model.volume_free,
+                      upstream=model.upstream, mixed_precision=model.mixed_precision, pad_mode=pad_mode)
+
+
+def evaluate(model, root, dataset="sintel", dstypes=DSTYPES, batch=1, workers=4, iters=None, warm_start=False):
     """Upstream RAFT's validation of a loaded networks.RAFT.RAFT model on a Sintel or KITTI-2015 training tree.
 
     The engine is built from the model's configuration (small, upstream, mixed_precision, volume_free, device, weights)
     with the protocol's iterations (iters overrides them) and padding.  Frames go in RGB with upstream=True and BGR
     otherwise, like the CLI.  A model with input_size is refused: validation runs frames at their own size.  Returns
     {"dataset", "iters", "pad_mode", "splits": {name: aggregate(...)}} with the splits 'clean' / 'final' (Sintel, those in
-    dstypes) or 'kitti'; the same for every batch and workers."""
-    if dataset not in PROTOCOLS:
-        raise ValueError(f"dataset must be one of {tuple(PROTOCOLS)} (got {dataset!r})")
-    if getattr(model, "input_size", None) is not None:
-        raise ValueError("evaluate: validation runs frames at their own size; build the model without input_size")
-    if int(batch) < 1 or int(workers) < 0:
-        raise ValueError(f"evaluate: batch must be >= 1 and workers >= 0 (got {batch}, {workers})")
-    if model._params is None:
-        raise RuntimeError("RAFT.load(<npz>) must be called before evaluate")
-    kitti = dataset == "kitti"
-    splits = ("kitti",) if kitti else tuple(dstypes)
-    if not kitti and (not splits or any(d not in DSTYPES for d in splits)):
-        raise ValueError(f"Sintel dstypes must be a non-empty subset of {DSTYPES} (got {dstypes!r})")
-    n_iters, pad_mode = PROTOCOLS[dataset]
-    n_iters = n_iters if iters is None else int(iters)
+    dstypes) or 'kitti'; the same for every batch and workers.
+
+    warm_start (Sintel only; an extension, upstream validates cold): every scene runs as a chain, each pair after the
+    first starting from forward_interpolate of the previous pair's 1/8-resolution flow, as in upstream's
+    create_sintel_submission(warm_start=True) -- the way to measure what the warm start does against ground truth."""
+    kitti, splits, n_iters, pad_mode = _setup(model, dataset, dstypes, batch, workers, iters, warm_start, "evaluate")
     lists = {s: kitti_pairs(root) if kitti else sintel_pairs(root, s) for s in splits}  # every file checked up front
-    engine = RaftEngine(model._params, small=model.small, iters=n_iters, device=model.device, volume_free=model.volume_free,
-                        upstream=model.upstream, mixed_precision=model.mixed_precision, pad_mode=pad_mode)
+    engine = _engine(model, n_iters, pad_mode)
     res = {"dataset": dataset, "iters": n_iters, "pad_mode": pad_mode, "splits": {}}
     for s, pairs in lists.items():
-        res["splits"][s] = aggregate(pairs, _run(engine, pairs, kitti, int(batch), int(workers), model.upstream), kitti)
+        stats = _run(engine, pairs, kitti, int(batch), int(workers), model.upstream, warm=bool(warm_start))
+        res["splits"][s] = aggregate(pairs, stats, kitti)
     return res
+
+
+# ---- test-split submissions ---------------------------------------------------------------------------------------
+TestPair = namedtuple("TestPair", "image1 image2 out")
+
+
+def sintel_test_pairs(root, dstype="clean"):
+    """MPI-Sintel test pairs of one pass, scene by scene in sorted order: the k-th frame (sorted) of
+    <root>/test/<dstype>/<scene>/ with the next one, written to <dstype>/<scene>/frame%04d.flo % (k + 1) (upstream's
+    create_sintel_submission)."""
+    if dstype not in DSTYPES:
+        raise ValueError(f"Sintel dstype must be one of {DSTYPES} (got {dstype!r})")
+    img_root = os.path.join(root, "test", dstype)
+    pairs = []
+    for scene in _listdir(img_root, "Sintel test"):
+        sdir = os.path.join(img_root, scene)
+        if not os.path.isdir(sdir):
+            continue
+        frames = [f for f in sorted(os.listdir(sdir)) if f.endswith(".png")]
+        for k, (a, b) in enumerate(zip(frames[:-1], frames[1:])):
+            pairs.append(TestPair(os.path.join(sdir, a), os.path.join(sdir, b),
+                                  os.path.join(dstype, scene, "frame%04d.flo" % (k + 1))))
+    if not pairs:
+        raise FileNotFoundError(f"Sintel: no frame pairs under {img_root}")
+    return pairs
+
+
+def kitti_test_pairs(root):
+    """KITTI-2015 test pairs in sorted id order: <root>/testing/image_2/<id>_10.png with <id>_11.png, written to
+    <id>_10.png (upstream's create_kitti_submission).  A missing second frame raises FileNotFoundError naming it."""
+    img_root = os.path.join(root, "testing", "image_2")
+    images = set(_listdir(img_root, "KITTI test"))
+    pairs = []
+    for f in sorted(images):
+        if not f.endswith("_10.png"):
+            continue
+        second = f[:-len("_10.png")] + "_11.png"
+        if second not in images:
+            raise FileNotFoundError(f"KITTI: second frame {os.path.join(img_root, second)} is missing")
+        pairs.append(TestPair(os.path.join(img_root, f), os.path.join(img_root, second), f))
+    if not pairs:
+        raise FileNotFoundError(f"KITTI: no frame pairs under {img_root}")
+    return pairs
+
+
+def submit(model, root, dataset, out, dstypes=DSTYPES, batch=1, workers=4, iters=None, warm_start=False):
+    """Upstream RAFT's create_sintel_submission / create_kitti_submission for a loaded networks.RAFT.RAFT model: the flow
+    of every test pair, at the frames' own size, in pixels (raft-small's reference-semantics flow is scaled by 8, exactly),
+    with the protocol's iterations and padding as in evaluate.  Sintel: <out>/<dstype>/<scene>/frame%04d.flo (write_flo);
+    KITTI: <out>/<id>_10.png (write_kitti_flow, upstream's 16-bit PNG).  warm_start (Sintel only): each scene as a chain
+    warm-started by forward_interpolate, as upstream's warm_start=True.  The files are the same bytes for every batch and
+    workers.  Returns the paths written, in dataset order."""
+    from flow_utils import write_flo, write_kitti_flow
+    kitti, splits, n_iters, pad_mode = _setup(model, dataset, dstypes, batch, workers, iters, warm_start, "submit")
+    lists = {s: kitti_test_pairs(root) if kitti else sintel_test_pairs(root, s) for s in splits}
+    engine = _engine(model, n_iters, pad_mode)
+    rgb, scale, written = model.upstream, np.float32(engine.flow_scale), []
+    for s, pairs in lists.items():
+        for row, flow, _ in _steps(engine, pairs, chains_of(pairs, warm_start), lambda p: _decode_frames(p, rgb),
+                                   int(batch), int(workers), bool(warm_start), False):
+            host = flow.cpu().numpy()
+            for k, i in enumerate(row):
+                if i is None:
+                    continue
+                path = os.path.join(out, pairs[i].out)
+                os.makedirs(os.path.dirname(path), exist_ok=True)
+                (write_kitti_flow if kitti else write_flo)(path, host[k] * scale)
+        written += [os.path.join(out, p.out) for p in pairs]
+    return written
 
 
 def summary_lines(res):
