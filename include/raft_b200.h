@@ -318,6 +318,25 @@ int rb_flow_forward_interpolate_workspace_bytes(int B, int h, int w, size_t* byt
 int rb_flow_forward_interpolate(const float* flow, float* out, int B, int h, int w, void* workspace,
                                 size_t workspace_bytes, void* stream);
 
+/* ---- F11: flow colour coding -- flow_utils.flow_to_color (the reference's flow_utils.py:95-121), batched ----------
+ * flow: [B,H,W,2] fp32; out: [B,H,W,3] uint8, RGB, or BGR with convert_to_bgr.  Each sample on its own: with clip,
+ * (u, v) = min(max((u, v), 0), clip_flow) first (the reference's np.clip(flow, 0, clip): negative components become 0).
+ * Per pixel, each operation rounded on its own (no FMA contraction), in numpy's types for a float32 flow:
+ *   fp32  rad = sqrt(u^2 + v^2); den = fl32(max_b rad + 1e-5f); u' = u / den, v' = v / den; r = sqrt(u'^2 + v'^2);
+ *         a = fl32(atan2((double)-v', (double)-u')) / fl32(pi); fk = ((a + 1) / 2) * 54 + 1;
+ *         k0 = min(floor(fk), 53), k1 = k0 + 1 (55 -> 1);
+ *   fp64  f = fk - k0; col = (1 - f) * (wheel[k0] / 255.0) + f * (wheel[k1] / 255.0);
+ *         col = r <= 1 ? 1 - r * (1 - col) : col * 0.75; out = floor(255 * col).
+ * wheel is make_colorwheel() (55 rows).  The one difference from numpy is arctan2, computed in fp64 and rounded once to
+ * fp32 (numpy's float32 arctan2 is not correctly rounded and depends on the machine).  Indices are clamped into the
+ * wheel, so non-finite flows read nothing out of bounds (their colours are unspecified).  The maximum radius is reduced
+ * per sample in fixed chunks into the workspace (rb_flow_to_color_workspace_bytes) by a first launch; a batch gives the
+ * per-sample bits, no allocation, no synchronisation, graph-capturable.  Null pointers, B/H/W <= 0, a non-finite
+ * clip_flow with clip, B > 65535 and a workspace that is too small -> RB_ERR_* before any CUDA call. */
+int rb_flow_to_color_workspace_bytes(int B, int H, int W, size_t* bytes);
+int rb_flow_to_color(const float* flow, int B, int H, int W, int clip, float clip_flow, int convert_to_bgr, uint8_t* out,
+                     void* workspace, size_t workspace_bytes, void* stream);
+
 /* ---- F3 (input edge): dataflow/test_dataflow.py:56-61,96-97 + the SURVEY 8(d) shape policy ------------------
  * src: [B,H,W,3] device frames, BGR like cv2.imdecode -- fp32 in [0,1] (src_is_u8 = 0) or uint8 in [0,255]
  * (src_is_u8 = 1: x/255.0f, the reference's np.float32(x)/255.0, bit for bit).  dst: [B,H+pt+pb,W+pl+pr,3] fp32

@@ -29,6 +29,12 @@ the validation, which upstream runs cold).  --split test writes upstream's test-
 
 Sintel: ``<out>/<dstype>/<scene>/frameNNNN.flo``; KITTI (no --warm-start): ``<out>/<id>_10.png``, 16-bit PNGs
 (raft_b200.evaluate.submit).
+
+--path DIR (upstream demo.py's flag): the flow of every consecutive pair of DIR's sorted *.png / *.jpg frames, written as
+``<--out>/flow_<k:06d>.png`` (and ``flow_<k:06d>.flo`` / ``.npy`` under the directories --flo / --npy name), each frame
+encoded once, --batch pairs per pass, coloured on the GPU (raft_b200.video):
+
+    python infer_raft.py --path frames/ --out flows/ --load raft-things.npz [--batch 8 | --warm-start]
 """
 import argparse
 import os
@@ -72,7 +78,8 @@ def parser():
     p.add_argument('--load', default='release_weight/raft-things.npz', help='npz checkpoint keyed by TF variable names')
     p.add_argument('-m', '--mode', default='test', choices=['train', 'val', 'test', 'export', 'flops'])
     p.add_argument('--out', default='./log', help='-m val: where val_<dataset>.json is written')
-    p.add_argument('--batch', default=1, type=int, help='-m val: frame pairs per engine pass (test mode runs one pair)')
+    p.add_argument('--batch', default=1, type=int,
+                   help='-m val and --path: frame pairs per engine pass (test mode runs one pair)')
     p.add_argument('-o', '--optimizer', default='adam', choices=['adam', 'adamw', 'sgd', 'sgd_cyclic', 'sgd_1cycle'])
     p.add_argument('--im1', default='frame_0010.png')
     p.add_argument('--im2', default='frame_0011.png')
@@ -82,15 +89,18 @@ def parser():
     p.add_argument('--dataset', default=None, choices=['sintel', 'kitti'], help='-m val: which training set --data holds')
     p.add_argument('--dstype', nargs='+', default=['clean', 'final'], choices=['clean', 'final'],
                    help='-m val, Sintel: the passes to evaluate')
-    p.add_argument('--workers', type=int, default=4, help='-m val: frame-decoding threads')
+    p.add_argument('--workers', type=int, default=4, help='-m val and --path: frame-decoding (and writing) threads')
     p.add_argument('--split', default='training', choices=['training', 'test'],
                    help='-m val: validate on the training split, or write the test-split submission under --out')
     p.add_argument('--warm-start', action='store_true',
-                   help="-m val, Sintel: warm-start each pair from the previous pair's flow in its scene (upstream's "
-                        "warm_start=True)")
+                   help="-m val, Sintel, and --path: warm-start each pair from the previous pair's flow (in its scene; "
+                        "upstream's warm_start=True)")
     p.add_argument('--keep-size', action='store_true', help='extension: pad to a multiple of 8 instead of resizing to 432x1024')
-    p.add_argument('--npy', default=None, help='extension: also save the raw [H,W,2] flow')
-    p.add_argument('--flo', default=None, help='extension: also save the flow as a Middlebury .flo file')
+    p.add_argument('--npy', default=None, help='extension: also save the raw [H,W,2] flow (--path: a directory)')
+    p.add_argument('--flo', default=None, help='extension: also save the flow as a Middlebury .flo file (--path: a directory)')
+    p.add_argument('--path', default=None,
+                   help="extension (upstream demo.py): a directory of frames; the flow of every consecutive pair is "
+                        "written as <--out>/flow_<k:06d>.png")
     p.add_argument('--bidirectional', action='store_true',
                    help='extension: also the backward flow and the forward-backward occlusion masks')
     p.add_argument('--interpolate', type=float, nargs='+', default=None, metavar='T',
@@ -120,6 +130,15 @@ def main(argv=None):
     if args.mode != 'test':
         print(f"mode '{args.mode}' has no implementation in the reference either (infer_raft.py:71-95); nothing to do")
         return 0
+    if args.path is not None:
+        if args.bidirectional or args.interpolate:
+            p.error('--path runs forward flow over a frame sequence; it cannot be combined with --bidirectional or '
+                    '--interpolate')
+        if args.warm_start and args.batch != 1:
+            p.error('--path --warm-start warm-starts each pair from the one before: it runs one pair per pass (--batch 1)')
+        if args.batch < 1 or args.workers < 0:
+            p.error('--path needs --batch >= 1 and --workers >= 0')
+        return run_video(args)
     from networks import RAFT
     import cv2
     from flow_utils import flow_to_color, resize_flow, write_flo
@@ -165,6 +184,21 @@ def main(argv=None):
         for k, frame in enumerate(frames):
             img = np.clip(np.rint(255.0 * frame[0]), 0, 255).astype(np.uint8)
             cv2.imwrite(f"raft_interp_{k}.png", cv2.cvtColor(img, cv2.COLOR_RGB2BGR) if rgb else img)
+    return 0
+
+
+def run_video(args):
+    """--path: raft_b200.video over the frames of --path, at 432x1024 like test mode (or their own size with --keep-size)."""
+    from networks import RAFT
+    from raft_b200.video import video
+    iters = 20 if args.iters is None else args.iters
+    size = None if args.keep_size else (432, 1024)
+    model = RAFT.RAFT(None if size is None else size + (3,), args, iters=iters, input_size=size, upstream=args.upstream,
+                      mixed_precision=args.mixed_precision).load(args.load)
+    files = video(model, args.path, args.out, batch=args.batch, workers=args.workers, warm_start=args.warm_start,
+                  flo=args.flo, npy=args.npy, native_flow=args.native_flow)
+    print(f"{len(files)} files written under {args.out}" + (" and the --flo / --npy directories" if args.flo or args.npy
+                                                            else ""))
     return 0
 
 

@@ -118,6 +118,24 @@ class RAFT(object):
         return tuple(t.clone() for t in out) if return_low else out.clone()
 
     @torch.no_grad()
+    def forward_sequence(self, frames, carry=False, flow_init=None, return_low=False):
+        """Extension (video): the flows between consecutive frames of [T+1,H,W,3] frames (dtypes and sources as for
+        ``forward``) -> fresh [T,H,W,2] flows, pair k bit-identical to ``forward(frames[k:k+1], frames[k+1:k+2])``, with
+        every frame encoded once.  carry=True continues the previous call with [T,H,W,3] new frames: the first pair
+        starts from that call's last frame, whose features are reused (RaftEngine.forward_sequence); it raises ValueError
+        without such a call, when T, the frame size, the dtype or the upstream / mixed-precision settings differ, or when a
+        call at another frame size came in between.  flow_init ([T,h,w,2]) and return_low as in ``forward``."""
+        eng = self._engine
+        if eng is not None and (eng.upstream, eng.mixed_precision) != (self.upstream, self.mixed_precision):
+            if carry:
+                raise ValueError("forward_sequence: carry=True after the upstream / mixed_precision settings changed")
+            self._engine = None  # the settings changed since the engine was built: build it again
+        if flow_init is not None and not isinstance(flow_init, torch.Tensor):
+            flow_init = torch.as_tensor(np.asarray(flow_init))
+        out = self.engine().forward_sequence(_as_tensor(frames), carry=carry, flow_init=flow_init, return_low=return_low)
+        return tuple(t.clone() for t in out) if return_low else out.clone()
+
+    @torch.no_grad()
     def forward_bidirectional(self, input_left, input_right, check=True):
         """Extension (frame interpolation needs flow both ways): the flows left -> right and right -> left of the same
         frames, each frame encoded once and both directions run as one batch.  Inputs as for ``forward``.  Returns fresh

@@ -101,6 +101,28 @@ def forward_interpolate(flow):
     return out
 
 
+def flow_to_color(flow, clip_flow=None, convert_to_bgr=False):
+    """flow_utils.flow_to_color (the reference's flow_utils.py:95-121) on a batch of CUDA flows (rb_flow_to_color): each
+    [H,W,2] sample of the [B,H,W,2] fp32 flow coloured by the Middlebury wheel, normalised by its own maximum radius.
+    Returns a fresh [B,H,W,3] uint8 tensor, RGB or BGR with convert_to_bgr.  Equal to the host function wherever numpy's
+    float32 arctan2 is correctly rounded; the kernel rounds the fp64 atan2 to fp32 instead (DESIGN §4)."""
+    if not (isinstance(flow, torch.Tensor) and flow.is_cuda and flow.dim() == 4 and flow.shape[-1] == 2
+            and flow.dtype == torch.float32):
+        raise ValueError(f"flow_to_color: flow must be a [B,H,W,2] float32 CUDA tensor (got "
+                         f"{getattr(flow, 'shape', None)} {getattr(flow, 'dtype', type(flow))})")
+    f = flow.contiguous()
+    B, H, W, _ = f.shape
+    out = torch.empty(B, H, W, 3, dtype=torch.uint8, device=f.device)
+    clip = clip_flow is not None
+    with torch.cuda.device(f.device):
+        nbytes = capi.size_query(capi.lib.rb_flow_to_color_workspace_bytes, B, H, W)
+        ws = torch.empty(nbytes, dtype=torch.uint8, device=f.device)
+        capi.check(capi.lib.rb_flow_to_color(capi.ptr(f), B, H, W, int(clip), float(clip_flow) if clip else 0.0,
+                                             int(bool(convert_to_bgr)), capi.ptr(out), capi.ptr(ws), nbytes,
+                                             capi.stream()))
+    return out
+
+
 def reverse_flow(flow, time_step=1.0, bg=None, im0=None):
     """The reference's flow_utils.py:166 reverse_flow_avg_skip_static on a batch of CUDA flows (rb_flow_reverse, bit for
     bit): projects the [B,H,W,2] flow 0 -> 1 to time `time_step` and returns the flow from there back to frame 0.

@@ -9,6 +9,9 @@ interpolate runs the same bidirectional pass (without the check) from its own gr
 and the frame blend (rb_flow_reverse, rb_frame_synthesize, csrc/interp.cu) eagerly on the same stream.
 forward(flow_init=..., return_low=True) is upstream's warm start: the same graph with rb_coords_init in place of
 rb_coords_grid and rb_coords_to_flow (flow_low) after the loop, captured as a mode of its own (FORWARD_WARM).
+forward_sequence(frames) is video: T + 1 frames give the T flows f_k -> f_(k+1), fnet once per frame, fmap1 = fmaps[:T] and
+fmap2 = fmaps[1:] as overlapping views (SEQUENCE); carry=True continues from the previous call's last frame, whose image
+and feature map the graph copies to row 0 before it encodes only the T new frames.
 With input_size set, every mode first resizes the frames to that size like the reference's cv2.resize (rb_frames_resize,
 csrc/resize.cu, in the graph in place of rb_frames_prepare), and its outputs come back at that size.
 """
@@ -26,8 +29,9 @@ from .weights import pack_update_block
 
 # what one pass computes: L->R only (forward), both directions (forward_bidirectional), both plus the occlusion check,
 # both directions for interpolate (which also holds the buffers of the per-t calls), L->R warm-started from flow_init with
-# the 1/8-resolution flow kept (forward(flow_init=..., return_low=True))
-FORWARD, BIDIRECTIONAL, BIDIRECTIONAL_CHECK, INTERPOLATE, FORWARD_WARM = 0, 1, 2, 3, 4
+# the 1/8-resolution flow kept (forward(flow_init=..., return_low=True)), T consecutive pairs of T + 1 frames, always
+# started from flow_init (forward_sequence)
+FORWARD, BIDIRECTIONAL, BIDIRECTIONAL_CHECK, INTERPOLATE, FORWARD_WARM, SEQUENCE = 0, 1, 2, 3, 4, 5
 # forward-backward consistency thresholds of UnFlow (Meister et al. 2018): |f+b|^2 > a1 (|f|^2 + |b|^2) + a2
 FB_ALPHA1, FB_ALPHA2 = 0.01, 0.5
 # smallest frame side: the 4-level correlation pyramid needs a 1/8-resolution grid of at least 8 (level 3 is grid >> 3),
@@ -39,11 +43,25 @@ MIN_FRAME_UPSTREAM = 121
 PAD_MODES = ("sintel", "kitti")
 
 
+def _kept(parked, key):
+    """Whether a call keyed `key` = (B, H, W, u8, mode) keeps the parked buffers of `parked`.  The pair modes keep each
+    other at one (B, H, W, u8), as before; the sequence buffers survive any pair-mode call at the same frame size (a carry
+    continues across them), and a sequence call keeps the pair modes' buffers at its frame size and dtype.  A sequence
+    call of another T or dtype replaces the sequence buffers."""
+    if parked[4] == SEQUENCE and key[4] == SEQUENCE:
+        return parked == key
+    if parked[4] == SEQUENCE:
+        return parked[1:3] == key[1:3]
+    if key[4] == SEQUENCE:
+        return parked[1:4] == key[1:4]
+    return parked[:4] == key[:4]
+
+
 class RaftEngine:
     # everything _ensure allocates for one (B, H, W, u8, mode); parked per mode so alternating modes re-captures nothing
     _STATE = ("_key", "src_hw", "pad", "h", "w", "Hp", "Wp", "pairs", "pyr_bytes", "pyramid", "cws_bytes", "corr_ws",
               "ws_bytes", "ws", "coords1", "mask", "flow_up", "occ", "rev_ws_bytes", "rev_ws", "flow_t", "empty_t", "flow_init", "flow_low", "fmaps", "fmap1", "fmap2", "cmap", "images", "staged", "raw",
-              "_shape", "_graph")
+              "seq_enc", "_shape", "_graph", "_graph_carry")
 
     def __init__(self, params: Dict[str, np.ndarray], small: bool = False, iters: int = 20,
                  device: Optional[torch.device] = None, use_graph: bool = True, math_mode: int = capi.RB_MATH_TC,
@@ -100,6 +118,10 @@ class RaftEngine:
         self._shape = None  # (B, H, W, u8, mode) at the size the network runs (input_size when set)
         self._key = None    # (B, H, W, u8, mode) at the frames' own size
         self._graph = None
+        self._graph_carry = None  # SEQUENCE: the graph of carry=True calls (self._graph runs the fresh ones)
+        self._carry = False       # the SEQUENCE pass being run continues from the previous one
+        self._seq_last = None     # (T, H, W, u8, SEQUENCE) of the last forward_sequence call: what carry=True continues
+        self.seq_enc = None
         self._parked = {}  # _key -> buffers and graph of the other modes at the current frame size
         self._enc_stream = None   # forked stream of the context encoder (encode())
         self._capture_stream = None  # CUDA-graph capture stream on this engine's device (run())
@@ -133,11 +155,12 @@ class RaftEngine:
         # alternating modes on one frame size keeps every mode's buffers and CUDA graph; a new frame size drops them
         if self._key is not None:
             self._parked[self._key] = {k: getattr(self, k) for k in self._STATE}
-        self._parked = {k: v for k, v in self._parked.items() if k[:4] == key[:4]}
+        self._parked = {k: v for k, v in self._parked.items() if _kept(k, key)}
         if key in self._parked:
             self.__dict__.update(self._parked.pop(key))
             return
-        bidir = mode not in (FORWARD, FORWARD_WARM)
+        bidir = mode not in (FORWARD, FORWARD_WARM, SEQUENCE)
+        seq = mode == SEQUENCE
         NB = 2 * B if bidir else B  # frame pairs through the hot path
         ph, pw = (-H) % 8, (-W) % 8
         top = 0 if self.pad_mode == "kitti" else ph // 2
@@ -168,23 +191,32 @@ class RaftEngine:
             self.empty_t = torch.empty(2, 2, B, H, W, dtype=torch.uint8, device=d)  # [empty | multi]
         else:
             self.rev_ws_bytes, self.rev_ws, self.flow_t, self.empty_t = 0, None, None, None
-        if mode == FORWARD_WARM:  # the caller's initial flow (copied in before each replay) and the final 1/8-res flow
+        if mode in (FORWARD_WARM, SEQUENCE):  # the caller's initial flow (copied in before each replay), the final 1/8-res flow
             self.flow_init = torch.zeros(B, h, w, 2, dtype=torch.float32, device=d)
             self.flow_low = torch.empty(B, h, w, 2, dtype=torch.float32, device=d)
         else:
             self.flow_init, self.flow_low = None, None
-        self.fmaps = torch.empty(NB + B, h, w, self.fdim, dtype=torch.float32, device=d)
-        self.fmap1, self.fmap2 = self.fmaps[:NB], self.fmaps[B:]
+        # SEQUENCE: B = T pairs of T + 1 frames; fmap1 = fmaps[:T] and fmap2 = fmaps[1:] overlap, no copy
+        nframes = B + 1 if seq else 2 * B
+        self.fmaps = torch.empty(nframes if seq else NB + B, h, w, self.fdim, dtype=torch.float32, device=d)
+        self.fmap1, self.fmap2 = self.fmaps[:NB], self.fmaps[1 if seq else B:]
         self.cmap = torch.empty(NB, h, w, self.hidden + self.ctx, dtype=torch.float32, device=d)
-        self.images = torch.empty(2 * B, Hp, Wp, 3, dtype=torch.float32, device=d)  # [left | right], [0,1], padded
+        self.images = torch.empty(nframes, Hp, Wp, 3, dtype=torch.float32, device=d)  # [left | right], [0,1], padded
         # staging buffer of the raw frames (uint8 or unpadded fp32, at the frames' own size); fp32 frames that need no
-        # resize and no padding go straight into self.images
-        self.staged = bool(u8 or ph or pw or self.input_size is not None)
-        self.raw = torch.empty(2 * B, *src_hw, 3, dtype=torch.uint8 if u8 else torch.float32, device=d) if self.staged else None
+        # resize and no padding go straight into self.images -- except in SEQUENCE, whose carry graph reads the previous
+        # call's last frame from self.images, so the new frames must not land there before the replay
+        self.staged = bool(u8 or ph or pw or self.input_size is not None or seq)
+        self.raw = torch.empty(nframes, *src_hw, 3, dtype=torch.uint8 if u8 else torch.float32, device=d) if self.staged else None
+        # SEQUENCE: the feature encoder sees T + 1 frames in the fresh graph and T in the carry graph, the context encoder T;
+        # encoders with workspaces of their own keep the pointers each graph was captured with (CudaEncoder reallocates its
+        # workspace when its batch changes), whatever the other modes run in between
+        self.seq_enc = ((self.fnet.with_own_workspace(), self.fnet.with_own_workspace(), self.cnet.with_own_workspace())
+                        if seq else None)
         self.src_hw = src_hw
         self._key = key
         self._shape = (B, H, W, u8, mode)
         self._graph = None
+        self._graph_carry = None
 
     # ---- stages --------------------------------------------------------------------------------
     def encode(self, defer_join: bool = False):
@@ -198,16 +230,27 @@ class RaftEngine:
         Bidirectional modes: cnet runs on all 2B frames (the R->L pairs need the context of R), and the last B feature
         maps are a device-to-device copy of the first B (a copy-engine transfer, no kernel)."""
         B, H, W, u8, mode = self._shape
-        bidir = mode not in (FORWARD, FORWARD_WARM)
+        bidir = mode not in (FORWARD, FORWARD_WARM, SEQUENCE)
         cnet, cframes = (self.cnet_bidir, self.images) if bidir else (self.cnet, self.images[:B])
-        fout = self.fmaps[:2 * B]  # [fL | fR]
+        fnet, fout = self.fnet, self.fmaps[:2 * B]  # [fL | fR]
+        raw, images = self.raw, self.images
         capi.check(capi.lib.rb_set_math_mode(self.math_mode))  # per-thread library state: set before ANY kernel of ours
         capi.check(capi.lib.rb_set_semantics(self.semantics))
+        if mode == SEQUENCE:  # B = T pairs; the T + 1 frames all staged in self.raw
+            fnet_fresh, fnet_carry, cnet = self.seq_enc
+            if self._carry:  # the previous call's last frame becomes frame 0; only the T new frames are encoded
+                self.images[0].copy_(self.images[B])
+                self.fmaps[0].copy_(self.fmaps[B])
+                raw, images = self.raw[1:], self.images[1:]
+                fnet, fout = fnet_carry, self.fmaps[1:]
+            else:
+                fnet, fout = fnet_fresh, self.fmaps
+        n = images.shape[0]
         if self.input_size is not None:  # F3: cv2 resize, u8 -> fp32 /255 and replicate padding in one pass (csrc/resize.cu)
-            capi.check(capi.lib.rb_frames_resize(capi.ptr(self.raw), int(u8), capi.ptr(self.images), 2 * B, *self.src_hw,
+            capi.check(capi.lib.rb_frames_resize(capi.ptr(raw), int(u8), capi.ptr(images), n, *self.src_hw,
                                                  H, W, *self.pad, capi.stream()))
         elif self.staged:  # F3: u8 -> fp32 /255 and replicate padding in one pass (csrc/frames.cu)
-            capi.check(capi.lib.rb_frames_prepare(capi.ptr(self.raw), int(u8), capi.ptr(self.images), 2 * B, H, W,
+            capi.check(capi.lib.rb_frames_prepare(capi.ptr(raw), int(u8), capi.ptr(images), n, H, W,
                                                   *self.pad, capi.stream()))
         main = torch.cuda.current_stream(self.device)
         if self._enc_stream is None:
@@ -216,7 +259,7 @@ class RaftEngine:
         side.wait_stream(main)  # fork: the frames are in place
         with torch.cuda.stream(side):
             cnet(cframes, out=self.cmap)
-        self.fnet(self.images, out=fout)
+        fnet(images, out=fout)
         self._cnet_pending = True
         if bidir:
             self.fmaps[2 * B:].copy_(self.fmaps[:B])  # contiguous, same dtype: cudaMemcpyAsync on the current stream
@@ -242,7 +285,7 @@ class RaftEngine:
                                          self.fdim, capi.ptr(self.corr_ws), self.cws_bytes, st))
         self._join_cnet()  # cmap (context encoder, forked stream) is first needed here
         capi.check(lib.rb_update_set_state_cnet(s, capi.ptr(self.blob), capi.ptr(self.ws), capi.ptr(self.cmap), B, h, w, st))
-        if mode == FORWARD_WARM:  # coords1 = grid + flow_init (upstream RAFT.forward)
+        if self.flow_init is not None:  # coords1 = grid + flow_init (upstream RAFT.forward)
             capi.check(lib.rb_coords_init(capi.ptr(self.coords1), capi.ptr(self.flow_init), B, h, w, st))
         else:
             capi.check(lib.rb_coords_grid(capi.ptr(self.coords1), B, h, w, st))
@@ -256,7 +299,7 @@ class RaftEngine:
         else:
             capi.check(lib.rb_raft_iterate(s, capi.ptr(self.blob), capi.ptr(self.ws), capi.ptr(self.pyramid),
                                            capi.ptr(self.coords1), capi.ptr(self.mask), B, h, w, self.iters, st))
-        if mode == FORWARD_WARM:
+        if self.flow_init is not None:
             capi.check(lib.rb_coords_to_flow(capi.ptr(self.coords1), capi.ptr(self.flow_low), B, h, w, st))
         top, left = self.pad[0], self.pad[2]  # crop the padding away while upsampling
         if self.small:
@@ -287,7 +330,8 @@ class RaftEngine:
         if not self.use_graph:
             self._all()
             return
-        if self._graph is None:
+        attr = "_graph_carry" if self._carry else "_graph"
+        if getattr(self, attr) is None:
             self._all()  # warm-up: function attributes, tensor-map cache
             torch.cuda.synchronize()
             g = torch.cuda.CUDAGraph()
@@ -298,8 +342,10 @@ class RaftEngine:
                 self._capture_stream = torch.cuda.Stream(device=self.device)
             with torch.cuda.graph(g, stream=self._capture_stream):
                 self._all()
-            self._graph = g
-        self._graph.replay()
+            setattr(self, attr, g)
+            if self._carry:  # the warm-up ran this pass; a replay would carry from the frame it has just encoded
+                return
+        getattr(self, attr).replay()
 
     @torch.no_grad()
     def forward(self, left: torch.Tensor, right: torch.Tensor, flow_init: Optional[torch.Tensor] = None,
@@ -325,6 +371,66 @@ class RaftEngine:
             raise ValueError(f"raft_b200: flow_init must be a float32 torch tensor (got "
                              f"{getattr(flow_init, 'dtype', type(flow_init))})")
         self._run_frames(left, right, FORWARD_WARM, flow_init)
+        return (self.flow_low, self.flow_up) if return_low else self.flow_up
+
+    @torch.no_grad()
+    def forward_sequence(self, frames: torch.Tensor, carry: bool = False, flow_init: Optional[torch.Tensor] = None,
+                         return_low: bool = False):
+        """Video: the flows between consecutive frames.  frames is [T+1,H,W,3] (dtypes, sizes, input_size and padding as
+        for forward()); the call returns the [T,H,W,2] flows f_k -> f_(k+1), each bit-identical to forward(f_k, f_(k+1)).
+        The feature encoder runs once per frame (fmap1 = fmaps[:T] and fmap2 = fmaps[1:] are overlapping views), the
+        context encoder on the first T frames, the hot path on T pairs.
+
+        carry=True continues the previous forward_sequence call: frames is [T,H,W,3], T new frames after that call's last
+        frame, giving the T pairs (last, g_0), (g_0, g_1), ...; the graph copies the last frame's image and feature map to
+        row 0 on the device and encodes only the new frames, so a stream of clips encodes every frame once, at any T.  It
+        raises ValueError without a preceding sequence call, when T, the frame size or the dtype differ from it, or when a
+        call at another frame size released the buffers in between (pair-mode calls at the same size do not).
+
+        Every sequence pass starts from coords = grid + flow_init ([T,h,w,2] on the padded 1/8-resolution grid, row i for
+        pair i; zeros when None, which is the cold start bit for bit), so cold and warm calls share the graphs.  With
+        return_low the call returns (flow_low, flow_up) as forward() does.  The returned tensors are engine-owned buffers,
+        overwritten by the next call; one buffer set serves the fresh and the carry graph."""
+        if not (isinstance(frames, torch.Tensor) and frames.dim() == 4 and frames.shape[-1] == 3
+                and frames.dtype in (torch.uint8, torch.float32)):
+            raise ValueError(f"raft_b200: frames must be a [N,H,W,3] uint8 or float32 tensor (got "
+                             f"{getattr(frames, 'shape', None)} {getattr(frames, 'dtype', type(frames))})")
+        T = frames.shape[0] if carry else frames.shape[0] - 1
+        if T < 1:
+            raise ValueError(f"raft_b200: forward_sequence needs {'one new frame' if carry else 'two frames'} at least "
+                             f"(got {frames.shape[0]})")
+        if flow_init is not None and (not isinstance(flow_init, torch.Tensor) or flow_init.dtype != torch.float32):
+            raise ValueError(f"raft_b200: flow_init must be a float32 torch tensor (got "
+                             f"{getattr(flow_init, 'dtype', type(flow_init))})")
+        key = (T, frames.shape[1], frames.shape[2], frames.dtype == torch.uint8, SEQUENCE)
+        if carry:
+            last = self._seq_last
+            if last is None:
+                raise ValueError("raft_b200: carry=True continues a forward_sequence call; there is none before it")
+            for i, what in ((0, "T"), (slice(1, 3), "frame size"), (3, "dtype (uint8)")):
+                if last[i] != key[i]:
+                    raise ValueError(f"raft_b200: carry=True with another {what} than the previous sequence call "
+                                     f"({key[i]} after {last[i]})")
+            if key != self._key and key not in self._parked:
+                raise ValueError("raft_b200: carry=True after a call at another frame size released the sequence buffers")
+        with torch.cuda.device(self.device):
+            self._ensure(*key)
+            if flow_init is None:
+                self.flow_init.zero_()
+            elif tuple(flow_init.shape) != tuple(self.flow_init.shape):
+                raise ValueError(f"raft_b200: flow_init must be [T,h,w,2] = {list(self.flow_init.shape)} on the padded "
+                                 f"1/8-resolution grid (got {list(flow_init.shape)})")
+            else:
+                self.flow_init.copy_(flow_init, non_blocking=True)
+            (self.raw[1:] if carry else self.raw).copy_(frames, non_blocking=True)
+            self._carry = bool(carry)
+            try:
+                self.run()
+            finally:
+                self._carry = False
+            self._seq_last = key
+            if not self._range_checked:
+                self._check_range()
         return (self.flow_low, self.flow_up) if return_low else self.flow_up
 
     @torch.no_grad()

@@ -1,0 +1,200 @@
+"""F11: optical flow over a video -- upstream RAFT's demo.py (a directory of frames in, one flow visualisation per
+consecutive pair out) on RaftEngine.forward_sequence, with the colour coding on the GPU (rb_flow_to_color).
+
+    from raft_b200.video import video
+    video(RAFT((432, 1024, 3), args, input_size=(432, 1024)).load("raft-things.npz"), "frames/", "out/")
+
+writes out/flow_000000.png (frame 0 -> 1), out/flow_000001.png, ...; BGR like the single-pair CLI's PNG.
+
+Schedule (schedule()): the first pass is a fresh forward_sequence on batch + 1 frames, every later pass a carry call on
+batch new frames, so every frame is decoded, uploaded and encoded once.  A short last pass is padded by repeating the last
+frame; its extra rows are idle and their flows discarded, so one pair of CUDA graphs serves the whole video.  warm_start
+runs T = 1 carry passes, each started from forward_interpolate of the previous pass's flow_low (upstream's warm start).
+
+Pipeline, as in raft_b200.evaluate: worker threads decode the frames of the next passes (cv2 releases the GIL) into two
+pinned slots used in turn, each refilled only after the event behind its pass has completed; the colour images (and the
+flows, when written) are copied to two pinned output slots and PNG-encoded and written by writer threads.  The files are
+the same bytes for every workers value.
+"""
+from __future__ import annotations
+
+import glob
+import os
+from collections import namedtuple
+from concurrent.futures import ThreadPoolExecutor
+
+import numpy as np
+import torch
+
+from .evaluate import _imread
+
+# one forward_sequence call: carry or fresh, the frame indices it uploads (T + 1 fresh, T carry; a short last pass repeats
+# the last frame), and per flow row the pair index k (frame k -> k + 1) or None for an idle row
+Pass = namedtuple("Pass", "carry frames pairs")
+
+
+def list_frames(frames):
+    """The frame paths of a video: a directory's *.png and *.jpg files in sorted order (upstream demo.py's glob), or a list
+    of paths as given.  Fewer than two frames raise ValueError."""
+    if isinstance(frames, (str, os.PathLike)):
+        root = os.fspath(frames)
+        if not os.path.isdir(root):
+            raise FileNotFoundError(f"video: no directory {root}")
+        paths = sorted(glob.glob(os.path.join(root, "*.png")) + glob.glob(os.path.join(root, "*.jpg")))
+    else:
+        paths = [os.fspath(p) for p in frames]
+    if len(paths) < 2:
+        raise ValueError(f"video: a flow needs two frames at least (got {len(paths)})")
+    return paths
+
+
+def schedule(n_frames, batch, warm_start=False):
+    """The passes over n_frames frames with T = batch pairs per pass (T = 1 with warm_start): pass j covers the pairs
+    j T .. j T + T - 1, a fresh call on frames 0 .. T for j = 0 and a carry call on frames j T + 1 .. j T + T after it.
+    Frame indices past the last frame repeat it; their rows are idle (None)."""
+    if int(n_frames) < 2:
+        raise ValueError(f"video: a flow needs two frames at least (got {n_frames})")
+    if int(batch) < 1:
+        raise ValueError(f"video: batch must be >= 1 (got {batch})")
+    if warm_start and int(batch) != 1:
+        raise ValueError(f"video: warm_start runs one pair per pass, each warm-started from the one before; batch must be 1 "
+                         f"(got {batch})")
+    T, n_pairs, last = int(batch), int(n_frames) - 1, int(n_frames) - 1
+    passes = []
+    for j in range(-(-n_pairs // T)):
+        first = j * T + (1 if j else 0)
+        frames = [min(i, last) for i in range(first, j * T + T + 1)]
+        passes.append(Pass(j > 0, frames, [k if k < n_pairs else None for k in range(j * T, j * T + T)]))
+    return passes
+
+
+class _Slot:
+    """Pinned host staging (frames in, or colour images and flows out) and the event behind the last pass that used it;
+    futures: the writer tasks that still read it."""
+
+    def __init__(self, **shapes):
+        for name, (shape, dtype) in shapes.items():
+            setattr(self, name, torch.zeros(*shape, dtype=dtype).pin_memory())
+        self.event = None
+        self.futures = []
+
+    def wait(self):
+        for f in self.futures:
+            f.result()
+        self.futures = []
+        if self.event is not None:
+            self.event.synchronize()
+
+
+def video(model, frames, out, batch=8, workers=4, warm_start=False, flo=None, npy=None, native_flow=False):
+    """The flow between every pair of consecutive frames of a loaded networks.RAFT.RAFT model, written as
+    <out>/flow_<k:06d>.png for pair k (frame k -> k + 1; the GPU colour coding of networks.utils.flow_to_color, BGR), and
+    with flo / npy (directories) also as flow_<k:06d>.flo / .npy.  frames: a directory (its sorted *.png and *.jpg) or a
+    list of paths; all frames must have one size (a mismatch raises ValueError naming the first such file).  Frames go in
+    RGB with model.upstream and BGR otherwise, like the CLI.  batch pairs run per pass (schedule()); warm_start warm-starts
+    every pair from the previous one (batch must be 1).  native_flow resizes the flows of a model with input_size back to
+    the frames' size (networks.utils.resize_flow) before they are coloured or saved.  Each flow equals the model's
+    forward(f_k, f_(k+1)) (warm_start: the chain forward(..., flow_init=forward_interpolate(flow_low))) bit for bit.
+    Returns the written paths, pair by pair."""
+    import cv2
+    from flow_utils import write_flo
+    from networks.utils import flow_to_color, forward_interpolate, resize_flow
+
+    paths = list_frames(frames)
+    batch, workers = int(batch), int(workers)
+    if workers < 0:
+        raise ValueError(f"video: workers must be >= 0 (got {workers})")
+    passes = schedule(len(paths), batch, warm_start)
+    T = batch
+    dirs = {"png": os.fspath(out), "flo": None if flo is None else os.fspath(flo),
+            "npy": None if npy is None else os.fspath(npy)}
+    for d in dirs.values():
+        if d is not None:
+            os.makedirs(d, exist_ok=True)
+    keep_flow = flo is not None or npy is not None
+    engine = model.engine()
+    rgb = bool(model.upstream)
+    dev = engine.device
+
+    def name(k, ext):
+        return os.path.join(dirs[ext], f"flow_{k:06d}.{ext}")
+
+    def write(slot, rows):  # writer thread: the files of one pass, once its copies have landed
+        slot.event.synchronize()
+        for r, k in rows:
+            if not cv2.imwrite(name(k, "png"), slot.color[r].numpy()):
+                raise OSError(f"cannot write {name(k, 'png')}")
+            if flo is not None:
+                write_flo(name(k, "flo"), slot.flow[r].numpy())
+            if npy is not None:
+                np.save(name(k, "npy"), slot.flow[r].numpy())
+
+    decoders = ThreadPoolExecutor(workers) if workers > 0 else None
+    writers = ThreadPoolExecutor(workers) if workers > 0 else None
+    depth = max(1, -(-workers // T))  # passes decoded ahead of the one the GPU is given
+
+    def submit(j):
+        if decoders is None:
+            return [(i, lambda i=i: _imread(paths[i], rgb)) for i in passes[j].frames]
+        return [(i, decoders.submit(_imread, paths[i], rgb).result) for i in passes[j].frames]
+
+    written, shape, ins, outs, init = [], None, None, None, None
+    try:
+        with torch.cuda.device(dev):
+            stream = torch.cuda.current_stream(dev)
+            ahead = [submit(j) for j in range(min(depth, len(passes)))]
+            for j, ps in enumerate(passes):
+                loads = ahead.pop(0)
+                if j + depth < len(passes):
+                    ahead.append(submit(j + depth))
+                imgs = []
+                for i, load in loads:
+                    img = load()
+                    if shape is None:
+                        shape = img.shape
+                    elif img.shape != shape:
+                        raise ValueError(f"video: {paths[i]} is a {img.shape[0]}x{img.shape[1]} frame, {paths[0]} is "
+                                         f"{shape[0]}x{shape[1]}: every frame needs one size")
+                    imgs.append(img)
+                if ins is None:
+                    ins = [_Slot(frames=((T + 1,) + shape, torch.uint8)) for _ in range(2)]
+                slot = ins[j % 2]
+                slot.wait()
+                host = slot.frames[:len(imgs)]
+                for r, img in enumerate(imgs):
+                    host[r].numpy()[...] = img
+                if warm_start:
+                    low, flow = engine.forward_sequence(host, carry=ps.carry, flow_init=init, return_low=True)
+                    init = forward_interpolate(low)  # before the next pass overwrites flow_low
+                else:
+                    flow = engine.forward_sequence(host, carry=ps.carry)
+                slot.event = torch.cuda.Event()
+                slot.event.record(stream)
+                if native_flow and tuple(flow.shape[1:3]) != tuple(shape[:2]):
+                    flow = resize_flow(flow, shape[:2])
+                color = flow_to_color(flow, convert_to_bgr=True)
+                if outs is None:
+                    fshape = tuple(flow.shape)
+                    outs = [_Slot(color=(fshape[:3] + (3,), torch.uint8),
+                                  **({"flow": (fshape, torch.float32)} if keep_flow else {})) for _ in range(2)]
+                o = outs[j % 2]
+                o.wait()
+                o.color.copy_(color, non_blocking=True)
+                if keep_flow:
+                    o.flow.copy_(flow, non_blocking=True)
+                o.event = torch.cuda.Event()
+                o.event.record(stream)
+                rows = [(r, k) for r, k in enumerate(ps.pairs) if k is not None]
+                if writers is None:
+                    write(o, rows)
+                else:
+                    o.futures.append(writers.submit(write, o, rows))
+                for _, k in rows:
+                    written += [name(k, e) for e in ("png", "flo", "npy") if dirs[e] is not None]
+            for o in outs or ():
+                o.wait()
+    finally:
+        for pool in (decoders, writers):
+            if pool is not None:
+                pool.shutdown(wait=True, cancel_futures=True)
+    return written
