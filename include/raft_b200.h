@@ -136,7 +136,13 @@ int rb_corr_build(const float* fmap1, const float* fmap2, float* pyramid, int B,
 /* ---- A2/A3: SampleCorr(corr_pyramid, coords, num_levels=4, radius)  model_utils.py:224-249 ----
  * with bilinear_sampler / tf_grid_sample semantics of networks/utils.py:39-103 (truncation toward
  * zero, index clamping, weights from the clamped x1/y1).  out: [B,h,w,4*(2r+1)^2] fp32, channel =
- * level*(2r+1)^2 + (x_off+r)*(2r+1) + (y_off+r). */
+ * level*(2r+1)^2 + (x_off+r)*(2r+1) + (y_off+r).
+ * Coordinates: any fp32 value is accepted.  Finite coordinates with |c| < 2^62 are bit-exact with the reference sampler
+ * and its 64-bit truncation (far right x0 = x1 = W_l - 1, far left x0 = x1 = 0, weights from the clamped x1/y1).  Beyond
+ * that and for +-inf / NaN the values are unspecified, but no memory outside the level is read, and rb_corr_lookup and
+ * rb_corr_otf_lookup (on a pyramid whose entries equal its dot products) give the same values.  Under
+ * RB_SEMANTICS_UPSTREAM every coordinate, non-finite ones included, follows the rule above (ix = -100).  The same holds
+ * for rb_update_lookup, rb_update_lookup_otf, rb_raft_iterate and rb_bilinear_sample (reference semantics only). */
 int rb_corr_lookup(const float* pyramid, const float* coords, float* out, int B, int h, int w,
                    int radius, void* stream);
 
@@ -213,7 +219,9 @@ int rb_raft_iterate(int small, const void* weights, void* workspace, const float
  * 4*N^2-byte volume.  Level l of the pyramid equals fmap1 . pool^l(fmap2)^T / sqrt(C) (pooling is linear), so each
  * iteration evaluates only the (2r+3) x (2r+3) entries per pixel and level that the bilinear taps can touch, as fp32
  * dot products against the pooled feature maps, and applies the same tap arithmetic as rb_corr_lookup.  Results equal
- * the materialised path up to the summation order / operand rounding of the dot products (parity is on the flow, 1e-3).
+ * the materialised path up to the summation order / operand rounding of the dot products (parity is on the flow, 1e-3);
+ * where those dot products are exact in fp32 (e.g. small-integer feature maps), the results are bit-identical to
+ * rb_corr_lookup on the pyramid fl(fmap1 . pool^l(fmap2) / fl(sqrt C)) at every coordinate (contract at rb_corr_lookup).
  * rb_corr_otf_prepare pools fmap2 once per pair into `workspace` (levels 1..3, fp32); C = 128 or 256. */
 int rb_corr_otf_workspace_bytes(int B, int h, int w, int C, size_t* bytes);
 int rb_corr_otf_prepare(const float* fmap2, void* workspace, size_t workspace_bytes, int B, int h, int w, int C,

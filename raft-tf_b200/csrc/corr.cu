@@ -134,10 +134,12 @@ __global__ void avgpool2_kernel(const float* __restrict__ src, float* __restrict
 // floor(ix) is floor(x) - 1, floor(x) or floor(x) + 1 -- only within those ulp of an integer.  The origin is therefore taken
 // from the round-tripped coordinate of window column / row 0 itself (not from x): with x_i = fl(x_0 + i) every column has
 // floor(ix_0) + i - 1 <= x0_i <= floor(ix_0) + i + 1, so x0 >= origin and x1 <= origin + 2r + 2 -- the same one column / row of
-// slack as the reference sampler (the `far` row, 3 alignment columns + 2r + 3 <= 16).  The origin is clamped to [-16, W_l]
+// slack as the reference sampler (the `far` row, 3 alignment columns + 2r + 3 <= 16).  The origin is clamped to [-16, W_l + 3]
 // (no int overflow for far-away or NaN coordinates); a clamped origin only occurs when every tap of the unit lies outside the
-// level, and the tap indices, clamped into the staged box, then read zeros.  The TMA box's out-of-bounds fill supplies the
-// zero padding; the plain-load fallback and the `far` loads check the level bounds themselves.
+// level, and the tap indices, clamped into the staged box, then read zeros.  That includes taps whose coordinate crossed 2^24
+// (ix = -100) while column 0's did not: W_l + 3 keeps the box outside the level after the alignment to 4 columns (with W_l,
+// a level whose width is not a multiple of 4 staged its last columns, and such a tap read one of them).  The TMA box's
+// out-of-bounds fill supplies the zero padding; the plain-load fallback and the `far` loads check the level bounds themselves.
 // ---------------------------------------------------------------------------------------------
 // RB_SEMANTICS_UPSTREAM coordinate of a tap: upstream's bilinear_sampler normalises (g = 2x / (n - 1) - 1), PyTorch's CUDA
 // grid sampler unnormalises (GridSampler.cuh: ((g + 1) / 2) * (n - 1)), every step rounded on its own; coordinates PyTorch
@@ -149,7 +151,11 @@ __device__ __forceinline__ float up_unnorm(float x, int n) {
   return fabsf(ix) <= 16777216.0f ? ix : -100.0f;
 }
 // footprint origin of a unit under RB_SEMANTICS_UPSTREAM from the coordinate of window column / row 0 (see above)
-__device__ __forceinline__ int up_origin(float x0, int n) { return min(max((int)floorf(up_unnorm(x0, n)), -16), n); }
+__device__ __forceinline__ int up_origin(float x0, int n) { return min(max((int)floorf(up_unnorm(x0, n)), -16), n + 3); }
+
+// x1 = x0 + 1 of the reference sampler without the signed overflow at x0 = INT_MAX: (int)x saturates for x >= 2^31 and +inf,
+// and the clamp then gives x0 = x1 = W - 1 as the reference's 64-bit truncation does (x0 + 1 would wrap to INT_MIN -> 0)
+__device__ __forceinline__ int sat_inc(int x0) { return min(x0, INT_MAX - 1) + 1; }
 
 struct PyramidView {
   const float* base[RB_NUM_LEVELS];
@@ -294,8 +300,8 @@ corr_lookup_kernel(const __grid_constant__ PyramidView pv, const __grid_constant
   } else {
     // x side of window column i = j (i walks x: model_utils.py:235-237)
     const float x = __fadd_rn(cx, (float)(j - R));
-    int x0 = (int)x;  // tf.cast truncates toward zero (utils.py:54-57)
-    int x1 = x0 + 1;
+    int x0 = (int)x;  // tf.cast truncates toward zero (utils.py:54-57); saturates at INT_MAX for x >= 2^31, +inf
+    int x1 = sat_inc(x0);
     x0 = min(max(x0, 0), W - 1);
     x1 = min(max(x1, 0), W - 1);
     const float qx = __fsub_rn((float)x1, x);  // utils.py:84 (clamped x1)
@@ -314,7 +320,7 @@ corr_lookup_kernel(const __grid_constant__ PyramidView pv, const __grid_constant
   } else {
     const float y = __fadd_rn(cy, (float)(j - R));
     y0 = (int)y;
-    y1 = y0 + 1;
+    y1 = sat_inc(y0);
     y0 = min(max(y0, 0), H - 1);
     y1 = min(max(y1, 0), H - 1);
     qy = __fsub_rn((float)y1, y);  // utils.py:85
@@ -491,12 +497,14 @@ corr_lookup_v5_kernel(const __grid_constant__ PyramidView pv, const float2* __re
         return;
       }
       const float x = __fadd_rn(cx, (float)(i - R));
-      int x0 = (int)x;  // tf.cast truncates toward zero (utils.py:54-57)
-      int x1 = x0 + 1;
+      int x0 = (int)x;  // tf.cast truncates toward zero (utils.py:54-57); saturates at INT_MAX for x >= 2^31, +inf
+      int x1 = sat_inc(x0);
       x0 = min(max(x0, 0), W - 1);
       x1 = min(max(x1, 0), W - 1);
       const float qx = __fsub_rn((float)x1, x);  // utils.py:84 (clamped x1)
-      const int a0 = x0 - bxk, a1 = x1 - bxk;
+      // patch columns, already in [0, 10] with the saturating x1; clamped (like r0 / r1) so that no coordinate, however far
+      // out or non-finite, can address outside the unit's slot
+      const int a0 = min(max(x0 - bxk, 0), 10), a1 = min(max(x1 - bxk, 0), 10);
       tab[k * L::TABN + i] = make_float4(qx, __fsub_rn(1.0f, qx), __int_as_float(a0 * 4), __int_as_float(a1 * 4));
     };
     auto y_entry = [&](int j) {
@@ -512,11 +520,11 @@ corr_lookup_v5_kernel(const __grid_constant__ PyramidView pv, const float2* __re
       }
       const float y = __fadd_rn(cy, (float)(j - R));
       int y0 = (int)y;
-      int y1 = y0 + 1;
+      int y1 = sat_inc(y0);
       y0 = min(max(y0, 0), H - 1);
       y1 = min(max(y1, 0), H - 1);
       const float qy = __fsub_rn((float)y1, y);  // utils.py:85
-      const int r0 = y0 - byk, r1 = y1 - byk;
+      const int r0 = min(max(y0 - byk, 0), L::ROWS - 1), r1 = min(max(y1 - byk, 0), L::ROWS - 1);
       const int uoff = (warp * 4 + k) * L::SLOT;  // slot offset from the 1024-byte aligned start of shared memory
       tab[k * L::TABN + D + j] = make_float4(qy, __fsub_rn(1.0f, qy), __int_as_float((int)patch0_u32 + uoff + v5_row_off(uoff, r0)),
                                              __int_as_float((int)patch0_u32 + uoff + v5_row_off(uoff, r1)));
@@ -649,7 +657,7 @@ __global__ void bilinear_sample_kernel(const float* __restrict__ img, const floa
   const float* im = img + (i / S) * (size_t)H * W;
   const float2 c = coords[i];
   int x0 = (int)c.x, y0 = (int)c.y;
-  int x1 = x0 + 1, y1 = y0 + 1;
+  int x1 = sat_inc(x0), y1 = sat_inc(y0);
   x0 = min(max(x0, 0), W - 1); x1 = min(max(x1, 0), W - 1);
   y0 = min(max(y0, 0), H - 1); y1 = min(max(y1, 0), H - 1);
   const float qx = __fsub_rn((float)x1, c.x), qy = __fsub_rn((float)y1, c.y);

@@ -89,7 +89,9 @@ def test_volume_free_lookup_matches_materialised_path(cuda, B, h, w, C, r):
     f1 = torch.randn(B, h, w, C, generator=g)
     f2 = torch.randn(B, h, w, C, generator=g)
     # in-image coordinates: far outside the image the reference's clamped-x1 weights grow like |x| and cancel (utils.py:84-98),
-    # which amplifies the 1e-6 relative differences between the three evaluations of the dot products beyond any fixed bound
+    # which amplifies the 1e-6 relative differences between the three evaluations of the dot products beyond any fixed bound.
+    # Off the image the volume-free lookup is held bit for bit on exact dot products, and under a per-tap a-priori bound on
+    # these randn maps, in test_gpu_volume_free_exact.py.
     gen = torch.Generator().manual_seed(17)
     coords = O.coords_grid(B, h, w) + (torch.rand(B, h, w, 2, generator=gen) * 2 - 1) * 5.0
     coords[..., 0].clamp_(0.0, w - 1.0)

@@ -228,7 +228,9 @@ def test_volume_free_teacher_forced_steps_match_fp64(cuda, weights, B, h, w, sma
     """rb_corr_otf_prepare + rb_update_lookup_otf inside the loop, against the fp64 pyramid of the same feature maps.
     Far outside the image the reference's clamped-x1 weights grow like |x| and amplify the fp32-vs-fp64 difference of
     the dot products (test_gpu_kernels.test_volume_free_lookup_matches_materialised_path); here the centroids stay
-    within a pixel of the grid, which is asserted so that the bound keeps meaning what it says."""
+    within a pixel of the grid, which is asserted so that the bound keeps meaning what it says.  The loop with most
+    centroids off the image is test_gpu_volume_free_exact.test_loop_off_the_image_bit_identical: bit-identical to the
+    materialised loop on feature maps whose dot products are exact."""
     _, outside = _teacher_forced(cuda, weights, small, _modes()["tc"], B, h, w, steps=6, volume_free=True)
     assert outside < 1.0, f"coords1 left the grid by {outside:.2f} px: the fixed tolerance no longer bounds the lookup"
 
