@@ -345,6 +345,29 @@ int rb_flow_to_color_workspace_bytes(int B, int H, int W, size_t* bytes);
 int rb_flow_to_color(const float* flow, int B, int H, int W, int clip, float clip_flow, int convert_to_bgr, uint8_t* out,
                      void* workspace, size_t workspace_bytes, void* stream);
 
+/* ---- F12: frame metrics -- PSNR / SSIM of interpolated frames (the Vimeo-90K triplet protocol) --------------------
+ * pred: [B,H,W,3], fp32 (pred_is_u8 = 0) or uint8 (1); gt: [B,H,W,3] uint8.  An fp32 value x is quantised as
+ * infer_raft.py --interpolate writes its PNGs, np.clip(np.rint(fl32(255 * x)), 0, 255): q = rintf(__fmul_rn(255.f, x))
+ * (ties to even), clamped to [0, 255]; a NaN becomes 0.  So the scores describe the 8-bit frame a user would write.
+ * stats: [B][RB_FRAME_STATS] fp64 per sample b:
+ *   stats[b][0] = SSE = sum over the H*W*3 values of (q - gt)^2, summed in integers: exact;
+ *   stats[b][1] = SSIM = the mean over the 3 channels of skimage's structural_similarity(gt_c, q_c,
+ *     gaussian_weights=True, sigma=1.5, use_sample_covariance=False, data_range=255), in fp64: with the 11-tap window
+ *     w_k = exp(-k^2 / (2 * 1.5^2)) / sum_j exp(-j^2 / (2 * 1.5^2)), k = -5..5 (scipy's gaussian_filter, truncate 3.5),
+ *     mx, my, Exx, Eyy, Exy the separable 11x11 weighted means, vx = Exx - mx^2, vy = Eyy - my^2, vxy = Exy - mx*my,
+ *     C1 = (0.01*255)^2, C2 = (0.03*255)^2, S = (2 mx my + C1)(2 vxy + C2) / ((mx^2 + my^2 + C1)(vx + vy + C2)), and SSIM
+ *     the mean of S over the crop [5, H-5) x [5, W-5) -- exactly the pixels whose window stays inside the frame, so
+ *     skimage's reflect padding never reaches a counted pixel.
+ * PSNR = 10 log10(255^2 * 3HW / SSE) follows on the host.  Each block reduces one fixed tile of one sample into the
+ * workspace (rb_frame_metrics_workspace_bytes) and a second launch adds each sample's partials in a fixed order: a sample's
+ * bits do not depend on B or its place in the batch; no allocation, no float atomics, graph-capturable.  Null pointers,
+ * pred_is_u8 not 0 or 1, B/H/W <= 0, H or W < 11 (skimage refuses a window larger than the image), B > 65535 and a
+ * workspace that is too small -> RB_ERR_* before any CUDA call. */
+#define RB_FRAME_STATS 2
+int rb_frame_metrics_workspace_bytes(int B, int H, int W, size_t* bytes);
+int rb_frame_metrics(const void* pred, int pred_is_u8, const uint8_t* gt, int B, int H, int W, double* stats,
+                     void* workspace, size_t workspace_bytes, void* stream);
+
 /* ---- F3 (input edge): dataflow/test_dataflow.py:56-61,96-97 + the SURVEY 8(d) shape policy ------------------
  * src: [B,H,W,3] device frames, BGR like cv2.imdecode -- fp32 in [0,1] (src_is_u8 = 0) or uint8 in [0,255]
  * (src_is_u8 = 1: x/255.0f, the reference's np.float32(x)/255.0, bit for bit).  dst: [B,H+pt+pb,W+pl+pr,3] fp32

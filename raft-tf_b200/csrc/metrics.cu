@@ -92,6 +92,126 @@ __global__ void __launch_bounds__(kMetricsThreads) flow_metrics_sample_kernel(co
 
 static int metrics_chunks(int H, int W) { return (int)(((size_t)H * W + kMetricsChunk - 1) / kMetricsChunk); }
 
+// ---- F12: frame metrics (SSE and SSIM of interpolated frames against ground truth) ------------------------------------
+// One block per (kFmTileH x kFmTileW output tile, sample).  The tile plus a kFmR-pixel halo of both images is staged in
+// shared memory as uint8 (pred quantised on load; pixels outside the image read as 0 -- they only reach outputs outside
+// the SSIM crop, which are not counted).  Per channel: a horizontal pass writes the five weighted row sums of x, y, x^2,
+// y^2, xy for every staged row, a vertical pass finishes the 11x11 means and S per output pixel, all in fp64.  The SSE
+// is summed exactly (integers) over the tile's pixels, halo excluded.  Partials {sse, sum S} per tile go to the
+// workspace in tile order; a second launch adds them per sample in a fixed order, as for the flow metrics.
+constexpr int kFmR = 5;                        // window radius: int(3.5 * 1.5 + 0.5), scipy's truncate = 3.5
+constexpr int kFmTileW = 32, kFmTileH = 16;    // output tile; 256 threads = 8 rows of 32
+constexpr int kFmSW = kFmTileW + 2 * kFmR;     // staged columns
+constexpr int kFmSH = kFmTileH + 2 * kFmR;     // staged rows
+constexpr int kFmStats = RB_FRAME_STATS;
+
+struct Gauss11 {
+  double w[kFmR + 1];  // w[k] = weight of offsets +-k
+};
+
+__device__ __forceinline__ uint8_t quantise(float x) {
+  // the CLI's np.clip(np.rint(fl32(255 * x)), 0, 255): ties to even; fmaxf(NaN, 0) = 0, so a NaN becomes 0
+  return (uint8_t)fminf(fmaxf(rintf(__fmul_rn(255.f, x)), 0.f), 255.f);
+}
+
+__global__ void __launch_bounds__(kMetricsThreads) frame_metrics_tile_kernel(
+    const void* __restrict__ pred, int pred_is_u8, const uint8_t* __restrict__ gt, int H, int W, int tiles_x,
+    Gauss11 g, double* __restrict__ partials) {
+  __shared__ uint8_t sx[3][kFmSH][kFmSW], sy[3][kFmSH][kFmSW];
+  __shared__ double hs[5][kFmSH][kFmTileW];
+  __shared__ double red[kMetricsThreads];
+  const int b = blockIdx.y, t = threadIdx.x;
+  const int x0 = (int)(blockIdx.x % tiles_x) * kFmTileW, y0 = (int)(blockIdx.x / tiles_x) * kFmTileH;
+  const size_t base = (size_t)b * H * W * 3;
+  unsigned long long sse = 0;
+  for (int e = t; e < kFmSH * kFmSW * 3; e += kMetricsThreads) {
+    const int c = e % 3, p = e / 3, r = p / kFmSW, col = p % kFmSW;
+    const int y = y0 - kFmR + r, x = x0 - kFmR + col;
+    uint8_t q = 0, v = 0;
+    if (y >= 0 && y < H && x >= 0 && x < W) {
+      const size_t i = base + ((size_t)y * W + x) * 3 + c;
+      q = pred_is_u8 ? static_cast<const uint8_t*>(pred)[i] : quantise(static_cast<const float*>(pred)[i]);
+      v = gt[i];
+      if (r >= kFmR && r < kFmR + kFmTileH && col >= kFmR && col < kFmR + kFmTileW) {
+        const int d = (int)q - (int)v;
+        sse += (unsigned long long)(d * d);
+      }
+    }
+    sx[c][r][col] = q;
+    sy[c][r][col] = v;
+  }
+  __syncthreads();
+  double ssim = 0.0;
+  constexpr double C1 = (0.01 * 255) * (0.01 * 255), C2 = (0.03 * 255) * (0.03 * 255);
+  for (int c = 0; c < 3; ++c) {
+    for (int e = t; e < kFmSH * kFmTileW; e += kMetricsThreads) {
+      const int r = e / kFmTileW, j = e % kFmTileW;
+      const uint8_t* rx = &sx[c][r][j + kFmR];
+      const uint8_t* ry = &sy[c][r][j + kFmR];
+      double a = (double)rx[0], bb = (double)ry[0];
+      double m[5] = {g.w[0] * a, g.w[0] * bb, g.w[0] * (a * a), g.w[0] * (bb * bb), g.w[0] * (a * bb)};
+#pragma unroll
+      for (int k = 1; k <= kFmR; ++k) {
+        const double a0 = rx[-k], a1 = rx[k], b0 = ry[-k], b1 = ry[k];
+        m[0] += g.w[k] * (a0 + a1);
+        m[1] += g.w[k] * (b0 + b1);
+        m[2] += g.w[k] * (a0 * a0 + a1 * a1);
+        m[3] += g.w[k] * (b0 * b0 + b1 * b1);
+        m[4] += g.w[k] * (a0 * b0 + a1 * b1);
+      }
+#pragma unroll
+      for (int i = 0; i < 5; ++i) hs[i][r][j] = m[i];
+    }
+    __syncthreads();
+    for (int e = t; e < kFmTileH * kFmTileW; e += kMetricsThreads) {
+      const int i = e / kFmTileW, j = e % kFmTileW, y = y0 + i, x = x0 + j;
+      double m[5];
+#pragma unroll
+      for (int n = 0; n < 5; ++n) {
+        double s = g.w[0] * hs[n][i + kFmR][j];
+#pragma unroll
+        for (int k = 1; k <= kFmR; ++k) s += g.w[k] * (hs[n][i + kFmR - k][j] + hs[n][i + kFmR + k][j]);
+        m[n] = s;
+      }
+      const double vx = m[2] - m[0] * m[0], vy = m[3] - m[1] * m[1], vxy = m[4] - m[0] * m[1];
+      const double S = ((2.0 * m[0] * m[1] + C1) * (2.0 * vxy + C2)) /
+                       ((m[0] * m[0] + m[1] * m[1] + C1) * (vx + vy + C2));
+      if (y >= kFmR && y < H - kFmR && x >= kFmR && x < W - kFmR) ssim += S;
+    }
+    __syncthreads();  // hs is rewritten by the next channel
+  }
+  const double v[kFmStats] = {(double)sse, ssim};  // sse < 2^53: exact
+  double* dst = partials + ((size_t)b * gridDim.x + blockIdx.x) * kFmStats;
+#pragma unroll
+  for (int i = 0; i < kFmStats; ++i) {
+    const double r = block_sum(v[i], red);
+    if (t == 0) dst[i] = r;
+  }
+}
+
+// one block per sample: thread t adds partials t, t + 256, ... in order, then the fixed tree; the S sum becomes the mean
+__global__ void __launch_bounds__(kMetricsThreads) frame_metrics_sample_kernel(const double* __restrict__ partials,
+                                                                               int tiles, double n_crop,
+                                                                               double* __restrict__ stats) {
+  __shared__ double red[kMetricsThreads];
+  const int b = blockIdx.x;
+  const double* src = partials + (size_t)b * tiles * kFmStats;
+  double v[kFmStats] = {0.0, 0.0};
+  for (int c = threadIdx.x; c < tiles; c += kMetricsThreads) {
+#pragma unroll
+    for (int i = 0; i < kFmStats; ++i) v[i] += src[(size_t)c * kFmStats + i];
+  }
+  const double sse = block_sum(v[0], red), ssim = block_sum(v[1], red);
+  if (threadIdx.x == 0) {
+    stats[(size_t)b * kFmStats + 0] = sse;
+    stats[(size_t)b * kFmStats + 1] = ssim / n_crop;
+  }
+}
+
+static size_t frame_metrics_tiles(int H, int W) {
+  return (size_t)((W + kFmTileW - 1) / kFmTileW) * (size_t)((H + kFmTileH - 1) / kFmTileH);
+}
+
 }  // namespace rb
 
 using namespace rb;
@@ -124,5 +244,44 @@ extern "C" int rb_flow_metrics(const float* flow, float flow_scale, const float*
   RB_CHECK_LAUNCH("flow_metrics_chunk_kernel");
   flow_metrics_sample_kernel<<<B, kMetricsThreads, 0, st>>>(partials, (int)chunks, stats);
   RB_CHECK_LAUNCH("flow_metrics_sample_kernel");
+  return RB_OK;
+}
+
+extern "C" int rb_frame_metrics_workspace_bytes(int B, int H, int W, size_t* bytes) {
+  RB_REQUIRE(bytes, RB_ERR_BAD_ARG, "rb_frame_metrics_workspace_bytes: null pointer");
+  RB_REQUIRE(B > 0 && H > 0 && W > 0, RB_ERR_BAD_SHAPE, "rb_frame_metrics_workspace_bytes: bad shape B=%d H=%d W=%d", B,
+             H, W);
+  *bytes = (size_t)B * frame_metrics_tiles(H, W) * kFmStats * sizeof(double);
+  return RB_OK;
+}
+
+extern "C" int rb_frame_metrics(const void* pred, int pred_is_u8, const uint8_t* gt, int B, int H, int W, double* stats,
+                                void* workspace, size_t workspace_bytes, void* stream) {
+  RB_REQUIRE(pred && gt && stats && workspace, RB_ERR_BAD_ARG, "rb_frame_metrics: null pointer");
+  RB_REQUIRE(pred_is_u8 == 0 || pred_is_u8 == 1, RB_ERR_BAD_ARG, "rb_frame_metrics: pred_is_u8 must be 0 or 1 (got %d)",
+             pred_is_u8);
+  RB_REQUIRE(B > 0 && H > 0 && W > 0, RB_ERR_BAD_SHAPE, "rb_frame_metrics: bad shape B=%d H=%d W=%d", B, H, W);
+  RB_REQUIRE(H >= 2 * kFmR + 1 && W >= 2 * kFmR + 1, RB_ERR_BAD_SHAPE,
+             "rb_frame_metrics: H=%d x W=%d is smaller than the 11x11 SSIM window", H, W);
+  const size_t tiles = frame_metrics_tiles(H, W);
+  RB_REQUIRE(B <= 65535 && tiles <= 0x7fffffffu, RB_ERR_BAD_SHAPE,
+             "rb_frame_metrics: B=%d samples of %dx%d pixels exceed one grid", B, H, W);
+  const size_t need = (size_t)B * tiles * kFmStats * sizeof(double);
+  RB_REQUIRE(workspace_bytes >= need, RB_ERR_WORKSPACE, "rb_frame_metrics: workspace of %zu bytes, %zu needed",
+             workspace_bytes, need);
+  // scipy's _gaussian_kernel1d(sigma = 1.5, radius 5): exp(-0.5 k^2 / sigma^2), normalised by the sum over k = -5..5
+  Gauss11 g;
+  double sum = 0.0;
+  for (int k = -kFmR; k <= kFmR; ++k) sum += exp(-0.5 * (double)(k * k) / (1.5 * 1.5));
+  for (int k = 0; k <= kFmR; ++k) g.w[k] = exp(-0.5 * (double)(k * k) / (1.5 * 1.5)) / sum;
+  const cudaStream_t st = (cudaStream_t)stream;
+  double* partials = static_cast<double*>(workspace);
+  const int tiles_x = (W + kFmTileW - 1) / kFmTileW;
+  frame_metrics_tile_kernel<<<dim3((unsigned)tiles, (unsigned)B), kMetricsThreads, 0, st>>>(pred, pred_is_u8, gt, H, W,
+                                                                                              tiles_x, g, partials);
+  RB_CHECK_LAUNCH("frame_metrics_tile_kernel");
+  const double n_crop = 3.0 * (double)(H - 2 * kFmR) * (double)(W - 2 * kFmR);
+  frame_metrics_sample_kernel<<<B, kMetricsThreads, 0, st>>>(partials, (int)tiles, n_crop, stats);
+  RB_CHECK_LAUNCH("frame_metrics_sample_kernel");
   return RB_OK;
 }

@@ -28,7 +28,13 @@ the validation, which upstream runs cold).  --split test writes upstream's test-
     python infer_raft.py -m val --split test --dataset sintel --data datasets/Sintel --out submission --load ... [--warm-start]
 
 Sintel: ``<out>/<dstype>/<scene>/frameNNNN.flo``; KITTI (no --warm-start): ``<out>/<id>_10.png``, 16-bit PNGs
-(raft_b200.evaluate.submit).
+(raft_b200.evaluate.submit).  --dataset vimeo scores frame interpolation on a Vimeo-90K triplet tree instead:
+
+    python infer_raft.py -m val --dataset vimeo --data datasets/vimeo_triplet --load raft-things.npz [--batch 8]
+
+im2 of every triplet in <data>/tri_testlist.txt is interpolated from im1 and im3 at t = 0.5 (20 iterations, like the
+reference), and the mean PSNR and SSIM of the 8-bit frames against im2 are printed (``Validation Vimeo-90K: PSNR: ...,
+SSIM: ...``) and written with the per-triplet records to ``<--out>/val_vimeo.json`` (no --split test, no --warm-start).
 
 --path DIR (upstream demo.py's flag): the flow of every consecutive pair of DIR's sorted *.png / *.jpg frames, written as
 ``<--out>/flow_<k:06d>.png`` (and ``flow_<k:06d>.flo`` / ``.npy`` under the directories --flo / --npy name), each frame
@@ -86,7 +92,9 @@ def parser():
     p.add_argument('--small', action='store_true')
     p.add_argument('--iters', type=int, default=None,
                    help='extension: GRU iterations (test mode: 20 like the reference; -m val: the protocol\'s 32 / 24)')
-    p.add_argument('--dataset', default=None, choices=['sintel', 'kitti'], help='-m val: which training set --data holds')
+    p.add_argument('--dataset', default=None, choices=['sintel', 'kitti', 'vimeo'],
+                   help='-m val: which dataset --data holds (Sintel / KITTI-2015 training sets: flow; Vimeo-90K '
+                        'triplets: frame interpolation)')
     p.add_argument('--dstype', nargs='+', default=['clean', 'final'], choices=['clean', 'final'],
                    help='-m val, Sintel: the passes to evaluate')
     p.add_argument('--workers', type=int, default=4, help='-m val and --path: frame-decoding (and writing) threads')
@@ -123,9 +131,14 @@ def main(argv=None):
         p.error('--interpolate: every T must be in [0, 1]')
     if args.mode == 'val':
         if not args.data or not args.dataset:
-            p.error('-m val needs --data <dataset root> and --dataset {sintel,kitti}')
+            p.error('-m val needs --data <dataset root> and --dataset {sintel,kitti,vimeo}')
         if args.warm_start and args.dataset == 'kitti':
             p.error("--warm-start needs frame sequences: KITTI's pairs are not sequences")
+        if args.dataset == 'vimeo' and args.split == 'test':
+            p.error('--split test writes a flow submission; Vimeo-90K has no hidden-ground-truth split (-m val scores '
+                    'its test list)')
+        if args.dataset == 'vimeo' and args.warm_start:
+            p.error("--warm-start needs frame sequences: Vimeo-90K's triplets are not chains")
         return validate(args)
     if args.mode != 'test':
         print(f"mode '{args.mode}' has no implementation in the reference either (infer_raft.py:71-95); nothing to do")

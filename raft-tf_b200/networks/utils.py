@@ -81,6 +81,36 @@ def flow_metrics(flow, gt, valid=None, flow_scale=1.0, return_epe=False):
     return (stats, epe) if return_epe else stats
 
 
+FRAME_STATS = ("sse", "ssim")  # the columns of frame_metrics' stats (RB_FRAME_STATS)
+
+
+def frame_metrics(pred, gt):
+    """Extension (the Vimeo-90K triplet protocol): SSE and SSIM of [B,H,W,3] CUDA frames pred (fp32 in [0,1], what
+    interpolate returns, or uint8) against uint8 ground truth gt (rb_frame_metrics), H and W >= 11.  An fp32 pred is first
+    quantised as infer_raft.py --interpolate writes its PNGs (np.clip(np.rint(fl32(255 * x)), 0, 255); NaN -> 0).  Returns a
+    fresh [B,2] fp64 tensor {sse, ssim} (FRAME_STATS): the exact sum of squared 8-bit errors, and skimage's
+    structural_similarity(gaussian_weights=True, sigma=1.5, use_sample_covariance=False, data_range=255) averaged over the
+    3 channels.  PSNR = 10 * log10(255^2 * 3HW / sse) (inf when sse = 0).  Wrong shapes or dtypes raise ValueError."""
+    for name, t, dtypes in (("pred", pred, (torch.float32, torch.uint8)), ("gt", gt, (torch.uint8,))):
+        if not (isinstance(t, torch.Tensor) and t.is_cuda and t.dim() == 4 and t.shape[-1] == 3 and t.dtype in dtypes):
+            raise ValueError(f"frame_metrics: {name} must be a [B,H,W,3] {' or '.join(str(d) for d in dtypes)} CUDA "
+                             f"tensor (got {getattr(t, 'shape', None)} {getattr(t, 'dtype', type(t))})")
+    if pred.shape != gt.shape or pred.device != gt.device:
+        raise ValueError(f"frame_metrics: pred {tuple(pred.shape)} on {pred.device} and gt {tuple(gt.shape)} on "
+                         f"{gt.device} must match")
+    B, H, W, _ = pred.shape
+    if H < 11 or W < 11:
+        raise ValueError(f"frame_metrics: frames of {H}x{W} are smaller than the 11x11 SSIM window")
+    p, g = pred.contiguous(), gt.contiguous()
+    stats = torch.empty(B, len(FRAME_STATS), dtype=torch.float64, device=p.device)
+    with torch.cuda.device(p.device):
+        nbytes = capi.size_query(capi.lib.rb_frame_metrics_workspace_bytes, B, H, W)
+        ws = torch.empty(nbytes, dtype=torch.uint8, device=p.device)
+        capi.check(capi.lib.rb_frame_metrics(capi.ptr(p), int(p.dtype == torch.uint8), capi.ptr(g), B, H, W,
+                                             capi.ptr(stats), capi.ptr(ws), nbytes, capi.stream()))
+    return stats
+
+
 def forward_interpolate(flow):
     """Extension (upstream RAFT's core/utils/utils.py forward_interpolate, on the GPU): every grid point of the [B,h,w,2]
     fp32 CUDA flow takes the flow of the nearest source pixel x + flow(x) that lands strictly inside the grid, per

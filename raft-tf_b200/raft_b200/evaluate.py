@@ -11,6 +11,11 @@ valid flag), 24 iterations, 'kitti' padding (bottom only), valid pixels counted.
 submit writes upstream's test-split submissions (create_sintel_submission, create_kitti_submission) the same way, and
 warm_start runs each Sintel scene as a chain warm-started by forward_interpolate (upstream's warm_start=True).
 
+Vimeo-90K (F12): the triplets <root>/sequences/<entry>/im1.png, im2.png, im3.png of <root>/tri_testlist.txt, in list
+order; im2 is interpolated from im1 and im3 at t = 0.5 (RaftEngine.interpolate, 20 iterations like the reference) and
+scored by rb_frame_metrics against the uploaded im2 on the same stream -- the predicted frame never leaves the GPU -- into
+per-triplet PSNR and SSIM, reported as their means over the list.
+
 Pipeline: pairs are grouped by frame size (one CUDA graph per size) and run in batches through RaftEngine.forward, whose
 flow stays on the GPU: rb_flow_metrics scores it against the uploaded ground truth on the same stream and writes per-pair
 stats into one device buffer, read back once per split.  Worker threads decode the next batches (cv2 releases the GIL)
@@ -33,11 +38,14 @@ from . import capi
 from .engine import RaftEngine
 
 # dataset -> (iterations, pad_mode): upstream's validate_sintel / validate_kitti
-PROTOCOLS = {"sintel": (32, "sintel"), "kitti": (24, "kitti")}
+PROTOCOLS = {"sintel": (32, "sintel"), "kitti": (24, "kitti"), "vimeo": (20, "sintel")}
 DSTYPES = ("clean", "final")
 STATS = 6  # RB_FLOW_STATS: n, sum of EPE, #(EPE < 1), #(EPE < 3), #(EPE < 5), #outliers
+FRAME_STATS = 2  # RB_FRAME_STATS: SSE, SSIM
 
 Pair = namedtuple("Pair", "image1 image2 gt")
+# Vimeo-90K: image1 = im1, image2 = im3 (the frames the engine reads), gt = im2; dir = the list entry
+Triplet = namedtuple("Triplet", "image1 image2 gt dir")
 
 
 # ---- dataset enumeration ----------------------------------------------------------------------------
@@ -104,6 +112,27 @@ def kitti_pairs(root):
     return pairs
 
 
+def vimeo_triplets(root):
+    """Vimeo-90K triplets in the order of <root>/tri_testlist.txt (one '00001/0389'-style entry per line; blank lines and
+    surrounding whitespace are ignored): <root>/sequences/<entry>/im1.png, im2.png, im3.png.  A missing list, a missing
+    frame or an empty list raises FileNotFoundError naming the path."""
+    lst = os.path.join(root, "tri_testlist.txt")
+    if not os.path.isfile(lst):
+        raise FileNotFoundError(f"Vimeo-90K: no triplet list {lst}")
+    with open(lst) as f:
+        entries = [e.strip() for e in f if e.strip()]
+    trips = []
+    for e in entries:
+        im1, im2, im3 = (os.path.join(root, "sequences", e, f"im{k}.png") for k in (1, 2, 3))
+        for p in (im1, im2, im3):
+            if not os.path.isfile(p):
+                raise FileNotFoundError(f"Vimeo-90K: frame {p} of triplet {e} is missing")
+        trips.append(Triplet(im1, im3, im2, e))
+    if not trips:
+        raise FileNotFoundError(f"Vimeo-90K: {lst} lists no triplets")
+    return trips
+
+
 # ---- decoding (worker threads) ------------------------------------------------------------------------
 def _png_size(path):
     """(H, W) from the PNG header, without decoding the image."""
@@ -130,6 +159,14 @@ def _decode_frames(pair, rgb):
     return left, right
 
 
+def _decode_triplet(trip, rgb):
+    left, right = _decode_frames(trip, rgb)
+    mid = _imread(trip.gt, rgb)
+    if mid.shape != left.shape:
+        raise ValueError(f"{trip.gt}: {mid.shape[:2]} frame, {trip.image1} is {left.shape[:2]}")
+    return left, right, mid
+
+
 def _decode(pair, kitti, rgb):
     from flow_utils import read_flo, read_kitti_flow
     left, right = _decode_frames(pair, rgb)
@@ -140,13 +177,14 @@ def _decode(pair, kitti, rgb):
 
 
 class _Slot:
-    """Pinned host staging of one batch (frames, and ground truth and mask when scored) and the event behind the last
-    batch that used it."""
+    """Pinned host staging of one batch (frames, and ground truth and mask when scored; with gt_frame the ground truth
+    is a uint8 [B,H,W,3] frame instead of a flow) and the event behind the last batch that used it."""
 
-    def __init__(self, B, H, W, kitti, scored=True):
+    def __init__(self, B, H, W, kitti, scored=True, gt_frame=False):
         self.left = torch.zeros(B, H, W, 3, dtype=torch.uint8).pin_memory()
         self.right = torch.zeros_like(self.left).pin_memory()
-        self.gt = torch.zeros(B, H, W, 2, dtype=torch.float32).pin_memory() if scored else None
+        gt_shape, gt_dtype = ((B, H, W, 3), torch.uint8) if gt_frame else ((B, H, W, 2), torch.float32)
+        self.gt = torch.zeros(*gt_shape, dtype=gt_dtype).pin_memory() if scored else None
         self.valid = torch.zeros(B, H, W, dtype=torch.uint8).pin_memory() if kitti and scored else None
         self.event = None
 
@@ -190,10 +228,12 @@ def warm_schedule(lengths, batch):
 
 
 # ---- the run ------------------------------------------------------------------------------------------
-def _steps(engine, pairs, chains, decode, batch, workers, warm, scored, kitti=False):
+def _steps(engine, pairs, chains, decode, batch, workers, warm, scored, kitti=False, run=None, gt_frame=False):
     """Runs every pair of chains (lists of indices into pairs) through engine.forward and yields (row, flow, slot) per
     batch: row[i] = the pair index in batch row i (None: idle, its flow is not meaningful), flow = the engine's flow
-    buffer, slot = the pinned staging that holds the batch's decoded frames (and ground truth when scored).
+    buffer, slot = the pinned staging that holds the batch's decoded frames (and ground truth when scored).  run (not
+    with warm): the engine call per batch instead, run(left, right) -> what is yielded in place of the flow; gt_frame:
+    the ground truth is a uint8 frame (_Slot).
 
     Chains are grouped by frame size (one CUDA graph per size), each group run by warm_schedule.  With warm, pair k > 0
     of a chain starts from forward_interpolate of the flow_low of pair k - 1 (computed on the device from the engine's
@@ -232,7 +272,7 @@ def _steps(engine, pairs, chains, decode, batch, workers, warm, scored, kitti=Fa
                     ahead.append(submit(j + depth))  # workers start on it now
                 if shape != (B, H, W):
                     shape, init = (B, H, W), None
-                    slots = [_Slot(B, H, W, kitti, scored), _Slot(B, H, W, kitti, scored)]
+                    slots = [_Slot(B, H, W, kitti, scored, gt_frame), _Slot(B, H, W, kitti, scored, gt_frame)]
                 slot = slots[j % 2]
                 if slot.event is not None:
                     slot.event.synchronize()  # its last batch's copies (and work) are done
@@ -250,6 +290,8 @@ def _steps(engine, pairs, chains, decode, batch, workers, warm, scored, kitti=Fa
                             if not c:
                                 init[k].zero_()  # a chain starts (or the row is idle): cold
                     low, flow = engine.forward(slot.left, slot.right, flow_init=init, return_low=True)
+                elif run is not None:
+                    flow = run(slot.left, slot.right)
                 else:
                     flow = engine.forward(slot.left, slot.right)
                 yield row, flow, slot
@@ -290,6 +332,53 @@ def _run(engine, pairs, kitti, batch, workers, rgb, warm=False):
         return stats.cpu().numpy()
 
 
+def _run_vimeo(engine, trips, batch, workers, rgb):
+    """Per-triplet stats [N, 3] fp64 (host, list order): {values 3HW, SSE, SSIM} of engine.interpolate(im1, im3, [0.5])
+    against im2, scored by rb_frame_metrics on the same stream."""
+    dev = engine.device
+    with torch.cuda.device(dev):
+        stats = torch.empty(len(trips), FRAME_STATS, dtype=torch.float64, device=dev)
+        values = np.zeros(len(trips), dtype=np.float64)
+        shape = None
+        for row, pred, slot in _steps(engine, trips, chains_of(trips, False), lambda t: _decode_triplet(t, rgb), batch,
+                                      workers, False, True, run=lambda l, r: engine.interpolate(l, r, [0.5])[0],
+                                      gt_frame=True):
+            B, H, W = pred.shape[:3]
+            if shape != (B, H, W):
+                shape = (B, H, W)
+                gt = torch.empty(B, H, W, 3, dtype=torch.uint8, device=dev)
+                ws_bytes = capi.size_query(capi.lib.rb_frame_metrics_workspace_bytes, B, H, W)
+                ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
+                part = torch.empty(B, FRAME_STATS, dtype=torch.float64, device=dev)
+            gt.copy_(slot.gt, non_blocking=True)
+            # every row is scored (idle rows too: the kernel is batch-invariant), the triplets' rows are kept
+            capi.check(capi.lib.rb_frame_metrics(capi.ptr(pred), 0, capi.ptr(gt), B, H, W, capi.ptr(part), capi.ptr(ws),
+                                                 ws_bytes, capi.stream()))
+            rows = [k for k, i in enumerate(row) if i is not None]
+            idx = [row[k] for k in rows]
+            stats.index_copy_(0, torch.tensor(idx, device=dev), part[rows])
+            values[idx] = 3.0 * H * W
+        return np.concatenate([values[:, None], stats.cpu().numpy()], axis=1)
+
+
+def psnr(sse, values):
+    """10 log10(255^2 * values / sse) in fp64: inf for sse = 0."""
+    with np.errstate(divide="ignore"):
+        return 10.0 * np.log10(255.0 ** 2 * np.asarray(values, np.float64) / np.asarray(sse, np.float64))
+
+
+def aggregate_vimeo(trips, stats):
+    """fp64 aggregates of the per-triplet stats [N, 3] {values, SSE, SSIM}: psnr = the mean of the per-triplet PSNRs and
+    ssim = the mean of the per-triplet SSIMs (as interpolation papers report them), and one record per triplet in list
+    order with its mse = SSE / values."""
+    s = np.asarray(stats, dtype=np.float64).reshape(-1, 3)
+    n, sse, ssim = s.T
+    p = psnr(sse, n)
+    return {"psnr": float(p.mean()), "ssim": float(ssim.mean()), "n_triplets": len(s),
+            "triplets": [{"dir": t.dir, "psnr": float(pi), "ssim": float(si), "mse": float(e / v)}
+                         for t, pi, si, e, v in zip(trips, p, ssim, sse, n)]}
+
+
 def aggregate(pairs, stats, kitti):
     """fp64 aggregates of the per-pair stats [N, STATS]: epe pooled over all counted pixels (Sintel) or the mean of the
     per-pair means (KITTI, as upstream's validate_kitti); 1px / 3px / 5px pooled fractions; f1 = 100 * outliers / pixels;
@@ -316,13 +405,15 @@ def _setup(model, dataset, dstypes, batch, workers, iters, warm_start, what):
         raise ValueError(f"{what}: frames run at their own size; build the model without input_size")
     if int(batch) < 1 or int(workers) < 0:
         raise ValueError(f"{what}: batch must be >= 1 and workers >= 0 (got {batch}, {workers})")
-    kitti = dataset == "kitti"
+    kitti, vimeo = dataset == "kitti", dataset == "vimeo"
     if kitti and warm_start:
         raise ValueError(f"{what}: warm_start needs frame sequences; KITTI's pairs are not sequences")
+    if vimeo and warm_start:
+        raise ValueError(f"{what}: warm_start needs frame sequences; Vimeo-90K's triplets are not chains")
     if model._params is None:
         raise RuntimeError(f"RAFT.load(<npz>) must be called before {what}")
-    splits = ("kitti",) if kitti else tuple(dstypes)
-    if not kitti and (not splits or any(d not in DSTYPES for d in splits)):
+    splits = ("kitti",) if kitti else ("vimeo",) if vimeo else tuple(dstypes)
+    if not kitti and not vimeo and (not splits or any(d not in DSTYPES for d in splits)):
         raise ValueError(f"Sintel dstypes must be a non-empty subset of {DSTYPES} (got {dstypes!r})")
     n_iters, pad_mode = PROTOCOLS[dataset]
     return kitti, splits, n_iters if iters is None else int(iters), pad_mode
@@ -334,7 +425,8 @@ def _engine(model, n_iters, pad_mode):
 
 
 def evaluate(model, root, dataset="sintel", dstypes=DSTYPES, batch=1, workers=4, iters=None, warm_start=False):
-    """Upstream RAFT's validation of a loaded networks.RAFT.RAFT model on a Sintel or KITTI-2015 training tree.
+    """Upstream RAFT's validation of a loaded networks.RAFT.RAFT model on a Sintel or KITTI-2015 training tree, or the
+    interpolation quality on a Vimeo-90K triplet tree (dataset 'vimeo').
 
     The engine is built from the model's configuration (small, upstream, mixed_precision, volume_free, device, weights)
     with the protocol's iterations (iters overrides them) and padding.  Frames go in RGB with upstream=True and BGR
@@ -344,8 +436,18 @@ def evaluate(model, root, dataset="sintel", dstypes=DSTYPES, batch=1, workers=4,
 
     warm_start (Sintel only; an extension, upstream validates cold): every scene runs as a chain, each pair after the
     first starting from forward_interpolate of the previous pair's 1/8-resolution flow, as in upstream's
-    create_sintel_submission(warm_start=True) -- the way to measure what the warm start does against ground truth."""
+    create_sintel_submission(warm_start=True) -- the way to measure what the warm start does against ground truth.
+
+    vimeo: im2 of every triplet of vimeo_triplets(root) interpolated from im1 and im3 at t = 0.5 and scored on the GPU
+    (rb_frame_metrics: PSNR of the 8-bit frame the CLI would write, SSIM as skimage's Gaussian-window form); the split
+    'vimeo' holds aggregate_vimeo(...).  dstypes is ignored and warm_start raises ValueError."""
     kitti, splits, n_iters, pad_mode = _setup(model, dataset, dstypes, batch, workers, iters, warm_start, "evaluate")
+    if dataset == "vimeo":
+        trips = vimeo_triplets(root)  # every file checked up front
+        engine = _engine(model, n_iters, pad_mode)
+        stats = _run_vimeo(engine, trips, int(batch), int(workers), model.upstream)
+        return {"dataset": dataset, "iters": n_iters, "pad_mode": pad_mode,
+                "splits": {"vimeo": aggregate_vimeo(trips, stats)}}
     lists = {s: kitti_pairs(root) if kitti else sintel_pairs(root, s) for s in splits}  # every file checked up front
     engine = _engine(model, n_iters, pad_mode)
     res = {"dataset": dataset, "iters": n_iters, "pad_mode": pad_mode, "splits": {}}
@@ -406,6 +508,8 @@ def submit(model, root, dataset, out, dstypes=DSTYPES, batch=1, workers=4, iters
     warm-started by forward_interpolate, as upstream's warm_start=True.  The files are the same bytes for every batch and
     workers.  Returns the paths written, in dataset order."""
     from flow_utils import write_flo, write_kitti_flow
+    if dataset == "vimeo":
+        raise ValueError("submit: Vimeo-90K has no test split with hidden ground truth; evaluate scores its test list")
     kitti, splits, n_iters, pad_mode = _setup(model, dataset, dstypes, batch, workers, iters, warm_start, "submit")
     lists = {s: kitti_test_pairs(root) if kitti else sintel_test_pairs(root, s) for s in splits}
     engine = _engine(model, n_iters, pad_mode)
@@ -426,7 +530,10 @@ def submit(model, root, dataset, out, dstypes=DSTYPES, batch=1, workers=4, iters
 
 def summary_lines(res):
     """upstream evaluate.py's lines: 'Validation (clean) EPE: ..., 1px: ..., 3px: ..., 5px: ...' per Sintel pass,
-    'Validation KITTI: <epe>, <f1>'."""
+    'Validation KITTI: <epe>, <f1>'; and for Vimeo-90K 'Validation Vimeo-90K: PSNR: ..., SSIM: ...'."""
+    if res["dataset"] == "vimeo":
+        r = res["splits"]["vimeo"]
+        return ["Validation Vimeo-90K: PSNR: %f, SSIM: %f" % (r["psnr"], r["ssim"])]
     if res["dataset"] == "kitti":
         r = res["splits"]["kitti"]
         return ["Validation KITTI: %f, %f" % (r["epe"], r["f1"])]

@@ -71,6 +71,33 @@ def write_sintel_tree(root: str, scenes: int, frames: int, H: int, W: int, seed:
     return scenes * (frames - 1)
 
 
+def write_vimeo_tree(root: str, sizes, seed: int = 4000, shift: int = 4):
+    """A dataset in Vimeo-90K's triplet layout under root: one triplet per (H, W) of sizes, <root>/sequences/<entry>/im1.png,
+    im2.png, im3.png (8-bit PNGs) cropped from one textured image that moves by a seeded (dx, dy), |dx|, |dy| <= shift, per
+    frame -- so im2 is the true middle frame -- and <root>/tri_testlist.txt listing the entries in order.  Returns them."""
+    import os
+
+    import cv2
+    rng = np.random.default_rng(seed)
+    entries = []
+    for i, (H, W) in enumerate(sizes):
+        m = 2 * shift
+        base = rng.random((H + 2 * m, W + 2 * m, 3), dtype=np.float32)
+        base = 0.6 * _blur(base, 3.0) + 0.4 * _blur(base, 1.0)
+        base = (base - base.min()) / max(float(base.max() - base.min()), 1e-6)
+        dy, dx = (int(v) for v in rng.integers(-shift, shift + 1, 2))
+        entry = f"{i // 7 + 1:05d}/{i % 7 + 1:04d}"
+        d = os.path.join(root, "sequences", entry)
+        os.makedirs(d, exist_ok=True)
+        for k in range(3):
+            y0, x0 = m + (k - 1) * dy, m + (k - 1) * dx
+            cv2.imwrite(os.path.join(d, f"im{k + 1}.png"), np.round(255 * base[y0:y0 + H, x0:x0 + W]).astype(np.uint8))
+        entries.append(entry)
+    with open(os.path.join(root, "tri_testlist.txt"), "w") as f:
+        f.write("\n".join(entries) + "\n")
+    return entries
+
+
 def make_batch(B: int, H: int, W: int, seed0: int = 1000):
     pairs = [make_pair(H, W, seed0 + i) for i in range(B)]
     return np.stack([p[0] for p in pairs]), np.stack([p[1] for p in pairs])
