@@ -291,6 +291,35 @@ int rb_frame_synthesize(const float* frames, int Hp, int Wp, int top, int left, 
                         const float* flow_t1, const uint8_t* empty0, const uint8_t* empty1, float t, float* out,
                         int B, int H, int W, void* stream);
 
+/* ---- F13: every time step of frame interpolation in one launch (frame sequences and many t per pair) --------------
+ * rb_flow_reverse_multi: the reversal of one flow01 [B,H,W,2] fp32 by n_steps time steps at once.  time_steps is a host
+ * array of n_steps finite values, copied into the kernel parameters (no host-to-device copy, no allocation, CUDA-graph
+ * capturable).  flow_t [n_steps,B,H,W,2] fp32, empty and multi [n_steps,B,H,W] uint8: sample (i, b) is bit for bit
+ * rb_flow_reverse(flow01[b], time_steps[i]) without bg / im0 (steps 1-7 above; no static mask, no eroded mask).  The
+ * n_steps * B samples share one key sort (keys up to n_steps*B*H*W) and one hole fill with n_steps*B*W column and
+ * n_steps*B*H row threads.  rb_flow_reverse is the n_steps = 1 case of the same kernels.  The workspace
+ * (rb_flow_reverse_multi_workspace_bytes; rb_flow_reverse_workspace_bytes is its n_steps = 1 value) holds CUB's
+ * temporary storage too.  Null pointers, n_steps < 1 or > RB_INTERP_MAX_STEPS, a non-finite step, B/H/W <= 0,
+ * n_steps*B*H*W + 1 >= 2^32 and a workspace smaller than its fixed part -> RB_ERR_* before any CUDA call. */
+#define RB_INTERP_MAX_STEPS 64
+int rb_flow_reverse_multi_workspace_bytes(int n_steps, int B, int H, int W, size_t* bytes);
+int rb_flow_reverse_multi(const float* flow01, const float* time_steps, int n_steps, float* flow_t, uint8_t* empty,
+                          uint8_t* multi, int B, int H, int W, void* workspace, size_t workspace_bytes, void* stream);
+/* rb_frame_synthesize_pairs: rb_frame_synthesize's blend for n_t times at once, with the two frames of every pair given
+ * apart: frames0, frames1 [B,Hp,Wp,3] fp32 (pair b blends frames0[b] and frames1[b]; for T consecutive pairs of T + 1
+ * frames these are images[:T] and images[1:], for B independent pairs the halves of [I0 | I1]).  ts: a host array of n_t
+ * times in [0, 1], copied into the kernel parameters; flow_t0, flow_t1 [n_t,B,H,W,2] and empty0, empty1 [n_t,B,H,W]
+ * (rb_flow_reverse_multi's outputs for the steps t and 1 - t); out [n_t,B,H,W,3]: fp32 (out_u8 = 0), the values of
+ * rb_frame_synthesize at each t, or uint8 (out_u8 = 1), each value quantised as rb_frame_metrics does,
+ * min(max(rintf(fl32(255 v)), 0), 255) with NaN -> 0 -- the CLI's np.clip(np.rint(255 v), 0, 255) for every finite v.
+ * bgr = 1 writes the channels in reverse order (RGB <-> BGR).  rb_frame_synthesize is this call with
+ * frames1 = frames + B*Hp*Wp*3, one t and fp32 output.  Null pointers, n_t < 1 or > RB_INTERP_MAX_STEPS, out_u8 or bgr
+ * not 0 / 1, a t outside [0, 1] (or NaN), bad shapes or a crop outside the frames -> RB_ERR_* before any CUDA call. */
+int rb_frame_synthesize_pairs(const float* frames0, const float* frames1, int Hp, int Wp, int top, int left,
+                              const float* flow_t0, const float* flow_t1, const uint8_t* empty0, const uint8_t* empty1,
+                              const float* ts, int n_t, void* out, int out_u8, int bgr, int B, int H, int W,
+                              void* stream);
+
 /* ---- F9: end-point-error metrics (upstream RAFT's evaluate.py validate_sintel / validate_kitti) ---------------------
  * flow, gt: [B,H,W,2] fp32; valid: [B,H,W] uint8, nonzero = the pixel counts (NULL: every pixel counts).  Per pixel,
  * every operation rounded on its own (no FMA contraction), so the values equal upstream's torch expressions bit for bit:

@@ -17,6 +17,7 @@ namespace rb {
 namespace {
 
 constexpr size_t kAlign = 256;
+constexpr int kMaxSteps = RB_INTERP_MAX_STEPS;
 
 // workspace: per-target counts and segment offsets, keys and values before / after the sort, the scaled flow of every
 // source, the up/down neighbour count of the hole fill, then CUB's temporary storage
@@ -59,17 +60,25 @@ cudaError_t cub_temp_bytes(size_t n, size_t* bytes) {
   return e;
 }
 
-// One thread per source pixel: static mask, scaled flow, target key; counts by integer atomics (order-free).
+// Time steps or times of one multi-step call, passed by value in the kernel parameters: nothing to copy or allocate
+struct Steps {
+  float v[kMaxSteps];
+};
+
+// One thread per source pixel of every (step, sample): static mask, scaled flow, target key; counts by integer atomics
+// (order-free).  Source i belongs to step i / n_flow and reads flow[i % n_flow]; its target lies in its own sample.
 __global__ void __launch_bounds__(256) reverse_keys_kernel(const float2* __restrict__ flow, const void* __restrict__ bg,
                                                            const void* __restrict__ im0, int u8, int C, int H, int W,
-                                                           uint32_t n, float ts, uint32_t* __restrict__ counts,
-                                                           uint32_t* __restrict__ keys, uint32_t* __restrict__ vals,
-                                                           float2* __restrict__ fs, uint8_t* __restrict__ static_out) {
+                                                           uint32_t n, uint32_t n_flow, Steps steps,
+                                                           uint32_t* __restrict__ counts, uint32_t* __restrict__ keys,
+                                                           uint32_t* __restrict__ vals, float2* __restrict__ fs,
+                                                           uint8_t* __restrict__ static_out) {
   const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   const uint32_t hw = (uint32_t)H * W;
   const int x = (int)(i % W), y = (int)((i / W) % H);
   const uint32_t base = i - (i % hw);
+  const float ts = steps.v[i / n_flow];
   bool st = false;
   if (bg != nullptr) {  // static: every channel differs by < 10 (uint8: the wrapped difference, as numpy computes it)
     st = true;
@@ -85,7 +94,7 @@ __global__ void __launch_bounds__(256) reverse_keys_kernel(const float2* __restr
     }
   }
   if (static_out != nullptr) static_out[i] = st ? 1 : 0;
-  float2 f = st ? make_float2(INFINITY, INFINITY) : flow[i];
+  float2 f = st ? make_float2(INFINITY, INFINITY) : flow[i % n_flow];
   f.x = __fmul_rn(f.x, ts);
   f.y = __fmul_rn(f.y, ts);
   fs[i] = f;
@@ -145,11 +154,11 @@ __global__ void __launch_bounds__(256) reverse_average_kernel(const uint32_t* __
 // pixel's flow_t holds the running sum (+0.0 + up) + down and nfound the neighbours found so far.  Only non-empty
 // pixels are read as neighbours, so the sums never see each other.
 __global__ void __launch_bounds__(128) fill_columns_kernel(float2* __restrict__ ft, const uint8_t* __restrict__ empty,
-                                                           uint8_t* __restrict__ nfound, int B, int H, int W) {
-  const int t = blockIdx.x * blockDim.x + threadIdx.x;
-  if (t >= B * W) return;
-  const int b = t / W, x = t % W;
-  const size_t col = (size_t)b * H * W + x;
+                                                           uint8_t* __restrict__ nfound, size_t S, int H, int W) {
+  const size_t t = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= S * W) return;
+  const size_t b = t / W, x = t % W;
+  const size_t col = b * H * W + x;
   bool have = false;
   float2 last = make_float2(0.f, 0.f);
   for (int y = 0; y < H; ++y) {
@@ -179,10 +188,10 @@ __global__ void __launch_bounds__(128) fill_columns_kernel(float2* __restrict__ 
 // Pass 2: one thread per (sample, row) adds the nearest non-empty pixel on the left, then the right, and divides by the
 // number found (fp32, correctly rounded); none found gives +0.0.
 __global__ void __launch_bounds__(128) fill_rows_kernel(float2* __restrict__ ft, const uint8_t* __restrict__ empty,
-                                                        uint8_t* __restrict__ nfound, int B, int H, int W) {
-  const int t = blockIdx.x * blockDim.x + threadIdx.x;
-  if (t >= B * H) return;
-  const size_t row = (size_t)t * W;
+                                                        uint8_t* __restrict__ nfound, size_t S, int H, int W) {
+  const size_t t = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= S * H) return;
+  const size_t row = t * W;
   bool have = false;
   float2 last = make_float2(0.f, 0.f);
   for (int x = 0; x < W; ++x) {
@@ -231,42 +240,58 @@ __global__ void __launch_bounds__(256) erode5_kernel(const uint8_t* __restrict__
   out[i] = m;
 }
 
-// One thread per output pixel: both frames sampled at p + F_tk(p) (clamped to the frame; NaN -> 0) with the bilinear
-// arithmetic of rb_flow_fb_check, blended by (1-t, t) with empty targets weighted 0.
-__global__ void __launch_bounds__(256) frame_synthesize_kernel(const float* __restrict__ frames, int Hp, int Wp, int top,
+// the CLI's np.clip(np.rint(fl32(255 * x)), 0, 255), as rb_frame_metrics quantises: ties to even; fmaxf(NaN, 0) = 0
+__device__ __forceinline__ uint8_t quantise(float x) { return (uint8_t)fminf(fmaxf(rintf(__fmul_rn(255.f, x)), 0.f), 255.f); }
+
+// One thread per output pixel, blockIdx.y striding over the (time, sample) pairs (32-bit pixel indices): both frames sampled at p + F_tk(p) (clamped to the frame; NaN -> 0)
+// with the bilinear arithmetic of rb_flow_fb_check, blended by (1-t, t) with empty targets weighted 0; written as fp32,
+// or quantised to uint8 (with bgr: channels reversed).
+__global__ void __launch_bounds__(256) frame_synthesize_kernel(const float* __restrict__ frames0,
+                                                               const float* __restrict__ frames1, int Hp, int Wp, int top,
                                                                int left, const float2* __restrict__ f0,
                                                                const float2* __restrict__ f1,
                                                                const uint8_t* __restrict__ e0,
-                                                               const uint8_t* __restrict__ e1, float t,
-                                                               float* __restrict__ out, int B, int H, int W) {
-  const size_t p = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-  const size_t npix = (size_t)B * H * W;
-  if (p >= npix) return;
-  const int x = (int)(p % W), y = (int)((p / W) % H), b = (int)(p / ((size_t)H * W));
-  const float s = __fsub_rn(1.f, t);
-  float w0 = e0[p] ? 0.f : s, w1 = e1[p] ? 0.f : t;
-  if (w0 == 0.f && w1 == 0.f) w0 = s, w1 = t;
-  float v[2][3];
-  for (int k = 0; k < 2; ++k) {
-    const float2 F = (k == 0 ? f0 : f1)[p];
-    const float qx = fminf(fmaxf(__fadd_rn((float)x, F.x), 0.f), (float)(W - 1));
-    const float qy = fminf(fmaxf(__fadd_rn((float)y, F.y), 0.f), (float)(H - 1));
-    const int x0 = (int)floorf(qx), y0 = (int)floorf(qy);
-    const int x1 = min(x0 + 1, W - 1), y1 = min(y0 + 1, H - 1);
-    const float ax = __fsub_rn(qx, (float)x0), ay = __fsub_rn(qy, (float)y0);
-    const float cx = __fsub_rn(1.f, ax), cy = __fsub_rn(1.f, ay);
-    const float* img = frames + ((size_t)(k * B + b) * Hp + top) * Wp * 3 + (size_t)left * 3;
-    const float* r0 = img + (size_t)y0 * Wp * 3;
-    const float* r1 = img + (size_t)y1 * Wp * 3;
+                                                               const uint8_t* __restrict__ e1, Steps times, void* out,
+                                                               int out_u8, int bgr, int n_t, int B, int H, int W) {
+  const uint32_t q = blockIdx.x * blockDim.x + threadIdx.x;
+  const uint32_t hw = (uint32_t)H * W;
+  if (q >= hw) return;
+  const int x = (int)(q % W), y = (int)(q / W);
+  for (uint32_t smp = blockIdx.y; smp < (uint32_t)n_t * B; smp += gridDim.y) {
+    const int b = (int)(smp % B);
+    const size_t p = (size_t)smp * hw + q;
+    const float t = times.v[smp / B];
+    const float s = __fsub_rn(1.f, t);
+    float w0 = e0[p] ? 0.f : s, w1 = e1[p] ? 0.f : t;
+    if (w0 == 0.f && w1 == 0.f) w0 = s, w1 = t;
+    float v[2][3];
+    for (int k = 0; k < 2; ++k) {
+      const float2 F = (k == 0 ? f0 : f1)[p];
+      const float qx = fminf(fmaxf(__fadd_rn((float)x, F.x), 0.f), (float)(W - 1));
+      const float qy = fminf(fmaxf(__fadd_rn((float)y, F.y), 0.f), (float)(H - 1));
+      const int x0 = (int)floorf(qx), y0 = (int)floorf(qy);
+      const int x1 = min(x0 + 1, W - 1), y1 = min(y0 + 1, H - 1);
+      const float ax = __fsub_rn(qx, (float)x0), ay = __fsub_rn(qy, (float)y0);
+      const float cx = __fsub_rn(1.f, ax), cy = __fsub_rn(1.f, ay);
+      const float* img = (k == 0 ? frames0 : frames1) + ((size_t)b * Hp + top) * Wp * 3 + (size_t)left * 3;
+      const float* r0 = img + (size_t)y0 * Wp * 3;
+      const float* r1 = img + (size_t)y1 * Wp * 3;
+      for (int c = 0; c < 3; ++c) {
+        const float t0 = __fadd_rn(__fmul_rn(cx, r0[x0 * 3 + c]), __fmul_rn(ax, r0[x1 * 3 + c]));
+        const float t1 = __fadd_rn(__fmul_rn(cx, r1[x0 * 3 + c]), __fmul_rn(ax, r1[x1 * 3 + c]));
+        v[k][c] = __fadd_rn(__fmul_rn(t0, cy), __fmul_rn(t1, ay));
+      }
+    }
+    const float den = __fadd_rn(w0, w1);
     for (int c = 0; c < 3; ++c) {
-      const float t0 = __fadd_rn(__fmul_rn(cx, r0[x0 * 3 + c]), __fmul_rn(ax, r0[x1 * 3 + c]));
-      const float t1 = __fadd_rn(__fmul_rn(cx, r1[x0 * 3 + c]), __fmul_rn(ax, r1[x1 * 3 + c]));
-      v[k][c] = __fadd_rn(__fmul_rn(t0, cy), __fmul_rn(t1, ay));
+      const float o = __fdiv_rn(__fadd_rn(__fmul_rn(w0, v[0][c]), __fmul_rn(w1, v[1][c])), den);
+      const int oc = bgr ? 2 - c : c;
+      if (out_u8)
+        static_cast<uint8_t*>(out)[p * 3 + oc] = quantise(o);
+      else
+        static_cast<float*>(out)[p * 3 + oc] = o;
     }
   }
-  const float den = __fadd_rn(w0, w1);
-  for (int c = 0; c < 3; ++c)
-    out[p * 3 + c] = __fdiv_rn(__fadd_rn(__fmul_rn(w0, v[0][c]), __fmul_rn(w1, v[1][c])), den);
 }
 
 }  // namespace
@@ -274,13 +299,78 @@ __global__ void __launch_bounds__(256) frame_synthesize_kernel(const float* __re
 
 using namespace rb;
 
+namespace {
+
+// checks of the multi-step entries' shapes; n = n_steps * B * H * W keys must stay below 2^32 with the skip key n
+int reverse_shape(const char* fn, int n_steps, int B, int H, int W, size_t* n) {
+  RB_REQUIRE(n_steps > 0 && n_steps <= kMaxSteps, RB_ERR_BAD_ARG, "%s: %d time steps (1..%d)", fn, n_steps, kMaxSteps);
+  RB_REQUIRE(B > 0 && H > 0 && W > 0, RB_ERR_BAD_SHAPE, "%s: bad shape B=%d H=%d W=%d", fn, B, H, W);
+  *n = (size_t)n_steps * B * H * W;
+  RB_REQUIRE(*n + 1 < (size_t(1) << 32), RB_ERR_BAD_SHAPE,
+             "%s: n_steps*B*H*W = %zu pixels: keys need n_steps*B*H*W + 1 < 2^32", fn, *n);
+  return RB_OK;
+}
+
+// The reversal of flow01 [B,H,W,2] by n_steps time steps into [n_steps,B,H,W] samples (arguments checked by the caller)
+int reverse_run(const char* fn, const float* flow01, const void* bg, const void* im0, int img_u8, int img_channels,
+                const Steps& steps, int n_steps, float* flow_t, uint8_t* empty, uint8_t* multi, uint8_t* static_mask,
+                int B, int H, int W, void* workspace, size_t workspace_bytes, void* stream) {
+  const size_t n = (size_t)n_steps * B * H * W;
+  const ReverseWs l = reverse_layout(n);
+  // the fixed part is known without CUDA; CUB's share needs a device query
+  RB_REQUIRE(workspace_bytes >= l.fixed, RB_ERR_WORKSPACE, "%s: workspace of %zu bytes is too small", fn,
+             workspace_bytes);
+  size_t temp = 0;
+  RB_CHECK_CUDA(cub_temp_bytes(n, &temp));
+  RB_REQUIRE(workspace_bytes >= l.fixed + temp, RB_ERR_WORKSPACE, "%s: workspace of %zu bytes is too small (need %zu)",
+             fn, workspace_bytes, l.fixed + temp);
+  char* ws = static_cast<char*>(workspace);
+  uint32_t* counts = reinterpret_cast<uint32_t*>(ws + l.counts);
+  uint32_t* offsets = reinterpret_cast<uint32_t*>(ws + l.offsets);
+  uint32_t* keys_in = reinterpret_cast<uint32_t*>(ws + l.keys_in);
+  uint32_t* keys_out = reinterpret_cast<uint32_t*>(ws + l.keys_out);
+  uint32_t* vals_in = reinterpret_cast<uint32_t*>(ws + l.vals_in);
+  uint32_t* vals_out = reinterpret_cast<uint32_t*>(ws + l.vals_out);
+  float2* fs = reinterpret_cast<float2*>(ws + l.fs);
+  uint8_t* nfound = reinterpret_cast<uint8_t*>(ws + l.nfound);
+  const cudaStream_t st = (cudaStream_t)stream;
+  const uint32_t n32 = (uint32_t)n;
+  const unsigned blocks = (unsigned)((n + 255) / 256);
+  const size_t S = (size_t)n_steps * B;  // samples of the hole fill
+
+  RB_CHECK_CUDA(cudaMemsetAsync(counts, 0, n * sizeof(uint32_t), st));
+  reverse_keys_kernel<<<blocks, 256, 0, st>>>(reinterpret_cast<const float2*>(flow01), bg, im0, img_u8, img_channels, H,
+                                              W, n32, (uint32_t)((size_t)B * H * W), steps, counts, keys_in, vals_in, fs,
+                                              static_mask);
+  RB_CHECK_LAUNCH("reverse_keys_kernel");
+  size_t tb = temp;
+  RB_CHECK_CUDA(cub::DeviceScan::ExclusiveSum(ws + l.temp, tb, counts, offsets, n32, st));
+  tb = temp;
+  RB_CHECK_CUDA(cub::DeviceRadixSort::SortPairs(ws + l.temp, tb, keys_in, keys_out, vals_in, vals_out, n32, 0,
+                                                key_bits(n), st));
+  reverse_average_kernel<<<blocks, 256, 0, st>>>(counts, offsets, vals_out, fs, n32, reinterpret_cast<float2*>(flow_t),
+                                                 empty, multi);
+  RB_CHECK_LAUNCH("reverse_average_kernel");
+  fill_columns_kernel<<<(unsigned)((S * W + 127) / 128), 128, 0, st>>>(reinterpret_cast<float2*>(flow_t), empty, nfound,
+                                                                       S, H, W);
+  RB_CHECK_LAUNCH("fill_columns_kernel");
+  fill_rows_kernel<<<(unsigned)((S * H + 127) / 128), 128, 0, st>>>(reinterpret_cast<float2*>(flow_t), empty, nfound, S,
+                                                                    H, W);
+  RB_CHECK_LAUNCH("fill_rows_kernel");
+  return RB_OK;
+}
+
+}  // namespace
+
 extern "C" int rb_flow_reverse_workspace_bytes(int B, int H, int W, size_t* bytes) {
+  return rb_flow_reverse_multi_workspace_bytes(1, B, H, W, bytes);
+}
+
+extern "C" int rb_flow_reverse_multi_workspace_bytes(int n_steps, int B, int H, int W, size_t* bytes) {
   RB_REQUIRE(bytes, RB_ERR_BAD_ARG, "rb_flow_reverse_workspace_bytes: null pointer");
-  RB_REQUIRE(B > 0 && H > 0 && W > 0, RB_ERR_BAD_SHAPE, "rb_flow_reverse_workspace_bytes: bad shape B=%d H=%d W=%d", B,
-             H, W);
-  const size_t n = (size_t)B * H * W;
-  RB_REQUIRE(n + 1 < (size_t(1) << 32), RB_ERR_BAD_SHAPE,
-             "rb_flow_reverse_workspace_bytes: B*H*W = %zu pixels: keys need B*H*W + 1 < 2^32", n);
+  size_t n = 0;
+  const int rc = reverse_shape("rb_flow_reverse_workspace_bytes", n_steps, B, H, W, &n);
+  if (rc != RB_OK) return rc;
   size_t temp = 0;
   RB_CHECK_CUDA(cub_temp_bytes(n, &temp));
   *bytes = reverse_layout(n).fixed + temp;
@@ -301,65 +391,70 @@ extern "C" int rb_flow_reverse(const float* flow01, const void* bg, const void* 
   const size_t n = (size_t)B * H * W;
   RB_REQUIRE(n + 1 < (size_t(1) << 32), RB_ERR_BAD_SHAPE,
              "rb_flow_reverse: B*H*W = %zu pixels: keys need B*H*W + 1 < 2^32", n);
-  const ReverseWs l = reverse_layout(n);
-  // the fixed part is known without CUDA; CUB's share needs a device query
-  RB_REQUIRE(workspace_bytes >= l.fixed, RB_ERR_WORKSPACE, "rb_flow_reverse: workspace of %zu bytes is too small",
-             workspace_bytes);
-  size_t temp = 0;
-  RB_CHECK_CUDA(cub_temp_bytes(n, &temp));
-  RB_REQUIRE(workspace_bytes >= l.fixed + temp, RB_ERR_WORKSPACE,
-             "rb_flow_reverse: workspace of %zu bytes is too small (need %zu)", workspace_bytes, l.fixed + temp);
-  char* ws = static_cast<char*>(workspace);
-  uint32_t* counts = reinterpret_cast<uint32_t*>(ws + l.counts);
-  uint32_t* offsets = reinterpret_cast<uint32_t*>(ws + l.offsets);
-  uint32_t* keys_in = reinterpret_cast<uint32_t*>(ws + l.keys_in);
-  uint32_t* keys_out = reinterpret_cast<uint32_t*>(ws + l.keys_out);
-  uint32_t* vals_in = reinterpret_cast<uint32_t*>(ws + l.vals_in);
-  uint32_t* vals_out = reinterpret_cast<uint32_t*>(ws + l.vals_out);
-  float2* fs = reinterpret_cast<float2*>(ws + l.fs);
-  uint8_t* nfound = reinterpret_cast<uint8_t*>(ws + l.nfound);
-  const cudaStream_t st = (cudaStream_t)stream;
-  const uint32_t n32 = (uint32_t)n;
-  const unsigned blocks = (unsigned)((n + 255) / 256);
-
-  RB_CHECK_CUDA(cudaMemsetAsync(counts, 0, n * sizeof(uint32_t), st));
-  reverse_keys_kernel<<<blocks, 256, 0, st>>>(reinterpret_cast<const float2*>(flow01), bg, im0, img_u8, img_channels, H,
-                                              W, n32, time_step, counts, keys_in, vals_in, fs, static_mask);
-  RB_CHECK_LAUNCH("reverse_keys_kernel");
-  size_t tb = temp;
-  RB_CHECK_CUDA(cub::DeviceScan::ExclusiveSum(ws + l.temp, tb, counts, offsets, n32, st));
-  tb = temp;
-  RB_CHECK_CUDA(cub::DeviceRadixSort::SortPairs(ws + l.temp, tb, keys_in, keys_out, vals_in, vals_out, n32, 0,
-                                                key_bits(n), st));
-  reverse_average_kernel<<<blocks, 256, 0, st>>>(counts, offsets, vals_out, fs, n32, reinterpret_cast<float2*>(flow_t),
-                                                 empty, multi);
-  RB_CHECK_LAUNCH("reverse_average_kernel");
-  fill_columns_kernel<<<(B * W + 127) / 128, 128, 0, st>>>(reinterpret_cast<float2*>(flow_t), empty, nfound, B, H, W);
-  RB_CHECK_LAUNCH("fill_columns_kernel");
-  fill_rows_kernel<<<(B * H + 127) / 128, 128, 0, st>>>(reinterpret_cast<float2*>(flow_t), empty, nfound, B, H, W);
-  RB_CHECK_LAUNCH("fill_rows_kernel");
+  Steps steps;
+  steps.v[0] = time_step;
+  const int rc = reverse_run("rb_flow_reverse", flow01, bg, im0, img_u8, img_channels, steps, 1, flow_t, empty, multi,
+                             static_mask, B, H, W, workspace, workspace_bytes, stream);
+  if (rc != RB_OK) return rc;
   if (empty_eroded != nullptr) {
-    erode5_kernel<<<blocks, 256, 0, st>>>(empty, empty_eroded, H, W, n32);
+    erode5_kernel<<<(unsigned)((n + 255) / 256), 256, 0, (cudaStream_t)stream>>>(empty, empty_eroded, H, W, (uint32_t)n);
     RB_CHECK_LAUNCH("erode5_kernel");
   }
+  return RB_OK;
+}
+
+extern "C" int rb_flow_reverse_multi(const float* flow01, const float* time_steps, int n_steps, float* flow_t,
+                                     uint8_t* empty, uint8_t* multi, int B, int H, int W, void* workspace,
+                                     size_t workspace_bytes, void* stream) {
+  RB_REQUIRE(flow01 && time_steps && flow_t && empty && multi && workspace, RB_ERR_BAD_ARG,
+             "rb_flow_reverse_multi: null pointer");
+  size_t n = 0;
+  const int rc = reverse_shape("rb_flow_reverse_multi", n_steps, B, H, W, &n);
+  if (rc != RB_OK) return rc;
+  Steps steps;
+  for (int i = 0; i < n_steps; ++i) {
+    RB_REQUIRE(isfinite(time_steps[i]), RB_ERR_BAD_ARG, "rb_flow_reverse_multi: time_steps[%d] must be finite (got %g)",
+               i, (double)time_steps[i]);
+    steps.v[i] = time_steps[i];
+  }
+  return reverse_run("rb_flow_reverse_multi", flow01, nullptr, nullptr, 0, 0, steps, n_steps, flow_t, empty, multi,
+                     nullptr, B, H, W, workspace, workspace_bytes, stream);
+}
+
+extern "C" int rb_frame_synthesize_pairs(const float* frames0, const float* frames1, int Hp, int Wp, int top, int left,
+                                         const float* flow_t0, const float* flow_t1, const uint8_t* empty0,
+                                         const uint8_t* empty1, const float* ts, int n_t, void* out, int out_u8,
+                                         int bgr, int B, int H, int W, void* stream) {
+  RB_REQUIRE(frames0 && frames1 && flow_t0 && flow_t1 && empty0 && empty1 && ts && out, RB_ERR_BAD_ARG,
+             "rb_frame_synthesize: null pointer");
+  RB_REQUIRE(n_t > 0 && n_t <= kMaxSteps, RB_ERR_BAD_ARG, "rb_frame_synthesize: %d times (1..%d)", n_t, kMaxSteps);
+  RB_REQUIRE((out_u8 == 0 || out_u8 == 1) && (bgr == 0 || bgr == 1), RB_ERR_BAD_ARG,
+             "rb_frame_synthesize: out_u8 and bgr must be 0 or 1 (got %d, %d)", out_u8, bgr);
+  Steps times;
+  for (int i = 0; i < n_t; ++i) {
+    RB_REQUIRE(ts[i] >= 0.f && ts[i] <= 1.f, RB_ERR_BAD_ARG, "rb_frame_synthesize: t must be in [0, 1] (got %g)",
+               (double)ts[i]);
+    times.v[i] = ts[i];
+  }
+  RB_REQUIRE(B > 0 && H > 0 && W > 0, RB_ERR_BAD_SHAPE, "rb_frame_synthesize: bad shape B=%d H=%d W=%d", B, H, W);
+  RB_REQUIRE(top >= 0 && left >= 0 && top + H <= Hp && left + W <= Wp, RB_ERR_BAD_SHAPE,
+             "rb_frame_synthesize: crop (%d, %d) + %dx%d outside the %dx%d frames", top, left, H, W, Hp, Wp);
+  const size_t hw = (size_t)H * W;
+  RB_REQUIRE(hw < (size_t(1) << 32) && (size_t)n_t * B < (size_t(1) << 32), RB_ERR_BAD_SHAPE,
+             "rb_frame_synthesize: %zu pixels per frame or %zu frames exceed 32-bit indices", hw, (size_t)n_t * B);
+  const dim3 grid((unsigned)((hw + 255) / 256), (unsigned)std::min<size_t>((size_t)n_t * B, 65535));
+  frame_synthesize_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(
+      frames0, frames1, Hp, Wp, top, left, reinterpret_cast<const float2*>(flow_t0),
+      reinterpret_cast<const float2*>(flow_t1), empty0, empty1, times, out, out_u8, bgr, n_t, B, H, W);
+  RB_CHECK_LAUNCH("frame_synthesize_kernel");
   return RB_OK;
 }
 
 extern "C" int rb_frame_synthesize(const float* frames, int Hp, int Wp, int top, int left, const float* flow_t0,
                                    const float* flow_t1, const uint8_t* empty0, const uint8_t* empty1, float t,
                                    float* out, int B, int H, int W, void* stream) {
-  RB_REQUIRE(frames && flow_t0 && flow_t1 && empty0 && empty1 && out, RB_ERR_BAD_ARG,
-             "rb_frame_synthesize: null pointer");
-  RB_REQUIRE(t >= 0.f && t <= 1.f, RB_ERR_BAD_ARG, "rb_frame_synthesize: t must be in [0, 1] (got %g)", (double)t);
-  RB_REQUIRE(B > 0 && H > 0 && W > 0, RB_ERR_BAD_SHAPE, "rb_frame_synthesize: bad shape B=%d H=%d W=%d", B, H, W);
-  RB_REQUIRE(top >= 0 && left >= 0 && top + H <= Hp && left + W <= Wp, RB_ERR_BAD_SHAPE,
-             "rb_frame_synthesize: crop (%d, %d) + %dx%d outside the %dx%d frames", top, left, H, W, Hp, Wp);
-  const size_t npix = (size_t)B * H * W;
-  const size_t blocks = (npix + 255) / 256;
-  RB_REQUIRE(blocks <= 0x7fffffffu, RB_ERR_BAD_SHAPE, "rb_frame_synthesize: %zu pixels exceed one grid", npix);
-  frame_synthesize_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(
-      frames, Hp, Wp, top, left, reinterpret_cast<const float2*>(flow_t0), reinterpret_cast<const float2*>(flow_t1),
-      empty0, empty1, t, out, B, H, W);
-  RB_CHECK_LAUNCH("frame_synthesize_kernel");
-  return RB_OK;
+  // frames = [I0 | I1]; a bad shape is refused by the call below, with frames1 = frames
+  const size_t frame1 = B > 0 && Hp > 0 && Wp > 0 ? (size_t)B * Hp * Wp * 3 : 0;
+  return rb_frame_synthesize_pairs(frames, frames == nullptr ? nullptr : frames + frame1, Hp, Wp, top, left, flow_t0,
+                                   flow_t1, empty0, empty1, &t, 1, out, 0, 0, B, H, W, stream);
 }

@@ -41,7 +41,14 @@ SSIM: ...``) and written with the per-triplet records to ``<--out>/val_vimeo.jso
 encoded once, --batch pairs per pass, coloured on the GPU (raft_b200.video):
 
     python infer_raft.py --path frames/ --out flows/ --load raft-things.npz [--batch 8 | --warm-start]
+
+--path DIR --interpolate T [T ...] is frame-rate up-conversion instead: DIR's frames and, between every consecutive pair,
+the frames at times T (strictly increasing inside (0, 1)), written as one sequence ``<--out>/frame_<n:06d>.png`` (input
+frame k is n = k (m + 1) for m times), --batch pairs per pass, each frame encoded once per pass (raft_b200.video):
+
+    python infer_raft.py --path frames/ --out slow/ --interpolate 0.25 0.5 0.75 --load raft-things.npz [--batch 8]
 """
+import glob
 import argparse
 import os
 import sys
@@ -112,7 +119,9 @@ def parser():
     p.add_argument('--bidirectional', action='store_true',
                    help='extension: also the backward flow and the forward-backward occlusion masks')
     p.add_argument('--interpolate', type=float, nargs='+', default=None, metavar='T',
-                   help='extension: also write the frames at times T in [0, 1] between im1 and im2 (raft_interp_<k>.png)')
+                   help='extension: also write the frames at times T in [0, 1] between im1 and im2 (raft_interp_<k>.png); '
+                        'with --path, the up-converted sequence <--out>/frame_<n:06d>.png (T strictly increasing inside '
+                        '(0, 1))')
     p.add_argument('--native-flow', action='store_true',
                    help="extension: resize the written flow(s) back to im1's size (flow_utils.resize_flow)")
     p.add_argument('--upstream', action='store_true',
@@ -144,9 +153,24 @@ def main(argv=None):
         print(f"mode '{args.mode}' has no implementation in the reference either (infer_raft.py:71-95); nothing to do")
         return 0
     if args.path is not None:
-        if args.bidirectional or args.interpolate:
-            p.error('--path runs forward flow over a frame sequence; it cannot be combined with --bidirectional or '
-                    '--interpolate')
+        if args.bidirectional:
+            p.error('--path runs forward flow or frame interpolation over a frame sequence; it cannot be combined with '
+                    '--bidirectional')
+        if args.interpolate:
+            for flag, given in (('--warm-start', args.warm_start), ('--native-flow', args.native_flow),
+                                ('--flo', args.flo), ('--npy', args.npy)):
+                if given:
+                    p.error(f'--path --interpolate writes frames, not flows: it cannot be combined with {flag}')
+            ts = args.interpolate
+            if not all(0.0 < t < 1.0 for t in ts) or any(b <= a for a, b in zip(ts, ts[1:])):
+                p.error('--path --interpolate: the times T must be strictly increasing inside (0, 1) (the input frames '
+                        'are the times 0 and 1)')
+            if args.batch < 1 or args.workers < 0:
+                p.error('--path needs --batch >= 1 and --workers >= 0')
+            n = len(glob.glob(os.path.join(args.path, '*.png')) + glob.glob(os.path.join(args.path, '*.jpg')))
+            if n < 2:
+                p.error(f'--path --interpolate: {args.path} holds {n} *.png / *.jpg frames; interpolation needs two')
+            return run_video_interpolate(args)
         if args.warm_start and args.batch != 1:
             p.error('--path --warm-start warm-starts each pair from the one before: it runs one pair per pass (--batch 1)')
         if args.batch < 1 or args.workers < 0:
@@ -212,6 +236,20 @@ def run_video(args):
                   flo=args.flo, npy=args.npy, native_flow=args.native_flow)
     print(f"{len(files)} files written under {args.out}" + (" and the --flo / --npy directories" if args.flo or args.npy
                                                             else ""))
+    return 0
+
+
+def run_video_interpolate(args):
+    """--path --interpolate: raft_b200.video.video_interpolate over the frames of --path, at 432x1024 like test mode (or
+    their own size with --keep-size)."""
+    from networks import RAFT
+    from raft_b200.video import video_interpolate
+    iters = 20 if args.iters is None else args.iters
+    size = None if args.keep_size else (432, 1024)
+    model = RAFT.RAFT(None if size is None else size + (3,), args, iters=iters, input_size=size, upstream=args.upstream,
+                      mixed_precision=args.mixed_precision).load(args.load)
+    files = video_interpolate(model, args.path, args.out, args.interpolate, batch=args.batch, workers=args.workers)
+    print(f"{len(files)} frames written under {args.out}")
     return 0
 
 

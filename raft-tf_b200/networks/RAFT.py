@@ -148,6 +148,28 @@ class RAFT(object):
         return tuple(None if t is None else t.clone() for t in out)
 
     @torch.no_grad()
+    def forward_sequence_bidirectional(self, frames, check=True):
+        """Extension (frame interpolation over a video): the flows both ways between consecutive frames of [T+1,H,W,3]
+        frames (dtypes and sources as for ``forward``), each frame encoded once and the 2T pairs run as one batch.  Returns
+        fresh tensors ``(flow_fw, flow_bw, occ_fw, occ_bw)`` in pair order: flow_fw[k] equals ``forward(f_k, f_(k+1))`` and
+        flow_bw[k] equals ``forward(f_(k+1), f_k)`` bit for bit ([T,H,W,2]), and the [T,H,W] uint8 masks are those of
+        ``forward_bidirectional(f_k, f_(k+1))``; check=False returns None for both masks."""
+        out = self.engine().forward_sequence_bidirectional(_as_tensor(frames), check=check)
+        return tuple(None if t is None else t.clone() for t in out)
+
+    @torch.no_grad()
+    def interpolate_sequence(self, frames, t=0.5, uint8=False, bgr=False):
+        """Extension (frame-rate up-conversion): the frames at time t (a float, or a sequence of times, each in [0, 1])
+        between every pair of consecutive frames of [T+1,H,W,3] frames, from one ``forward_sequence_bidirectional`` pass.
+        A float t gives a fresh [T,H,W,3] tensor, a sequence of n times [n,T,H,W,3]; pair k equals
+        ``interpolate(frames[k:k+1], frames[k+1:k+2], t)`` bit for bit.  fp32 in [0,1] by default; uint8=True quantises
+        on the GPU exactly as infer_raft.py writes PNGs (np.clip(np.rint(255 x), 0, 255)), and bgr=True (with uint8)
+        reverses the channels, for RGB frames written by cv2.  A t outside [0, 1] raises ValueError."""
+        scalar = np.ndim(t) == 0
+        out = self.engine().interpolate_sequence(_as_tensor(frames), [t] if scalar else list(t), uint8=uint8, bgr=bgr)
+        return out[0] if scalar else out
+
+    @torch.no_grad()
     def interpolate(self, input_left, input_right, t=0.5):
         """Extension (the reference computes the flow for frame interpolation and projects it to time t with
         flow_utils.py:166 on the CPU): the frames at time t between left (t = 0) and right (t = 1).  One bidirectional

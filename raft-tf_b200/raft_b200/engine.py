@@ -12,6 +12,10 @@ rb_coords_grid and rb_coords_to_flow (flow_low) after the loop, captured as a mo
 forward_sequence(frames) is video: T + 1 frames give the T flows f_k -> f_(k+1), fnet once per frame, fmap1 = fmaps[:T] and
 fmap2 = fmaps[1:] as overlapping views (SEQUENCE); carry=True continues from the previous call's last frame, whose image
 and feature map the graph copies to row 0 before it encodes only the T new frames.
+forward_sequence_bidirectional(frames) runs both directions of the T pairs of T + 1 frames as 2T pairs in the palindrome
+order (0->1), ..., (T-1->T), (T->T-1), ..., (1->0): fmaps = [f_0 .. f_T, f_(T-1) .. f_0], so fmap1 = fmaps[:2T] and
+fmap2 = fmaps[1:] overlap as in SEQUENCE, fnet and cnet run once per frame and the mirrored rows are device copies
+(SEQUENCE_BIDIRECTIONAL); interpolate_sequence adds the per-t work of interpolate to it.
 With input_size set, every mode first resizes the frames to that size like the reference's cv2.resize (rb_frames_resize,
 csrc/resize.cu, in the graph in place of rb_frames_prepare), and its outputs come back at that size.
 """
@@ -30,8 +34,10 @@ from .weights import pack_update_block
 # what one pass computes: L->R only (forward), both directions (forward_bidirectional), both plus the occlusion check,
 # both directions for interpolate (which also holds the buffers of the per-t calls), L->R warm-started from flow_init with
 # the 1/8-resolution flow kept (forward(flow_init=..., return_low=True)), T consecutive pairs of T + 1 frames, always
-# started from flow_init (forward_sequence)
-FORWARD, BIDIRECTIONAL, BIDIRECTIONAL_CHECK, INTERPOLATE, FORWARD_WARM, SEQUENCE = 0, 1, 2, 3, 4, 5
+# started from flow_init (forward_sequence), both directions of T consecutive pairs (forward_sequence_bidirectional and
+# interpolate_sequence)
+FORWARD, BIDIRECTIONAL, BIDIRECTIONAL_CHECK, INTERPOLATE, FORWARD_WARM, SEQUENCE, SEQUENCE_BIDIRECTIONAL = range(7)
+SEQUENCES = (SEQUENCE, SEQUENCE_BIDIRECTIONAL)
 # forward-backward consistency thresholds of UnFlow (Meister et al. 2018): |f+b|^2 > a1 (|f|^2 + |b|^2) + a2
 FB_ALPHA1, FB_ALPHA2 = 0.01, 0.5
 # smallest frame side: the 4-level correlation pyramid needs a 1/8-resolution grid of at least 8 (level 3 is grid >> 3),
@@ -41,18 +47,22 @@ MIN_FRAME = 57
 MIN_FRAME_UPSTREAM = 121
 # upstream InputPadder's modes (pad_mode)
 PAD_MODES = ("sintel", "kitti")
+# most bytes the flow-reversal workspace of one interpolation chunk may take: interpolate and interpolate_sequence reverse
+# the flows of as many times at once as fit (rb_flow_reverse_multi), at least one; the results do not depend on it
+REVERSE_WS_BOUND = 1 << 30
+RB_INTERP_MAX_STEPS = 64  # include/raft_b200.h: times per rb_flow_reverse_multi / rb_frame_synthesize_pairs call
 
 
 def _kept(parked, key):
     """Whether a call keyed `key` = (B, H, W, u8, mode) keeps the parked buffers of `parked`.  The pair modes keep each
-    other at one (B, H, W, u8), as before; the sequence buffers survive any pair-mode call at the same frame size (a carry
-    continues across them), and a sequence call keeps the pair modes' buffers at its frame size and dtype.  A sequence
-    call of another T or dtype replaces the sequence buffers."""
-    if parked[4] == SEQUENCE and key[4] == SEQUENCE:
+    other at one (B, H, W, u8), as before; the buffers of each sequence mode survive any call of another mode at the same
+    frame size (a carry continues across them), and a sequence call keeps the pair modes' buffers at its frame size and
+    dtype.  A sequence call of another T or dtype replaces the buffers of its own mode."""
+    if parked[4] == key[4] and key[4] in SEQUENCES:
         return parked == key
-    if parked[4] == SEQUENCE:
+    if parked[4] in SEQUENCES:
         return parked[1:3] == key[1:3]
-    if key[4] == SEQUENCE:
+    if key[4] in SEQUENCES:
         return parked[1:4] == key[1:4]
     return parked[:4] == key[:4]
 
@@ -60,7 +70,7 @@ def _kept(parked, key):
 class RaftEngine:
     # everything _ensure allocates for one (B, H, W, u8, mode); parked per mode so alternating modes re-captures nothing
     _STATE = ("_key", "src_hw", "pad", "h", "w", "Hp", "Wp", "pairs", "pyr_bytes", "pyramid", "cws_bytes", "corr_ws",
-              "ws_bytes", "ws", "coords1", "mask", "flow_up", "occ", "rev_ws_bytes", "rev_ws", "flow_t", "empty_t", "flow_init", "flow_low", "fmaps", "fmap1", "fmap2", "cmap", "images", "staged", "raw",
+              "ws_bytes", "ws", "coords1", "mask", "flow_up", "occ", "rev_ws_bytes", "rev_ws", "rev_steps", "flow_t", "empty_t", "flow_bw", "flow_init", "flow_low", "fmaps", "fmap1", "fmap2", "cmap", "images", "staged", "raw",
               "seq_enc", "_shape", "_graph", "_graph_carry")
 
     def __init__(self, params: Dict[str, np.ndarray], small: bool = False, iters: int = 20,
@@ -160,7 +170,7 @@ class RaftEngine:
             self.__dict__.update(self._parked.pop(key))
             return
         bidir = mode not in (FORWARD, FORWARD_WARM, SEQUENCE)
-        seq = mode == SEQUENCE
+        seq = mode in SEQUENCES
         NB = 2 * B if bidir else B  # frame pairs through the hot path
         ph, pw = (-H) % 8, (-W) % 8
         top = 0 if self.pad_mode == "kitti" else ph // 2
@@ -183,35 +193,40 @@ class RaftEngine:
         self.coords1 = torch.empty(NB, h, w, 2, dtype=torch.float32, device=d)
         self.mask = None if self.small else torch.empty(NB, h, w, 576, dtype=torch.float32, device=d)
         self.flow_up = torch.empty(NB, H, W, 2, dtype=torch.float32, device=d)  # bidirectional: [L->R | R->L]
-        self.occ = torch.empty(2 * B, H, W, dtype=torch.uint8, device=d) if mode == BIDIRECTIONAL_CHECK else None
-        if mode == INTERPOLATE:  # per t: flow and empty mask from time t to frame 0 ([0]) and to frame 1 ([1])
-            self.rev_ws_bytes = capi.size_query(lib.rb_flow_reverse_workspace_bytes, B, H, W)
-            self.rev_ws = torch.empty(self.rev_ws_bytes, dtype=torch.uint8, device=d)
-            self.flow_t = torch.empty(2, B, H, W, 2, dtype=torch.float32, device=d)
-            self.empty_t = torch.empty(2, 2, B, H, W, dtype=torch.uint8, device=d)  # [empty | multi]
-        else:
-            self.rev_ws_bytes, self.rev_ws, self.flow_t, self.empty_t = 0, None, None, None
+        self.occ = (torch.empty(2 * B, H, W, dtype=torch.uint8, device=d)
+                    if mode in (BIDIRECTIONAL_CHECK, SEQUENCE_BIDIRECTIONAL) else None)
+        # SEQUENCE_BIDIRECTIONAL: the backward flows in pair order (the pass leaves them in rows 2T-1 .. T)
+        self.flow_bw = torch.empty(B, H, W, 2, dtype=torch.float32, device=d) if mode == SEQUENCE_BIDIRECTIONAL else None
+        # the per-t buffers of interpolate / interpolate_sequence, allocated by _synthesize for the chunk it runs
+        self.rev_ws_bytes, self.rev_ws, self.rev_steps, self.flow_t, self.empty_t = 0, None, 0, None, None
         if mode in (FORWARD_WARM, SEQUENCE):  # the caller's initial flow (copied in before each replay), the final 1/8-res flow
             self.flow_init = torch.zeros(B, h, w, 2, dtype=torch.float32, device=d)
             self.flow_low = torch.empty(B, h, w, 2, dtype=torch.float32, device=d)
         else:
             self.flow_init, self.flow_low = None, None
-        # SEQUENCE: B = T pairs of T + 1 frames; fmap1 = fmaps[:T] and fmap2 = fmaps[1:] overlap, no copy
+        # SEQUENCE: B = T pairs of T + 1 frames; fmap1 = fmaps[:T] and fmap2 = fmaps[1:] overlap, no copy.
+        # SEQUENCE_BIDIRECTIONAL: 2T pairs, fmaps = [f_0 .. f_T, f_(T-1) .. f_0] (2T + 1 rows), fmap1 = fmaps[:2T] and
+        # fmap2 = fmaps[1:]; cmap = [c_0 .. c_T, c_(T-1) .. c_1]
         nframes = B + 1 if seq else 2 * B
-        self.fmaps = torch.empty(nframes if seq else NB + B, h, w, self.fdim, dtype=torch.float32, device=d)
+        self.fmaps = torch.empty(NB + 1 if seq else NB + B, h, w, self.fdim, dtype=torch.float32, device=d)
         self.fmap1, self.fmap2 = self.fmaps[:NB], self.fmaps[1 if seq else B:]
         self.cmap = torch.empty(NB, h, w, self.hidden + self.ctx, dtype=torch.float32, device=d)
         self.images = torch.empty(nframes, Hp, Wp, 3, dtype=torch.float32, device=d)  # [left | right], [0,1], padded
         # staging buffer of the raw frames (uint8 or unpadded fp32, at the frames' own size); fp32 frames that need no
         # resize and no padding go straight into self.images -- except in SEQUENCE, whose carry graph reads the previous
         # call's last frame from self.images, so the new frames must not land there before the replay
-        self.staged = bool(u8 or ph or pw or self.input_size is not None or seq)
+        self.staged = bool(u8 or ph or pw or self.input_size is not None or mode == SEQUENCE)
         self.raw = torch.empty(nframes, *src_hw, 3, dtype=torch.uint8 if u8 else torch.float32, device=d) if self.staged else None
         # SEQUENCE: the feature encoder sees T + 1 frames in the fresh graph and T in the carry graph, the context encoder T;
         # encoders with workspaces of their own keep the pointers each graph was captured with (CudaEncoder reallocates its
         # workspace when its batch changes), whatever the other modes run in between
-        self.seq_enc = ((self.fnet.with_own_workspace(), self.fnet.with_own_workspace(), self.cnet.with_own_workspace())
-                        if seq else None)
+        # SEQUENCE_BIDIRECTIONAL: both encoders see the T + 1 frames (twins for the same reason)
+        if mode == SEQUENCE:
+            self.seq_enc = (self.fnet.with_own_workspace(), self.fnet.with_own_workspace(), self.cnet.with_own_workspace())
+        elif mode == SEQUENCE_BIDIRECTIONAL:
+            self.seq_enc = (self.fnet.with_own_workspace(), self.cnet.with_own_workspace())
+        else:
+            self.seq_enc = None
         self.src_hw = src_hw
         self._key = key
         self._shape = (B, H, W, u8, mode)
@@ -230,9 +245,10 @@ class RaftEngine:
         Bidirectional modes: cnet runs on all 2B frames (the R->L pairs need the context of R), and the last B feature
         maps are a device-to-device copy of the first B (a copy-engine transfer, no kernel)."""
         B, H, W, u8, mode = self._shape
-        bidir = mode not in (FORWARD, FORWARD_WARM, SEQUENCE)
+        bidir = mode not in (FORWARD, FORWARD_WARM, SEQUENCE, SEQUENCE_BIDIRECTIONAL)
         cnet, cframes = (self.cnet_bidir, self.images) if bidir else (self.cnet, self.images[:B])
         fnet, fout = self.fnet, self.fmaps[:2 * B]  # [fL | fR]
+        cout = self.cmap
         raw, images = self.raw, self.images
         capi.check(capi.lib.rb_set_math_mode(self.math_mode))  # per-thread library state: set before ANY kernel of ours
         capi.check(capi.lib.rb_set_semantics(self.semantics))
@@ -245,6 +261,9 @@ class RaftEngine:
                 fnet, fout = fnet_carry, self.fmaps[1:]
             else:
                 fnet, fout = fnet_fresh, self.fmaps
+        elif mode == SEQUENCE_BIDIRECTIONAL:  # B = T: both encoders on the T + 1 frames, the mirrored rows copied below
+            fnet, cnet = self.seq_enc
+            fout, cframes, cout = self.fmaps[:B + 1], self.images, self.cmap[:B + 1]
         n = images.shape[0]
         if self.input_size is not None:  # F3: cv2 resize, u8 -> fp32 /255 and replicate padding in one pass (csrc/resize.cu)
             capi.check(capi.lib.rb_frames_resize(capi.ptr(raw), int(u8), capi.ptr(images), n, *self.src_hw,
@@ -258,11 +277,17 @@ class RaftEngine:
         side = self._enc_stream
         side.wait_stream(main)  # fork: the frames are in place
         with torch.cuda.stream(side):
-            cnet(cframes, out=self.cmap)
+            cnet(cframes, out=cout)
+            if mode == SEQUENCE_BIDIRECTIONAL:  # cmap row T + i = c_(T-1-i): T - 1 copies
+                for i in range(B - 1):
+                    self.cmap[B + 1 + i].copy_(self.cmap[B - 1 - i])
         fnet(images, out=fout)
         self._cnet_pending = True
         if bidir:
             self.fmaps[2 * B:].copy_(self.fmaps[:B])  # contiguous, same dtype: cudaMemcpyAsync on the current stream
+        elif mode == SEQUENCE_BIDIRECTIONAL:  # fmaps row T + 1 + i = f_(T-1-i): T copies
+            for i in range(B):
+                self.fmaps[B + 1 + i].copy_(self.fmaps[B - 1 - i])
         if self._cnet_pending and not defer_join:
             self._join_cnet()
 
@@ -312,6 +337,9 @@ class RaftEngine:
             capi.check(lib.rb_flow_fb_check(capi.ptr(self.flow_up[:B0]), capi.ptr(self.flow_up[B0:]), capi.ptr(self.occ[:B0]),
                                             capi.ptr(self.occ[B0:]), B0, H, W, self.flow_scale, FB_ALPHA1,
                                             FB_ALPHA2, st))
+        elif mode == SEQUENCE_BIDIRECTIONAL:  # pair (k+1 -> k) is row 2T-1-k: T copies into pair order
+            for k in range(B0):
+                self.flow_bw[k].copy_(self.flow_up[2 * B0 - 1 - k])
 
     def _all(self):
         self.encode(defer_join=True)
@@ -449,37 +477,111 @@ class RaftEngine:
         return (self.flow_up[:B], self.flow_up[B:]) + occ
 
     @torch.no_grad()
+    def forward_sequence_bidirectional(self, frames: torch.Tensor, check: bool = True):
+        """Both directions of the T pairs of [T+1,H,W,3] frames (dtypes, sizes, input_size and padding as for forward())
+        in one pass.  Returns (flow_fw, flow_bw, occ_fw, occ_bw): [T,H,W,2] fp32 flows in pair order, flow_fw[k] = f_k ->
+        f_(k+1) bit-identical to forward(f_k, f_(k+1)) and flow_bw[k] = f_(k+1) -> f_k bit-identical to
+        forward(f_(k+1), f_k), and the [T,H,W] uint8 masks of forward_bidirectional(f_k, f_(k+1)) (None when check is
+        False; the check runs eagerly after the replay).  The 2T pairs run as one batch in the palindrome order (0->1), ...,
+        (T-1->T), (T->T-1), ..., (1->0), so each frame goes through fnet once and cnet once; the mirrored feature and context
+        rows and the backward flows in pair order are device copies in the graph.  Views of engine-owned buffers,
+        overwritten by the next call.  Alternating with the other modes at one frame size keeps every mode's buffers and
+        graph, and a pending forward_sequence carry survives it."""
+        self._run_sequence(frames)
+        T, H, W = self._shape[:3]
+        if not check:
+            return self.flow_up[:T], self.flow_bw, None, None
+        with torch.cuda.device(self.device):
+            capi.check(capi.lib.rb_flow_fb_check(capi.ptr(self.flow_up[:T]), capi.ptr(self.flow_bw),
+                                                 capi.ptr(self.occ[:T]), capi.ptr(self.occ[T:]), T, H, W, self.flow_scale,
+                                                 FB_ALPHA1, FB_ALPHA2, capi.stream()))
+        return self.flow_up[:T], self.flow_bw, self.occ[:T], self.occ[T:]
+
+    @torch.no_grad()
     def interpolate(self, left: torch.Tensor, right: torch.Tensor, ts) -> torch.Tensor:
         """Frames at times ts (each in [0, 1]; 0 = left, 1 = right) between B frame pairs: one bidirectional pass (as
-        forward_bidirectional(check=False), from a graph of its own), then per t, eagerly on the same stream,
-        rb_flow_reverse(flow_fw, t) -> flow and empty mask from t to left, rb_flow_reverse(flow_bw, 1 - t) -> from t to
-        right, and rb_frame_synthesize on the padded frames the pass used.  raft-small's reference flow is in 1/8-resolution
-        units, so its time steps are 8t and 8(1 - t) (exact: scaling by 8 commutes with fp32 rounding); upstream, t.  Frames as for
-        forward().  Returns a fresh [T,B,H,W,3] fp32 tensor, BGR in [0,1] (uint8 frames are divided by 255 first)."""
-        ts = [float(t) for t in ts]
-        if not ts or not all(0.0 <= t <= 1.0 for t in ts):
-            raise ValueError(f"raft_b200: interpolation times must be a non-empty list in [0, 1] (got {ts})")
+        forward_bidirectional(check=False), from a graph of its own), then eagerly on the same stream, for as many times
+        at once as REVERSE_WS_BOUND allows, rb_flow_reverse_multi(flow_fw, t) -> flow and empty mask from t to left,
+        rb_flow_reverse_multi(flow_bw, 1 - t) -> from t to right, and rb_frame_synthesize_pairs on the padded frames the
+        pass used.  raft-small's reference flow is in 1/8-resolution units, so its time steps are 8t and 8(1 - t) (exact:
+        scaling by 8 commutes with fp32 rounding); upstream, t.  Frames as for forward().  Returns a fresh [T,B,H,W,3] fp32
+        tensor, BGR in [0,1] (uint8 frames are divided by 255 first)."""
+        ts = _times(ts)
         self._run_frames(left, right, INTERPOLATE)
+        B = self._shape[0]
+        return self._synthesize(self.flow_up[:B], self.flow_up[B:], self.images[:B], self.images[B:], ts)
+
+    @torch.no_grad()
+    def interpolate_sequence(self, frames: torch.Tensor, ts, uint8: bool = False, bgr: bool = False) -> torch.Tensor:
+        """Frame-rate up-conversion: the frames at times ts (each in [0, 1]) between every pair of consecutive frames of
+        [T+1,H,W,3] frames, from one forward_sequence_bidirectional(check=False) pass and the per-t work of interpolate
+        on its flows.  Returns a fresh [len(ts),T,H,W,3] tensor; [:, k] equals interpolate(f_k, f_(k+1), ts)[:, 0] bit for
+        bit.  uint8=True quantises on the GPU as the CLI writes its PNGs (np.clip(np.rint(255 x), 0, 255), NaN -> 0), and
+        bgr=True then reverses the channels (RGB frames of an upstream model written as BGR)."""
+        ts = _times(ts)
+        if bgr and not uint8:
+            raise ValueError("raft_b200: bgr swaps the channels of uint8 output; pass uint8=True")
+        self._run_sequence(frames)
+        T = self._shape[0]
+        return self._synthesize(self.flow_up[:T], self.flow_bw, self.images[:T], self.images[1:], ts, uint8, bgr)
+
+    def _synthesize(self, flow_fw, flow_bw, frames0, frames1, ts, uint8=False, bgr=False) -> torch.Tensor:
+        """The per-t work of interpolate and interpolate_sequence on the B pairs of the last pass: per chunk of times, one
+        multi-step reversal per direction (steps s t and s (1 - t), s = flow_scale) and one blend of frames0[b] and
+        frames1[b] into a fresh [len(ts),B,H,W,3] tensor.  A chunk is as many times as keep the reversal workspace within
+        REVERSE_WS_BOUND (at least one, at most RB_INTERP_MAX_STEPS); each sample's bits do not depend on it."""
         B, H, W = self._shape[:3]
-        out = torch.empty(len(ts), B, H, W, 3, dtype=torch.float32, device=self.device)
+        lib = capi.lib
+        out = torch.empty(len(ts), B, H, W, 3, dtype=torch.uint8 if uint8 else torch.float32, device=self.device)
+        chunk = min(len(ts), RB_INTERP_MAX_STEPS)
+        while chunk > 1 and capi.size_query(lib.rb_flow_reverse_multi_workspace_bytes, chunk, B, H, W) > REVERSE_WS_BOUND:
+            chunk = max(1, chunk // 2)
         with torch.cuda.device(self.device):
-            for k, t in enumerate(ts):
-                self._interpolate_at(t, out[k])
+            for i in range(0, len(ts), chunk):
+                self._reverse_and_blend(flow_fw, flow_bw, frames0, frames1, ts[i:i + chunk], out[i:i + chunk], uint8, bgr)
         return out
 
     def _interpolate_at(self, t: float, out: torch.Tensor):
-        """The per-t work of interpolate on the flows of the last INTERPOLATE pass: two reversals and the blend into
-        out [B,H,W,3]."""
+        """The per-t work of interpolate for one t on the flows of the last INTERPOLATE pass, into out [B,H,W,3] fp32."""
+        B = self._shape[0]
+        self._reverse_and_blend(self.flow_up[:B], self.flow_up[B:], self.images[:B], self.images[B:], [t], out[None])
+
+    def _reverse_and_blend(self, flow_fw, flow_bw, frames0, frames1, ts, out, uint8=False, bgr=False):
+        """One chunk: rb_flow_reverse_multi of flow_fw by s t and of flow_bw by s (1 - t) for the n = len(ts) times, then
+        rb_frame_synthesize_pairs into out [n,B,H,W,3]; the reversal buffers are (re)allocated for n times."""
         B, H, W = self._shape[:3]
-        s = self.flow_scale
-        lib, st, ptr = capi.lib, capi.stream(), capi.ptr
-        for d, (flow, step) in enumerate(((self.flow_up[:B], s * t), (self.flow_up[B:], s * (1.0 - t)))):
-            capi.check(lib.rb_flow_reverse(ptr(flow), None, None, 0, 0, step, ptr(self.flow_t[d]), ptr(self.empty_t[0, d]),
-                                           ptr(self.empty_t[1, d]), None, None, B, H, W, ptr(self.rev_ws),
-                                           self.rev_ws_bytes, st))
-        capi.check(lib.rb_frame_synthesize(ptr(self.images), self.Hp, self.Wp, self.pad[0], self.pad[2],
-                                           ptr(self.flow_t[0]), ptr(self.flow_t[1]), ptr(self.empty_t[0, 0]),
-                                           ptr(self.empty_t[0, 1]), t, ptr(out), B, H, W, st))
+        n, s, d = len(ts), self.flow_scale, self.device
+        lib, ptr = capi.lib, capi.ptr
+        if self.rev_steps != n:
+            self.rev_ws_bytes = capi.size_query(lib.rb_flow_reverse_multi_workspace_bytes, n, B, H, W)
+            self.rev_ws = torch.empty(self.rev_ws_bytes, dtype=torch.uint8, device=d)
+            self.flow_t = torch.empty(2, n, B, H, W, 2, dtype=torch.float32, device=d)  # from t to frame 0 | to frame 1
+            self.empty_t = torch.empty(2, 2, n, B, H, W, dtype=torch.uint8, device=d)  # [empty | multi] x direction
+            self.rev_steps = n
+        st = capi.stream()
+        for k, (flow, steps) in enumerate(((flow_fw, [s * t for t in ts]), (flow_bw, [s * (1.0 - t) for t in ts]))):
+            capi.check(lib.rb_flow_reverse_multi(ptr(flow), _floats(steps), n, ptr(self.flow_t[k]), ptr(self.empty_t[0, k]),
+                                                 ptr(self.empty_t[1, k]), B, H, W, ptr(self.rev_ws), self.rev_ws_bytes, st))
+        capi.check(lib.rb_frame_synthesize_pairs(ptr(frames0), ptr(frames1), self.Hp, self.Wp, self.pad[0], self.pad[2],
+                                                 ptr(self.flow_t[0]), ptr(self.flow_t[1]), ptr(self.empty_t[0, 0]),
+                                                 ptr(self.empty_t[0, 1]), _floats(ts), n, ptr(out), int(uint8), int(bgr),
+                                                 B, H, W, st))
+
+    def _run_sequence(self, frames: torch.Tensor):
+        """One SEQUENCE_BIDIRECTIONAL pass on [T+1,H,W,3] frames."""
+        if not (isinstance(frames, torch.Tensor) and frames.dim() == 4 and frames.shape[-1] == 3
+                and frames.dtype in (torch.uint8, torch.float32)):
+            raise ValueError(f"raft_b200: frames must be a [N,H,W,3] uint8 or float32 tensor (got "
+                             f"{getattr(frames, 'shape', None)} {getattr(frames, 'dtype', type(frames))})")
+        T = frames.shape[0] - 1
+        if T < 1:
+            raise ValueError(f"raft_b200: a frame sequence needs two frames at least (got {frames.shape[0]})")
+        with torch.cuda.device(self.device):
+            self._ensure(T, frames.shape[1], frames.shape[2], frames.dtype == torch.uint8, SEQUENCE_BIDIRECTIONAL)
+            (self.raw if self.staged else self.images).copy_(frames, non_blocking=True)
+            self.run()
+            if not self._range_checked:
+                self._check_range()
 
     def _run_frames(self, left: torch.Tensor, right: torch.Tensor, mode: int, flow_init: Optional[torch.Tensor] = None):
         assert left.shape == right.shape and left.dim() == 4 and left.shape[-1] == 3 and left.dtype == right.dtype
@@ -522,3 +624,16 @@ class RaftEngine:
         g = torch.stack(torch.meshgrid(torch.arange(self.w, device=self.device),
                                        torch.arange(self.h, device=self.device), indexing="xy"), -1).float()
         return self.coords1 - g[None]
+
+
+def _times(ts):
+    ts = [float(t) for t in ts]
+    if not ts or not all(0.0 <= t <= 1.0 for t in ts):
+        raise ValueError(f"raft_b200: interpolation times must be a non-empty list in [0, 1] (got {ts})")
+    return ts
+
+
+def _floats(values):
+    """A host float array for the entries that copy their time steps into the kernel parameters."""
+    import ctypes
+    return (ctypes.c_float * len(values))(*values)

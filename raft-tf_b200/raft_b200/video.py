@@ -6,6 +6,11 @@ consecutive pair out) on RaftEngine.forward_sequence, with the colour coding on 
 
 writes out/flow_000000.png (frame 0 -> 1), out/flow_000001.png, ...; BGR like the single-pair CLI's PNG.
 
+video_interpolate(model, "frames/", "out/", ts=[0.5]) is frame-rate up-conversion on RaftEngine.interpolate_sequence: the
+input frames and, between every consecutive pair, the frames at times ts, written as one numbered sequence
+out/frame_<n:06d>.png.  Each pass is a fresh call on batch + 1 frames (interp_schedule()), the frames quantised to uint8
+on the GPU.
+
 Schedule (schedule()): the first pass is a fresh forward_sequence on batch + 1 frames, every later pass a carry call on
 batch new frames, so every frame is decoded, uploaded and encoded once.  A short last pass is padded by repeating the last
 frame; its extra rows are idle and their flows discarded, so one pair of CUDA graphs serves the whole video.  warm_start
@@ -66,6 +71,34 @@ def schedule(n_frames, batch, warm_start=False):
         frames = [min(i, last) for i in range(first, j * T + T + 1)]
         passes.append(Pass(j > 0, frames, [k if k < n_pairs else None for k in range(j * T, j * T + T)]))
     return passes
+
+
+def check_times(ts):
+    """The interpolation times of video_interpolate as floats: strictly increasing inside (0, 1), at least one (the input
+    frames themselves are the times 0 and 1 of the output sequence).  Anything else raises ValueError."""
+    ts = [float(t) for t in ts]
+    if not ts or not all(0.0 < t < 1.0 for t in ts) or any(b <= a for a, b in zip(ts, ts[1:])):
+        raise ValueError(f"video_interpolate: the times must be strictly increasing inside (0, 1) (got {ts})")
+    return ts
+
+
+def interp_schedule(n_frames, batch):
+    """The passes of video_interpolate over n_frames frames with T = batch pairs per pass: pass j is a fresh call on the
+    frames j T .. j T + T and covers the pairs j T .. j T + T - 1.  Frame indices past the last frame repeat it; their
+    rows are idle (None), so every pass has the same T."""
+    if int(n_frames) < 2:
+        raise ValueError(f"video: interpolation needs two frames at least (got {n_frames})")
+    if int(batch) < 1:
+        raise ValueError(f"video: batch must be >= 1 (got {batch})")
+    T, n_pairs, last = int(batch), int(n_frames) - 1, int(n_frames) - 1
+    return [Pass(False, [min(i, last) for i in range(j * T, j * T + T + 1)],
+                 [k if k < n_pairs else None for k in range(j * T, j * T + T)]) for j in range(-(-n_pairs // T))]
+
+
+def frame_number(k, m, j=None):
+    """The output index of input frame k (j None), or of the j-th of the m frames interpolated between frames k and k + 1:
+    k (m + 1) and k (m + 1) + j + 1.  N input frames give (N - 1)(m + 1) + 1 outputs."""
+    return k * (m + 1) + (0 if j is None else j + 1)
 
 
 class _Slot:
@@ -198,3 +231,106 @@ def video(model, frames, out, batch=8, workers=4, warm_start=False, flo=None, np
             if pool is not None:
                 pool.shutdown(wait=True, cancel_futures=True)
     return written
+
+
+def video_interpolate(model, frames, out, ts, batch=8, workers=4):
+    """Frame-rate up-conversion with a loaded networks.RAFT.RAFT model: the frames (a directory's sorted *.png / *.jpg, or
+    a list of paths, all of one size) and the m = len(ts) frames at times ts (strictly increasing inside (0, 1)) between
+    every consecutive pair, written as <out>/frame_<n:06d>.png with n = frame_number(k, m[, j]).  Every pass runs
+    interpolate_sequence on batch + 1 frames (interp_schedule()) and quantises on the GPU, so an interpolated frame equals
+    the single-pair CLI's PNG of model.interpolate(f_k, f_(k+1), ts) byte for byte.  The input frames are written as the
+    network saw them: the decoded bytes, or with model.input_size exactly the bytes of cv2.resize of them (which the GPU
+    resize reproduces).  Frames go in RGB with model.upstream and BGR otherwise, like the CLI; the files are BGR.  The
+    files do not depend on batch or workers.  Returns the written paths in output order."""
+    import cv2
+
+    paths = list_frames(frames)
+    ts = check_times(ts)
+    batch, workers, m = int(batch), int(workers), len(ts)
+    if workers < 0:
+        raise ValueError(f"video: workers must be >= 0 (got {workers})")
+    passes = interp_schedule(len(paths), batch)
+    T = batch
+    out = os.fspath(out)
+    os.makedirs(out, exist_ok=True)
+    engine = model.engine()
+    rgb = bool(model.upstream)
+    size = model.input_size
+    dev = engine.device
+    last = len(paths) - 1
+
+    def name(n):
+        return os.path.join(out, f"frame_{n:06d}.png")
+
+    def original(img):  # the frame as the network saw it, BGR
+        if size is not None:
+            img = cv2.resize(img, dsize=(size[1], size[0]))
+        return cv2.cvtColor(img, cv2.COLOR_RGB2BGR) if rgb else img
+
+    def write(slot, rows, originals):  # writer thread: the files of one pass, once its copies have landed
+        for k, img in originals:
+            if not cv2.imwrite(name(frame_number(k, m)), original(img)):
+                raise OSError(f"cannot write {name(frame_number(k, m))}")
+        slot.event.synchronize()
+        for r, k in rows:
+            for j in range(m):
+                if not cv2.imwrite(name(frame_number(k, m, j)), slot.frames[j, r].numpy()):
+                    raise OSError(f"cannot write {name(frame_number(k, m, j))}")
+
+    decoders = ThreadPoolExecutor(workers) if workers > 0 else None
+    writers = ThreadPoolExecutor(workers) if workers > 0 else None
+    depth = max(1, -(-workers // T))  # passes decoded ahead of the one the GPU is given
+
+    def submit(j):
+        if decoders is None:
+            return [(i, lambda i=i: _imread(paths[i], rgb)) for i in passes[j].frames]
+        return [(i, decoders.submit(_imread, paths[i], rgb).result) for i in passes[j].frames]
+
+    shape, ins, outs = None, None, None
+    try:
+        with torch.cuda.device(dev):
+            stream = torch.cuda.current_stream(dev)
+            ahead = [submit(j) for j in range(min(depth, len(passes)))]
+            for j, ps in enumerate(passes):
+                loads = ahead.pop(0)
+                if j + depth < len(passes):
+                    ahead.append(submit(j + depth))
+                imgs = []
+                for i, load in loads:
+                    img = load()
+                    if shape is None:
+                        shape = img.shape
+                    elif img.shape != shape:
+                        raise ValueError(f"video: {paths[i]} is a {img.shape[0]}x{img.shape[1]} frame, {paths[0]} is "
+                                         f"{shape[0]}x{shape[1]}: every frame needs one size")
+                    imgs.append(img)
+                if ins is None:
+                    ins = [_Slot(frames=((T + 1,) + shape, torch.uint8)) for _ in range(2)]
+                slot = ins[j % 2]
+                slot.wait()
+                for r, img in enumerate(imgs):
+                    slot.frames[r].numpy()[...] = img
+                res = engine.interpolate_sequence(slot.frames, ts, uint8=True, bgr=rgb)
+                slot.event = torch.cuda.Event()
+                slot.event.record(stream)
+                if outs is None:
+                    outs = [_Slot(frames=(tuple(res.shape), torch.uint8)) for _ in range(2)]
+                o = outs[j % 2]
+                o.wait()
+                o.frames.copy_(res, non_blocking=True)
+                o.event = torch.cuda.Event()
+                o.event.record(stream)
+                rows = [(r, k) for r, k in enumerate(ps.pairs) if k is not None]
+                originals = [(k, imgs[r]) for r, k in rows] + ([(last, imgs[rows[-1][0] + 1])] if j == len(passes) - 1
+                                                                else [])
+                if writers is None:
+                    write(o, rows, originals)
+                else:
+                    o.futures.append(writers.submit(write, o, rows, originals))
+            for o in outs or ():
+                o.wait()
+    finally:
+        for pool in (decoders, writers):
+            if pool is not None:
+                pool.shutdown(wait=True, cancel_futures=True)
+    return [name(n) for n in range(frame_number(last, m) + 1)]
