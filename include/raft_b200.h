@@ -320,6 +320,33 @@ int rb_frame_synthesize_pairs(const float* frames0, const float* frames1, int Hp
                               const float* ts, int n_t, void* out, int out_u8, int bgr, int B, int H, int W,
                               void* stream);
 
+/* ---- F14: per-item reversal and blend (frame-rate conversion: every pair its own times) ----------------------------
+ * An item is one (sample, time) of its own, so a call does only the work its items need, whatever times the other
+ * samples want.  item_sample (int32) and item_step / item_t (fp32) are host arrays of n_items entries, copied into the
+ * kernel parameters like rb_flow_reverse_multi's steps (no copy, no allocation, CUDA-graph capturable).  Both entries run
+ * the kernels of the multi-step entries above, whose sample -> (time, row) map takes the item table instead.
+ * rb_flow_reverse_items: item i reverses flow01[item_sample[i]] (flow01 [B,H,W,2] fp32) by item_step[i] into flow_t
+ * [n_items,H,W,2] fp32 and empty, multi [n_items,H,W] uint8; item i is bit for bit
+ * rb_flow_reverse_multi(flow01[item_sample[i]], {item_step[i]}, 1, ..., B = 1): the same keys, the same stable sort, the
+ * same raster-order sums and the same hole fill, whichever other items share the call (samples may repeat and come in
+ * any order).  The workspace is rb_flow_reverse_multi_workspace_bytes(n_items, 1, H, W).  Null pointers, n_items < 1 or
+ * > RB_INTERP_MAX_STEPS, B/H/W <= 0, n_items*H*W + 1 >= 2^32, a sample outside [0, B), a non-finite step and a
+ * workspace smaller than its fixed part -> RB_ERR_* before any CUDA call (the rest of the size check queries the
+ * device).
+ * rb_frame_synthesize_items: item i blends frames0[item_sample[i]] and frames1[item_sample[i]] ([B,Hp,Wp,3] fp32, crop
+ * as in rb_frame_synthesize_pairs) at item_t[i] with flow_t0, flow_t1 [n_items,H,W,2] and empty0, empty1 [n_items,H,W]
+ * (rb_flow_reverse_items' outputs for the steps s t and s (1 - t)) into out [n_items,H,W,3]: fp32 (out_u8 = 0) or uint8
+ * (out_u8 = 1) with bgr, each item bit for bit rb_frame_synthesize_pairs of that sample at that t.  Null pointers,
+ * n_items < 1 or > RB_INTERP_MAX_STEPS, out_u8 or bgr not 0 / 1, a t outside [0, 1] (or NaN), B/H/W <= 0, a sample
+ * outside [0, B) and a crop outside the frames -> RB_ERR_* before any CUDA call. */
+int rb_flow_reverse_items(const float* flow01, int B, const int32_t* item_sample, const float* item_step, int n_items,
+                          float* flow_t, uint8_t* empty, uint8_t* multi, int H, int W, void* workspace,
+                          size_t workspace_bytes, void* stream);
+int rb_frame_synthesize_items(const float* frames0, const float* frames1, int Hp, int Wp, int top, int left,
+                              const float* flow_t0, const float* flow_t1, const uint8_t* empty0, const uint8_t* empty1,
+                              const int32_t* item_sample, const float* item_t, int n_items, void* out, int out_u8,
+                              int bgr, int B, int H, int W, void* stream);
+
 /* ---- F9: end-point-error metrics (upstream RAFT's evaluate.py validate_sintel / validate_kitti) ---------------------
  * flow, gt: [B,H,W,2] fp32; valid: [B,H,W] uint8, nonzero = the pixel counts (NULL: every pixel counts).  Per pixel,
  * every operation rounded on its own (no FMA contraction), so the values equal upstream's torch expressions bit for bit:

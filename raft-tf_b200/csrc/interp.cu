@@ -60,13 +60,18 @@ cudaError_t cub_temp_bytes(size_t n, size_t* bytes) {
   return e;
 }
 
-// Time steps or times of one multi-step call, passed by value in the kernel parameters: nothing to copy or allocate
+// Time steps or times of one call, passed by value in the kernel parameters: nothing to copy or allocate.  Sample s of a
+// call over B flow rows (or frame pairs) is time v[s / B] on row s % B; an item call (items = 1, launched with B = 1)
+// gives every sample its own row: time v[s] on row row[s].
 struct Steps {
   float v[kMaxSteps];
+  int32_t row[kMaxSteps];
+  int items;
 };
 
 // One thread per source pixel of every (step, sample): static mask, scaled flow, target key; counts by integer atomics
-// (order-free).  Source i belongs to step i / n_flow and reads flow[i % n_flow]; its target lies in its own sample.
+// (order-free).  Source i belongs to step j = i / n_flow and reads flow[i % n_flow] (an item call, n_flow = H W:
+// flow[row[j] n_flow + i % n_flow]); its target lies in its own sample.
 __global__ void __launch_bounds__(256) reverse_keys_kernel(const float2* __restrict__ flow, const void* __restrict__ bg,
                                                            const void* __restrict__ im0, int u8, int C, int H, int W,
                                                            uint32_t n, uint32_t n_flow, Steps steps,
@@ -78,7 +83,9 @@ __global__ void __launch_bounds__(256) reverse_keys_kernel(const float2* __restr
   const uint32_t hw = (uint32_t)H * W;
   const int x = (int)(i % W), y = (int)((i / W) % H);
   const uint32_t base = i - (i % hw);
-  const float ts = steps.v[i / n_flow];
+  const uint32_t j = i / n_flow;
+  const float ts = steps.v[j];
+  const size_t src = (steps.items ? (size_t)steps.row[j] * n_flow : 0) + i % n_flow;
   bool st = false;
   if (bg != nullptr) {  // static: every channel differs by < 10 (uint8: the wrapped difference, as numpy computes it)
     st = true;
@@ -94,7 +101,7 @@ __global__ void __launch_bounds__(256) reverse_keys_kernel(const float2* __restr
     }
   }
   if (static_out != nullptr) static_out[i] = st ? 1 : 0;
-  float2 f = st ? make_float2(INFINITY, INFINITY) : flow[i % n_flow];
+  float2 f = st ? make_float2(INFINITY, INFINITY) : flow[src];
   f.x = __fmul_rn(f.x, ts);
   f.y = __fmul_rn(f.y, ts);
   fs[i] = f;
@@ -243,9 +250,10 @@ __global__ void __launch_bounds__(256) erode5_kernel(const uint8_t* __restrict__
 // the CLI's np.clip(np.rint(fl32(255 * x)), 0, 255), as rb_frame_metrics quantises: ties to even; fmaxf(NaN, 0) = 0
 __device__ __forceinline__ uint8_t quantise(float x) { return (uint8_t)fminf(fmaxf(rintf(__fmul_rn(255.f, x)), 0.f), 255.f); }
 
-// One thread per output pixel, blockIdx.y striding over the (time, sample) pairs (32-bit pixel indices): both frames sampled at p + F_tk(p) (clamped to the frame; NaN -> 0)
-// with the bilinear arithmetic of rb_flow_fb_check, blended by (1-t, t) with empty targets weighted 0; written as fp32,
-// or quantised to uint8 (with bgr: channels reversed).
+// One thread per output pixel, blockIdx.y striding over the (time, sample) pairs (32-bit pixel indices; a pair is
+// (times.v[smp / B], smp % B), or an item's (v[smp], row[smp]), Steps): both frames sampled at p + F_tk(p) (clamped to
+// the frame; NaN -> 0) with the bilinear arithmetic of rb_flow_fb_check, blended by (1-t, t) with empty targets weighted
+// 0; written as fp32, or quantised to uint8 (with bgr: channels reversed).
 __global__ void __launch_bounds__(256) frame_synthesize_kernel(const float* __restrict__ frames0,
                                                                const float* __restrict__ frames1, int Hp, int Wp, int top,
                                                                int left, const float2* __restrict__ f0,
@@ -258,9 +266,10 @@ __global__ void __launch_bounds__(256) frame_synthesize_kernel(const float* __re
   if (q >= hw) return;
   const int x = (int)(q % W), y = (int)(q / W);
   for (uint32_t smp = blockIdx.y; smp < (uint32_t)n_t * B; smp += gridDim.y) {
-    const int b = (int)(smp % B);
+    const uint32_t j = smp / (uint32_t)B;
+    const int b = times.items ? times.row[j] : (int)(smp % B);
     const size_t p = (size_t)smp * hw + q;
-    const float t = times.v[smp / B];
+    const float t = times.v[j];
     const float s = __fsub_rn(1.f, t);
     float w0 = e0[p] ? 0.f : s, w1 = e1[p] ? 0.f : t;
     if (w0 == 0.f && w1 == 0.f) w0 = s, w1 = t;
@@ -311,7 +320,8 @@ int reverse_shape(const char* fn, int n_steps, int B, int H, int W, size_t* n) {
   return RB_OK;
 }
 
-// The reversal of flow01 [B,H,W,2] by n_steps time steps into [n_steps,B,H,W] samples (arguments checked by the caller)
+// The reversal of flow01 [B,H,W,2] by n_steps time steps into [n_steps,B,H,W] samples, or with steps.items (B = 1) of
+// flow01[steps.row[i]] by step i into sample i (arguments checked by the caller)
 int reverse_run(const char* fn, const float* flow01, const void* bg, const void* im0, int img_u8, int img_channels,
                 const Steps& steps, int n_steps, float* flow_t, uint8_t* empty, uint8_t* multi, uint8_t* static_mask,
                 int B, int H, int W, void* workspace, size_t workspace_bytes, void* stream) {
@@ -391,7 +401,7 @@ extern "C" int rb_flow_reverse(const float* flow01, const void* bg, const void* 
   const size_t n = (size_t)B * H * W;
   RB_REQUIRE(n + 1 < (size_t(1) << 32), RB_ERR_BAD_SHAPE,
              "rb_flow_reverse: B*H*W = %zu pixels: keys need B*H*W + 1 < 2^32", n);
-  Steps steps;
+  Steps steps{};
   steps.v[0] = time_step;
   const int rc = reverse_run("rb_flow_reverse", flow01, bg, im0, img_u8, img_channels, steps, 1, flow_t, empty, multi,
                              static_mask, B, H, W, workspace, workspace_bytes, stream);
@@ -411,7 +421,7 @@ extern "C" int rb_flow_reverse_multi(const float* flow01, const float* time_step
   size_t n = 0;
   const int rc = reverse_shape("rb_flow_reverse_multi", n_steps, B, H, W, &n);
   if (rc != RB_OK) return rc;
-  Steps steps;
+  Steps steps{};
   for (int i = 0; i < n_steps; ++i) {
     RB_REQUIRE(isfinite(time_steps[i]), RB_ERR_BAD_ARG, "rb_flow_reverse_multi: time_steps[%d] must be finite (got %g)",
                i, (double)time_steps[i]);
@@ -420,6 +430,59 @@ extern "C" int rb_flow_reverse_multi(const float* flow01, const float* time_step
   return reverse_run("rb_flow_reverse_multi", flow01, nullptr, nullptr, 0, 0, steps, n_steps, flow_t, empty, multi,
                      nullptr, B, H, W, workspace, workspace_bytes, stream);
 }
+
+extern "C" int rb_flow_reverse_items(const float* flow01, int B, const int32_t* item_sample, const float* item_step,
+                                     int n_items, float* flow_t, uint8_t* empty, uint8_t* multi, int H, int W,
+                                     void* workspace, size_t workspace_bytes, void* stream) {
+  RB_REQUIRE(flow01 && item_sample && item_step && flow_t && empty && multi && workspace, RB_ERR_BAD_ARG,
+             "rb_flow_reverse_items: null pointer");
+  RB_REQUIRE(n_items > 0 && n_items <= kMaxSteps, RB_ERR_BAD_ARG, "rb_flow_reverse_items: %d items (1..%d)", n_items,
+             kMaxSteps);
+  RB_REQUIRE(B > 0 && H > 0 && W > 0, RB_ERR_BAD_SHAPE, "rb_flow_reverse_items: bad shape B=%d H=%d W=%d", B, H, W);
+  const size_t n = (size_t)n_items * H * W;
+  RB_REQUIRE(n + 1 < (size_t(1) << 32), RB_ERR_BAD_SHAPE,
+             "rb_flow_reverse_items: n_items*H*W = %zu pixels: keys need n_items*H*W + 1 < 2^32", n);
+  Steps steps{};
+  steps.items = 1;
+  for (int i = 0; i < n_items; ++i) {
+    RB_REQUIRE(item_sample[i] >= 0 && item_sample[i] < B, RB_ERR_BAD_ARG,
+               "rb_flow_reverse_items: item_sample[%d] = %d outside [0, %d)", i, item_sample[i], B);
+    RB_REQUIRE(isfinite(item_step[i]), RB_ERR_BAD_ARG, "rb_flow_reverse_items: item_step[%d] must be finite (got %g)", i,
+               (double)item_step[i]);
+    steps.row[i] = item_sample[i];
+    steps.v[i] = item_step[i];
+  }
+  // one row per item: the kernels read flow01[row[i]] for sample i
+  return reverse_run("rb_flow_reverse_items", flow01, nullptr, nullptr, 0, 0, steps, n_items, flow_t, empty, multi,
+                     nullptr, 1, H, W, workspace, workspace_bytes, stream);
+}
+
+namespace {
+
+// The blend entries after their pointer, count, flag and time checks: the shape, the item rows against the B frame
+// pairs, the crop, then one launch over n_t times x B pairs, or over the n_t items (launched with B = 1)
+int synthesize_run(const char* fn, const float* frames0, const float* frames1, int Hp, int Wp, int top, int left,
+                   const float* flow_t0, const float* flow_t1, const uint8_t* empty0, const uint8_t* empty1,
+                   const Steps& times, int n_t, void* out, int out_u8, int bgr, int B, int H, int W, void* stream) {
+  RB_REQUIRE(B > 0 && H > 0 && W > 0, RB_ERR_BAD_SHAPE, "%s: bad shape B=%d H=%d W=%d", fn, B, H, W);
+  for (int i = 0; times.items && i < n_t; ++i)
+    RB_REQUIRE(times.row[i] >= 0 && times.row[i] < B, RB_ERR_BAD_ARG, "%s: item_sample[%d] = %d outside [0, %d)", fn, i,
+               times.row[i], B);
+  RB_REQUIRE(top >= 0 && left >= 0 && top + H <= Hp && left + W <= Wp, RB_ERR_BAD_SHAPE,
+             "%s: crop (%d, %d) + %dx%d outside the %dx%d frames", fn, top, left, H, W, Hp, Wp);
+  const size_t hw = (size_t)H * W;
+  const int rows = times.items ? 1 : B;
+  RB_REQUIRE(hw < (size_t(1) << 32) && (size_t)n_t * rows < (size_t(1) << 32), RB_ERR_BAD_SHAPE,
+             "%s: %zu pixels per frame or %zu frames exceed 32-bit indices", fn, hw, (size_t)n_t * rows);
+  const dim3 grid((unsigned)((hw + 255) / 256), (unsigned)std::min<size_t>((size_t)n_t * rows, 65535));
+  frame_synthesize_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(
+      frames0, frames1, Hp, Wp, top, left, reinterpret_cast<const float2*>(flow_t0),
+      reinterpret_cast<const float2*>(flow_t1), empty0, empty1, times, out, out_u8, bgr, n_t, rows, H, W);
+  RB_CHECK_LAUNCH("frame_synthesize_kernel");
+  return RB_OK;
+}
+
+}  // namespace
 
 extern "C" int rb_frame_synthesize_pairs(const float* frames0, const float* frames1, int Hp, int Wp, int top, int left,
                                          const float* flow_t0, const float* flow_t1, const uint8_t* empty0,
@@ -430,24 +493,37 @@ extern "C" int rb_frame_synthesize_pairs(const float* frames0, const float* fram
   RB_REQUIRE(n_t > 0 && n_t <= kMaxSteps, RB_ERR_BAD_ARG, "rb_frame_synthesize: %d times (1..%d)", n_t, kMaxSteps);
   RB_REQUIRE((out_u8 == 0 || out_u8 == 1) && (bgr == 0 || bgr == 1), RB_ERR_BAD_ARG,
              "rb_frame_synthesize: out_u8 and bgr must be 0 or 1 (got %d, %d)", out_u8, bgr);
-  Steps times;
+  Steps times{};
   for (int i = 0; i < n_t; ++i) {
     RB_REQUIRE(ts[i] >= 0.f && ts[i] <= 1.f, RB_ERR_BAD_ARG, "rb_frame_synthesize: t must be in [0, 1] (got %g)",
                (double)ts[i]);
     times.v[i] = ts[i];
   }
-  RB_REQUIRE(B > 0 && H > 0 && W > 0, RB_ERR_BAD_SHAPE, "rb_frame_synthesize: bad shape B=%d H=%d W=%d", B, H, W);
-  RB_REQUIRE(top >= 0 && left >= 0 && top + H <= Hp && left + W <= Wp, RB_ERR_BAD_SHAPE,
-             "rb_frame_synthesize: crop (%d, %d) + %dx%d outside the %dx%d frames", top, left, H, W, Hp, Wp);
-  const size_t hw = (size_t)H * W;
-  RB_REQUIRE(hw < (size_t(1) << 32) && (size_t)n_t * B < (size_t(1) << 32), RB_ERR_BAD_SHAPE,
-             "rb_frame_synthesize: %zu pixels per frame or %zu frames exceed 32-bit indices", hw, (size_t)n_t * B);
-  const dim3 grid((unsigned)((hw + 255) / 256), (unsigned)std::min<size_t>((size_t)n_t * B, 65535));
-  frame_synthesize_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(
-      frames0, frames1, Hp, Wp, top, left, reinterpret_cast<const float2*>(flow_t0),
-      reinterpret_cast<const float2*>(flow_t1), empty0, empty1, times, out, out_u8, bgr, n_t, B, H, W);
-  RB_CHECK_LAUNCH("frame_synthesize_kernel");
-  return RB_OK;
+  return synthesize_run("rb_frame_synthesize", frames0, frames1, Hp, Wp, top, left, flow_t0, flow_t1, empty0, empty1,
+                        times, n_t, out, out_u8, bgr, B, H, W, stream);
+}
+
+extern "C" int rb_frame_synthesize_items(const float* frames0, const float* frames1, int Hp, int Wp, int top, int left,
+                                         const float* flow_t0, const float* flow_t1, const uint8_t* empty0,
+                                         const uint8_t* empty1, const int32_t* item_sample, const float* item_t,
+                                         int n_items, void* out, int out_u8, int bgr, int B, int H, int W,
+                                         void* stream) {
+  RB_REQUIRE(frames0 && frames1 && flow_t0 && flow_t1 && empty0 && empty1 && item_sample && item_t && out,
+             RB_ERR_BAD_ARG, "rb_frame_synthesize_items: null pointer");
+  RB_REQUIRE(n_items > 0 && n_items <= kMaxSteps, RB_ERR_BAD_ARG, "rb_frame_synthesize_items: %d items (1..%d)",
+             n_items, kMaxSteps);
+  RB_REQUIRE((out_u8 == 0 || out_u8 == 1) && (bgr == 0 || bgr == 1), RB_ERR_BAD_ARG,
+             "rb_frame_synthesize_items: out_u8 and bgr must be 0 or 1 (got %d, %d)", out_u8, bgr);
+  Steps times{};
+  times.items = 1;
+  for (int i = 0; i < n_items; ++i) {
+    RB_REQUIRE(item_t[i] >= 0.f && item_t[i] <= 1.f, RB_ERR_BAD_ARG,
+               "rb_frame_synthesize_items: item_t[%d] must be in [0, 1] (got %g)", i, (double)item_t[i]);
+    times.v[i] = item_t[i];
+    times.row[i] = item_sample[i];
+  }
+  return synthesize_run("rb_frame_synthesize_items", frames0, frames1, Hp, Wp, top, left, flow_t0, flow_t1, empty0,
+                        empty1, times, n_items, out, out_u8, bgr, B, H, W, stream);
 }
 
 extern "C" int rb_frame_synthesize(const float* frames, int Hp, int Wp, int top, int left, const float* flow_t0,

@@ -47,11 +47,19 @@ the frames at times T (strictly increasing inside (0, 1)), written as one sequen
 frame k is n = k (m + 1) for m times), --batch pairs per pass, each frame encoded once per pass (raft_b200.video):
 
     python infer_raft.py --path frames/ --out slow/ --interpolate 0.25 0.5 0.75 --load raft-things.npz [--batch 8]
+
+--path DIR --input-fps IN --fps OUT converts DIR's frames from IN to OUT frames per second (OUT > IN; rates such as 24,
+59.94 or 24000/1001): output frame n, at input time s = n IN / OUT, is input frame s where s is an integer and otherwise
+the frame interpolated at time s - floor(s) between frames floor(s) and floor(s) + 1, written as
+``<--out>/frame_<n:06d>.png`` (raft_b200.video):
+
+    python infer_raft.py --path film/ --out tv/ --input-fps 24 --fps 60 --load raft-things.npz [--batch 8]
 """
 import glob
 import argparse
 import os
 import sys
+from fractions import Fraction
 
 import numpy as np
 
@@ -122,6 +130,12 @@ def parser():
                    help='extension: also write the frames at times T in [0, 1] between im1 and im2 (raft_interp_<k>.png); '
                         'with --path, the up-converted sequence <--out>/frame_<n:06d>.png (T strictly increasing inside '
                         '(0, 1))')
+    p.add_argument('--input-fps', default=None, metavar='IN',
+                   help='extension, with --path and --fps: the frame rate of the --path frames (24, 25, 23.976, '
+                        '24000/1001, ...)')
+    p.add_argument('--fps', default=None, metavar='OUT',
+                   help='extension, with --path and --input-fps: convert the frames to OUT frames per second (above IN), '
+                        'written as <--out>/frame_<n:06d>.png')
     p.add_argument('--native-flow', action='store_true',
                    help="extension: resize the written flow(s) back to im1's size (flow_utils.resize_flow)")
     p.add_argument('--upstream', action='store_true',
@@ -136,6 +150,20 @@ def parser():
 def main(argv=None):
     p = parser()
     args = p.parse_args(argv)
+    fps = None
+    if args.fps is not None or args.input_fps is not None:
+        if args.fps is None or args.input_fps is None:
+            p.error('--fps OUT and --input-fps IN go together: frame-rate conversion needs both rates')
+        if args.path is None:
+            p.error('--fps / --input-fps convert the frame rate of a frame directory: they need --path DIR')
+        for flag, given in (('--interpolate', args.interpolate), ('--warm-start', args.warm_start),
+                            ('--native-flow', args.native_flow), ('--flo', args.flo), ('--npy', args.npy),
+                            ('--bidirectional', args.bidirectional)):
+            if given:
+                p.error(f'--fps writes the frames of one output rate: it cannot be combined with {flag}')
+        fps = (_rate(p, '--input-fps', args.input_fps), _rate(p, '--fps', args.fps))
+        if fps[1] <= fps[0]:
+            p.error(f'--fps {args.fps} must exceed --input-fps {args.input_fps}: frame-rate conversion goes up only')
     if args.interpolate and not all(0.0 <= t <= 1.0 for t in args.interpolate):
         p.error('--interpolate: every T must be in [0, 1]')
     if args.mode == 'val':
@@ -165,12 +193,14 @@ def main(argv=None):
             if not all(0.0 < t < 1.0 for t in ts) or any(b <= a for a, b in zip(ts, ts[1:])):
                 p.error('--path --interpolate: the times T must be strictly increasing inside (0, 1) (the input frames '
                         'are the times 0 and 1)')
+        if args.interpolate or fps is not None:
             if args.batch < 1 or args.workers < 0:
                 p.error('--path needs --batch >= 1 and --workers >= 0')
             n = len(glob.glob(os.path.join(args.path, '*.png')) + glob.glob(os.path.join(args.path, '*.jpg')))
             if n < 2:
-                p.error(f'--path --interpolate: {args.path} holds {n} *.png / *.jpg frames; interpolation needs two')
-            return run_video_interpolate(args)
+                p.error(f'--path {"--fps" if fps else "--interpolate"}: {args.path} holds {n} *.png / *.jpg frames; '
+                        'interpolation needs two')
+            return run_video_interpolate(args, fps)
         if args.warm_start and args.batch != 1:
             p.error('--path --warm-start warm-starts each pair from the one before: it runs one pair per pass (--batch 1)')
         if args.batch < 1 or args.workers < 0:
@@ -239,16 +269,17 @@ def run_video(args):
     return 0
 
 
-def run_video_interpolate(args):
-    """--path --interpolate: raft_b200.video.video_interpolate over the frames of --path, at 432x1024 like test mode (or
-    their own size with --keep-size)."""
+def run_video_interpolate(args, fps=None):
+    """--path --interpolate, or --path --input-fps --fps (fps = the two rates): raft_b200.video.video_interpolate over the
+    frames of --path, at 432x1024 like test mode (or their own size with --keep-size)."""
     from networks import RAFT
     from raft_b200.video import video_interpolate
     iters = 20 if args.iters is None else args.iters
     size = None if args.keep_size else (432, 1024)
     model = RAFT.RAFT(None if size is None else size + (3,), args, iters=iters, input_size=size, upstream=args.upstream,
                       mixed_precision=args.mixed_precision).load(args.load)
-    files = video_interpolate(model, args.path, args.out, args.interpolate, batch=args.batch, workers=args.workers)
+    files = video_interpolate(model, args.path, args.out, args.interpolate, batch=args.batch, workers=args.workers,
+                              fps=fps)
     print(f"{len(files)} frames written under {args.out}")
     return 0
 
@@ -273,6 +304,17 @@ def validate(args):
     with open(os.path.join(args.out, f"val_{args.dataset}.json"), "w") as f:
         json.dump(res, f, indent=1)
     return 0
+
+
+def _rate(p, flag, text):
+    """A frame-rate flag as a Fraction ("24", "59.94", "24000/1001"); anything else, zero or negative is a usage error."""
+    try:
+        rate = Fraction(text)
+    except (ValueError, ZeroDivisionError):
+        rate = None
+    if rate is None or rate <= 0:
+        p.error(f'{flag}: {text!r} is not a frame rate (a positive number such as 24, 59.94 or 24000/1001)')
+    return rate
 
 
 def _bw_path(path):

@@ -170,6 +170,16 @@ class RAFT(object):
         return out[0] if scalar else out
 
     @torch.no_grad()
+    def interpolate_sequence_at(self, frames, items, uint8=False, bgr=False):
+        """Extension (frame-rate conversion to any rate): the frames at per-pair times of [T+1,H,W,3] frames (dtypes and
+        sources as for ``forward``).  items is a list of (k, t) with 0 <= k < T and t in [0, 1], each the frame at time t
+        between frames k and k + 1; one ``forward_sequence_bidirectional`` pass, then only the work of the listed items.
+        Returns a fresh [len(items),H,W,3] tensor whose row i equals ``interpolate(frames[k:k+1], frames[k+1:k+2], t)[0]``
+        bit for bit.  uint8 and bgr as for ``interpolate_sequence``.  An empty list, a k outside [0, T) or a t outside
+        [0, 1] raises ValueError."""
+        return self.engine().interpolate_sequence_at(_as_tensor(frames), items, uint8=uint8, bgr=bgr)
+
+    @torch.no_grad()
     def interpolate(self, input_left, input_right, t=0.5):
         """Extension (the reference computes the flow for frame interpolation and projects it to time t with
         flow_utils.py:166 on the CPU): the frames at time t between left (t = 0) and right (t = 1).  One bidirectional

@@ -15,7 +15,9 @@ and feature map the graph copies to row 0 before it encodes only the T new frame
 forward_sequence_bidirectional(frames) runs both directions of the T pairs of T + 1 frames as 2T pairs in the palindrome
 order (0->1), ..., (T-1->T), (T->T-1), ..., (1->0): fmaps = [f_0 .. f_T, f_(T-1) .. f_0], so fmap1 = fmaps[:2T] and
 fmap2 = fmaps[1:] overlap as in SEQUENCE, fnet and cnet run once per frame and the mirrored rows are device copies
-(SEQUENCE_BIDIRECTIONAL); interpolate_sequence adds the per-t work of interpolate to it.
+(SEQUENCE_BIDIRECTIONAL); interpolate_sequence adds the per-t work of interpolate to it, and interpolate_sequence_at the
+work of per-pair times, each (pair, t) item reversed and blended on its own (rb_flow_reverse_items,
+rb_frame_synthesize_items).
 With input_size set, every mode first resizes the frames to that size like the reference's cv2.resize (rb_frames_resize,
 csrc/resize.cu, in the graph in place of rb_frames_prepare), and its outputs come back at that size.
 """
@@ -47,10 +49,11 @@ MIN_FRAME = 57
 MIN_FRAME_UPSTREAM = 121
 # upstream InputPadder's modes (pad_mode)
 PAD_MODES = ("sintel", "kitti")
-# most bytes the flow-reversal workspace of one interpolation chunk may take: interpolate and interpolate_sequence reverse
-# the flows of as many times at once as fit (rb_flow_reverse_multi), at least one; the results do not depend on it
+# most bytes the flow-reversal workspace of one interpolation chunk may take: interpolate, interpolate_sequence and
+# interpolate_sequence_at reverse the flows of as many times (items) at once as fit, at least one; the results do not
+# depend on it
 REVERSE_WS_BOUND = 1 << 30
-RB_INTERP_MAX_STEPS = 64  # include/raft_b200.h: times per rb_flow_reverse_multi / rb_frame_synthesize_pairs call
+RB_INTERP_MAX_STEPS = 64  # include/raft_b200.h: times (items) per reversal / blend call
 
 
 def _kept(parked, key):
@@ -70,7 +73,7 @@ def _kept(parked, key):
 class RaftEngine:
     # everything _ensure allocates for one (B, H, W, u8, mode); parked per mode so alternating modes re-captures nothing
     _STATE = ("_key", "src_hw", "pad", "h", "w", "Hp", "Wp", "pairs", "pyr_bytes", "pyramid", "cws_bytes", "corr_ws",
-              "ws_bytes", "ws", "coords1", "mask", "flow_up", "occ", "rev_ws_bytes", "rev_ws", "rev_steps", "flow_t", "empty_t", "flow_bw", "flow_init", "flow_low", "fmaps", "fmap1", "fmap2", "cmap", "images", "staged", "raw",
+              "ws_bytes", "ws", "coords1", "mask", "flow_up", "occ", "rev_ws_bytes", "rev_ws", "rev_rows", "flow_t", "empty_t", "flow_bw", "flow_init", "flow_low", "fmaps", "fmap1", "fmap2", "cmap", "images", "staged", "raw",
               "seq_enc", "_shape", "_graph", "_graph_carry")
 
     def __init__(self, params: Dict[str, np.ndarray], small: bool = False, iters: int = 20,
@@ -198,7 +201,7 @@ class RaftEngine:
         # SEQUENCE_BIDIRECTIONAL: the backward flows in pair order (the pass leaves them in rows 2T-1 .. T)
         self.flow_bw = torch.empty(B, H, W, 2, dtype=torch.float32, device=d) if mode == SEQUENCE_BIDIRECTIONAL else None
         # the per-t buffers of interpolate / interpolate_sequence, allocated by _synthesize for the chunk it runs
-        self.rev_ws_bytes, self.rev_ws, self.rev_steps, self.flow_t, self.empty_t = 0, None, 0, None, None
+        self.rev_ws_bytes, self.rev_ws, self.rev_rows, self.flow_t, self.empty_t = 0, None, 0, None, None
         if mode in (FORWARD_WARM, SEQUENCE):  # the caller's initial flow (copied in before each replay), the final 1/8-res flow
             self.flow_init = torch.zeros(B, h, w, 2, dtype=torch.float32, device=d)
             self.flow_low = torch.empty(B, h, w, 2, dtype=torch.float32, device=d)
@@ -525,20 +528,41 @@ class RaftEngine:
         T = self._shape[0]
         return self._synthesize(self.flow_up[:T], self.flow_bw, self.images[:T], self.images[1:], ts, uint8, bgr)
 
-    def _synthesize(self, flow_fw, flow_bw, frames0, frames1, ts, uint8=False, bgr=False) -> torch.Tensor:
-        """The per-t work of interpolate and interpolate_sequence on the B pairs of the last pass: per chunk of times, one
-        multi-step reversal per direction (steps s t and s (1 - t), s = flow_scale) and one blend of frames0[b] and
-        frames1[b] into a fresh [len(ts),B,H,W,3] tensor.  A chunk is as many times as keep the reversal workspace within
-        REVERSE_WS_BOUND (at least one, at most RB_INTERP_MAX_STEPS); each sample's bits do not depend on it."""
+    @torch.no_grad()
+    def interpolate_sequence_at(self, frames: torch.Tensor, items, uint8: bool = False, bgr: bool = False) -> torch.Tensor:
+        """Frame-rate conversion: the frames at per-pair times of [T+1,H,W,3] frames.  items is a list of (k, t), 0 <= k < T
+        and t in [0, 1]: the frame at time t between frames k and k + 1.  One forward_sequence_bidirectional(check=False)
+        pass, then per item only that item's work: rb_flow_reverse_items of flow_fw[k] by s t and of flow_bw[k] by
+        s (1 - t) (s = flow_scale, as in interpolate) and rb_frame_synthesize_items, for as many items at once as
+        REVERSE_WS_BOUND allows.  Returns a fresh [len(items),H,W,3] tensor; row i equals interpolate(f_k, f_(k+1), [t])[0, 0]
+        bit for bit.  uint8 and bgr as for interpolate_sequence.  An empty list, a k outside [0, T) or a t outside [0, 1]
+        raises ValueError before the pass."""
+        ks, ts = _items(items, _sequence_length(frames))
+        if bgr and not uint8:
+            raise ValueError("raft_b200: bgr swaps the channels of uint8 output; pass uint8=True")
+        self._run_sequence(frames)
+        T = self._shape[0]
+        return self._synthesize(self.flow_up[:T], self.flow_bw, self.images[:T], self.images[1:], ts, uint8, bgr, ks)
+
+    def _synthesize(self, flow_fw, flow_bw, frames0, frames1, ts, uint8=False, bgr=False, samples=None) -> torch.Tensor:
+        """The per-t work of interpolate, interpolate_sequence and interpolate_sequence_at on the B pairs of the last pass:
+        per chunk, one reversal per direction (steps s t and s (1 - t), s = flow_scale) and one blend of frames0[b] and
+        frames1[b].  Without samples every time applies to every pair, into a fresh [len(ts),B,H,W,3] tensor; with
+        samples, time ts[i] applies to pair samples[i] alone, into a fresh [len(ts),H,W,3] tensor.  A chunk is as many
+        times (items) as keep the reversal workspace within REVERSE_WS_BOUND (at least one, at most RB_INTERP_MAX_STEPS);
+        each sample's bits do not depend on it."""
         B, H, W = self._shape[:3]
+        rows = B if samples is None else 1  # reversal samples per time
         lib = capi.lib
-        out = torch.empty(len(ts), B, H, W, 3, dtype=torch.uint8 if uint8 else torch.float32, device=self.device)
+        out = torch.empty((len(ts),) + ((B,) if samples is None else ()) + (H, W, 3),
+                          dtype=torch.uint8 if uint8 else torch.float32, device=self.device)
         chunk = min(len(ts), RB_INTERP_MAX_STEPS)
-        while chunk > 1 and capi.size_query(lib.rb_flow_reverse_multi_workspace_bytes, chunk, B, H, W) > REVERSE_WS_BOUND:
+        while chunk > 1 and capi.size_query(lib.rb_flow_reverse_multi_workspace_bytes, chunk, rows, H, W) > REVERSE_WS_BOUND:
             chunk = max(1, chunk // 2)
         with torch.cuda.device(self.device):
             for i in range(0, len(ts), chunk):
-                self._reverse_and_blend(flow_fw, flow_bw, frames0, frames1, ts[i:i + chunk], out[i:i + chunk], uint8, bgr)
+                self._reverse_and_blend(flow_fw, flow_bw, frames0, frames1, ts[i:i + chunk], out[i:i + chunk], uint8, bgr,
+                                        None if samples is None else samples[i:i + chunk])
         return out
 
     def _interpolate_at(self, t: float, out: torch.Tensor):
@@ -546,36 +570,42 @@ class RaftEngine:
         B = self._shape[0]
         self._reverse_and_blend(self.flow_up[:B], self.flow_up[B:], self.images[:B], self.images[B:], [t], out[None])
 
-    def _reverse_and_blend(self, flow_fw, flow_bw, frames0, frames1, ts, out, uint8=False, bgr=False):
-        """One chunk: rb_flow_reverse_multi of flow_fw by s t and of flow_bw by s (1 - t) for the n = len(ts) times, then
-        rb_frame_synthesize_pairs into out [n,B,H,W,3]; the reversal buffers are (re)allocated for n times."""
+    def _reverse_and_blend(self, flow_fw, flow_bw, frames0, frames1, ts, out, uint8=False, bgr=False, samples=None):
+        """One chunk: the reversal of flow_fw by s t and of flow_bw by s (1 - t) for the n = len(ts) times, then the blend
+        into out -- rb_flow_reverse_multi and rb_frame_synthesize_pairs on all B pairs into out [n,B,H,W,3], or with
+        samples rb_flow_reverse_items and rb_frame_synthesize_items on pair samples[i] at ts[i] into out [n,H,W,3].  The
+        reversal buffers are (re)allocated for the n B (n) samples."""
         B, H, W = self._shape[:3]
         n, s, d = len(ts), self.flow_scale, self.device
+        per_t = B if samples is None else 1
+        rows = n * per_t
         lib, ptr = capi.lib, capi.ptr
-        if self.rev_steps != n:
-            self.rev_ws_bytes = capi.size_query(lib.rb_flow_reverse_multi_workspace_bytes, n, B, H, W)
+        if self.rev_rows != rows:  # the workspace depends on the n B (n) samples alone
+            self.rev_ws_bytes = capi.size_query(lib.rb_flow_reverse_multi_workspace_bytes, n, per_t, H, W)
             self.rev_ws = torch.empty(self.rev_ws_bytes, dtype=torch.uint8, device=d)
-            self.flow_t = torch.empty(2, n, B, H, W, 2, dtype=torch.float32, device=d)  # from t to frame 0 | to frame 1
-            self.empty_t = torch.empty(2, 2, n, B, H, W, dtype=torch.uint8, device=d)  # [empty | multi] x direction
-            self.rev_steps = n
+            self.flow_t = torch.empty(2, rows, H, W, 2, dtype=torch.float32, device=d)  # from t to frame 0 | to frame 1
+            self.empty_t = torch.empty(2, 2, rows, H, W, dtype=torch.uint8, device=d)  # [empty | multi] x direction
+            self.rev_rows = rows
         st = capi.stream()
         for k, (flow, steps) in enumerate(((flow_fw, [s * t for t in ts]), (flow_bw, [s * (1.0 - t) for t in ts]))):
-            capi.check(lib.rb_flow_reverse_multi(ptr(flow), _floats(steps), n, ptr(self.flow_t[k]), ptr(self.empty_t[0, k]),
-                                                 ptr(self.empty_t[1, k]), B, H, W, ptr(self.rev_ws), self.rev_ws_bytes, st))
-        capi.check(lib.rb_frame_synthesize_pairs(ptr(frames0), ptr(frames1), self.Hp, self.Wp, self.pad[0], self.pad[2],
-                                                 ptr(self.flow_t[0]), ptr(self.flow_t[1]), ptr(self.empty_t[0, 0]),
-                                                 ptr(self.empty_t[0, 1]), _floats(ts), n, ptr(out), int(uint8), int(bgr),
-                                                 B, H, W, st))
+            bufs = ptr(self.flow_t[k]), ptr(self.empty_t[0, k]), ptr(self.empty_t[1, k])
+            if samples is None:
+                capi.check(lib.rb_flow_reverse_multi(ptr(flow), _floats(steps), n, *bufs, B, H, W, ptr(self.rev_ws),
+                                                     self.rev_ws_bytes, st))
+            else:
+                capi.check(lib.rb_flow_reverse_items(ptr(flow), B, _ints(samples), _floats(steps), n, *bufs, H, W,
+                                                     ptr(self.rev_ws), self.rev_ws_bytes, st))
+        frames = (ptr(frames0), ptr(frames1), self.Hp, self.Wp, self.pad[0], self.pad[2], ptr(self.flow_t[0]),
+                  ptr(self.flow_t[1]), ptr(self.empty_t[0, 0]), ptr(self.empty_t[0, 1]))
+        if samples is None:
+            capi.check(lib.rb_frame_synthesize_pairs(*frames, _floats(ts), n, ptr(out), int(uint8), int(bgr), B, H, W, st))
+        else:
+            capi.check(lib.rb_frame_synthesize_items(*frames, _ints(samples), _floats(ts), n, ptr(out), int(uint8),
+                                                     int(bgr), B, H, W, st))
 
     def _run_sequence(self, frames: torch.Tensor):
         """One SEQUENCE_BIDIRECTIONAL pass on [T+1,H,W,3] frames."""
-        if not (isinstance(frames, torch.Tensor) and frames.dim() == 4 and frames.shape[-1] == 3
-                and frames.dtype in (torch.uint8, torch.float32)):
-            raise ValueError(f"raft_b200: frames must be a [N,H,W,3] uint8 or float32 tensor (got "
-                             f"{getattr(frames, 'shape', None)} {getattr(frames, 'dtype', type(frames))})")
-        T = frames.shape[0] - 1
-        if T < 1:
-            raise ValueError(f"raft_b200: a frame sequence needs two frames at least (got {frames.shape[0]})")
+        T = _sequence_length(frames)
         with torch.cuda.device(self.device):
             self._ensure(T, frames.shape[1], frames.shape[2], frames.dtype == torch.uint8, SEQUENCE_BIDIRECTIONAL)
             (self.raw if self.staged else self.images).copy_(frames, non_blocking=True)
@@ -633,7 +663,44 @@ def _times(ts):
     return ts
 
 
+def _sequence_length(frames):
+    """T of [T+1,H,W,3] uint8 or float32 frames (T >= 1); anything else raises ValueError."""
+    if not (isinstance(frames, torch.Tensor) and frames.dim() == 4 and frames.shape[-1] == 3
+            and frames.dtype in (torch.uint8, torch.float32)):
+        raise ValueError(f"raft_b200: frames must be a [N,H,W,3] uint8 or float32 tensor (got "
+                         f"{getattr(frames, 'shape', None)} {getattr(frames, 'dtype', type(frames))})")
+    if frames.shape[0] < 2:
+        raise ValueError(f"raft_b200: a frame sequence needs two frames at least (got {frames.shape[0]})")
+    return frames.shape[0] - 1
+
+
+def _items(items, T):
+    """The pairs and times of interpolate_sequence_at's items (k, t): a non-empty list, each k an integer in [0, T) and
+    each t in [0, 1]; anything else raises ValueError."""
+    items = list(items)
+    if not items:
+        raise ValueError("raft_b200: interpolate_sequence_at needs one (k, t) item at least")
+    ks, ts = [], []
+    for item in items:
+        try:
+            k, t = item
+            ok = int(k) == k and 0 <= k < T and 0.0 <= float(t) <= 1.0
+        except (TypeError, ValueError):
+            ok = False
+        if not ok:
+            raise ValueError(f"raft_b200: item {item!r}: (k, t) needs an integer k in [0, {T}) and t in [0, 1]")
+        ks.append(int(k))
+        ts.append(float(t))
+    return ks, ts
+
+
 def _floats(values):
     """A host float array for the entries that copy their time steps into the kernel parameters."""
     import ctypes
     return (ctypes.c_float * len(values))(*values)
+
+
+def _ints(values):
+    """A host int32 array for the entries that copy their item samples into the kernel parameters."""
+    import ctypes
+    return (ctypes.c_int32 * len(values))(*values)

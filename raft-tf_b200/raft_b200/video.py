@@ -9,7 +9,9 @@ writes out/flow_000000.png (frame 0 -> 1), out/flow_000001.png, ...; BGR like th
 video_interpolate(model, "frames/", "out/", ts=[0.5]) is frame-rate up-conversion on RaftEngine.interpolate_sequence: the
 input frames and, between every consecutive pair, the frames at times ts, written as one numbered sequence
 out/frame_<n:06d>.png.  Each pass is a fresh call on batch + 1 frames (interp_schedule()), the frames quantised to uint8
-on the GPU.
+on the GPU.  video_interpolate(model, "frames/", "out/", fps=(24, 60)) converts to another frame rate instead: output
+frame n sits at input time n 24 / 60, so every pair gets its own times (fps_schedule()), and each pass runs
+RaftEngine.interpolate_sequence_at on the (pair, time) items of its pairs alone.
 
 Schedule (schedule()): the first pass is a fresh forward_sequence on batch + 1 frames, every later pass a carry call on
 batch new frames, so every frame is decoded, uploaded and encoded once.  A short last pass is padded by repeating the last
@@ -27,6 +29,7 @@ import glob
 import os
 from collections import namedtuple
 from concurrent.futures import ThreadPoolExecutor
+from fractions import Fraction
 
 import numpy as np
 import torch
@@ -36,6 +39,9 @@ from .evaluate import _imread
 # one forward_sequence call: carry or fresh, the frame indices it uploads (T + 1 fresh, T carry; a short last pass repeats
 # the last frame), and per flow row the pair index k (frame k -> k + 1) or None for an idle row
 Pass = namedtuple("Pass", "carry frames pairs")
+# one interpolate_sequence_at call of frame-rate conversion (fps_schedule()): the frames and pairs of its Pass, the output
+# frames it interpolates as (n, k, t) (output index, pair, time) and the input frames it copies as (n, i)
+FpsPass = namedtuple("FpsPass", "frames pairs items copies")
 
 
 def list_frames(frames):
@@ -93,6 +99,43 @@ def interp_schedule(n_frames, batch):
     T, n_pairs, last = int(batch), int(n_frames) - 1, int(n_frames) - 1
     return [Pass(False, [min(i, last) for i in range(j * T, j * T + T + 1)],
                  [k if k < n_pairs else None for k in range(j * T, j * T + T)]) for j in range(-(-n_pairs // T))]
+
+
+def parse_rate(rate):
+    """A frame rate as a Fraction: anything Fraction parses ("60", "59.94", "60000/1001", 24, Fraction(...)); a float by its
+    shortest decimal repr (59.94 is 2997/50, not the nearest binary fraction).  Not positive raises ValueError."""
+    try:
+        r = Fraction(repr(rate)) if isinstance(rate, float) else Fraction(rate)
+    except (TypeError, ValueError, ZeroDivisionError, OverflowError):
+        raise ValueError(f"video: a frame rate must be a positive finite number (got {rate!r})") from None
+    if r <= 0:
+        raise ValueError(f"video: a frame rate must be a positive finite number (got {rate!r})")
+    return r
+
+
+def fps_schedule(n_frames, input_fps, output_fps, batch):
+    """The passes of video_interpolate(fps=(input_fps, output_fps)) over n_frames frames: interp_schedule()'s passes, each
+    with the output frames it writes.  Output frame n sits at input time s = n input_fps / output_fps, for n = 0 ..
+    floor((n_frames - 1) output_fps / input_fps), computed exactly in Fractions.  An integer s is a copy of input frame s
+    (written by the pass that holds pair min(s, n_frames - 2)); any other s is the item (k, t) = (floor(s), float(s - k))
+    of the pass that holds pair k.  Returns a list of FpsPass(frames, pairs, items, copies): items are (n, k, t) and
+    copies (n, i), both with global frame indices.  Needs output_fps > input_fps (up-conversion); anything else raises
+    ValueError."""
+    fin, fout = parse_rate(input_fps), parse_rate(output_fps)
+    if fout <= fin:
+        raise ValueError(f"video: frame-rate conversion goes up: the output rate must exceed the input rate "
+                         f"(got {fin} -> {fout})")
+    passes = interp_schedule(n_frames, batch)
+    T, last = int(batch), int(n_frames) - 1
+    items, copies = [[] for _ in passes], [[] for _ in passes]
+    for n in range(last * fout // fin + 1):
+        s = n * fin / fout
+        k = s.numerator // s.denominator
+        if s.denominator == 1:
+            copies[min(k, last - 1) // T].append((n, k))
+        else:
+            items[k // T].append((n, k, float(s - k)))
+    return [FpsPass(p.frames, p.pairs, i, c) for p, i, c in zip(passes, items, copies)]
 
 
 def frame_number(k, m, j=None):
@@ -233,23 +276,41 @@ def video(model, frames, out, batch=8, workers=4, warm_start=False, flo=None, np
     return written
 
 
-def video_interpolate(model, frames, out, ts, batch=8, workers=4):
-    """Frame-rate up-conversion with a loaded networks.RAFT.RAFT model: the frames (a directory's sorted *.png / *.jpg, or
-    a list of paths, all of one size) and the m = len(ts) frames at times ts (strictly increasing inside (0, 1)) between
-    every consecutive pair, written as <out>/frame_<n:06d>.png with n = frame_number(k, m[, j]).  Every pass runs
-    interpolate_sequence on batch + 1 frames (interp_schedule()) and quantises on the GPU, so an interpolated frame equals
-    the single-pair CLI's PNG of model.interpolate(f_k, f_(k+1), ts) byte for byte.  The input frames are written as the
-    network saw them: the decoded bytes, or with model.input_size exactly the bytes of cv2.resize of them (which the GPU
-    resize reproduces).  Frames go in RGB with model.upstream and BGR otherwise, like the CLI; the files are BGR.  The
-    files do not depend on batch or workers.  Returns the written paths in output order."""
+def video_interpolate(model, frames, out, ts=None, batch=8, workers=4, fps=None):
+    """Frame-rate up-conversion with a loaded networks.RAFT.RAFT model of the frames (a directory's sorted *.png / *.jpg,
+    or a list of paths, all of one size), written as one numbered sequence <out>/frame_<n:06d>.png.  Give exactly one of:
+
+    - ts: the m = len(ts) frames at times ts (strictly increasing inside (0, 1)) between every consecutive pair, n =
+      frame_number(k, m[, j]).  Every pass runs interpolate_sequence on batch + 1 frames (interp_schedule()), so an
+      interpolated frame equals the single-pair CLI's PNG of model.interpolate(f_k, f_(k+1), ts) byte for byte.
+    - fps = (input_fps, output_fps): the sequence at output_fps > input_fps (rates as parse_rate() takes them), output
+      frame n at input time s = n input_fps / output_fps (fps_schedule()).  Every pass runs interpolate_sequence_at on
+      batch + 1 frames with the (pair, time) items of its pairs alone, so a frame at a fractional s equals the single-pair
+      CLI's PNG of model.interpolate(f_k, f_(k+1), float(s - k)) byte for byte; an integer s is input frame s.
+
+    Both quantise on the GPU.  The input frames are written as the network saw them: the decoded bytes, or with
+    model.input_size exactly the bytes of cv2.resize of them (which the GPU resize reproduces).  Frames go in RGB with
+    model.upstream and BGR otherwise, like the CLI; the files are BGR.  The files do not depend on batch or workers.
+    Returns the written paths in output order."""
     import cv2
 
     paths = list_frames(frames)
-    ts = check_times(ts)
-    batch, workers, m = int(batch), int(workers), len(ts)
+    if (ts is None) == (fps is None):
+        raise ValueError("video_interpolate: give the times ts or the rates fps = (input_fps, output_fps), exactly one")
+    batch, workers = int(batch), int(workers)
     if workers < 0:
         raise ValueError(f"video: workers must be >= 0 (got {workers})")
-    passes = interp_schedule(len(paths), batch)
+    last = len(paths) - 1
+    if fps is None:
+        ts = check_times(ts)
+        m = len(ts)
+        passes = interp_schedule(len(paths), batch)
+        n_out = frame_number(last, m) + 1
+        rows = m * batch  # output rows of one pass
+    else:
+        passes = fps_schedule(len(paths), *fps, batch)
+        n_out = sum(len(p.items) + len(p.copies) for p in passes)
+        rows = max(len(p.items) for p in passes)
     T = batch
     out = os.fspath(out)
     os.makedirs(out, exist_ok=True)
@@ -257,7 +318,6 @@ def video_interpolate(model, frames, out, ts, batch=8, workers=4):
     rgb = bool(model.upstream)
     size = model.input_size
     dev = engine.device
-    last = len(paths) - 1
 
     def name(n):
         return os.path.join(out, f"frame_{n:06d}.png")
@@ -267,15 +327,14 @@ def video_interpolate(model, frames, out, ts, batch=8, workers=4):
             img = cv2.resize(img, dsize=(size[1], size[0]))
         return cv2.cvtColor(img, cv2.COLOR_RGB2BGR) if rgb else img
 
-    def write(slot, rows, originals):  # writer thread: the files of one pass, once its copies have landed
-        for k, img in originals:
-            if not cv2.imwrite(name(frame_number(k, m)), original(img)):
-                raise OSError(f"cannot write {name(frame_number(k, m))}")
+    def write(slot, made, copies):  # writer thread: the files of one pass, once its copies have landed
+        for n, img in copies:
+            if not cv2.imwrite(name(n), original(img)):
+                raise OSError(f"cannot write {name(n)}")
         slot.event.synchronize()
-        for r, k in rows:
-            for j in range(m):
-                if not cv2.imwrite(name(frame_number(k, m, j)), slot.frames[j, r].numpy()):
-                    raise OSError(f"cannot write {name(frame_number(k, m, j))}")
+        for n, r in made:
+            if not cv2.imwrite(name(n), slot.frames[r].numpy()):
+                raise OSError(f"cannot write {name(n)}")
 
     decoders = ThreadPoolExecutor(workers) if workers > 0 else None
     writers = ThreadPoolExecutor(workers) if workers > 0 else None
@@ -310,27 +369,36 @@ def video_interpolate(model, frames, out, ts, batch=8, workers=4):
                 slot.wait()
                 for r, img in enumerate(imgs):
                     slot.frames[r].numpy()[...] = img
-                res = engine.interpolate_sequence(slot.frames, ts, uint8=True, bgr=rgb)
+                first = ps.frames[0]  # frame i is row i - first of the pass
+                if fps is None:  # row j T + r: pair r of the pass at ts[j]
+                    res = engine.interpolate_sequence(slot.frames, ts, uint8=True, bgr=rgb).flatten(0, 1)
+                    pairs = [(r, k) for r, k in enumerate(ps.pairs) if k is not None]
+                    made = [(frame_number(k, m, jt), jt * T + r) for r, k in pairs for jt in range(m)]
+                    copies = [(frame_number(k, m), k) for _, k in pairs] + ([(n_out - 1, last)]
+                                                                            if j == len(passes) - 1 else [])
+                else:  # row i: item i of the pass
+                    res = engine.interpolate_sequence_at(slot.frames, [(k - first, t) for _, k, t in ps.items],
+                                                         uint8=True, bgr=rgb)
+                    made = [(n, i) for i, (n, _, _) in enumerate(ps.items)]
+                    copies = ps.copies
                 slot.event = torch.cuda.Event()
                 slot.event.record(stream)
                 if outs is None:
-                    outs = [_Slot(frames=(tuple(res.shape), torch.uint8)) for _ in range(2)]
+                    outs = [_Slot(frames=((rows,) + tuple(res.shape[1:]), torch.uint8)) for _ in range(2)]
                 o = outs[j % 2]
                 o.wait()
-                o.frames.copy_(res, non_blocking=True)
+                o.frames[:len(res)].copy_(res, non_blocking=True)
                 o.event = torch.cuda.Event()
                 o.event.record(stream)
-                rows = [(r, k) for r, k in enumerate(ps.pairs) if k is not None]
-                originals = [(k, imgs[r]) for r, k in rows] + ([(last, imgs[rows[-1][0] + 1])] if j == len(passes) - 1
-                                                                else [])
+                copies = [(n, imgs[i - first]) for n, i in copies]
                 if writers is None:
-                    write(o, rows, originals)
+                    write(o, made, copies)
                 else:
-                    o.futures.append(writers.submit(write, o, rows, originals))
+                    o.futures.append(writers.submit(write, o, made, copies))
             for o in outs or ():
                 o.wait()
     finally:
         for pool in (decoders, writers):
             if pool is not None:
                 pool.shutdown(wait=True, cancel_futures=True)
-    return [name(n) for n in range(frame_number(last, m) + 1)]
+    return [name(n) for n in range(n_out)]
