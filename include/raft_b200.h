@@ -424,6 +424,20 @@ int rb_frame_metrics_workspace_bytes(int B, int H, int W, size_t* bytes);
 int rb_frame_metrics(const void* pred, int pred_is_u8, const uint8_t* gt, int B, int H, int W, double* stats,
                      void* workspace, size_t workspace_bytes, void* stream);
 
+/* ---- F15: scene-cut scores -- where frame-rate conversion and warm-started video flow stop ------------------------
+ * frames: [N,H,W,3] uint8, the decoded frames at their own size (any channel order: the bins are symmetric in it).
+ * hist: [N][RB_SCENE_BINS] int32, frame n's joint colour histogram, pixel (c0, c1, c2) in bin
+ *   (c0 >> 5) * 64 + (c1 >> 5) * 8 + (c2 >> 5) (8 levels per channel), each pixel counted once; zeroed by the call.
+ * scores: [N-1] fp32, scores[k] = fl32((double)(H*W - sum_b min(hist[k][b], hist[k+1][b])) / (double)(H*W)): one minus
+ *   the histogram intersection of frames k and k + 1, in [0, 1] -- 0 for frames with one histogram, 1 for frames that
+ *   share no bin.
+ * Counts are integers (warp-aggregated shared-memory atomics, then one global atomic per block and nonzero bin), so both
+ * outputs are exact and independent of the launch order.  A memset and two launches on the stream; no allocation, no
+ * synchronisation, graph-capturable.  Null pointers, N < 2, H/W <= 0, H*W >= 2^31 and N frames that exceed one grid ->
+ * RB_ERR_* before any CUDA call. */
+#define RB_SCENE_BINS 512
+int rb_scene_cut_scores(const uint8_t* frames, int N, int H, int W, int32_t* hist, float* scores, void* stream);
+
 /* ---- F3 (input edge): dataflow/test_dataflow.py:56-61,96-97 + the SURVEY 8(d) shape policy ------------------
  * src: [B,H,W,3] device frames, BGR like cv2.imdecode -- fp32 in [0,1] (src_is_u8 = 0) or uint8 in [0,255]
  * (src_is_u8 = 1: x/255.0f, the reference's np.float32(x)/255.0, bit for bit).  dst: [B,H+pt+pb,W+pl+pr,3] fp32

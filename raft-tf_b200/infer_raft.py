@@ -54,6 +54,11 @@ the frame interpolated at time s - floor(s) between frames floor(s) and floor(s)
 ``<--out>/frame_<n:06d>.png`` (raft_b200.video):
 
     python infer_raft.py --path film/ --out tv/ --input-fps 24 --fps 60 --load raft-things.npz [--batch 8]
+
+--scene-cut THRESH (with --path and --interpolate, --input-fps/--fps or --warm-start) scores every consecutive pair on the
+GPU (one minus the intersection of the frames' colour histograms, in [0, 1]); a pair above THRESH is a scene cut.  There
+interpolated frames are copies of the nearer input frame, and warm-started flow restarts cold.  The run prints
+``scene cuts: <count> at pairs <k> ...``.  No default: pick the threshold for the footage.
 """
 import glob
 import argparse
@@ -136,6 +141,10 @@ def parser():
     p.add_argument('--fps', default=None, metavar='OUT',
                    help='extension, with --path and --input-fps: convert the frames to OUT frames per second (above IN), '
                         'written as <--out>/frame_<n:06d>.png')
+    p.add_argument('--scene-cut', type=float, default=None, metavar='THRESH',
+                   help='extension, with --path and one of --interpolate, --input-fps/--fps or --warm-start: a threshold '
+                        'in [0, 1] on the colour-histogram score of each frame pair; a pair above it is a scene cut, '
+                        'where interpolation copies the nearer frame and warm-started flow restarts cold')
     p.add_argument('--native-flow', action='store_true',
                    help="extension: resize the written flow(s) back to im1's size (flow_utils.resize_flow)")
     p.add_argument('--upstream', action='store_true',
@@ -166,6 +175,14 @@ def main(argv=None):
             p.error(f'--fps {args.fps} must exceed --input-fps {args.input_fps}: frame-rate conversion goes up only')
     if args.interpolate and not all(0.0 <= t <= 1.0 for t in args.interpolate):
         p.error('--interpolate: every T must be in [0, 1]')
+    if args.scene_cut is not None:
+        if not 0.0 <= args.scene_cut <= 1.0:
+            p.error(f'--scene-cut: {args.scene_cut} is not a threshold in [0, 1]')
+        if args.mode != 'test' or args.path is None:
+            p.error('--scene-cut finds the cuts of a frame directory: it needs --path DIR (and no -m val)')
+        if not (args.interpolate or fps is not None or args.warm_start):
+            p.error('--scene-cut needs --interpolate, --input-fps/--fps or --warm-start: cold flows over --path do not '
+                    'depend on neighbouring pairs, so a cut changes nothing')
     if args.mode == 'val':
         if not args.data or not args.dataset:
             p.error('-m val needs --data <dataset root> and --dataset {sintel,kitti,vimeo}')
@@ -263,7 +280,9 @@ def run_video(args):
     model = RAFT.RAFT(None if size is None else size + (3,), args, iters=iters, input_size=size, upstream=args.upstream,
                       mixed_precision=args.mixed_precision).load(args.load)
     files = video(model, args.path, args.out, batch=args.batch, workers=args.workers, warm_start=args.warm_start,
-                  flo=args.flo, npy=args.npy, native_flow=args.native_flow)
+                  flo=args.flo, npy=args.npy, native_flow=args.native_flow, scene_cut=args.scene_cut)
+    if args.scene_cut is not None:
+        files = _print_cuts(*files)
     print(f"{len(files)} files written under {args.out}" + (" and the --flo / --npy directories" if args.flo or args.npy
                                                             else ""))
     return 0
@@ -279,9 +298,17 @@ def run_video_interpolate(args, fps=None):
     model = RAFT.RAFT(None if size is None else size + (3,), args, iters=iters, input_size=size, upstream=args.upstream,
                       mixed_precision=args.mixed_precision).load(args.load)
     files = video_interpolate(model, args.path, args.out, args.interpolate, batch=args.batch, workers=args.workers,
-                              fps=fps)
+                              fps=fps, scene_cut=args.scene_cut)
+    if args.scene_cut is not None:
+        files = _print_cuts(*files)
     print(f"{len(files)} frames written under {args.out}")
     return 0
+
+
+def _print_cuts(files, cuts):
+    """--scene-cut: the number of cut pairs and their indices (pair k: frame k -> k + 1); returns files."""
+    print(f"scene cuts: {len(cuts)}" + (" at pairs " + " ".join(str(k) for k in cuts) if cuts else ""))
+    return files
 
 
 def validate(args):

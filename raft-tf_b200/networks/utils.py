@@ -111,6 +111,28 @@ def frame_metrics(pred, gt):
     return stats
 
 
+SCENE_BINS = 512  # RB_SCENE_BINS: 8 levels per channel
+
+
+def scene_cut_scores(frames, return_hist=False):
+    """Extension (scene cuts of a video): the [N-1] fp32 scores of [N,H,W,3] uint8 CUDA frames (N >= 2, any channel
+    order), scores[k] = 1 - the intersection of the joint colour histograms of frames k and k + 1 (8 levels per channel,
+    bin (c0 >> 5) 64 + (c1 >> 5) 8 + (c2 >> 5)) over H W, rounded once to fp32: 0 for frames with one histogram, 1 for
+    frames that share no bin (rb_scene_cut_scores; exact).  With return_hist also the [N,512] int32 histograms.  Wrong
+    shapes or dtypes raise ValueError."""
+    if not (isinstance(frames, torch.Tensor) and frames.is_cuda and frames.dim() == 4 and frames.shape[-1] == 3
+            and frames.dtype == torch.uint8 and frames.shape[0] >= 2):
+        raise ValueError(f"scene_cut_scores: frames must be a [N,H,W,3] uint8 CUDA tensor with N >= 2 (got "
+                         f"{getattr(frames, 'shape', None)} {getattr(frames, 'dtype', type(frames))})")
+    f = frames.contiguous()
+    N, H, W, _ = f.shape
+    hist = torch.empty(N, SCENE_BINS, dtype=torch.int32, device=f.device)
+    scores = torch.empty(N - 1, dtype=torch.float32, device=f.device)
+    with torch.cuda.device(f.device):
+        capi.check(capi.lib.rb_scene_cut_scores(capi.ptr(f), N, H, W, capi.ptr(hist), capi.ptr(scores), capi.stream()))
+    return (scores, hist) if return_hist else scores
+
+
 def forward_interpolate(flow):
     """Extension (upstream RAFT's core/utils/utils.py forward_interpolate, on the GPU): every grid point of the [B,h,w,2]
     fp32 CUDA flow takes the flow of the nearest source pixel x + flow(x) that lands strictly inside the grid, per

@@ -84,6 +84,7 @@ SIGNATURES = {
     "rb_flow_metrics": (_i, [_vp, _f, _vp, _vp, _i, _i, _i, _vp, _vp, _vp, _sz, _vp]),
     "rb_frame_metrics_workspace_bytes": (_i, [_i, _i, _i, _psz]),
     "rb_frame_metrics": (_i, [_vp, _i, _vp, _i, _i, _i, _vp, _vp, _sz, _vp]),
+    "rb_scene_cut_scores": (_i, [_vp, _i, _i, _i, _vp, _vp, _vp]),
     "rb_flow_forward_interpolate_workspace_bytes": (_i, [_i, _i, _i, _psz]),
     "rb_flow_forward_interpolate": (_i, [_vp, _vp, _i, _i, _i, _vp, _sz, _vp]),
     "rb_flow_to_color_workspace_bytes": (_i, [_i, _i, _i, _psz]),

@@ -22,6 +22,12 @@ Pipeline, as in raft_b200.evaluate: worker threads decode the frames of the next
 pinned slots used in turn, each refilled only after the event behind its pass has completed; the colour images (and the
 flows, when written) are copied to two pinned output slots and PNG-encoded and written by writer threads.  The files are
 the same bytes for every workers value.
+
+Scene cuts (scene_cut=<threshold in [0, 1]>, video_interpolate and warm-started video): each pass's decoded frames are
+copied to the GPU once and scored there (networks.utils.scene_cut_scores: one minus the intersection of consecutive
+frames' colour histograms); a pair whose score exceeds the threshold is a cut.  Frame-rate conversion copies the nearer
+input frame instead of blending two shots (cut_copy(), split_cut_items()), and warm-started flow restarts its chain
+(cold_start()).  Without a threshold none of this runs.
 """
 from __future__ import annotations
 
@@ -138,6 +144,43 @@ def fps_schedule(n_frames, input_fps, output_fps, batch):
     return [FpsPass(p.frames, p.pairs, i, c) for p, i, c in zip(passes, items, copies)]
 
 
+def check_scene_cut(scene_cut):
+    """A scene-cut threshold as a float in [0, 1]: pair k (frame k -> k + 1) is a cut when its score (networks.utils.
+    scene_cut_scores) exceeds it, so 1.0 finds none.  Anything else raises ValueError."""
+    try:
+        thr = float(scene_cut)
+    except (TypeError, ValueError):
+        thr = None
+    if thr is None or not 0.0 <= thr <= 1.0:
+        raise ValueError(f"video: scene_cut must be a threshold in [0, 1] (got {scene_cut!r})")
+    return thr
+
+
+def pass_cuts(pairs, scores, thr):
+    """The cut pairs of one pass, in order: the pair k of row r is a cut when float(scores[r]) > thr; idle rows (None)
+    are ignored."""
+    return [k for r, k in enumerate(pairs) if k is not None and float(scores[r]) > thr]
+
+
+def cut_copy(k, t):
+    """The input frame that stands in for the frame at time t of pair k when the pair is a scene cut: the nearer one, k
+    for t <= 0.5 and k + 1 after it (blending two shots would give a ghosted cross-dissolve)."""
+    return k if t <= 0.5 else k + 1
+
+
+def split_cut_items(items, cuts):
+    """The (n, k, t) items of an fps pass (fps_schedule()) split by the cut pairs: (the items of pairs that are not cuts,
+    in order; the copies (n, cut_copy(k, t)) that replace the others)."""
+    return ([it for it in items if it[1] not in cuts],
+            [(n, cut_copy(k, t)) for n, k, t in items if k in cuts])
+
+
+def cold_start(k, cuts):
+    """Whether pair k of a warm-started video runs cold: the first pair, a cut pair (it spans two shots) and the pair
+    after a cut (the first of a shot), so each shot runs the chain it would run alone."""
+    return k == 0 or k in cuts or k - 1 in cuts
+
+
 def frame_number(k, m, j=None):
     """The output index of input frame k (j None), or of the j-th of the m frames interpolated between frames k and k + 1:
     k (m + 1) and k (m + 1) + j + 1.  N input frames give (N - 1)(m + 1) + 1 outputs."""
@@ -162,7 +205,8 @@ class _Slot:
             self.event.synchronize()
 
 
-def video(model, frames, out, batch=8, workers=4, warm_start=False, flo=None, npy=None, native_flow=False):
+def video(model, frames, out, batch=8, workers=4, warm_start=False, flo=None, npy=None, native_flow=False,
+          scene_cut=None):
     """The flow between every pair of consecutive frames of a loaded networks.RAFT.RAFT model, written as
     <out>/flow_<k:06d>.png for pair k (frame k -> k + 1; the GPU colour coding of networks.utils.flow_to_color, BGR), and
     with flo / npy (directories) also as flow_<k:06d>.flo / .npy.  frames: a directory (its sorted *.png and *.jpg) or a
@@ -171,15 +215,24 @@ def video(model, frames, out, batch=8, workers=4, warm_start=False, flo=None, np
     every pair from the previous one (batch must be 1).  native_flow resizes the flows of a model with input_size back to
     the frames' size (networks.utils.resize_flow) before they are coloured or saved.  Each flow equals the model's
     forward(f_k, f_(k+1)) (warm_start: the chain forward(..., flow_init=forward_interpolate(flow_low))) bit for bit.
-    Returns the written paths, pair by pair."""
+
+    scene_cut (warm_start only; a threshold in [0, 1]) restarts the chain at scene cuts: every pair is scored on the GPU
+    (networks.utils.scene_cut_scores of the decoded frames k and k + 1, the previous one kept on the device), pair k is a
+    cut when its score exceeds scene_cut, and it runs cold when cold_start(k, cuts) -- so each shot's flows equal those of
+    video(warm_start=True) on that shot's frames alone, and a cut pair's flow is the cold forward(f_k, f_(k+1)).
+    Returns the written paths, pair by pair; with scene_cut the tuple (paths, cuts), cuts the increasing cut pairs."""
     import cv2
     from flow_utils import write_flo
-    from networks.utils import flow_to_color, forward_interpolate, resize_flow
+    from networks.utils import flow_to_color, forward_interpolate, resize_flow, scene_cut_scores
 
     paths = list_frames(frames)
     batch, workers = int(batch), int(workers)
     if workers < 0:
         raise ValueError(f"video: workers must be >= 0 (got {workers})")
+    thr = None if scene_cut is None else check_scene_cut(scene_cut)
+    if thr is not None and not warm_start:
+        raise ValueError("video: scene_cut restarts the warm-start chain at cuts; without warm_start every pair runs cold, "
+                         "so a cut changes nothing")
     passes = schedule(len(paths), batch, warm_start)
     T = batch
     dirs = {"png": os.fspath(out), "flo": None if flo is None else os.fspath(flo),
@@ -215,6 +268,7 @@ def video(model, frames, out, batch=8, workers=4, warm_start=False, flo=None, np
         return [(i, decoders.submit(_imread, paths[i], rgb).result) for i in passes[j].frames]
 
     written, shape, ins, outs, init = [], None, None, None, None
+    on_dev, cuts = None, []  # scene_cut: frames k and k + 1 in rows k % 2 and (k + 1) % 2 (the score is symmetric)
     try:
         with torch.cuda.device(dev):
             stream = torch.cuda.current_stream(dev)
@@ -239,6 +293,19 @@ def video(model, frames, out, batch=8, workers=4, warm_start=False, flo=None, np
                 host = slot.frames[:len(imgs)]
                 for r, img in enumerate(imgs):
                     host[r].numpy()[...] = img
+                if thr is not None:  # one pair per pass: score it, then hand the engine the device rows
+                    k = ps.pairs[0]
+                    if on_dev is None:
+                        on_dev = torch.empty((2,) + shape, dtype=torch.uint8, device=dev)
+                    if ps.carry:
+                        on_dev[(k + 1) % 2].copy_(host[0], non_blocking=True)
+                        host = on_dev[(k + 1) % 2][None]
+                    else:
+                        on_dev.copy_(host, non_blocking=True)
+                        host = on_dev
+                    cuts += pass_cuts(ps.pairs, scene_cut_scores(on_dev).cpu(), thr)
+                    if cold_start(k, cuts):
+                        init = None
                 if warm_start:
                     low, flow = engine.forward_sequence(host, carry=ps.carry, flow_init=init, return_low=True)
                     init = forward_interpolate(low)  # before the next pass overwrites flow_low
@@ -273,10 +340,10 @@ def video(model, frames, out, batch=8, workers=4, warm_start=False, flo=None, np
         for pool in (decoders, writers):
             if pool is not None:
                 pool.shutdown(wait=True, cancel_futures=True)
-    return written
+    return written if thr is None else (written, cuts)
 
 
-def video_interpolate(model, frames, out, ts=None, batch=8, workers=4, fps=None):
+def video_interpolate(model, frames, out, ts=None, batch=8, workers=4, fps=None, scene_cut=None):
     """Frame-rate up-conversion with a loaded networks.RAFT.RAFT model of the frames (a directory's sorted *.png / *.jpg,
     or a list of paths, all of one size), written as one numbered sequence <out>/frame_<n:06d>.png.  Give exactly one of:
 
@@ -291,8 +358,15 @@ def video_interpolate(model, frames, out, ts=None, batch=8, workers=4, fps=None)
     Both quantise on the GPU.  The input frames are written as the network saw them: the decoded bytes, or with
     model.input_size exactly the bytes of cv2.resize of them (which the GPU resize reproduces).  Frames go in RGB with
     model.upstream and BGR otherwise, like the CLI; the files are BGR.  The files do not depend on batch or workers.
-    Returns the written paths in output order."""
+
+    scene_cut (a threshold in [0, 1]) stops interpolation at scene cuts: each pass's frames are copied to the GPU once and
+    scored there (networks.utils.scene_cut_scores of the decoded frames), and pair k is a cut when its score exceeds
+    scene_cut.  Every frame of a cut pair at time t is then a copy of the nearer input frame (cut_copy(): k for t <= 0.5,
+    else k + 1), written like the input frames; only the other pairs' frames are interpolated, and a pass with none of
+    them makes no engine call.  The other files are the bytes of the run without scene_cut.
+    Returns the written paths in output order; with scene_cut the tuple (paths, cuts), cuts the increasing cut pairs."""
     import cv2
+    from networks.utils import scene_cut_scores
 
     paths = list_frames(frames)
     if (ts is None) == (fps is None):
@@ -300,6 +374,7 @@ def video_interpolate(model, frames, out, ts=None, batch=8, workers=4, fps=None)
     batch, workers = int(batch), int(workers)
     if workers < 0:
         raise ValueError(f"video: workers must be >= 0 (got {workers})")
+    thr = None if scene_cut is None else check_scene_cut(scene_cut)
     last = len(paths) - 1
     if fps is None:
         ts = check_times(ts)
@@ -327,10 +402,12 @@ def video_interpolate(model, frames, out, ts=None, batch=8, workers=4, fps=None)
             img = cv2.resize(img, dsize=(size[1], size[0]))
         return cv2.cvtColor(img, cv2.COLOR_RGB2BGR) if rgb else img
 
-    def write(slot, made, copies):  # writer thread: the files of one pass, once its copies have landed
+    def write(slot, made, copies):  # writer thread: the files of one pass, once its copies have landed (slot None: none)
         for n, img in copies:
             if not cv2.imwrite(name(n), original(img)):
                 raise OSError(f"cannot write {name(n)}")
+        if slot is None:
+            return
         slot.event.synchronize()
         for n, r in made:
             if not cv2.imwrite(name(n), slot.frames[r].numpy()):
@@ -346,6 +423,7 @@ def video_interpolate(model, frames, out, ts=None, batch=8, workers=4, fps=None)
         return [(i, decoders.submit(_imread, paths[i], rgb).result) for i in passes[j].frames]
 
     shape, ins, outs = None, None, None
+    on_dev, cuts, loose = None, [], []  # scene_cut: the pass's frames on the GPU; the writes of passes without a call
     try:
         with torch.cuda.device(dev):
             stream = torch.cuda.current_stream(dev)
@@ -370,35 +448,53 @@ def video_interpolate(model, frames, out, ts=None, batch=8, workers=4, fps=None)
                 for r, img in enumerate(imgs):
                     slot.frames[r].numpy()[...] = img
                 first = ps.frames[0]  # frame i is row i - first of the pass
+                src, cut = slot.frames, ()
+                if thr is not None:  # score the pass on the GPU; the engine then reads the frames from there too
+                    if on_dev is None:
+                        on_dev = torch.empty(slot.frames.shape, dtype=torch.uint8, device=dev)
+                    on_dev.copy_(slot.frames, non_blocking=True)
+                    src, cut = on_dev, pass_cuts(ps.pairs, scene_cut_scores(on_dev).cpu(), thr)
+                    cuts += cut
+                res = None
                 if fps is None:  # row j T + r: pair r of the pass at ts[j]
-                    res = engine.interpolate_sequence(slot.frames, ts, uint8=True, bgr=rgb).flatten(0, 1)
                     pairs = [(r, k) for r, k in enumerate(ps.pairs) if k is not None]
-                    made = [(frame_number(k, m, jt), jt * T + r) for r, k in pairs for jt in range(m)]
+                    live = [(r, k) for r, k in pairs if k not in cut]
+                    if live:
+                        res = engine.interpolate_sequence(src, ts, uint8=True, bgr=rgb).flatten(0, 1)
+                    made = [(frame_number(k, m, jt), jt * T + r) for r, k in live for jt in range(m)]
                     copies = [(frame_number(k, m), k) for _, k in pairs] + ([(n_out - 1, last)]
                                                                             if j == len(passes) - 1 else [])
+                    copies += [(frame_number(k, m, jt), cut_copy(k, t)) for k in cut for jt, t in enumerate(ts)]
                 else:  # row i: item i of the pass
-                    res = engine.interpolate_sequence_at(slot.frames, [(k - first, t) for _, k, t in ps.items],
-                                                         uint8=True, bgr=rgb)
-                    made = [(n, i) for i, (n, _, _) in enumerate(ps.items)]
-                    copies = ps.copies
+                    items, cut_copies = split_cut_items(ps.items, cut)
+                    if items:
+                        res = engine.interpolate_sequence_at(src, [(k - first, t) for _, k, t in items], uint8=True,
+                                                             bgr=rgb)
+                    made = [(n, i) for i, (n, _, _) in enumerate(items)]
+                    copies = ps.copies + cut_copies
                 slot.event = torch.cuda.Event()
                 slot.event.record(stream)
-                if outs is None:
-                    outs = [_Slot(frames=((rows,) + tuple(res.shape[1:]), torch.uint8)) for _ in range(2)]
-                o = outs[j % 2]
-                o.wait()
-                o.frames[:len(res)].copy_(res, non_blocking=True)
-                o.event = torch.cuda.Event()
-                o.event.record(stream)
+                o = None
+                if res is not None:
+                    if outs is None:
+                        outs = [_Slot(frames=((rows,) + tuple(res.shape[1:]), torch.uint8)) for _ in range(2)]
+                    o = outs[j % 2]
+                    o.wait()
+                    o.frames[:len(res)].copy_(res, non_blocking=True)
+                    o.event = torch.cuda.Event()
+                    o.event.record(stream)
                 copies = [(n, imgs[i - first]) for n, i in copies]
                 if writers is None:
                     write(o, made, copies)
                 else:
-                    o.futures.append(writers.submit(write, o, made, copies))
+                    (loose if o is None else o.futures).append(writers.submit(write, o, made, copies))
             for o in outs or ():
                 o.wait()
+            for f in loose:
+                f.result()
     finally:
         for pool in (decoders, writers):
             if pool is not None:
                 pool.shutdown(wait=True, cancel_futures=True)
-    return [name(n) for n in range(n_out)]
+    paths = [name(n) for n in range(n_out)]
+    return paths if thr is None else (paths, cuts)
