@@ -59,6 +59,8 @@ enum {
  *                      into the weights first) and sums in cuDNN's order.
  *                    The flow misses the 1e-3 bar of RB_MATH_TC by design: about 1e-2 max-abs against fp64 at 64x96 and
  *                    8 iterations, 1e-1 at 128x256 and 32 (DESIGN section 2).
+ * On operands whose products and partial sums are exact in fp32, every back end returns the exact value of its own
+ * arithmetic, whatever the tile configuration (tests/test_gpu_exact_conv.py pins this bit for bit).
  * Like the semantics, the mode is per thread and read when a kernel is launched (it may be set inside graph capture). */
 enum { RB_MATH_TC = 0, RB_MATH_SIMT = 1, RB_MATH_TC_FP16 = 2 };
 

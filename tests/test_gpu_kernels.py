@@ -193,32 +193,34 @@ CONV_CASES = [
 @pytest.mark.parametrize("mode", ["tc", "simt"])
 @pytest.mark.parametrize("case", CONV_CASES, ids=lambda c: "x".join(map(str, c)))
 def test_conv2d(cuda, mode, case):
-    """tensorpack Conv2D(stride 1,'same')+bias+ReLU (A14) against torch fp64."""
+    """tensorpack Conv2D(stride 1,'same')+bias (A14) against torch fp64, with ReLU and without (negative outputs compared
+    too).  Bit for bit on exact operands: test_gpu_exact_conv.py."""
     from raft_b200 import capi
     B, h, w, cin, cout, kh, kw = case
     g = torch.Generator().manual_seed(sum(case))
     x = torch.randn(B, h, w, cin, generator=g)
     W = torch.randn(kh, kw, cin, cout, generator=g) * (2.0 / (kh * kw * cin)) ** 0.5
     b = torch.randn(cout, generator=g) * 0.1
-    ref = O.conv2d(x.double(), W.double(), b.double(), 1, torch.relu)
     lib = capi.lib
     xd = x.to(cuda)
-    y = torch.full((B, h, w, cout), float("nan"), device=cuda)
     wsb = capi.size_query(lib.rb_conv2d_workspace_bytes, B, h, w, cin, cout, kh, kw)
     ws = torch.zeros(wsb, dtype=torch.uint8, device=cuda)
     Wn, bn = np.ascontiguousarray(W.numpy()), np.ascontiguousarray(b.numpy())
-    capi.check(lib.rb_set_math_mode(dict(_modes())[mode]))
-    try:
-        capi.check(lib.rb_conv2d(capi.ptr(xd), Wn.ctypes.data, bn.ctypes.data, capi.ptr(y), B, h, w, cin, cout, kh, kw,
-                                 1, capi.ptr(ws), wsb, capi.stream()))
-        torch.cuda.synchronize()
-    finally:
-        lib.rb_set_math_mode(capi.RB_MATH_TC)
-    yc = y.cpu().double()
-    assert torch.isfinite(yc).all(), f"{int((~torch.isfinite(yc)).sum())} non-finite outputs (unwritten?)"
-    err = (yc - ref).abs().max().item()
-    scale = ref.abs().max().item()
-    assert err < 2e-5 * max(scale, 1.0), f"max abs err {err:.3e} (scale {scale:.2f})"
+    for relu in (1, 0):
+        ref = O.conv2d(x.double(), W.double(), b.double(), 1, torch.relu if relu else None)
+        y = torch.full((B, h, w, cout), float("nan"), device=cuda)
+        capi.check(lib.rb_set_math_mode(dict(_modes())[mode]))
+        try:
+            capi.check(lib.rb_conv2d(capi.ptr(xd), Wn.ctypes.data, bn.ctypes.data, capi.ptr(y), B, h, w, cin, cout, kh, kw,
+                                     relu, capi.ptr(ws), wsb, capi.stream()))
+            torch.cuda.synchronize()
+        finally:
+            lib.rb_set_math_mode(capi.RB_MATH_TC)
+        yc = y.cpu().double()
+        assert torch.isfinite(yc).all(), f"relu={relu}: {int((~torch.isfinite(yc)).sum())} non-finite outputs (unwritten?)"
+        err = (yc - ref).abs().max().item()
+        scale = ref.abs().max().item()
+        assert err < 2e-5 * max(scale, 1.0), f"relu={relu}: max abs err {err:.3e} (scale {scale:.2f})"
 
 
 @pytest.mark.parametrize("mode", ["tc", "simt"])
@@ -234,25 +236,26 @@ def test_conv2d_stride2(cuda, mode, case):
     x = torch.randn(B, h, w, cin, generator=g)
     W = torch.randn(k, k, cin, cout, generator=g) * (2.0 / (k * k * cin)) ** 0.5
     b = torch.randn(cout, generator=g) * 0.1
-    ref = O.conv2d(x.double(), W.double(), b.double(), 2, torch.relu)
     lib = capi.lib
     oh, ow = (h + 1) // 2, (w + 1) // 2
-    assert ref.shape == (B, oh, ow, cout)
-    y = torch.full((B, oh, ow, cout), float("nan"), device=cuda)
     wsb = capi.size_query(lib.rb_conv2d_workspace_bytes, B, h, w, cin, cout, k, k)
     ws = torch.zeros(wsb, dtype=torch.uint8, device=cuda)
     Wn, bn = np.ascontiguousarray(W.numpy()), np.ascontiguousarray(b.numpy())
-    capi.check(lib.rb_set_math_mode(dict(_modes())[mode]))
-    try:
-        capi.check(lib.rb_conv2d_strided(capi.ptr(x.to(cuda)), Wn.ctypes.data, bn.ctypes.data, capi.ptr(y), B, h, w, cin, cout,
-                                         k, k, 2, 1, capi.ptr(ws), wsb, capi.stream()))
-        torch.cuda.synchronize()
-    finally:
-        lib.rb_set_math_mode(capi.RB_MATH_TC)
-    yc = y.cpu().double()
-    assert torch.isfinite(yc).all(), f"{int((~torch.isfinite(yc)).sum())} non-finite outputs (unwritten?)"
-    err = (yc - ref).abs().max().item()
-    assert err < 2e-5 * max(ref.abs().max().item(), 1.0), f"max abs err {err:.3e}"
+    for relu in (1, 0):  # without ReLU the negative outputs are compared too
+        ref = O.conv2d(x.double(), W.double(), b.double(), 2, torch.relu if relu else None)
+        assert ref.shape == (B, oh, ow, cout)
+        y = torch.full((B, oh, ow, cout), float("nan"), device=cuda)
+        capi.check(lib.rb_set_math_mode(dict(_modes())[mode]))
+        try:
+            capi.check(lib.rb_conv2d_strided(capi.ptr(x.to(cuda)), Wn.ctypes.data, bn.ctypes.data, capi.ptr(y), B, h, w, cin,
+                                             cout, k, k, 2, relu, capi.ptr(ws), wsb, capi.stream()))
+            torch.cuda.synchronize()
+        finally:
+            lib.rb_set_math_mode(capi.RB_MATH_TC)
+        yc = y.cpu().double()
+        assert torch.isfinite(yc).all(), f"relu={relu}: {int((~torch.isfinite(yc)).sum())} non-finite outputs (unwritten?)"
+        err = (yc - ref).abs().max().item()
+        assert err < 2e-5 * max(ref.abs().max().item(), 1.0), f"relu={relu}: max abs err {err:.3e}"
     assert lib.rb_conv2d_strided(capi.ptr(y), Wn.ctypes.data, None, capi.ptr(y), B, h, w, cin, cout, k, k, 3, 0, capi.ptr(ws), wsb,
                                  capi.stream()) == -3  # RB_ERR_UNSUPPORTED: stride 3
 
