@@ -349,6 +349,40 @@ int rb_frame_synthesize_items(const float* frames0, const float* frames1, int Hp
                               const int32_t* item_sample, const float* item_t, int n_items, void* out, int out_u8,
                               int bgr, int B, int H, int W, void* stream);
 
+/* ---- F16: the blend at the frames' own size from flows at the network size ----------------------------------------
+ * The network runs at H x W (an engine's input_size); the frames have their own Hs x Ws.  The reversal stays at H x W
+ * (flow_t0, flow_t1 [n,H,W,2] fp32 and empty0, empty1 [n,H,W] uint8 from rb_flow_reverse_multi / _items), and output
+ * pixel p = (x, y) of Hs x Ws of sample i is, bit for bit,
+ *   rb_frame_synthesize_*(prepare(frames0), prepare(frames1), Hs, Ws, 0, 0, resize_flow(flow_t0), resize_flow(flow_t1),
+ *                         nearest(empty0), nearest(empty1), ...)
+ * without any Hs x Ws fp32 intermediate, where
+ *   resize_flow = rb_flow_resize(flow_t[i], Hs, Ws): cv2's float bilinear resize (copy / OpenCV / IPP as there), then
+ *                 u *= fl32(Ws / W), v *= fl32(Hs / H) -- the flow in the frames' pixels;
+ *   nearest     = empty[i][ys][xs], ys = ((2y+1) H) div (2 Hs), xs = ((2x+1) W) div (2 Ws) in 64-bit integers: the network
+ *                 pixel whose area holds p's centre.  This is neither cv2's INTER_NEAREST nor INTER_NEAREST_EXACT (both
+ *                 pick other pixels at 432x1024 -> 1080x1920);
+ *   prepare     = uint8 frames (frames_u8 = 1) divided as rb_frames_prepare does (np.float32(u) / 255), fp32 frames
+ *                 (frames_u8 = 0) as they are.
+ * frames0, frames1 [B,Hs,Ws,3], unpadded (an engine's staging buffer of raw frames); out as rb_frame_synthesize_pairs /
+ * _items at Hs x Ws, fp32 (out_u8 = 0) or quantised uint8 (out_u8 = 1, bgr = 1 reverses the channels).  Hs x Ws = H x W
+ * is the existing blend bit for bit, and t = 0 with uint8 frames and uint8 output returns frames0 byte for byte.
+ * One thread per output pixel; the low-resolution flows and masks are read through the read-only path, uint8 frames as
+ * bytes.  No allocation, no synchronisation, graph-capturable.
+ * rb_frame_synthesize_pairs_resized: ts, n_t, pair b of time i as rb_frame_synthesize_pairs; out [n_t,B,Hs,Ws,3].
+ * rb_frame_synthesize_items_resized: item i blends frames0[item_sample[i]] and frames1[item_sample[i]] at item_t[i] as
+ * rb_frame_synthesize_items; out [n_items,Hs,Ws,3].
+ * Null pointers, frames_u8 / out_u8 / bgr not 0 or 1, n < 1 or > RB_INTERP_MAX_STEPS, a t outside [0, 1] (or NaN), a
+ * sample outside [0, B), B/H/W/Hs/Ws <= 0 and Hs*Ws >= 2^32 -> RB_ERR_* before any CUDA call. */
+int rb_frame_synthesize_pairs_resized(const void* frames0, const void* frames1, int frames_u8, int Hs, int Ws,
+                                      const float* flow_t0, const float* flow_t1, const uint8_t* empty0,
+                                      const uint8_t* empty1, int H, int W, const float* ts, int n_t, void* out,
+                                      int out_u8, int bgr, int B, void* stream);
+int rb_frame_synthesize_items_resized(const void* frames0, const void* frames1, int frames_u8, int Hs, int Ws,
+                                      const float* flow_t0, const float* flow_t1, const uint8_t* empty0,
+                                      const uint8_t* empty1, int H, int W, const int32_t* item_sample,
+                                      const float* item_t, int n_items, void* out, int out_u8, int bgr, int B,
+                                      void* stream);
+
 /* ---- F9: end-point-error metrics (upstream RAFT's evaluate.py validate_sintel / validate_kitti) ---------------------
  * flow, gt: [B,H,W,2] fp32; valid: [B,H,W] uint8, nonzero = the pixel counts (NULL: every pixel counts).  Per pixel,
  * every operation rounded on its own (no FMA contraction), so the values equal upstream's torch expressions bit for bit:

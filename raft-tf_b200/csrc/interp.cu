@@ -1,5 +1,7 @@
 // F6: frame interpolation.  rb_flow_reverse is the reference's flow reversal (flow_utils.py:166-274,
 // reverse_flow_avg_skip_static) batched and bit for bit; rb_frame_synthesize warps both frames to time t and blends them.
+// The *_resized blends do the same at the frames' own size from flows reversed at the network size, resizing each flow
+// (resize_px.cuh, rb_flow_resize's arithmetic) inside the kernel.
 //
 // Reversal: every source pixel of frame 0 is moved by time_step * flow to its nearest target pixel, and each target
 // averages -time_step * flow over its sources in source raster order (the reference's loop order).  The fixed order
@@ -11,7 +13,7 @@
 #include <cub/device/device_scan.cuh>
 #include <math.h>
 
-#include "common.cuh"
+#include "resize_px.cuh"
 
 namespace rb {
 namespace {
@@ -250,10 +252,63 @@ __global__ void __launch_bounds__(256) erode5_kernel(const uint8_t* __restrict__
 // the CLI's np.clip(np.rint(fl32(255 * x)), 0, 255), as rb_frame_metrics quantises: ties to even; fmaxf(NaN, 0) = 0
 __device__ __forceinline__ uint8_t quantise(float x) { return (uint8_t)fminf(fmaxf(rintf(__fmul_rn(255.f, x)), 0.f), 255.f); }
 
+// One frame of a blend as fp32 values: pixel (y, x), channel c of frame `img`, rows `row` values apart.  CropF32 reads
+// fp32 frames (the engine's padded images from the crop's first pixel, or raw frames); RawU8 reads uint8 frames and
+// scales them as rb_frames_prepare does (np.float32(u) / 255, from a table of the 256 quotients).
+struct CropF32 {
+  const float* img;
+  size_t row;
+  __device__ __forceinline__ float operator()(int y, int x, int c) const { return img[(size_t)y * row + (size_t)x * 3 + c]; }
+};
+struct RawU8 {
+  const uint8_t* img;
+  size_t row;
+  const float* lut;
+  __device__ __forceinline__ float operator()(int y, int x, int c) const {
+    return lut[img[(size_t)y * row + (size_t)x * 3 + c]];
+  }
+};
+
+// The blend of one output pixel (x, y) of an H x W frame: both frames sampled at p + F_k (clamped to the frame; NaN ->
+// 0) with the bilinear arithmetic of rb_flow_fb_check, blended by (1-t, t) with empty targets weighted 0; written to
+// out[p] as fp32, or quantised to uint8 (with bgr: channels reversed).
+template <class Frame>
+__device__ __forceinline__ void synthesize_px(const Frame& i0, const Frame& i1, int x, int y, int H, int W, float2 F0,
+                                              float2 F1, bool empty0, bool empty1, float t, void* out, size_t p,
+                                              int out_u8, int bgr) {
+  const float s = __fsub_rn(1.f, t);
+  float w0 = empty0 ? 0.f : s, w1 = empty1 ? 0.f : t;
+  if (w0 == 0.f && w1 == 0.f) w0 = s, w1 = t;
+  float v[2][3];
+  for (int k = 0; k < 2; ++k) {
+    const float2 F = k == 0 ? F0 : F1;
+    const Frame& img = k == 0 ? i0 : i1;
+    const float qx = fminf(fmaxf(__fadd_rn((float)x, F.x), 0.f), (float)(W - 1));
+    const float qy = fminf(fmaxf(__fadd_rn((float)y, F.y), 0.f), (float)(H - 1));
+    const int x0 = (int)floorf(qx), y0 = (int)floorf(qy);
+    const int x1 = min(x0 + 1, W - 1), y1 = min(y0 + 1, H - 1);
+    const float ax = __fsub_rn(qx, (float)x0), ay = __fsub_rn(qy, (float)y0);
+    const float cx = __fsub_rn(1.f, ax), cy = __fsub_rn(1.f, ay);
+    for (int c = 0; c < 3; ++c) {
+      const float t0 = __fadd_rn(__fmul_rn(cx, img(y0, x0, c)), __fmul_rn(ax, img(y0, x1, c)));
+      const float t1 = __fadd_rn(__fmul_rn(cx, img(y1, x0, c)), __fmul_rn(ax, img(y1, x1, c)));
+      v[k][c] = __fadd_rn(__fmul_rn(t0, cy), __fmul_rn(t1, ay));
+    }
+  }
+  const float den = __fadd_rn(w0, w1);
+  for (int c = 0; c < 3; ++c) {
+    const float o = __fdiv_rn(__fadd_rn(__fmul_rn(w0, v[0][c]), __fmul_rn(w1, v[1][c])), den);
+    const int oc = bgr ? 2 - c : c;
+    if (out_u8)
+      static_cast<uint8_t*>(out)[p * 3 + oc] = quantise(o);
+    else
+      static_cast<float*>(out)[p * 3 + oc] = o;
+  }
+}
+
 // One thread per output pixel, blockIdx.y striding over the (time, sample) pairs (32-bit pixel indices; a pair is
-// (times.v[smp / B], smp % B), or an item's (v[smp], row[smp]), Steps): both frames sampled at p + F_tk(p) (clamped to
-// the frame; NaN -> 0) with the bilinear arithmetic of rb_flow_fb_check, blended by (1-t, t) with empty targets weighted
-// 0; written as fp32, or quantised to uint8 (with bgr: channels reversed).
+// (times.v[smp / B], smp % B), or an item's (v[smp], row[smp]), Steps): synthesize_px on the crop of the padded frames
+// with the flows and masks of the same pixel.
 __global__ void __launch_bounds__(256) frame_synthesize_kernel(const float* __restrict__ frames0,
                                                                const float* __restrict__ frames1, int Hp, int Wp, int top,
                                                                int left, const float2* __restrict__ f0,
@@ -269,36 +324,53 @@ __global__ void __launch_bounds__(256) frame_synthesize_kernel(const float* __re
     const uint32_t j = smp / (uint32_t)B;
     const int b = times.items ? times.row[j] : (int)(smp % B);
     const size_t p = (size_t)smp * hw + q;
-    const float t = times.v[j];
-    const float s = __fsub_rn(1.f, t);
-    float w0 = e0[p] ? 0.f : s, w1 = e1[p] ? 0.f : t;
-    if (w0 == 0.f && w1 == 0.f) w0 = s, w1 = t;
-    float v[2][3];
-    for (int k = 0; k < 2; ++k) {
-      const float2 F = (k == 0 ? f0 : f1)[p];
-      const float qx = fminf(fmaxf(__fadd_rn((float)x, F.x), 0.f), (float)(W - 1));
-      const float qy = fminf(fmaxf(__fadd_rn((float)y, F.y), 0.f), (float)(H - 1));
-      const int x0 = (int)floorf(qx), y0 = (int)floorf(qy);
-      const int x1 = min(x0 + 1, W - 1), y1 = min(y0 + 1, H - 1);
-      const float ax = __fsub_rn(qx, (float)x0), ay = __fsub_rn(qy, (float)y0);
-      const float cx = __fsub_rn(1.f, ax), cy = __fsub_rn(1.f, ay);
-      const float* img = (k == 0 ? frames0 : frames1) + ((size_t)b * Hp + top) * Wp * 3 + (size_t)left * 3;
-      const float* r0 = img + (size_t)y0 * Wp * 3;
-      const float* r1 = img + (size_t)y1 * Wp * 3;
-      for (int c = 0; c < 3; ++c) {
-        const float t0 = __fadd_rn(__fmul_rn(cx, r0[x0 * 3 + c]), __fmul_rn(ax, r0[x1 * 3 + c]));
-        const float t1 = __fadd_rn(__fmul_rn(cx, r1[x0 * 3 + c]), __fmul_rn(ax, r1[x1 * 3 + c]));
-        v[k][c] = __fadd_rn(__fmul_rn(t0, cy), __fmul_rn(t1, ay));
-      }
-    }
-    const float den = __fadd_rn(w0, w1);
-    for (int c = 0; c < 3; ++c) {
-      const float o = __fdiv_rn(__fadd_rn(__fmul_rn(w0, v[0][c]), __fmul_rn(w1, v[1][c])), den);
-      const int oc = bgr ? 2 - c : c;
-      if (out_u8)
-        static_cast<uint8_t*>(out)[p * 3 + oc] = quantise(o);
-      else
-        static_cast<float*>(out)[p * 3 + oc] = o;
+    const size_t crop = ((size_t)b * Hp + top) * Wp * 3 + (size_t)left * 3;
+    const CropF32 i0{frames0 + crop, (size_t)Wp * 3}, i1{frames1 + crop, (size_t)Wp * 3};
+    synthesize_px(i0, i1, x, y, H, W, f0[p], f1[p], e0[p] != 0, e1[p] != 0, times.v[j], out, p, out_u8, bgr);
+  }
+}
+
+// The blend at the frames' own Hs x Ws from flows and masks at the network's H x W: one thread per output pixel,
+// blockIdx.y striding over the (time, sample) pairs as in frame_synthesize_kernel.  Per pixel, F_k is rb_flow_resize's
+// value there (resize_f32_px of the sample's low-resolution flow, then u *= su, v *= sv) and the empty mask that of the
+// network pixel whose area holds the pixel's centre, (((2x+1) W) div (2 Ws), ((2y+1) H) div (2 Hs)) in 64-bit integers.
+// The low-resolution reads go through the read-only path; uint8 frames are read as bytes.
+template <bool U8>
+__global__ void __launch_bounds__(256) frame_synthesize_resized_kernel(
+    const void* __restrict__ frames0, const void* __restrict__ frames1, int Hs, int Ws, const float* __restrict__ f0,
+    const float* __restrict__ f1, const uint8_t* __restrict__ e0, const uint8_t* __restrict__ e1, int H, int W,
+    int mode, float su, float sv, Steps times, void* out, int out_u8, int bgr, int n_t, int B) {
+  __shared__ float lut[256];
+  if (U8) {
+    for (int i = threadIdx.x; i < 256; i += blockDim.x) lut[i] = __fdiv_rn((float)i, 255.0f);
+    __syncthreads();
+  }
+  const uint32_t q = blockIdx.x * blockDim.x + threadIdx.x;
+  const uint32_t hw = (uint32_t)Hs * (uint32_t)Ws;
+  if (q >= hw) return;
+  const int x = (int)(q % (uint32_t)Ws), y = (int)(q / (uint32_t)Ws);
+  const size_t lhw = (size_t)H * W;
+  const size_t near = (size_t)(((2 * (uint64_t)y + 1) * (uint64_t)H) / (2 * (uint64_t)Hs)) * W +
+                      (size_t)(((2 * (uint64_t)x + 1) * (uint64_t)W) / (2 * (uint64_t)Ws));
+  const size_t frame = (size_t)hw * 3;
+  for (uint32_t smp = blockIdx.y; smp < (uint32_t)n_t * B; smp += gridDim.y) {
+    const uint32_t j = smp / (uint32_t)B;
+    const int b = times.items ? times.row[j] : (int)(smp % B);
+    const size_t p = (size_t)smp * hw + q;
+    float a[2], c[2];
+    resize_f32_px<2>(f0 + (size_t)smp * lhw * 2, H, W, Hs, Ws, y, x, mode, a);
+    resize_f32_px<2>(f1 + (size_t)smp * lhw * 2, H, W, Hs, Ws, y, x, mode, c);
+    const float2 F0 = make_float2(__fmul_rn(a[0], su), __fmul_rn(a[1], sv));
+    const float2 F1 = make_float2(__fmul_rn(c[0], su), __fmul_rn(c[1], sv));
+    const bool m0 = __ldg(e0 + (size_t)smp * lhw + near) != 0, m1 = __ldg(e1 + (size_t)smp * lhw + near) != 0;
+    if (U8) {
+      const RawU8 i0{static_cast<const uint8_t*>(frames0) + b * frame, (size_t)Ws * 3, lut};
+      const RawU8 i1{static_cast<const uint8_t*>(frames1) + b * frame, (size_t)Ws * 3, lut};
+      synthesize_px(i0, i1, x, y, Hs, Ws, F0, F1, m0, m1, times.v[j], out, p, out_u8, bgr);
+    } else {
+      const CropF32 i0{static_cast<const float*>(frames0) + b * frame, (size_t)Ws * 3};
+      const CropF32 i1{static_cast<const float*>(frames1) + b * frame, (size_t)Ws * 3};
+      synthesize_px(i0, i1, x, y, Hs, Ws, F0, F1, m0, m1, times.v[j], out, p, out_u8, bgr);
     }
   }
 }
@@ -533,4 +605,84 @@ extern "C" int rb_frame_synthesize(const float* frames, int Hp, int Wp, int top,
   const size_t frame1 = B > 0 && Hp > 0 && Wp > 0 ? (size_t)B * Hp * Wp * 3 : 0;
   return rb_frame_synthesize_pairs(frames, frames == nullptr ? nullptr : frames + frame1, Hp, Wp, top, left, flow_t0,
                                    flow_t1, empty0, empty1, &t, 1, out, 0, 0, B, H, W, stream);
+}
+
+namespace {
+
+// The resized blend entries after their pointer, count, flag and time checks: the shapes, the item rows against the B
+// frame pairs, then one launch over n_t times x B pairs, or over the n_t items (launched with B = 1)
+int synthesize_resized_run(const char* fn, const void* frames0, const void* frames1, int frames_u8, int Hs, int Ws,
+                           const float* flow_t0, const float* flow_t1, const uint8_t* empty0, const uint8_t* empty1,
+                           int H, int W, const Steps& times, int n_t, void* out, int out_u8, int bgr, int B,
+                           void* stream) {
+  RB_REQUIRE(B > 0 && H > 0 && W > 0 && Hs > 0 && Ws > 0, RB_ERR_BAD_SHAPE, "%s: bad shape B=%d H=%d W=%d Hs=%d Ws=%d",
+             fn, B, H, W, Hs, Ws);
+  for (int i = 0; times.items && i < n_t; ++i)
+    RB_REQUIRE(times.row[i] >= 0 && times.row[i] < B, RB_ERR_BAD_ARG, "%s: item_sample[%d] = %d outside [0, %d)", fn, i,
+               times.row[i], B);
+  const size_t hw = (size_t)Hs * Ws;
+  const int rows = times.items ? 1 : B;
+  RB_REQUIRE(hw < (size_t(1) << 32) && (size_t)n_t * rows < (size_t(1) << 32), RB_ERR_BAD_SHAPE,
+             "%s: %zu pixels per frame or %zu frames exceed 32-bit indices", fn, hw, (size_t)n_t * rows);
+  const dim3 grid((unsigned)((hw + 255) / 256), (unsigned)std::min<size_t>((size_t)n_t * rows, 65535));
+  const int mode = float_mode(H, W, Hs, Ws);
+  const float su = flow_scale_u(W, Ws), sv = flow_scale_v(H, Hs);
+  const cudaStream_t st = (cudaStream_t)stream;
+  if (frames_u8)
+    frame_synthesize_resized_kernel<true><<<grid, 256, 0, st>>>(frames0, frames1, Hs, Ws, flow_t0, flow_t1, empty0,
+                                                                empty1, H, W, mode, su, sv, times, out, out_u8, bgr, n_t,
+                                                                rows);
+  else
+    frame_synthesize_resized_kernel<false><<<grid, 256, 0, st>>>(frames0, frames1, Hs, Ws, flow_t0, flow_t1, empty0,
+                                                                 empty1, H, W, mode, su, sv, times, out, out_u8, bgr,
+                                                                 n_t, rows);
+  RB_CHECK_LAUNCH("frame_synthesize_resized_kernel");
+  return RB_OK;
+}
+
+}  // namespace
+
+extern "C" int rb_frame_synthesize_pairs_resized(const void* frames0, const void* frames1, int frames_u8, int Hs, int Ws,
+                                                 const float* flow_t0, const float* flow_t1, const uint8_t* empty0,
+                                                 const uint8_t* empty1, int H, int W, const float* ts, int n_t,
+                                                 void* out, int out_u8, int bgr, int B, void* stream) {
+  RB_REQUIRE(frames0 && frames1 && flow_t0 && flow_t1 && empty0 && empty1 && ts && out, RB_ERR_BAD_ARG,
+             "rb_frame_synthesize_pairs_resized: null pointer");
+  RB_REQUIRE(n_t > 0 && n_t <= kMaxSteps, RB_ERR_BAD_ARG, "rb_frame_synthesize_pairs_resized: %d times (1..%d)", n_t,
+             kMaxSteps);
+  RB_REQUIRE((frames_u8 == 0 || frames_u8 == 1) && (out_u8 == 0 || out_u8 == 1) && (bgr == 0 || bgr == 1),
+             RB_ERR_BAD_ARG, "rb_frame_synthesize_pairs_resized: frames_u8, out_u8 and bgr must be 0 or 1 (got %d, %d, %d)",
+             frames_u8, out_u8, bgr);
+  Steps times{};
+  for (int i = 0; i < n_t; ++i) {
+    RB_REQUIRE(ts[i] >= 0.f && ts[i] <= 1.f, RB_ERR_BAD_ARG,
+               "rb_frame_synthesize_pairs_resized: ts[%d] must be in [0, 1] (got %g)", i, (double)ts[i]);
+    times.v[i] = ts[i];
+  }
+  return synthesize_resized_run("rb_frame_synthesize_pairs_resized", frames0, frames1, frames_u8, Hs, Ws, flow_t0,
+                                flow_t1, empty0, empty1, H, W, times, n_t, out, out_u8, bgr, B, stream);
+}
+
+extern "C" int rb_frame_synthesize_items_resized(const void* frames0, const void* frames1, int frames_u8, int Hs, int Ws,
+                                                 const float* flow_t0, const float* flow_t1, const uint8_t* empty0,
+                                                 const uint8_t* empty1, int H, int W, const int32_t* item_sample,
+                                                 const float* item_t, int n_items, void* out, int out_u8, int bgr, int B,
+                                                 void* stream) {
+  RB_REQUIRE(frames0 && frames1 && flow_t0 && flow_t1 && empty0 && empty1 && item_sample && item_t && out,
+             RB_ERR_BAD_ARG, "rb_frame_synthesize_items_resized: null pointer");
+  RB_REQUIRE(n_items > 0 && n_items <= kMaxSteps, RB_ERR_BAD_ARG, "rb_frame_synthesize_items_resized: %d items (1..%d)",
+             n_items, kMaxSteps);
+  RB_REQUIRE((frames_u8 == 0 || frames_u8 == 1) && (out_u8 == 0 || out_u8 == 1) && (bgr == 0 || bgr == 1),
+             RB_ERR_BAD_ARG, "rb_frame_synthesize_items_resized: frames_u8, out_u8 and bgr must be 0 or 1 (got %d, %d, %d)",
+             frames_u8, out_u8, bgr);
+  Steps times{};
+  times.items = 1;
+  for (int i = 0; i < n_items; ++i) {
+    RB_REQUIRE(item_t[i] >= 0.f && item_t[i] <= 1.f, RB_ERR_BAD_ARG,
+               "rb_frame_synthesize_items_resized: item_t[%d] must be in [0, 1] (got %g)", i, (double)item_t[i]);
+    times.v[i] = item_t[i];
+    times.row[i] = item_sample[i];
+  }
+  return synthesize_resized_run("rb_frame_synthesize_items_resized", frames0, frames1, frames_u8, Hs, Ws, flow_t0,
+                                flow_t1, empty0, empty1, H, W, times, n_items, out, out_u8, bgr, B, stream);
 }

@@ -8,19 +8,9 @@
 // rounded operations, so no FMA contraction changes them).
 #include <climits>
 
-#include "common.cuh"
+#include "resize_px.cuh"
 
 namespace rb {
-
-enum { RS_COPY = 0, RS_OPENCV = 1, RS_IPP = 2 };
-
-// OpenCV's per-axis coordinate (resize.cpp, resizeGeneric): f = fl32((d + 0.5) * scale - 0.5), scale = 1 / (dst / src)
-__device__ __forceinline__ void cv_coord(int d, double scale, int& s, float& f) {
-  const float c = __double2float_rn(__dadd_rn(__dmul_rn(__dadd_rn((double)d, 0.5), scale), -0.5));
-  const float fl = floorf(c);
-  s = (int)fl;
-  f = __fsub_rn(c, fl);
-}
 
 // uint8 resize of pixel (y, x) of one channel-interleaved [H,W,C] plane; returns the 0..255 value per channel
 template <int C>
@@ -45,74 +35,6 @@ __device__ __forceinline__ void resize_u8_px(const uint8_t* __restrict__ p, int 
     const int v = (((b0 * (s0 >> 4)) >> 16) + ((b1 * (s1 >> 4)) >> 16) + 2) >> 2;
     out[c] = min(max(v, 0), 255);
   }
-}
-
-// IPP's per-axis coordinate: c = (d + 0.5) * (src / dst) - 0.5 in float64, weight fl32(c - floor(c))
-__device__ __forceinline__ void ipp_coord(int d, double scale, int src, int& i0, int& i1, float& w) {
-  const double c = __dadd_rn(__dmul_rn(__dadd_rn((double)d, 0.5), scale), -0.5);
-  const double fl = floor(c);
-  w = __double2float_rn(__dsub_rn(c, fl));
-  const int s = (int)fl;
-  i0 = min(max(s, 0), src - 1);
-  i1 = min(max(s + 1, 0), src - 1);
-}
-
-__device__ __forceinline__ float lerp_fma(float p0, float p1, float w) { return __fmaf_rn(w, __fsub_rn(p1, p0), p0); }
-
-// float32 resize of pixel (y, x) of one channel-interleaved [H,W,C] plane, as cv2 computes it (mode RS_*)
-template <int C>
-__device__ __forceinline__ void resize_f32_px(const float* __restrict__ p, int H, int W, int Ho, int Wo, int y, int x,
-                                              int mode, float out[C]) {
-  if (mode == RS_COPY) {
-#pragma unroll
-    for (int c = 0; c < C; ++c) out[c] = p[((size_t)y * W + x) * C + c];
-    return;
-  }
-  if (mode == RS_IPP) {
-    int x0, x1, y0, y1;
-    float wx, wy;
-    ipp_coord(x, (double)W / Wo, W, x0, x1, wx);
-    ipp_coord(y, (double)H / Ho, H, y0, y1, wy);
-    // IPP's border strips: a column whose taps clamping merged copies its pixel (rows likewise), but the corners run
-    // the general formula -- only visible with inf / NaN inputs, where inf - inf gives NaN
-    const bool cx = x0 == x1, cy = y0 == y1;
-    const float *r0 = p + (size_t)y0 * W * C, *r1 = p + (size_t)y1 * W * C;
-#pragma unroll
-    for (int c = 0; c < C; ++c) {
-      float h0, h1;
-      if (cx && !cy) {
-        h0 = r0[x0 * C + c];
-        h1 = r1[x0 * C + c];
-      } else {
-        h0 = lerp_fma(r0[x0 * C + c], r0[x1 * C + c], wx);
-        h1 = lerp_fma(r1[x0 * C + c], r1[x1 * C + c], wx);
-      }
-      out[c] = (cy && !cx) ? h0 : lerp_fma(h0, h1, wy);
-    }
-    return;
-  }
-  // RS_OPENCV: OpenCV's own float code (single-row or single-column sources)
-  int sx, sy;
-  float fx, fy;
-  cv_coord(x, 1.0 / ((double)Wo / W), sx, fx);
-  cv_coord(y, 1.0 / ((double)Ho / H), sy, fy);
-  if (sx < 0) { sx = 0; fx = 0.f; }
-  if (sx >= W - 1) { sx = W - 1; fx = 0.f; }
-  const bool one_tap = sx >= W - 1;  // OpenCV's xmax: from there on S[sx] alone
-  const int x0 = sx, x1 = min(sx + 1, W - 1);
-  const int y0 = min(max(sy, 0), H - 1), y1 = min(max(sy + 1, 0), H - 1);
-  const float a0 = __fsub_rn(1.f, fx), b0 = __fsub_rn(1.f, fy);
-  const float *r0 = p + (size_t)y0 * W * C, *r1 = p + (size_t)y1 * W * C;
-#pragma unroll
-  for (int c = 0; c < C; ++c) {
-    const float h0 = one_tap ? r0[x0 * C + c] : __fadd_rn(__fmul_rn(r0[x0 * C + c], a0), __fmul_rn(r0[x1 * C + c], fx));
-    const float h1 = one_tap ? r1[x0 * C + c] : __fadd_rn(__fmul_rn(r1[x0 * C + c], a0), __fmul_rn(r1[x1 * C + c], fx));
-    out[c] = __fadd_rn(__fmul_rn(h0, b0), __fmul_rn(h1, fy));
-  }
-}
-
-__host__ __device__ inline int float_mode(int H, int W, int Ho, int Wo) {
-  return (H == Ho && W == Wo) ? RS_COPY : (H == 1 || W == 1) ? RS_OPENCV : RS_IPP;
 }
 
 // dst [B,Hp,Wp,3] fp32 in [0,1]: the Ho x Wo resize of src [B,H,W,3], replicate-padded by (pad_top, pad_left, ...)
@@ -180,8 +102,7 @@ extern "C" int rb_flow_resize(const float* flow, float* dst, int B, int H, int W
              "rb_flow_resize: bad shape B=%d H=%d W=%d Ho=%d Wo=%d", B, H, W, Ho, Wo);
   RB_REQUIRE((long long)H * W * 2 <= INT_MAX && (long long)Ho * Wo * 2 <= INT_MAX, RB_ERR_BAD_SHAPE,
              "rb_flow_resize: flow too large (%d x %d -> %d x %d)", H, W, Ho, Wo);
-  // u *= dW / float(W_), v *= dH / float(H_): the float64 quotient rounded to fp32 (numpy >= 2, float32 array)
-  const float su = (float)((double)Wo / (double)W), sv = (float)((double)Ho / (double)H);
+  const float su = flow_scale_u(W, Wo), sv = flow_scale_v(H, Ho);
   const size_t n = (size_t)B * Ho * Wo;
   flow_resize_kernel<<<(unsigned)((n + 255) / 256), 256, 0, (cudaStream_t)stream>>>(flow, dst, B, H, W, Ho, Wo,
                                                                                     float_mode(H, W, Ho, Wo), su, sv);

@@ -59,6 +59,13 @@ the frame interpolated at time s - floor(s) between frames floor(s) and floor(s)
 GPU (one minus the intersection of the frames' colour histograms, in [0, 1]); a pair above THRESH is a scene cut.  There
 interpolated frames are copies of the nearer input frame, and warm-started flow restarts cold.  The run prints
 ``scene cuts: <count> at pairs <k> ...``.  No default: pick the threshold for the footage.
+
+--native-frames (with --interpolate, or --path with --interpolate or --input-fps/--fps) writes the interpolated frames,
+and with --path the copied input frames, at the input's own size: the flow is estimated and reversed at the network size,
+then resized inside the blend, which warps the decoded frames.  --flow-size H W sets that network size in place of
+432x1024 wherever the CLI resizes (e.g. --flow-size 544 960 keeps 16:9 footage's aspect ratio):
+
+    python infer_raft.py --path film/ --out tv/ --input-fps 24 --fps 60 --native-frames --flow-size 544 960 --load ...
 """
 import glob
 import argparse
@@ -147,6 +154,11 @@ def parser():
                         'where interpolation copies the nearer frame and warm-started flow restarts cold')
     p.add_argument('--native-flow', action='store_true',
                    help="extension: resize the written flow(s) back to im1's size (flow_utils.resize_flow)")
+    p.add_argument('--native-frames', action='store_true',
+                   help="extension, with --interpolate or --path --input-fps/--fps: write the interpolated (and, with "
+                        "--path, the copied input) frames at the input's own size, from flow estimated at the network size")
+    p.add_argument('--flow-size', type=int, nargs=2, default=None, metavar=('H', 'W'),
+                   help='extension: the network size frames are resized to, in place of 432x1024 (test mode and --path)')
     p.add_argument('--upstream', action='store_true',
                    help='extension: weights converted from an official princeton-vl RAFT .pth (raft_b200.convert): RGB '
                         'frames and the upstream numerics (RAFT(..., upstream=True))')
@@ -173,6 +185,23 @@ def main(argv=None):
         fps = (_rate(p, '--input-fps', args.input_fps), _rate(p, '--fps', args.fps))
         if fps[1] <= fps[0]:
             p.error(f'--fps {args.fps} must exceed --input-fps {args.input_fps}: frame-rate conversion goes up only')
+    if args.native_frames:
+        if args.keep_size:
+            p.error('--native-frames resizes the flow of a smaller network size to the frames; with --keep-size the '
+                    'network already runs at their size')
+        if args.mode == 'val':
+            p.error('--native-frames writes interpolated frames: it has no effect with -m val')
+        if not (args.interpolate or fps is not None):
+            p.error('--native-frames needs an interpolation mode: --interpolate, or --path with --input-fps/--fps')
+    if args.flow_size is not None:
+        if args.keep_size:
+            p.error('--flow-size sets the size frames are resized to; --keep-size runs them at their own size')
+        if args.mode == 'val':
+            p.error('--flow-size: -m val runs the validation protocol at the datasets\' own sizes')
+        least = 121 if args.upstream else 57
+        if min(args.flow_size) < least:
+            p.error(f'--flow-size {args.flow_size[0]} {args.flow_size[1]}: each side must be at least {least} (the '
+                    f'4-level correlation pyramid{" of --upstream" if args.upstream else ""})')
     if args.interpolate and not all(0.0 <= t <= 1.0 for t in args.interpolate):
         p.error('--interpolate: every T must be in [0, 1]')
     if args.scene_cut is not None:
@@ -232,12 +261,16 @@ def main(argv=None):
         left, right = read_pair(args.im1, args.im2, None, rgb)
         model = RAFT.RAFT(left.shape[1:], args, iters=args.iters, upstream=args.upstream,
                           mixed_precision=args.mixed_precision).load(args.load)
-    else:  # the reference's 432x1024 (infer_raft.py:69,76), resized and scaled on the GPU
+    else:  # the reference's 432x1024 (infer_raft.py:69,76) or --flow-size, resized and scaled on the GPU
+        size = _flow_size(args)
         left, right = decode_pair(args.im1, args.im2, rgb)
         native = left.shape[1:3]
         if left.shape != right.shape:  # one engine pass takes one frame size: resize such a pair on the host, as before
-            left, right = read_pair(args.im1, args.im2, (432, 1024), rgb)
-        model = RAFT.RAFT((432, 1024, 3), args, iters=args.iters, input_size=(432, 1024),
+            if args.native_frames:
+                p.error(f'--native-frames: {args.im1} is {left.shape[1]}x{left.shape[2]} and {args.im2} '
+                               f'{right.shape[1]}x{right.shape[2]}; frames at their own size need one size')
+            left, right = read_pair(args.im1, args.im2, size, rgb)
+        model = RAFT.RAFT(size + (3,), args, iters=args.iters, input_size=size,
                           upstream=args.upstream, mixed_precision=args.mixed_precision).load(args.load)
     if args.bidirectional:
         flow, flow_bw, occ_fw, occ_bw = (t.cpu().numpy() for t in model.forward_bidirectional(left, right))
@@ -264,7 +297,7 @@ def main(argv=None):
         if args.flo:
             write_flo(_bw_path(args.flo), flow_bw[0])
     if args.interpolate:
-        frames = model.interpolate(left, right, args.interpolate).cpu().numpy()
+        frames = model.interpolate(left, right, args.interpolate, native=args.native_frames).cpu().numpy()
         for k, frame in enumerate(frames):
             img = np.clip(np.rint(255.0 * frame[0]), 0, 255).astype(np.uint8)
             cv2.imwrite(f"raft_interp_{k}.png", cv2.cvtColor(img, cv2.COLOR_RGB2BGR) if rgb else img)
@@ -272,11 +305,12 @@ def main(argv=None):
 
 
 def run_video(args):
-    """--path: raft_b200.video over the frames of --path, at 432x1024 like test mode (or their own size with --keep-size)."""
+    """--path: raft_b200.video over the frames of --path, at 432x1024 (or --flow-size) like test mode (or their own size
+    with --keep-size)."""
     from networks import RAFT
     from raft_b200.video import video
     iters = 20 if args.iters is None else args.iters
-    size = None if args.keep_size else (432, 1024)
+    size = None if args.keep_size else _flow_size(args)
     model = RAFT.RAFT(None if size is None else size + (3,), args, iters=iters, input_size=size, upstream=args.upstream,
                       mixed_precision=args.mixed_precision).load(args.load)
     files = video(model, args.path, args.out, batch=args.batch, workers=args.workers, warm_start=args.warm_start,
@@ -290,19 +324,25 @@ def run_video(args):
 
 def run_video_interpolate(args, fps=None):
     """--path --interpolate, or --path --input-fps --fps (fps = the two rates): raft_b200.video.video_interpolate over the
-    frames of --path, at 432x1024 like test mode (or their own size with --keep-size)."""
+    frames of --path, at 432x1024 (or --flow-size) like test mode (or their own size with --keep-size); --native-frames
+    writes the frames at their own size."""
     from networks import RAFT
     from raft_b200.video import video_interpolate
     iters = 20 if args.iters is None else args.iters
-    size = None if args.keep_size else (432, 1024)
+    size = None if args.keep_size else _flow_size(args)
     model = RAFT.RAFT(None if size is None else size + (3,), args, iters=iters, input_size=size, upstream=args.upstream,
                       mixed_precision=args.mixed_precision).load(args.load)
     files = video_interpolate(model, args.path, args.out, args.interpolate, batch=args.batch, workers=args.workers,
-                              fps=fps, scene_cut=args.scene_cut)
+                              fps=fps, scene_cut=args.scene_cut, native=args.native_frames)
     if args.scene_cut is not None:
         files = _print_cuts(*files)
     print(f"{len(files)} frames written under {args.out}")
     return 0
+
+
+def _flow_size(args):
+    """The network size of test mode and --path: --flow-size H W, or the reference's 432x1024."""
+    return (432, 1024) if args.flow_size is None else tuple(args.flow_size)
 
 
 def _print_cuts(files, cuts):

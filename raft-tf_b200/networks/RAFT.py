@@ -158,38 +158,45 @@ class RAFT(object):
         return tuple(None if t is None else t.clone() for t in out)
 
     @torch.no_grad()
-    def interpolate_sequence(self, frames, t=0.5, uint8=False, bgr=False):
+    def interpolate_sequence(self, frames, t=0.5, uint8=False, bgr=False, native=False):
         """Extension (frame-rate up-conversion): the frames at time t (a float, or a sequence of times, each in [0, 1])
         between every pair of consecutive frames of [T+1,H,W,3] frames, from one ``forward_sequence_bidirectional`` pass.
         A float t gives a fresh [T,H,W,3] tensor, a sequence of n times [n,T,H,W,3]; pair k equals
         ``interpolate(frames[k:k+1], frames[k+1:k+2], t)`` bit for bit.  fp32 in [0,1] by default; uint8=True quantises
         on the GPU exactly as infer_raft.py writes PNGs (np.clip(np.rint(255 x), 0, 255)), and bgr=True (with uint8)
-        reverses the channels, for RGB frames written by cv2.  A t outside [0, 1] raises ValueError."""
+        reverses the channels, for RGB frames written by cv2.  native as for ``interpolate``.  A t outside [0, 1] raises
+        ValueError."""
         scalar = np.ndim(t) == 0
-        out = self.engine().interpolate_sequence(_as_tensor(frames), [t] if scalar else list(t), uint8=uint8, bgr=bgr)
+        out = self.engine().interpolate_sequence(_as_tensor(frames), [t] if scalar else list(t), uint8=uint8, bgr=bgr,
+                                                 native=native)
         return out[0] if scalar else out
 
     @torch.no_grad()
-    def interpolate_sequence_at(self, frames, items, uint8=False, bgr=False):
+    def interpolate_sequence_at(self, frames, items, uint8=False, bgr=False, native=False):
         """Extension (frame-rate conversion to any rate): the frames at per-pair times of [T+1,H,W,3] frames (dtypes and
         sources as for ``forward``).  items is a list of (k, t) with 0 <= k < T and t in [0, 1], each the frame at time t
         between frames k and k + 1; one ``forward_sequence_bidirectional`` pass, then only the work of the listed items.
         Returns a fresh [len(items),H,W,3] tensor whose row i equals ``interpolate(frames[k:k+1], frames[k+1:k+2], t)[0]``
-        bit for bit.  uint8 and bgr as for ``interpolate_sequence``.  An empty list, a k outside [0, T) or a t outside
-        [0, 1] raises ValueError."""
-        return self.engine().interpolate_sequence_at(_as_tensor(frames), items, uint8=uint8, bgr=bgr)
+        bit for bit.  uint8 and bgr as for ``interpolate_sequence``, native as for ``interpolate``.  An empty list, a k
+        outside [0, T) or a t outside [0, 1] raises ValueError."""
+        return self.engine().interpolate_sequence_at(_as_tensor(frames), items, uint8=uint8, bgr=bgr, native=native)
 
     @torch.no_grad()
-    def interpolate(self, input_left, input_right, t=0.5):
+    def interpolate(self, input_left, input_right, t=0.5, native=False):
         """Extension (the reference computes the flow for frame interpolation and projects it to time t with
         flow_utils.py:166 on the CPU): the frames at time t between left (t = 0) and right (t = 1).  One bidirectional
         pass, then per t the flows from time t to both frames by the reference's flow reversal (rb_flow_reverse, bit for
         bit) and a blend of both frames warped by them (rb_frame_synthesize; a frame whose reversed flow is empty at a
         pixel gets weight 0 there).  Inputs as for ``forward``.  A float t in [0, 1] gives a fresh [B,H,W,3] fp32 tensor,
         BGR in [0,1] (uint8 frames are divided by 255); a sequence of T times gives [T,B,H,W,3] from one pass.  t = 0
-        and t = 1 return the frames themselves exactly.  A t outside [0, 1] raises ValueError."""
+        and t = 1 return the frames themselves exactly.  A t outside [0, 1] raises ValueError.
+
+        native=True (with input_size) returns the frames at the inputs' own size rather than input_size: the flow is
+        estimated and reversed at input_size as always, then resized to the frames' size inside the blend, which warps
+        the frames as given (not their resized copies).  Without input_size it changes nothing."""
         scalar = np.ndim(t) == 0
-        out = self.engine().interpolate(_as_tensor(input_left), _as_tensor(input_right), [t] if scalar else list(t))
+        out = self.engine().interpolate(_as_tensor(input_left), _as_tensor(input_right), [t] if scalar else list(t),
+                                        native=native)
         return out[0] if scalar else out
 
 

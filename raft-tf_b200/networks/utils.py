@@ -1,5 +1,7 @@
 """Drop-in mirror of the reference's ``networks/utils.py`` on torch CUDA tensors; every function
 runs a raft_b200 CUDA kernel through the C ABI (no TF, no CPU fallback).  NHWC like the reference."""
+import ctypes
+
 import torch
 
 from raft_b200 import capi
@@ -226,6 +228,35 @@ def synthesize(frame0, frame1, flow_t0, flow_t1, empty0, empty1, t):
         capi.check(capi.lib.rb_frame_synthesize(capi.ptr(frames), H, W, 0, 0, capi.ptr(f0), capi.ptr(f1), capi.ptr(e0),
                                                 capi.ptr(e1), t, capi.ptr(out), B, H, W, capi.stream()))
     return out
+
+
+def synthesize_resized(frame0, frame1, flow_t0, flow_t1, empty0, empty1, t, uint8=False, bgr=False):
+    """Extension: synthesize at the frames' own size from flows at the network size (rb_frame_synthesize_pairs_resized).
+    frame0, frame1: [B,Hs,Ws,3] CUDA frames, uint8 (divided by 255 like rb_frames_prepare) or fp32; flow_t0, flow_t1
+    [B,H,W,2] and empty0, empty1 [B,H,W] at the network size (e.g. reverse_flow of the flows the network estimated).
+    Each flow is resized to Hs x Ws as resize_flow does and each mask taken at the network pixel that holds the output
+    pixel's centre, then blended as synthesize does, bit for bit, without those Hs x Ws intermediates.  -> [B,Hs,Ws,3]
+    fp32, or with uint8 quantised as infer_raft.py writes PNGs (bgr: channels reversed)."""
+    t = float(t)
+    if not 0.0 <= t <= 1.0:
+        raise ValueError(f"synthesize_resized: t must be in [0, 1] (got {t})")
+    if bgr and not uint8:
+        raise ValueError("synthesize_resized: bgr swaps the channels of uint8 output; pass uint8=True")
+    assert frame0.shape == frame1.shape and frame0.dim() == 4 and frame0.shape[-1] == 3, (frame0.shape, frame1.shape)
+    assert frame0.dtype == frame1.dtype and frame0.dtype in (torch.uint8, torch.float32), (frame0.dtype, frame1.dtype)
+    B, Hs, Ws, _ = frame0.shape
+    H, W = flow_t0.shape[1:3]
+    assert flow_t0.shape == flow_t1.shape == (B, H, W, 2) and empty0.shape == empty1.shape == (B, H, W)
+    i0, i1 = frame0.contiguous(), frame1.contiguous()
+    f0, f1 = flow_t0.contiguous().float(), flow_t1.contiguous().float()
+    e0, e1 = empty0.contiguous().to(torch.uint8), empty1.contiguous().to(torch.uint8)
+    out = torch.empty(1, B, Hs, Ws, 3, dtype=torch.uint8 if uint8 else torch.float32, device=i0.device)
+    ts = (ctypes.c_float * 1)(t)
+    with torch.cuda.device(out.device):
+        capi.check(capi.lib.rb_frame_synthesize_pairs_resized(
+            capi.ptr(i0), capi.ptr(i1), int(i0.dtype == torch.uint8), Hs, Ws, capi.ptr(f0), capi.ptr(f1), capi.ptr(e0),
+            capi.ptr(e1), H, W, ts, 1, capi.ptr(out), int(uint8), int(bgr), B, capi.stream()))
+    return out[0]
 
 
 def resize_frames(frames, size, pad=(0, 0, 0, 0)):

@@ -80,6 +80,10 @@ SIGNATURES = {
     "rb_flow_reverse_items": (_i, [_vp, _i, _vp, _vp, _i, _vp, _vp, _vp, _i, _i, _vp, _sz, _vp]),
     "rb_frame_synthesize_items": (_i, [_vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _i, _vp, _i, _i, _i, _i,
                                        _i, _vp]),
+    "rb_frame_synthesize_pairs_resized": (_i, [_vp, _vp, _i, _i, _i, _vp, _vp, _vp, _vp, _i, _i, _vp, _i, _vp, _i, _i,
+                                               _i, _vp]),
+    "rb_frame_synthesize_items_resized": (_i, [_vp, _vp, _i, _i, _i, _vp, _vp, _vp, _vp, _i, _i, _vp, _vp, _i, _vp, _i,
+                                               _i, _i, _vp]),
     "rb_flow_metrics_workspace_bytes": (_i, [_i, _i, _i, _psz]),
     "rb_flow_metrics": (_i, [_vp, _f, _vp, _vp, _i, _i, _i, _vp, _vp, _vp, _sz, _vp]),
     "rb_frame_metrics_workspace_bytes": (_i, [_i, _i, _i, _psz]),

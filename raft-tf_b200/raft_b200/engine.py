@@ -19,7 +19,9 @@ fmap2 = fmaps[1:] overlap as in SEQUENCE, fnet and cnet run once per frame and t
 work of per-pair times, each (pair, t) item reversed and blended on its own (rb_flow_reverse_items,
 rb_frame_synthesize_items).
 With input_size set, every mode first resizes the frames to that size like the reference's cv2.resize (rb_frames_resize,
-csrc/resize.cu, in the graph in place of rb_frames_prepare), and its outputs come back at that size.
+csrc/resize.cu, in the graph in place of rb_frames_prepare), and its outputs come back at that size -- except the frames
+of interpolate* with native=True, blended at the frames' own size from the reversed flows at the network size
+(rb_frame_synthesize_pairs_resized / _items_resized).
 """
 from __future__ import annotations
 
@@ -501,60 +503,83 @@ class RaftEngine:
         return self.flow_up[:T], self.flow_bw, self.occ[:T], self.occ[T:]
 
     @torch.no_grad()
-    def interpolate(self, left: torch.Tensor, right: torch.Tensor, ts) -> torch.Tensor:
+    def interpolate(self, left: torch.Tensor, right: torch.Tensor, ts, native: bool = False) -> torch.Tensor:
         """Frames at times ts (each in [0, 1]; 0 = left, 1 = right) between B frame pairs: one bidirectional pass (as
         forward_bidirectional(check=False), from a graph of its own), then eagerly on the same stream, for as many times
         at once as REVERSE_WS_BOUND allows, rb_flow_reverse_multi(flow_fw, t) -> flow and empty mask from t to left,
         rb_flow_reverse_multi(flow_bw, 1 - t) -> from t to right, and rb_frame_synthesize_pairs on the padded frames the
         pass used.  raft-small's reference flow is in 1/8-resolution units, so its time steps are 8t and 8(1 - t) (exact:
         scaling by 8 commutes with fp32 rounding); upstream, t.  Frames as for forward().  Returns a fresh [T,B,H,W,3] fp32
-        tensor, BGR in [0,1] (uint8 frames are divided by 255 first)."""
+        tensor, BGR in [0,1] (uint8 frames are divided by 255 first).
+
+        native=True with input_size set blends the frames at their own size Hs x Ws instead of the resized ones the
+        network saw: the reversal is unchanged, then rb_frame_synthesize_pairs_resized resizes each reversed flow to
+        Hs x Ws (rb_flow_resize's bits), picks each empty mask at the network pixel holding the output pixel's centre and
+        blends the raw frames, into [T,B,Hs,Ws,3].  Without input_size the frames already run at their own size and
+        native changes nothing."""
         ts = _times(ts)
         self._run_frames(left, right, INTERPOLATE)
         B = self._shape[0]
-        return self._synthesize(self.flow_up[:B], self.flow_up[B:], self.images[:B], self.images[B:], ts)
+        raw = self._native_frames(native, slice(None, B), slice(B, None))
+        return self._synthesize(self.flow_up[:B], self.flow_up[B:], self.images[:B], self.images[B:], ts, raw=raw)
 
     @torch.no_grad()
-    def interpolate_sequence(self, frames: torch.Tensor, ts, uint8: bool = False, bgr: bool = False) -> torch.Tensor:
+    def interpolate_sequence(self, frames: torch.Tensor, ts, uint8: bool = False, bgr: bool = False,
+                             native: bool = False) -> torch.Tensor:
         """Frame-rate up-conversion: the frames at times ts (each in [0, 1]) between every pair of consecutive frames of
         [T+1,H,W,3] frames, from one forward_sequence_bidirectional(check=False) pass and the per-t work of interpolate
         on its flows.  Returns a fresh [len(ts),T,H,W,3] tensor; [:, k] equals interpolate(f_k, f_(k+1), ts)[:, 0] bit for
         bit.  uint8=True quantises on the GPU as the CLI writes its PNGs (np.clip(np.rint(255 x), 0, 255), NaN -> 0), and
-        bgr=True then reverses the channels (RGB frames of an upstream model written as BGR)."""
+        bgr=True then reverses the channels (RGB frames of an upstream model written as BGR).  native as for interpolate:
+        [len(ts),T,Hs,Ws,3] at the frames' own size."""
         ts = _times(ts)
         if bgr and not uint8:
             raise ValueError("raft_b200: bgr swaps the channels of uint8 output; pass uint8=True")
         self._run_sequence(frames)
         T = self._shape[0]
-        return self._synthesize(self.flow_up[:T], self.flow_bw, self.images[:T], self.images[1:], ts, uint8, bgr)
+        raw = self._native_frames(native, slice(None, T), slice(1, None))
+        return self._synthesize(self.flow_up[:T], self.flow_bw, self.images[:T], self.images[1:], ts, uint8, bgr, raw=raw)
 
     @torch.no_grad()
-    def interpolate_sequence_at(self, frames: torch.Tensor, items, uint8: bool = False, bgr: bool = False) -> torch.Tensor:
+    def interpolate_sequence_at(self, frames: torch.Tensor, items, uint8: bool = False, bgr: bool = False,
+                                native: bool = False) -> torch.Tensor:
         """Frame-rate conversion: the frames at per-pair times of [T+1,H,W,3] frames.  items is a list of (k, t), 0 <= k < T
         and t in [0, 1]: the frame at time t between frames k and k + 1.  One forward_sequence_bidirectional(check=False)
         pass, then per item only that item's work: rb_flow_reverse_items of flow_fw[k] by s t and of flow_bw[k] by
         s (1 - t) (s = flow_scale, as in interpolate) and rb_frame_synthesize_items, for as many items at once as
         REVERSE_WS_BOUND allows.  Returns a fresh [len(items),H,W,3] tensor; row i equals interpolate(f_k, f_(k+1), [t])[0, 0]
-        bit for bit.  uint8 and bgr as for interpolate_sequence.  An empty list, a k outside [0, T) or a t outside [0, 1]
-        raises ValueError before the pass."""
+        bit for bit.  uint8 and bgr as for interpolate_sequence, native as for interpolate ([len(items),Hs,Ws,3], through
+        rb_frame_synthesize_items_resized).  An empty list, a k outside [0, T) or a t outside [0, 1] raises ValueError
+        before the pass."""
         ks, ts = _items(items, _sequence_length(frames))
         if bgr and not uint8:
             raise ValueError("raft_b200: bgr swaps the channels of uint8 output; pass uint8=True")
         self._run_sequence(frames)
         T = self._shape[0]
-        return self._synthesize(self.flow_up[:T], self.flow_bw, self.images[:T], self.images[1:], ts, uint8, bgr, ks)
+        raw = self._native_frames(native, slice(None, T), slice(1, None))
+        return self._synthesize(self.flow_up[:T], self.flow_bw, self.images[:T], self.images[1:], ts, uint8, bgr, ks,
+                                raw=raw)
 
-    def _synthesize(self, flow_fw, flow_bw, frames0, frames1, ts, uint8=False, bgr=False, samples=None) -> torch.Tensor:
+    def _native_frames(self, native, rows0, rows1):
+        """The raw frames a native blend reads, rows rows0 and rows1 of the staging buffer at the frames' own size, or
+        None: without native, and without input_size, where the network already runs at the frames' own size (and fp32
+        frames that need no padding are not staged)."""
+        return (self.raw[rows0], self.raw[rows1]) if native and self.input_size is not None else None
+
+    def _synthesize(self, flow_fw, flow_bw, frames0, frames1, ts, uint8=False, bgr=False, samples=None,
+                    raw=None) -> torch.Tensor:
         """The per-t work of interpolate, interpolate_sequence and interpolate_sequence_at on the B pairs of the last pass:
         per chunk, one reversal per direction (steps s t and s (1 - t), s = flow_scale) and one blend of frames0[b] and
         frames1[b].  Without samples every time applies to every pair, into a fresh [len(ts),B,H,W,3] tensor; with
         samples, time ts[i] applies to pair samples[i] alone, into a fresh [len(ts),H,W,3] tensor.  A chunk is as many
         times (items) as keep the reversal workspace within REVERSE_WS_BOUND (at least one, at most RB_INTERP_MAX_STEPS);
-        each sample's bits do not depend on it."""
+        each sample's bits do not depend on it.  raw = (frames0, frames1) at the frames' own size: the blend reads them
+        instead, into [..., Hs,Ws,3]."""
         B, H, W = self._shape[:3]
         rows = B if samples is None else 1  # reversal samples per time
         lib = capi.lib
-        out = torch.empty((len(ts),) + ((B,) if samples is None else ()) + (H, W, 3),
+        size = (H, W) if raw is None else self.src_hw
+        out = torch.empty((len(ts),) + ((B,) if samples is None else ()) + size + (3,),
                           dtype=torch.uint8 if uint8 else torch.float32, device=self.device)
         chunk = min(len(ts), RB_INTERP_MAX_STEPS)
         while chunk > 1 and capi.size_query(lib.rb_flow_reverse_multi_workspace_bytes, chunk, rows, H, W) > REVERSE_WS_BOUND:
@@ -562,7 +587,7 @@ class RaftEngine:
         with torch.cuda.device(self.device):
             for i in range(0, len(ts), chunk):
                 self._reverse_and_blend(flow_fw, flow_bw, frames0, frames1, ts[i:i + chunk], out[i:i + chunk], uint8, bgr,
-                                        None if samples is None else samples[i:i + chunk])
+                                        None if samples is None else samples[i:i + chunk], raw)
         return out
 
     def _interpolate_at(self, t: float, out: torch.Tensor):
@@ -570,10 +595,12 @@ class RaftEngine:
         B = self._shape[0]
         self._reverse_and_blend(self.flow_up[:B], self.flow_up[B:], self.images[:B], self.images[B:], [t], out[None])
 
-    def _reverse_and_blend(self, flow_fw, flow_bw, frames0, frames1, ts, out, uint8=False, bgr=False, samples=None):
+    def _reverse_and_blend(self, flow_fw, flow_bw, frames0, frames1, ts, out, uint8=False, bgr=False, samples=None,
+                           raw=None):
         """One chunk: the reversal of flow_fw by s t and of flow_bw by s (1 - t) for the n = len(ts) times, then the blend
         into out -- rb_flow_reverse_multi and rb_frame_synthesize_pairs on all B pairs into out [n,B,H,W,3], or with
-        samples rb_flow_reverse_items and rb_frame_synthesize_items on pair samples[i] at ts[i] into out [n,H,W,3].  The
+        samples rb_flow_reverse_items and rb_frame_synthesize_items on pair samples[i] at ts[i] into out [n,H,W,3].  With
+        raw = (frames0, frames1) at the frames' own Hs x Ws, the *_resized blends of those into out [n,(B,)Hs,Ws,3].  The
         reversal buffers are (re)allocated for the n B (n) samples."""
         B, H, W = self._shape[:3]
         n, s, d = len(ts), self.flow_scale, self.device
@@ -595,6 +622,17 @@ class RaftEngine:
             else:
                 capi.check(lib.rb_flow_reverse_items(ptr(flow), B, _ints(samples), _floats(steps), n, *bufs, H, W,
                                                      ptr(self.rev_ws), self.rev_ws_bytes, st))
+        if raw is not None:
+            Hs, Ws = self.src_hw
+            frames = (ptr(raw[0]), ptr(raw[1]), int(raw[0].dtype == torch.uint8), Hs, Ws, ptr(self.flow_t[0]),
+                      ptr(self.flow_t[1]), ptr(self.empty_t[0, 0]), ptr(self.empty_t[0, 1]), H, W)
+            if samples is None:
+                capi.check(lib.rb_frame_synthesize_pairs_resized(*frames, _floats(ts), n, ptr(out), int(uint8), int(bgr),
+                                                                 B, st))
+            else:
+                capi.check(lib.rb_frame_synthesize_items_resized(*frames, _ints(samples), _floats(ts), n, ptr(out),
+                                                                 int(uint8), int(bgr), B, st))
+            return
         frames = (ptr(frames0), ptr(frames1), self.Hp, self.Wp, self.pad[0], self.pad[2], ptr(self.flow_t[0]),
                   ptr(self.flow_t[1]), ptr(self.empty_t[0, 0]), ptr(self.empty_t[0, 1]))
         if samples is None:

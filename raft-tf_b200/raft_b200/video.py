@@ -343,7 +343,7 @@ def video(model, frames, out, batch=8, workers=4, warm_start=False, flo=None, np
     return written if thr is None else (written, cuts)
 
 
-def video_interpolate(model, frames, out, ts=None, batch=8, workers=4, fps=None, scene_cut=None):
+def video_interpolate(model, frames, out, ts=None, batch=8, workers=4, fps=None, scene_cut=None, native=False):
     """Frame-rate up-conversion with a loaded networks.RAFT.RAFT model of the frames (a directory's sorted *.png / *.jpg,
     or a list of paths, all of one size), written as one numbered sequence <out>/frame_<n:06d>.png.  Give exactly one of:
 
@@ -358,6 +358,11 @@ def video_interpolate(model, frames, out, ts=None, batch=8, workers=4, fps=None,
     Both quantise on the GPU.  The input frames are written as the network saw them: the decoded bytes, or with
     model.input_size exactly the bytes of cv2.resize of them (which the GPU resize reproduces).  Frames go in RGB with
     model.upstream and BGR otherwise, like the CLI; the files are BGR.  The files do not depend on batch or workers.
+
+    native=True (a model with input_size) writes every frame at the decoded size: the flows are estimated and reversed at
+    input_size, and the interpolated frames blended from the decoded frames (RaftEngine's native blend), so each equals
+    the single-pair CLI's --native-frames PNG byte for byte; input frames and scene-cut copies are the decoded frames
+    (only converted to BGR).
 
     scene_cut (a threshold in [0, 1]) stops interpolation at scene cuts: each pass's frames are copied to the GPU once and
     scored there (networks.utils.scene_cut_scores of the decoded frames), and pair k is a cut when its score exceeds
@@ -398,7 +403,7 @@ def video_interpolate(model, frames, out, ts=None, batch=8, workers=4, fps=None,
         return os.path.join(out, f"frame_{n:06d}.png")
 
     def original(img):  # the frame as the network saw it, BGR
-        if size is not None:
+        if size is not None and not native:
             img = cv2.resize(img, dsize=(size[1], size[0]))
         return cv2.cvtColor(img, cv2.COLOR_RGB2BGR) if rgb else img
 
@@ -460,7 +465,7 @@ def video_interpolate(model, frames, out, ts=None, batch=8, workers=4, fps=None,
                     pairs = [(r, k) for r, k in enumerate(ps.pairs) if k is not None]
                     live = [(r, k) for r, k in pairs if k not in cut]
                     if live:
-                        res = engine.interpolate_sequence(src, ts, uint8=True, bgr=rgb).flatten(0, 1)
+                        res = engine.interpolate_sequence(src, ts, uint8=True, bgr=rgb, native=native).flatten(0, 1)
                     made = [(frame_number(k, m, jt), jt * T + r) for r, k in live for jt in range(m)]
                     copies = [(frame_number(k, m), k) for _, k in pairs] + ([(n_out - 1, last)]
                                                                             if j == len(passes) - 1 else [])
@@ -469,7 +474,7 @@ def video_interpolate(model, frames, out, ts=None, batch=8, workers=4, fps=None,
                     items, cut_copies = split_cut_items(ps.items, cut)
                     if items:
                         res = engine.interpolate_sequence_at(src, [(k - first, t) for _, k, t in items], uint8=True,
-                                                             bgr=rgb)
+                                                             bgr=rgb, native=native)
                     made = [(n, i) for i, (n, _, _) in enumerate(items)]
                     copies = ps.copies + cut_copies
                 slot.event = torch.cuda.Event()
