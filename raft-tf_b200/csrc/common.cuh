@@ -151,7 +151,8 @@ struct SplitPtr {
 enum Epilogue : int {
   EPI_ACT = 0,    // y = act(acc+bias) -> split planes d0 (and d1)
   EPI_ZR = 1,     // c<hidden: z=sigmoid -> f0 ; else r=sigmoid, r*h(f1) -> d0
-  EPI_Q = 2,      // q=tanh ; h=(1-z)h+zq -> f1 and d0
+  EPI_Q = 2,      // q=tanh ; h=(1-z)h+zq -> f1 and d0, rounded as fma(z, q, fl32(fl32(1-z)*h)) in both epilogues
+                  // (explicit intrinsics, so no compiler contraction choice can change the bits; tests/test_gpu_exact_gates.py)
   EPI_DELTA = 3,  // c<2: coords1(f1)[c] += v ; optional copy to f2
   EPI_F32 = 4     // f0[pix*cout+c] = scale*v
 };
@@ -236,6 +237,9 @@ __device__ __forceinline__ float div_rn(float v, const ConvParams& p) {
 
 // Gate non-linearities on the SFU: exp via ex2.approx (abs. error of the gate < 3e-7 for |x| < 16, i.e.
 // below the 2^-22 operand truncation of the split GEMM that feeds them), reciprocal via rcp.approx.
+// Deterministic functions of their fp32 input; tests/test_gpu_exact_gates.py measures them on the H100 over every multiple
+// of 2^-6 in [-24, 24] and the saturation points (largest error 1.07e-7 for sigmoid_f, 2.02e-7 for tanh_f; exact 0 / 1 / +-1
+// at |x| >= 100) and holds every conv path to the measured bits.
 // r01 profile: with libm expf/tanhf + IEEE division the GRU epilogues took as long as their MMA loops.
 __device__ __forceinline__ float ex2_fast(float x) {
   float y;
@@ -401,7 +405,7 @@ __device__ __forceinline__ void epilogue_store(const ConvParams& p, int pix, int
 #pragma unroll
       for (int i = 0; i < NV; ++i) {
         const float q = tanh_f(y[i]);
-        y[i] = (1.0f - z[i]) * hprev[i] + z[i] * q;  // model_utils.py:147,155,168
+        y[i] = __fmaf_rn(z[i], q, __fmul_rn(1.0f - z[i], hprev[i]));  // model_utils.py:147,155,168; rounding: EPI_Q
       }
       store_f32(p.f1 + (size_t)pix * p.hidden + c, y);
       store_split(p.d0_hi, p.d0_lo, p.d0_stride, p.d0_choff, c, y);
@@ -540,7 +544,7 @@ __device__ __forceinline__ void epilogue_wide16(const ConvParams& p, int pix, in
 #pragma unroll
       for (int i = 0; i < 16; ++i) {
         const float q = tanh_f(y[i]);
-        y[i] = (1.0f - z[i]) * hprev[i] + z[i] * q;  // model_utils.py:147,155,168
+        y[i] = __fmaf_rn(z[i], q, __fmul_rn(1.0f - z[i], hprev[i]));  // model_utils.py:147,155,168; rounding: EPI_Q
       }
       store_f32(hp, 0);
       store_split(p.d0_hi, p.d0_lo, (size_t)pix * p.d0_stride + p.d0_choff, 0);

@@ -35,9 +35,9 @@ __global__ void __launch_bounds__(256) upsample_convex_kernel(const float2* __re
       fx = 8.0f * (c.x - (float)xx);
       fy = 8.0f * (c.y - (float)yy);
     }
-    const float p = v[k] / sum;
-    ax += fx * p;
-    ay += fy * p;
+    const float p = v[k] / sum;  // IEEE quotient
+    ax = __fmaf_rn(fx, p, ax);
+    ay = __fmaf_rn(fy, p, ay);
   }
   const int oy = y * 8 + (t >> 3) - top, ox = x * 8 + (t & 7) - left;
   if (oy >= 0 && oy < oH && ox >= 0 && ox < oW) out[((size_t)b * oH + oy) * oW + ox] = make_float2(ax, ay);
