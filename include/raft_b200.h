@@ -266,6 +266,27 @@ int rb_upflow8_crop(const float* coords1, float* out, int B, int h, int w, float
 int rb_flow_fb_check(const float* flow_fw, const float* flow_bw, uint8_t* occ_fw, uint8_t* occ_bw,
                      int B, int H, int W, float flow_scale, float alpha1, float alpha2, void* stream);
 
+/* ---- F16: point tracking -- consecutive flows chained per point, with the F5 test at every step -------------------
+ * flow_fw, flow_bw: [T,H,W,2] fp32 in pair order (flow_fw[k] frame k -> k+1, flow_bw[k] k+1 -> k, as
+ * forward_sequence_bidirectional returns them); the first n_steps (1 <= n_steps <= T) pairs are used.  N queries:
+ * qframe [N] int32 (a global frame index) and qpos [N,2] fp32 (x, y in the flows' pixels); first_frame is the global
+ * index of flow frame 0.  pos [N,2] fp32 and state [N] uint8 carry a query across calls: read for a query with
+ * qframe < first_frame, and always written with the last row.  Outputs, frame-major: tracks [n_steps+1,N,2] fp32 and
+ * status [n_steps+1,N] uint8, row j = frame first_frame + j.  Status: 0 consistent, 1 inconsistent (occluded), 2 left
+ * the frame, 3 before the query frame.  Rows before qframe are (NaN, NaN) with 3; the row of qframe is qpos with 0; a
+ * query with qframe < first_frame has row 0 = (pos, state).  Each step k -> k+1 from a position q with status 0 or 1:
+ * f = s * (bilinear sample of flow_fw[k] at q), the sample and its arithmetic those of rb_flow_fb_check (s = flow_scale);
+ * q' = q + f; status 2 and position NaN unless q' is inside [0, W-1] x [0, H-1] (NaN counts as outside), and status 2
+ * is final; otherwise b = s * (sample of flow_bw[k] at q'), status 1 if |f+b|^2 > alpha1 (|f|^2 + |b|^2) + alpha2 else
+ * 0, position q'.  Status 1 is not final: the position keeps integrating.  A qpos outside the frame leaves it at the
+ * first step.  Every operation is rounded on its own, left to right (bit-reproducible by an fp32 restatement), and
+ * each query is computed alone: its rows do not depend on N, the other queries or how a clip is split into calls.
+ * Null pointers, T/H/W/N <= 0, n_steps outside [1, T], flow_scale <= 0 or non-finite, negative or non-finite alphas
+ * -> RB_ERR_* before any CUDA call. */
+int rb_track_points(const float* flow_fw, const float* flow_bw, int T, int H, int W, int n_steps, float flow_scale,
+                    float alpha1, float alpha2, const int32_t* qframe, const float* qpos, int N, int first_frame,
+                    float* pos, uint8_t* state, float* tracks, uint8_t* status, void* stream);
+
 /* ---- F6: frame interpolation -- flow_utils.py:166-274 reverse_flow_avg_skip_static, batched, and the frame blend -----
  * rb_flow_reverse: per sample of flow01 [B,H,W,2] fp32, bit for bit with the reference under numpy >= 2:
  *  1. static(p) = every channel c has d_c < 10, d_c = uint8(bg - im0) (img_u8 = 1: wraps, like numpy's uint8) or

@@ -4,6 +4,7 @@
 #include <math.h>
 
 #include "common.cuh"
+#include "fb_sample.cuh"
 
 namespace rb {
 
@@ -24,31 +25,14 @@ __global__ void __launch_bounds__(256) flow_fb_check_kernel(const float2* __rest
   const int x = (int)(p % W), y = (int)((p / W) % H);
   const size_t img = p - ((size_t)y * W + x);  // first pixel of this sample
   const float2 fr = fsrc[p];
-  const float fx = __fmul_rn(s, fr.x), fy = __fmul_rn(s, fr.y);
-  const float qx = __fadd_rn((float)x, fx), qy = __fadd_rn((float)y, fy);
-  // written so that a NaN target also counts as leaving the frame
-  if (!(qx >= 0.f && qx <= (float)(W - 1) && qy >= 0.f && qy <= (float)(H - 1))) {
+  const float2 f = make_float2(__fmul_rn(s, fr.x), __fmul_rn(s, fr.y));
+  const float qx = __fadd_rn((float)x, f.x), qy = __fadd_rn((float)y, f.y);
+  if (!inside_frame(qx, qy, H, W)) {
     out[p] = 2;
     return;
   }
-  const int x0 = (int)floorf(qx), y0 = (int)floorf(qy);
-  const int x1 = min(x0 + 1, W - 1), y1 = min(y0 + 1, H - 1);
-  const float ax = __fsub_rn(qx, (float)x0), ay = __fsub_rn(qy, (float)y0);
-  const float cx = __fsub_rn(1.f, ax), cy = __fsub_rn(1.f, ay);
-  const float2 b00 = bsrc[img + (size_t)y0 * W + x0], b01 = bsrc[img + (size_t)y0 * W + x1];
-  const float2 b10 = bsrc[img + (size_t)y1 * W + x0], b11 = bsrc[img + (size_t)y1 * W + x1];
-  auto bilerp = [&](float v00, float v01, float v10, float v11) {
-    const float t0 = __fadd_rn(__fmul_rn(cx, v00), __fmul_rn(ax, v01));
-    const float t1 = __fadd_rn(__fmul_rn(cx, v10), __fmul_rn(ax, v11));
-    return __fadd_rn(__fmul_rn(t0, cy), __fmul_rn(t1, ay));
-  };
-  const float bx = __fmul_rn(s, bilerp(b00.x, b01.x, b10.x, b11.x));
-  const float by = __fmul_rn(s, bilerp(b00.y, b01.y, b10.y, b11.y));
-  const float ex = __fadd_rn(fx, bx), ey = __fadd_rn(fy, by);
-  const float d = __fadd_rn(__fmul_rn(ex, ex), __fmul_rn(ey, ey));
-  const float mag = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(fx, fx), __fmul_rn(fy, fy)), __fmul_rn(bx, bx)), __fmul_rn(by, by));
-  const float m = __fadd_rn(__fmul_rn(a1, mag), a2);
-  out[p] = d > m ? 1 : 0;
+  const float2 b = sample_flow(bsrc + img, W, bilerp_at(qx, qy, H, W), s);
+  out[p] = fb_inconsistent(f, b, a1, a2);
 }
 
 }  // namespace rb

@@ -60,6 +60,14 @@ GPU (one minus the intersection of the frames' colour histograms, in [0, 1]); a 
 interpolated frames are copies of the nearer input frame, and warm-started flow restarts cold.  The run prints
 ``scene cuts: <count> at pairs <k> ...``.  No default: pick the threshold for the footage.
 
+--path DIR --track POINTS.txt tracks points through DIR's frames (one `frame x y` line per point, in the frames' own
+pixels; --track-grid STEP [--track-frame K] puts one at every STEP-th pixel of frame K instead): every point is chained
+through the consecutive flows with a forward-backward check at each step, and ``<--out>/tracks.npy`` [F,N,2] and
+``<--out>/status.npy`` [F,N] (0 consistent, 1 occluded, 2 left the frame, 3 before the query frame) are written;
+--track-vis DIR also draws the visible points on every frame (raft_b200.video.video_track):
+
+    python infer_raft.py --path frames/ --out tracks/ --track points.txt --load raft-things.npz [--track-vis vis/]
+
 --native-frames (with --interpolate, or --path with --interpolate or --input-fps/--fps) writes the interpolated frames,
 and with --path the copied input frames, at the input's own size: the flow is estimated and reversed at the network size,
 then resized inside the blend, which warps the decoded frames.  --flow-size H W sets that network size in place of
@@ -159,6 +167,15 @@ def parser():
                         "--path, the copied input) frames at the input's own size, from flow estimated at the network size")
     p.add_argument('--flow-size', type=int, nargs=2, default=None, metavar=('H', 'W'),
                    help='extension: the network size frames are resized to, in place of 432x1024 (test mode and --path)')
+    p.add_argument('--track', default=None, metavar='POINTS.txt',
+                   help="extension, with --path: track the points of a text file (one `frame x y` line per point, in "
+                        "the frames' own pixels) through the frames; writes <--out>/tracks.npy and status.npy")
+    p.add_argument('--track-grid', type=int, default=None, metavar='STEP',
+                   help='extension, with --path: track a point at every STEP-th pixel of frame --track-frame (1: dense)')
+    p.add_argument('--track-frame', type=int, default=0, metavar='K',
+                   help='extension, with --track-grid: the frame the grid is laid on (default 0)')
+    p.add_argument('--track-vis', default=None, metavar='DIR',
+                   help='extension, with --track or --track-grid: also write every frame with the visible points drawn')
     p.add_argument('--upstream', action='store_true',
                    help='extension: weights converted from an official princeton-vl RAFT .pth (raft_b200.convert): RGB '
                         'frames and the upstream numerics (RAFT(..., upstream=True))')
@@ -171,6 +188,26 @@ def parser():
 def main(argv=None):
     p = parser()
     args = p.parse_args(argv)
+    if args.track is not None or args.track_grid is not None:
+        if args.track is not None and args.track_grid is not None:
+            p.error('--track and --track-grid are two ways to give the points: pass one')
+        flag = '--track' if args.track is not None else '--track-grid'
+        if args.path is None or args.mode != 'test':
+            p.error(f'{flag} tracks points through a frame directory: it needs --path DIR (and no -m val)')
+        for other, given in (('--interpolate', args.interpolate), ('--fps', args.fps), ('--input-fps', args.input_fps),
+                             ('--warm-start', args.warm_start), ('--scene-cut', args.scene_cut is not None),
+                             ('--bidirectional', args.bidirectional), ('--native-flow', args.native_flow),
+                             ('--native-frames', args.native_frames), ('--flo', args.flo), ('--npy', args.npy)):
+            if given:
+                p.error(f'{flag} writes point tracks: it cannot be combined with {other}')
+        if args.track_grid is not None and args.track_grid < 1:
+            p.error(f'--track-grid: the step must be >= 1 (got {args.track_grid})')
+        if args.batch < 1 or args.workers < 0:
+            p.error('--path needs --batch >= 1 and --workers >= 0')
+        return run_track(args, p)
+    for flag, given in (('--track-frame', args.track_frame != 0), ('--track-vis', args.track_vis is not None)):
+        if given:
+            p.error(f'{flag} goes with --track-grid' + (' or --track' if flag == '--track-vis' else ''))
     fps = None
     if args.fps is not None or args.input_fps is not None:
         if args.fps is None or args.input_fps is None:
@@ -337,6 +374,31 @@ def run_video_interpolate(args, fps=None):
     if args.scene_cut is not None:
         files = _print_cuts(*files)
     print(f"{len(files)} frames written under {args.out}")
+    return 0
+
+
+def run_track(args, p):
+    """--path --track / --track-grid: raft_b200.video.video_track over the frames of --path, at 432x1024 (or --flow-size)
+    like test mode (or their own size with --keep-size); the points are given and tracked in the frames' own pixels.
+    Prints the point count, the frame count and how many points are consistent (status 0) in the last frame."""
+    from networks import RAFT
+    from raft_b200.video import read_queries, video_track
+    queries = None
+    if args.track is not None:
+        try:
+            queries = read_queries(args.track)
+        except (OSError, ValueError) as e:
+            p.error(f'--track: {e}')
+    iters = 20 if args.iters is None else args.iters
+    size = None if args.keep_size else _flow_size(args)
+    model = RAFT.RAFT(None if size is None else size + (3,), args, iters=iters, input_size=size, upstream=args.upstream,
+                      mixed_precision=args.mixed_precision).load(args.load)
+    tracks, status = video_track(model, args.path, args.out, queries=queries, grid=args.track_grid,
+                                 grid_frame=args.track_frame, batch=args.batch, workers=args.workers, vis=args.track_vis)
+    st = np.load(status, mmap_mode='r')
+    F, N = st.shape
+    print(f"{N} points tracked through {F} frames: {int((st[-1] == 0).sum())} consistent (status 0) in the last frame; "
+          f"{tracks} and {status} written")
     return 0
 
 

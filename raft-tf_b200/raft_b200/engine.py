@@ -503,6 +503,26 @@ class RaftEngine:
         return self.flow_up[:T], self.flow_bw, self.occ[:T], self.occ[T:]
 
     @torch.no_grad()
+    def track(self, frames: torch.Tensor, queries):
+        """Point tracking: queries [N,3] rows (frame, x, y), x and y in the frames' own pixels, followed from their frame
+        to the last of the [F,H,W,3] frames (dtypes, sizes and input_size as for forward()).  One
+        forward_sequence_bidirectional(check=False) pass, then one rb_track_points launch on its flows (flow_scale as in
+        the occlusion check).  With input_size the positions are mapped to the network grid and the tracks back
+        (track_queries, tracks_to_frames).  Returns fresh (tracks [F,N,2] fp32, status [F,N] uint8) CUDA tensors in the
+        frames' own pixels: status 0 consistent, 1 inconsistent (occluded; the track goes on), 2 left the frame (NaN from
+        then on), 3 before the query frame (NaN).  Bad queries raise ValueError before the pass."""
+        F = _sequence_length(frames) + 1
+        src_hw = tuple(frames.shape[1:3])
+        net_hw = self.input_size if self.input_size is not None else src_hw
+        qframe, qpos = track_queries(queries, F, src_hw, net_hw)
+        from networks.utils import track_points
+        flow_fw, flow_bw, _, _ = self.forward_sequence_bidirectional(frames, check=False)
+        with torch.cuda.device(self.device):
+            tracks, status, _ = track_points(flow_fw, flow_bw, qframe, qpos, flow_scale=self.flow_scale,
+                                             alpha1=FB_ALPHA1, alpha2=FB_ALPHA2)
+            return tracks_to_frames(tracks, src_hw, net_hw), status
+
+    @torch.no_grad()
     def interpolate(self, left: torch.Tensor, right: torch.Tensor, ts, native: bool = False) -> torch.Tensor:
         """Frames at times ts (each in [0, 1]; 0 = left, 1 = right) between B frame pairs: one bidirectional pass (as
         forward_bidirectional(check=False), from a graph of its own), then eagerly on the same stream, for as many times
@@ -730,6 +750,46 @@ def _items(items, T):
         ks.append(int(k))
         ts.append(float(t))
     return ks, ts
+
+
+def track_queries(queries, F, src_hw, net_hw):
+    """The query points of RaftEngine.track as kernel inputs: queries [N,3] rows (frame, x, y) in the frames' own Hs x Ws
+    pixels -> (qframe [N] int32, qpos [N,2] fp32 on the network's Hn x Wn grid).  With another network size the
+    positions map by cv2's pixel-centre convention, x_n = (x + 0.5) Wn / Ws - 0.5 (the ratio resize_flow applies to
+    displacements), in fp64, rounded once to fp32 and clamped into [0, Wn - 1] x [0, Hn - 1]: the clamp moves only
+    queries within half a source pixel of the edge, by less than half a network pixel, and keeps every query inside the
+    frame the flow covers.  A frame outside [0, F), a non-integer frame, a non-finite position or one outside
+    [0, Ws - 1] x [0, Hs - 1], an empty list or a wrong shape raises ValueError."""
+    try:
+        q = np.asarray(queries.cpu() if isinstance(queries, torch.Tensor) else queries, dtype=np.float64)
+    except (TypeError, ValueError):
+        raise ValueError("raft_b200: queries must be an [N,3] array of (frame, x, y) rows") from None
+    if q.ndim != 2 or q.shape[1] != 3 or q.shape[0] < 1:
+        raise ValueError(f"raft_b200: queries must be an [N,3] array of (frame, x, y) rows, N >= 1 (got {q.shape})")
+    (Hs, Ws), (Hn, Wn) = src_hw, net_hw
+    frame, x, y = q[:, 0], q[:, 1], q[:, 2]
+    with np.errstate(invalid="ignore"):
+        bad = ~((frame >= 0) & (frame < F) & (frame == np.floor(frame)) & np.isfinite(x) & np.isfinite(y)
+                & (x >= 0) & (x <= Ws - 1) & (y >= 0) & (y <= Hs - 1))
+    if bad.any():
+        i = int(np.flatnonzero(bad)[0])
+        raise ValueError(f"raft_b200: query {i} = {tuple(q[i].tolist())}: needs an integer frame in [0, {F}) and a "
+                         f"finite (x, y) in [0, {Ws - 1}] x [0, {Hs - 1}]")
+    if (Hn, Wn) != (Hs, Ws):
+        x = np.clip(((x + 0.5) * (Wn / Ws) - 0.5).astype(np.float32), np.float32(0), np.float32(Wn - 1))
+        y = np.clip(((y + 0.5) * (Hn / Hs) - 0.5).astype(np.float32), np.float32(0), np.float32(Hn - 1))
+    return frame.astype(np.int32), np.stack([x, y], axis=-1).astype(np.float32)
+
+
+def tracks_to_frames(tracks, src_hw, net_hw):
+    """Tracks [...,2] fp32 on the network's Hn x Wn grid back to the frames' own Hs x Ws pixels, the inverse of
+    track_queries' map, x = (x_n + 0.5) Ws / Wn - 0.5 in fp64 rounded once to fp32 (NaN stays NaN); the tensor itself
+    when the sizes agree."""
+    (Hs, Ws), (Hn, Wn) = src_hw, net_hw
+    if (Hn, Wn) == (Hs, Ws):
+        return tracks
+    scale = torch.tensor([Ws / Wn, Hs / Hn], dtype=torch.float64, device=tracks.device)
+    return ((tracks.double() + 0.5) * scale - 0.5).float()
 
 
 def _floats(values):

@@ -23,6 +23,11 @@ pinned slots used in turn, each refilled only after the event behind its pass ha
 flows, when written) are copied to two pinned output slots and PNG-encoded and written by writer threads.  The files are
 the same bytes for every workers value.
 
+video_track(model, "frames/", "out/", queries=[[0, 120.0, 64.5], ...]) tracks points through the clip (grid=STEP: a point
+at every STEP-th pixel of one frame): interp_schedule()'s passes of forward_sequence_bidirectional, each followed by one
+rb_track_points launch that carries the points' positions and states on the GPU, the rows streamed into out/tracks.npy and
+out/status.npy.
+
 Scene cuts (scene_cut=<threshold in [0, 1]>, video_interpolate and warm-started video): each pass's decoded frames are
 copied to the GPU once and scored there (networks.utils.scene_cut_scores: one minus the intersection of consecutive
 frames' colour histograms); a pair whose score exceeds the threshold is a cut.  Frame-rate conversion copies the nearer
@@ -503,3 +508,167 @@ def video_interpolate(model, frames, out, ts=None, batch=8, workers=4, fps=None,
                 pool.shutdown(wait=True, cancel_futures=True)
     paths = [name(n) for n in range(n_out)]
     return paths if thr is None else (paths, cuts)
+
+
+def read_queries(path):
+    """The query points of a text file, one `frame x y` line per point (frame an integer, x and y pixels of the frames'
+    own size); blank lines and text after '#' are skipped.  Returns an [N,3] float64 array; a malformed line or a file
+    without points raises ValueError."""
+    rows = []
+    with open(path) as f:
+        for n, line in enumerate(f, 1):
+            parts = line.split("#", 1)[0].split()
+            if not parts:
+                continue
+            try:
+                if len(parts) != 3:
+                    raise ValueError
+                rows.append((int(parts[0]), float(parts[1]), float(parts[2])))
+            except ValueError:
+                raise ValueError(f"video: {path}:{n}: expected `frame x y` with an integer frame "
+                                 f"(got {line.strip()!r})") from None
+    if not rows:
+        raise ValueError(f"video: {path} holds no query points")
+    return np.array(rows, dtype=np.float64)
+
+
+def track_grid(H, W, step, frame=0):
+    """The queries of a grid on frame `frame` of H x W frames: a point at every step-th pixel, x in {0, step, ...} <= W - 1
+    and y likewise, row by row.  Returns an [N,3] float64 array of (frame, x, y); step = 1 is every pixel.  A step below
+    1 raises ValueError."""
+    if int(step) != step or int(step) < 1:
+        raise ValueError(f"video: the grid step must be an integer >= 1 (got {step!r})")
+    ys, xs = np.meshgrid(np.arange(0, int(H), int(step)), np.arange(0, int(W), int(step)), indexing="ij")
+    return np.stack([np.full(xs.size, int(frame)), xs.ravel(), ys.ravel()], axis=-1).astype(np.float64)
+
+
+def track_colors(N):
+    """The fixed BGR colour of each of N query points in video_track's drawings (a seeded draw, so every run and every
+    batch paints a point alike)."""
+    return np.random.default_rng(0).integers(40, 256, size=(N, 3)).astype(np.uint8)
+
+
+def video_track(model, frames, out, queries=None, grid=None, grid_frame=0, batch=8, workers=4, vis=None):
+    """Point tracking through a video of any length with a loaded networks.RAFT.RAFT model: the frames (a directory's
+    sorted *.png / *.jpg, or a list of paths, all of one size) and the query points as `queries` ([N,3] rows (frame, x,
+    y) in the frames' own pixels) or `grid` = STEP (track_grid() on frame grid_frame; give exactly one).  Every pass runs
+    forward_sequence_bidirectional(check=False) on batch + 1 frames (interp_schedule()) and one rb_track_points launch
+    (networks.utils.track_points), the points' positions and states carried from pass to pass on the GPU.  Writes
+    <out>/tracks.npy [F,N,2] fp32 and <out>/status.npy [F,N] uint8 (RaftEngine.track's outputs), each pass's rows
+    streamed into them through memory maps, so host memory does not grow with F.  vis (a directory) also writes every
+    frame at its own size as <vis>/frame_<i:06d>.png with each point of status 0 drawn as a dot in its own colour
+    (track_colors()).  The files are the same bytes for every batch and workers value, and equal RAFT.track on the whole
+    clip.  Frames go in RGB with model.upstream and BGR otherwise, like the CLI.  Returns (tracks path, status path)."""
+    import cv2
+    from networks.utils import track_points
+    from .engine import FB_ALPHA1, FB_ALPHA2, track_queries, tracks_to_frames
+
+    paths = list_frames(frames)
+    if (queries is None) == (grid is None):
+        raise ValueError("video_track: give the query points or a grid step, exactly one")
+    batch, workers = int(batch), int(workers)
+    if workers < 0:
+        raise ValueError(f"video: workers must be >= 0 (got {workers})")
+    passes = interp_schedule(len(paths), batch)
+    F, T = len(paths), batch
+    out = os.fspath(out)
+    os.makedirs(out, exist_ok=True)
+    if vis is not None:
+        vis = os.fspath(vis)
+        os.makedirs(vis, exist_ok=True)
+    engine = model.engine()
+    rgb = bool(model.upstream)
+    dev = engine.device
+    files = (os.path.join(out, "tracks.npy"), os.path.join(out, "status.npy"))
+
+    def write(slot, first, rows, imgs):  # writer thread: the rows of one pass, once its copies have landed
+        slot.event.synchronize()
+        tracks_mm[first + rows.start:first + rows.stop] = slot.tracks[rows.start:rows.stop].numpy()
+        status_mm[first + rows.start:first + rows.stop] = slot.status[rows.start:rows.stop].numpy()
+        if vis is None:
+            return
+        for r in rows:
+            img = cv2.cvtColor(imgs[r], cv2.COLOR_RGB2BGR) if rgb else imgs[r].copy()
+            seen = np.flatnonzero(slot.status[r].numpy() == 0)
+            xy = np.rint(slot.tracks[r].numpy()[seen]).astype(np.int64)
+            for i, (x, y) in zip(seen, xy):
+                cv2.circle(img, (int(x), int(y)), 2, colors[i].tolist(), -1)
+            name = os.path.join(vis, f"frame_{first + r:06d}.png")
+            if not cv2.imwrite(name, img):
+                raise OSError(f"cannot write {name}")
+
+    decoders = ThreadPoolExecutor(workers) if workers > 0 else None
+    writers = ThreadPoolExecutor(workers) if workers > 0 else None
+    depth = max(1, -(-workers // T))  # passes decoded ahead of the one the GPU is given
+
+    def submit(j):
+        if decoders is None:
+            return [(i, lambda i=i: _imread(paths[i], rgb)) for i in passes[j].frames]
+        return [(i, decoders.submit(_imread, paths[i], rgb).result) for i in passes[j].frames]
+
+    shape, ins, outs, qframe, qpos, state = None, None, None, None, None, None
+    tracks_mm = status_mm = colors = None
+    try:
+        with torch.cuda.device(dev):
+            stream = torch.cuda.current_stream(dev)
+            ahead = [submit(j) for j in range(min(depth, len(passes)))]
+            for j, ps in enumerate(passes):
+                loads = ahead.pop(0)
+                if j + depth < len(passes):
+                    ahead.append(submit(j + depth))
+                imgs = []
+                for i, load in loads:
+                    img = load()
+                    if shape is None:
+                        shape = img.shape
+                    elif img.shape != shape:
+                        raise ValueError(f"video: {paths[i]} is a {img.shape[0]}x{img.shape[1]} frame, {paths[0]} is "
+                                         f"{shape[0]}x{shape[1]}: every frame needs one size")
+                    imgs.append(img)
+                if ins is None:  # the first pass: the queries, now that the frame size is known
+                    src_hw = tuple(shape[:2])
+                    net_hw = engine.input_size if engine.input_size is not None else src_hw
+                    q = track_grid(*src_hw, grid, grid_frame) if grid is not None else queries
+                    qf, qp = track_queries(q, F, src_hw, net_hw)
+                    qframe, qpos = torch.from_numpy(qf).to(dev), torch.from_numpy(qp).to(dev)
+                    N = len(qf)
+                    colors = track_colors(N) if vis is not None else None
+                    tracks_mm = np.lib.format.open_memmap(files[0], mode="w+", dtype=np.float32, shape=(F, N, 2))
+                    status_mm = np.lib.format.open_memmap(files[1], mode="w+", dtype=np.uint8, shape=(F, N))
+                    ins = [_Slot(frames=((T + 1,) + shape, torch.uint8)) for _ in range(2)]
+                    outs = [_Slot(tracks=((T + 1, N, 2), torch.float32), status=((T + 1, N), torch.uint8))
+                            for _ in range(2)]
+                slot = ins[j % 2]
+                slot.wait()
+                for r, img in enumerate(imgs):
+                    slot.frames[r].numpy()[...] = img
+                flow_fw, flow_bw, _, _ = engine.forward_sequence_bidirectional(slot.frames, check=False)
+                n_steps = sum(k is not None for k in ps.pairs)
+                first = ps.frames[0]
+                tracks, status, state = track_points(flow_fw, flow_bw, qframe, qpos, state=state, first_frame=first,
+                                                     n_steps=n_steps, flow_scale=engine.flow_scale, alpha1=FB_ALPHA1,
+                                                     alpha2=FB_ALPHA2)
+                tracks = tracks_to_frames(tracks, src_hw, net_hw)
+                slot.event = torch.cuda.Event()
+                slot.event.record(stream)
+                o = outs[j % 2]
+                o.wait()
+                o.tracks[:n_steps + 1].copy_(tracks, non_blocking=True)
+                o.status[:n_steps + 1].copy_(status, non_blocking=True)
+                o.event = torch.cuda.Event()
+                o.event.record(stream)
+                rows = range(0 if j == 0 else 1, n_steps + 1)  # row 0 of a later pass is the last row of the one before
+                if writers is None:
+                    write(o, first, rows, imgs)
+                else:
+                    o.futures.append(writers.submit(write, o, first, rows, imgs))
+            for o in outs or ():
+                o.wait()
+    finally:
+        for pool in (decoders, writers):
+            if pool is not None:
+                pool.shutdown(wait=True, cancel_futures=True)
+        for mm in (tracks_mm, status_mm):
+            if mm is not None:
+                mm.flush()
+    return files
