@@ -344,12 +344,8 @@ def main(argv=None):
 def run_video(args):
     """--path: raft_b200.video over the frames of --path, at 432x1024 (or --flow-size) like test mode (or their own size
     with --keep-size)."""
-    from networks import RAFT
     from raft_b200.video import video
-    iters = 20 if args.iters is None else args.iters
-    size = None if args.keep_size else _flow_size(args)
-    model = RAFT.RAFT(None if size is None else size + (3,), args, iters=iters, input_size=size, upstream=args.upstream,
-                      mixed_precision=args.mixed_precision).load(args.load)
+    model = _video_model(args)
     files = video(model, args.path, args.out, batch=args.batch, workers=args.workers, warm_start=args.warm_start,
                   flo=args.flo, npy=args.npy, native_flow=args.native_flow, scene_cut=args.scene_cut)
     if args.scene_cut is not None:
@@ -363,12 +359,8 @@ def run_video_interpolate(args, fps=None):
     """--path --interpolate, or --path --input-fps --fps (fps = the two rates): raft_b200.video.video_interpolate over the
     frames of --path, at 432x1024 (or --flow-size) like test mode (or their own size with --keep-size); --native-frames
     writes the frames at their own size."""
-    from networks import RAFT
     from raft_b200.video import video_interpolate
-    iters = 20 if args.iters is None else args.iters
-    size = None if args.keep_size else _flow_size(args)
-    model = RAFT.RAFT(None if size is None else size + (3,), args, iters=iters, input_size=size, upstream=args.upstream,
-                      mixed_precision=args.mixed_precision).load(args.load)
+    model = _video_model(args)
     files = video_interpolate(model, args.path, args.out, args.interpolate, batch=args.batch, workers=args.workers,
                               fps=fps, scene_cut=args.scene_cut, native=args.native_frames)
     if args.scene_cut is not None:
@@ -381,7 +373,6 @@ def run_track(args, p):
     """--path --track / --track-grid: raft_b200.video.video_track over the frames of --path, at 432x1024 (or --flow-size)
     like test mode (or their own size with --keep-size); the points are given and tracked in the frames' own pixels.
     Prints the point count, the frame count and how many points are consistent (status 0) in the last frame."""
-    from networks import RAFT
     from raft_b200.video import read_queries, video_track
     queries = None
     if args.track is not None:
@@ -389,10 +380,7 @@ def run_track(args, p):
             queries = read_queries(args.track)
         except (OSError, ValueError) as e:
             p.error(f'--track: {e}')
-    iters = 20 if args.iters is None else args.iters
-    size = None if args.keep_size else _flow_size(args)
-    model = RAFT.RAFT(None if size is None else size + (3,), args, iters=iters, input_size=size, upstream=args.upstream,
-                      mixed_precision=args.mixed_precision).load(args.load)
+    model = _video_model(args)
     tracks, status = video_track(model, args.path, args.out, queries=queries, grid=args.track_grid,
                                  grid_frame=args.track_frame, batch=args.batch, workers=args.workers, vis=args.track_vis)
     st = np.load(status, mmap_mode='r')
@@ -400,6 +388,14 @@ def run_track(args, p):
     print(f"{N} points tracked through {F} frames: {int((st[-1] == 0).sum())} consistent (status 0) in the last frame; "
           f"{tracks} and {status} written")
     return 0
+
+
+def _video_model(args):
+    """The model of --path: at 432x1024 (or --flow-size) like test mode, or at the frames' own size with --keep-size."""
+    from networks import RAFT
+    size = None if args.keep_size else _flow_size(args)
+    return RAFT.RAFT(None if size is None else size + (3,), args, iters=20 if args.iters is None else args.iters,
+                     input_size=size, upstream=args.upstream, mixed_precision=args.mixed_precision).load(args.load)
 
 
 def _flow_size(args):

@@ -18,10 +18,10 @@ batch new frames, so every frame is decoded, uploaded and encoded once.  A short
 frame; its extra rows are idle and their flows discarded, so one pair of CUDA graphs serves the whole video.  warm_start
 runs T = 1 carry passes, each started from forward_interpolate of the previous pass's flow_low (upstream's warm start).
 
-Pipeline, as in raft_b200.evaluate: worker threads decode the frames of the next passes (cv2 releases the GIL) into two
-pinned slots used in turn, each refilled only after the event behind its pass has completed; the colour images (and the
-flows, when written) are copied to two pinned output slots and PNG-encoded and written by writer threads.  The files are
-the same bytes for every workers value.
+Pipeline (_Pipeline, shared by video, video_interpolate and video_track): worker threads decode the frames of the next
+passes (cv2 releases the GIL) into two pinned slots used in turn, each refilled only after the event behind its pass has
+completed; each pass's outputs (colour images and flows, interpolated frames, track rows) are copied to two pinned output
+slots and encoded and written by writer threads.  The files are the same bytes for every workers value.
 
 video_track(model, "frames/", "out/", queries=[[0, 120.0, 64.5], ...]) tracks points through the clip (grid=STEP: a point
 at every STEP-th pixel of one frame): interp_schedule()'s passes of forward_sequence_bidirectional, each followed by one
@@ -41,6 +41,7 @@ import os
 from collections import namedtuple
 from concurrent.futures import ThreadPoolExecutor
 from fractions import Fraction
+from functools import partial
 
 import numpy as np
 import torch
@@ -193,8 +194,8 @@ def frame_number(k, m, j=None):
 
 
 class _Slot:
-    """Pinned host staging (frames in, or colour images and flows out) and the event behind the last pass that used it;
-    futures: the writer tasks that still read it."""
+    """Pinned host staging (frames in, or a pass's outputs) and the event behind the last pass that used it; futures:
+    the writer tasks that still read it."""
 
     def __init__(self, **shapes):
         for name, (shape, dtype) in shapes.items():
@@ -208,6 +209,110 @@ class _Slot:
         self.futures = []
         if self.event is not None:
             self.event.synchronize()
+
+
+def _workers(workers):
+    """The decode and write threads of a _Pipeline as an int (0: none); a negative count raises ValueError."""
+    workers = int(workers)
+    if workers < 0:
+        raise ValueError(f"video: workers must be >= 0 (got {workers})")
+    return workers
+
+
+class _Pipeline:
+    """The passes of a video on the host, on `device`'s current stream:
+
+        with _Pipeline(paths, passes, rgb, batch, workers, device) as pipe:
+            for j, ps, imgs, frames in pipe:  # pass j = passes[j]: its decoded frames, and the pinned rows holding them
+                ...                           # the GPU work of the pass
+                pipe.emit(write, rows, name=device_output, ...)
+
+    The frames of passes[j].frames (paths, decoded RGB with rgb, else BGR) are decoded depth passes ahead by `workers`
+    threads (workers = 0: on this thread when the pass is due) into two pinned input slots of batch + 1 rows used in
+    turn; every frame needs the size of paths[0].  emit() copies the pass's device outputs into two pinned output slots
+    used in turn (allocated on first use with `rows` rows, default the output's own) and records one event behind them
+    and the pass's work; write(slot) then runs on a writer thread (workers = 0: inline) and calls slot.event.synchronize()
+    before it reads the slot (slot None: the pass had no outputs).  A slot is refilled only once its event has completed
+    and its writers have returned, so a writer's exception reaches the caller there or when the pipeline exits."""
+
+    def __init__(self, paths, passes, rgb, batch, workers, device):
+        self.paths, self.passes, self.rgb, self.T, self.workers, self.device = paths, passes, rgb, batch, workers, device
+        self.depth = max(1, -(-workers // batch))  # passes decoded ahead of the one the GPU is given
+        self.ins = self.outs = None
+        self.loose = []  # the writes of passes without outputs
+
+    def __enter__(self):
+        self.decoders = ThreadPoolExecutor(self.workers) if self.workers > 0 else None
+        self.writers = ThreadPoolExecutor(self.workers) if self.workers > 0 else None
+        self.on_device = torch.cuda.device(self.device)
+        self.on_device.__enter__()
+        self.stream = torch.cuda.current_stream(self.device)
+        return self
+
+    def __exit__(self, exc_type, exc, tb):
+        try:
+            if exc_type is None:
+                for o in self.outs or ():
+                    o.wait()
+                for f in self.loose:
+                    f.result()
+        finally:
+            self.on_device.__exit__(None, None, None)
+            for pool in (self.decoders, self.writers):
+                if pool is not None:
+                    pool.shutdown(wait=True, cancel_futures=True)
+
+    def _submit(self, j):
+        if self.decoders is None:
+            return [(i, lambda i=i: _imread(self.paths[i], self.rgb)) for i in self.passes[j].frames]
+        return [(i, self.decoders.submit(_imread, self.paths[i], self.rgb).result) for i in self.passes[j].frames]
+
+    def __iter__(self):
+        paths, depth, shape = self.paths, self.depth, None
+        ahead = [self._submit(j) for j in range(min(depth, len(self.passes)))]
+        for j, ps in enumerate(self.passes):
+            loads = ahead.pop(0)
+            if j + depth < len(self.passes):
+                ahead.append(self._submit(j + depth))
+            imgs = []
+            for i, load in loads:
+                img = load()
+                if shape is None:
+                    shape = img.shape
+                elif img.shape != shape:
+                    raise ValueError(f"video: {paths[i]} is a {img.shape[0]}x{img.shape[1]} frame, {paths[0]} is "
+                                     f"{shape[0]}x{shape[1]}: every frame needs one size")
+                imgs.append(img)
+            if self.ins is None:
+                self.ins = [_Slot(frames=((self.T + 1,) + shape, torch.uint8)) for _ in range(2)]
+            self.j, self.slot = j, self.ins[j % 2]
+            self.slot.wait()
+            frames = self.slot.frames[:len(imgs)]
+            for r, img in enumerate(imgs):
+                frames[r].numpy()[...] = img
+            yield j, ps, imgs, frames
+
+    def emit(self, write, rows=None, **outputs):
+        """Ends the current pass: stages its device outputs (those not None) and hands write the slot."""
+        outputs = {name: t for name, t in outputs.items() if t is not None}
+        o = None
+        if outputs:
+            if self.outs is None:
+                self.outs = [_Slot(**{name: ((rows or len(t),) + tuple(t.shape[1:]), t.dtype)
+                                      for name, t in outputs.items()}) for _ in range(2)]
+            o = self.outs[self.j % 2]
+            o.wait()
+            for name, t in outputs.items():
+                getattr(o, name)[:len(t)].copy_(t, non_blocking=True)
+        event = torch.cuda.Event()  # behind the pass's reads of its input slot and its copies to o
+        event.record(self.stream)
+        self.slot.event = event
+        if o is not None:
+            o.event = event
+        if self.writers is None:
+            write(o)
+        else:
+            (self.loose if o is None else o.futures).append(self.writers.submit(write, o))
 
 
 def video(model, frames, out, batch=8, workers=4, warm_start=False, flo=None, npy=None, native_flow=False,
@@ -231,15 +336,12 @@ def video(model, frames, out, batch=8, workers=4, warm_start=False, flo=None, np
     from networks.utils import flow_to_color, forward_interpolate, resize_flow, scene_cut_scores
 
     paths = list_frames(frames)
-    batch, workers = int(batch), int(workers)
-    if workers < 0:
-        raise ValueError(f"video: workers must be >= 0 (got {workers})")
+    batch, workers = int(batch), _workers(workers)
     thr = None if scene_cut is None else check_scene_cut(scene_cut)
     if thr is not None and not warm_start:
         raise ValueError("video: scene_cut restarts the warm-start chain at cuts; without warm_start every pair runs cold, "
                          "so a cut changes nothing")
     passes = schedule(len(paths), batch, warm_start)
-    T = batch
     dirs = {"png": os.fspath(out), "flo": None if flo is None else os.fspath(flo),
             "npy": None if npy is None else os.fspath(npy)}
     for d in dirs.values():
@@ -263,88 +365,36 @@ def video(model, frames, out, batch=8, workers=4, warm_start=False, flo=None, np
             if npy is not None:
                 np.save(name(k, "npy"), slot.flow[r].numpy())
 
-    decoders = ThreadPoolExecutor(workers) if workers > 0 else None
-    writers = ThreadPoolExecutor(workers) if workers > 0 else None
-    depth = max(1, -(-workers // T))  # passes decoded ahead of the one the GPU is given
-
-    def submit(j):
-        if decoders is None:
-            return [(i, lambda i=i: _imread(paths[i], rgb)) for i in passes[j].frames]
-        return [(i, decoders.submit(_imread, paths[i], rgb).result) for i in passes[j].frames]
-
-    written, shape, ins, outs, init = [], None, None, None, None
+    written, init = [], None
     on_dev, cuts = None, []  # scene_cut: frames k and k + 1 in rows k % 2 and (k + 1) % 2 (the score is symmetric)
-    try:
-        with torch.cuda.device(dev):
-            stream = torch.cuda.current_stream(dev)
-            ahead = [submit(j) for j in range(min(depth, len(passes)))]
-            for j, ps in enumerate(passes):
-                loads = ahead.pop(0)
-                if j + depth < len(passes):
-                    ahead.append(submit(j + depth))
-                imgs = []
-                for i, load in loads:
-                    img = load()
-                    if shape is None:
-                        shape = img.shape
-                    elif img.shape != shape:
-                        raise ValueError(f"video: {paths[i]} is a {img.shape[0]}x{img.shape[1]} frame, {paths[0]} is "
-                                         f"{shape[0]}x{shape[1]}: every frame needs one size")
-                    imgs.append(img)
-                if ins is None:
-                    ins = [_Slot(frames=((T + 1,) + shape, torch.uint8)) for _ in range(2)]
-                slot = ins[j % 2]
-                slot.wait()
-                host = slot.frames[:len(imgs)]
-                for r, img in enumerate(imgs):
-                    host[r].numpy()[...] = img
-                if thr is not None:  # one pair per pass: score it, then hand the engine the device rows
-                    k = ps.pairs[0]
-                    if on_dev is None:
-                        on_dev = torch.empty((2,) + shape, dtype=torch.uint8, device=dev)
-                    if ps.carry:
-                        on_dev[(k + 1) % 2].copy_(host[0], non_blocking=True)
-                        host = on_dev[(k + 1) % 2][None]
-                    else:
-                        on_dev.copy_(host, non_blocking=True)
-                        host = on_dev
-                    cuts += pass_cuts(ps.pairs, scene_cut_scores(on_dev).cpu(), thr)
-                    if cold_start(k, cuts):
-                        init = None
-                if warm_start:
-                    low, flow = engine.forward_sequence(host, carry=ps.carry, flow_init=init, return_low=True)
-                    init = forward_interpolate(low)  # before the next pass overwrites flow_low
+    with _Pipeline(paths, passes, rgb, batch, workers, dev) as pipe:
+        for j, ps, imgs, host in pipe:
+            shape = imgs[0].shape
+            if thr is not None:  # one pair per pass: score it, then hand the engine the device rows
+                k = ps.pairs[0]
+                if on_dev is None:
+                    on_dev = torch.empty((2,) + shape, dtype=torch.uint8, device=dev)
+                if ps.carry:
+                    on_dev[(k + 1) % 2].copy_(host[0], non_blocking=True)
+                    host = on_dev[(k + 1) % 2][None]
                 else:
-                    flow = engine.forward_sequence(host, carry=ps.carry)
-                slot.event = torch.cuda.Event()
-                slot.event.record(stream)
-                if native_flow and tuple(flow.shape[1:3]) != tuple(shape[:2]):
-                    flow = resize_flow(flow, shape[:2])
-                color = flow_to_color(flow, convert_to_bgr=True)
-                if outs is None:
-                    fshape = tuple(flow.shape)
-                    outs = [_Slot(color=(fshape[:3] + (3,), torch.uint8),
-                                  **({"flow": (fshape, torch.float32)} if keep_flow else {})) for _ in range(2)]
-                o = outs[j % 2]
-                o.wait()
-                o.color.copy_(color, non_blocking=True)
-                if keep_flow:
-                    o.flow.copy_(flow, non_blocking=True)
-                o.event = torch.cuda.Event()
-                o.event.record(stream)
-                rows = [(r, k) for r, k in enumerate(ps.pairs) if k is not None]
-                if writers is None:
-                    write(o, rows)
-                else:
-                    o.futures.append(writers.submit(write, o, rows))
-                for _, k in rows:
-                    written += [name(k, e) for e in ("png", "flo", "npy") if dirs[e] is not None]
-            for o in outs or ():
-                o.wait()
-    finally:
-        for pool in (decoders, writers):
-            if pool is not None:
-                pool.shutdown(wait=True, cancel_futures=True)
+                    on_dev.copy_(host, non_blocking=True)
+                    host = on_dev
+                cuts += pass_cuts(ps.pairs, scene_cut_scores(on_dev).cpu(), thr)
+                if cold_start(k, cuts):
+                    init = None
+            if warm_start:
+                low, flow = engine.forward_sequence(host, carry=ps.carry, flow_init=init, return_low=True)
+                init = forward_interpolate(low)  # before the next pass overwrites flow_low
+            else:
+                flow = engine.forward_sequence(host, carry=ps.carry)
+            if native_flow and tuple(flow.shape[1:3]) != tuple(shape[:2]):
+                flow = resize_flow(flow, shape[:2])
+            rows = [(r, k) for r, k in enumerate(ps.pairs) if k is not None]
+            pipe.emit(partial(write, rows=rows), color=flow_to_color(flow, convert_to_bgr=True),
+                      flow=flow if keep_flow else None)
+            for _, k in rows:
+                written += [name(k, e) for e in ("png", "flo", "npy") if dirs[e] is not None]
     return written if thr is None else (written, cuts)
 
 
@@ -381,9 +431,7 @@ def video_interpolate(model, frames, out, ts=None, batch=8, workers=4, fps=None,
     paths = list_frames(frames)
     if (ts is None) == (fps is None):
         raise ValueError("video_interpolate: give the times ts or the rates fps = (input_fps, output_fps), exactly one")
-    batch, workers = int(batch), int(workers)
-    if workers < 0:
-        raise ValueError(f"video: workers must be >= 0 (got {workers})")
+    batch, workers = int(batch), _workers(workers)
     thr = None if scene_cut is None else check_scene_cut(scene_cut)
     last = len(paths) - 1
     if fps is None:
@@ -423,89 +471,36 @@ def video_interpolate(model, frames, out, ts=None, batch=8, workers=4, fps=None,
             if not cv2.imwrite(name(n), slot.frames[r].numpy()):
                 raise OSError(f"cannot write {name(n)}")
 
-    decoders = ThreadPoolExecutor(workers) if workers > 0 else None
-    writers = ThreadPoolExecutor(workers) if workers > 0 else None
-    depth = max(1, -(-workers // T))  # passes decoded ahead of the one the GPU is given
-
-    def submit(j):
-        if decoders is None:
-            return [(i, lambda i=i: _imread(paths[i], rgb)) for i in passes[j].frames]
-        return [(i, decoders.submit(_imread, paths[i], rgb).result) for i in passes[j].frames]
-
-    shape, ins, outs = None, None, None
-    on_dev, cuts, loose = None, [], []  # scene_cut: the pass's frames on the GPU; the writes of passes without a call
-    try:
-        with torch.cuda.device(dev):
-            stream = torch.cuda.current_stream(dev)
-            ahead = [submit(j) for j in range(min(depth, len(passes)))]
-            for j, ps in enumerate(passes):
-                loads = ahead.pop(0)
-                if j + depth < len(passes):
-                    ahead.append(submit(j + depth))
-                imgs = []
-                for i, load in loads:
-                    img = load()
-                    if shape is None:
-                        shape = img.shape
-                    elif img.shape != shape:
-                        raise ValueError(f"video: {paths[i]} is a {img.shape[0]}x{img.shape[1]} frame, {paths[0]} is "
-                                         f"{shape[0]}x{shape[1]}: every frame needs one size")
-                    imgs.append(img)
-                if ins is None:
-                    ins = [_Slot(frames=((T + 1,) + shape, torch.uint8)) for _ in range(2)]
-                slot = ins[j % 2]
-                slot.wait()
-                for r, img in enumerate(imgs):
-                    slot.frames[r].numpy()[...] = img
-                first = ps.frames[0]  # frame i is row i - first of the pass
-                src, cut = slot.frames, ()
-                if thr is not None:  # score the pass on the GPU; the engine then reads the frames from there too
-                    if on_dev is None:
-                        on_dev = torch.empty(slot.frames.shape, dtype=torch.uint8, device=dev)
-                    on_dev.copy_(slot.frames, non_blocking=True)
-                    src, cut = on_dev, pass_cuts(ps.pairs, scene_cut_scores(on_dev).cpu(), thr)
-                    cuts += cut
-                res = None
-                if fps is None:  # row j T + r: pair r of the pass at ts[j]
-                    pairs = [(r, k) for r, k in enumerate(ps.pairs) if k is not None]
-                    live = [(r, k) for r, k in pairs if k not in cut]
-                    if live:
-                        res = engine.interpolate_sequence(src, ts, uint8=True, bgr=rgb, native=native).flatten(0, 1)
-                    made = [(frame_number(k, m, jt), jt * T + r) for r, k in live for jt in range(m)]
-                    copies = [(frame_number(k, m), k) for _, k in pairs] + ([(n_out - 1, last)]
-                                                                            if j == len(passes) - 1 else [])
-                    copies += [(frame_number(k, m, jt), cut_copy(k, t)) for k in cut for jt, t in enumerate(ts)]
-                else:  # row i: item i of the pass
-                    items, cut_copies = split_cut_items(ps.items, cut)
-                    if items:
-                        res = engine.interpolate_sequence_at(src, [(k - first, t) for _, k, t in items], uint8=True,
-                                                             bgr=rgb, native=native)
-                    made = [(n, i) for i, (n, _, _) in enumerate(items)]
-                    copies = ps.copies + cut_copies
-                slot.event = torch.cuda.Event()
-                slot.event.record(stream)
-                o = None
-                if res is not None:
-                    if outs is None:
-                        outs = [_Slot(frames=((rows,) + tuple(res.shape[1:]), torch.uint8)) for _ in range(2)]
-                    o = outs[j % 2]
-                    o.wait()
-                    o.frames[:len(res)].copy_(res, non_blocking=True)
-                    o.event = torch.cuda.Event()
-                    o.event.record(stream)
-                copies = [(n, imgs[i - first]) for n, i in copies]
-                if writers is None:
-                    write(o, made, copies)
-                else:
-                    (loose if o is None else o.futures).append(writers.submit(write, o, made, copies))
-            for o in outs or ():
-                o.wait()
-            for f in loose:
-                f.result()
-    finally:
-        for pool in (decoders, writers):
-            if pool is not None:
-                pool.shutdown(wait=True, cancel_futures=True)
+    on_dev, cuts = None, []  # scene_cut: the pass's frames on the GPU
+    with _Pipeline(paths, passes, rgb, batch, workers, dev) as pipe:
+        for j, ps, imgs, src in pipe:
+            first = ps.frames[0]  # frame i is row i - first of the pass
+            cut = ()
+            if thr is not None:  # score the pass on the GPU; the engine then reads the frames from there too
+                if on_dev is None:
+                    on_dev = torch.empty(src.shape, dtype=torch.uint8, device=dev)
+                on_dev.copy_(src, non_blocking=True)
+                src, cut = on_dev, pass_cuts(ps.pairs, scene_cut_scores(on_dev).cpu(), thr)
+                cuts += cut
+            res = None
+            if fps is None:  # row j T + r: pair r of the pass at ts[j]
+                pairs = [(r, k) for r, k in enumerate(ps.pairs) if k is not None]
+                live = [(r, k) for r, k in pairs if k not in cut]
+                if live:
+                    res = engine.interpolate_sequence(src, ts, uint8=True, bgr=rgb, native=native).flatten(0, 1)
+                made = [(frame_number(k, m, jt), jt * T + r) for r, k in live for jt in range(m)]
+                copies = [(frame_number(k, m), k) for _, k in pairs] + ([(n_out - 1, last)]
+                                                                        if j == len(passes) - 1 else [])
+                copies += [(frame_number(k, m, jt), cut_copy(k, t)) for k in cut for jt, t in enumerate(ts)]
+            else:  # row i: item i of the pass
+                items, cut_copies = split_cut_items(ps.items, cut)
+                if items:
+                    res = engine.interpolate_sequence_at(src, [(k - first, t) for _, k, t in items], uint8=True,
+                                                         bgr=rgb, native=native)
+                made = [(n, i) for i, (n, _, _) in enumerate(items)]
+                copies = ps.copies + cut_copies
+            copies = [(n, imgs[i - first]) for n, i in copies]
+            pipe.emit(partial(write, made=made, copies=copies), rows, frames=res)
     paths = [name(n) for n in range(n_out)]
     return paths if thr is None else (paths, cuts)
 
@@ -566,9 +561,7 @@ def video_track(model, frames, out, queries=None, grid=None, grid_frame=0, batch
     paths = list_frames(frames)
     if (queries is None) == (grid is None):
         raise ValueError("video_track: give the query points or a grid step, exactly one")
-    batch, workers = int(batch), int(workers)
-    if workers < 0:
-        raise ValueError(f"video: workers must be >= 0 (got {workers})")
+    batch, workers = int(batch), _workers(workers)
     passes = interp_schedule(len(paths), batch)
     F, T = len(paths), batch
     out = os.fspath(out)
@@ -597,36 +590,12 @@ def video_track(model, frames, out, queries=None, grid=None, grid_frame=0, batch
             if not cv2.imwrite(name, img):
                 raise OSError(f"cannot write {name}")
 
-    decoders = ThreadPoolExecutor(workers) if workers > 0 else None
-    writers = ThreadPoolExecutor(workers) if workers > 0 else None
-    depth = max(1, -(-workers // T))  # passes decoded ahead of the one the GPU is given
-
-    def submit(j):
-        if decoders is None:
-            return [(i, lambda i=i: _imread(paths[i], rgb)) for i in passes[j].frames]
-        return [(i, decoders.submit(_imread, paths[i], rgb).result) for i in passes[j].frames]
-
-    shape, ins, outs, qframe, qpos, state = None, None, None, None, None, None
-    tracks_mm = status_mm = colors = None
+    state = tracks_mm = status_mm = None
     try:
-        with torch.cuda.device(dev):
-            stream = torch.cuda.current_stream(dev)
-            ahead = [submit(j) for j in range(min(depth, len(passes)))]
-            for j, ps in enumerate(passes):
-                loads = ahead.pop(0)
-                if j + depth < len(passes):
-                    ahead.append(submit(j + depth))
-                imgs = []
-                for i, load in loads:
-                    img = load()
-                    if shape is None:
-                        shape = img.shape
-                    elif img.shape != shape:
-                        raise ValueError(f"video: {paths[i]} is a {img.shape[0]}x{img.shape[1]} frame, {paths[0]} is "
-                                         f"{shape[0]}x{shape[1]}: every frame needs one size")
-                    imgs.append(img)
-                if ins is None:  # the first pass: the queries, now that the frame size is known
-                    src_hw = tuple(shape[:2])
+        with _Pipeline(paths, passes, rgb, batch, workers, dev) as pipe:
+            for j, ps, imgs, frames in pipe:
+                if j == 0:  # the queries, now that the frame size is known
+                    src_hw = tuple(frames.shape[1:3])
                     net_hw = engine.input_size if engine.input_size is not None else src_hw
                     q = track_grid(*src_hw, grid, grid_frame) if grid is not None else queries
                     qf, qp = track_queries(q, F, src_hw, net_hw)
@@ -635,39 +604,16 @@ def video_track(model, frames, out, queries=None, grid=None, grid_frame=0, batch
                     colors = track_colors(N) if vis is not None else None
                     tracks_mm = np.lib.format.open_memmap(files[0], mode="w+", dtype=np.float32, shape=(F, N, 2))
                     status_mm = np.lib.format.open_memmap(files[1], mode="w+", dtype=np.uint8, shape=(F, N))
-                    ins = [_Slot(frames=((T + 1,) + shape, torch.uint8)) for _ in range(2)]
-                    outs = [_Slot(tracks=((T + 1, N, 2), torch.float32), status=((T + 1, N), torch.uint8))
-                            for _ in range(2)]
-                slot = ins[j % 2]
-                slot.wait()
-                for r, img in enumerate(imgs):
-                    slot.frames[r].numpy()[...] = img
-                flow_fw, flow_bw, _, _ = engine.forward_sequence_bidirectional(slot.frames, check=False)
+                flow_fw, flow_bw, _, _ = engine.forward_sequence_bidirectional(frames, check=False)
                 n_steps = sum(k is not None for k in ps.pairs)
                 first = ps.frames[0]
                 tracks, status, state = track_points(flow_fw, flow_bw, qframe, qpos, state=state, first_frame=first,
                                                      n_steps=n_steps, flow_scale=engine.flow_scale, alpha1=FB_ALPHA1,
                                                      alpha2=FB_ALPHA2)
-                tracks = tracks_to_frames(tracks, src_hw, net_hw)
-                slot.event = torch.cuda.Event()
-                slot.event.record(stream)
-                o = outs[j % 2]
-                o.wait()
-                o.tracks[:n_steps + 1].copy_(tracks, non_blocking=True)
-                o.status[:n_steps + 1].copy_(status, non_blocking=True)
-                o.event = torch.cuda.Event()
-                o.event.record(stream)
                 rows = range(0 if j == 0 else 1, n_steps + 1)  # row 0 of a later pass is the last row of the one before
-                if writers is None:
-                    write(o, first, rows, imgs)
-                else:
-                    o.futures.append(writers.submit(write, o, first, rows, imgs))
-            for o in outs or ():
-                o.wait()
+                pipe.emit(partial(write, first=first, rows=rows, imgs=imgs), T + 1,
+                          tracks=tracks_to_frames(tracks, src_hw, net_hw), status=status)
     finally:
-        for pool in (decoders, writers):
-            if pool is not None:
-                pool.shutdown(wait=True, cancel_futures=True)
         for mm in (tracks_mm, status_mm):
             if mm is not None:
                 mm.flush()

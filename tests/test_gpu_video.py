@@ -311,16 +311,38 @@ def test_video_warm_and_native_flow(cuda, frame_dir, tmp_path):
         video(m, frame_dir, str(tmp_path / "x"), batch=8, warm_start=True)
 
 
-def test_video_size_mismatch_names_file(cuda, frame_dir, tmp_path):
+def _mixed_sizes(frame_dir, tmp_path):
+    """A copy of frame_dir whose frame_0006.png is 8 rows short."""
     import cv2
     import shutil
-    from raft_b200.video import video
     d = tmp_path / "mixed"
     shutil.copytree(frame_dir, d)
     bad = d / "frame_0006.png"
     cv2.imwrite(str(bad), cv2.imread(str(bad))[:-8])
+    return str(d)
+
+
+def test_video_size_mismatch_names_file(cuda, frame_dir, tmp_path):
+    from raft_b200.video import video
     with pytest.raises(ValueError, match="frame_0006.png"):
-        video(_model(), str(d), str(tmp_path / "out"), batch=3, workers=2)
+        video(_model(), _mixed_sizes(frame_dir, tmp_path), str(tmp_path / "out"), batch=3, workers=2)
+
+
+@pytest.mark.parametrize("entry,kw", [("video_interpolate", {"ts": [0.5]}), ("video_track", {"grid": 16})],
+                         ids=["video_interpolate", "video_track"])
+def test_interpolate_and_track_size_mismatch_names_file(cuda, frame_dir, tmp_path, entry, kw):
+    import raft_b200.video as rv
+    with pytest.raises(ValueError, match="frame_0006.png"):
+        getattr(rv, entry)(_model(), _mixed_sizes(frame_dir, tmp_path), str(tmp_path / "out"), batch=3, workers=2, **kw)
+
+
+@pytest.mark.parametrize("workers", [0, 4])
+def test_video_write_error_reaches_caller(cuda, frame_dir, tmp_path, workers):
+    from raft_b200.video import video
+    out = tmp_path / "out"
+    (out / "flow_000004.png").mkdir(parents=True)  # cv2.imwrite cannot write over a directory
+    with pytest.raises(OSError, match="flow_000004.png"):
+        video(_model(), frame_dir, str(out), batch=3, workers=workers)
 
 
 def test_cli_path(cuda, frame_dir, tmp_path):
