@@ -287,6 +287,23 @@ int rb_track_points(const float* flow_fw, const float* flow_bw, int T, int H, in
                     float alpha1, float alpha2, const int32_t* qframe, const float* qpos, int N, int first_frame,
                     float* pos, uint8_t* state, float* tracks, uint8_t* status, void* stream);
 
+/* ---- F17: point tracking backward in time -- F16 from the query frame down to frame first_frame -------------------
+ * Arguments, checks and outputs as rb_track_points (row j = frame first_frame + j, q0 = qframe - first_frame); the rows
+ * run from n_steps down to 0.  0 <= q0 <= n_steps: row q0 = qpos with status 0.  Rows after the query frame (j > q0)
+ * are not stored, so a launch after rb_track_points on the same tracks / status completes them in place and leaves the
+ * rows at and after the query frame as the forward launch wrote them.  q0 > n_steps (the query frame lies in a later call
+ * of a reverse sweep): row n_steps = the carried (pos, state), and the point goes on from there.  q0 < 0 (the query frame
+ * lies in an earlier call's frames): nothing is stored and pos / state are left as they are.  Each step k+1 -> k from a
+ * position q with status 0 or 1 is rb_track_points' step with the flows' roles swapped at pair k: f = s * (sample of
+ * flow_bw[k] at q), q' = q + f, status 2 and NaN unless q' is inside the frame (final), else b = s * (sample of
+ * flow_fw[k] at q') and the same test of f and b.  After the rows, pos / state = row 0 for every query with q0 >= 0.  On
+ * the clip reversed (fw'[k] = flow_bw[T-1-k], bw'[k] = flow_fw[T-1-k]) this is rb_track_points from query frame T - q
+ * with its rows reversed, on the rows up to q, bit for bit.  One thread per query, no atomics, every operation rounded on
+ * its own left to right. */
+int rb_track_points_backward(const float* flow_fw, const float* flow_bw, int T, int H, int W, int n_steps,
+                             float flow_scale, float alpha1, float alpha2, const int32_t* qframe, const float* qpos, int N,
+                             int first_frame, float* pos, uint8_t* state, float* tracks, uint8_t* status, void* stream);
+
 /* ---- F6: frame interpolation -- flow_utils.py:166-274 reverse_flow_avg_skip_static, batched, and the frame blend -----
  * rb_flow_reverse: per sample of flow01 [B,H,W,2] fp32, bit for bit with the reference under numpy >= 2:
  *  1. static(p) = every channel c has d_c < 10, d_c = uint8(bg - im0) (img_u8 = 1: wraps, like numpy's uint8) or

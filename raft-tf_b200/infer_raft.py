@@ -35,6 +35,14 @@ Sintel: ``<out>/<dstype>/<scene>/frameNNNN.flo``; KITTI (no --warm-start): ``<ou
 im2 of every triplet in <data>/tri_testlist.txt is interpolated from im1 and im3 at t = 0.5 (20 iterations, like the
 reference), and the mean PSNR and SSIM of the 8-bit frames against im2 are printed (``Validation Vimeo-90K: PSNR: ...,
 SSIM: ...``) and written with the per-triplet records to ``<--out>/val_vimeo.json`` (no --split test, no --warm-start).
+--dataset tapvid scores point tracking on TAP-Vid instead (raft_b200.tapvid):
+
+    python infer_raft.py -m val --dataset tapvid --data tapvid_davis.pkl --load raft-things.npz [--query-mode strided]
+
+--data is a .pkl file or a directory of .pkl shards; the frames run at 256x256 with 20 iterations, and the mean Average
+Jaccard, fraction of points within 1-16 px and occlusion accuracy are printed (``Validation TAP-Vid (first): AJ: ...``)
+and written with the per-video records to ``<--out>/val_tapvid.json``.  --query-mode first (default) tracks each point
+from its first visible frame, strided from every 5th frame, backward too (no --split test, no --warm-start).
 
 --path DIR (upstream demo.py's flag): the flow of every consecutive pair of DIR's sorted *.png / *.jpg frames, written as
 ``<--out>/flow_<k:06d>.png`` (and ``flow_<k:06d>.flo`` / ``.npy`` under the directories --flo / --npy name), each frame
@@ -67,6 +75,10 @@ through the consecutive flows with a forward-backward check at each step, and ``
 --track-vis DIR also draws the visible points on every frame (raft_b200.video.video_track):
 
     python infer_raft.py --path frames/ --out tracks/ --track points.txt --load raft-things.npz [--track-vis vis/]
+
+--track-backward also follows every point back from its frame to frame 0, so the rows before a query frame hold positions
+and status 0 / 1 / 2 instead of 3; the flow passes over the frames before the last query frame run a second time, in
+reverse order.
 
 --native-frames (with --interpolate, or --path with --interpolate or --input-fps/--fps) writes the interpolated frames,
 and with --path the copied input frames, at the input's own size: the flow is estimated and reversed at the network size,
@@ -127,9 +139,12 @@ def parser():
     p.add_argument('--small', action='store_true')
     p.add_argument('--iters', type=int, default=None,
                    help='extension: GRU iterations (test mode: 20 like the reference; -m val: the protocol\'s 32 / 24)')
-    p.add_argument('--dataset', default=None, choices=['sintel', 'kitti', 'vimeo'],
+    p.add_argument('--dataset', default=None, choices=['sintel', 'kitti', 'vimeo', 'tapvid'],
                    help='-m val: which dataset --data holds (Sintel / KITTI-2015 training sets: flow; Vimeo-90K '
-                        'triplets: frame interpolation)')
+                        'triplets: frame interpolation; TAP-Vid .pkl file or directory of .pkl shards: point tracking)')
+    p.add_argument('--query-mode', default=None, choices=['first', 'strided'],
+                   help="-m val --dataset tapvid: TAP-Vid's query mode (default first: each track from its first visible "
+                        "frame; strided: from every 5th frame, tracked forward and backward)")
     p.add_argument('--dstype', nargs='+', default=['clean', 'final'], choices=['clean', 'final'],
                    help='-m val, Sintel: the passes to evaluate')
     p.add_argument('--workers', type=int, default=4, help='-m val and --path: frame-decoding (and writing) threads')
@@ -176,6 +191,9 @@ def parser():
                    help='extension, with --track-grid: the frame the grid is laid on (default 0)')
     p.add_argument('--track-vis', default=None, metavar='DIR',
                    help='extension, with --track or --track-grid: also write every frame with the visible points drawn')
+    p.add_argument('--track-backward', action='store_true',
+                   help='extension, with --track or --track-grid: also track every point back from its frame to frame 0 '
+                        '(a second flow sweep over the frames before the last query frame)')
     p.add_argument('--upstream', action='store_true',
                    help='extension: weights converted from an official princeton-vl RAFT .pth (raft_b200.convert): RGB '
                         'frames and the upstream numerics (RAFT(..., upstream=True))')
@@ -205,9 +223,10 @@ def main(argv=None):
         if args.batch < 1 or args.workers < 0:
             p.error('--path needs --batch >= 1 and --workers >= 0')
         return run_track(args, p)
-    for flag, given in (('--track-frame', args.track_frame != 0), ('--track-vis', args.track_vis is not None)):
+    for flag, given in (('--track-frame', args.track_frame != 0), ('--track-vis', args.track_vis is not None),
+                        ('--track-backward', args.track_backward)):
         if given:
-            p.error(f'{flag} goes with --track-grid' + (' or --track' if flag == '--track-vis' else ''))
+            p.error(f'{flag} goes with --track-grid' + (' or --track' if flag != '--track-frame' else ''))
     fps = None
     if args.fps is not None or args.input_fps is not None:
         if args.fps is None or args.input_fps is None:
@@ -251,7 +270,7 @@ def main(argv=None):
                     'depend on neighbouring pairs, so a cut changes nothing')
     if args.mode == 'val':
         if not args.data or not args.dataset:
-            p.error('-m val needs --data <dataset root> and --dataset {sintel,kitti,vimeo}')
+            p.error('-m val needs --data <dataset root> and --dataset {sintel,kitti,vimeo,tapvid}')
         if args.warm_start and args.dataset == 'kitti':
             p.error("--warm-start needs frame sequences: KITTI's pairs are not sequences")
         if args.dataset == 'vimeo' and args.split == 'test':
@@ -259,6 +278,14 @@ def main(argv=None):
                     'its test list)')
         if args.dataset == 'vimeo' and args.warm_start:
             p.error("--warm-start needs frame sequences: Vimeo-90K's triplets are not chains")
+        if args.dataset == 'tapvid' and args.split == 'test':
+            p.error('--split test writes a flow submission; TAP-Vid has no hidden-ground-truth split (-m val scores its '
+                    'videos)')
+        if args.dataset == 'tapvid' and args.warm_start:
+            p.error('--warm-start warm-starts flow validation; TAP-Vid tracks points through cold flows')
+    if args.query_mode is not None and (args.mode != 'val' or args.dataset != 'tapvid'):
+        p.error('--query-mode goes with -m val --dataset tapvid')
+    if args.mode == 'val':
         return validate(args)
     if args.mode != 'test':
         print(f"mode '{args.mode}' has no implementation in the reference either (infer_raft.py:71-95); nothing to do")
@@ -382,7 +409,8 @@ def run_track(args, p):
             p.error(f'--track: {e}')
     model = _video_model(args)
     tracks, status = video_track(model, args.path, args.out, queries=queries, grid=args.track_grid,
-                                 grid_frame=args.track_frame, batch=args.batch, workers=args.workers, vis=args.track_vis)
+                                 grid_frame=args.track_frame, batch=args.batch, workers=args.workers, vis=args.track_vis,
+                                 backward=args.track_backward)
     st = np.load(status, mmap_mode='r')
     F, N = st.shape
     print(f"{N} points tracked through {F} frames: {int((st[-1] == 0).sum())} consistent (status 0) in the last frame; "
@@ -422,7 +450,7 @@ def validate(args):
         print(f"{len(files)} flows written under {args.out}")
         return 0
     res = evaluate(model, args.data, args.dataset, dstypes=tuple(args.dstype), batch=args.batch, workers=args.workers,
-                   iters=args.iters, warm_start=args.warm_start)
+                   iters=args.iters, warm_start=args.warm_start, query_mode=args.query_mode)
     for line in summary_lines(res):
         print(line)
     os.makedirs(args.out, exist_ok=True)

@@ -158,16 +158,18 @@ class RAFT(object):
         return tuple(None if t is None else t.clone() for t in out)
 
     @torch.no_grad()
-    def track(self, frames, queries):
+    def track(self, frames, queries, backward=False):
         """Extension (point tracking): where each query point of [F,H,W,3] frames (dtypes and sources as for ``forward``)
         goes in the later frames, and whether it stayed visible.  queries is [N,3] rows (frame, x, y), x and y in the
         frames' own pixels (with input_size too).  One ``forward_sequence_bidirectional`` pass, then every point chained
         through the forward flows with the forward-backward test of ``forward_bidirectional`` at each step
         (RaftEngine.track).  Returns fresh (tracks [F,N,2] fp32, status [F,N] uint8) CUDA tensors: status 0 consistent, 1
         inconsistent (occluded; the position keeps integrating), 2 left the frame (NaN from then on), 3 before the query
-        frame (NaN).  A query frame outside [0, F), a non-finite position or one outside the frame, an empty list or a
-        wrong shape raises ValueError."""
-        return self.engine().track(_as_tensor(frames), queries)
+        frame (NaN).  backward=True also tracks each point back from its frame to frame 0 through the backward flows of
+        the same pass, so the rows before the query frame hold positions and status 0, 1 or 2 (never 3); the rows at and
+        after it are unchanged.  A query frame outside [0, F), a non-finite position or one outside the frame, an empty
+        list or a wrong shape raises ValueError."""
+        return self.engine().track(_as_tensor(frames), queries, backward=bool(backward))
 
     @torch.no_grad()
     def interpolate_sequence(self, frames, t=0.5, uint8=False, bgr=False, native=False):

@@ -57,6 +57,35 @@ def fb_consistency(flow_fw, flow_bw, alpha1=0.01, alpha2=0.5, flow_scale=1.0):
     return occ_fw, occ_bw
 
 
+def _track_args(what, flow_fw, flow_bw, qframe, qpos, state):
+    """The argument checks of track_points and track_points_backward -> (T, H, W, N, qframe, qpos, state) with the
+    queries as contiguous device tensors and state fresh (NaN, 3) when None."""
+    for name, t in (("flow_fw", flow_fw), ("flow_bw", flow_bw)):
+        if not (isinstance(t, torch.Tensor) and t.is_cuda and t.dim() == 4 and t.shape[-1] == 2
+                and t.dtype == torch.float32):
+            raise ValueError(f"{what}: {name} must be a [T,H,W,2] float32 CUDA tensor (got "
+                             f"{getattr(t, 'shape', None)} {getattr(t, 'dtype', type(t))})")
+    if flow_fw.shape != flow_bw.shape or flow_fw.device != flow_bw.device:
+        raise ValueError(f"{what}: flow_fw {tuple(flow_fw.shape)} and flow_bw {tuple(flow_bw.shape)} must match")
+    T, H, W, _ = flow_fw.shape
+    dev = flow_fw.device
+    qframe = torch.as_tensor(qframe).to(device=dev, dtype=torch.int32).contiguous()
+    qpos = torch.as_tensor(qpos).to(device=dev, dtype=torch.float32).contiguous()
+    N = qframe.shape[0] if qframe.dim() == 1 else -1
+    if N < 1 or tuple(qpos.shape) != (N, 2):
+        raise ValueError(f"{what}: qframe must be [N] and qpos [N,2], N >= 1 (got {tuple(qframe.shape)} and "
+                         f"{tuple(qpos.shape)})")
+    if state is None:
+        state = (torch.full((N, 2), float("nan"), dtype=torch.float32, device=dev),
+                 torch.full((N,), 3, dtype=torch.uint8, device=dev))
+    pos, st = state
+    if not (tuple(pos.shape) == (N, 2) and pos.dtype == torch.float32 and tuple(st.shape) == (N,)
+            and st.dtype == torch.uint8 and pos.device == dev and st.device == dev and pos.is_contiguous()
+            and st.is_contiguous()):
+        raise ValueError(f"{what}: state must be contiguous (pos [N,2] float32, state [N] uint8) on {dev}")
+    return T, H, W, N, qframe, qpos, (pos, st)
+
+
 def track_points(flow_fw, flow_bw, qframe, qpos, state=None, first_frame=0, n_steps=None, flow_scale=1.0, alpha1=0.01,
                  alpha2=0.5):
     """Extension (point tracking): N query points chained through the consecutive flows of one pass on the GPU
@@ -67,29 +96,8 @@ def track_points(flow_fw, flow_bw, qframe, qpos, state=None, first_frame=0, n_st
     flow_scale, alpha1, alpha2 as in fb_consistency.  Returns (tracks [n_steps+1,N,2] fp32, status [n_steps+1,N] uint8,
     state): row j is frame first_frame + j; status 0 consistent, 1 inconsistent (occluded; the track goes on), 2 left
     the frame (NaN from then on), 3 before the query frame (NaN)."""
-    for name, t in (("flow_fw", flow_fw), ("flow_bw", flow_bw)):
-        if not (isinstance(t, torch.Tensor) and t.is_cuda and t.dim() == 4 and t.shape[-1] == 2
-                and t.dtype == torch.float32):
-            raise ValueError(f"track_points: {name} must be a [T,H,W,2] float32 CUDA tensor (got "
-                             f"{getattr(t, 'shape', None)} {getattr(t, 'dtype', type(t))})")
-    if flow_fw.shape != flow_bw.shape or flow_fw.device != flow_bw.device:
-        raise ValueError(f"track_points: flow_fw {tuple(flow_fw.shape)} and flow_bw {tuple(flow_bw.shape)} must match")
-    T, H, W, _ = flow_fw.shape
+    T, H, W, N, qframe, qpos, (pos, st) = _track_args("track_points", flow_fw, flow_bw, qframe, qpos, state)
     dev = flow_fw.device
-    qframe = torch.as_tensor(qframe).to(device=dev, dtype=torch.int32).contiguous()
-    qpos = torch.as_tensor(qpos).to(device=dev, dtype=torch.float32).contiguous()
-    N = qframe.shape[0] if qframe.dim() == 1 else -1
-    if N < 1 or tuple(qpos.shape) != (N, 2):
-        raise ValueError(f"track_points: qframe must be [N] and qpos [N,2], N >= 1 (got {tuple(qframe.shape)} and "
-                         f"{tuple(qpos.shape)})")
-    if state is None:
-        state = (torch.full((N, 2), float("nan"), dtype=torch.float32, device=dev),
-                 torch.full((N,), 3, dtype=torch.uint8, device=dev))
-    pos, st = state
-    if not (tuple(pos.shape) == (N, 2) and pos.dtype == torch.float32 and tuple(st.shape) == (N,)
-            and st.dtype == torch.uint8 and pos.device == dev and st.device == dev and pos.is_contiguous()
-            and st.is_contiguous()):
-        raise ValueError(f"track_points: state must be contiguous (pos [N,2] float32, state [N] uint8) on {dev}")
     n_steps = T if n_steps is None else int(n_steps)
     tracks = torch.empty(n_steps + 1, N, 2, dtype=torch.float32, device=dev)
     status = torch.empty(n_steps + 1, N, dtype=torch.uint8, device=dev)
@@ -99,6 +107,38 @@ def track_points(flow_fw, flow_bw, qframe, qpos, state=None, first_frame=0, n_st
                                             float(alpha1), float(alpha2), capi.ptr(qframe), capi.ptr(qpos), N,
                                             int(first_frame), capi.ptr(pos), capi.ptr(st), capi.ptr(tracks),
                                             capi.ptr(status), capi.stream()))
+    return tracks, status, (pos, st)
+
+
+def track_points_backward(flow_fw, flow_bw, qframe, qpos, tracks=None, status=None, state=None, first_frame=0,
+                          n_steps=None, flow_scale=1.0, alpha1=0.01, alpha2=0.5):
+    """Extension (point tracking backward in time): the mirror of track_points (rb_track_points_backward), each query
+    followed from its frame back to the flows' frame 0.  Arguments as for track_points.  tracks [n_steps+1,N,2] fp32 and
+    status [n_steps+1,N] uint8 (contiguous, on the flows' device; e.g. track_points' outputs) are completed in place:
+    rows after a query's frame keep what they hold, the row of its frame becomes (qpos, 0) and the rows before it the
+    backward track.  Without them they start as NaN / 3.  state carries a reverse sweep of calls from later frames to
+    earlier ones: read for a query whose frame lies after the flows' last frame (its row n_steps is the carried state),
+    written with row 0 for every query whose frame is at or after first_frame, untouched for the others.  Returns
+    (tracks, status, state)."""
+    T, H, W, N, qframe, qpos, (pos, st) = _track_args("track_points_backward", flow_fw, flow_bw, qframe, qpos, state)
+    dev = flow_fw.device
+    n_steps = T if n_steps is None else int(n_steps)
+    if tracks is None:
+        tracks = torch.full((n_steps + 1, N, 2), float("nan"), dtype=torch.float32, device=dev)
+    if status is None:
+        status = torch.full((n_steps + 1, N), 3, dtype=torch.uint8, device=dev)
+    if not (tuple(tracks.shape) == (n_steps + 1, N, 2) and tracks.dtype == torch.float32 and tracks.device == dev
+            and tracks.is_contiguous() and tuple(status.shape) == (n_steps + 1, N) and status.dtype == torch.uint8
+            and status.device == dev and status.is_contiguous()):
+        raise ValueError(f"track_points_backward: tracks and status must be contiguous [n_steps+1,N,2] float32 and "
+                         f"[n_steps+1,N] uint8 on {dev} with n_steps + 1 = {n_steps + 1}, N = {N} (got "
+                         f"{tuple(tracks.shape)} {tracks.dtype} and {tuple(status.shape)} {status.dtype})")
+    fw, bw = flow_fw.contiguous(), flow_bw.contiguous()
+    with torch.cuda.device(dev):
+        capi.check(capi.lib.rb_track_points_backward(capi.ptr(fw), capi.ptr(bw), T, H, W, n_steps, float(flow_scale),
+                                                     float(alpha1), float(alpha2), capi.ptr(qframe), capi.ptr(qpos), N,
+                                                     int(first_frame), capi.ptr(pos), capi.ptr(st), capi.ptr(tracks),
+                                                     capi.ptr(status), capi.stream()))
     return tracks, status, (pos, st)
 
 

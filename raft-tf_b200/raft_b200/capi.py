@@ -71,6 +71,7 @@ SIGNATURES = {
     "rb_upflow8_crop": (_i, [_vp, _vp, _i, _i, _i, _f, _i, _i, _i, _i, _vp]),
     "rb_flow_fb_check": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _f, _f, _f, _vp]),
     "rb_track_points": (_i, [_vp, _vp, _i, _i, _i, _i, _f, _f, _f, _vp, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp]),
+    "rb_track_points_backward": (_i, [_vp, _vp, _i, _i, _i, _i, _f, _f, _f, _vp, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp]),
     "rb_flow_reverse_workspace_bytes": (_i, [_i, _i, _i, _psz]),
     "rb_flow_reverse": (_i, [_vp, _vp, _vp, _i, _i, _f, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _vp, _sz, _vp]),
     "rb_frame_synthesize": (_i, [_vp, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _f, _vp, _i, _i, _i, _vp]),

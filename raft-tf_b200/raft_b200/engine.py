@@ -503,23 +503,30 @@ class RaftEngine:
         return self.flow_up[:T], self.flow_bw, self.occ[:T], self.occ[T:]
 
     @torch.no_grad()
-    def track(self, frames: torch.Tensor, queries):
+    def track(self, frames: torch.Tensor, queries, backward: bool = False):
         """Point tracking: queries [N,3] rows (frame, x, y), x and y in the frames' own pixels, followed from their frame
         to the last of the [F,H,W,3] frames (dtypes, sizes and input_size as for forward()).  One
         forward_sequence_bidirectional(check=False) pass, then one rb_track_points launch on its flows (flow_scale as in
         the occlusion check).  With input_size the positions are mapped to the network grid and the tracks back
         (track_queries, tracks_to_frames).  Returns fresh (tracks [F,N,2] fp32, status [F,N] uint8) CUDA tensors in the
         frames' own pixels: status 0 consistent, 1 inconsistent (occluded; the track goes on), 2 left the frame (NaN from
-        then on), 3 before the query frame (NaN).  Bad queries raise ValueError before the pass."""
+        then on), 3 before the query frame (NaN).  Bad queries raise ValueError before the pass.
+
+        backward=True also follows each point from its frame back to frame 0: after the forward launch, one
+        rb_track_points_backward launch on the same flows and buffers fills the rows before each query frame (status 0,
+        1 or 2; 3 no longer occurs).  The rows at and after it are the bits of backward=False."""
         F = _sequence_length(frames) + 1
         src_hw = tuple(frames.shape[1:3])
         net_hw = self.input_size if self.input_size is not None else src_hw
         qframe, qpos = track_queries(queries, F, src_hw, net_hw)
-        from networks.utils import track_points
+        from networks.utils import track_points, track_points_backward
         flow_fw, flow_bw, _, _ = self.forward_sequence_bidirectional(frames, check=False)
         with torch.cuda.device(self.device):
             tracks, status, _ = track_points(flow_fw, flow_bw, qframe, qpos, flow_scale=self.flow_scale,
                                              alpha1=FB_ALPHA1, alpha2=FB_ALPHA2)
+            if backward:
+                track_points_backward(flow_fw, flow_bw, qframe, qpos, tracks, status, flow_scale=self.flow_scale,
+                                      alpha1=FB_ALPHA1, alpha2=FB_ALPHA2)
             return tracks_to_frames(tracks, src_hw, net_hw), status
 
     @torch.no_grad()

@@ -16,6 +16,9 @@ order; im2 is interpolated from im1 and im3 at t = 0.5 (RaftEngine.interpolate, 
 scored by rb_frame_metrics against the uploaded im2 on the same stream -- the predicted frame never leaves the GPU -- into
 per-triplet PSNR and SSIM, reported as their means over the list.
 
+TAP-Vid (F17, raft_b200.tapvid): point tracking scored by Average Jaccard, the fraction of points within 1-16 pixels and
+occlusion accuracy, at 256 x 256 with 20 iterations, in the 'first' or 'strided' query mode.
+
 Pipeline: pairs are grouped by frame size (one CUDA graph per size) and run in batches through RaftEngine.forward, whose
 flow stays on the GPU: rb_flow_metrics scores it against the uploaded ground truth on the same stream and writes per-pair
 stats into one device buffer, read back once per split.  Worker threads decode the next batches (cv2 releases the GIL)
@@ -38,8 +41,9 @@ from . import capi
 from .engine import RaftEngine
 
 # dataset -> (iterations, pad_mode): upstream's validate_sintel / validate_kitti
-PROTOCOLS = {"sintel": (32, "sintel"), "kitti": (24, "kitti"), "vimeo": (20, "sintel")}
+PROTOCOLS = {"sintel": (32, "sintel"), "kitti": (24, "kitti"), "vimeo": (20, "sintel"), "tapvid": (20, "sintel")}
 DSTYPES = ("clean", "final")
+QUERY_MODES = ("first", "strided")  # TAP-Vid's (raft_b200.tapvid)
 STATS = 6  # RB_FLOW_STATS: n, sum of EPE, #(EPE < 1), #(EPE < 3), #(EPE < 5), #outliers
 FRAME_STATS = 2  # RB_FRAME_STATS: SSE, SSIM
 
@@ -402,6 +406,9 @@ def _setup(model, dataset, dstypes, batch, workers, iters, warm_start, what):
     if dataset not in PROTOCOLS:
         raise ValueError(f"dataset must be one of {tuple(PROTOCOLS)} (got {dataset!r})")
     if getattr(model, "input_size", None) is not None:
+        if dataset == "tapvid":
+            raise ValueError(f"{what}: TAP-Vid runs its frames at 256x256 by its protocol; build the model without "
+                             "input_size")
         raise ValueError(f"{what}: frames run at their own size; build the model without input_size")
     if int(batch) < 1 or int(workers) < 0:
         raise ValueError(f"{what}: batch must be >= 1 and workers >= 0 (got {batch}, {workers})")
@@ -410,21 +417,25 @@ def _setup(model, dataset, dstypes, batch, workers, iters, warm_start, what):
         raise ValueError(f"{what}: warm_start needs frame sequences; KITTI's pairs are not sequences")
     if vimeo and warm_start:
         raise ValueError(f"{what}: warm_start needs frame sequences; Vimeo-90K's triplets are not chains")
+    if dataset == "tapvid" and warm_start:
+        raise ValueError(f"{what}: warm_start warm-starts flow validation; TAP-Vid tracks points through cold flows")
     if model._params is None:
         raise RuntimeError(f"RAFT.load(<npz>) must be called before {what}")
-    splits = ("kitti",) if kitti else ("vimeo",) if vimeo else tuple(dstypes)
-    if not kitti and not vimeo and (not splits or any(d not in DSTYPES for d in splits)):
+    splits = ("kitti",) if kitti else ("vimeo",) if vimeo else ("tapvid",) if dataset == "tapvid" else tuple(dstypes)
+    if dataset == "sintel" and (not splits or any(d not in DSTYPES for d in splits)):
         raise ValueError(f"Sintel dstypes must be a non-empty subset of {DSTYPES} (got {dstypes!r})")
     n_iters, pad_mode = PROTOCOLS[dataset]
     return kitti, splits, n_iters if iters is None else int(iters), pad_mode
 
 
-def _engine(model, n_iters, pad_mode):
+def _engine(model, n_iters, pad_mode, input_size=None):
     return RaftEngine(model._params, small=model.small, iters=n_iters, device=model.device, volume_free=model.volume_free,
-                      upstream=model.upstream, mixed_precision=model.mixed_precision, pad_mode=pad_mode)
+                      upstream=model.upstream, mixed_precision=model.mixed_precision, pad_mode=pad_mode,
+                      input_size=input_size)
 
 
-def evaluate(model, root, dataset="sintel", dstypes=DSTYPES, batch=1, workers=4, iters=None, warm_start=False):
+def evaluate(model, root, dataset="sintel", dstypes=DSTYPES, batch=1, workers=4, iters=None, warm_start=False,
+             query_mode=None):
     """Upstream RAFT's validation of a loaded networks.RAFT.RAFT model on a Sintel or KITTI-2015 training tree, or the
     interpolation quality on a Vimeo-90K triplet tree (dataset 'vimeo').
 
@@ -440,8 +451,25 @@ def evaluate(model, root, dataset="sintel", dstypes=DSTYPES, batch=1, workers=4,
 
     vimeo: im2 of every triplet of vimeo_triplets(root) interpolated from im1 and im3 at t = 0.5 and scored on the GPU
     (rb_frame_metrics: PSNR of the 8-bit frame the CLI would write, SSIM as skimage's Gaussian-window form); the split
-    'vimeo' holds aggregate_vimeo(...).  dstypes is ignored and warm_start raises ValueError."""
+    'vimeo' holds aggregate_vimeo(...).  dstypes is ignored and warm_start raises ValueError.
+
+    tapvid: root is a TAP-Vid .pkl file or a directory of .pkl shards, scored in query_mode 'first' (the default) or
+    'strided' at 256 x 256 (raft_b200.tapvid: the engine resizes the frames on the GPU); returns {"dataset", "iters",
+    "query_mode", "resolution": [256, 256], "splits": {"tapvid": aggregate_tapvid(...)}}.  dstypes and workers are
+    ignored, warm_start raises ValueError, and query_mode is refused for the other datasets."""
+    if query_mode is not None and dataset != "tapvid":
+        raise ValueError(f"evaluate: query_mode belongs to TAP-Vid's point tracking (got dataset {dataset!r})")
+    if dataset == "tapvid" and query_mode not in (None,) + QUERY_MODES:
+        raise ValueError(f"evaluate: query_mode must be one of {QUERY_MODES} (got {query_mode!r})")
     kitti, splits, n_iters, pad_mode = _setup(model, dataset, dstypes, batch, workers, iters, warm_start, "evaluate")
+    if dataset == "tapvid":
+        from . import tapvid
+        mode = "first" if query_mode is None else query_mode
+        tapvid.tapvid_files(root)  # the files checked up front
+        engine = _engine(model, n_iters, pad_mode, input_size=tapvid.SIZE)
+        records = tapvid.run(engine, root, mode, int(batch), model.upstream)
+        return {"dataset": dataset, "iters": n_iters, "query_mode": mode, "resolution": list(tapvid.SIZE),
+                "splits": {"tapvid": tapvid.aggregate_tapvid(records)}}
     if dataset == "vimeo":
         trips = vimeo_triplets(root)  # every file checked up front
         engine = _engine(model, n_iters, pad_mode)
@@ -510,6 +538,8 @@ def submit(model, root, dataset, out, dstypes=DSTYPES, batch=1, workers=4, iters
     from flow_utils import write_flo, write_kitti_flow
     if dataset == "vimeo":
         raise ValueError("submit: Vimeo-90K has no test split with hidden ground truth; evaluate scores its test list")
+    if dataset == "tapvid":
+        raise ValueError("submit: TAP-Vid has no test split with hidden ground truth; evaluate scores its videos")
     kitti, splits, n_iters, pad_mode = _setup(model, dataset, dstypes, batch, workers, iters, warm_start, "submit")
     lists = {s: kitti_test_pairs(root) if kitti else sintel_test_pairs(root, s) for s in splits}
     engine = _engine(model, n_iters, pad_mode)
@@ -530,7 +560,13 @@ def submit(model, root, dataset, out, dstypes=DSTYPES, batch=1, workers=4, iters
 
 def summary_lines(res):
     """upstream evaluate.py's lines: 'Validation (clean) EPE: ..., 1px: ..., 3px: ..., 5px: ...' per Sintel pass,
-    'Validation KITTI: <epe>, <f1>'; and for Vimeo-90K 'Validation Vimeo-90K: PSNR: ..., SSIM: ...'."""
+    'Validation KITTI: <epe>, <f1>'; for Vimeo-90K 'Validation Vimeo-90K: PSNR: ..., SSIM: ...'; and for TAP-Vid
+    'Validation TAP-Vid (<query mode>): AJ: ..., <δ_avg>: ..., OA: ...'."""
+    if res["dataset"] == "tapvid":
+        r = res["splits"]["tapvid"]
+        return ["Validation TAP-Vid (%s): AJ: %f, <δ_avg>: %f, OA: %f" % (res["query_mode"], r["average_jaccard"],
+                                                                          r["average_pts_within_thresh"],
+                                                                          r["occlusion_accuracy"])]
     if res["dataset"] == "vimeo":
         r = res["splits"]["vimeo"]
         return ["Validation Vimeo-90K: PSNR: %f, SSIM: %f" % (r["psnr"], r["ssim"])]

@@ -543,7 +543,7 @@ def track_colors(N):
     return np.random.default_rng(0).integers(40, 256, size=(N, 3)).astype(np.uint8)
 
 
-def video_track(model, frames, out, queries=None, grid=None, grid_frame=0, batch=8, workers=4, vis=None):
+def video_track(model, frames, out, queries=None, grid=None, grid_frame=0, batch=8, workers=4, vis=None, backward=False):
     """Point tracking through a video of any length with a loaded networks.RAFT.RAFT model: the frames (a directory's
     sorted *.png / *.jpg, or a list of paths, all of one size) and the query points as `queries` ([N,3] rows (frame, x,
     y) in the frames' own pixels) or `grid` = STEP (track_grid() on frame grid_frame; give exactly one).  Every pass runs
@@ -553,9 +553,17 @@ def video_track(model, frames, out, queries=None, grid=None, grid_frame=0, batch
     streamed into them through memory maps, so host memory does not grow with F.  vis (a directory) also writes every
     frame at its own size as <vis>/frame_<i:06d>.png with each point of status 0 drawn as a dot in its own colour
     (track_colors()).  The files are the same bytes for every batch and workers value, and equal RAFT.track on the whole
-    clip.  Frames go in RGB with model.upstream and BGR otherwise, like the CLI.  Returns (tracks path, status path)."""
+    clip.  Frames go in RGB with model.upstream and BGR otherwise, like the CLI.  Returns (tracks path, status path).
+
+    backward=True also tracks every point back from its frame to frame 0 (RAFT.track(backward=True)).  After the forward
+    sweep a reverse sweep runs the same passes again, last to first, each followed by one rb_track_points_backward launch
+    (networks.utils.track_points_backward) that carries the points from later passes to earlier ones; only the passes
+    whose first frame lies before the largest query frame run, so a grid on frame 0 costs nothing more.  The entries
+    (f, i) with f before point i's frame are merged into the memory maps, and with vis the frames before the largest
+    query frame are drawn in the reverse sweep from the merged rows.  The flow passes of the reverse sweep are computed a
+    second time: that is the price of streaming a clip of any length without keeping its flows."""
     import cv2
-    from networks.utils import track_points
+    from networks.utils import track_points, track_points_backward
     from .engine import FB_ALPHA1, FB_ALPHA2, track_queries, tracks_to_frames
 
     paths = list_frames(frames)
@@ -573,6 +581,17 @@ def video_track(model, frames, out, queries=None, grid=None, grid_frame=0, batch
     rgb = bool(model.upstream)
     dev = engine.device
     files = (os.path.join(out, "tracks.npy"), os.path.join(out, "status.npy"))
+    kw = dict(flow_scale=engine.flow_scale, alpha1=FB_ALPHA1, alpha2=FB_ALPHA2)
+
+    def draw(f, img, tr, st):  # frame f with the points of status 0 of its rows tr, st
+        img = cv2.cvtColor(img, cv2.COLOR_RGB2BGR) if rgb else img.copy()
+        seen = np.flatnonzero(st == 0)
+        xy = np.rint(tr[seen]).astype(np.int64)
+        for i, (x, y) in zip(seen, xy):
+            cv2.circle(img, (int(x), int(y)), 2, colors[i].tolist(), -1)
+        name = os.path.join(vis, f"frame_{f:06d}.png")
+        if not cv2.imwrite(name, img):
+            raise OSError(f"cannot write {name}")
 
     def write(slot, first, rows, imgs):  # writer thread: the rows of one pass, once its copies have landed
         slot.event.synchronize()
@@ -581,16 +600,22 @@ def video_track(model, frames, out, queries=None, grid=None, grid_frame=0, batch
         if vis is None:
             return
         for r in rows:
-            img = cv2.cvtColor(imgs[r], cv2.COLOR_RGB2BGR) if rgb else imgs[r].copy()
-            seen = np.flatnonzero(slot.status[r].numpy() == 0)
-            xy = np.rint(slot.tracks[r].numpy()[seen]).astype(np.int64)
-            for i, (x, y) in zip(seen, xy):
-                cv2.circle(img, (int(x), int(y)), 2, colors[i].tolist(), -1)
-            name = os.path.join(vis, f"frame_{first + r:06d}.png")
-            if not cv2.imwrite(name, img):
-                raise OSError(f"cannot write {name}")
+            if first + r >= vis_from:  # with backward, the frames before vis_from are drawn by the reverse sweep
+                draw(first + r, imgs[r], slot.tracks[r].numpy(), slot.status[r].numpy())
+
+    def merge(slot, first, rows, imgs):  # writer thread, reverse sweep: the entries before each point's frame
+        slot.event.synchronize()
+        for r in rows:
+            f = first + r
+            before = f < qf
+            tr, st = tracks_mm[f], status_mm[f]
+            tr[before] = slot.tracks[r].numpy()[before]
+            st[before] = slot.status[r].numpy()[before]
+            if vis is not None:
+                draw(f, imgs[r], tr, st)
 
     state = tracks_mm = status_mm = None
+    vis_from = 0
     try:
         with _Pipeline(paths, passes, rgb, batch, workers, dev) as pipe:
             for j, ps, imgs, frames in pipe:
@@ -601,6 +626,7 @@ def video_track(model, frames, out, queries=None, grid=None, grid_frame=0, batch
                     qf, qp = track_queries(q, F, src_hw, net_hw)
                     qframe, qpos = torch.from_numpy(qf).to(dev), torch.from_numpy(qp).to(dev)
                     N = len(qf)
+                    vis_from = int(qf.max()) if backward else 0
                     colors = track_colors(N) if vis is not None else None
                     tracks_mm = np.lib.format.open_memmap(files[0], mode="w+", dtype=np.float32, shape=(F, N, 2))
                     status_mm = np.lib.format.open_memmap(files[1], mode="w+", dtype=np.uint8, shape=(F, N))
@@ -608,11 +634,25 @@ def video_track(model, frames, out, queries=None, grid=None, grid_frame=0, batch
                 n_steps = sum(k is not None for k in ps.pairs)
                 first = ps.frames[0]
                 tracks, status, state = track_points(flow_fw, flow_bw, qframe, qpos, state=state, first_frame=first,
-                                                     n_steps=n_steps, flow_scale=engine.flow_scale, alpha1=FB_ALPHA1,
-                                                     alpha2=FB_ALPHA2)
+                                                     n_steps=n_steps, **kw)
                 rows = range(0 if j == 0 else 1, n_steps + 1)  # row 0 of a later pass is the last row of the one before
                 pipe.emit(partial(write, first=first, rows=rows, imgs=imgs), T + 1,
                           tracks=tracks_to_frames(tracks, src_hw, net_hw), status=status)
+        # the reverse sweep: the passes before the largest query frame, last to first; each owns its rows below its last
+        # (the row of the last frame of the latest such pass lies at or after every query frame: nothing to merge there)
+        reverse = [ps for ps in passes if ps.frames[0] < vis_from][::-1]
+        if reverse:
+            state = None
+            with _Pipeline(paths, reverse, rgb, batch, workers, dev) as pipe:
+                for j, ps, imgs, frames in pipe:
+                    flow_fw, flow_bw, _, _ = engine.forward_sequence_bidirectional(frames, check=False)
+                    n_steps = sum(k is not None for k in ps.pairs)
+                    first = ps.frames[0]
+                    tracks, status, state = track_points_backward(flow_fw, flow_bw, qframe, qpos, state=state,
+                                                                  first_frame=first, n_steps=n_steps, **kw)
+                    rows = range(0, min(n_steps, vis_from - first))
+                    pipe.emit(partial(merge, first=first, rows=rows, imgs=imgs), T + 1,
+                              tracks=tracks_to_frames(tracks, src_hw, net_hw), status=status)
     finally:
         for mm in (tracks_mm, status_mm):
             if mm is not None:

@@ -11,7 +11,9 @@
    The first launch is checked against tests/track_oracle.py bit for bit.
 2. video_track: end to end (decode, upload, bidirectional flow, tracking, memory-mapped writes) on a seeded synthetic
    24-frame 436x1024 pan as PNG files, batch 8, 4 workers, 1 024 sparse queries and a grid of every 4th pixel; host clock
-   around each call, which returns after its last write; median of `--steps` runs per query set.
+   around each call, which returns after its last write; median of `--steps` runs per query set.  The cost of
+   video_track(backward=True): 1 024 sparse queries on random frames, the largest query frame the last one, so the reverse
+   sweep re-runs every flow pass; timed like the others with backward=False and backward=True, in alternation.
 3. flow only: forward_sequence_bidirectional(check=False) alone on the same clip's passes (frames already on the
    device), the same passes video_track runs; CUDA events around all passes, median of `--steps`.
 
@@ -141,6 +143,30 @@ def main(argv=None):
                               "s_per_clip": t, "ms_per_frame": t * 1e3 / N_CLIP, "runs_s": times,
                               "status_counts_last_frame": [int((st[-1] == k).sum()) for k in range(4)], **ctx}),
                   flush=True)
+        spread = np.concatenate([rng.integers(0, N_CLIP, (N_SPARSE, 1)), sparse.astype(np.float64)], -1)
+        spread[-1, 0] = N_CLIP - 1  # the largest query frame is the last frame: the reverse sweep runs every pass
+        times = {False: [], True: []}
+        for i in range(args.steps + 1):
+            for backward in (False, True):
+                out = os.path.join(tmp, "out")
+                shutil.rmtree(out, ignore_errors=True)
+                torch.cuda.synchronize()
+                t0 = time.perf_counter()
+                video_track(model, d, out, queries=spread, batch=T, workers=4, backward=backward)
+                torch.cuda.synchronize()
+                if i:
+                    times[backward].append(time.perf_counter() - t0)
+        st = np.load(os.path.join(tmp, "out", "status.npy"))
+        fwd, both = statistics.median(times[False]), statistics.median(times[True])
+        print(json.dumps({"benchmark": "video_track_backward", "queries": "spread", "N": N_SPARSE,
+                          "largest_query_frame": N_CLIP - 1,
+                          "workload": f"video_track with and without backward=True, raft-things {H_IMG}x{W_IMG}, "
+                                      f"{ITERS} iterations, {N_CLIP}-frame seeded synthetic pan as PNG files, batch {T}, "
+                                      f"4 workers, queries on random frames",
+                          "s_per_clip_forward": fwd, "s_per_clip_backward": both, "ratio": both / fwd,
+                          "runs_forward_s": times[False], "runs_backward_s": times[True],
+                          "status_counts_first_frame": [int((st[0] == k).sum()) for k in range(4)], **ctx}),
+              flush=True)
         engine = model.engine()
         passes = interp_schedule(N_CLIP, T)
         clips = [torch.from_numpy(np.stack([pan[i] for i in p.frames])).to(dev) for p in passes]
