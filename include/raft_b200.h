@@ -304,6 +304,47 @@ int rb_track_points_backward(const float* flow_fw, const float* flow_bw, int T, 
                              float flow_scale, float alpha1, float alpha2, const int32_t* qframe, const float* qpos, int N,
                              int first_frame, float* pos, uint8_t* state, float* tracks, uint8_t* status, void* stream);
 
+/* ---- F18: flow accumulation -- per pixel of every frame, the displacement back to a keyframe ---------------------
+ * flow_fw, flow_bw: [T,H,W,2] fp32 as for rb_track_points (flow_fw[j] frame j -> j+1, flow_bw[j] j+1 -> j); the first
+ * n_steps (1 <= n_steps <= T) pairs are used.  acc [n_steps+1,H,W,2] fp32: row r holds, per pixel of frame r, the
+ * displacement to the keyframe; status [n_steps+1,H,W] uint8: 0 consistent at every step back to the keyframe, 1
+ * inconsistent (occluded) at some step, 2 entered through the frame edge at some step (the larger value wins).  Row
+ * `start` (0 <= start <= n_steps) is the input state (zeros for the keyframe; the previous pass's last row for a later
+ * pass).  rb_flow_accumulate writes rows start+1 .. n_steps, rb_flow_accumulate_backward rows start-1 .. 0; no other
+ * row is touched.  Forward step r-1 -> r at pixel p = (x, y), s = flow_scale:
+ *   f = s * flow_bw[r-1][p], q = p + f (rb_flow_fb_check's f and q);
+ *   q inside [0, W-1] x [0, H-1]: d = f, step = the F5 test of f and s * (bilinear sample of flow_fw[r-1] at q);
+ *   otherwise: qc = q clamped into the frame (fminf / fmaxf: NaN -> 0; replicate border), d = qc - p, step = 2;
+ *   acc[r][p] = d + (bilinear sample of acc[r-1] at qc, no scale), componentwise;
+ *   status[r][p] = max(step, status[r-1] at qc's nearest tap: x1 if ax > 0.5 else x0, rows likewise).
+ * The backward entry is the mirror (step r+1 -> r: f from flow_fw[r], the test against flow_bw[r], row r+1 sampled):
+ * on the clip reversed (fw'[k] = flow_bw[T-1-k], bw'[k] = flow_fw[T-1-k]) it is the forward entry bit for bit.  Every
+ * operation is rounded on its own, left to right; one launch per step on the stream, no atomics, no allocation.  Null
+ * pointers, T/H/W <= 0, H*W >= 2^31, n_steps outside [1, T], start outside [0, n_steps], flow_scale <= 0 or non-finite,
+ * negative or non-finite alphas -> RB_ERR_* before any CUDA call. */
+int rb_flow_accumulate(const float* flow_fw, const float* flow_bw, int T, int H, int W, int n_steps, float flow_scale,
+                       float alpha1, float alpha2, int start, float* acc, uint8_t* status, void* stream);
+int rb_flow_accumulate_backward(const float* flow_fw, const float* flow_bw, int T, int H, int W, int n_steps,
+                                float flow_scale, float alpha1, float alpha2, int start, float* acc, uint8_t* status,
+                                void* stream);
+
+/* ---- F19: label propagation -- the keyframe's labels pulled along F18's displacements -----------------------------
+ * acc [n,H,W,2] fp32 and status [n,H,W] uint8 (F18's rows) at the network size; key [Hs,Ws] uint8 the keyframe's label
+ * map at the frames' own size; labels, status_out [n,Hs,Ws] uint8.  Per output pixel p = (x, y) of row i:
+ *   A' = rb_flow_resize's value of acc[i] at p (cv2's float bilinear resize, a copy when H x W = Hs x Ws, then
+ *        u *= fl32(Ws / W), v *= fl32(Hs / H));
+ *   o  = p + A', clamped into [0, Ws-1] x [0, Hs-1];
+ *   status_out = status[i] at the network pixel holding p's centre (rb_frame_synthesize_*_resized's `nearest`), 2 if
+ *        the clamp moved o (or o is NaN);
+ *   labels = the vote of o's four bilinear taps of key (x0 = floor(o.x), x1 = min(x0+1, Ws-1), ax = o.x - x0, rows
+ *        likewise) with weights (1-ax)(1-ay), ax(1-ay), (1-ax)ay, ax ay: each distinct label scores the sum of its taps'
+ *        weights in tap order 00, 01, 10, 11, the largest score wins and a tie goes to the smaller label.
+ * Labels never blend into ids that do not exist, an integer displacement copies exactly, and a zero row reproduces key.
+ * One thread per output pixel, blockIdx.y over the rows; no allocation.  Null pointers, n/H/W/Hs/Ws <= 0 and Hs*Ws >=
+ * 2^32 -> RB_ERR_* before any CUDA call. */
+int rb_labels_propagate(const float* acc, const uint8_t* status, int n, int H, int W, const uint8_t* key, int Hs, int Ws,
+                        uint8_t* labels, uint8_t* status_out, void* stream);
+
 /* ---- F6: frame interpolation -- flow_utils.py:166-274 reverse_flow_avg_skip_static, batched, and the frame blend -----
  * rb_flow_reverse: per sample of flow01 [B,H,W,2] fp32, bit for bit with the reference under numpy >= 2:
  *  1. static(p) = every channel c has d_c < 10, d_c = uint8(bg - im0) (img_u8 = 1: wraps, like numpy's uint8) or
@@ -503,6 +544,22 @@ int rb_flow_to_color(const float* flow, int B, int H, int W, int clip, float cli
 int rb_frame_metrics_workspace_bytes(int B, int H, int W, size_t* bytes);
 int rb_frame_metrics(const void* pred, int pred_is_u8, const uint8_t* gt, int B, int H, int W, double* stats,
                      void* workspace, size_t workspace_bytes, void* stream);
+
+/* ---- F20: label metrics -- DAVIS-2017's J (region) and F (boundary) as integer counts ----------------------------
+ * pred, gt: [n,H,W] uint8 label maps.  counts: [n][n_objects][RB_LABEL_STATS] int64, zeroed by the call on the stream.
+ * For frame i and object o = 1..n_objects, with P = (pred == o) and G = (gt == o):
+ *   {|P and G|, |P or G|, #boundary(P), #boundary(G), #(boundary(P) with a boundary(G) pixel in the disk),
+ *    #(boundary(G) with a boundary(P) pixel in the disk)}.
+ * boundary is davis2017-evaluation's _seg2bmap at the map's own size: b = (m ^ e) | (m ^ s) | (m ^ se), e / s / se the
+ * right / down / down-right neighbours (0 outside the image), the last row m ^ e, the last column m ^ s, the last pixel
+ * 0.  The disk is skimage.morphology.disk(bound_pix), the offsets with dx^2 + dy^2 <= bound_pix^2; pixels outside the
+ * image never match (cv2.dilate's default border).  Tiles of 32 x 32 pixels with a halo of bound_pix + 1 in shared
+ * memory; block counts reach global memory through 64-bit integer atomics, so they are exact and deterministic.  Null
+ * pointers, n/H/W <= 0, n > 65535, n_objects outside [1, 255] and bound_pix outside [1, 32] -> RB_ERR_* before any CUDA
+ * call.  DAVIS's bound_pix = ceil(0.008 * hypot(H, W)): 8 at 480p, 18 at 1080p. */
+#define RB_LABEL_STATS 6
+int rb_label_metrics(const uint8_t* pred, const uint8_t* gt, int n, int H, int W, int n_objects, int bound_pix,
+                     int64_t* counts, void* stream);
 
 /* ---- F15: scene-cut scores -- where frame-rate conversion and warm-started video flow stop ------------------------
  * frames: [N,H,W,3] uint8, the decoded frames at their own size (any channel order: the bins are symmetric in it).

@@ -212,6 +212,128 @@ static size_t frame_metrics_tiles(int H, int W) {
   return (size_t)((W + kFmTileW - 1) / kFmTileW) * (size_t)((H + kFmTileH - 1) / kFmTileH);
 }
 
+// ---- F20: label metrics (DAVIS-2017's region similarity J and boundary accuracy F, as integer counts) -----------------
+// One block per (kLmTile x kLmTile output tile, frame).  Both label maps are staged with a halo of R = r + 1 (r =
+// bound_pix); per object present in the staged labels, the _seg2bmap boundaries of P = (pred == o) and G = (gt == o) are
+// computed for the tile plus a halo of r (bit 0: P, bit 1: G; 0 outside the image), then every pixel of the tile adds
+// its counts; a boundary pixel searches the disk dx^2 + dy^2 <= r^2 for the other map's boundary.  The block's counts go
+// to global memory with one 64-bit integer atomic per (object, count): exact, so the result does not depend on the order.
+constexpr int kLmTile = 32;
+constexpr int kLmThreads = 256;
+constexpr int kLmMaxR = 32;
+
+__device__ __forceinline__ uint8_t lm_bit(const uint8_t* lab, int ls, int r, int c, uint8_t o) {
+  return lab[r * ls + c] == o;
+}
+
+__global__ void __launch_bounds__(kLmThreads) label_metrics_kernel(const uint8_t* __restrict__ pred,
+                                                                   const uint8_t* __restrict__ gt, int H, int W,
+                                                                   int tiles_x, int n_objects, int rad,
+                                                                   unsigned long long* __restrict__ counts) {
+  extern __shared__ uint8_t lm_smem[];
+  __shared__ unsigned present[2][8];  // the labels of the staged pred / gt as 256-bit sets
+  __shared__ int half[kLmMaxR + 1];   // half[|dy|] = the largest dx with dx^2 + dy^2 <= r^2
+  __shared__ unsigned long long red[RB_LABEL_STATS];
+  const int t = threadIdx.x, f = blockIdx.y;
+  const int R = rad + 1, ls = kLmTile + 2 * R, bs = kLmTile + 2 * rad;
+  uint8_t* sp = lm_smem;
+  uint8_t* sg = sp + ls * ls;
+  uint8_t* bm = sg + ls * ls;
+  const int x0 = (int)(blockIdx.x % tiles_x) * kLmTile, y0 = (int)(blockIdx.x / tiles_x) * kLmTile;
+  if (t < 16) present[t / 8][t % 8] = 0;
+  if (t <= rad) {
+    int h = 0;
+    while ((h + 1) * (h + 1) + t * t <= rad * rad) ++h;
+    half[t] = h;
+  }
+  __syncthreads();
+  const size_t base = (size_t)f * H * W;
+  for (int e = t; e < ls * ls; e += kLmThreads) {
+    const int y = y0 - R + e / ls, x = x0 - R + e % ls;
+    uint8_t p = 0, g = 0;
+    if (y >= 0 && y < H && x >= 0 && x < W) {
+      p = pred[base + (size_t)y * W + x];
+      g = gt[base + (size_t)y * W + x];
+      atomicOr(&present[0][p >> 5], 1u << (p & 31));
+      atomicOr(&present[1][g >> 5], 1u << (g & 31));
+    }
+    sp[e] = p;
+    sg[e] = g;
+  }
+  __syncthreads();
+  for (int o = 1; o <= n_objects; ++o) {
+    if (!((present[0][o >> 5] | present[1][o >> 5]) >> (o & 31) & 1u)) continue;  // the same in every thread
+    const uint8_t ob = (uint8_t)o;
+    // boundaries of the tile plus a halo of r: b = (m ^ e) | (m ^ s) | (m ^ se), e / s / se 0 outside the image;
+    // the last row m ^ e, the last column m ^ s, the last pixel 0
+    for (int e = t; e < bs * bs; e += kLmThreads) {
+      const int br = e / bs, bc = e % bs, y = y0 - rad + br, x = x0 - rad + bc;
+      uint8_t v = 0;
+      if (y >= 0 && y < H && x >= 0 && x < W) {
+        const int r = br + 1, c = bc + 1;  // in the staged labels
+        const bool last_r = y == H - 1, last_c = x == W - 1;
+#pragma unroll
+        for (int k = 0; k < 2; ++k) {
+          const uint8_t* lab = k ? sg : sp;
+          const uint8_t m = lm_bit(lab, ls, r, c, ob);
+          const uint8_t me = last_c ? 0 : lm_bit(lab, ls, r, c + 1, ob);
+          const uint8_t ms = last_r ? 0 : lm_bit(lab, ls, r + 1, c, ob);
+          const uint8_t mse = (last_r || last_c) ? 0 : lm_bit(lab, ls, r + 1, c + 1, ob);
+          uint8_t b;
+          if (last_r && last_c) b = 0;
+          else if (last_r) b = m ^ me;
+          else if (last_c) b = m ^ ms;
+          else b = (m ^ me) | (m ^ ms) | (m ^ mse);
+          v |= b << k;
+        }
+      }
+      bm[e] = v;
+    }
+    if (t < RB_LABEL_STATS) red[t] = 0;
+    __syncthreads();
+    unsigned c[RB_LABEL_STATS] = {0, 0, 0, 0, 0, 0};
+    for (int e = t; e < kLmTile * kLmTile; e += kLmThreads) {
+      const int i = e / kLmTile, j = e % kLmTile, y = y0 + i, x = x0 + j;
+      if (y >= H || x >= W) continue;
+      const bool P = sp[(i + R) * ls + j + R] == ob, G = sg[(i + R) * ls + j + R] == ob;
+      c[0] += P && G;
+      c[1] += P || G;
+      const uint8_t v = bm[(i + rad) * bs + j + rad];
+#pragma unroll
+      for (int k = 0; k < 2; ++k) {
+        if (!(v >> k & 1)) continue;
+        ++c[2 + k];
+        const uint8_t other = (uint8_t)(2 >> k);  // P's boundary looks for G's and G's for P's
+        bool hit = false;
+        for (int dy = -rad; dy <= rad && !hit; ++dy) {
+          const int h = half[dy < 0 ? -dy : dy];
+          const uint8_t* row = bm + (i + rad + dy) * bs + j + rad;
+          for (int dx = -h; dx <= h; ++dx)
+            if (row[dx] & other) {
+              hit = true;
+              break;
+            }
+        }
+        c[4 + k] += hit;
+      }
+    }
+#pragma unroll
+    for (int k = 0; k < RB_LABEL_STATS; ++k) {
+      unsigned v = c[k];
+      for (int s = 16; s > 0; s >>= 1) v += __shfl_down_sync(0xffffffffu, v, s);
+      if ((t & 31) == 0 && v) atomicAdd(&red[k], (unsigned long long)v);
+    }
+    __syncthreads();
+    if (t < RB_LABEL_STATS && red[t]) atomicAdd(&counts[((size_t)f * n_objects + (o - 1)) * RB_LABEL_STATS + t], red[t]);
+    __syncthreads();  // bm and red are rewritten by the next object
+  }
+}
+
+static size_t label_metrics_smem(int rad) {
+  const size_t ls = kLmTile + 2 * (rad + 1), bs = kLmTile + 2 * rad;
+  return 2 * ls * ls + bs * bs;
+}
+
 }  // namespace rb
 
 using namespace rb;
@@ -283,5 +405,25 @@ extern "C" int rb_frame_metrics(const void* pred, int pred_is_u8, const uint8_t*
   const double n_crop = 3.0 * (double)(H - 2 * kFmR) * (double)(W - 2 * kFmR);
   frame_metrics_sample_kernel<<<B, kMetricsThreads, 0, st>>>(partials, (int)tiles, n_crop, stats);
   RB_CHECK_LAUNCH("frame_metrics_sample_kernel");
+  return RB_OK;
+}
+
+extern "C" int rb_label_metrics(const uint8_t* pred, const uint8_t* gt, int n, int H, int W, int n_objects,
+                                int bound_pix, int64_t* counts, void* stream) {
+  RB_REQUIRE(pred && gt && counts, RB_ERR_BAD_ARG, "rb_label_metrics: null pointer");
+  RB_REQUIRE(n > 0 && H > 0 && W > 0, RB_ERR_BAD_SHAPE, "rb_label_metrics: bad shape n=%d H=%d W=%d", n, H, W);
+  RB_REQUIRE(n_objects >= 1 && n_objects <= 255, RB_ERR_BAD_ARG, "rb_label_metrics: n_objects must be in [1, 255] (got %d)",
+             n_objects);
+  RB_REQUIRE(bound_pix >= 1 && bound_pix <= kLmMaxR, RB_ERR_BAD_ARG,
+             "rb_label_metrics: bound_pix must be in [1, %d] (got %d)", kLmMaxR, bound_pix);
+  const size_t tiles = (size_t)((W + kLmTile - 1) / kLmTile) * (size_t)((H + kLmTile - 1) / kLmTile);
+  RB_REQUIRE(n <= 65535 && tiles <= 0x7fffffffu, RB_ERR_BAD_SHAPE,
+             "rb_label_metrics: n=%d frames of %dx%d pixels exceed one grid", n, H, W);
+  const cudaStream_t st = (cudaStream_t)stream;
+  RB_CHECK_CUDA(cudaMemsetAsync(counts, 0, (size_t)n * n_objects * RB_LABEL_STATS * sizeof(int64_t), st));
+  label_metrics_kernel<<<dim3((unsigned)tiles, (unsigned)n), kLmThreads, label_metrics_smem(bound_pix), st>>>(
+      pred, gt, H, W, (W + kLmTile - 1) / kLmTile, n_objects, bound_pix,
+      reinterpret_cast<unsigned long long*>(counts));
+  RB_CHECK_LAUNCH("label_metrics_kernel");
   return RB_OK;
 }

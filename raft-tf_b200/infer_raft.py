@@ -80,6 +80,18 @@ through the consecutive flows with a forward-backward check at each step, and ``
 and status 0 / 1 / 2 instead of 3; the flow passes over the frames before the last query frame run a second time, in
 reverse order.
 
+--path DIR --propagate KEY.png [--propagate-frame K] carries the label map of frame K (default 0; a palette or 8-bit
+grey PNG at the frames' own size: a segmentation mask, a class map) to every frame of DIR: per pixel of every frame, the
+displacement back to frame K is composed through the consecutive flows on the GPU and the key's label there taken by a
+vote of its four nearest pixels.  ``<--out>/label_<i:06d>.png`` is written for every frame, in the key's palette
+(raft_b200.video.video_propagate):
+
+    python infer_raft.py --path frames/ --out labels/ --propagate key.png --load raft-things.npz [--batch 8]
+
+-m val --dataset davis scores it on DAVIS-2017's val split (raft_b200.davis): frame 0's annotation of every sequence
+propagated at 480p with 20 iterations, J&F printed (``Validation DAVIS-2017 (val): J&F: ...``) and written to
+``<--out>/val_davis.json``, the predicted masks to ``<--out>/davis_val/<seq>/`` in DAVIS's results layout.
+
 --native-frames (with --interpolate, or --path with --interpolate or --input-fps/--fps) writes the interpolated frames,
 and with --path the copied input frames, at the input's own size: the flow is estimated and reversed at the network size,
 then resized inside the blend, which warps the decoded frames.  --flow-size H W sets that network size in place of
@@ -139,9 +151,10 @@ def parser():
     p.add_argument('--small', action='store_true')
     p.add_argument('--iters', type=int, default=None,
                    help='extension: GRU iterations (test mode: 20 like the reference; -m val: the protocol\'s 32 / 24)')
-    p.add_argument('--dataset', default=None, choices=['sintel', 'kitti', 'vimeo', 'tapvid'],
+    p.add_argument('--dataset', default=None, choices=['sintel', 'kitti', 'vimeo', 'tapvid', 'davis'],
                    help='-m val: which dataset --data holds (Sintel / KITTI-2015 training sets: flow; Vimeo-90K '
-                        'triplets: frame interpolation; TAP-Vid .pkl file or directory of .pkl shards: point tracking)')
+                        'triplets: frame interpolation; TAP-Vid .pkl file or directory of .pkl shards: point tracking; '
+                        'DAVIS-2017 tree: label propagation)')
     p.add_argument('--query-mode', default=None, choices=['first', 'strided'],
                    help="-m val --dataset tapvid: TAP-Vid's query mode (default first: each track from its first visible "
                         "frame; strided: from every 5th frame, tracked forward and backward)")
@@ -194,6 +207,11 @@ def parser():
     p.add_argument('--track-backward', action='store_true',
                    help='extension, with --track or --track-grid: also track every point back from its frame to frame 0 '
                         '(a second flow sweep over the frames before the last query frame)')
+    p.add_argument('--propagate', default=None, metavar='KEY.png',
+                   help="extension, with --path: carry the label map KEY.png (palette or 8-bit grey, the frames' size) "
+                        "of frame --propagate-frame to every frame; writes <--out>/label_<i:06d>.png")
+    p.add_argument('--propagate-frame', type=int, default=None, metavar='K',
+                   help='extension, with --propagate: the frame the key labels belong to (default 0)')
     p.add_argument('--upstream', action='store_true',
                    help='extension: weights converted from an official princeton-vl RAFT .pth (raft_b200.convert): RGB '
                         'frames and the upstream numerics (RAFT(..., upstream=True))')
@@ -206,6 +224,23 @@ def parser():
 def main(argv=None):
     p = parser()
     args = p.parse_args(argv)
+    if args.propagate is not None:
+        if args.path is None or args.mode != 'test':
+            p.error('--propagate carries labels through a frame directory: it needs --path DIR (and no -m val)')
+        for other, given in (('--track', args.track is not None), ('--track-grid', args.track_grid is not None),
+                             ('--track-frame', args.track_frame != 0), ('--track-vis', args.track_vis is not None),
+                             ('--track-backward', args.track_backward), ('--interpolate', args.interpolate),
+                             ('--fps', args.fps), ('--input-fps', args.input_fps), ('--warm-start', args.warm_start),
+                             ('--scene-cut', args.scene_cut is not None), ('--bidirectional', args.bidirectional),
+                             ('--native-flow', args.native_flow), ('--native-frames', args.native_frames),
+                             ('--flo', args.flo), ('--npy', args.npy)):
+            if given:
+                p.error(f'--propagate writes label maps: it cannot be combined with {other}')
+        if args.batch < 1 or args.workers < 0:
+            p.error('--path needs --batch >= 1 and --workers >= 0')
+        return run_propagate(args, p)
+    if args.propagate_frame is not None:
+        p.error('--propagate-frame goes with --propagate')
     if args.track is not None or args.track_grid is not None:
         if args.track is not None and args.track_grid is not None:
             p.error('--track and --track-grid are two ways to give the points: pass one')
@@ -283,6 +318,11 @@ def main(argv=None):
                     'videos)')
         if args.dataset == 'tapvid' and args.warm_start:
             p.error('--warm-start warm-starts flow validation; TAP-Vid tracks points through cold flows')
+        if args.dataset == 'davis' and args.split == 'test':
+            p.error('--split test writes a flow submission; DAVIS-2017 test-dev submissions are not supported (-m val '
+                    'scores the val split)')
+        if args.dataset == 'davis' and args.warm_start:
+            p.error('--warm-start warm-starts flow validation; DAVIS propagates labels through cold flows')
     if args.query_mode is not None and (args.mode != 'val' or args.dataset != 'tapvid'):
         p.error('--query-mode goes with -m val --dataset tapvid')
     if args.mode == 'val':
@@ -418,6 +458,32 @@ def run_track(args, p):
     return 0
 
 
+def run_propagate(args, p):
+    """--path --propagate: raft_b200.video.video_propagate over the frames of --path, at 432x1024 (or --flow-size) like
+    test mode (or their own size with --keep-size); the key and the written label maps are at the frames' own size.
+    Prints the frame count and how many pixels of the last frame are consistent (status 0) all the way to the key."""
+    import cv2
+    from raft_b200.video import list_frames, read_labels, video_propagate
+    try:
+        key, _ = read_labels(args.propagate)
+        paths = list_frames(args.path)
+    except (OSError, ValueError) as e:
+        p.error(f'--propagate: {e}')
+    frame = 0 if args.propagate_frame is None else args.propagate_frame
+    if not 0 <= frame < len(paths):
+        p.error(f'--propagate-frame {frame}: {args.path} holds {len(paths)} frames')
+    first = cv2.imread(paths[0], cv2.IMREAD_COLOR)
+    if first is not None and first.shape[:2] != key.shape:
+        p.error(f'--propagate: {args.propagate} is {key.shape[0]}x{key.shape[1]}, the frames of {args.path} are '
+                f'{first.shape[0]}x{first.shape[1]}; the key labels need the frames\' size')
+    model = _video_model(args)
+    files, last = video_propagate(model, paths, args.out, args.propagate, frame=frame, batch=args.batch,
+                                  workers=args.workers)
+    print(f"labels of frame {frame} propagated through {len(files)} frames: {int((last == 0).sum())} of {last.size} "
+          f"pixels of the last frame consistent (status 0); written under {args.out}")
+    return 0
+
+
 def _video_model(args):
     """The model of --path: at 432x1024 (or --flow-size) like test mode, or at the frames' own size with --keep-size."""
     from networks import RAFT
@@ -450,7 +516,8 @@ def validate(args):
         print(f"{len(files)} flows written under {args.out}")
         return 0
     res = evaluate(model, args.data, args.dataset, dstypes=tuple(args.dstype), batch=args.batch, workers=args.workers,
-                   iters=args.iters, warm_start=args.warm_start, query_mode=args.query_mode)
+                   iters=args.iters, warm_start=args.warm_start, query_mode=args.query_mode,
+                   masks_out=os.path.join(args.out, 'davis_val') if args.dataset == 'davis' else None)
     for line in summary_lines(res):
         print(line)
     os.makedirs(args.out, exist_ok=True)

@@ -172,6 +172,18 @@ class RAFT(object):
         return self.engine().track(_as_tensor(frames), queries, backward=bool(backward))
 
     @torch.no_grad()
+    def propagate(self, frames, labels, frame=0):
+        """Extension (keyframe label propagation): the [Hs,Ws] uint8 label map `labels` of frame `frame` (a segmentation
+        mask, a class map, ...) carried through all of [F,Hs,Ws,3] frames (dtypes and sources as for ``forward``).  One
+        ``forward_sequence_bidirectional`` pass; per pixel of every frame, the displacement back to the keyframe composed
+        through the consecutive flows on the GPU, and the keyframe's label there by a vote of its four nearest pixels
+        (RaftEngine.propagate).  Returns fresh (labels [F,Hs,Ws] uint8, status [F,Hs,Ws] uint8) CUDA tensors at the frames'
+        own size (with input_size too): status 0 consistent at every step back to the keyframe, 1 occluded at some step,
+        2 entered through the frame edge; labels[frame] equals the key.  A key that is not [Hs,Ws] uint8 or a frame
+        outside [0, F) raises ValueError."""
+        return self.engine().propagate(_as_tensor(frames), labels, frame=frame)
+
+    @torch.no_grad()
     def interpolate_sequence(self, frames, t=0.5, uint8=False, bgr=False, native=False):
         """Extension (frame-rate up-conversion): the frames at time t (a float, or a sequence of times, each in [0, 1])
         between every pair of consecutive frames of [T+1,H,W,3] frames, from one ``forward_sequence_bidirectional`` pass.

@@ -57,9 +57,8 @@ def fb_consistency(flow_fw, flow_bw, alpha1=0.01, alpha2=0.5, flow_scale=1.0):
     return occ_fw, occ_bw
 
 
-def _track_args(what, flow_fw, flow_bw, qframe, qpos, state):
-    """The argument checks of track_points and track_points_backward -> (T, H, W, N, qframe, qpos, state) with the
-    queries as contiguous device tensors and state fresh (NaN, 3) when None."""
+def _flow_pair(what, flow_fw, flow_bw):
+    """(T, H, W) of two matching [T,H,W,2] float32 CUDA flows; anything else raises ValueError."""
     for name, t in (("flow_fw", flow_fw), ("flow_bw", flow_bw)):
         if not (isinstance(t, torch.Tensor) and t.is_cuda and t.dim() == 4 and t.shape[-1] == 2
                 and t.dtype == torch.float32):
@@ -67,7 +66,13 @@ def _track_args(what, flow_fw, flow_bw, qframe, qpos, state):
                              f"{getattr(t, 'shape', None)} {getattr(t, 'dtype', type(t))})")
     if flow_fw.shape != flow_bw.shape or flow_fw.device != flow_bw.device:
         raise ValueError(f"{what}: flow_fw {tuple(flow_fw.shape)} and flow_bw {tuple(flow_bw.shape)} must match")
-    T, H, W, _ = flow_fw.shape
+    return tuple(flow_fw.shape[:3])
+
+
+def _track_args(what, flow_fw, flow_bw, qframe, qpos, state):
+    """The argument checks of track_points and track_points_backward -> (T, H, W, N, qframe, qpos, state) with the
+    queries as contiguous device tensors and state fresh (NaN, 3) when None."""
+    T, H, W = _flow_pair(what, flow_fw, flow_bw)
     dev = flow_fw.device
     qframe = torch.as_tensor(qframe).to(device=dev, dtype=torch.int32).contiguous()
     qpos = torch.as_tensor(qpos).to(device=dev, dtype=torch.float32).contiguous()
@@ -140,6 +145,106 @@ def track_points_backward(flow_fw, flow_bw, qframe, qpos, tracks=None, status=No
                                                      int(first_frame), capi.ptr(pos), capi.ptr(st), capi.ptr(tracks),
                                                      capi.ptr(status), capi.stream()))
     return tracks, status, (pos, st)
+
+
+def _accumulate(what, fn, flow_fw, flow_bw, acc, status, start, n_steps, flow_scale, alpha1, alpha2):
+    """The checks and the call of accumulate_flow / accumulate_flow_backward."""
+    T, H, W = _flow_pair(what, flow_fw, flow_bw)
+    dev = flow_fw.device
+    n_steps = T if n_steps is None else int(n_steps)
+    if not (isinstance(acc, torch.Tensor) and isinstance(status, torch.Tensor)
+            and tuple(acc.shape) == (n_steps + 1, H, W, 2) and acc.dtype == torch.float32 and acc.device == dev
+            and acc.is_contiguous() and tuple(status.shape) == (n_steps + 1, H, W) and status.dtype == torch.uint8
+            and status.device == dev and status.is_contiguous()):
+        raise ValueError(f"{what}: acc and status must be contiguous [n_steps+1,H,W,2] float32 and [n_steps+1,H,W] uint8 "
+                         f"on {dev} with n_steps + 1 = {n_steps + 1}, H x W = {H}x{W} (got "
+                         f"{tuple(getattr(acc, 'shape', ()))} and {tuple(getattr(status, 'shape', ()))})")
+    fw, bw = flow_fw.contiguous(), flow_bw.contiguous()
+    with torch.cuda.device(dev):
+        capi.check(fn(capi.ptr(fw), capi.ptr(bw), T, H, W, n_steps, float(flow_scale), float(alpha1), float(alpha2),
+                      int(start), capi.ptr(acc), capi.ptr(status), capi.stream()))
+    return acc, status
+
+
+def accumulate_flow(flow_fw, flow_bw, acc, status, start=0, n_steps=None, flow_scale=1.0, alpha1=0.01, alpha2=0.5):
+    """Extension (keyframe label propagation): per pixel of every later frame, the displacement back to the frame of row
+    `start`, composed through the consecutive flows of one pass on the GPU (rb_flow_accumulate).  flow_fw, flow_bw:
+    [T,H,W,2] fp32 CUDA flows in pair order (forward_sequence_bidirectional's); the first n_steps pairs (default T) are
+    used.  acc [n_steps+1,H,W,2] fp32 and status [n_steps+1,H,W] uint8 are written in place: row `start` is the input
+    (zeros for the keyframe, or the last row of the previous pass), rows start+1 .. n_steps are written, no other row is
+    touched.  Status: 0 consistent at every step back to the keyframe, 1 occluded at some step (the forward-backward test
+    of fb_consistency failed), 2 entered through the frame edge at some step.  flow_scale, alpha1, alpha2 as in
+    fb_consistency.  Returns (acc, status)."""
+    return _accumulate("accumulate_flow", capi.lib.rb_flow_accumulate, flow_fw, flow_bw, acc, status, start, n_steps,
+                       flow_scale, alpha1, alpha2)
+
+
+def accumulate_flow_backward(flow_fw, flow_bw, acc, status, start=0, n_steps=None, flow_scale=1.0, alpha1=0.01,
+                             alpha2=0.5):
+    """The mirror of accumulate_flow for the frames before the keyframe (rb_flow_accumulate_backward): rows start-1 .. 0
+    are written from row `start`, each step r+1 -> r pulling with flow_fw[r] and testing against flow_bw[r]."""
+    return _accumulate("accumulate_flow_backward", capi.lib.rb_flow_accumulate_backward, flow_fw, flow_bw, acc, status,
+                       start, n_steps, flow_scale, alpha1, alpha2)
+
+
+def propagate_labels(acc, status, key):
+    """Extension (keyframe label propagation): the [Hs,Ws] uint8 CUDA label map `key` of the keyframe carried to every row
+    of acc [n,H,W,2] / status [n,H,W] (accumulate_flow's, at the network size) at the key's own size (rb_labels_propagate):
+    per output pixel, the displacement resized as resize_flow does, the origin clamped into the key, and the label of the
+    largest summed bilinear weight among the origin's four pixels (ties to the smaller label).  Returns fresh (labels
+    [n,Hs,Ws] uint8, status [n,Hs,Ws] uint8): status as accumulate_flow's at the network pixel that holds the output pixel's
+    centre, 2 where the origin had to be clamped."""
+    if not (isinstance(acc, torch.Tensor) and acc.is_cuda and acc.dim() == 4 and acc.shape[-1] == 2
+            and acc.dtype == torch.float32):
+        raise ValueError(f"propagate_labels: acc must be an [n,H,W,2] float32 CUDA tensor (got "
+                         f"{getattr(acc, 'shape', None)} {getattr(acc, 'dtype', type(acc))})")
+    n, H, W, _ = acc.shape
+    if not (isinstance(status, torch.Tensor) and tuple(status.shape) == (n, H, W) and status.dtype == torch.uint8
+            and status.device == acc.device):
+        raise ValueError(f"propagate_labels: status must be an [n,H,W] = {[n, H, W]} uint8 tensor on {acc.device}")
+    if not (isinstance(key, torch.Tensor) and key.dim() == 2 and key.dtype == torch.uint8 and key.device == acc.device):
+        raise ValueError(f"propagate_labels: key must be an [Hs,Ws] uint8 tensor on {acc.device} (got "
+                         f"{getattr(key, 'shape', None)} {getattr(key, 'dtype', type(key))})")
+    Hs, Ws = key.shape
+    a, s, k = acc.contiguous(), status.contiguous(), key.contiguous()
+    labels = torch.empty(n, Hs, Ws, dtype=torch.uint8, device=a.device)
+    st = torch.empty_like(labels)
+    with torch.cuda.device(a.device):
+        capi.check(capi.lib.rb_labels_propagate(capi.ptr(a), capi.ptr(s), n, H, W, capi.ptr(k), Hs, Ws,
+                                                capi.ptr(labels), capi.ptr(st), capi.stream()))
+    return labels, st
+
+
+LABEL_STATS = ("intersection", "union", "boundary_pred", "boundary_gt", "matched_pred", "matched_gt")  # RB_LABEL_STATS
+
+
+def label_metrics(pred, gt, n_objects, bound_pix=None):
+    """Extension (DAVIS-2017's J and F): the integer counts of [n,H,W] uint8 CUDA label maps pred against gt for the
+    objects 1..n_objects (rb_label_metrics).  Returns a fresh [n, n_objects, 6] int64 tensor (LABEL_STATS): |P and G|,
+    |P or G|, the boundary pixels of P and of G (davis2017-evaluation's _seg2bmap), and those of each with a boundary
+    pixel of the other within a disk of radius bound_pix (default ceil(0.008 hypot(H, W)), DAVIS's; 1 to 32).  Wrong
+    shapes or dtypes raise ValueError."""
+    for name, t in (("pred", pred), ("gt", gt)):
+        if not (isinstance(t, torch.Tensor) and t.is_cuda and t.dim() == 3 and t.dtype == torch.uint8):
+            raise ValueError(f"label_metrics: {name} must be an [n,H,W] uint8 CUDA tensor (got "
+                             f"{getattr(t, 'shape', None)} {getattr(t, 'dtype', type(t))})")
+    if pred.shape != gt.shape or pred.device != gt.device:
+        raise ValueError(f"label_metrics: pred {tuple(pred.shape)} and gt {tuple(gt.shape)} must match")
+    n, H, W = pred.shape
+    if bound_pix is None:
+        bound_pix = davis_bound_pix(H, W)
+    p, g = pred.contiguous(), gt.contiguous()
+    counts = torch.empty(n, int(n_objects), len(LABEL_STATS), dtype=torch.int64, device=p.device)
+    with torch.cuda.device(p.device):
+        capi.check(capi.lib.rb_label_metrics(capi.ptr(p), capi.ptr(g), n, H, W, int(n_objects), int(bound_pix),
+                                             capi.ptr(counts), capi.stream()))
+    return counts
+
+
+def davis_bound_pix(H, W):
+    """davis2017-evaluation's f_measure radius: ceil(0.008 * hypot(H, W)) (8 at 480x854, 18 at 1080x1920)."""
+    import math
+    return int(math.ceil(0.008 * math.hypot(H, W)))
 
 
 FLOW_STATS = ("n", "sum_epe", "lt1", "lt3", "lt5", "outliers")  # the columns of flow_metrics' stats (RB_FLOW_STATS)

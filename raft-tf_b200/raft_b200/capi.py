@@ -72,6 +72,9 @@ SIGNATURES = {
     "rb_flow_fb_check": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _f, _f, _f, _vp]),
     "rb_track_points": (_i, [_vp, _vp, _i, _i, _i, _i, _f, _f, _f, _vp, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp]),
     "rb_track_points_backward": (_i, [_vp, _vp, _i, _i, _i, _i, _f, _f, _f, _vp, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp]),
+    "rb_flow_accumulate": (_i, [_vp, _vp, _i, _i, _i, _i, _f, _f, _f, _i, _vp, _vp, _vp]),
+    "rb_flow_accumulate_backward": (_i, [_vp, _vp, _i, _i, _i, _i, _f, _f, _f, _i, _vp, _vp, _vp]),
+    "rb_labels_propagate": (_i, [_vp, _vp, _i, _i, _i, _vp, _i, _i, _vp, _vp, _vp]),
     "rb_flow_reverse_workspace_bytes": (_i, [_i, _i, _i, _psz]),
     "rb_flow_reverse": (_i, [_vp, _vp, _vp, _i, _i, _f, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _vp, _sz, _vp]),
     "rb_frame_synthesize": (_i, [_vp, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _f, _vp, _i, _i, _i, _vp]),
@@ -90,6 +93,7 @@ SIGNATURES = {
     "rb_flow_metrics": (_i, [_vp, _f, _vp, _vp, _i, _i, _i, _vp, _vp, _vp, _sz, _vp]),
     "rb_frame_metrics_workspace_bytes": (_i, [_i, _i, _i, _psz]),
     "rb_frame_metrics": (_i, [_vp, _i, _vp, _i, _i, _i, _vp, _vp, _sz, _vp]),
+    "rb_label_metrics": (_i, [_vp, _vp, _i, _i, _i, _i, _i, _vp, _vp]),
     "rb_scene_cut_scores": (_i, [_vp, _i, _i, _i, _vp, _vp, _vp]),
     "rb_flow_forward_interpolate_workspace_bytes": (_i, [_i, _i, _i, _psz]),
     "rb_flow_forward_interpolate": (_i, [_vp, _vp, _i, _i, _i, _vp, _sz, _vp]),

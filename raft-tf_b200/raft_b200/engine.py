@@ -530,6 +530,38 @@ class RaftEngine:
             return tracks_to_frames(tracks, src_hw, net_hw), status
 
     @torch.no_grad()
+    def propagate(self, frames: torch.Tensor, labels, frame: int = 0):
+        """Keyframe label propagation: the [Hs,Ws] uint8 label map `labels` of frame `frame` carried to every one of the
+        [F,Hs,Ws,3] frames (dtypes, sizes and input_size as for forward()).  One forward_sequence_bidirectional(check=False)
+        pass; a zero row at `frame`, one rb_flow_accumulate and one rb_flow_accumulate_backward launch on its flows
+        (flow_scale and the forward-backward test as in the occlusion check), and one rb_labels_propagate over all rows
+        at the frames' own size.  Returns fresh (labels [F,Hs,Ws] uint8, status [F,Hs,Ws] uint8) CUDA tensors: status 0
+        consistent at every step back to the keyframe, 1 occluded at some step, 2 entered through the frame edge at some
+        step; labels[frame] equals the key bit for bit.  A key that is not [Hs,Ws] uint8 or a frame outside [0, F) raises
+        ValueError before the pass."""
+        from networks.utils import accumulate_flow, accumulate_flow_backward, propagate_labels
+        F = _sequence_length(frames) + 1
+        Hs, Ws = frames.shape[1:3]
+        key = torch.as_tensor(labels)
+        if not (key.dim() == 2 and key.dtype == torch.uint8 and tuple(key.shape) == (Hs, Ws)):
+            raise ValueError(f"raft_b200: the key labels must be an [Hs,Ws] = [{Hs},{Ws}] uint8 map (got "
+                             f"{list(key.shape)} {key.dtype})")
+        if not (isinstance(frame, (int, np.integer)) and 0 <= frame < F):
+            raise ValueError(f"raft_b200: the key frame must be an integer in [0, {F}) (got {frame!r})")
+        frame = int(frame)
+        flow_fw, flow_bw, _, _ = self.forward_sequence_bidirectional(frames, check=False)
+        T, H, W = flow_fw.shape[:3]
+        with torch.cuda.device(self.device):
+            acc = torch.empty(F, H, W, 2, dtype=torch.float32, device=self.device)
+            status = torch.empty(F, H, W, dtype=torch.uint8, device=self.device)
+            acc[frame].zero_()
+            status[frame].zero_()
+            kw = dict(start=frame, flow_scale=self.flow_scale, alpha1=FB_ALPHA1, alpha2=FB_ALPHA2)
+            accumulate_flow(flow_fw, flow_bw, acc, status, **kw)
+            accumulate_flow_backward(flow_fw, flow_bw, acc, status, **kw)
+            return propagate_labels(acc, status, key.to(self.device))
+
+    @torch.no_grad()
     def interpolate(self, left: torch.Tensor, right: torch.Tensor, ts, native: bool = False) -> torch.Tensor:
         """Frames at times ts (each in [0, 1]; 0 = left, 1 = right) between B frame pairs: one bidirectional pass (as
         forward_bidirectional(check=False), from a graph of its own), then eagerly on the same stream, for as many times

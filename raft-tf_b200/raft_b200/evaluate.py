@@ -19,6 +19,9 @@ per-triplet PSNR and SSIM, reported as their means over the list.
 TAP-Vid (F17, raft_b200.tapvid): point tracking scored by Average Jaccard, the fraction of points within 1-16 pixels and
 occlusion accuracy, at 256 x 256 with 20 iterations, in the 'first' or 'strided' query mode.
 
+DAVIS-2017 (F20, raft_b200.davis): keyframe label propagation from each sequence's first annotation, scored by region
+similarity J and boundary accuracy F (davis2017-evaluation's semi-supervised protocol) at 480p with 20 iterations.
+
 Pipeline: pairs are grouped by frame size (one CUDA graph per size) and run in batches through RaftEngine.forward, whose
 flow stays on the GPU: rb_flow_metrics scores it against the uploaded ground truth on the same stream and writes per-pair
 stats into one device buffer, read back once per split.  Worker threads decode the next batches (cv2 releases the GIL)
@@ -41,7 +44,8 @@ from . import capi
 from .engine import RaftEngine
 
 # dataset -> (iterations, pad_mode): upstream's validate_sintel / validate_kitti
-PROTOCOLS = {"sintel": (32, "sintel"), "kitti": (24, "kitti"), "vimeo": (20, "sintel"), "tapvid": (20, "sintel")}
+PROTOCOLS = {"sintel": (32, "sintel"), "kitti": (24, "kitti"), "vimeo": (20, "sintel"), "tapvid": (20, "sintel"),
+             "davis": (20, "sintel")}
 DSTYPES = ("clean", "final")
 QUERY_MODES = ("first", "strided")  # TAP-Vid's (raft_b200.tapvid)
 STATS = 6  # RB_FLOW_STATS: n, sum of EPE, #(EPE < 1), #(EPE < 3), #(EPE < 5), #outliers
@@ -419,9 +423,12 @@ def _setup(model, dataset, dstypes, batch, workers, iters, warm_start, what):
         raise ValueError(f"{what}: warm_start needs frame sequences; Vimeo-90K's triplets are not chains")
     if dataset == "tapvid" and warm_start:
         raise ValueError(f"{what}: warm_start warm-starts flow validation; TAP-Vid tracks points through cold flows")
+    if dataset == "davis" and warm_start:
+        raise ValueError(f"{what}: warm_start warm-starts flow validation; DAVIS propagates labels through cold flows")
     if model._params is None:
         raise RuntimeError(f"RAFT.load(<npz>) must be called before {what}")
-    splits = ("kitti",) if kitti else ("vimeo",) if vimeo else ("tapvid",) if dataset == "tapvid" else tuple(dstypes)
+    splits = ("kitti",) if kitti else ("vimeo",) if vimeo else (dataset,) if dataset in ("tapvid", "davis") \
+        else tuple(dstypes)
     if dataset == "sintel" and (not splits or any(d not in DSTYPES for d in splits)):
         raise ValueError(f"Sintel dstypes must be a non-empty subset of {DSTYPES} (got {dstypes!r})")
     n_iters, pad_mode = PROTOCOLS[dataset]
@@ -435,7 +442,7 @@ def _engine(model, n_iters, pad_mode, input_size=None):
 
 
 def evaluate(model, root, dataset="sintel", dstypes=DSTYPES, batch=1, workers=4, iters=None, warm_start=False,
-             query_mode=None):
+             query_mode=None, masks_out=None):
     """Upstream RAFT's validation of a loaded networks.RAFT.RAFT model on a Sintel or KITTI-2015 training tree, or the
     interpolation quality on a Vimeo-90K triplet tree (dataset 'vimeo').
 
@@ -456,7 +463,15 @@ def evaluate(model, root, dataset="sintel", dstypes=DSTYPES, batch=1, workers=4,
     tapvid: root is a TAP-Vid .pkl file or a directory of .pkl shards, scored in query_mode 'first' (the default) or
     'strided' at 256 x 256 (raft_b200.tapvid: the engine resizes the frames on the GPU); returns {"dataset", "iters",
     "query_mode", "resolution": [256, 256], "splits": {"tapvid": aggregate_tapvid(...)}}.  dstypes and workers are
-    ignored, warm_start raises ValueError, and query_mode is refused for the other datasets."""
+    ignored, warm_start raises ValueError, and query_mode is refused for the other datasets.
+
+    davis: root is a DAVIS-2017 tree; frame 0's annotation of every sequence of ImageSets/2017/val.txt is propagated
+    through the sequence at its own size and scored by J and F (raft_b200.davis); returns {"dataset", "iters",
+    "pad_mode", "splits": {"val": aggregate_davis(...)}}.  masks_out (a directory) also receives the predicted masks in
+    DAVIS's results layout.  dstypes and workers are ignored and warm_start raises ValueError; masks_out is refused for
+    the other datasets."""
+    if masks_out is not None and dataset != "davis":
+        raise ValueError(f"evaluate: masks_out writes DAVIS-2017 predictions (got dataset {dataset!r})")
     if query_mode is not None and dataset != "tapvid":
         raise ValueError(f"evaluate: query_mode belongs to TAP-Vid's point tracking (got dataset {dataset!r})")
     if dataset == "tapvid" and query_mode not in (None,) + QUERY_MODES:
@@ -470,6 +485,13 @@ def evaluate(model, root, dataset="sintel", dstypes=DSTYPES, batch=1, workers=4,
         records = tapvid.run(engine, root, mode, int(batch), model.upstream)
         return {"dataset": dataset, "iters": n_iters, "query_mode": mode, "resolution": list(tapvid.SIZE),
                 "splits": {"tapvid": tapvid.aggregate_tapvid(records)}}
+    if dataset == "davis":
+        from . import davis
+        seqs = davis.davis_sequences(root)  # every file checked up front
+        engine = _engine(model, n_iters, pad_mode)
+        records = davis.run(engine, seqs, int(batch), model.upstream, masks_out)
+        return {"dataset": dataset, "iters": n_iters, "pad_mode": pad_mode,
+                "splits": {"val": davis.aggregate_davis(records)}}
     if dataset == "vimeo":
         trips = vimeo_triplets(root)  # every file checked up front
         engine = _engine(model, n_iters, pad_mode)
@@ -540,6 +562,8 @@ def submit(model, root, dataset, out, dstypes=DSTYPES, batch=1, workers=4, iters
         raise ValueError("submit: Vimeo-90K has no test split with hidden ground truth; evaluate scores its test list")
     if dataset == "tapvid":
         raise ValueError("submit: TAP-Vid has no test split with hidden ground truth; evaluate scores its videos")
+    if dataset == "davis":
+        raise ValueError("submit: DAVIS-2017 test-dev submissions are not supported; evaluate scores the val split")
     kitti, splits, n_iters, pad_mode = _setup(model, dataset, dstypes, batch, workers, iters, warm_start, "submit")
     lists = {s: kitti_test_pairs(root) if kitti else sintel_test_pairs(root, s) for s in splits}
     engine = _engine(model, n_iters, pad_mode)
@@ -561,7 +585,11 @@ def submit(model, root, dataset, out, dstypes=DSTYPES, batch=1, workers=4, iters
 def summary_lines(res):
     """upstream evaluate.py's lines: 'Validation (clean) EPE: ..., 1px: ..., 3px: ..., 5px: ...' per Sintel pass,
     'Validation KITTI: <epe>, <f1>'; for Vimeo-90K 'Validation Vimeo-90K: PSNR: ..., SSIM: ...'; and for TAP-Vid
-    'Validation TAP-Vid (<query mode>): AJ: ..., <δ_avg>: ..., OA: ...'."""
+    'Validation TAP-Vid (<query mode>): AJ: ..., <δ_avg>: ..., OA: ...'; for DAVIS-2017
+    'Validation DAVIS-2017 (val): J&F: ..., J: ..., F: ...'."""
+    if res["dataset"] == "davis":
+        r = res["splits"]["val"]
+        return ["Validation DAVIS-2017 (val): J&F: %f, J: %f, F: %f" % (r["J&F-Mean"], r["J-Mean"], r["F-Mean"])]
     if res["dataset"] == "tapvid":
         r = res["splits"]["tapvid"]
         return ["Validation TAP-Vid (%s): AJ: %f, <δ_avg>: %f, OA: %f" % (res["query_mode"], r["average_jaccard"],

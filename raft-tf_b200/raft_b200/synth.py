@@ -98,6 +98,56 @@ def write_vimeo_tree(root: str, sizes, seed: int = 4000, shift: int = 4):
     return entries
 
 
+# PASCAL VOC's first colours, as DAVIS's annotations use them
+DAVIS_PALETTE = np.array([[0, 0, 0], [128, 0, 0], [0, 128, 0], [128, 128, 0], [0, 0, 128], [128, 0, 128],
+                          [0, 128, 128], [128, 128, 128], [64, 0, 0], [192, 0, 0], [64, 128, 0], [192, 128, 0],
+                          [64, 0, 128]] + [[i, i, i] for i in range(13, 256)], dtype=np.uint8)
+
+
+def write_davis_tree(root: str, sequences, H: int = 480, W: int = 854, objects: int = 2, seed: int = 5000,
+                     shift: int = 3):
+    """A dataset in DAVIS-2017's layout under root: per (name, n_frames) of sequences, <root>/JPEGImages/480p/<name>/
+    NNNNN.jpg frames and <root>/Annotations/480p/<name>/NNNNN.png palette annotations, and <root>/ImageSets/2017/val.txt
+    listing the names in order.  Each frame is a textured background with `objects` textured ellipses (labels 1..objects,
+    drawn in label order, so a later one occludes an earlier one) moving by seeded whole-pixel steps of at most `shift`
+    per frame; the annotations are the exact label maps.  Returns the names."""
+    import os
+
+    import cv2
+    from PIL import Image
+    rng = np.random.default_rng(seed)
+    names = []
+    for name, n in sequences:
+        fdir = os.path.join(root, "JPEGImages", "480p", name)
+        adir = os.path.join(root, "Annotations", "480p", name)
+        os.makedirs(fdir, exist_ok=True)
+        os.makedirs(adir, exist_ok=True)
+        tex = [_blur(rng.random((H, W, 3), dtype=np.float32), 2.0) for _ in range(objects + 1)]
+        tex = [(t - t.min()) / max(float(t.max() - t.min()), 1e-6) for t in tex]
+        ys, xs = np.mgrid[0:H, 0:W]
+        centre = rng.uniform([0.25 * W, 0.25 * H], [0.75 * W, 0.75 * H], (objects, 2))
+        radii = rng.uniform(0.06, 0.16, (objects, 2)) * np.array([W, H])
+        step = rng.integers(-shift, shift + 1, (objects, 2))
+        for k in range(n):
+            img = tex[0].copy()
+            lab = np.zeros((H, W), np.uint8)
+            for o in range(objects):
+                cx, cy = centre[o] + k * step[o]
+                inside = ((xs - cx) / radii[o, 0]) ** 2 + ((ys - cy) / radii[o, 1]) ** 2 <= 1.0
+                lab[inside] = o + 1
+                img[inside] = np.roll(tex[o + 1], (int(k * step[o, 1]), int(k * step[o, 0])), (0, 1))[inside]
+            cv2.imwrite(os.path.join(fdir, f"{k:05d}.jpg"), np.round(255 * img).astype(np.uint8),
+                        [cv2.IMWRITE_JPEG_QUALITY, 95])
+            im = Image.frombytes("P", (W, H), lab.tobytes())
+            im.putpalette(DAVIS_PALETTE.reshape(-1).tolist())
+            im.save(os.path.join(adir, f"{k:05d}.png"))
+        names.append(name)
+    os.makedirs(os.path.join(root, "ImageSets", "2017"), exist_ok=True)
+    with open(os.path.join(root, "ImageSets", "2017", "val.txt"), "w") as f:
+        f.write("\n".join(names) + "\n")
+    return names
+
+
 def make_batch(B: int, H: int, W: int, seed0: int = 1000):
     pairs = [make_pair(H, W, seed0 + i) for i in range(B)]
     return np.stack([p[0] for p in pairs]), np.stack([p[1] for p in pairs])

@@ -28,6 +28,10 @@ at every STEP-th pixel of one frame): interp_schedule()'s passes of forward_sequ
 rb_track_points launch that carries the points' positions and states on the GPU, the rows streamed into out/tracks.npy and
 out/status.npy.
 
+video_propagate(model, "frames/", "out/", "key.png", frame=K) carries frame K's label map to every frame: the same passes,
+each followed by rb_flow_accumulate (and, before the key frame, rb_flow_accumulate_backward) launches that carry the
+per-pixel displacement to the key frame on the GPU and one rb_labels_propagate launch, written as out/label_<i:06d>.png.
+
 Scene cuts (scene_cut=<threshold in [0, 1]>, video_interpolate and warm-started video): each pass's decoded frames are
 copied to the GPU once and scored there (networks.utils.scene_cut_scores: one minus the intersection of consecutive
 frames' colour histograms); a pair whose score exceeds the threshold is a cut.  Frame-rate conversion copies the nearer
@@ -658,3 +662,125 @@ def video_track(model, frames, out, queries=None, grid=None, grid_frame=0, batch
             if mm is not None:
                 mm.flush()
     return files
+
+
+def read_labels(path):
+    """A label map from a PNG: palette (mode P) images give their indices, 8-bit grey (mode L) images their values.
+    Returns (labels [H,W] uint8, palette [n,3] uint8 or None for grey).  Any other image raises ValueError (an RGB mask
+    holds colours, not label ids).  Needs Pillow: cv2 expands a palette PNG to colours and loses the indices."""
+    from PIL import Image
+    with Image.open(os.fspath(path)) as im:
+        if im.mode not in ("P", "L"):
+            raise ValueError(f"video: {path} is a mode {im.mode} image; label maps are palette (P) or 8-bit grey (L) PNGs")
+        labels = np.array(im, dtype=np.uint8)
+        palette = None
+        if im.mode == "P":
+            palette = np.array(im.getpalette() or [], dtype=np.uint8).reshape(-1, 3)
+    return labels, palette
+
+
+def write_labels(path, labels, palette=None):
+    """Writes an [H,W] uint8 label map as a PNG: with the [n,3] palette as a palette image (DAVIS's annotation format),
+    without one as 8-bit grey."""
+    from PIL import Image
+    arr = np.ascontiguousarray(labels, dtype=np.uint8)
+    im = Image.frombytes("L" if palette is None else "P", (arr.shape[1], arr.shape[0]), arr.tobytes())
+    if palette is not None:
+        im.putpalette(np.asarray(palette, dtype=np.uint8).reshape(-1).tolist())
+    im.save(os.fspath(path), format="PNG")
+
+
+def video_propagate(model, frames, out, labels, frame=0, batch=8, workers=4):
+    """Keyframe label propagation through a video of any length with a loaded networks.RAFT.RAFT model: the label map of
+    frame `frame` (`labels`: a palette or grey PNG path, or an [Hs,Ws] uint8 array at the frames' size) carried to every
+    frame (a directory's sorted *.png / *.jpg, or a list of paths, all of one size).  Writes <out>/label_<i:06d>.png for
+    every frame, in the key's palette when it has one and grey otherwise.  Returns (the paths, the [Hs,Ws] uint8 status
+    of the last frame: 0 consistent at every step back to the key frame, 1 occluded at some step, 2 entered through the
+    frame edge).
+
+    Passes come from interp_schedule(): forward_sequence_bidirectional(check=False) on batch + 1 frames.  The forward
+    sweep starts at the pass holding `frame`: a zero row there, one rb_flow_accumulate launch to the pass's last frame and
+    one rb_flow_accumulate_backward launch to its first; each later pass starts from the last row of the one before.  A
+    reverse sweep then runs the passes before that one again, last to first, each with one rb_flow_accumulate_backward
+    launch from the first row of the pass after it (as video_track(backward=True) does), so frame = 0 costs nothing
+    more.  Every row's labels come from one rb_labels_propagate launch at the frames' own size.  The files are the same
+    bytes for every batch and workers value, and equal RAFT.propagate on the whole clip.  Frames go in RGB with
+    model.upstream and BGR otherwise, like the CLI."""
+    from networks.utils import accumulate_flow, accumulate_flow_backward, propagate_labels
+    from .engine import FB_ALPHA1, FB_ALPHA2
+
+    paths = list_frames(frames)
+    F = len(paths)
+    if not (isinstance(frame, (int, np.integer)) and 0 <= frame < F):
+        raise ValueError(f"video_propagate: the key frame must be an integer in [0, {F}) (got {frame!r})")
+    if isinstance(labels, (str, os.PathLike)):
+        key, palette = read_labels(labels)
+    else:
+        key, palette = np.asarray(labels), None
+        if key.ndim != 2 or key.dtype != np.uint8:
+            raise ValueError(f"video_propagate: labels must be a PNG path or an [Hs,Ws] uint8 map (got {key.shape} "
+                             f"{key.dtype})")
+    batch, workers, frame = int(batch), _workers(workers), int(frame)
+    passes = interp_schedule(F, batch)
+    T = batch
+    j0 = min(frame // T, len(passes) - 1)  # the pass holding the key frame
+    out = os.fspath(out)
+    os.makedirs(out, exist_ok=True)
+    engine = model.engine()
+    rgb = bool(model.upstream)
+    dev = engine.device
+    kw = dict(flow_scale=engine.flow_scale, alpha1=FB_ALPHA1, alpha2=FB_ALPHA2)
+    names = [os.path.join(out, f"label_{i:06d}.png") for i in range(F)]
+
+    def write(slot, first, rows):  # writer thread: the label maps of one pass, once its copies have landed
+        slot.event.synchronize()
+        for r in rows:
+            write_labels(names[first + r], slot.labels[r].numpy(), palette)
+
+    state = {}
+
+    def run(sweep, backward):
+        with _Pipeline(paths, sweep, rgb, batch, workers, dev) as pipe:
+            for j, ps, imgs, frames in pipe:
+                if "key" not in state:
+                    if tuple(frames.shape[1:3]) != key.shape:
+                        raise ValueError(f"video_propagate: the key is {key.shape[0]}x{key.shape[1]}, the frames "
+                                         f"{frames.shape[1]}x{frames.shape[2]}")
+                    state["key"] = torch.from_numpy(np.ascontiguousarray(key)).to(dev)
+                flow_fw, flow_bw, _, _ = engine.forward_sequence_bidirectional(frames, check=False)
+                n_steps = sum(k is not None for k in ps.pairs)
+                first = ps.frames[0]
+                if "acc" not in state:
+                    H, W = flow_fw.shape[1:3]
+                    state["acc"] = torch.empty(T + 1, H, W, 2, dtype=torch.float32, device=dev)
+                    state["status"] = torch.empty(T + 1, H, W, dtype=torch.uint8, device=dev)
+                acc, status = state["acc"][:n_steps + 1], state["status"][:n_steps + 1]
+                if backward:  # the last row is the first row of the pass after this one
+                    acc[n_steps].copy_(state["carry_bw"][0])
+                    status[n_steps].copy_(state["carry_bw"][1])
+                    accumulate_flow_backward(flow_fw, flow_bw, acc, status, start=n_steps, n_steps=n_steps, **kw)
+                    rows = range(0, n_steps)
+                elif "carry_fw" not in state:  # the first pass of the forward sweep holds the key frame
+                    acc[frame - first].zero_()
+                    status[frame - first].zero_()
+                    accumulate_flow(flow_fw, flow_bw, acc, status, start=frame - first, n_steps=n_steps, **kw)
+                    accumulate_flow_backward(flow_fw, flow_bw, acc, status, start=frame - first, n_steps=n_steps, **kw)
+                    rows = range(0, n_steps + 1)
+                else:  # row 0 is the last row of the pass before
+                    acc[0].copy_(state["carry_fw"][0])
+                    status[0].copy_(state["carry_fw"][1])
+                    accumulate_flow(flow_fw, flow_bw, acc, status, start=0, n_steps=n_steps, **kw)
+                    rows = range(1, n_steps + 1)
+                if backward or "carry_fw" not in state:  # what the reverse sweep starts from
+                    state["carry_bw"] = (acc[0].clone(), status[0].clone())
+                if not backward:
+                    state["carry_fw"] = (acc[n_steps].clone(), status[n_steps].clone())
+                labels_out, st_out = propagate_labels(acc, status, state["key"])
+                if not backward:
+                    state["last"] = st_out[n_steps]
+                pipe.emit(partial(write, first=first, rows=rows), T + 1, labels=labels_out)
+
+    run(passes[j0:], backward=False)
+    if j0 > 0:
+        run(passes[:j0][::-1], backward=True)
+    return names, state["last"].cpu().numpy()
