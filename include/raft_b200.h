@@ -345,6 +345,30 @@ int rb_flow_accumulate_backward(const float* flow_fw, const float* flow_bw, int 
 int rb_labels_propagate(const float* acc, const uint8_t* status, int n, int H, int W, const uint8_t* key, int Hs, int Ws,
                         uint8_t* labels, uint8_t* status_out, void* stream);
 
+/* ---- F21: several keyframes -- each frame's labels voted between the keyframes on either side of it ---------------
+ * acc_a / acc_b [n,H,W,2] fp32 and status_a / status_b [n,H,W] uint8: row i's displacement to the keyframe before it
+ * (side A, F18's forward chain) and to the keyframe after it (side B, F18's backward chain) at the network size; keys
+ * [m,Hs,Ws] uint8 the keyframes' label maps at the frames' own size; rows [n,4] int32 in device memory, 16-byte aligned,
+ * per row (slot_a, slot_b, w_a, w_b): the key of each side, -1 for an absent side, and the two sides' integer weights;
+ * labels, status_out [n,Hs,Ws] uint8.  The C entry cannot read the device table: the kernel treats any slot outside
+ * [-1, m) as absent too, so a bad table is memory-safe.  Per output pixel p of row i and per present side, exactly
+ * rb_labels_propagate's work on that side's row and key: A' (rb_flow_resize's value), o = p + A' clamped, S = 2 if the
+ * clamp moved o else the side's status at the network pixel holding p's centre, and o's four taps with the bilinear
+ * weights (1-ax)(1-ay), ax(1-ay), (1-ax)ay, ax ay.  Then:
+ *   voters  = the present sides whose S is the smallest (0 consistent beats 1 occluded beats 2 entered at the edge);
+ *   one     : the vote of its four taps with its plain weights -- rb_labels_propagate's labels and status, bit for bit;
+ *   two     : side A's weights times fl32(w_a), side B's times fl32(w_b) (each product rounded on its own), the eight
+ *             candidates A00 A01 A10 A11 B00 B01 B10 B11 each score the sum, left to right, of the weights of the
+ *             candidates carrying its label; the largest score wins, a tie goes to the smaller label;
+ *   status_out = the smallest S; no present side: label 0, status 3.
+ * raft_b200.video.keyframe_rows builds the table: w_a = K_j - t and w_b = t - K_i for frame t between keys K_i and
+ * K_j, so the nearer key weighs more, and labels never blend into ids that do not exist.  Every operation is rounded on
+ * its own, no FMA contraction.  One thread per output pixel, blockIdx.y over the rows; no allocation.  Null pointers, a
+ * misaligned table, n/H/W/m/Hs/Ws <= 0 and Hs*Ws >= 2^32 -> RB_ERR_* before any CUDA call. */
+int rb_labels_propagate_keys(const float* acc_a, const uint8_t* status_a, const float* acc_b, const uint8_t* status_b,
+                             const int32_t* rows, int n, int H, int W, const uint8_t* keys, int m, int Hs, int Ws,
+                             uint8_t* labels, uint8_t* status_out, void* stream);
+
 /* ---- F6: frame interpolation -- flow_utils.py:166-274 reverse_flow_avg_skip_static, batched, and the frame blend -----
  * rb_flow_reverse: per sample of flow01 [B,H,W,2] fp32, bit for bit with the reference under numpy >= 2:
  *  1. static(p) = every channel c has d_c < 10, d_c = uint8(bg - im0) (img_u8 = 1: wraps, like numpy's uint8) or

@@ -88,9 +88,15 @@ vote of its four nearest pixels.  ``<--out>/label_<i:06d>.png`` is written for e
 
     python infer_raft.py --path frames/ --out labels/ --propagate key.png --load raft-things.npz [--batch 8]
 
+Several keyframes: --propagate K0.png K1.png ... --propagate-frame 0 8 ... (one frame per map, strictly increasing); each
+frame votes between the nearest keys before and after it.  With keyframes, --scene-cut THRESH stops propagation at scene
+cuts (the cuts are printed; pixels that no key reaches get label 0, and the final line counts them in the last frame).
+The single-key form is unchanged and refuses --scene-cut; video_propagate(..., scene_cut=THRESH) takes one key too.
+
 -m val --dataset davis scores it on DAVIS-2017's val split (raft_b200.davis): frame 0's annotation of every sequence
 propagated at 480p with 20 iterations, J&F printed (``Validation DAVIS-2017 (val): J&F: ...``) and written to
 ``<--out>/val_davis.json``, the predicted masks to ``<--out>/davis_val/<seq>/`` in DAVIS's results layout.
+--keyframe-step N uses the annotations of frames 0, N, 2N, ... as keyframes and scores the other frames.
 
 --native-frames (with --interpolate, or --path with --interpolate or --input-fps/--fps) writes the interpolated frames,
 and with --path the copied input frames, at the input's own size: the flow is estimated and reversed at the network size,
@@ -185,9 +191,10 @@ def parser():
                    help='extension, with --path and --input-fps: convert the frames to OUT frames per second (above IN), '
                         'written as <--out>/frame_<n:06d>.png')
     p.add_argument('--scene-cut', type=float, default=None, metavar='THRESH',
-                   help='extension, with --path and one of --interpolate, --input-fps/--fps or --warm-start: a threshold '
-                        'in [0, 1] on the colour-histogram score of each frame pair; a pair above it is a scene cut, '
-                        'where interpolation copies the nearer frame and warm-started flow restarts cold')
+                   help='extension, with --path and one of --interpolate, --input-fps/--fps, --warm-start or two or more '
+                        '--propagate maps: a threshold in [0, 1] on the colour-histogram score of each frame pair; a pair '
+                        'above it is a scene cut, where interpolation copies the nearer frame, warm-started flow restarts '
+                        'cold and no label crosses from a keyframe')
     p.add_argument('--native-flow', action='store_true',
                    help="extension: resize the written flow(s) back to im1's size (flow_utils.resize_flow)")
     p.add_argument('--native-frames', action='store_true',
@@ -207,11 +214,16 @@ def parser():
     p.add_argument('--track-backward', action='store_true',
                    help='extension, with --track or --track-grid: also track every point back from its frame to frame 0 '
                         '(a second flow sweep over the frames before the last query frame)')
-    p.add_argument('--propagate', default=None, metavar='KEY.png',
+    p.add_argument('--propagate', default=None, nargs='+', metavar='KEY.png',
                    help="extension, with --path: carry the label map KEY.png (palette or 8-bit grey, the frames' size) "
-                        "of frame --propagate-frame to every frame; writes <--out>/label_<i:06d>.png")
-    p.add_argument('--propagate-frame', type=int, default=None, metavar='K',
-                   help='extension, with --propagate: the frame the key labels belong to (default 0)')
+                        "of frame --propagate-frame to every frame; writes <--out>/label_<i:06d>.png.  Several maps are "
+                        "keyframes, one per --propagate-frame: each frame votes between the nearest two")
+    p.add_argument('--propagate-frame', type=int, nargs='+', default=None, metavar='K',
+                   help='extension, with --propagate: the frame each key label map belongs to (default 0; strictly '
+                        'increasing)')
+    p.add_argument('--keyframe-step', type=int, default=None, metavar='N',
+                   help='extension, -m val --dataset davis: the annotations of frames 0, N, 2N, ... are keyframes, the '
+                        'other frames are scored')
     p.add_argument('--upstream', action='store_true',
                    help='extension: weights converted from an official princeton-vl RAFT .pth (raft_b200.convert): RGB '
                         'frames and the upstream numerics (RAFT(..., upstream=True))')
@@ -231,13 +243,19 @@ def main(argv=None):
                              ('--track-frame', args.track_frame != 0), ('--track-vis', args.track_vis is not None),
                              ('--track-backward', args.track_backward), ('--interpolate', args.interpolate),
                              ('--fps', args.fps), ('--input-fps', args.input_fps), ('--warm-start', args.warm_start),
-                             ('--scene-cut', args.scene_cut is not None), ('--bidirectional', args.bidirectional),
+                             ('--bidirectional', args.bidirectional),
                              ('--native-flow', args.native_flow), ('--native-frames', args.native_frames),
                              ('--flo', args.flo), ('--npy', args.npy)):
             if given:
                 p.error(f'--propagate writes label maps: it cannot be combined with {other}')
+        if args.scene_cut is not None and len(args.propagate) == 1:  # the single-key form is kept as it was
+            p.error('--propagate with one key map cannot be combined with --scene-cut: scene cuts go with keyframes '
+                    '(two or more key maps and their --propagate-frame); for one key, video_propagate(..., '
+                    'scene_cut=THRESH) stops it at cuts')
         if args.batch < 1 or args.workers < 0:
             p.error('--path needs --batch >= 1 and --workers >= 0')
+        if args.scene_cut is not None and not 0.0 <= args.scene_cut <= 1.0:
+            p.error(f'--scene-cut: {args.scene_cut} is not a threshold in [0, 1]')
         return run_propagate(args, p)
     if args.propagate_frame is not None:
         p.error('--propagate-frame goes with --propagate')
@@ -325,6 +343,11 @@ def main(argv=None):
             p.error('--warm-start warm-starts flow validation; DAVIS propagates labels through cold flows')
     if args.query_mode is not None and (args.mode != 'val' or args.dataset != 'tapvid'):
         p.error('--query-mode goes with -m val --dataset tapvid')
+    if args.keyframe_step is not None:
+        if args.mode != 'val' or args.dataset != 'davis':
+            p.error('--keyframe-step goes with -m val --dataset davis')
+        if args.keyframe_step < 1:
+            p.error(f'--keyframe-step: the step must be >= 1 (got {args.keyframe_step})')
     if args.mode == 'val':
         return validate(args)
     if args.mode != 'test':
@@ -460,27 +483,44 @@ def run_track(args, p):
 
 def run_propagate(args, p):
     """--path --propagate: raft_b200.video.video_propagate over the frames of --path, at 432x1024 (or --flow-size) like
-    test mode (or their own size with --keep-size); the key and the written label maps are at the frames' own size.
-    Prints the frame count and how many pixels of the last frame are consistent (status 0) all the way to the key."""
+    test mode (or their own size with --keep-size); the keys and the written label maps are at the frames' own size.
+    Prints the frame count and how many pixels of the last frame are consistent (status 0) all the way to a key, and
+    with --scene-cut the cuts and how many of its pixels no key reaches (status 3)."""
     import cv2
     from raft_b200.video import list_frames, read_labels, video_propagate
+    frames = [0] if args.propagate_frame is None else args.propagate_frame
+    if len(frames) != len(args.propagate):
+        p.error(f'--propagate gives {len(args.propagate)} key label maps and --propagate-frame {len(frames)} frames: '
+                'the counts must match')
+    if any(b <= a for a, b in zip(frames, frames[1:])):
+        p.error(f'--propagate-frame {" ".join(map(str, frames))}: the key frames must be strictly increasing')
     try:
-        key, _ = read_labels(args.propagate)
+        keys = [read_labels(k)[0] for k in args.propagate]
         paths = list_frames(args.path)
     except (OSError, ValueError) as e:
         p.error(f'--propagate: {e}')
-    frame = 0 if args.propagate_frame is None else args.propagate_frame
-    if not 0 <= frame < len(paths):
-        p.error(f'--propagate-frame {frame}: {args.path} holds {len(paths)} frames')
+    for frame in frames:
+        if not 0 <= frame < len(paths):
+            p.error(f'--propagate-frame {frame}: {args.path} holds {len(paths)} frames')
     first = cv2.imread(paths[0], cv2.IMREAD_COLOR)
-    if first is not None and first.shape[:2] != key.shape:
-        p.error(f'--propagate: {args.propagate} is {key.shape[0]}x{key.shape[1]}, the frames of {args.path} are '
-                f'{first.shape[0]}x{first.shape[1]}; the key labels need the frames\' size')
+    for name, key in zip(args.propagate, keys):
+        if first is not None and first.shape[:2] != key.shape:
+            p.error(f'--propagate: {name} is {key.shape[0]}x{key.shape[1]}, the frames of {args.path} are '
+                    f'{first.shape[0]}x{first.shape[1]}; the key labels need the frames\' size')
     model = _video_model(args)
-    files, last = video_propagate(model, paths, args.out, args.propagate, frame=frame, batch=args.batch,
-                                  workers=args.workers)
-    print(f"labels of frame {frame} propagated through {len(files)} frames: {int((last == 0).sum())} of {last.size} "
-          f"pixels of the last frame consistent (status 0); written under {args.out}")
+    single = len(frames) == 1
+    res = video_propagate(model, paths, args.out, args.propagate[0] if single else args.propagate,
+                          frame=frames[0] if single else frames, batch=args.batch, workers=args.workers,
+                          scene_cut=args.scene_cut)
+    if args.scene_cut is not None:
+        files, last, cuts = res
+        _print_cuts(files, cuts)
+    else:
+        files, last = res
+    which = f"frame {frames[0]}" if single else f"frames {', '.join(map(str, frames))}"
+    unreached = f", {int((last == 3).sum())} reached by no key (status 3)" if args.scene_cut is not None else ""
+    print(f"labels of {which} propagated through {len(files)} frames: {int((last == 0).sum())} of {last.size} "
+          f"pixels of the last frame consistent (status 0){unreached}; written under {args.out}")
     return 0
 
 
@@ -517,7 +557,8 @@ def validate(args):
         return 0
     res = evaluate(model, args.data, args.dataset, dstypes=tuple(args.dstype), batch=args.batch, workers=args.workers,
                    iters=args.iters, warm_start=args.warm_start, query_mode=args.query_mode,
-                   masks_out=os.path.join(args.out, 'davis_val') if args.dataset == 'davis' else None)
+                   masks_out=os.path.join(args.out, 'davis_val') if args.dataset == 'davis' else None,
+                   keyframe_step=args.keyframe_step)
     for line in summary_lines(res):
         print(line)
     os.makedirs(args.out, exist_ok=True)

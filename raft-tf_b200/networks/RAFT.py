@@ -172,7 +172,7 @@ class RAFT(object):
         return self.engine().track(_as_tensor(frames), queries, backward=bool(backward))
 
     @torch.no_grad()
-    def propagate(self, frames, labels, frame=0):
+    def propagate(self, frames, labels, frame=0, cuts=None):
         """Extension (keyframe label propagation): the [Hs,Ws] uint8 label map `labels` of frame `frame` (a segmentation
         mask, a class map, ...) carried through all of [F,Hs,Ws,3] frames (dtypes and sources as for ``forward``).  One
         ``forward_sequence_bidirectional`` pass; per pixel of every frame, the displacement back to the keyframe composed
@@ -180,8 +180,14 @@ class RAFT(object):
         (RaftEngine.propagate).  Returns fresh (labels [F,Hs,Ws] uint8, status [F,Hs,Ws] uint8) CUDA tensors at the frames'
         own size (with input_size too): status 0 consistent at every step back to the keyframe, 1 occluded at some step,
         2 entered through the frame edge; labels[frame] equals the key.  A key that is not [Hs,Ws] uint8 or a frame
-        outside [0, F) raises ValueError."""
-        return self.engine().propagate(_as_tensor(frames), labels, frame=frame)
+        outside [0, F) raises ValueError.
+
+        Several keyframes (an annotation every N-th frame): labels [m,Hs,Ws] uint8 and frame a strictly increasing
+        sequence of m frame indices.  Each frame takes its labels from the nearest keyframe before it and the nearest
+        after it, a vote weighted toward the nearer one, and never from a keyframe on the other side of a scene cut
+        (cuts: pair indices k, the cut between frames k and k + 1).  Status 3 (label 0): no keyframe reaches the frame.
+        Wrong counts, orders, shapes or cuts raise ValueError before the flow pass."""
+        return self.engine().propagate(_as_tensor(frames), labels, frame=frame, cuts=cuts)
 
     @torch.no_grad()
     def interpolate_sequence(self, frames, t=0.5, uint8=False, bgr=False, native=False):

@@ -215,6 +215,56 @@ def propagate_labels(acc, status, key):
     return labels, st
 
 
+def propagate_labels_keys(acc_a, status_a, acc_b, status_b, keys, rows):
+    """Extension (several keyframes): the labels of every row voted between the keyframes on either side of it
+    (rb_labels_propagate_keys).  acc_a / status_a and acc_b / status_b: [n,H,W,2] fp32 and [n,H,W] uint8 CUDA rows of
+    accumulate_flow's forward chain from the key before each row (side A) and accumulate_flow_backward's chain from the
+    key after it (side B); keys [m,Hs,Ws] uint8 the keyframes' label maps at the frames' own size; rows [n,4] int32 per
+    row (slot_a, slot_b, w_a, w_b): the key index of each side (-1: absent) and, where both are present, their positive
+    integer weights (raft_b200.video.keyframe_rows builds it).  Per pixel the present sides with the smallest status vote
+    -- one alone with propagate_labels' bits, two over their eight taps with side A's bilinear weights times w_a and side
+    B's times w_b.  Returns fresh (labels [n,Hs,Ws] uint8, status [n,Hs,Ws] uint8): the smallest status of the voters,
+    3 (label 0) where no side is present.  Bad shapes or a bad table raise ValueError before the upload."""
+    if not (isinstance(acc_a, torch.Tensor) and acc_a.is_cuda and acc_a.dim() == 4 and acc_a.shape[-1] == 2
+            and acc_a.dtype == torch.float32):
+        raise ValueError(f"propagate_labels_keys: acc_a must be an [n,H,W,2] float32 CUDA tensor (got "
+                         f"{getattr(acc_a, 'shape', None)} {getattr(acc_a, 'dtype', type(acc_a))})")
+    n, H, W, _ = acc_a.shape
+    dev = acc_a.device
+    if not (isinstance(acc_b, torch.Tensor) and acc_b.shape == acc_a.shape and acc_b.dtype == torch.float32
+            and acc_b.device == dev):
+        raise ValueError(f"propagate_labels_keys: acc_b must be an [n,H,W,2] = {[n, H, W, 2]} float32 tensor on {dev}")
+    for name, t in (("status_a", status_a), ("status_b", status_b)):
+        if not (isinstance(t, torch.Tensor) and tuple(t.shape) == (n, H, W) and t.dtype == torch.uint8
+                and t.device == dev):
+            raise ValueError(f"propagate_labels_keys: {name} must be an [n,H,W] = {[n, H, W]} uint8 tensor on {dev}")
+    if not (isinstance(keys, torch.Tensor) and keys.dim() == 3 and keys.shape[0] >= 1 and keys.dtype == torch.uint8
+            and keys.device == dev):
+        raise ValueError(f"propagate_labels_keys: keys must be an [m,Hs,Ws] uint8 tensor on {dev} (got "
+                         f"{getattr(keys, 'shape', None)} {getattr(keys, 'dtype', type(keys))})")
+    m, Hs, Ws = keys.shape
+    table = torch.as_tensor(rows).cpu()
+    if not (tuple(table.shape) == (n, 4) and not table.is_floating_point() and not table.is_complex()):
+        raise ValueError(f"propagate_labels_keys: rows must be an [n,4] = {[n, 4]} integer table (got "
+                         f"{list(table.shape)} {table.dtype})")
+    table = table.to(torch.int64)
+    sa, sb, wa, wb = table.unbind(1)
+    if not (((sa >= -1) & (sa < m)).all() and ((sb >= -1) & (sb < m)).all()):
+        raise ValueError(f"propagate_labels_keys: the slots must be key indices in [0, {m}) or -1 (absent)")
+    both = (sa >= 0) & (sb >= 0)
+    if not (((wa > 0) & (wa < 1 << 24) & (wb > 0) & (wb < 1 << 24)) | ~both).all():
+        raise ValueError("propagate_labels_keys: where both sides are present, the weights must be integers in [1, 2^24)")
+    table = table.to(device=dev, dtype=torch.int32).contiguous()
+    aa, a_s, ab, b_s, k = (t.contiguous() for t in (acc_a, status_a, acc_b, status_b, keys))
+    labels = torch.empty(n, Hs, Ws, dtype=torch.uint8, device=dev)
+    st = torch.empty_like(labels)
+    with torch.cuda.device(dev):
+        capi.check(capi.lib.rb_labels_propagate_keys(capi.ptr(aa), capi.ptr(a_s), capi.ptr(ab), capi.ptr(b_s),
+                                                     capi.ptr(table), n, H, W, capi.ptr(k), m, Hs, Ws,
+                                                     capi.ptr(labels), capi.ptr(st), capi.stream()))
+    return labels, st
+
+
 LABEL_STATS = ("intersection", "union", "boundary_pred", "boundary_gt", "matched_pred", "matched_gt")  # RB_LABEL_STATS
 
 

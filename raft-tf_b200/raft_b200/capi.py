@@ -75,6 +75,7 @@ SIGNATURES = {
     "rb_flow_accumulate": (_i, [_vp, _vp, _i, _i, _i, _i, _f, _f, _f, _i, _vp, _vp, _vp]),
     "rb_flow_accumulate_backward": (_i, [_vp, _vp, _i, _i, _i, _i, _f, _f, _f, _i, _vp, _vp, _vp]),
     "rb_labels_propagate": (_i, [_vp, _vp, _i, _i, _i, _vp, _i, _i, _vp, _vp, _vp]),
+    "rb_labels_propagate_keys": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _vp, _i, _i, _i, _vp, _vp, _vp]),
     "rb_flow_reverse_workspace_bytes": (_i, [_i, _i, _i, _psz]),
     "rb_flow_reverse": (_i, [_vp, _vp, _vp, _i, _i, _f, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _vp, _sz, _vp]),
     "rb_frame_synthesize": (_i, [_vp, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _f, _vp, _i, _i, _i, _vp]),

@@ -8,7 +8,9 @@ Data: the sequences of <root>/ImageSets/2017/val.txt, frames <root>/JPEGImages/4
 stem, is checked up front.
 
 Protocol: frame 0's annotation is propagated forward through the sequence at the frames' own size, 20 iterations,
-'sintel' padding (PROTOCOLS["davis"]).  The flows come from interp_schedule(F, batch) passes of
+'sintel' padding (PROTOCOLS["davis"]).  With keyframe_step N (F21) the annotations of frames 0, N, 2N, ... < F are the
+keyframes, each frame votes between the nearest two (RaftEngine.propagate with a list of keys), and the keyframes are
+dropped from the scored frames.  The flows come from interp_schedule(F, batch) passes of
 forward_sequence_bidirectional(check=False); each pass continues the accumulation from the last row of the one before
 (rb_flow_accumulate) and labels its rows (rb_labels_propagate), so the predictions are the same bits for every batch.
 The void label 255 of an annotation is background.  With masks_out the predictions of every frame are written in DAVIS's
@@ -132,42 +134,50 @@ def aggregate_davis(records):
 
 
 # ---- prediction ------------------------------------------------------------------------------------------------------
-def propagate_clip(engine, frames, key, batch=1):
-    """Frame 0's [Hs,Ws] uint8 labels `key` propagated through frames [F,Hs,Ws,3] uint8 (the engine's channel order, numpy
-    or torch) in interp_schedule(F, batch) passes, the accumulation carried from pass to pass on the GPU.  Returns (labels
-    [F,Hs,Ws] uint8, status [F,Hs,Ws] uint8) CUDA tensors: RaftEngine.propagate(frames, key, 0)'s bits for every batch."""
-    from networks.utils import accumulate_flow, propagate_labels
-    from .engine import FB_ALPHA1, FB_ALPHA2
-    from .video import interp_schedule
+def propagate_clip(engine, frames, key, batch=1, frame=0):
+    """The [Hs,Ws] uint8 labels `key` of frame `frame` (or the [m,Hs,Ws] keys of the strictly increasing frames `frame`)
+    propagated through frames [F,Hs,Ws,3] uint8 (the engine's channel order, numpy or torch) in interp_schedule(F, batch)
+    passes, the accumulation carried from pass to pass on the GPU (raft_b200.video.KeyframeSweep).  Returns (labels
+    [F,Hs,Ws] uint8, status [F,Hs,Ws] uint8) CUDA tensors: RaftEngine.propagate(frames, key, frame)'s bits for every
+    batch."""
+    from .video import KeyframeSweep, check_keyframes, interp_schedule
     F = len(frames)
+    K = check_keyframes(frame, F, "DAVIS")
     dev = engine.device
-    kw = dict(flow_scale=engine.flow_scale, alpha1=FB_ALPHA1, alpha2=FB_ALPHA2)
     with torch.cuda.device(dev):
         clip = torch.as_tensor(np.ascontiguousarray(frames) if isinstance(frames, np.ndarray) else frames).to(dev)
-        key = torch.as_tensor(np.ascontiguousarray(key)).to(dev)
-        labels = torch.empty(F, *key.shape, dtype=torch.uint8, device=dev)
+        keys = torch.as_tensor(np.ascontiguousarray(key) if isinstance(key, np.ndarray) else key).to(dev)
+        keys = keys[None] if keys.dim() == 2 else keys
+        labels = torch.empty(F, *keys.shape[1:], dtype=torch.uint8, device=dev)
         status = torch.empty_like(labels)
-        acc = st = None
-        for ps in interp_schedule(F, batch):
-            fw, bw, _, _ = engine.forward_sequence_bidirectional(clip[ps.frames], check=False)
-            n = sum(k is not None for k in ps.pairs)
-            first = ps.frames[0]
-            if acc is None:
-                acc = torch.zeros(batch + 1, *fw.shape[1:], dtype=torch.float32, device=dev)
-                st = torch.zeros(batch + 1, *fw.shape[1:3], dtype=torch.uint8, device=dev)
-            else:  # row 0 is the last row of the pass before
-                acc[0].copy_(acc[last])
-                st[0].copy_(st[last])
-            accumulate_flow(fw, bw, acc[:n + 1], st[:n + 1], start=0, n_steps=n, **kw)
-            lab, s = propagate_labels(acc[:n + 1], st[:n + 1], key)
-            labels[first:first + n + 1], status[first:first + n + 1] = lab, s
-            last = n
+        sweep = KeyframeSweep(engine, keys, K, F, batch, [], simple=isinstance(frame, (int, np.integer)))
+        passes = interp_schedule(F, batch)
+        j0 = sweep.first_pass(len(passes))
+        for part, step in ((passes[j0:], sweep.forward), (passes[:j0][::-1], sweep.reverse)):
+            for ps in part:
+                fw, bw, _, _ = engine.forward_sequence_bidirectional(clip[ps.frames], check=False)
+                for a, lab, st in step(ps, fw, bw):
+                    labels[a:a + len(lab)], status[a:a + len(lab)] = lab, st
     return labels, status
 
 
-def run(engine, seqs, batch=1, rgb=False, masks_out=None):
+def keyframe_frames(F, step):
+    """The keyframes of a clip of F frames annotated every `step` frames: 0, step, 2 step, ... < F."""
+    return list(range(0, int(F), int(step)))
+
+
+def scored_frames(F, keyframes=(0,)):
+    """The frames DAVIS scores: 1 .. F - 2 (the evaluator drops the first and the last), minus the keyframes."""
+    keys = set(keyframes)
+    return [t for t in range(1, F - 1) if t not in keys]
+
+
+def run(engine, seqs, batch=1, rgb=False, masks_out=None, keyframe_step=None):
     """Every sequence of davis_sequences() through propagate_clip (frames in RGB with rgb, else BGR) and scored by
-    rb_label_metrics: returns the per-sequence records, in list order, each {name, n_frames, n_objects, objects: [...]}."""
+    rb_label_metrics: returns the per-sequence records, in list order, each {name, n_frames, n_objects, objects: [...]}.
+    keyframe_step N propagates the annotations of frames 0, N, 2N, ... < F as keyframes (each frame votes between the
+    nearest two) and scores frames 1 .. F-2 minus those keyframes, in order; the objects stay frame 0's (labels above
+    them in later keys are propagated, not scored), so numbers compare across steps."""
     from networks.utils import davis_bound_pix, label_metrics
     from .evaluate import _imread
     from .video import read_labels, write_labels
@@ -187,11 +197,18 @@ def run(engine, seqs, batch=1, rgb=False, masks_out=None):
         gt[gt == 255] = 0
         n_obj = int(gt[0].max())
         F, H, W = gt.shape
-        pred, _ = propagate_clip(engine, frames, gt[0], batch)
+        if keyframe_step is None:
+            pred, _ = propagate_clip(engine, frames, gt[0], batch)
+            scored = list(range(1, F - 1))
+        else:
+            K = keyframe_frames(F, keyframe_step)
+            pred, _ = propagate_clip(engine, frames, gt[K], batch, frame=K)
+            scored = scored_frames(F, K)
         objects = [dict(zip(SUMMARY[1:], (float("nan"),) * 6)) for _ in range(n_obj)]
-        if n_obj and F > 2:
+        if n_obj and scored:
             with torch.cuda.device(engine.device):
-                counts = label_metrics(pred[1:-1], torch.from_numpy(gt[1:-1]).to(engine.device), n_obj,
+                idx = torch.tensor(scored, device=engine.device)
+                counts = label_metrics(pred[idx], torch.from_numpy(gt[scored]).to(engine.device), n_obj,
                                        davis_bound_pix(H, W)).cpu().numpy()
             J, Fm = frame_scores(counts)
             for o in range(n_obj):

@@ -530,7 +530,7 @@ class RaftEngine:
             return tracks_to_frames(tracks, src_hw, net_hw), status
 
     @torch.no_grad()
-    def propagate(self, frames: torch.Tensor, labels, frame: int = 0):
+    def propagate(self, frames: torch.Tensor, labels, frame=0, cuts=None):
         """Keyframe label propagation: the [Hs,Ws] uint8 label map `labels` of frame `frame` carried to every one of the
         [F,Hs,Ws,3] frames (dtypes, sizes and input_size as for forward()).  One forward_sequence_bidirectional(check=False)
         pass; a zero row at `frame`, one rb_flow_accumulate and one rb_flow_accumulate_backward launch on its flows
@@ -538,28 +538,65 @@ class RaftEngine:
         at the frames' own size.  Returns fresh (labels [F,Hs,Ws] uint8, status [F,Hs,Ws] uint8) CUDA tensors: status 0
         consistent at every step back to the keyframe, 1 occluded at some step, 2 entered through the frame edge at some
         step; labels[frame] equals the key bit for bit.  A key that is not [Hs,Ws] uint8 or a frame outside [0, F) raises
-        ValueError before the pass."""
-        from networks.utils import accumulate_flow, accumulate_flow_backward, propagate_labels
+        ValueError before the pass.
+
+        Several keyframes: labels [m,Hs,Ws] uint8 and frame a strictly increasing sequence of m frame indices; cuts an
+        iterable of scene-cut pairs (pair k between frames k and k + 1).  Each frame votes between the keyframes on
+        either side of it that no cut separates from it (raft_b200.video.keyframe_rows): after the same pass, a zero row
+        at every key, rb_flow_accumulate from each key to the frame before the next one and rb_flow_accumulate_backward
+        from each key to the frame after the previous one (slices of the same flows), then one rb_labels_propagate_keys
+        launch.  Status 3 (label 0): no keyframe reaches the frame.  A one-element list without cuts gives the single-key
+        bits.  A count mismatch, keys not strictly increasing or outside [0, F), a key of the wrong size or dtype, or a
+        cut outside [0, F - 1) raises ValueError before the pass."""
+        from networks.utils import accumulate_flow, accumulate_flow_backward, propagate_labels, propagate_labels_keys
+        from .video import check_cuts, check_keyframes, keyframe_rows
         F = _sequence_length(frames) + 1
         Hs, Ws = frames.shape[1:3]
         key = torch.as_tensor(labels)
-        if not (key.dim() == 2 and key.dtype == torch.uint8 and tuple(key.shape) == (Hs, Ws)):
-            raise ValueError(f"raft_b200: the key labels must be an [Hs,Ws] = [{Hs},{Ws}] uint8 map (got "
-                             f"{list(key.shape)} {key.dtype})")
-        if not (isinstance(frame, (int, np.integer)) and 0 <= frame < F):
-            raise ValueError(f"raft_b200: the key frame must be an integer in [0, {F}) (got {frame!r})")
-        frame = int(frame)
+        several = cuts is not None or not isinstance(frame, (int, np.integer))
+        if not several:
+            if not (key.dim() == 2 and key.dtype == torch.uint8 and tuple(key.shape) == (Hs, Ws)):
+                raise ValueError(f"raft_b200: the key labels must be an [Hs,Ws] = [{Hs},{Ws}] uint8 map (got "
+                                 f"{list(key.shape)} {key.dtype})")
+            if not (0 <= frame < F):
+                raise ValueError(f"raft_b200: the key frame must be an integer in [0, {F}) (got {frame!r})")
+        else:
+            K = check_keyframes(frame, F, "raft_b200")
+            cuts = check_cuts(() if cuts is None else cuts, F, "raft_b200")
+            if key.dim() == 2 and isinstance(frame, (int, np.integer)):
+                key = key[None]
+            if not (key.dim() == 3 and key.dtype == torch.uint8 and tuple(key.shape[1:]) == (Hs, Ws)):
+                raise ValueError(f"raft_b200: the key labels must be an [m,Hs,Ws] = [m,{Hs},{Ws}] uint8 stack (got "
+                                 f"{list(key.shape)} {key.dtype})")
+            if key.shape[0] != len(K):
+                raise ValueError(f"raft_b200: {key.shape[0]} key label maps for {len(K)} key frames")
+        frame = int(frame) if not several else None
         flow_fw, flow_bw, _, _ = self.forward_sequence_bidirectional(frames, check=False)
         T, H, W = flow_fw.shape[:3]
+        kw = dict(flow_scale=self.flow_scale, alpha1=FB_ALPHA1, alpha2=FB_ALPHA2)
         with torch.cuda.device(self.device):
-            acc = torch.empty(F, H, W, 2, dtype=torch.float32, device=self.device)
-            status = torch.empty(F, H, W, dtype=torch.uint8, device=self.device)
-            acc[frame].zero_()
-            status[frame].zero_()
-            kw = dict(start=frame, flow_scale=self.flow_scale, alpha1=FB_ALPHA1, alpha2=FB_ALPHA2)
-            accumulate_flow(flow_fw, flow_bw, acc, status, **kw)
-            accumulate_flow_backward(flow_fw, flow_bw, acc, status, **kw)
-            return propagate_labels(acc, status, key.to(self.device))
+            if not several:
+                acc = torch.empty(F, H, W, 2, dtype=torch.float32, device=self.device)
+                status = torch.empty(F, H, W, dtype=torch.uint8, device=self.device)
+                acc[frame].zero_()
+                status[frame].zero_()
+                accumulate_flow(flow_fw, flow_bw, acc, status, start=frame, **kw)
+                accumulate_flow_backward(flow_fw, flow_bw, acc, status, start=frame, **kw)
+                return propagate_labels(acc, status, key.to(self.device))
+            acc = torch.empty(2, F, H, W, 2, dtype=torch.float32, device=self.device)  # side A, side B
+            status = torch.empty(2, F, H, W, dtype=torch.uint8, device=self.device)
+            for i, k in enumerate(K):
+                acc[:, k].zero_()
+                status[:, k].zero_()
+                hi = K[i + 1] - 1 if i + 1 < len(K) else F - 1  # side A of frames k .. hi
+                if hi > k:
+                    accumulate_flow(flow_fw[k:hi], flow_bw[k:hi], acc[0, k:hi + 1], status[0, k:hi + 1], **kw)
+                lo = K[i - 1] + 1 if i > 0 else 0  # side B of frames lo .. k - 1
+                if k > lo:
+                    accumulate_flow_backward(flow_fw[lo:k], flow_bw[lo:k], acc[1, lo:k + 1], status[1, lo:k + 1],
+                                             start=k - lo, **kw)
+            return propagate_labels_keys(acc[0], status[0], acc[1], status[1], key.to(self.device),
+                                         keyframe_rows(F, K, cuts))
 
     @torch.no_grad()
     def interpolate(self, left: torch.Tensor, right: torch.Tensor, ts, native: bool = False) -> torch.Tensor:

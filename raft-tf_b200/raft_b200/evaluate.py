@@ -442,7 +442,7 @@ def _engine(model, n_iters, pad_mode, input_size=None):
 
 
 def evaluate(model, root, dataset="sintel", dstypes=DSTYPES, batch=1, workers=4, iters=None, warm_start=False,
-             query_mode=None, masks_out=None):
+             query_mode=None, masks_out=None, keyframe_step=None):
     """Upstream RAFT's validation of a loaded networks.RAFT.RAFT model on a Sintel or KITTI-2015 training tree, or the
     interpolation quality on a Vimeo-90K triplet tree (dataset 'vimeo').
 
@@ -469,13 +469,20 @@ def evaluate(model, root, dataset="sintel", dstypes=DSTYPES, batch=1, workers=4,
     through the sequence at its own size and scored by J and F (raft_b200.davis); returns {"dataset", "iters",
     "pad_mode", "splits": {"val": aggregate_davis(...)}}.  masks_out (a directory) also receives the predicted masks in
     DAVIS's results layout.  dstypes and workers are ignored and warm_start raises ValueError; masks_out is refused for
-    the other datasets."""
+    the other datasets.  keyframe_step N (an integer >= 1) propagates the annotations of frames 0, N, 2N, ... as
+    keyframes instead and scores the other frames (raft_b200.davis.run); the result then records "keyframe_step"."""
     if masks_out is not None and dataset != "davis":
         raise ValueError(f"evaluate: masks_out writes DAVIS-2017 predictions (got dataset {dataset!r})")
     if query_mode is not None and dataset != "tapvid":
         raise ValueError(f"evaluate: query_mode belongs to TAP-Vid's point tracking (got dataset {dataset!r})")
     if dataset == "tapvid" and query_mode not in (None,) + QUERY_MODES:
         raise ValueError(f"evaluate: query_mode must be one of {QUERY_MODES} (got {query_mode!r})")
+    if keyframe_step is not None:
+        if dataset != "davis":
+            raise ValueError(f"evaluate: keyframe_step belongs to DAVIS-2017 label propagation (got dataset {dataset!r})")
+        if isinstance(keyframe_step, bool) or int(keyframe_step) != keyframe_step or int(keyframe_step) < 1:
+            raise ValueError(f"evaluate: keyframe_step must be an integer >= 1 (got {keyframe_step!r})")
+        keyframe_step = int(keyframe_step)
     kitti, splits, n_iters, pad_mode = _setup(model, dataset, dstypes, batch, workers, iters, warm_start, "evaluate")
     if dataset == "tapvid":
         from . import tapvid
@@ -489,9 +496,11 @@ def evaluate(model, root, dataset="sintel", dstypes=DSTYPES, batch=1, workers=4,
         from . import davis
         seqs = davis.davis_sequences(root)  # every file checked up front
         engine = _engine(model, n_iters, pad_mode)
-        records = davis.run(engine, seqs, int(batch), model.upstream, masks_out)
-        return {"dataset": dataset, "iters": n_iters, "pad_mode": pad_mode,
-                "splits": {"val": davis.aggregate_davis(records)}}
+        records = davis.run(engine, seqs, int(batch), model.upstream, masks_out, keyframe_step)
+        res = {"dataset": dataset, "iters": n_iters, "pad_mode": pad_mode}
+        if keyframe_step is not None:
+            res["keyframe_step"] = keyframe_step
+        return {**res, "splits": {"val": davis.aggregate_davis(records)}}
     if dataset == "vimeo":
         trips = vimeo_triplets(root)  # every file checked up front
         engine = _engine(model, n_iters, pad_mode)
@@ -586,10 +595,11 @@ def summary_lines(res):
     """upstream evaluate.py's lines: 'Validation (clean) EPE: ..., 1px: ..., 3px: ..., 5px: ...' per Sintel pass,
     'Validation KITTI: <epe>, <f1>'; for Vimeo-90K 'Validation Vimeo-90K: PSNR: ..., SSIM: ...'; and for TAP-Vid
     'Validation TAP-Vid (<query mode>): AJ: ..., <δ_avg>: ..., OA: ...'; for DAVIS-2017
-    'Validation DAVIS-2017 (val): J&F: ..., J: ..., F: ...'."""
+    'Validation DAVIS-2017 (val): J&F: ..., J: ..., F: ...' ('(val, a keyframe every N)' with keyframe_step N)."""
     if res["dataset"] == "davis":
         r = res["splits"]["val"]
-        return ["Validation DAVIS-2017 (val): J&F: %f, J: %f, F: %f" % (r["J&F-Mean"], r["J-Mean"], r["F-Mean"])]
+        split = "val" if res.get("keyframe_step") is None else f"val, a keyframe every {res['keyframe_step']}"
+        return ["Validation DAVIS-2017 (%s): J&F: %f, J: %f, F: %f" % (split, r["J&F-Mean"], r["J-Mean"], r["F-Mean"])]
     if res["dataset"] == "tapvid":
         r = res["splits"]["tapvid"]
         return ["Validation TAP-Vid (%s): AJ: %f, <δ_avg>: %f, OA: %f" % (res["query_mode"], r["average_jaccard"],

@@ -31,6 +31,8 @@ out/status.npy.
 video_propagate(model, "frames/", "out/", "key.png", frame=K) carries frame K's label map to every frame: the same passes,
 each followed by rb_flow_accumulate (and, before the key frame, rb_flow_accumulate_backward) launches that carry the
 per-pixel displacement to the key frame on the GPU and one rb_labels_propagate launch, written as out/label_<i:06d>.png.
+With several keyframes (frame=[K_0, K_1, ...]) every frame votes between the nearest keys on either side
+(keyframe_rows(), KeyframeSweep, rb_labels_propagate_keys), and scene_cut keeps labels from crossing a cut.
 
 Scene cuts (scene_cut=<threshold in [0, 1]>, video_interpolate and warm-started video): each pass's decoded frames are
 copied to the GPU once and scored there (networks.utils.scene_cut_scores: one minus the intersection of consecutive
@@ -690,7 +692,214 @@ def write_labels(path, labels, palette=None):
     im.save(os.fspath(path), format="PNG")
 
 
-def video_propagate(model, frames, out, labels, frame=0, batch=8, workers=4):
+def check_keyframes(frames, F, what="video_propagate"):
+    """The keyframe indices as a list of ints: one int, or a strictly increasing sequence of at least one index, each in
+    [0, F).  Anything else raises ValueError."""
+    seq = [frames] if isinstance(frames, (int, np.integer)) else frames
+    try:
+        keys = list(seq)
+    except TypeError:
+        keys = None
+    if not keys or not all(isinstance(k, (int, np.integer)) and not isinstance(k, bool) for k in keys):
+        raise ValueError(f"{what}: the key frames must be an integer or a sequence of integers (got {frames!r})")
+    keys = [int(k) for k in keys]
+    if not all(0 <= k < F for k in keys) or any(b <= a for a, b in zip(keys, keys[1:])):
+        raise ValueError(f"{what}: the key frames must be strictly increasing integers in [0, {F}) (got {keys})")
+    return keys
+
+
+def check_cuts(cuts, F, what="video_propagate"):
+    """Scene-cut pairs as a sorted list of distinct ints in [0, F - 1) (pair k: frames k and k + 1).  Anything else
+    raises ValueError."""
+    try:
+        cuts = list(cuts)
+        cs = [int(c) for c in cuts if not isinstance(c, bool) and int(c) == c]
+        ok = len(cs) == len(cuts)
+    except (TypeError, ValueError):
+        ok = False
+    if not ok or not all(0 <= c < F - 1 for c in cs):
+        raise ValueError(f"{what}: the cuts must be integer pair indices in [0, {F - 1}) (got {cuts!r})")
+    return sorted(set(cs))
+
+
+def keyframe_rows(F, frames, cuts=()):
+    """The per-frame table of several-keyframe propagation (rb_labels_propagate_keys' rows): [F,4] int32, row t =
+    (slot_a, slot_b, w_a, w_b).  With keyframes K_0 < ... < K_(m-1) (frames) and the cut pairs `cuts` (pair k between
+    frames k and k + 1):
+      side A = i, the latest key K_i <= t, when no cut lies among pairs K_i .. t - 1, else -1;
+      side B = j, the earliest key K_j > t, when no cut lies among pairs t .. K_j - 1, else -1;
+      a keyframe row t = K_i has side A only (its key, bit for bit);
+      w_a = K_j - t and w_b = t - K_i when both sides are present (the nearer key weighs more), else 0.
+    A row without sides (only possible with cuts) gets label 0 and status 3."""
+    keys = np.asarray(check_keyframes(frames, F, "keyframe_rows"), dtype=np.int64)
+    cuts = np.asarray(check_cuts(cuts, F, "keyframe_rows"), dtype=np.int64)
+    t = np.arange(int(F), dtype=np.int64)
+    i = np.searchsorted(keys, t, side="right") - 1  # latest K_i <= t
+    j = i + 1  # earliest K_j > t
+    has_a = i >= 0
+    has_b = j < len(keys)
+    ka = keys[np.clip(i, 0, None)]
+    kb = keys[np.clip(j, None, len(keys) - 1)]
+    n_cuts_before = np.searchsorted(cuts, t, side="left")  # cuts < t, i.e. pairs .. t - 1
+    has_a &= np.searchsorted(cuts, ka, side="left") == n_cuts_before  # no cut in [K_i, t)
+    has_b &= np.searchsorted(cuts, kb, side="left") == n_cuts_before  # no cut in [t, K_j)
+    has_b &= ~np.isin(t, keys)
+    both = has_a & has_b
+    return np.stack([np.where(has_a, i, -1), np.where(has_b, j, -1), np.where(both, kb - t, 0),
+                     np.where(both, t - ka, 0)], axis=1).astype(np.int32)
+
+
+class KeyframeSweep:
+    """The GPU side of streaming keyframe propagation over interp_schedule(F, T) passes (video_propagate and
+    raft_b200.davis.propagate_clip): the labels of every frame with the bits of RaftEngine.propagate on the whole clip.
+
+        sweep = KeyframeSweep(engine, keys, K, F, T, cuts)
+        for ps in sweep.forward_passes(passes):  # flows of each: forward_sequence_bidirectional(check=False)
+            chunks = sweep.forward(ps, flow_fw, flow_bw)
+        for ps in sweep.reverse_passes(passes):  # the passes before the first key's, last to first
+            chunks = sweep.reverse(ps, flow_fw, flow_bw)
+
+    Each call returns the frames it completes as chunks (first frame, labels [n,Hs,Ws], status [n,Hs,Ws]) of device
+    tensors, valid until the next call.  `cuts` is a list the caller extends with each pass's cut pairs before the call.
+    - Frames before the first key K_0 take side B from K_0 alone: the pass holding K_0 chains back from it, and the
+      reverse sweep carries that chain to frame 0 (as video_track(backward=True) does).
+    - Frames from the last key K_(m-1) on take side A from it alone: a forward chain carried from pass to pass.
+    - Between K_0 and K_(m-1) the flows of the current keyframe interval are copied to the device as their passes arrive;
+      when the next key is reached, both chains run over the interval, one rb_labels_propagate_keys launch labels its
+      frames, and the store is reused.  Memory therefore grows with the longest keyframe interval L, not the clip: 16 B
+      per network pixel per pair for the two flows and 18 B per pixel per frame for the two chains, about 15 MB per
+      interval frame at 432x1024 (by arithmetic).
+    With one key and no scene-cut detection (simple) this is the single-key path: one chain buffer per pass and
+    rb_labels_propagate."""
+
+    def __init__(self, engine, keys, K, F, T, cuts, simple):
+        from .engine import FB_ALPHA1, FB_ALPHA2
+        self.keys, self.K, self.F, self.T, self.cuts, self.simple = keys, list(K), int(F), int(T), cuts, simple
+        self.kw = dict(flow_scale=engine.flow_scale, alpha1=FB_ALPHA1, alpha2=FB_ALPHA2)
+        self.dev = engine.device
+        self.L = max((b - a for a, b in zip(self.K, self.K[1:])), default=0)  # the longest interval
+        self.acc = self.store = None
+        self.cur, self.next_pair = 0, self.K[0]  # the interval being stored, the next pair it needs
+        self.carry_fw = self.carry_bw = None
+
+    def first_pass(self, n_passes):
+        """The pass the forward sweep starts at: the one holding K_0 (the last pass when K_0 is the last frame)."""
+        return min(self.K[0] // self.T, n_passes - 1)
+
+    def _buffers(self, H, W):
+        if self.acc is None:
+            self.acc = torch.empty(self.T + 1, H, W, 2, dtype=torch.float32, device=self.dev)
+            self.status = torch.empty(self.T + 1, H, W, dtype=torch.uint8, device=self.dev)
+            if self.L:
+                self.store = torch.empty(2, self.L, H, W, 2, dtype=torch.float32, device=self.dev)  # flow_fw, flow_bw
+                self.ia = torch.empty(2, self.L + 1, H, W, 2, dtype=torch.float32, device=self.dev)  # side A, side B
+                self.ist = torch.empty(2, self.L + 1, H, W, dtype=torch.uint8, device=self.dev)
+
+    def _one_sided(self, first, n, acc, status):
+        """Labels of the pass rows first .. first + n (one chain buffer, the head's and the tail's rows): the table of
+        keyframe_rows with the rows between K_0 and K_(m-1) absent (the intervals label those)."""
+        from networks.utils import propagate_labels, propagate_labels_keys
+        if self.simple:
+            return propagate_labels(acc, status, self.keys[0])
+        rows = keyframe_rows(self.F, self.K, self.cuts)[first:first + n + 1].copy()
+        t = np.arange(first, first + n + 1)
+        rows[(t >= self.K[0]) & (t < self.K[-1])] = (-1, -1, 0, 0)
+        return propagate_labels_keys(acc, status, acc, status, self.keys, rows)
+
+    def forward(self, ps, flow_fw, flow_bw):
+        from networks.utils import accumulate_flow, accumulate_flow_backward
+        n = sum(k is not None for k in ps.pairs)
+        first, K0, Kl = ps.frames[0], self.K[0], self.K[-1]
+        self._buffers(*flow_fw.shape[1:3])
+        acc, status, kw = self.acc[:n + 1], self.status[:n + 1], self.kw
+        chunks, pass_rows = [], []
+        if self.carry_bw is None:  # the pass holding K_0: side B of the frames before it
+            acc[K0 - first].zero_()
+            status[K0 - first].zero_()
+            accumulate_flow_backward(flow_fw, flow_bw, acc, status, start=K0 - first, n_steps=n, **kw)
+            self.carry_bw = (acc[0].clone(), status[0].clone())
+            pass_rows.append((first, K0))
+        if self.carry_fw is not None:  # past K_(m-1): row 0 is the last row of the pass before
+            acc[0].copy_(self.carry_fw[0])
+            status[0].copy_(self.carry_fw[1])
+            accumulate_flow(flow_fw, flow_bw, acc, status, start=0, n_steps=n, **kw)
+            pass_rows.append((first + 1, first + n + 1))
+        elif first <= Kl <= first + n:  # the pass holding K_(m-1): side A from it
+            acc[Kl - first].zero_()
+            status[Kl - first].zero_()
+            accumulate_flow(flow_fw, flow_bw, acc, status, start=Kl - first, n_steps=n, **kw)
+            pass_rows.append((Kl, first + n + 1))
+        if any(a < b for a, b in pass_rows):
+            self.carry_fw = (acc[n].clone(), status[n].clone()) if pass_rows[-1][1] == first + n + 1 else None
+            labels, st = self._one_sided(first, n, acc, status)
+            chunks += [(a, labels[a - first:b - first], st[a - first:b - first]) for a, b in pass_rows if a < b]
+        p = max(first, self.next_pair)  # the interval store: pairs K_0 .. K_(m-1) - 1
+        while p < min(first + n, Kl):
+            Ki, Kj = self.K[self.cur], self.K[self.cur + 1]
+            end = min(first + n, Kj)
+            self.store[0, p - Ki:end - Ki].copy_(flow_fw[p - first:end - first])
+            self.store[1, p - Ki:end - Ki].copy_(flow_bw[p - first:end - first])
+            p = end
+            if end == Kj:
+                chunks.append(self._interval(Ki, Kj))
+                self.cur += 1
+        self.next_pair = p
+        return sorted(chunks, key=lambda c: c[0])
+
+    def _interval(self, Ki, Kj):
+        """Both chains over the stored flows of pairs Ki .. Kj - 1 and the labels of frames Ki .. Kj - 1."""
+        from networks.utils import accumulate_flow, accumulate_flow_backward, propagate_labels_keys
+        L = Kj - Ki
+        fw, bw = self.store[0, :L], self.store[1, :L]
+        self.ia[:, 0].zero_()  # side A of frames Ki .. Kj - 1 in rows 0 .. L - 1
+        self.ist[:, 0].zero_()
+        self.ia[1, L].zero_()  # side B of frames Ki + 1 .. Kj in rows 1 .. L
+        self.ist[1, L].zero_()
+        if L > 1:
+            accumulate_flow(fw, bw, self.ia[0, :L], self.ist[0, :L], start=0, n_steps=L - 1, **self.kw)
+            accumulate_flow_backward(fw[1:], bw[1:], self.ia[1, 1:L + 1], self.ist[1, 1:L + 1], start=L - 1,
+                                     **self.kw)
+        rows = keyframe_rows(self.F, self.K, self.cuts)[Ki:Kj]
+        labels, st = propagate_labels_keys(self.ia[0, :L], self.ist[0, :L], self.ia[1, :L], self.ist[1, :L],
+                                           self.keys, rows)
+        return Ki, labels, st
+
+    def reverse(self, ps, flow_fw, flow_bw):
+        from networks.utils import accumulate_flow_backward
+        n = sum(k is not None for k in ps.pairs)
+        first = ps.frames[0]
+        acc, status = self.acc[:n + 1], self.status[:n + 1]
+        acc[n].copy_(self.carry_bw[0])  # the last row is the first row of the pass after this one
+        status[n].copy_(self.carry_bw[1])
+        accumulate_flow_backward(flow_fw, flow_bw, acc, status, start=n, n_steps=n, **self.kw)
+        self.carry_bw = (acc[0].clone(), status[0].clone())
+        labels, st = self._one_sided(first, n, acc, status)
+        return [(first, labels[:n], st[:n])]
+
+
+def _read_keys(labels, frame, F, what):
+    """video_propagate's keys: (K, [m,Hs,Ws] uint8 array, palette of the first PNG or None)."""
+    several = not isinstance(frame, (int, np.integer))
+    K = check_keyframes(frame, F, what)
+    items = list(labels) if several and not isinstance(labels, (str, os.PathLike)) else [labels]
+    if len(items) != len(K):
+        raise ValueError(f"{what}: {len(items)} key label maps for {len(K)} key frames")
+    keys, palette = [], None
+    for i, item in enumerate(items):
+        if isinstance(item, (str, os.PathLike)):
+            key, pal = read_labels(item)
+            palette = pal if i == 0 else palette
+        else:
+            key = np.asarray(item)
+            if key.ndim != 2 or key.dtype != np.uint8:
+                raise ValueError(f"{what}: labels must be PNG paths or [Hs,Ws] uint8 maps (got {key.shape} {key.dtype})")
+        if keys and key.shape != keys[0].shape:
+            raise ValueError(f"{what}: the key label maps differ in size ({keys[0].shape} and {key.shape})")
+        keys.append(key)
+    return K, np.stack(keys), palette
+
+
+def video_propagate(model, frames, out, labels, frame=0, batch=8, workers=4, scene_cut=None):
     """Keyframe label propagation through a video of any length with a loaded networks.RAFT.RAFT model: the label map of
     frame `frame` (`labels`: a palette or grey PNG path, or an [Hs,Ws] uint8 array at the frames' size) carried to every
     frame (a directory's sorted *.png / *.jpg, or a list of paths, all of one size).  Writes <out>/label_<i:06d>.png for
@@ -705,82 +914,76 @@ def video_propagate(model, frames, out, labels, frame=0, batch=8, workers=4):
     launch from the first row of the pass after it (as video_track(backward=True) does), so frame = 0 costs nothing
     more.  Every row's labels come from one rb_labels_propagate launch at the frames' own size.  The files are the same
     bytes for every batch and workers value, and equal RAFT.propagate on the whole clip.  Frames go in RGB with
-    model.upstream and BGR otherwise, like the CLI."""
-    from networks.utils import accumulate_flow, accumulate_flow_backward, propagate_labels
-    from .engine import FB_ALPHA1, FB_ALPHA2
+    model.upstream and BGR otherwise, like the CLI.
+
+    Several keyframes: `labels` a list of PNG paths or maps (or an [m,Hs,Ws] array) and `frame` the strictly increasing
+    list of their frames; the files are in the first PNG's palette.  Each frame votes between the nearest keyframes
+    before and after it (RAFT.propagate with a list; KeyframeSweep streams it).  The flows of one keyframe interval are
+    kept on the GPU until the next key is reached, so memory is bounded by the longest interval, not the clip: 16 B per
+    network pixel per pair plus 18 B per pixel per frame, about 15 MB per interval frame at 432x1024 (by arithmetic).
+
+    scene_cut (a threshold in [0, 1]) scores each pass's decoded frames on the GPU (networks.utils.scene_cut_scores; the
+    reverse sweep scores its own passes), and no frame takes labels from a keyframe across a cut pair: the files are
+    RAFT.propagate(..., cuts=<the cuts found>)'s, status 3 (label 0) where no keyframe reaches a frame.  It then returns
+    (paths, last status, cuts), cuts the increasing cut pairs."""
+    from networks.utils import scene_cut_scores
 
     paths = list_frames(frames)
     F = len(paths)
-    if not (isinstance(frame, (int, np.integer)) and 0 <= frame < F):
-        raise ValueError(f"video_propagate: the key frame must be an integer in [0, {F}) (got {frame!r})")
-    if isinstance(labels, (str, os.PathLike)):
-        key, palette = read_labels(labels)
-    else:
-        key, palette = np.asarray(labels), None
-        if key.ndim != 2 or key.dtype != np.uint8:
-            raise ValueError(f"video_propagate: labels must be a PNG path or an [Hs,Ws] uint8 map (got {key.shape} "
-                             f"{key.dtype})")
-    batch, workers, frame = int(batch), _workers(workers), int(frame)
+    K, keys_np, palette = _read_keys(labels, frame, F, "video_propagate")
+    thr = None if scene_cut is None else check_scene_cut(scene_cut)
+    batch, workers = int(batch), _workers(workers)
     passes = interp_schedule(F, batch)
-    T = batch
-    j0 = min(frame // T, len(passes) - 1)  # the pass holding the key frame
     out = os.fspath(out)
     os.makedirs(out, exist_ok=True)
     engine = model.engine()
     rgb = bool(model.upstream)
     dev = engine.device
-    kw = dict(flow_scale=engine.flow_scale, alpha1=FB_ALPHA1, alpha2=FB_ALPHA2)
     names = [os.path.join(out, f"label_{i:06d}.png") for i in range(F)]
+    cuts, last = [], None
+    with torch.cuda.device(dev):
+        keys = torch.from_numpy(np.ascontiguousarray(keys_np)).to(dev)
+    sweep = KeyframeSweep(engine, keys, K, F, batch, cuts, simple=len(K) == 1 and thr is None)
+    j0 = sweep.first_pass(len(passes))
+    rows = batch + 1 + sweep.L  # the most frames one pass completes
 
-    def write(slot, first, rows):  # writer thread: the label maps of one pass, once its copies have landed
+    def write(slot, spans):  # writer thread: the label maps a pass completed, once its copies have landed
+        if slot is None:
+            return
         slot.event.synchronize()
-        for r in rows:
-            write_labels(names[first + r], slot.labels[r].numpy(), palette)
+        r = 0
+        for a, n in spans:
+            for f in range(a, a + n):
+                write_labels(names[f], slot.labels[r].numpy(), palette)
+                r += 1
 
-    state = {}
+    def run(sweep_passes, step):
+        nonlocal last
+        on_dev = None
+        with _Pipeline(paths, sweep_passes, rgb, batch, workers, dev) as pipe:
+            for j, ps, imgs, src in pipe:
+                if j == 0 and tuple(src.shape[1:3]) != keys_np.shape[1:]:
+                    raise ValueError(f"video_propagate: the key is {keys_np.shape[1]}x{keys_np.shape[2]}, the frames "
+                                     f"{src.shape[1]}x{src.shape[2]}")
+                if thr is not None:  # score the pass on the GPU; the engine then reads the frames from there too
+                    if on_dev is None:
+                        on_dev = torch.empty(src.shape, dtype=torch.uint8, device=dev)
+                    on_dev.copy_(src, non_blocking=True)
+                    src = on_dev
+                    cuts.extend(pass_cuts(ps.pairs, scene_cut_scores(on_dev).cpu(), thr))
+                    cuts.sort()
+                flow_fw, flow_bw, _, _ = engine.forward_sequence_bidirectional(src, check=False)
+                chunks = step(ps, flow_fw, flow_bw)
+                spans = [(a, len(lab)) for a, lab, _ in chunks]
+                for a, lab, st in chunks:
+                    if a + len(lab) == F:
+                        last = st[-1].clone()
+                labels_out = (None if not chunks else chunks[0][1] if len(chunks) == 1
+                              else torch.cat([lab for _, lab, _ in chunks]))
+                pipe.emit(partial(write, spans=spans), rows, labels=labels_out)
 
-    def run(sweep, backward):
-        with _Pipeline(paths, sweep, rgb, batch, workers, dev) as pipe:
-            for j, ps, imgs, frames in pipe:
-                if "key" not in state:
-                    if tuple(frames.shape[1:3]) != key.shape:
-                        raise ValueError(f"video_propagate: the key is {key.shape[0]}x{key.shape[1]}, the frames "
-                                         f"{frames.shape[1]}x{frames.shape[2]}")
-                    state["key"] = torch.from_numpy(np.ascontiguousarray(key)).to(dev)
-                flow_fw, flow_bw, _, _ = engine.forward_sequence_bidirectional(frames, check=False)
-                n_steps = sum(k is not None for k in ps.pairs)
-                first = ps.frames[0]
-                if "acc" not in state:
-                    H, W = flow_fw.shape[1:3]
-                    state["acc"] = torch.empty(T + 1, H, W, 2, dtype=torch.float32, device=dev)
-                    state["status"] = torch.empty(T + 1, H, W, dtype=torch.uint8, device=dev)
-                acc, status = state["acc"][:n_steps + 1], state["status"][:n_steps + 1]
-                if backward:  # the last row is the first row of the pass after this one
-                    acc[n_steps].copy_(state["carry_bw"][0])
-                    status[n_steps].copy_(state["carry_bw"][1])
-                    accumulate_flow_backward(flow_fw, flow_bw, acc, status, start=n_steps, n_steps=n_steps, **kw)
-                    rows = range(0, n_steps)
-                elif "carry_fw" not in state:  # the first pass of the forward sweep holds the key frame
-                    acc[frame - first].zero_()
-                    status[frame - first].zero_()
-                    accumulate_flow(flow_fw, flow_bw, acc, status, start=frame - first, n_steps=n_steps, **kw)
-                    accumulate_flow_backward(flow_fw, flow_bw, acc, status, start=frame - first, n_steps=n_steps, **kw)
-                    rows = range(0, n_steps + 1)
-                else:  # row 0 is the last row of the pass before
-                    acc[0].copy_(state["carry_fw"][0])
-                    status[0].copy_(state["carry_fw"][1])
-                    accumulate_flow(flow_fw, flow_bw, acc, status, start=0, n_steps=n_steps, **kw)
-                    rows = range(1, n_steps + 1)
-                if backward or "carry_fw" not in state:  # what the reverse sweep starts from
-                    state["carry_bw"] = (acc[0].clone(), status[0].clone())
-                if not backward:
-                    state["carry_fw"] = (acc[n_steps].clone(), status[n_steps].clone())
-                labels_out, st_out = propagate_labels(acc, status, state["key"])
-                if not backward:
-                    state["last"] = st_out[n_steps]
-                pipe.emit(partial(write, first=first, rows=rows), T + 1, labels=labels_out)
-
-    run(passes[j0:], backward=False)
+    run(passes[j0:], sweep.forward)
     if j0 > 0:
-        run(passes[:j0][::-1], backward=True)
-    return names, state["last"].cpu().numpy()
+        run(passes[:j0][::-1], sweep.reverse)
+    last = last.cpu().numpy()
+    return (names, last) if thr is None else (names, last, cuts)
