@@ -369,6 +369,44 @@ int rb_labels_propagate_keys(const float* acc_a, const uint8_t* status_a, const 
                              const int32_t* rows, int n, int H, int W, const uint8_t* keys, int m, int Hs, int Ws,
                              uint8_t* labels, uint8_t* status_out, void* stream);
 
+/* ---- F22: global motion -- a robust similarity fit of each frame pair's camera motion to its flow -----------------
+ * flow_fw [B,Hn,Wn,2] fp32 on the network grid and occ_fw [B,Hn,Wn] uint8 (rb_flow_fb_check's masks) of B pairs whose
+ * frames are Hs x Ws.  In the frames' own pixels, centred on ((Ws-1)/2, (Hs-1)/2): network pixel (i, j) is the point
+ * p = ((j+0.5) Ws/Wn - 0.5, (i+0.5) Hs/Hn - 0.5) - centre (cv2's pixel-centre rule) and its target q = p + flow_scale
+ * (u Ws/Wn, v Hs/Hn).  The similarity M = [[a, -b, tx], [b, a, ty]] (frame k -> frame k+1) is fitted by weighted least
+ * squares from the 8 sums (RB_MOTION_SUMS, in this order) S = sum w, sum w px, sum w py, sum w |p|^2,
+ * sum w (px qx + py qy), sum w (px qy - py qx), sum w qx, sum w qy, solved in fp64 in closed form:
+ *   a = (U S - X Qx - Y Qy) / D,  b = (V S - X Qy + Y Qx) / D,  D = P S - X^2 - Y^2,
+ *   tx = (Qx - a X + b Y) / S,    ty = (Qy - b X - a Y) / S.
+ * Round 0 weighs a pixel by 1 where occ == 0 and the flow is finite, else 0; rounds 1..rounds by that times the Cauchy
+ * weight 1 / (1 + (r / cauchy_c)^2), r = |M p - q| of the previous round in network pixels (x divided by Ws/Wn, y by
+ * Hs/Hn).  Outputs: params [B,4] fp64 (a, b, tx, ty); weight [B] fp64, round 0's S / (Hn Wn); flags [B] uint8, 1 for an
+ * unreliable pair -- weight below min_weight, or a singular system in any round (S = 0 or D <= 1e-9 P S) -- which gets
+ * the identity (1, 0, 0, 0); sums (nullable) [B,8] fp64, the last round's sums.  Per round, a chunk launch reduces
+ * fixed 4096-pixel chunks of each pair in fp64 in a fixed tree into the workspace (rb_global_motion_workspace_bytes) and
+ * a per-pair launch adds them in a fixed order and solves; the rounds stay on the device (no synchronisation), the
+ * chunking depends on Hn x Wn only, so a pair's bits depend neither on B nor on its place in the batch; no allocation,
+ * no atomics.  Null pointers, B/Hn/Wn/Hs/Ws <= 0, B > 65535, flow_scale or cauchy_c <= 0 or non-finite, rounds outside
+ * [0, RB_MOTION_MAX_ROUNDS], min_weight outside [0, 1] and a workspace that is too small -> RB_ERR_* before any CUDA
+ * call. */
+#define RB_MOTION_SUMS 8
+#define RB_MOTION_MAX_ROUNDS 32
+int rb_global_motion_workspace_bytes(int B, int Hn, int Wn, size_t* bytes);
+int rb_global_motion(const float* flow_fw, const uint8_t* occ_fw, int B, int Hn, int Wn, int Hs, int Ws, float flow_scale,
+                     int rounds, double cauchy_c, double min_weight, double* params, double* weight, uint8_t* flags,
+                     double* sums, void* workspace, size_t workspace_bytes, void* stream);
+
+/* ---- F23: affine warp of uint8 frames -- the stabilized frames at their own size ----------------------------------
+ * frames, out: [F,H,W,C] uint8 (C in [1, 4], any channel order), out not aliasing frames; A: [F,2,3] fp64 in device
+ * memory, per frame the matrix from an output pixel (x, y) (uncentred, integer) to its source position:
+ *   sx = fl64(fl64(A00 x) + fl64(A01 y)) + A02,  sy likewise with row 1 (each operation rounded on its own, no FMA),
+ * rounded once to fp32, clamped into [0, W-1] x [0, H-1] (the border replicates; NaN -> 0), and sampled per channel with
+ * fb_sample.cuh's bilinear taps on the byte values as fp32 (rounded on its own), then rintf and clamped to [0, 255].
+ * The identity returns the frame byte for byte.  One thread per output pixel, blockIdx.y over the frames; no
+ * allocation.  Null pointers, F/H/W <= 0, F > 65535, H or W >= 2^24 and C outside [1, 4] -> RB_ERR_* before any CUDA
+ * call. */
+int rb_frames_warp_affine(const uint8_t* frames, const double* A, int F, int H, int W, int C, uint8_t* out, void* stream);
+
 /* ---- F6: frame interpolation -- flow_utils.py:166-274 reverse_flow_avg_skip_static, batched, and the frame blend -----
  * rb_flow_reverse: per sample of flow01 [B,H,W,2] fp32, bit for bit with the reference under numpy >= 2:
  *  1. static(p) = every channel c has d_c < 10, d_c = uint8(bg - im0) (img_u8 = 1: wraps, like numpy's uint8) or

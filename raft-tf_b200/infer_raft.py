@@ -93,6 +93,16 @@ frame votes between the nearest keys before and after it.  With keyframes, --sce
 cuts (the cuts are printed; pixels that no key reaches get label 0, and the final line counts them in the last frame).
 The single-key form is unchanged and refuses --scene-cut; video_propagate(..., scene_cut=THRESH) takes one key too.
 
+--path DIR --stabilize SIGMA removes the camera's shake from DIR's frames: each consecutive pair's camera motion (a
+similarity: zoom, rotation, shift) is fitted robustly on the GPU to the flow of its consistent pixels, the camera path is
+smoothed by a Gaussian of SIGMA frames (no default: pick it for the footage; larger is steadier), and every frame is
+warped at its own size by its correction, zoomed just enough to hide the borders up to --stabilize-zoom Z (default 1.25).
+``<--out>/frame_<i:06d>.png`` and ``<--out>/transforms.npy`` [F,2,3] are written, and the zoom per shot, the cuts and the
+number of unreliable pairs printed; with --scene-cut THRESH the path restarts at every cut (raft_b200.video.
+video_stabilize):
+
+    python infer_raft.py --path frames/ --out stable/ --stabilize 10 --load raft-things.npz [--batch 8]
+
 -m val --dataset davis scores it on DAVIS-2017's val split (raft_b200.davis): frame 0's annotation of every sequence
 propagated at 480p with 20 iterations, J&F printed (``Validation DAVIS-2017 (val): J&F: ...``) and written to
 ``<--out>/val_davis.json``, the predicted masks to ``<--out>/davis_val/<seq>/`` in DAVIS's results layout.
@@ -107,6 +117,7 @@ then resized inside the blend, which warps the decoded frames.  --flow-size H W 
 """
 import glob
 import argparse
+import math
 import os
 import sys
 from fractions import Fraction
@@ -191,10 +202,11 @@ def parser():
                    help='extension, with --path and --input-fps: convert the frames to OUT frames per second (above IN), '
                         'written as <--out>/frame_<n:06d>.png')
     p.add_argument('--scene-cut', type=float, default=None, metavar='THRESH',
-                   help='extension, with --path and one of --interpolate, --input-fps/--fps, --warm-start or two or more '
-                        '--propagate maps: a threshold in [0, 1] on the colour-histogram score of each frame pair; a pair '
-                        'above it is a scene cut, where interpolation copies the nearer frame, warm-started flow restarts '
-                        'cold and no label crosses from a keyframe')
+                   help='extension, with --path and one of --interpolate, --input-fps/--fps, --warm-start, '
+                        '--stabilize or two or more --propagate maps: a threshold in [0, 1] on the colour-histogram '
+                        'score of each frame pair; a pair above it is a scene cut, where interpolation copies the nearer '
+                        'frame, warm-started flow restarts cold, the stabilized camera path restarts and no label '
+                        'crosses from a keyframe')
     p.add_argument('--native-flow', action='store_true',
                    help="extension: resize the written flow(s) back to im1's size (flow_utils.resize_flow)")
     p.add_argument('--native-frames', action='store_true',
@@ -224,6 +236,13 @@ def parser():
     p.add_argument('--keyframe-step', type=int, default=None, metavar='N',
                    help='extension, -m val --dataset davis: the annotations of frames 0, N, 2N, ... are keyframes, the '
                         'other frames are scored')
+    p.add_argument('--stabilize', type=float, default=None, metavar='SIGMA',
+                   help="extension, with --path: stabilize the frames, smoothing the camera path with a Gaussian of "
+                        "SIGMA frames (no default); writes <--out>/frame_<i:06d>.png at the frames' own size and "
+                        "<--out>/transforms.npy")
+    p.add_argument('--stabilize-zoom', type=float, default=None, metavar='Z',
+                   help='extension, with --stabilize: the largest zoom per shot that hides the borders (default 1.25; '
+                        'past it the border replicates)')
     p.add_argument('--upstream', action='store_true',
                    help='extension: weights converted from an official princeton-vl RAFT .pth (raft_b200.convert): RGB '
                         'frames and the upstream numerics (RAFT(..., upstream=True))')
@@ -236,6 +255,32 @@ def parser():
 def main(argv=None):
     p = parser()
     args = p.parse_args(argv)
+    if args.stabilize is not None:
+        if args.path is None or args.mode != 'test':
+            p.error('--stabilize stabilizes a frame directory: it needs --path DIR (and no -m val)')
+        for other, given in (('--propagate', args.propagate is not None),
+                             ('--propagate-frame', args.propagate_frame is not None),
+                             ('--track', args.track is not None), ('--track-grid', args.track_grid is not None),
+                             ('--track-frame', args.track_frame != 0), ('--track-vis', args.track_vis is not None),
+                             ('--track-backward', args.track_backward), ('--interpolate', args.interpolate),
+                             ('--fps', args.fps), ('--input-fps', args.input_fps), ('--warm-start', args.warm_start),
+                             ('--bidirectional', args.bidirectional), ('--native-flow', args.native_flow),
+                             ('--native-frames', args.native_frames), ('--flo', args.flo), ('--npy', args.npy)):
+            if given:
+                p.error(f'--stabilize writes stabilized frames: it cannot be combined with {other}')
+        if not (math.isfinite(args.stabilize) and args.stabilize > 0):
+            p.error(f'--stabilize: SIGMA must be a number of frames > 0 (got {args.stabilize})')
+        if args.stabilize_zoom is not None and not (math.isfinite(args.stabilize_zoom) and args.stabilize_zoom >= 1):
+            p.error(f'--stabilize-zoom: Z must be a zoom >= 1 (got {args.stabilize_zoom})')
+        if args.scene_cut is not None and not 0.0 <= args.scene_cut <= 1.0:
+            p.error(f'--scene-cut: {args.scene_cut} is not a threshold in [0, 1]')
+        if args.flow_size is not None and args.keep_size:
+            p.error('--flow-size sets the size frames are resized to; --keep-size runs them at their own size')
+        if args.batch < 1 or args.workers < 0:
+            p.error('--path needs --batch >= 1 and --workers >= 0')
+        return run_stabilize(args)
+    if args.stabilize_zoom is not None:
+        p.error('--stabilize-zoom goes with --stabilize')
     if args.propagate is not None:
         if args.path is None or args.mode != 'test':
             p.error('--propagate carries labels through a frame directory: it needs --path DIR (and no -m val)')
@@ -521,6 +566,17 @@ def run_propagate(args, p):
     unreached = f", {int((last == 3).sum())} reached by no key (status 3)" if args.scene_cut is not None else ""
     print(f"labels of {which} propagated through {len(files)} frames: {int((last == 0).sum())} of {last.size} "
           f"pixels of the last frame consistent (status 0){unreached}; written under {args.out}")
+    return 0
+
+
+def run_stabilize(args):
+    """--path --stabilize: raft_b200.video.video_stabilize over the frames of --path, the flow at 432x1024 (or
+    --flow-size) like test mode (or the frames' own size with --keep-size), the frames written at their own size."""
+    from raft_b200.video import video_stabilize
+    model = _video_model(args)
+    files, _ = video_stabilize(model, args.path, args.out, args.stabilize, batch=args.batch, workers=args.workers,
+                               scene_cut=args.scene_cut, max_zoom=args.stabilize_zoom)
+    print(f"{len(files)} stabilized frames and transforms.npy written under {args.out}")
     return 0
 
 

@@ -190,6 +190,19 @@ class RAFT(object):
         return self.engine().propagate(_as_tensor(frames), labels, frame=frame, cuts=cuts)
 
     @torch.no_grad()
+    def stabilize(self, frames, sigma, cuts=None, max_zoom=None):
+        """Extension (video stabilization): [F,Hs,Ws,3] uint8 frames (sources as for ``forward``) with the camera's
+        shake removed.  One ``forward_sequence_bidirectional`` pass; per pair a similarity (zoom, rotation, shift) fitted
+        robustly on the GPU to the flow of its consistent pixels; the camera path, restarted at every scene cut (cuts:
+        pair indices k, the cut between frames k and k + 1), smoothed by a Gaussian of sigma frames; and every frame
+        warped at its own size (with input_size too) by its correction and one zoom per shot that keeps the borders out
+        of view, up to max_zoom (default raft_b200.stabilize.DEFAULT_MAX_ZOOM; past it the border replicates)
+        (RaftEngine.stabilize).  Returns fresh (frames [F,Hs,Ws,3] uint8, transforms [F,2,3] fp64) CUDA tensors, each
+        transform mapping an output pixel to its source position.  Non-uint8 frames, a bad sigma, max_zoom or cuts raise
+        ValueError before the flow pass."""
+        return self.engine().stabilize(_as_tensor(frames), sigma, cuts=cuts, max_zoom=max_zoom)
+
+    @torch.no_grad()
     def interpolate_sequence(self, frames, t=0.5, uint8=False, bgr=False, native=False):
         """Extension (frame-rate up-conversion): the frames at time t (a float, or a sequence of times, each in [0, 1])
         between every pair of consecutive frames of [T+1,H,W,3] frames, from one ``forward_sequence_bidirectional`` pass.

@@ -526,3 +526,75 @@ def resize_flow(flow, size):
     with torch.cuda.device(flow.device):
         capi.check(capi.lib.rb_flow_resize(capi.ptr(flow), capi.ptr(out), B, H, W, Ho, Wo, capi.stream()))
     return out
+
+
+MOTION_SUMS = 8  # RB_MOTION_SUMS
+
+
+def global_motion(flow_fw, occ_fw, frame_hw, flow_scale=1.0, rounds=None, cauchy_c=None, min_weight=None,
+                  return_sums=False):
+    """Extension (video stabilization): the camera motion of B frame pairs, a similarity M = [[a, -b, tx], [b, a, ty]]
+    from frame k to frame k + 1 fitted robustly to each pair's flow on the GPU (rb_global_motion).  flow_fw [B,Hn,Wn,2]
+    fp32 CUDA flows on the network grid (forward_sequence_bidirectional's) and occ_fw [B,Hn,Wn] uint8 their
+    forward-backward masks (only pixels with 0 count); frame_hw = (Hs, Ws), the frames' own size, in whose pixels,
+    centred on the frame centre, the similarity is expressed.  flow_scale as in fb_consistency.  A plain least-squares
+    round, then `rounds` Cauchy reweighting rounds of scale cauchy_c network pixels, all on the device (defaults:
+    raft_b200.stabilize's MOTION_ROUNDS, MOTION_CAUCHY, MOTION_MIN_WEIGHT, chosen on synthetic flows only).  Returns
+    fresh (params [B,4] fp64 (a, b, tx, ty), weight [B] fp64, the fraction of consistent pixels, reliable [B] bool);
+    an unreliable pair (weight below min_weight, or a singular fit) has the identity.  With return_sums also the [B,8]
+    fp64 weighted sums of the last round (MOTION_SUMS in rb_global_motion's order).  Wrong shapes or dtypes raise
+    ValueError."""
+    from raft_b200.stabilize import MOTION_CAUCHY, MOTION_MIN_WEIGHT, MOTION_ROUNDS
+    if not (isinstance(flow_fw, torch.Tensor) and flow_fw.is_cuda and flow_fw.dim() == 4 and flow_fw.shape[-1] == 2
+            and flow_fw.dtype == torch.float32):
+        raise ValueError(f"global_motion: flow_fw must be a [B,Hn,Wn,2] float32 CUDA tensor (got "
+                         f"{getattr(flow_fw, 'shape', None)} {getattr(flow_fw, 'dtype', type(flow_fw))})")
+    B, Hn, Wn, _ = flow_fw.shape
+    dev = flow_fw.device
+    if not (isinstance(occ_fw, torch.Tensor) and tuple(occ_fw.shape) == (B, Hn, Wn) and occ_fw.dtype == torch.uint8
+            and occ_fw.device == dev):
+        raise ValueError(f"global_motion: occ_fw must be a [B,Hn,Wn] = {[B, Hn, Wn]} uint8 tensor on {dev}")
+    try:
+        Hs, Ws = (int(v) for v in frame_hw)
+    except (TypeError, ValueError):
+        raise ValueError(f"global_motion: frame_hw must be (Hs, Ws) (got {frame_hw!r})") from None
+    if Hs < 1 or Ws < 1:
+        raise ValueError(f"global_motion: frame_hw must be positive (got {frame_hw!r})")
+    rounds = MOTION_ROUNDS if rounds is None else int(rounds)
+    cauchy_c = MOTION_CAUCHY if cauchy_c is None else float(cauchy_c)
+    min_weight = MOTION_MIN_WEIGHT if min_weight is None else float(min_weight)
+    f, o = flow_fw.contiguous(), occ_fw.contiguous()
+    params = torch.empty(B, 4, dtype=torch.float64, device=dev)
+    weight = torch.empty(B, dtype=torch.float64, device=dev)
+    flags = torch.empty(B, dtype=torch.uint8, device=dev)
+    sums = torch.empty(B, MOTION_SUMS, dtype=torch.float64, device=dev) if return_sums else None
+    with torch.cuda.device(dev):
+        nbytes = capi.size_query(capi.lib.rb_global_motion_workspace_bytes, B, Hn, Wn)
+        ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+        capi.check(capi.lib.rb_global_motion(capi.ptr(f), capi.ptr(o), B, Hn, Wn, Hs, Ws, float(flow_scale), rounds,
+                                             cauchy_c, min_weight, capi.ptr(params), capi.ptr(weight), capi.ptr(flags),
+                                             capi.ptr(sums), capi.ptr(ws), nbytes, capi.stream()))
+    out = (params, weight, flags == 0)
+    return out + (sums,) if return_sums else out
+
+
+def warp_frames(frames, A):
+    """Extension (video stabilization): every frame of [F,H,W,C] uint8 CUDA frames (C in 1..4, any channel order) warped
+    by its [2,3] matrix of A [F,2,3] (fp64, host or device), which maps an output pixel (x, y) to its source position in
+    the frame's own pixels (rb_frames_warp_affine): the position in fp64, rounded once to fp32, clamped into the frame
+    (the border replicates), sampled bilinearly and rounded to bytes.  The identity returns the frames byte for byte.
+    Returns a fresh [F,H,W,C] uint8 tensor.  Wrong shapes or dtypes raise ValueError."""
+    if not (isinstance(frames, torch.Tensor) and frames.is_cuda and frames.dim() == 4 and frames.dtype == torch.uint8
+            and 1 <= frames.shape[-1] <= 4):
+        raise ValueError(f"warp_frames: frames must be an [F,H,W,C] uint8 CUDA tensor with C in 1..4 (got "
+                         f"{getattr(frames, 'shape', None)} {getattr(frames, 'dtype', type(frames))})")
+    F, H, W, C = frames.shape
+    m = torch.as_tensor(A)
+    if not (tuple(m.shape) == (F, 2, 3) and m.is_floating_point()):
+        raise ValueError(f"warp_frames: A must be an [F,2,3] = {[F, 2, 3]} float array (got {list(m.shape)} {m.dtype})")
+    m = m.to(device=frames.device, dtype=torch.float64).contiguous()
+    f = frames.contiguous()
+    out = torch.empty_like(f)
+    with torch.cuda.device(f.device):
+        capi.check(capi.lib.rb_frames_warp_affine(capi.ptr(f), capi.ptr(m), F, H, W, C, capi.ptr(out), capi.stream()))
+    return out

@@ -16,7 +16,7 @@ if not os.path.exists(LIB_PATH):
                       "run `python raft-tf_b200/build.py`")
 lib = C.CDLL(LIB_PATH)
 
-_vp, _i, _sz, _f = C.c_void_p, C.c_int, C.c_size_t, C.c_float
+_vp, _i, _sz, _f, _d = C.c_void_p, C.c_int, C.c_size_t, C.c_float, C.c_double
 _pi, _psz = C.POINTER(C.c_int), C.POINTER(C.c_size_t)
 
 # name -> (restype, argtypes); mirrors include/raft_b200.h one to one
@@ -76,6 +76,9 @@ SIGNATURES = {
     "rb_flow_accumulate_backward": (_i, [_vp, _vp, _i, _i, _i, _i, _f, _f, _f, _i, _vp, _vp, _vp]),
     "rb_labels_propagate": (_i, [_vp, _vp, _i, _i, _i, _vp, _i, _i, _vp, _vp, _vp]),
     "rb_labels_propagate_keys": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _vp, _i, _i, _i, _vp, _vp, _vp]),
+    "rb_global_motion_workspace_bytes": (_i, [_i, _i, _i, _psz]),
+    "rb_global_motion": (_i, [_vp, _vp, _i, _i, _i, _i, _i, _f, _i, _d, _d, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
+    "rb_frames_warp_affine": (_i, [_vp, _vp, _i, _i, _i, _i, _vp, _vp]),
     "rb_flow_reverse_workspace_bytes": (_i, [_i, _i, _i, _psz]),
     "rb_flow_reverse": (_i, [_vp, _vp, _vp, _i, _i, _f, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _vp, _sz, _vp]),
     "rb_frame_synthesize": (_i, [_vp, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _f, _vp, _i, _i, _i, _vp]),

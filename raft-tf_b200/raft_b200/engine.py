@@ -599,6 +599,34 @@ class RaftEngine:
                                          keyframe_rows(F, K, cuts))
 
     @torch.no_grad()
+    def stabilize(self, frames: torch.Tensor, sigma, cuts=None, max_zoom=None):
+        """Video stabilization of [F,Hs,Ws,3] uint8 frames (sizes and input_size as for forward()): one
+        forward_sequence_bidirectional pass with the occlusion check, one rb_global_motion launch (networks.utils.
+        global_motion: each pair's camera motion, a similarity fitted robustly to its consistent pixels), the host path
+        of raft_b200.stabilize (the camera path per shot, smoothed by a Gaussian of sigma frames, one zoom per shot capped
+        at max_zoom, default DEFAULT_MAX_ZOOM) and one rb_frames_warp_affine launch on the frames at their own size.
+        cuts: scene-cut pair indices (pair k between frames k and k + 1), where the path restarts.  Returns fresh
+        (frames [F,Hs,Ws,3] uint8, transforms [F,2,3] fp64) CUDA tensors, each transform mapping an output pixel to its
+        source position in the frame's own pixels.  Non-uint8 frames, a sigma that is not finite and > 0, a max_zoom
+        below 1 or bad cuts raise ValueError before the pass."""
+        from networks.utils import global_motion, warp_frames
+        from .stabilize import DEFAULT_MAX_ZOOM, camera_transforms, check_max_zoom, check_sigma
+        from .video import check_cuts
+        F = _sequence_length(frames) + 1
+        if frames.dtype != torch.uint8:
+            raise ValueError(f"raft_b200: stabilize writes bytes: the frames must be uint8 (got {frames.dtype})")
+        sigma = check_sigma(sigma, "raft_b200")
+        max_zoom = check_max_zoom(DEFAULT_MAX_ZOOM if max_zoom is None else max_zoom, "raft_b200")
+        cuts = check_cuts(() if cuts is None else cuts, F, "raft_b200")
+        hw = tuple(frames.shape[1:3])
+        flow_fw, _, occ_fw, _ = self.forward_sequence_bidirectional(frames, check=True)
+        with torch.cuda.device(self.device):
+            params, _, _ = global_motion(flow_fw, occ_fw, hw, flow_scale=self.flow_scale)
+            A, _, _ = camera_transforms(params.cpu().numpy(), hw, sigma, cuts, max_zoom)
+            A = torch.from_numpy(A).to(self.device)
+            return warp_frames(frames.to(self.device), A), A
+
+    @torch.no_grad()
     def interpolate(self, left: torch.Tensor, right: torch.Tensor, ts, native: bool = False) -> torch.Tensor:
         """Frames at times ts (each in [0, 1]; 0 = left, 1 = right) between B frame pairs: one bidirectional pass (as
         forward_bidirectional(check=False), from a graph of its own), then eagerly on the same stream, for as many times

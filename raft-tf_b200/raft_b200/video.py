@@ -34,11 +34,16 @@ per-pixel displacement to the key frame on the GPU and one rb_labels_propagate l
 With several keyframes (frame=[K_0, K_1, ...]) every frame votes between the nearest keys on either side
 (keyframe_rows(), KeyframeSweep, rb_labels_propagate_keys), and scene_cut keeps labels from crossing a cut.
 
-Scene cuts (scene_cut=<threshold in [0, 1]>, video_interpolate and warm-started video): each pass's decoded frames are
-copied to the GPU once and scored there (networks.utils.scene_cut_scores: one minus the intersection of consecutive
-frames' colour histograms); a pair whose score exceeds the threshold is a cut.  Frame-rate conversion copies the nearer
-input frame instead of blending two shots (cut_copy(), split_cut_items()), and warm-started flow restarts its chain
-(cold_start()).  Without a threshold none of this runs.
+video_stabilize(model, "frames/", "out/", sigma=10) removes the camera's shake: a motion sweep of interp_schedule()'s
+passes fits each pair's camera motion on the GPU (rb_global_motion), the host smooths the camera path per shot
+(raft_b200.stabilize), and a warp sweep decodes every frame again and warps it at its own size (rb_frames_warp_affine),
+written as out/frame_<i:06d>.png with out/transforms.npy.
+
+Scene cuts (scene_cut=<threshold in [0, 1]>, video_interpolate, video_stabilize and warm-started video): each pass's
+decoded frames are copied to the GPU once and scored there (networks.utils.scene_cut_scores: one minus the intersection
+of consecutive frames' colour histograms); a pair whose score exceeds the threshold is a cut.  Frame-rate conversion
+copies the nearer input frame instead of blending two shots (cut_copy(), split_cut_items()), warm-started flow restarts
+its chain (cold_start()) and stabilization restarts the camera path.  Without a threshold none of this runs.
 """
 from __future__ import annotations
 
@@ -987,3 +992,93 @@ def video_propagate(model, frames, out, labels, frame=0, batch=8, workers=4, sce
         run(passes[:j0][::-1], sweep.reverse)
     last = last.cpu().numpy()
     return (names, last) if thr is None else (names, last, cuts)
+
+
+def video_stabilize(model, frames, out, sigma, batch=8, workers=4, scene_cut=None, max_zoom=None):
+    """Video stabilization of a clip of any length with a loaded networks.RAFT.RAFT model: the frames (a directory's
+    sorted *.png / *.jpg, or a list of paths, all of one size) written as <out>/frame_<i:06d>.png at their own size with
+    the camera's shake removed, equal byte for byte to RAFT.stabilize on the whole clip.  Two sweeps:
+
+    - motion: interp_schedule()'s passes of forward_sequence_bidirectional (with the occlusion check) and one
+      rb_global_motion launch each (networks.utils.global_motion); only the F x 4 motion parameters stay, so host and
+      device memory do not grow with F.  scene_cut (a threshold in [0, 1]) scores each pass's decoded frames on the GPU
+      (networks.utils.scene_cut_scores), and a pair above it is a cut: its motion is the identity and the camera path
+      restarts after it.
+    - warp: the host path of raft_b200.stabilize (sigma frames, max_zoom, default DEFAULT_MAX_ZOOM), then every frame
+      decoded and uploaded again, batch at a time, and warped at its own size (networks.utils.warp_frames).
+
+    Also writes <out>/transforms.npy [F,2,3] fp64 (RAFT.stabilize's transforms) and prints the zoom of every shot, the
+    cuts and the number of unreliable pairs.  Frames go in RGB with model.upstream and BGR otherwise, like the CLI; the
+    files are BGR and do not depend on batch or workers.  Returns (paths, info), info a dict of "zooms" (per shot),
+    "capped" (the shots whose zoom hit max_zoom), "cuts" and "unreliable" (pair indices)."""
+    import cv2
+    from networks.utils import global_motion, scene_cut_scores, warp_frames
+    from .stabilize import DEFAULT_MAX_ZOOM, camera_transforms, check_max_zoom, check_sigma
+
+    paths = list_frames(frames)
+    sigma = check_sigma(sigma, "video_stabilize")
+    max_zoom = check_max_zoom(DEFAULT_MAX_ZOOM if max_zoom is None else max_zoom, "video_stabilize")
+    batch, workers = int(batch), _workers(workers)
+    thr = None if scene_cut is None else check_scene_cut(scene_cut)
+    F = len(paths)
+    passes = interp_schedule(F, batch)
+    out = os.fspath(out)
+    os.makedirs(out, exist_ok=True)
+    engine = model.engine()
+    rgb = bool(model.upstream)
+    dev = engine.device
+    motions = np.zeros((F - 1, 4))
+    reliable = np.ones(F - 1, dtype=bool)
+    hw = None
+
+    def keep(slot, pairs):  # writer thread: the motions of one pass, once its copies have landed
+        slot.event.synchronize()
+        for r, k in pairs:
+            motions[k] = slot.params[r].numpy()
+            reliable[k] = bool(slot.reliable[r])
+
+    on_dev, cuts = None, []
+    with _Pipeline(paths, passes, rgb, batch, workers, dev) as pipe:
+        for j, ps, imgs, src in pipe:
+            hw = tuple(src.shape[1:3])
+            if thr is not None:  # score the pass on the GPU; the engine then reads the frames from there too
+                if on_dev is None:
+                    on_dev = torch.empty(src.shape, dtype=torch.uint8, device=dev)
+                on_dev.copy_(src, non_blocking=True)
+                src = on_dev
+                cuts += pass_cuts(ps.pairs, scene_cut_scores(on_dev).cpu(), thr)
+            flow_fw, _, occ_fw, _ = engine.forward_sequence_bidirectional(src, check=True)
+            params, _, rel = global_motion(flow_fw, occ_fw, hw, flow_scale=engine.flow_scale)
+            pipe.emit(partial(keep, pairs=[(r, k) for r, k in enumerate(ps.pairs) if k is not None]), batch,
+                      params=params, reliable=rel)
+    motions[cuts] = (1.0, 0.0, 0.0, 0.0)
+    transforms, zooms, capped = camera_transforms(motions, hw, sigma, cuts, max_zoom)
+    np.save(os.path.join(out, "transforms.npy"), transforms)
+
+    def name(i):
+        return os.path.join(out, f"frame_{i:06d}.png")
+
+    def write(slot, first, n):  # writer thread: the warped frames of one chunk
+        slot.event.synchronize()
+        for r in range(n):
+            img = slot.frames[r].numpy()
+            if not cv2.imwrite(name(first + r), cv2.cvtColor(img, cv2.COLOR_RGB2BGR) if rgb else img):
+                raise OSError(f"cannot write {name(first + r)}")
+
+    chunks = [Pass(False, list(range(i, min(i + batch, F))), []) for i in range(0, F, batch)]
+    A = torch.from_numpy(transforms).to(dev)
+    with _Pipeline(paths, chunks, rgb, batch, workers, dev) as pipe:
+        on_dev = None
+        for j, ps, imgs, src in pipe:
+            if on_dev is None:
+                on_dev = torch.empty(src.shape, dtype=torch.uint8, device=dev)
+            n, first = len(ps.frames), ps.frames[0]
+            on_dev[:n].copy_(src, non_blocking=True)
+            res = warp_frames(on_dev[:n], A[first:first + n])
+            pipe.emit(partial(write, first=first, n=n), batch, frames=res)
+    unreliable = [k for k in np.flatnonzero(~reliable).tolist() if k not in cuts]
+    print("stabilize: zoom per shot " + " ".join(f"{z:.4f}" for z in zooms)
+          + (f" (shots {' '.join(map(str, capped))} capped at {max_zoom:g})" if capped else ""))
+    print(f"scene cuts: {len(cuts)}" + (" at pairs " + " ".join(str(k) for k in cuts) if cuts else ""))
+    print(f"unreliable pairs (identity motion): {len(unreliable)}")
+    return [name(i) for i in range(F)], {"zooms": zooms, "capped": capped, "cuts": cuts, "unreliable": unreliable}
