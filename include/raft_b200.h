@@ -407,6 +407,75 @@ int rb_global_motion(const float* flow_fw, const uint8_t* occ_fw, int B, int Hn,
  * call. */
 int rb_frames_warp_affine(const uint8_t* frames, const double* A, int F, int H, int W, int C, uint8_t* out, void* stream);
 
+/* ---- F24: masked fill -- the membrane (Laplace) fill of a field inside a hole --------------------------------------
+ * values [B,H,W,C] fp32 (C = 2 or 3), filled in place; hole [B,H,W] uint8, non-zero = the pixel is unknown.  Each field
+ * approximates the 4-neighbour discrete Laplace equation on its hole pixels with the known pixels as Dirichlet data
+ * (neighbours outside the image left out of the stencil); the known pixels keep their bits.  Method, every fp32
+ * operation rounded on its own, no FMA contraction (tests/inpaint_oracle.py restates it bit for bit):
+ *   pyramid  level l+1 halves level l with ceil down to 1 x 1; a coarse pixel's children are (2i,2j), (2i,2j+1),
+ *            (2i+1,2j), (2i+1,2j+1) (this tap order) inside level l;
+ *   mean     of values v_0, v_1, ... in order: s = 0 + v_0 + v_1 + ..., s / n, clamped by comparisons into the values'
+ *            [min, max];
+ *   guess    a coarse pixel is known when any child is, with the mean of its known children (0 when none); from the
+ *            coarsest level to level 0 each hole pixel takes its parent's value (nearest), then RB_FILL_INIT_SWEEPS
+ *            red-black Gauss-Seidel sweeps (red: x + y even, first) set each hole pixel to the mean of its neighbours
+ *            up, down, left, right (omega = 1);
+ *   cycles   RB_FILL_CYCLES multigrid V-cycles for the correction of level 0.  Level l >= 1's unknowns are the pixels
+ *            whose children are all unknowns of level l - 1 (level 0's: the hole).  Down: the right-hand side of level
+ *            l + 1 is 0 + the residuals s - n e of the four children in tap order (0 for a child outside the level or off
+ *            its unknowns; s = f + the neighbours' e in order, f = 0 and e = the field on level 0), its correction e
+ *            starts at 0, and RB_FILL_SMOOTH red-black sweeps e_p = s / n run on it; at 1 x 1 nothing moves.  Up: each
+ *            unknown adds the cell-centred bilinear value of the coarser correction (weights 1/4, 3/4 per axis, taps
+ *            clamped, ((wx0 e00 + wx1 e01) wy0) + ((wx0 e10 + wx1 e11) wy1)), then RB_FILL_SMOOTH sweeps.  On level 0
+ *            the sum is clamped into the field's [min, max] of known values per channel, and the sweeps are the
+ *            guess's mean sweeps.
+ * Every value the fill writes lies in [min, max] of the field's known values per channel, bit for bit, and a constant
+ * field stays bit for bit.  A field without a known pixel becomes zeros and flags[b] = 1 (flags nullable, [B] uint8,
+ * else 0).  Levels of at most 4096 pixels run their part of each V-cycle in one CTA per field.  Deterministic, no
+ * atomics, no allocation (workspace: rb_masked_fill_workspace_bytes), and a field's bits depend neither on B nor on its
+ * place in the batch.  The holes must stay unchanged during the call.  Null pointers, B/H/W <= 0, C not 2 or 3,
+ * B > 65535, H*W >= 2^31 and a workspace that is too small -> RB_ERR_* before any CUDA call. */
+#define RB_FILL_INIT_SWEEPS 4
+#define RB_FILL_CYCLES 6
+#define RB_FILL_SMOOTH 3
+int rb_masked_fill_workspace_bytes(int B, int H, int W, int C, size_t* bytes);
+int rb_masked_fill(float* values, const uint8_t* hole, int B, int H, int W, int C, uint8_t* flags, void* workspace,
+                   size_t workspace_bytes, void* stream);
+
+/* ---- F25: object removal -- the hole masks and the temporal fill from the nearest frames that see behind a hole ----
+ * rb_inpaint_masks: masks [F,Hs,Ws] uint8 (label maps at the frames' own size); select [256] uint8 in device memory,
+ * non-zero = that label is removed.  hole [F,Hs,Ws] uint8 (not aliasing masks) = 1 where some pixel of the
+ * (2 dilate + 1)^2 square around it (clipped to the frame) has a selected label, else 0.  hole_net [F,Hn,Wn] uint8: network
+ * pixel (i, j) is 1 when any frame pixel (y, x) with floor((y + 0.5) Hn / Hs) = i and floor((x + 0.5) Wn / Ws) = j
+ * (64-bit integers) is a hole; a row or column that no frame pixel maps to takes the one holding its centre,
+ * floor((i + 0.5) Hs / Hn).  Null pointers, F/Hs/Ws/Hn/Wn <= 0, F > 65535, a frame of >= 2^31 pixels and dilate outside
+ * [0, RB_INPAINT_MAX_DILATE] -> RB_ERR_* before any CUDA call.
+ * rb_inpaint_propagate: frames [F,Hs,Ws,3] uint8 and hole [F,Hs,Ws] (rb_inpaint_masks' hole) of F consecutive frames;
+ * flow_fw, flow_bw [F-1,Hn,Wn,2] fp32 (flow_fw[k] frame k -> k+1, flow_bw[k] k+1 -> k, completed inside the holes by
+ * rb_masked_fill); rows [n_rows,3] int32 in device memory, row r = (t, nf, nb): frame t and the steps each side may
+ * take.  Outputs colour [n_rows,Hs,Ws,3] fp32 and status [n_rows,Hs,Ws] uint8.  Per pixel p = (x, y) of row r:
+ *   not a hole: colour = the frame's bytes, status 0;
+ *   a hole: p0 = (fl32((x + 0.5) Wn/Ws - 0.5), fl32((y + 0.5) Hn/Hs - 0.5)) in fp64 (each operation rounded), clamped
+ *     into the grid (track_queries' map).  Forward side: up to min(nf, F-1-t) steps of rb_track_points' step from p0
+ *     (f = s * sample of flow_fw[k] at q, q' = q + f; the side stops when q' leaves the grid or the F5 test against
+ *     s * flow_bw[k] at q' fails).  After step n the position maps back to frame pixels, o = fl32((q' + 0.5) Ws/Wn -
+ *     0.5) per axis in fp64, clamped into the frame; when none of o's four bilinear taps (fb_sample.cuh's) is a hole in
+ *     frame t + n, the side is found at distance n_f = n with colour c_f = the bilinear sample of frame t + n's bytes at
+ *     o.  Backward side: the mirror (flow_bw[k] pulls, flow_fw[k] tests, k = t - n, up to min(nb, t) steps) -- on the
+ *     reversed clip it is the forward side, bit for bit.
+ *     Both found: colour = fl32(fl32(n_b c_f) + fl32(n_f c_b)) / (n_f + n_b) per channel, status 1; one: its colour,
+ *     status 2; none: colour 0, status 3 (left for the spatial fill).
+ * A row whose t lies outside [0, F) is absent (colour 0, status 3) and nf / nb are clamped into the clip, so a bad table
+ * reads nothing out of bounds.  Every fp32 operation is rounded on its own.  One thread per frame pixel, blockIdx.y over
+ * the rows; no allocation.  Null pointers (the flows may be null when F = 1), F/Hs/Ws/Hn/Wn/n_rows <= 0, a frame of
+ * >= 2^31 pixels, flow_scale <= 0 or non-finite and negative or non-finite alphas -> RB_ERR_* before any CUDA call. */
+#define RB_INPAINT_MAX_DILATE 32
+int rb_inpaint_masks(const uint8_t* masks, const uint8_t* select, int F, int Hs, int Ws, int dilate, int Hn, int Wn,
+                     uint8_t* hole, uint8_t* hole_net, void* stream);
+int rb_inpaint_propagate(const uint8_t* frames, const uint8_t* hole, int F, int Hs, int Ws, const float* flow_fw,
+                         const float* flow_bw, int Hn, int Wn, float flow_scale, float alpha1, float alpha2,
+                         const int32_t* rows, int n_rows, float* colour, uint8_t* status, void* stream);
+
 /* ---- F6: frame interpolation -- flow_utils.py:166-274 reverse_flow_avg_skip_static, batched, and the frame blend -----
  * rb_flow_reverse: per sample of flow01 [B,H,W,2] fp32, bit for bit with the reference under numpy >= 2:
  *  1. static(p) = every channel c has d_c < 10, d_c = uint8(bg - im0) (img_u8 = 1: wraps, like numpy's uint8) or

@@ -93,6 +93,15 @@ frame votes between the nearest keys before and after it.  With keyframes, --sce
 cuts (the cuts are printed; pixels that no key reaches get label 0, and the final line counts them in the last frame).
 The single-key form is unchanged and refuses --scene-cut; video_propagate(..., scene_cut=THRESH) takes one key too.
 
+--path DIR --inpaint MASKDIR removes objects: MASKDIR holds one palette or grey label PNG per frame (sorted), and the
+pixels with a non-zero label (--inpaint-labels L ...: those labels), grown by --inpaint-dilate R pixels (default 2), are
+filled from the nearest frames, at most --inpaint-window N (default 10) each way and never across a --scene-cut, that see
+behind them through the completed flow; what no frame sees is filled spatially (raft_b200.video.video_inpaint).  Annotate
+one frame, then remove the object from the whole clip:
+
+    python infer_raft.py --path frames/ --out masks/ --propagate key.png --load raft-things.npz
+    python infer_raft.py --path frames/ --out clean/ --inpaint masks/ --load raft-things.npz [--batch 8]
+
 --path DIR --stabilize SIGMA removes the camera's shake from DIR's frames: each consecutive pair's camera motion (a
 similarity: zoom, rotation, shift) is fitted robustly on the GPU to the flow of its consistent pixels, the camera path is
 smoothed by a Gaussian of SIGMA frames (no default: pick it for the footage; larger is steadier), and every frame is
@@ -243,6 +252,17 @@ def parser():
     p.add_argument('--stabilize-zoom', type=float, default=None, metavar='Z',
                    help='extension, with --stabilize: the largest zoom per shot that hides the borders (default 1.25; '
                         'past it the border replicates)')
+    p.add_argument('--inpaint', default=None, metavar='MASKDIR',
+                   help="extension, with --path: remove the masked objects -- MASKDIR holds one palette or grey PNG "
+                        "label map per frame (sorted; e.g. what --propagate key.png --out MASKDIR wrote); each hole is "
+                        "filled from the nearest frames that see behind it, the rest spatially; writes "
+                        "<--out>/frame_<i:06d>.png at the frames' own size")
+    p.add_argument('--inpaint-labels', type=int, nargs='+', default=None, metavar='L',
+                   help='extension, with --inpaint: remove only these labels (default: every non-zero label)')
+    p.add_argument('--inpaint-window', type=int, default=None, metavar='N',
+                   help='extension, with --inpaint: the frames each side may look ahead or back (default 10; not tuned)')
+    p.add_argument('--inpaint-dilate', type=int, default=None, metavar='R',
+                   help='extension, with --inpaint: grow the masks by R pixels (default 2; not tuned)')
     p.add_argument('--upstream', action='store_true',
                    help='extension: weights converted from an official princeton-vl RAFT .pth (raft_b200.convert): RGB '
                         'frames and the upstream numerics (RAFT(..., upstream=True))')
@@ -255,6 +275,37 @@ def parser():
 def main(argv=None):
     p = parser()
     args = p.parse_args(argv)
+    if args.inpaint is not None:
+        if args.path is None or args.mode != 'test':
+            p.error('--inpaint removes objects from a frame directory: it needs --path DIR (and no -m val)')
+        for other, given in (('--stabilize', args.stabilize is not None),
+                             ('--stabilize-zoom', args.stabilize_zoom is not None),
+                             ('--propagate', args.propagate is not None),
+                             ('--propagate-frame', args.propagate_frame is not None),
+                             ('--track', args.track is not None), ('--track-grid', args.track_grid is not None),
+                             ('--track-frame', args.track_frame != 0), ('--track-vis', args.track_vis is not None),
+                             ('--track-backward', args.track_backward), ('--interpolate', args.interpolate),
+                             ('--fps', args.fps), ('--input-fps', args.input_fps), ('--warm-start', args.warm_start),
+                             ('--bidirectional', args.bidirectional), ('--native-flow', args.native_flow),
+                             ('--native-frames', args.native_frames), ('--flo', args.flo), ('--npy', args.npy)):
+            if given:
+                p.error(f'--inpaint writes frames with the objects removed: it cannot be combined with {other}')
+        if args.inpaint_window is not None and args.inpaint_window < 1:
+            p.error(f'--inpaint-window: N must be >= 1 (got {args.inpaint_window})')
+        if args.inpaint_dilate is not None and not 0 <= args.inpaint_dilate <= 32:
+            p.error(f'--inpaint-dilate: R must be in [0, 32] (got {args.inpaint_dilate})')
+        if args.inpaint_labels is not None and not all(0 <= v <= 255 for v in args.inpaint_labels):
+            p.error(f'--inpaint-labels: labels are in [0, 255] (got {args.inpaint_labels})')
+        if args.scene_cut is not None and not 0.0 <= args.scene_cut <= 1.0:
+            p.error(f'--scene-cut: {args.scene_cut} is not a threshold in [0, 1]')
+        if args.flow_size is not None and args.keep_size:
+            p.error('--flow-size sets the size frames are resized to; --keep-size runs them at their own size')
+        if args.batch < 1 or args.workers < 0:
+            p.error('--path needs --batch >= 1 and --workers >= 0')
+        return run_inpaint(args)
+    for sub in ('labels', 'window', 'dilate'):
+        if getattr(args, f'inpaint_{sub}') is not None:
+            p.error(f'--inpaint-{sub} goes with --inpaint')
     if args.stabilize is not None:
         if args.path is None or args.mode != 'test':
             p.error('--stabilize stabilizes a frame directory: it needs --path DIR (and no -m val)')
@@ -577,6 +628,19 @@ def run_stabilize(args):
     files, _ = video_stabilize(model, args.path, args.out, args.stabilize, batch=args.batch, workers=args.workers,
                                scene_cut=args.scene_cut, max_zoom=args.stabilize_zoom)
     print(f"{len(files)} stabilized frames and transforms.npy written under {args.out}")
+    return 0
+
+
+def run_inpaint(args):
+    """--path --inpaint: raft_b200.video.video_inpaint over the frames of --path and the masks of --inpaint, the flow at
+    432x1024 (or --flow-size) like test mode (or the frames' own size with --keep-size), the frames written at their own
+    size."""
+    from raft_b200.video import video_inpaint
+    model = _video_model(args)
+    files, _ = video_inpaint(model, args.path, args.out, args.inpaint, window=args.inpaint_window,
+                             dilate=args.inpaint_dilate, labels=args.inpaint_labels, batch=args.batch,
+                             workers=args.workers, scene_cut=args.scene_cut)
+    print(f"{len(files)} frames with the masked objects removed written under {args.out}")
     return 0
 
 

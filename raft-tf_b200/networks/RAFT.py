@@ -203,6 +203,17 @@ class RAFT(object):
         return self.engine().stabilize(_as_tensor(frames), sigma, cuts=cuts, max_zoom=max_zoom)
 
     @torch.no_grad()
+    def inpaint(self, frames, masks, window=None, dilate=None, labels=None, cuts=None):
+        """Extension (object removal): [F,Hs,Ws,3] uint8 frames (sources as for ``forward``) with the pixels of the
+        [F,Hs,Ws] uint8 masks removed (non-zero values, or with labels those labels, dilated by `dilate` pixels).  One
+        ``forward_sequence_bidirectional`` pass; each flow completed inside the holes on the GPU; every hole pixel
+        followed through the completed flows up to `window` frames each way, never across a scene-cut pair of cuts, to
+        the nearest frames that see behind it, and what no frame sees filled spatially (RaftEngine.inpaint).  Returns
+        fresh (frames [F,Hs,Ws,3] uint8, status [F,Hs,Ws] uint8) CUDA tensors: status 0 not a hole, 1 filled from both
+        sides, 2 from one, 3 spatially.  Bad masks, window, dilate, labels or cuts raise ValueError before the pass."""
+        return self.engine().inpaint(_as_tensor(frames), masks, window=window, dilate=dilate, labels=labels, cuts=cuts)
+
+    @torch.no_grad()
     def interpolate_sequence(self, frames, t=0.5, uint8=False, bgr=False, native=False):
         """Extension (frame-rate up-conversion): the frames at time t (a float, or a sequence of times, each in [0, 1])
         between every pair of consecutive frames of [T+1,H,W,3] frames, from one ``forward_sequence_bidirectional`` pass.

@@ -598,3 +598,100 @@ def warp_frames(frames, A):
     with torch.cuda.device(f.device):
         capi.check(capi.lib.rb_frames_warp_affine(capi.ptr(f), capi.ptr(m), F, H, W, C, capi.ptr(out), capi.stream()))
     return out
+
+
+def masked_fill(values, hole):
+    """Extension (object removal): the membrane (Laplace) fill of [B,H,W,C] float32 CUDA fields (C = 2 flows or 3
+    colours) inside the holes of [B,H,W] uint8 (or bool) masks, non-zero = unknown (rb_masked_fill: a coarse-to-fine
+    initial guess and multigrid V-cycles of red-black Gauss-Seidel, include/raft_b200.h F24).  The known pixels keep
+    their bits, every filled value lies within the field's known [min, max] per channel, and a field's bits depend
+    neither on B nor on its place in the batch.  Returns fresh (filled [B,H,W,C] float32, empty [B] bool): empty marks a
+    field without a known pixel, filled with zeros.  Wrong shapes or dtypes raise ValueError."""
+    if not (isinstance(values, torch.Tensor) and values.is_cuda and values.dim() == 4 and values.shape[-1] in (2, 3)
+            and values.dtype == torch.float32):
+        raise ValueError(f"masked_fill: values must be a [B,H,W,C] float32 CUDA tensor with C in (2, 3) (got "
+                         f"{getattr(values, 'shape', None)} {getattr(values, 'dtype', type(values))})")
+    B, H, W, C = values.shape
+    if not (isinstance(hole, torch.Tensor) and tuple(hole.shape) == (B, H, W) and hole.dtype in (torch.uint8, torch.bool)
+            and hole.device == values.device):
+        raise ValueError(f"masked_fill: hole must be a [B,H,W] = {[B, H, W]} uint8 or bool tensor on {values.device}")
+    dev = values.device
+    out = values.clone(memory_format=torch.contiguous_format)
+    h = hole.contiguous().view(torch.uint8)
+    flags = torch.empty(B, dtype=torch.uint8, device=dev)
+    with torch.cuda.device(dev):
+        nbytes = capi.size_query(capi.lib.rb_masked_fill_workspace_bytes, B, H, W, C)
+        ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+        capi.check(capi.lib.rb_masked_fill(capi.ptr(out), capi.ptr(h), B, H, W, C, capi.ptr(flags), capi.ptr(ws), nbytes,
+                                           capi.stream()))
+    return out, flags != 0
+
+
+def inpaint_masks(masks, net_hw, dilate=2, labels=None):
+    """Extension (object removal): the holes of [F,Hs,Ws] uint8 CUDA label maps (rb_inpaint_masks).  A pixel is removed
+    when its value is non-zero, or with labels when it is one of them; the removed pixels are dilated by the
+    (2 dilate + 1)^2 square.  Returns fresh (hole [F,Hs,Ws] uint8 0 / 1, hole_net [F,Hn,Wn] uint8): hole_net[i, j] is 1
+    when any frame pixel whose centre maps into network pixel (i, j) of net_hw = (Hn, Wn) is a hole (the pixel holding
+    its centre when none maps into it).  Bad arguments raise ValueError."""
+    from raft_b200.inpaint import check_dilate, selection_table
+    if not (isinstance(masks, torch.Tensor) and masks.is_cuda and masks.dim() == 3 and masks.dtype == torch.uint8):
+        raise ValueError(f"inpaint_masks: masks must be an [F,Hs,Ws] uint8 CUDA tensor (got "
+                         f"{getattr(masks, 'shape', None)} {getattr(masks, 'dtype', type(masks))})")
+    dilate = check_dilate(dilate, "inpaint_masks")
+    try:
+        Hn, Wn = (int(v) for v in net_hw)
+    except (TypeError, ValueError):
+        raise ValueError(f"inpaint_masks: net_hw must be (Hn, Wn) (got {net_hw!r})") from None
+    if Hn < 1 or Wn < 1:
+        raise ValueError(f"inpaint_masks: net_hw must be positive (got {net_hw!r})")
+    dev = masks.device
+    m = masks.contiguous()
+    F, Hs, Ws = m.shape
+    select = torch.from_numpy(selection_table(labels, "inpaint_masks")).to(dev)
+    hole = torch.empty(F, Hs, Ws, dtype=torch.uint8, device=dev)
+    hole_net = torch.empty(F, Hn, Wn, dtype=torch.uint8, device=dev)
+    with torch.cuda.device(dev):
+        capi.check(capi.lib.rb_inpaint_masks(capi.ptr(m), capi.ptr(select), F, Hs, Ws, dilate, Hn, Wn, capi.ptr(hole),
+                                             capi.ptr(hole_net), capi.stream()))
+    return hole, hole_net
+
+
+def inpaint_propagate(frames, hole, flow_fw, flow_bw, rows, flow_scale=1.0, alpha1=0.01, alpha2=0.5):
+    """Extension (object removal): the temporal fill of the holes of F frames from the nearest frames that see behind
+    them (rb_inpaint_propagate).  frames [F,Hs,Ws,3] uint8 and hole [F,Hs,Ws] uint8 CUDA tensors (inpaint_masks' hole);
+    flow_fw, flow_bw [F-1,Hn,Wn,2] float32 consecutive flows completed inside the holes (masked_fill); rows [n,3] integer
+    table (t, nf, nb) (raft_b200.inpaint.inpaint_rows): the frame of each output row and how many steps each side may
+    chain.  Each side follows the flows with the forward-backward test of fb_consistency at every step and stops at the
+    first frame where the four taps of its position are all visible; two sides blend weighted toward the nearer frame.
+    Returns fresh (colour [n,Hs,Ws,3] float32, status [n,Hs,Ws] uint8): status 0 not a hole (the frame's bytes), 1
+    filled from both sides, 2 from one, 3 from none (colour 0).  Bad shapes or a bad table raise ValueError."""
+    if not (isinstance(frames, torch.Tensor) and frames.is_cuda and frames.dim() == 4 and frames.shape[-1] == 3
+            and frames.dtype == torch.uint8):
+        raise ValueError(f"inpaint_propagate: frames must be an [F,Hs,Ws,3] uint8 CUDA tensor (got "
+                         f"{getattr(frames, 'shape', None)} {getattr(frames, 'dtype', type(frames))})")
+    F, Hs, Ws, _ = frames.shape
+    dev = frames.device
+    if not (isinstance(hole, torch.Tensor) and tuple(hole.shape) == (F, Hs, Ws) and hole.dtype == torch.uint8
+            and hole.device == dev):
+        raise ValueError(f"inpaint_propagate: hole must be an [F,Hs,Ws] = {[F, Hs, Ws]} uint8 tensor on {dev}")
+    T, Hn, Wn = _flow_pair("inpaint_propagate", flow_fw, flow_bw)
+    if T != F - 1 or flow_fw.device != dev:
+        raise ValueError(f"inpaint_propagate: {F} frames need [F-1,Hn,Wn,2] = [{F - 1},Hn,Wn,2] flows on {dev} (got "
+                         f"{tuple(flow_fw.shape)})")
+    table = torch.as_tensor(rows).cpu()
+    if not (table.dim() == 2 and table.shape[0] >= 1 and table.shape[1] == 3 and not table.is_floating_point()
+            and not table.is_complex()):
+        raise ValueError(f"inpaint_propagate: rows must be an [n,3] integer table (got {list(table.shape)} {table.dtype})")
+    t, nf, nb = table.to(torch.int64).unbind(1)
+    if not (((t >= 0) & (t < F) & (nf >= 0) & (t + nf <= F - 1) & (nb >= 0) & (nb <= t)).all()):
+        raise ValueError(f"inpaint_propagate: each row (t, nf, nb) needs t in [0, {F}), 0 <= nf <= F-1-t and 0 <= nb <= t")
+    table = table.to(device=dev, dtype=torch.int32).contiguous()
+    n = table.shape[0]
+    f, h, fw, bw = frames.contiguous(), hole.contiguous(), flow_fw.contiguous(), flow_bw.contiguous()
+    colour = torch.empty(n, Hs, Ws, 3, dtype=torch.float32, device=dev)
+    status = torch.empty(n, Hs, Ws, dtype=torch.uint8, device=dev)
+    with torch.cuda.device(dev):
+        capi.check(capi.lib.rb_inpaint_propagate(capi.ptr(f), capi.ptr(h), F, Hs, Ws, capi.ptr(fw), capi.ptr(bw), Hn, Wn,
+                                                 float(flow_scale), float(alpha1), float(alpha2), capi.ptr(table), n,
+                                                 capi.ptr(colour), capi.ptr(status), capi.stream()))
+    return colour, status

@@ -627,6 +627,40 @@ class RaftEngine:
             return warp_frames(frames.to(self.device), A), A
 
     @torch.no_grad()
+    def inpaint(self, frames: torch.Tensor, masks, window=None, dilate=None, labels=None, cuts=None):
+        """Object removal from [F,Hs,Ws,3] uint8 frames (sizes and input_size as for forward()): masks [F,Hs,Ws] uint8
+        label maps at the frames' size, a pixel removed where its value is non-zero (with labels: one of them), dilated
+        by the (2 dilate + 1)^2 square (default raft_b200.inpaint.DEFAULT_DILATE).  One forward_sequence_bidirectional
+        (check=False) pass; rb_inpaint_masks; the 2T flows completed inside the holes on the network grid as one
+        rb_masked_fill batch; one rb_inpaint_propagate launch, each hole pixel followed through the completed flows up to
+        `window` frames each way (default DEFAULT_WINDOW; never across a scene-cut pair of cuts) to the nearest frames
+        that see behind it; one rb_masked_fill of what no frame sees, and the rounding.  Returns fresh (frames
+        [F,Hs,Ws,3] uint8, status [F,Hs,Ws] uint8) CUDA tensors: status 0 not a hole (the bytes as they were), 1 filled
+        from both sides, 2 from one, 3 spatially.  Non-uint8 frames, bad masks, window, dilate, labels or cuts raise
+        ValueError before the pass."""
+        from networks.utils import inpaint_masks
+        from .inpaint import (DEFAULT_DILATE, DEFAULT_WINDOW, check_dilate, check_window, complete_flows, fill_frames,
+                              inpaint_rows, selection_table)
+        from .video import check_cuts
+        F = _sequence_length(frames) + 1
+        if frames.dtype != torch.uint8:
+            raise ValueError(f"raft_b200: inpaint writes bytes: the frames must be uint8 (got {frames.dtype})")
+        Hs, Ws = frames.shape[1:3]
+        m = torch.as_tensor(masks)
+        if not (m.dtype == torch.uint8 and tuple(m.shape) == (F, Hs, Ws)):
+            raise ValueError(f"raft_b200: the masks must be [F,Hs,Ws] = [{F},{Hs},{Ws}] uint8 label maps (got "
+                             f"{list(m.shape)} {m.dtype})")
+        window = check_window(DEFAULT_WINDOW if window is None else window, "raft_b200")
+        dilate = check_dilate(DEFAULT_DILATE if dilate is None else dilate, "raft_b200")
+        selection_table(labels, "raft_b200")
+        rows = inpaint_rows(F, window, check_cuts(() if cuts is None else cuts, F, "raft_b200"))
+        flow_fw, flow_bw, _, _ = self.forward_sequence_bidirectional(frames, check=False)
+        with torch.cuda.device(self.device):
+            hole, hole_net = inpaint_masks(m.to(self.device), flow_fw.shape[1:3], dilate, labels)
+            fw, bw = complete_flows(flow_fw, flow_bw, hole_net)
+            return fill_frames(frames.to(self.device), hole, fw, bw, rows, self.flow_scale)
+
+    @torch.no_grad()
     def interpolate(self, left: torch.Tensor, right: torch.Tensor, ts, native: bool = False) -> torch.Tensor:
         """Frames at times ts (each in [0, 1]; 0 = left, 1 = right) between B frame pairs: one bidirectional pass (as
         forward_bidirectional(check=False), from a graph of its own), then eagerly on the same stream, for as many times

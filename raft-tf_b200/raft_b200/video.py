@@ -39,7 +39,12 @@ passes fits each pair's camera motion on the GPU (rb_global_motion), the host sm
 (raft_b200.stabilize), and a warp sweep decodes every frame again and warps it at its own size (rb_frames_warp_affine),
 written as out/frame_<i:06d>.png with out/transforms.npy.
 
-Scene cuts (scene_cut=<threshold in [0, 1]>, video_interpolate, video_stabilize and warm-started video): each pass's
+video_inpaint(model, "frames/", "out/", "masks/") removes the masked objects: one sweep of interp_schedule()'s passes,
+each pass's flows completed inside the holes on the GPU (rb_masked_fill), every frame filled from the nearest frames that
+see behind its holes (rb_inpaint_propagate) once the pairs it may reach have run, and the rest filled spatially; written
+as out/frame_<i:06d>.png.
+
+Scene cuts (scene_cut=<threshold in [0, 1]>, video_interpolate, video_stabilize, video_inpaint and warm-started video): each pass's
 decoded frames are copied to the GPU once and scored there (networks.utils.scene_cut_scores: one minus the intersection
 of consecutive frames' colour histograms); a pair whose score exceeds the threshold is a cut.  Frame-rate conversion
 copies the nearer input frame instead of blending two shots (cut_copy(), split_cut_items()), warm-started flow restarts
@@ -49,6 +54,7 @@ from __future__ import annotations
 
 import glob
 import os
+import threading
 from collections import namedtuple
 from concurrent.futures import ThreadPoolExecutor
 from fractions import Fraction
@@ -1082,3 +1088,134 @@ def video_stabilize(model, frames, out, sigma, batch=8, workers=4, scene_cut=Non
     print(f"scene cuts: {len(cuts)}" + (" at pairs " + " ".join(str(k) for k in cuts) if cuts else ""))
     print(f"unreliable pairs (identity motion): {len(unreliable)}")
     return [name(i) for i in range(F)], {"zooms": zooms, "capped": capped, "cuts": cuts, "unreliable": unreliable}
+
+
+def list_masks(masks, F, what="video_inpaint"):
+    """The mask paths of video_inpaint: a directory's *.png files in sorted order (one per frame), or a list of paths.
+    A count other than F raises ValueError."""
+    if isinstance(masks, (str, os.PathLike)):
+        root = os.fspath(masks)
+        if not os.path.isdir(root):
+            raise FileNotFoundError(f"{what}: no directory {root}")
+        paths = sorted(glob.glob(os.path.join(root, "*.png")))
+    else:
+        paths = [os.fspath(p) for p in masks]
+    if len(paths) != F:
+        raise ValueError(f"{what}: {len(paths)} masks for {F} frames: one mask PNG per frame")
+    return paths
+
+
+def video_inpaint(model, frames, out, masks, window=None, dilate=None, labels=None, batch=8, workers=4, scene_cut=None):
+    """Object removal from a clip of any length with a loaded networks.RAFT.RAFT model, in one sweep: the frames (a
+    directory's sorted *.png / *.jpg, or a list of paths, all of one size) with the pixels of their masks (a directory
+    of one palette or grey PNG per frame in sorted order, read_labels(), at the frames' size; non-zero values are
+    removed, or with labels those labels) filled from the nearest frames that see behind them, written as
+    <out>/frame_<i:06d>.png, equal byte for byte to RAFT.inpaint on the whole clip for every batch and workers value.
+
+    Passes come from interp_schedule(): forward_sequence_bidirectional(check=False) on batch + 1 frames, the pass's
+    masks read on the host and turned into holes on the GPU (rb_inpaint_masks), and its flows completed inside the holes
+    as one rb_masked_fill batch.  A window of the clip stays on the GPU: the uploaded frames, their holes and the
+    completed flows of the frames from t - window to the newest.  Frame t is filled (rb_inpaint_propagate, the spatial
+    fill and the rounding) and written once the pairs up to min(t + window, F - 1) have run, and the frames no later
+    frame reaches are dropped, so memory is bounded by the window, not the clip: 4 Hs Ws bytes (frame and hole) plus
+    Hn Wn (grid hole) plus 16 Hn Wn (the two completed flows) per kept frame, at most 2 window + batch + 2 of them --
+    about 15.8 MB per frame for 1080x1920 frames and 432x1024 flows (by arithmetic), 0.47 GB at window 10, batch 8.
+    scene_cut (a threshold in [0, 1]) scores each pass's frames on the GPU (networks.utils.scene_cut_scores); no side
+    crosses a cut pair.  Prints the pixel counts of status 1 / 2 / 3 and the cuts.  Frames go in RGB with model.upstream
+    and BGR otherwise, like the CLI; the files are BGR.  Returns (paths, info), info a dict of "counts" (pixels filled
+    from both sides, one side, spatially) and "cuts"."""
+    import cv2
+    from networks.utils import inpaint_masks, scene_cut_scores
+    from .inpaint import (DEFAULT_DILATE, DEFAULT_WINDOW, check_dilate, check_window, complete_flows, fill_frames,
+                          inpaint_rows, selection_table)
+
+    paths = list_frames(frames)
+    F = len(paths)
+    mask_paths = list_masks(masks, F)
+    window = check_window(DEFAULT_WINDOW if window is None else window, "video_inpaint")
+    dilate = check_dilate(DEFAULT_DILATE if dilate is None else dilate, "video_inpaint")
+    selection_table(labels, "video_inpaint")
+    thr = None if scene_cut is None else check_scene_cut(scene_cut)
+    batch, workers = int(batch), _workers(workers)
+    passes = interp_schedule(F, batch)
+    out = os.fspath(out)
+    os.makedirs(out, exist_ok=True)
+    engine = model.engine()
+    rgb = bool(model.upstream)
+    dev = engine.device
+    cap = min(F, 2 * window + batch + 2)  # frames kept on the GPU
+    names = [os.path.join(out, f"frame_{i:06d}.png") for i in range(F)]
+    counts, lock = np.zeros(4, np.int64), threading.Lock()
+    cuts, on_dev, store = [], None, None
+    base = have = done = 0  # store row 0 is frame base; frames base .. base + have - 1 are kept; frames < done written
+
+    def write(slot, first, n):  # writer thread: the filled frames of one pass, once its copies have landed
+        if slot is None:
+            return
+        slot.event.synchronize()
+        for r in range(n):
+            img = slot.frames[r].numpy()
+            if not cv2.imwrite(names[first + r], cv2.cvtColor(img, cv2.COLOR_RGB2BGR) if rgb else img):
+                raise OSError(f"cannot write {names[first + r]}")
+        c = np.bincount(slot.status[:n].numpy().reshape(-1), minlength=4)[:4]
+        with lock:
+            counts[:] += c
+
+    with _Pipeline(paths, passes, rgb, batch, workers, dev) as pipe:
+        for j, ps, imgs, src in pipe:
+            Hs, Ws = src.shape[1:3]
+            if on_dev is None:
+                on_dev = torch.empty(src.shape, dtype=torch.uint8, device=dev)
+            on_dev.copy_(src, non_blocking=True)
+            if thr is not None:
+                cuts += pass_cuts(ps.pairs, scene_cut_scores(on_dev).cpu(), thr)
+            flow_fw, flow_bw, _, _ = engine.forward_sequence_bidirectional(on_dev, check=False)
+            n = sum(k is not None for k in ps.pairs)
+            first = ps.frames[0]
+            if store is None:
+                Hn, Wn = flow_fw.shape[1:3]
+                store = dict(frames=torch.empty(cap, Hs, Ws, 3, dtype=torch.uint8, device=dev),
+                             hole=torch.empty(cap, Hs, Ws, dtype=torch.uint8, device=dev),
+                             hole_net=torch.empty(cap, Hn, Wn, dtype=torch.uint8, device=dev),
+                             fw=torch.empty(cap, Hn, Wn, 2, dtype=torch.float32, device=dev),
+                             bw=torch.empty(cap, Hn, Wn, 2, dtype=torch.float32, device=dev))
+            new = list(range(base + have, first + n + 1))  # the pass's frames not kept yet
+            if have + len(new) > cap:  # drop the frames no frame still to be written reaches
+                drop = max(done - window, base) - base
+                for t in store.values():
+                    t[:have - drop].copy_(t[drop:have].clone())
+                base, have = base + drop, have - drop
+            lab = []
+            for i in new:
+                m, _ = read_labels(mask_paths[i])
+                if m.shape != (Hs, Ws):
+                    raise ValueError(f"video_inpaint: {mask_paths[i]} is {m.shape[0]}x{m.shape[1]}, the frames "
+                                     f"{Hs}x{Ws}")
+                lab.append(m)
+            r0 = have
+            rows_new = slice(r0, r0 + len(new))
+            store["frames"][rows_new].copy_(on_dev[new[0] - first:new[-1] - first + 1])
+            h, hn = inpaint_masks(torch.from_numpy(np.stack(lab)).to(dev), (Hn, Wn), dilate, labels)
+            store["hole"][rows_new].copy_(h)
+            store["hole_net"][rows_new].copy_(hn)
+            have += len(new)
+            fw, bw = complete_flows(flow_fw[:n], flow_bw[:n], store["hole_net"][first - base:first - base + n + 1])
+            store["fw"][first - base:first - base + n].copy_(fw)
+            store["bw"][first - base:first - base + n].copy_(bw)
+            ran = first + n  # pairs 0 .. ran - 1 have run
+            last = done
+            while last < F and min(last + window, F - 1) <= ran:
+                last += 1
+            res = None
+            if last > done:
+                rows = inpaint_rows(F, window, sorted(cuts))[done:last].copy()
+                rows[:, 0] -= base
+                res = fill_frames(store["frames"][:have], store["hole"][:have], store["fw"][:have - 1],
+                                  store["bw"][:have - 1], rows, engine.flow_scale)
+            pipe.emit(partial(write, first=done, n=last - done), cap, frames=None if res is None else res[0],
+                      status=None if res is None else res[1])
+            done = last
+    cuts = sorted(cuts)
+    print(f"inpaint: pixels filled from both sides {counts[1]}, from one side {counts[2]}, spatially {counts[3]}")
+    print(f"scene cuts: {len(cuts)}" + (" at pairs " + " ".join(str(k) for k in cuts) if cuts else ""))
+    return names, {"counts": counts[1:].tolist(), "cuts": cuts}
