@@ -476,6 +476,50 @@ int rb_inpaint_propagate(const uint8_t* frames, const uint8_t* hole, int F, int 
                          const float* flow_bw, int Hn, int Wn, float flow_scale, float alpha1, float alpha2,
                          const int32_t* rows, int n_rows, float* colour, uint8_t* status, void* stream);
 
+/* ---- F26: full-frame stabilization -- flows extended past the frame edge, and the borders filled from other frames ---
+ * Geometry: B flows [B,Hn,Wn,2] fp32 on the network grid of Hs x Ws frames, extended by my, mx >= 0 network pixels per
+ * side onto the canvas Hc x Wc = (Hn + 2 my) x (Wn + 2 mx); canvas pixel (i, j) is network position (x, y) =
+ * (j - mx, i - my).  motions [B,4] fp64 in device memory, per field the similarity (a, b, tx, ty) of F22 (for a
+ * backward flow the inverse of the pair's, computed by the caller).  The global flow at (x, y), in fp64 with every
+ * operation rounded on its own and rounded once to fp32:
+ *   px = ((x + 0.5) Ws/Wn - 0.5) - (Ws-1)/2,  py likewise,
+ *   g = ((((a px - b py) + tx) - px) / (Ws/Wn) / flow_scale,  (((b px + a py) + ty) - py) / (Hs/Hn) / flow_scale).
+ * rb_flow_extend_residual: resid [B,Hc,Wc,2] fp32 = fl32(flow - g) inside the grid and 0 on the band; hole [B,Hc,Wc]
+ *   uint8 = 0 inside, 1 on the band -- the input of rb_masked_fill (F24), which bends the residual, not the linear g.
+ * rb_flow_extend_finish: ext [B,Hc,Wc,2] fp32 = the flow bit for bit inside the grid and fl32(resid + g) on the band;
+ *   ext may alias resid.
+ * One thread per canvas pixel, blockIdx.y over the fields; no allocation.  Null pointers, B/Hn/Wn/Hs/Ws <= 0, negative
+ * margins, B > 65535, a canvas of >= 2^31 pixels, flow_scale <= 0 or non-finite and an output aliasing the flow ->
+ * RB_ERR_* before any CUDA call.
+ * rb_frames_warp_affine_fill: frames [F,Hs,Ws,3] uint8; ext_fw, ext_bw [F-1,Hc,Wc,2] fp32 (rb_flow_extend_finish's, ext_fw[k]
+ * frame k -> k+1, ext_bw[k] k+1 -> k); A [n_rows,2,3] fp64 in device memory; rows [n_rows,3] int32 in device memory, row
+ * r = (t, nf, nb).  Outputs colour [n_rows,Hs,Ws,3] fp32 and status [n_rows,Hs,Ws] uint8.  Per output pixel (x, y) of
+ * row r, the source (sx, sy) is computed in fp64 from A[r] exactly as rb_frames_warp_affine (F23) does, then:
+ *   inside: when fl32(sx), fl32(sy) lie in [0, Ws-1] x [0, Hs-1] or either is NaN, colour = F23's bilinear value of frame t
+ *     before rintf, status 0 -- rounded and clamped it is rb_frames_warp_affine's byte;
+ *   outside: the canvas position p = (fl32(fl64((sx + 0.5) Wn/Ws - 0.5) + mx), likewise y) (the pixel-centre rule,
+ *     unclamped).  Forward side: when p lies on the canvas, up to min(nf, F-1-t) steps of rb_track_points' step on
+ *     the canvas (f = flow_scale * the bilinear sample of ext_fw[k] at p, q = p + f; the side stops when q leaves the
+ *     canvas or the F5 test against flow_scale * ext_bw[k] at q fails).  After step n the position maps back to frame
+ *     pixels unclamped, o = fl32(((q - m) + 0.5) Ws/Wn - 0.5) per axis in fp64; the side is found at distance n_f = n
+ *     at the first step where o lies in frame t + n, with colour c_f = the bilinear sample of that frame's bytes at o.
+ *     Backward side: the mirror (ext_bw[k] pulls, ext_fw[k] tests, k = t - n, up to min(nb, t) steps).
+ *     Both found: colour = fl32(fl32(n_b c_f) + fl32(n_f c_b)) / (n_f + n_b), status 1; one: its colour, status 2; none:
+ *     colour 0, status 3 (left for the spatial fill).
+ * A row whose t lies outside [0, F) is absent (colour 0, status 3) and nf / nb are clamped into the clip, as in
+ * rb_inpaint_propagate.  Every operation is rounded on its own.  One thread per output pixel, blockIdx.y over the rows;
+ * no allocation.  Null pointers (the flows may be null when F = 1), F/Hs/Ws/Hn/Wn/n_rows <= 0, negative margins, a
+ * frame or canvas of >= 2^31 pixels, flow_scale <= 0 or non-finite and negative or non-finite alphas -> RB_ERR_* before
+ * any CUDA call. */
+int rb_flow_extend_residual(const float* flow, const double* motions, int B, int Hn, int Wn, int Hs, int Ws, int my,
+                            int mx, float flow_scale, float* resid, uint8_t* hole, void* stream);
+int rb_flow_extend_finish(const float* flow, const double* motions, int B, int Hn, int Wn, int Hs, int Ws, int my,
+                          int mx, float flow_scale, const float* resid, float* ext, void* stream);
+int rb_frames_warp_affine_fill(const uint8_t* frames, int F, int Hs, int Ws, const float* ext_fw, const float* ext_bw,
+                               int Hn, int Wn, int my, int mx, float flow_scale, float alpha1, float alpha2,
+                               const double* A, const int32_t* rows, int n_rows, float* colour, uint8_t* status,
+                               void* stream);
+
 /* ---- F6: frame interpolation -- flow_utils.py:166-274 reverse_flow_avg_skip_static, batched, and the frame blend -----
  * rb_flow_reverse: per sample of flow01 [B,H,W,2] fp32, bit for bit with the reference under numpy >= 2:
  *  1. static(p) = every channel c has d_c < 10, d_c = uint8(bg - im0) (img_u8 = 1: wraps, like numpy's uint8) or

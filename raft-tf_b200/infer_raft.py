@@ -112,6 +112,13 @@ video_stabilize):
 
     python infer_raft.py --path frames/ --out stable/ --stabilize 10 --load raft-things.npz [--batch 8]
 
+--stabilize-fill keeps the whole frame instead: --stabilize-zoom defaults to 1, and the borders the correction uncovers
+are filled from the neighbouring frames, at most --stabilize-window N (default 10) each way and never across a
+--scene-cut, that saw them along the flow extended past the frame edge; what none saw is filled spatially.  The pixel
+counts filled from both sides, one side and spatially are printed:
+
+    python infer_raft.py --path frames/ --out stable/ --stabilize 10 --stabilize-fill --load raft-things.npz
+
 -m val --dataset davis scores it on DAVIS-2017's val split (raft_b200.davis): frame 0's annotation of every sequence
 propagated at 480p with 20 iterations, J&F printed (``Validation DAVIS-2017 (val): J&F: ...``) and written to
 ``<--out>/val_davis.json``, the predicted masks to ``<--out>/davis_val/<seq>/`` in DAVIS's results layout.
@@ -252,6 +259,13 @@ def parser():
     p.add_argument('--stabilize-zoom', type=float, default=None, metavar='Z',
                    help='extension, with --stabilize: the largest zoom per shot that hides the borders (default 1.25; '
                         'past it the border replicates)')
+    p.add_argument('--stabilize-fill', action='store_true',
+                   help='extension, with --stabilize: keep the whole frame -- fill the borders the correction uncovers '
+                        'from the neighbouring frames that saw them (what none saw spatially) instead of zooming '
+                        '(--stabilize-zoom then defaults to 1)')
+    p.add_argument('--stabilize-window', type=int, default=None, metavar='N',
+                   help='extension, with --stabilize-fill: the frames each side may look ahead or back (default 10; not '
+                        'tuned)')
     p.add_argument('--inpaint', default=None, metavar='MASKDIR',
                    help="extension, with --path: remove the masked objects -- MASKDIR holds one palette or grey PNG "
                         "label map per frame (sorted; e.g. what --propagate key.png --out MASKDIR wrote); each hole is "
@@ -280,6 +294,8 @@ def main(argv=None):
             p.error('--inpaint removes objects from a frame directory: it needs --path DIR (and no -m val)')
         for other, given in (('--stabilize', args.stabilize is not None),
                              ('--stabilize-zoom', args.stabilize_zoom is not None),
+                             ('--stabilize-fill', args.stabilize_fill),
+                             ('--stabilize-window', args.stabilize_window is not None),
                              ('--propagate', args.propagate is not None),
                              ('--propagate-frame', args.propagate_frame is not None),
                              ('--track', args.track is not None), ('--track-grid', args.track_grid is not None),
@@ -323,6 +339,10 @@ def main(argv=None):
             p.error(f'--stabilize: SIGMA must be a number of frames > 0 (got {args.stabilize})')
         if args.stabilize_zoom is not None and not (math.isfinite(args.stabilize_zoom) and args.stabilize_zoom >= 1):
             p.error(f'--stabilize-zoom: Z must be a zoom >= 1 (got {args.stabilize_zoom})')
+        if args.stabilize_window is not None and not args.stabilize_fill:
+            p.error('--stabilize-window goes with --stabilize-fill')
+        if args.stabilize_window is not None and args.stabilize_window < 1:
+            p.error(f'--stabilize-window: N must be >= 1 (got {args.stabilize_window})')
         if args.scene_cut is not None and not 0.0 <= args.scene_cut <= 1.0:
             p.error(f'--scene-cut: {args.scene_cut} is not a threshold in [0, 1]')
         if args.flow_size is not None and args.keep_size:
@@ -330,8 +350,10 @@ def main(argv=None):
         if args.batch < 1 or args.workers < 0:
             p.error('--path needs --batch >= 1 and --workers >= 0')
         return run_stabilize(args)
-    if args.stabilize_zoom is not None:
-        p.error('--stabilize-zoom goes with --stabilize')
+    for flag, given in (('zoom', args.stabilize_zoom is not None), ('fill', args.stabilize_fill),
+                        ('window', args.stabilize_window is not None)):
+        if given:
+            p.error(f'--stabilize-{flag} goes with --stabilize')
     if args.propagate is not None:
         if args.path is None or args.mode != 'test':
             p.error('--propagate carries labels through a frame directory: it needs --path DIR (and no -m val)')
@@ -626,7 +648,8 @@ def run_stabilize(args):
     from raft_b200.video import video_stabilize
     model = _video_model(args)
     files, _ = video_stabilize(model, args.path, args.out, args.stabilize, batch=args.batch, workers=args.workers,
-                               scene_cut=args.scene_cut, max_zoom=args.stabilize_zoom)
+                               scene_cut=args.scene_cut, max_zoom=args.stabilize_zoom, fill=args.stabilize_fill,
+                               window=args.stabilize_window)
     print(f"{len(files)} stabilized frames and transforms.npy written under {args.out}")
     return 0
 

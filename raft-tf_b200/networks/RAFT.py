@@ -190,7 +190,7 @@ class RAFT(object):
         return self.engine().propagate(_as_tensor(frames), labels, frame=frame, cuts=cuts)
 
     @torch.no_grad()
-    def stabilize(self, frames, sigma, cuts=None, max_zoom=None):
+    def stabilize(self, frames, sigma, cuts=None, max_zoom=None, fill=False, window=None):
         """Extension (video stabilization): [F,Hs,Ws,3] uint8 frames (sources as for ``forward``) with the camera's
         shake removed.  One ``forward_sequence_bidirectional`` pass; per pair a similarity (zoom, rotation, shift) fitted
         robustly on the GPU to the flow of its consistent pixels; the camera path, restarted at every scene cut (cuts:
@@ -199,8 +199,14 @@ class RAFT(object):
         of view, up to max_zoom (default raft_b200.stabilize.DEFAULT_MAX_ZOOM; past it the border replicates)
         (RaftEngine.stabilize).  Returns fresh (frames [F,Hs,Ws,3] uint8, transforms [F,2,3] fp64) CUDA tensors, each
         transform mapping an output pixel to its source position.  Non-uint8 frames, a bad sigma, max_zoom or cuts raise
-        ValueError before the flow pass."""
-        return self.engine().stabilize(_as_tensor(frames), sigma, cuts=cuts, max_zoom=max_zoom)
+        ValueError before the flow pass.
+
+        fill=True gives full-frame output: max_zoom defaults to 1 (no crop) and the borders the correction uncovers are
+        filled from the neighbouring frames, up to window frames each way (default raft_b200.inpaint.DEFAULT_WINDOW),
+        that saw them, along the flows extended past the frame edge; what none saw is filled spatially.  Returns
+        (frames, transforms, status [F,Hs,Ws] uint8): 0 the source lies in the frame, 1 filled from both sides, 2 from
+        one, 3 spatially."""
+        return self.engine().stabilize(_as_tensor(frames), sigma, cuts=cuts, max_zoom=max_zoom, fill=fill, window=window)
 
     @torch.no_grad()
     def inpaint(self, frames, masks, window=None, dilate=None, labels=None, cuts=None):

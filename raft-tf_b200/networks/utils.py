@@ -695,3 +695,102 @@ def inpaint_propagate(frames, hole, flow_fw, flow_bw, rows, flow_scale=1.0, alph
                                                  float(flow_scale), float(alpha1), float(alpha2), capi.ptr(table), n,
                                                  capi.ptr(colour), capi.ptr(status), capi.stream()))
     return colour, status
+
+
+def _margin(what, margin):
+    try:
+        my, mx = (int(v) for v in margin)
+    except (TypeError, ValueError):
+        raise ValueError(f"{what}: margin must be (my, mx) (got {margin!r})") from None
+    if my < 0 or mx < 0:
+        raise ValueError(f"{what}: margin must be >= 0 (got {margin!r})")
+    return my, mx
+
+
+def _hw(what, name, hw):
+    try:
+        h, w = (int(v) for v in hw)
+    except (TypeError, ValueError):
+        raise ValueError(f"{what}: {name} must be (H, W) (got {hw!r})") from None
+    if h < 1 or w < 1:
+        raise ValueError(f"{what}: {name} must be positive (got {hw!r})")
+    return h, w
+
+
+def extend_flows(flow_fw, flow_bw, motions, frame_hw, margin, flow_scale=1.0):
+    """Extension (full-frame stabilization): the consecutive flows [T,Hn,Wn,2] float32 CUDA tensors extended by margin =
+    (my, mx) network pixels per side onto the canvas [T,Hn+2my,Wn+2mx,2] (include/raft_b200.h F26).  motions [T,4] fp64
+    (host or device): each pair's similarity (a, b, tx, ty) in the centred pixels of frame_hw = (Hs, Ws), as
+    raft_b200.stabilize.camera_transforms takes them (the identity at cuts and unreliable pairs); the backward flow uses
+    its inverse, computed here in fp64.  The residual after the global motion is filled over the band by rb_masked_fill,
+    all 2T canvases in one batch, and the global motion added back; inside the grid the flows keep their bits.  Returns
+    fresh (ext_fw, ext_bw).  Wrong shapes or dtypes raise ValueError."""
+    import numpy as np
+    from raft_b200.stabilize import motion_matrix
+    T, Hn, Wn = _flow_pair("extend_flows", flow_fw, flow_bw)
+    Hs, Ws = _hw("extend_flows", "frame_hw", frame_hw)
+    my, mx = _margin("extend_flows", margin)
+    m = torch.as_tensor(motions).cpu().to(torch.float64).numpy()
+    if m.shape != (T, 4):
+        raise ValueError(f"extend_flows: motions must be [T,4] = [{T},4] (got {list(m.shape)})")
+    inv = np.linalg.inv(motion_matrix(m))
+    both = np.concatenate([m, np.stack([inv[:, 0, 0], inv[:, 1, 0], inv[:, 0, 2], inv[:, 1, 2]], 1)])
+    dev = flow_fw.device
+    flows = torch.cat([flow_fw, flow_bw]).contiguous()
+    mot = torch.from_numpy(both).to(dev)
+    Hc, Wc = Hn + 2 * my, Wn + 2 * mx
+    resid = torch.empty(2 * T, Hc, Wc, 2, dtype=torch.float32, device=dev)
+    hole = torch.empty(2 * T, Hc, Wc, dtype=torch.uint8, device=dev)
+    args = (capi.ptr(flows), capi.ptr(mot), 2 * T, Hn, Wn, Hs, Ws, my, mx, float(flow_scale))
+    with torch.cuda.device(dev):
+        capi.check(capi.lib.rb_flow_extend_residual(*args, capi.ptr(resid), capi.ptr(hole), capi.stream()))
+        if my or mx:  # without a band there is nothing to fill, and the fill would leave every known value as it is
+            resid, _ = masked_fill(resid, hole)
+        capi.check(capi.lib.rb_flow_extend_finish(*args, capi.ptr(resid), capi.ptr(resid), capi.stream()))
+    return resid[:T], resid[T:]
+
+
+def warp_frames_fill(frames, ext_fw, ext_bw, net_hw, margin, A, rows, flow_scale=1.0, alpha1=0.01, alpha2=0.5):
+    """Extension (full-frame stabilization): rb_frames_warp_affine_fill (include/raft_b200.h F26).  frames [F,Hs,Ws,3]
+    uint8 CUDA; ext_fw, ext_bw [F-1,Hc,Wc,2] float32 (extend_flows' canvases of the net_hw = (Hn, Wn) grid with margin
+    (my, mx)); A [n,2,3] float (host or device), row r's warp as warp_frames takes it; rows [n,3] integer table (t, nf,
+    nb) (raft_b200.inpaint.inpaint_rows).  A pixel whose source lies in frame t gets warp_frames' value before rounding
+    (status 0); any other follows the extended flows up to nf frames forward and nb back, with the forward-backward test
+    of fb_consistency at every step, to the first frame that holds it: status 1 both sides (blended toward the nearer
+    frame), 2 one side, 3 none (colour 0).  Returns fresh (colour [n,Hs,Ws,3] float32, status [n,Hs,Ws] uint8).  Bad
+    shapes or a bad table raise ValueError."""
+    if not (isinstance(frames, torch.Tensor) and frames.is_cuda and frames.dim() == 4 and frames.shape[-1] == 3
+            and frames.dtype == torch.uint8):
+        raise ValueError(f"warp_frames_fill: frames must be an [F,Hs,Ws,3] uint8 CUDA tensor (got "
+                         f"{getattr(frames, 'shape', None)} {getattr(frames, 'dtype', type(frames))})")
+    F, Hs, Ws, _ = frames.shape
+    dev = frames.device
+    Hn, Wn = _hw("warp_frames_fill", "net_hw", net_hw)
+    my, mx = _margin("warp_frames_fill", margin)
+    T, Hc, Wc = _flow_pair("warp_frames_fill", ext_fw, ext_bw)
+    if T != F - 1 or (Hc, Wc) != (Hn + 2 * my, Wn + 2 * mx) or ext_fw.device != dev:
+        raise ValueError(f"warp_frames_fill: {F} frames need [F-1,Hn+2my,Wn+2mx,2] = [{F - 1},{Hn + 2 * my},"
+                         f"{Wn + 2 * mx},2] flows on {dev} (got {tuple(ext_fw.shape)})")
+    table = torch.as_tensor(rows).cpu()
+    if not (table.dim() == 2 and table.shape[0] >= 1 and table.shape[1] == 3 and not table.is_floating_point()
+            and not table.is_complex()):
+        raise ValueError(f"warp_frames_fill: rows must be an [n,3] integer table (got {list(table.shape)} {table.dtype})")
+    t, nf, nb = table.to(torch.int64).unbind(1)
+    if not (((t >= 0) & (t < F) & (nf >= 0) & (t + nf <= F - 1) & (nb >= 0) & (nb <= t)).all()):
+        raise ValueError(f"warp_frames_fill: each row (t, nf, nb) needs t in [0, {F}), 0 <= nf <= F-1-t and 0 <= nb <= t")
+    n = table.shape[0]
+    m = torch.as_tensor(A)
+    if not (tuple(m.shape) == (n, 2, 3) and m.is_floating_point()):
+        raise ValueError(f"warp_frames_fill: A must be an [n,2,3] = {[n, 2, 3]} float array (got {list(m.shape)} "
+                         f"{m.dtype})")
+    m = m.to(device=dev, dtype=torch.float64).contiguous()
+    table = table.to(device=dev, dtype=torch.int32).contiguous()
+    f, fw, bw = frames.contiguous(), ext_fw.contiguous(), ext_bw.contiguous()
+    colour = torch.empty(n, Hs, Ws, 3, dtype=torch.float32, device=dev)
+    status = torch.empty(n, Hs, Ws, dtype=torch.uint8, device=dev)
+    with torch.cuda.device(dev):
+        capi.check(capi.lib.rb_frames_warp_affine_fill(capi.ptr(f), F, Hs, Ws, capi.ptr(fw), capi.ptr(bw), Hn, Wn, my, mx,
+                                                       float(flow_scale), float(alpha1), float(alpha2), capi.ptr(m),
+                                                       capi.ptr(table), n, capi.ptr(colour), capi.ptr(status),
+                                                       capi.stream()))
+    return colour, status

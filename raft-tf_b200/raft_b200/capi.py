@@ -83,6 +83,10 @@ SIGNATURES = {
     "rb_masked_fill": (_i, [_vp, _vp, _i, _i, _i, _i, _vp, _vp, _sz, _vp]),
     "rb_inpaint_masks": (_i, [_vp, _vp, _i, _i, _i, _i, _i, _i, _vp, _vp, _vp]),
     "rb_inpaint_propagate": (_i, [_vp, _vp, _i, _i, _i, _vp, _vp, _i, _i, _f, _f, _f, _vp, _i, _vp, _vp, _vp]),
+    "rb_flow_extend_residual": (_i, [_vp, _vp, _i, _i, _i, _i, _i, _i, _i, _f, _vp, _vp, _vp]),
+    "rb_flow_extend_finish": (_i, [_vp, _vp, _i, _i, _i, _i, _i, _i, _i, _f, _vp, _vp, _vp]),
+    "rb_frames_warp_affine_fill": (_i, [_vp, _i, _i, _i, _vp, _vp, _i, _i, _i, _i, _f, _f, _f, _vp, _vp, _i, _vp, _vp,
+                                        _vp]),
     "rb_flow_reverse_workspace_bytes": (_i, [_i, _i, _i, _psz]),
     "rb_flow_reverse": (_i, [_vp, _vp, _vp, _i, _i, _f, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _vp, _sz, _vp]),
     "rb_frame_synthesize": (_i, [_vp, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _f, _vp, _i, _i, _i, _vp]),

@@ -599,7 +599,7 @@ class RaftEngine:
                                          keyframe_rows(F, K, cuts))
 
     @torch.no_grad()
-    def stabilize(self, frames: torch.Tensor, sigma, cuts=None, max_zoom=None):
+    def stabilize(self, frames: torch.Tensor, sigma, cuts=None, max_zoom=None, fill=False, window=None):
         """Video stabilization of [F,Hs,Ws,3] uint8 frames (sizes and input_size as for forward()): one
         forward_sequence_bidirectional pass with the occlusion check, one rb_global_motion launch (networks.utils.
         global_motion: each pair's camera motion, a similarity fitted robustly to its consistent pixels), the host path
@@ -608,23 +608,49 @@ class RaftEngine:
         cuts: scene-cut pair indices (pair k between frames k and k + 1), where the path restarts.  Returns fresh
         (frames [F,Hs,Ws,3] uint8, transforms [F,2,3] fp64) CUDA tensors, each transform mapping an output pixel to its
         source position in the frame's own pixels.  Non-uint8 frames, a sigma that is not finite and > 0, a max_zoom
-        below 1 or bad cuts raise ValueError before the pass."""
-        from networks.utils import global_motion, warp_frames
-        from .stabilize import DEFAULT_MAX_ZOOM, camera_transforms, check_max_zoom, check_sigma
+        below 1 or bad cuts raise ValueError before the pass.
+
+        fill=True fills the borders the correction uncovers instead of zooming them away (max_zoom then defaults to
+        1.0; a larger cap keeps camera_transforms' zoom logic): after the same pass, fit and transforms, the flows of that
+        pass are extended by raft_b200.stabilize.fill_margin's canvas margin (networks.utils.extend_flows), and one
+        rb_frames_warp_affine_fill launch over raft_b200.inpaint.inpaint_rows(F, window, cuts) (window default
+        DEFAULT_WINDOW frames each way; no side crosses a cut) and the spatial fill follow (raft_b200.stabilize.
+        fill_warp).  Returns fresh (frames, transforms, status [F,Hs,Ws] uint8): status 0 the source lies in the frame
+        (rb_frames_warp_affine's byte), 1 filled from both sides, 2 from one, 3 spatially.  A bad window, or a window
+        without fill, raises ValueError before the pass."""
+        from networks.utils import extend_flows, global_motion, warp_frames
+        from .inpaint import DEFAULT_WINDOW, check_window, inpaint_rows
+        from .stabilize import (DEFAULT_MAX_ZOOM, camera_transforms, check_max_zoom, check_sigma, fill_margin,
+                                fill_motions, fill_warp)
         from .video import check_cuts
         F = _sequence_length(frames) + 1
         if frames.dtype != torch.uint8:
             raise ValueError(f"raft_b200: stabilize writes bytes: the frames must be uint8 (got {frames.dtype})")
         sigma = check_sigma(sigma, "raft_b200")
-        max_zoom = check_max_zoom(DEFAULT_MAX_ZOOM if max_zoom is None else max_zoom, "raft_b200")
+        if max_zoom is None:
+            max_zoom = 1.0 if fill else DEFAULT_MAX_ZOOM
+        max_zoom = check_max_zoom(max_zoom, "raft_b200")
         cuts = check_cuts(() if cuts is None else cuts, F, "raft_b200")
+        if window is not None and not fill:
+            raise ValueError("raft_b200: stabilize's window is the reach of fill=True")
+        if fill:
+            window = check_window(DEFAULT_WINDOW if window is None else window, "raft_b200")
         hw = tuple(frames.shape[1:3])
-        flow_fw, _, occ_fw, _ = self.forward_sequence_bidirectional(frames, check=True)
+        flow_fw, flow_bw, occ_fw, _ = self.forward_sequence_bidirectional(frames, check=True)
         with torch.cuda.device(self.device):
             params, _, _ = global_motion(flow_fw, occ_fw, hw, flow_scale=self.flow_scale)
-            A, _, _ = camera_transforms(params.cpu().numpy(), hw, sigma, cuts, max_zoom)
+            motions = params.cpu().numpy()
+            A, _, _ = camera_transforms(motions, hw, sigma, cuts, max_zoom)
+            if not fill:
+                A = torch.from_numpy(A).to(self.device)
+                return warp_frames(frames.to(self.device), A), A
+            net_hw = tuple(flow_fw.shape[1:3])
+            margin = fill_margin(A, hw, net_hw)
+            ext_fw, ext_bw = extend_flows(flow_fw, flow_bw, fill_motions(motions, cuts), hw, margin, self.flow_scale)
             A = torch.from_numpy(A).to(self.device)
-            return warp_frames(frames.to(self.device), A), A
+            out, status = fill_warp(frames.to(self.device), ext_fw, ext_bw, net_hw, margin, A,
+                                    inpaint_rows(F, window, cuts), self.flow_scale)
+            return out, A, status
 
     @torch.no_grad()
     def inpaint(self, frames: torch.Tensor, masks, window=None, dilate=None, labels=None, cuts=None):

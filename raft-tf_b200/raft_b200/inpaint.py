@@ -91,9 +91,17 @@ def fill_frames(frames, hole, flow_fw, flow_bw, rows, flow_scale):
     forward-backward test of the occlusion check), one rb_masked_fill of the colours the temporal fill left (status 3),
     everything else as known data, then rounded half to even (rintf) and clamped to bytes.  Returns fresh (frames
     [n,Hs,Ws,3] uint8, status [n,Hs,Ws] uint8)."""
-    from networks.utils import inpaint_propagate, masked_fill
+    from networks.utils import inpaint_propagate
     from .engine import FB_ALPHA1, FB_ALPHA2
     colour, status = inpaint_propagate(frames, hole, flow_fw, flow_bw, rows, flow_scale=flow_scale, alpha1=FB_ALPHA1,
                                        alpha2=FB_ALPHA2)
+    return finish_frames(colour, status), status
+
+
+def finish_frames(colour, status):
+    """The bytes of temporally filled frames: one rb_masked_fill of the colours [n,Hs,Ws,3] fp32 where status [n,Hs,Ws]
+    is 3 (what no frame saw), every other pixel known data that keeps its bits, then rounded half to even (rintf) and
+    clamped to bytes.  Returns fresh frames [n,Hs,Ws,3] uint8."""
+    from networks.utils import masked_fill
     colour, _ = masked_fill(colour, status == 3)
-    return colour.round_().clamp_(0, 255).to(torch.uint8), status
+    return colour.round_().clamp_(0, 255).to(torch.uint8)

@@ -30,6 +30,10 @@ MOTION_MIN_WEIGHT = 0.05
 DEFAULT_MAX_ZOOM = 1.25
 # how far (pixels) a corner may land outside the frame and still count as inside: fp64 rounding of the path
 ZOOM_SLACK = 1e-9
+# full-frame stabilization (fill=True): the largest canvas margin per side as a fraction of the network grid, and the
+# network pixels added to the farthest source for the bilinear taps; the cap is not tuned
+FILL_MARGIN_CAP = 0.5
+FILL_MARGIN_TAPS = 2
 
 
 def check_sigma(sigma, what="stabilize"):
@@ -191,3 +195,58 @@ def camera_transforms(motions, hw, sigma, cuts=(), max_zoom=DEFAULT_MAX_ZOOM):
             capped.append(i)
         A[s:e + 1] = B[s:e + 1] @ np.diag([1.0 / z, 1.0 / z, 1.0])
     return centred_to_pixels(A, hw), zooms, capped
+
+
+def fill_margin(transforms, frame_hw, net_hw):
+    """The canvas margin (my, mx) in network pixels per side that full-frame stabilization extends the flows by, for the
+    transforms [F,2,3] of a whole clip of frame_hw = (Hs, Ws) frames and an (Hn, Wn) network grid.  (0, 0) when every
+    source (rb_frames_warp_affine's fp64 position) lies in [0, Ws-1] x [0, Hs-1]: nothing is filled.  Otherwise per axis
+    the largest distance by which a source's network position (the pixel-centre rule, (s + 0.5) Wn / Ws - 0.5) falls
+    outside the grid [0, Wn-1], rounded up, plus FILL_MARGIN_TAPS for the bilinear taps, capped at FILL_MARGIN_CAP of the
+    grid (a source beyond the canvas is filled spatially).  The sources are affine in the output pixel, so the farthest
+    lie under the four output corners; the frame's own edge pixels map up to half a network pixel outside the grid when
+    the frames are larger than it, so both axes get a margin once any source leaves the frame.  Non-finite transform
+    entries are ignored."""
+    A = np.asarray(transforms, dtype=np.float64)
+    Hs, Ws = (int(v) for v in frame_hw)
+    Hn, Wn = (int(v) for v in net_hw)
+    if A.ndim != 3 or A.shape[1:] != (2, 3):
+        raise ValueError(f"fill_margin: transforms must be [F,2,3] (got {list(A.shape)})")
+    x = np.array([0.0, Ws - 1, 0.0, Ws - 1])
+    y = np.array([0.0, 0.0, Hs - 1, Hs - 1])
+    src, leaves = [], False
+    for row, n_src in ((1, Hs), (0, Ws)):
+        s = (A[:, row, 0, None] * x + A[:, row, 1, None] * y) + A[:, row, 2, None]
+        s = s[np.isfinite(s)]
+        leaves = leaves or bool(((s < 0) | (s > n_src - 1)).any())
+        src.append(np.concatenate([s, [0.0, n_src - 1.0]]))  # the frame's own edges too
+    if not leaves:
+        return 0, 0
+    out = []
+    for s, n_src, n_net in ((src[0], Hs, Hn), (src[1], Ws, Wn)):
+        p = (s + 0.5) * (n_net / n_src) - 0.5
+        over = max(0.0, float((-p).max()), float((p - (n_net - 1)).max()))
+        out.append(min(math.ceil(over) + FILL_MARGIN_TAPS, int(FILL_MARGIN_CAP * n_net)))
+    return tuple(out)
+
+
+def fill_motions(motions, cuts=()):
+    """The per-pair similarities [F-1,4] the flows are extended with: the motions (rb_global_motion's params, already the
+    identity at unreliable pairs) with the identity at the cut pairs."""
+    m = np.array(motions, dtype=np.float64)
+    m[list(cuts)] = (1.0, 0.0, 0.0, 0.0)
+    return m
+
+
+def fill_warp(frames, ext_fw, ext_bw, net_hw, margin, A, rows, flow_scale):
+    """The full-frame stabilized frames of the table's rows (raft_b200.inpaint.inpaint_rows): one
+    rb_frames_warp_affine_fill launch on the extended flows (networks.utils.warp_frames_fill, the forward-backward test
+    of the occlusion check), A [n,2,3] the rows' transforms, then raft_b200.inpaint.finish_frames -- the spatial fill of
+    what no frame saw (status 3) and the rounding.  Status-0 pixels are rb_frames_warp_affine's bytes.  Returns fresh
+    (frames [n,Hs,Ws,3] uint8, status [n,Hs,Ws] uint8)."""
+    from networks.utils import warp_frames_fill
+    from .engine import FB_ALPHA1, FB_ALPHA2
+    from .inpaint import finish_frames
+    colour, status = warp_frames_fill(frames, ext_fw, ext_bw, net_hw, margin, A, rows, flow_scale=flow_scale,
+                                      alpha1=FB_ALPHA1, alpha2=FB_ALPHA2)
+    return finish_frames(colour, status), status

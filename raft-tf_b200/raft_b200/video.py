@@ -39,6 +39,10 @@ passes fits each pair's camera motion on the GPU (rb_global_motion), the host sm
 (raft_b200.stabilize), and a warp sweep decodes every frame again and warps it at its own size (rb_frames_warp_affine),
 written as out/frame_<i:06d>.png with out/transforms.npy.
 
+video_stabilize(..., fill=True) keeps the frames whole instead of zooming: the fill sweep reruns the flow passes, extends
+each pass's flows past the frame edge (rb_flow_extend_residual / rb_masked_fill / rb_flow_extend_finish) and fills each
+uncovered border pixel from the neighbouring frames that saw it (rb_frames_warp_affine_fill).
+
 video_inpaint(model, "frames/", "out/", "masks/") removes the masked objects: one sweep of interp_schedule()'s passes,
 each pass's flows completed inside the holes on the GPU (rb_masked_fill), every frame filled from the nearest frames that
 see behind its holes (rb_inpaint_propagate) once the pairs it may reach have run, and the rest filled spatially; written
@@ -1000,7 +1004,8 @@ def video_propagate(model, frames, out, labels, frame=0, batch=8, workers=4, sce
     return (names, last) if thr is None else (names, last, cuts)
 
 
-def video_stabilize(model, frames, out, sigma, batch=8, workers=4, scene_cut=None, max_zoom=None):
+def video_stabilize(model, frames, out, sigma, batch=8, workers=4, scene_cut=None, max_zoom=None, fill=False,
+                    window=None):
     """Video stabilization of a clip of any length with a loaded networks.RAFT.RAFT model: the frames (a directory's
     sorted *.png / *.jpg, or a list of paths, all of one size) written as <out>/frame_<i:06d>.png at their own size with
     the camera's shake removed, equal byte for byte to RAFT.stabilize on the whole clip.  Two sweeps:
@@ -1016,14 +1021,31 @@ def video_stabilize(model, frames, out, sigma, batch=8, workers=4, scene_cut=Non
     Also writes <out>/transforms.npy [F,2,3] fp64 (RAFT.stabilize's transforms) and prints the zoom of every shot, the
     cuts and the number of unreliable pairs.  Frames go in RGB with model.upstream and BGR otherwise, like the CLI; the
     files are BGR and do not depend on batch or workers.  Returns (paths, info), info a dict of "zooms" (per shot),
-    "capped" (the shots whose zoom hit max_zoom), "cuts" and "unreliable" (pair indices)."""
+    "capped" (the shots whose zoom hit max_zoom), "cuts" and "unreliable" (pair indices).
+
+    fill=True writes full-frame output, the bytes of RAFT.stabilize(fill=True) (max_zoom then defaults to 1.0; window
+    to raft_b200.inpaint.DEFAULT_WINDOW): the motion sweep and the transforms as above, then the canvas margin of the
+    whole clip (raft_b200.stabilize.fill_margin) and a fill sweep instead of the warp sweep -- interp_schedule()'s passes
+    again with check=False, each pass's flows extended past the frame edge as one batch (networks.utils.extend_flows).
+    A window of the clip stays on the GPU: the frames and extended flows from t - window to the newest, at most
+    2 window + batch + 2 frames of 3 Hs Ws + 16 Hc Wc bytes each (Hc x Wc the canvas).  For 1080x1920 frames and
+    432x1024 flows that is 17.3 MB per frame at a margin of 12.5 % of the grid per side and 34.5 MB at the cap (half the
+    grid per side), by arithmetic: 0.52 GB and 1.04 GB at window 10, batch 8.  Frame t is filled (raft_b200.stabilize.
+    fill_warp over inpaint_rows(F, window, cuts)) and written once the pairs up to min(t + window, F - 1) have run.  It
+    also prints the pixel counts of status 1 / 2 / 3, and info gains "counts" (pixels filled from both sides, one side,
+    spatially) and "margin" ((my, mx) network pixels)."""
     import cv2
     from networks.utils import global_motion, scene_cut_scores, warp_frames
+    from .inpaint import DEFAULT_WINDOW, check_window
     from .stabilize import DEFAULT_MAX_ZOOM, camera_transforms, check_max_zoom, check_sigma
 
     paths = list_frames(frames)
     sigma = check_sigma(sigma, "video_stabilize")
-    max_zoom = check_max_zoom(DEFAULT_MAX_ZOOM if max_zoom is None else max_zoom, "video_stabilize")
+    max_zoom = check_max_zoom((1.0 if fill else DEFAULT_MAX_ZOOM) if max_zoom is None else max_zoom, "video_stabilize")
+    if window is not None and not fill:
+        raise ValueError("video_stabilize: window is the reach of fill=True")
+    if fill:
+        window = check_window(DEFAULT_WINDOW if window is None else window, "video_stabilize")
     batch, workers = int(batch), _workers(workers)
     thr = None if scene_cut is None else check_scene_cut(scene_cut)
     F = len(paths)
@@ -1071,23 +1093,101 @@ def video_stabilize(model, frames, out, sigma, batch=8, workers=4, scene_cut=Non
             if not cv2.imwrite(name(first + r), cv2.cvtColor(img, cv2.COLOR_RGB2BGR) if rgb else img):
                 raise OSError(f"cannot write {name(first + r)}")
 
-    chunks = [Pass(False, list(range(i, min(i + batch, F))), []) for i in range(0, F, batch)]
     A = torch.from_numpy(transforms).to(dev)
-    with _Pipeline(paths, chunks, rgb, batch, workers, dev) as pipe:
-        on_dev = None
-        for j, ps, imgs, src in pipe:
-            if on_dev is None:
-                on_dev = torch.empty(src.shape, dtype=torch.uint8, device=dev)
-            n, first = len(ps.frames), ps.frames[0]
-            on_dev[:n].copy_(src, non_blocking=True)
-            res = warp_frames(on_dev[:n], A[first:first + n])
-            pipe.emit(partial(write, first=first, n=n), batch, frames=res)
+    if fill:
+        counts, margin = _stabilize_fill_sweep(engine, paths, passes, rgb, batch, workers, hw, motions, transforms, A,
+                                               sorted(cuts), window, name)
+    else:
+        chunks = [Pass(False, list(range(i, min(i + batch, F))), []) for i in range(0, F, batch)]
+        with _Pipeline(paths, chunks, rgb, batch, workers, dev) as pipe:
+            on_dev = None
+            for j, ps, imgs, src in pipe:
+                if on_dev is None:
+                    on_dev = torch.empty(src.shape, dtype=torch.uint8, device=dev)
+                n, first = len(ps.frames), ps.frames[0]
+                on_dev[:n].copy_(src, non_blocking=True)
+                res = warp_frames(on_dev[:n], A[first:first + n])
+                pipe.emit(partial(write, first=first, n=n), batch, frames=res)
     unreliable = [k for k in np.flatnonzero(~reliable).tolist() if k not in cuts]
     print("stabilize: zoom per shot " + " ".join(f"{z:.4f}" for z in zooms)
           + (f" (shots {' '.join(map(str, capped))} capped at {max_zoom:g})" if capped else ""))
     print(f"scene cuts: {len(cuts)}" + (" at pairs " + " ".join(str(k) for k in cuts) if cuts else ""))
     print(f"unreliable pairs (identity motion): {len(unreliable)}")
-    return [name(i) for i in range(F)], {"zooms": zooms, "capped": capped, "cuts": cuts, "unreliable": unreliable}
+    info = {"zooms": zooms, "capped": capped, "cuts": cuts, "unreliable": unreliable}
+    if fill:
+        print(f"stabilize fill: pixels filled from both sides {counts[1]}, from one side {counts[2]}, spatially "
+              f"{counts[3]}")
+        info.update(counts=counts[1:].tolist(), margin=margin)
+    return [name(i) for i in range(F)], info
+
+
+def _stabilize_fill_sweep(engine, paths, passes, rgb, batch, workers, hw, motions, transforms, A, cuts, window, name):
+    """video_stabilize's fill sweep: writes every frame, full-frame stabilized, with name(i).  Returns (counts [4] int64
+    of each status, margin)."""
+    import cv2
+    from networks.utils import extend_flows
+    from .inpaint import inpaint_rows
+    from .stabilize import fill_margin, fill_warp
+    F, dev = len(paths), engine.device
+    cap = min(F, 2 * window + batch + 2)  # frames kept on the GPU
+    rows_all = inpaint_rows(F, window, cuts)
+    counts, lock = np.zeros(4, np.int64), threading.Lock()
+    on_dev = store = net_hw = margin = None
+    base = have = done = 0  # store row 0 is frame base; frames base .. base + have - 1 are kept; frames < done written
+
+    def write(slot, first, n):  # writer thread: the filled frames of one pass, once its copies have landed
+        if slot is None:
+            return
+        slot.event.synchronize()
+        for r in range(n):
+            img = slot.frames[r].numpy()
+            if not cv2.imwrite(name(first + r), cv2.cvtColor(img, cv2.COLOR_RGB2BGR) if rgb else img):
+                raise OSError(f"cannot write {name(first + r)}")
+        c = np.bincount(slot.status[:n].numpy().reshape(-1), minlength=4)[:4]
+        with lock:
+            counts[:] += c
+
+    with _Pipeline(paths, passes, rgb, batch, workers, dev) as pipe:
+        for j, ps, imgs, src in pipe:
+            if on_dev is None:
+                on_dev = torch.empty(src.shape, dtype=torch.uint8, device=dev)
+            on_dev.copy_(src, non_blocking=True)
+            flow_fw, flow_bw, _, _ = engine.forward_sequence_bidirectional(on_dev, check=False)
+            n = sum(k is not None for k in ps.pairs)
+            first = ps.frames[0]
+            if store is None:
+                net_hw = tuple(flow_fw.shape[1:3])
+                margin = fill_margin(transforms, hw, net_hw)
+                Hc, Wc = net_hw[0] + 2 * margin[0], net_hw[1] + 2 * margin[1]
+                store = dict(frames=torch.empty(cap, *hw, 3, dtype=torch.uint8, device=dev),
+                             fw=torch.empty(cap, Hc, Wc, 2, dtype=torch.float32, device=dev),
+                             bw=torch.empty(cap, Hc, Wc, 2, dtype=torch.float32, device=dev))
+            new = list(range(base + have, first + n + 1))  # the pass's frames not kept yet
+            if have + len(new) > cap:  # drop the frames no frame still to be written reaches
+                drop = max(done - window, base) - base
+                for t in store.values():
+                    t[:have - drop].copy_(t[drop:have].clone())
+                base, have = base + drop, have - drop
+            store["frames"][have:have + len(new)].copy_(on_dev[new[0] - first:new[-1] - first + 1])
+            have += len(new)
+            # copies out of the engine's views, which the next pass overwrites
+            fw, bw = extend_flows(flow_fw[:n], flow_bw[:n], motions[first:first + n], hw, margin, engine.flow_scale)
+            store["fw"][first - base:first - base + n].copy_(fw)
+            store["bw"][first - base:first - base + n].copy_(bw)
+            ran = first + n  # pairs 0 .. ran - 1 have run
+            last = done
+            while last < F and min(last + window, F - 1) <= ran:
+                last += 1
+            res = None
+            if last > done:
+                rows = rows_all[done:last].copy()
+                rows[:, 0] -= base
+                res = fill_warp(store["frames"][:have], store["fw"][:have - 1], store["bw"][:have - 1], net_hw, margin,
+                                A[done:last], rows, engine.flow_scale)
+            pipe.emit(partial(write, first=done, n=last - done), cap, frames=None if res is None else res[0],
+                      status=None if res is None else res[1])
+            done = last
+    return counts, margin
 
 
 def list_masks(masks, F, what="video_inpaint"):
