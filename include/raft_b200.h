@@ -48,9 +48,9 @@ enum {
  *                      fp16(a) * fp16(w), both the round-to-nearest hi plane (what autocast's cast gives), accumulated
  *                      in fp32 registers; the lo planes are not read;
  *                    - as in RB_MATH_TC: the correlation build (3 products), the lookups and the volume-free path, every
- *                      epilogue and elementwise op in fp32 (GRU gates, instance-norm statistics and apply, residuals,
- *                      coords1 += delta, mask softmax, upsampling), every buffer layout -- epilogues still write both
- *                      planes, so a workspace stays valid when the mode changes between calls;
+ *                      epilogue and elementwise op in fp32 (GRU gates, instance-norm apply, residuals, coords1 += delta,
+ *                      mask softmax, upsampling), the instance-norm sums in fp64, every buffer layout -- epilogues still
+ *                      write both planes, so a workspace stays valid when the mode changes between calls;
  *                    - combines with either semantics, the volume-free lookup and rb_frames_resize;
  *                    - deterministic like RB_MATH_TC: the same K order and split-K halves, so batched runs equal
  *                      per-sample runs and every tile configuration gives the same bits;

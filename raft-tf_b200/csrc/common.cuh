@@ -568,17 +568,21 @@ __device__ __forceinline__ void epilogue_wide16(const ConvParams& p, int pix, in
 
 // Per-channel sum and sum of squares over the 32 pixels (lanes) of a warp for the 16 channels each lane holds
 // (instance-norm statistics fused into the conv epilogue).  Recursive halving: after the xor-16/8/4/2 exchanges lane l
-// owns channel 8*b4 + 4*b3 + 2*b2 + b1 (b_i = bit i of l), the xor-1 step completes the sum; 32 shuffles, fixed order.
-__device__ __forceinline__ void warp_stats16(const float* y, float& s, float& s2, int& ch) {
+// owns channel 8*b4 + 4*b3 + 2*b2 + b1 (b_i = bit i of l), the xor-1 step completes the sum; fixed order.
+// The sums are fp64 of exact squares, like the stand-alone pass: inorm_final_kernel forms var = E[v^2] - mean^2, whose
+// error grows like (|mean| / std)^2 times the unit roundoff of the sums -- in fp32 a channel with |mean| / std ~ 3e3 loses
+// its variance entirely.
+__device__ __forceinline__ void warp_stats16(const float* y, double& s, double& s2, int& ch) {
   const unsigned lane = threadIdx.x & 31u;
-  float a[8], b[8];
+  double a[8], b[8];
   {
     const bool up = (lane & 16u) != 0;
 #pragma unroll
     for (int i = 0; i < 8; ++i) {
       const float keep = up ? y[i + 8] : y[i], send = up ? y[i] : y[i + 8];
-      a[i] = keep + __shfl_xor_sync(0xffffffffu, send, 16);
-      b[i] = keep * keep + __shfl_xor_sync(0xffffffffu, send * send, 16);
+      const double got = (double)__shfl_xor_sync(0xffffffffu, send, 16);
+      a[i] = (double)keep + got;
+      b[i] = (double)keep * keep + got * got;
     }
   }
 #pragma unroll
@@ -586,8 +590,8 @@ __device__ __forceinline__ void warp_stats16(const float* y, float& s, float& s2
     const bool up = (lane & (unsigned)(2 * w)) != 0;
 #pragma unroll
     for (int i = 0; i < w; ++i) {
-      const float ka = up ? a[i + w] : a[i], sa = up ? a[i] : a[i + w];
-      const float kb = up ? b[i + w] : b[i], sb = up ? b[i] : b[i + w];
+      const double ka = up ? a[i + w] : a[i], sa = up ? a[i] : a[i + w];
+      const double kb = up ? b[i + w] : b[i], sb = up ? b[i] : b[i + w];
       a[i] = ka + __shfl_xor_sync(0xffffffffu, sa, 2 * w);
       b[i] = kb + __shfl_xor_sync(0xffffffffu, sb, 2 * w);
     }

@@ -327,13 +327,13 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
 #pragma unroll
               for (int i = 0; i < 16; ++i) v[i] = 0.f;
             }
-            float s1, s2;
+            double s1, s2;
             int ch;
             warp_stats16(v, s1, s2, ch);
             if ((lane & 1) == 0 && mt < g.m_tiles) {
               double* dst = p.stat_part + ((size_t)(b * p.stat_strips + trem * 4 + (r >> 5)) * 2) * p.cout + n0 + c + ch;
-              dst[0] = (double)s1;
-              dst[p.cout] = (double)s2;
+              dst[0] = s1;
+              dst[p.cout] = s2;
             }
           }
         }
