@@ -520,6 +520,49 @@ int rb_frames_warp_affine_fill(const uint8_t* frames, int F, int Hs, int Ws, con
                                const double* A, const int32_t* rows, int n_rows, float* colour, uint8_t* status,
                                void* stream);
 
+/* ---- F27: video denoising -- each pixel merged with its patch matches along the chained flow of neighbouring frames --
+ * rb_denoise_merge: frames [F,Hs,Ws,3] uint8 of F consecutive frames; flow_fw, flow_bw [F-1,Hn,Wn,2] fp32 (flow_fw[k]
+ * frame k -> k+1, flow_bw[k] k+1 -> k, as for rb_inpaint_propagate); rows [n_rows,3] int32 in device memory, row r =
+ * (t, nf, nb): frame t and the steps each side may take (raft_b200.inpaint.inpaint_rows' table); sigma the noise's
+ * standard deviation in grey levels.  Outputs out [n_rows,Hs,Ws,3] uint8 (not aliasing frames) and support
+ * [n_rows,Hs,Ws] uint8.  Per pixel p = (x, y) of row r:
+ *   chain: p0 = (fl32((x + 0.5) Wn/Ws - 0.5), fl32((y + 0.5) Hn/Hs - 0.5)) in fp64 (each operation rounded), clamped into
+ *     the grid.  Forward side: up to min(nf, F-1-t) steps of rb_track_points' step from p0 (f = s * sample of flow_fw[k]
+ *     at q, q' = q + f; the side stops at the first step where q' leaves the grid or the F5 test against s * flow_bw[k]
+ *     at q' fails).  Every passing step n is a match in frame t + n at o_n = fl32((q' + 0.5) Ws/Wn - 0.5) per axis in
+ *     fp64, clamped into the frame.  Backward side: the mirror (flow_bw[k] pulls, flow_fw[k] tests, k = t - n, up to
+ *     min(nb, t) steps) -- on the reversed clip it is the forward side, bit for bit.  support = the matched frames of
+ *     both sides.
+ *   candidates: in frame t the integer pixels p + s, in each matched frame the positions o_n + s, for the
+ *     (2 RB_DENOISE_SEARCH + 1)^2 integer offsets s.  A sample at o + delta (delta integer) is the replicate-padded frame
+ *     sampled there: o's bilinear weights (fb_sample.cuh's bilerp_at / bilerp1 arithmetic) on the taps x0 + delta_x,
+ *     x0 + 1 + delta_x (likewise y), each clamped into the frame.  In frame t, o = p: the bytes themselves.
+ *   weight: d = the mean over the (2 RB_DENOISE_PATCH + 1)^2 * 3 values of (candidate patch - frame t's patch at p)^2,
+ *     summed from 0 in raster order, channel innermost, then divided by 27; x = max(d - 2 sigma^2, 0) / (RB_DENOISE_H
+ *     sigma)^2 (x = 0 when the numerator is 0), w = (1 - x)^2 for x < 1, else 0 -- Tukey's biweight above the noise
+ *     floor.  The centre candidate (frame t, s = 0) has d = 0 and w = 1.
+ *   out = clamp(rintf(sum w c / sum w), 0, 255) per channel, c the candidate's centre sample; the sums run from 0 over
+ *     frame t, then the forward matches n = 1, 2, ..., then the backward ones, each frame's offsets in raster order.
+ * A row whose t lies outside [0, F) is absent (out 0, support 0); nf / nb are clamped into [0, RB_DENOISE_MAX_WINDOW] and
+ * into the clip, so a bad table reads nothing out of bounds.  Every fp32 operation is rounded on its own.  One thread
+ * per output pixel, blockIdx.y over the rows; no atomics, no allocation.  Null pointers (the flows may be null when
+ * F = 1), F/Hs/Ws/Hn/Wn/n_rows <= 0, a frame of >= 2^31 pixels, flow_scale <= 0 or non-finite, negative or non-finite
+ * alphas, sigma <= 0 or non-finite and out aliasing frames -> RB_ERR_* before any CUDA call.
+ * ---- F28: the noise estimate behind sigma = "auto" ----
+ * rb_noise_sums: frames [N,H,W,3] uint8; sums [N,3] int64 = sum over the interior pixels (1 <= x <= W-2, 1 <= y <= H-2)
+ * of |I * M| per frame and channel, M = [[1,-2,1],[-2,4,-2],[1,-2,1]] (Immerkaer, "Fast noise variance estimation",
+ * CVIU 1996).  The host takes sigma = sqrt(pi/2) S / (6 (H-2)(W-2)) per frame and channel.  Integer sums: exact and
+ * deterministic with int64 atomics; one memset and one launch, no allocation.  Null pointers, N <= 0, H or W < 3,
+ * N > 65535 and H*W >= 2^31 -> RB_ERR_* before any CUDA call. */
+#define RB_DENOISE_SEARCH 1
+#define RB_DENOISE_PATCH 1
+#define RB_DENOISE_MAX_WINDOW 16
+#define RB_DENOISE_H 3.0f
+int rb_denoise_merge(const uint8_t* frames, int F, int Hs, int Ws, const float* flow_fw, const float* flow_bw, int Hn,
+                     int Wn, float flow_scale, float alpha1, float alpha2, const int32_t* rows, int n_rows, float sigma,
+                     uint8_t* out, uint8_t* support, void* stream);
+int rb_noise_sums(const uint8_t* frames, int N, int H, int W, int64_t* sums, void* stream);
+
 /* ---- F6: frame interpolation -- flow_utils.py:166-274 reverse_flow_avg_skip_static, batched, and the frame blend -----
  * rb_flow_reverse: per sample of flow01 [B,H,W,2] fp32, bit for bit with the reference under numpy >= 2:
  *  1. static(p) = every channel c has d_c < 10, d_c = uint8(bg - im0) (img_u8 = 1: wraps, like numpy's uint8) or

@@ -119,6 +119,19 @@ counts filled from both sides, one side and spatially are printed:
 
     python infer_raft.py --path frames/ --out stable/ --stabilize 10 --stabilize-fill --load raft-things.npz
 
+--path DIR --denoise SIGMA removes additive noise of standard deviation SIGMA grey levels ('auto': estimated from the
+first 8 frames): each pixel is followed through the flow, at most --denoise-window N (default 3) frames each way, never
+across a --scene-cut and only while the forward-backward test holds, and merged with the patches that match it there
+and around it in its own frame (raft_b200.video.video_denoise).  The sigma used and the mean number of matched frames are
+printed:
+
+    python infer_raft.py --path noisy/ --out clean/ --denoise 20 --load raft-things.npz [--batch 8]
+
+-m val --dataset davis --denoise SIGMA scores it on DAVIS-2017 test-dev (raft_b200.davis.evaluate_denoise): seeded
+Gaussian noise of SIGMA added to every frame, the flow at the frames' own size with 20 iterations, PSNR and SSIM of the
+output and of the noisy input printed (``Validation DAVIS-2017 denoising (test-dev, sigma S): ...``) and written to
+``<--out>/val_davis_denoise.json``.
+
 -m val --dataset davis scores it on DAVIS-2017's val split (raft_b200.davis): frame 0's annotation of every sequence
 propagated at 480p with 20 iterations, J&F printed (``Validation DAVIS-2017 (val): J&F: ...``) and written to
 ``<--out>/val_davis.json``, the predicted masks to ``<--out>/davis_val/<seq>/`` in DAVIS's results layout.
@@ -277,6 +290,15 @@ def parser():
                    help='extension, with --inpaint: the frames each side may look ahead or back (default 10; not tuned)')
     p.add_argument('--inpaint-dilate', type=int, default=None, metavar='R',
                    help='extension, with --inpaint: grow the masks by R pixels (default 2; not tuned)')
+    p.add_argument('--denoise', default=None, metavar='SIGMA',
+                   help="extension, with --path: remove additive noise of standard deviation SIGMA grey levels (0-255) "
+                        "or 'auto' (estimated from the first frames) -- each pixel is merged with its patch matches in "
+                        "the neighbouring frames the flow reaches consistently; writes <--out>/frame_<i:06d>.png at the "
+                        "frames' own size.  With -m val --dataset davis: score denoising on DAVIS-2017 test-dev at "
+                        "noise SIGMA")
+    p.add_argument('--denoise-window', type=int, default=None, metavar='N',
+                   help='extension, with --denoise: the frames each side may look ahead or back (default 3, at most '
+                        '16; not tuned)')
     p.add_argument('--upstream', action='store_true',
                    help='extension: weights converted from an official princeton-vl RAFT .pth (raft_b200.convert): RGB '
                         'frames and the upstream numerics (RAFT(..., upstream=True))')
@@ -289,6 +311,63 @@ def parser():
 def main(argv=None):
     p = parser()
     args = p.parse_args(argv)
+    if args.denoise is not None:
+        sigma = args.denoise
+        if sigma != 'auto':
+            try:
+                sigma = float(sigma)
+            except ValueError:
+                sigma = None
+            if sigma is None or not (math.isfinite(sigma) and sigma > 0):
+                p.error(f"--denoise: SIGMA must be a number > 0 (grey levels) or 'auto' (got {args.denoise})")
+        if args.denoise_window is not None and not 1 <= args.denoise_window <= 16:
+            p.error(f'--denoise-window: N must be in [1, 16] (got {args.denoise_window})')
+        if args.mode == 'val':
+            if args.dataset != 'davis':
+                p.error('-m val --denoise scores video denoising on DAVIS-2017 test-dev: it needs --dataset davis')
+            if sigma == 'auto':
+                p.error('-m val --denoise adds noise of a known level: give SIGMA, not auto')
+            if args.warm_start:
+                p.error('--warm-start warm-starts flow validation; denoising merges along cold flows')
+            if args.split == 'test':
+                p.error('--split test writes a flow submission; -m val --denoise scores the test-dev frames')
+            for other, given in (('--keyframe-step', args.keyframe_step is not None),
+                                 ('--scene-cut', args.scene_cut is not None), ('--path', args.path is not None)):
+                if given:
+                    p.error(f'-m val --denoise cannot be combined with {other}')
+            if not args.data:
+                p.error('-m val needs --data <dataset root>')
+            return validate_denoise(args, sigma)
+        if args.path is None or args.mode != 'test':
+            p.error('--denoise removes noise from a frame directory: it needs --path DIR (or -m val --dataset davis)')
+        for other, given in (('--inpaint', args.inpaint is not None),
+                             ('--inpaint-labels', args.inpaint_labels is not None),
+                             ('--inpaint-window', args.inpaint_window is not None),
+                             ('--inpaint-dilate', args.inpaint_dilate is not None),
+                             ('--stabilize', args.stabilize is not None),
+                             ('--stabilize-zoom', args.stabilize_zoom is not None),
+                             ('--stabilize-fill', args.stabilize_fill),
+                             ('--stabilize-window', args.stabilize_window is not None),
+                             ('--propagate', args.propagate is not None),
+                             ('--propagate-frame', args.propagate_frame is not None),
+                             ('--track', args.track is not None), ('--track-grid', args.track_grid is not None),
+                             ('--track-frame', args.track_frame != 0), ('--track-vis', args.track_vis is not None),
+                             ('--track-backward', args.track_backward), ('--interpolate', args.interpolate),
+                             ('--fps', args.fps), ('--input-fps', args.input_fps), ('--warm-start', args.warm_start),
+                             ('--bidirectional', args.bidirectional), ('--native-flow', args.native_flow),
+                             ('--native-frames', args.native_frames), ('--flo', args.flo), ('--npy', args.npy),
+                             ('--keyframe-step', args.keyframe_step is not None)):
+            if given:
+                p.error(f'--denoise writes denoised frames: it cannot be combined with {other}')
+        if args.scene_cut is not None and not 0.0 <= args.scene_cut <= 1.0:
+            p.error(f'--scene-cut: {args.scene_cut} is not a threshold in [0, 1]')
+        if args.flow_size is not None and args.keep_size:
+            p.error('--flow-size sets the size frames are resized to; --keep-size runs them at their own size')
+        if args.batch < 1 or args.workers < 0:
+            p.error('--path needs --batch >= 1 and --workers >= 0')
+        return run_denoise(args, sigma)
+    if args.denoise_window is not None:
+        p.error('--denoise-window goes with --denoise')
     if args.inpaint is not None:
         if args.path is None or args.mode != 'test':
             p.error('--inpaint removes objects from a frame directory: it needs --path DIR (and no -m val)')
@@ -664,6 +743,33 @@ def run_inpaint(args):
                              dilate=args.inpaint_dilate, labels=args.inpaint_labels, batch=args.batch,
                              workers=args.workers, scene_cut=args.scene_cut)
     print(f"{len(files)} frames with the masked objects removed written under {args.out}")
+    return 0
+
+
+def run_denoise(args, sigma):
+    """--path --denoise: raft_b200.video.video_denoise over the frames of --path, the flow at 432x1024 (or --flow-size)
+    like test mode (or the frames' own size with --keep-size), the frames written at their own size."""
+    from raft_b200.video import video_denoise
+    model = _video_model(args)
+    files, _ = video_denoise(model, args.path, args.out, sigma, window=args.denoise_window, batch=args.batch,
+                             workers=args.workers, scene_cut=args.scene_cut)
+    print(f"{len(files)} denoised frames written under {args.out}")
+    return 0
+
+
+def validate_denoise(args, sigma):
+    """-m val --dataset davis --denoise SIGMA: raft_b200.davis.evaluate_denoise on --data, the summary line on stdout,
+    the per-sequence records in <--out>/val_davis_denoise.json."""
+    import json
+    from networks import RAFT
+    from raft_b200.davis import evaluate_denoise, denoise_summary
+    model = RAFT.RAFT(None, args, upstream=args.upstream, mixed_precision=args.mixed_precision).load(args.load)
+    res = evaluate_denoise(model, args.data, sigma, window=args.denoise_window, batch=args.batch,
+                           iters=args.iters)
+    print(denoise_summary(res))
+    os.makedirs(args.out, exist_ok=True)
+    with open(os.path.join(args.out, "val_davis_denoise.json"), "w") as f:
+        json.dump(res, f, indent=1)
     return 0
 
 

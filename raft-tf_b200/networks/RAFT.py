@@ -220,6 +220,18 @@ class RAFT(object):
         return self.engine().inpaint(_as_tensor(frames), masks, window=window, dilate=dilate, labels=labels, cuts=cuts)
 
     @torch.no_grad()
+    def denoise(self, frames, sigma, window=None, cuts=None):
+        """Extension (video denoising): [F,Hs,Ws,3] uint8 frames (sources as for ``forward``) with additive noise of
+        standard deviation sigma grey levels removed (sigma="auto": estimated from the first frames).  One
+        ``forward_sequence_bidirectional`` pass; every pixel followed through the flows up to `window` frames each way
+        (default raft_b200.denoise.DEFAULT_WINDOW), stopping at the first step that fails the forward-backward test and
+        never crossing a scene-cut pair of cuts, and merged with the patches that match it there and around it in its
+        own frame (RaftEngine.denoise).  Returns fresh (frames [F,Hs,Ws,3] uint8, support [F,Hs,Ws] uint8: the frames
+        matched per pixel) CUDA tensors at the frames' own size.  A bad sigma, window or cuts raise ValueError before
+        the pass."""
+        return self.engine().denoise(_as_tensor(frames), sigma, window=window, cuts=cuts)
+
+    @torch.no_grad()
     def interpolate_sequence(self, frames, t=0.5, uint8=False, bgr=False, native=False):
         """Extension (frame-rate up-conversion): the frames at time t (a float, or a sequence of times, each in [0, 1])
         between every pair of consecutive frames of [T+1,H,W,3] frames, from one ``forward_sequence_bidirectional`` pass.

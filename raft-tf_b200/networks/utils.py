@@ -697,6 +697,80 @@ def inpaint_propagate(frames, hole, flow_fw, flow_bw, rows, flow_scale=1.0, alph
     return colour, status
 
 
+def _rows_table(what, rows, F, dev):
+    """An [n,3] integer (t, nf, nb) table checked against F frames, as int32 on dev."""
+    table = torch.as_tensor(rows).cpu()
+    if not (table.dim() == 2 and table.shape[0] >= 1 and table.shape[1] == 3 and not table.is_floating_point()
+            and not table.is_complex()):
+        raise ValueError(f"{what}: rows must be an [n,3] integer table (got {list(table.shape)} {table.dtype})")
+    t, nf, nb = table.to(torch.int64).unbind(1)
+    if not (((t >= 0) & (t < F) & (nf >= 0) & (t + nf <= F - 1) & (nb >= 0) & (nb <= t)).all()):
+        raise ValueError(f"{what}: each row (t, nf, nb) needs t in [0, {F}), 0 <= nf <= F-1-t and 0 <= nb <= t")
+    return table.to(device=dev, dtype=torch.int32).contiguous()
+
+
+def denoise_merge(frames, flow_fw, flow_bw, rows, sigma, flow_scale=1.0, alpha1=0.01, alpha2=0.5):
+    """Extension (video denoising): each pixel of F frames merged with its patch matches along the chained flows
+    (rb_denoise_merge).  frames [F,Hs,Ws,3] uint8 CUDA tensor; flow_fw, flow_bw [F-1,Hn,Wn,2] float32 consecutive flows;
+    rows [n,3] integer table (t, nf, nb) (raft_b200.inpaint.inpaint_rows): the frame of each output row and how many
+    steps each side may chain (at most raft_b200.denoise.MAX_WINDOW count); sigma > 0 the noise's standard deviation in
+    grey levels.  Each side follows the flows with the forward-backward test of fb_consistency at every step and stops
+    at the first step that fails; every frame reached is a match.  Returns fresh (frames [n,Hs,Ws,3] uint8, support
+    [n,Hs,Ws] uint8: the matched frames of both sides).  Bad shapes, a bad table or a bad sigma raise ValueError."""
+    import math
+    if not (isinstance(frames, torch.Tensor) and frames.is_cuda and frames.dim() == 4 and frames.shape[-1] == 3
+            and frames.dtype == torch.uint8):
+        raise ValueError(f"denoise_merge: frames must be an [F,Hs,Ws,3] uint8 CUDA tensor (got "
+                         f"{getattr(frames, 'shape', None)} {getattr(frames, 'dtype', type(frames))})")
+    F, Hs, Ws, _ = frames.shape
+    dev = frames.device
+    T, Hn, Wn = _flow_pair("denoise_merge", flow_fw, flow_bw)
+    if T != F - 1 or flow_fw.device != dev:
+        raise ValueError(f"denoise_merge: {F} frames need [F-1,Hn,Wn,2] = [{F - 1},Hn,Wn,2] flows on {dev} (got "
+                         f"{tuple(flow_fw.shape)})")
+    try:
+        sigma = float(sigma)
+    except (TypeError, ValueError):
+        sigma = float("nan")
+    if not (math.isfinite(sigma) and sigma > 0):
+        raise ValueError("denoise_merge: sigma must be a finite number > 0")
+    table = _rows_table("denoise_merge", rows, F, dev)
+    n = table.shape[0]
+    f, fw, bw = frames.contiguous(), flow_fw.contiguous(), flow_bw.contiguous()
+    out = torch.empty(n, Hs, Ws, 3, dtype=torch.uint8, device=dev)
+    support = torch.empty(n, Hs, Ws, dtype=torch.uint8, device=dev)
+    with torch.cuda.device(dev):
+        capi.check(capi.lib.rb_denoise_merge(capi.ptr(f), F, Hs, Ws, capi.ptr(fw), capi.ptr(bw), Hn, Wn,
+                                             float(flow_scale), float(alpha1), float(alpha2), capi.ptr(table), n,
+                                             sigma, capi.ptr(out), capi.ptr(support), capi.stream()))
+    return out, support
+
+
+def noise_sums(frames):
+    """Extension (video denoising): rb_noise_sums of [N,H,W,3] uint8 CUDA frames (H, W >= 3) -- the [N,3] int64 sums of
+    |I * M| over the interior pixels per frame and channel, M Immerkaer's mask [[1,-2,1],[-2,4,-2],[1,-2,1]]."""
+    if not (isinstance(frames, torch.Tensor) and frames.is_cuda and frames.dim() == 4 and frames.shape[-1] == 3
+            and frames.dtype == torch.uint8 and frames.shape[0] >= 1 and min(frames.shape[1:3]) >= 3):
+        raise ValueError(f"noise_sums: frames must be an [N,H,W,3] uint8 CUDA tensor with N >= 1 and H, W >= 3 (got "
+                         f"{getattr(frames, 'shape', None)} {getattr(frames, 'dtype', type(frames))})")
+    N, H, W, _ = frames.shape
+    f = frames.contiguous()
+    sums = torch.empty(N, 3, dtype=torch.int64, device=f.device)
+    with torch.cuda.device(f.device):
+        capi.check(capi.lib.rb_noise_sums(capi.ptr(f), N, H, W, capi.ptr(sums), capi.stream()))
+    return sums
+
+
+def noise_sigma(frames):
+    """Extension (video denoising): Immerkaer's estimate ("Fast noise variance estimation", CVIU 1996) of the
+    standard deviation of additive white noise in [N,H,W,3] uint8 CUDA frames, in grey levels: sqrt(pi/2) S /
+    (6 (H-2)(W-2)) per frame and channel from noise_sums, averaged over both.  Exactly 0 on frames that are locally
+    linear (flat frames, ramps)."""
+    from raft_b200.denoise import sigma_from_sums
+    sums = noise_sums(frames)
+    return sigma_from_sums(sums.cpu().numpy(), frames.shape[1], frames.shape[2])
+
+
 def _margin(what, margin):
     try:
         my, mx = (int(v) for v in margin)

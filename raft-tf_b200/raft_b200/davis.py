@@ -223,3 +223,132 @@ def run(engine, seqs, batch=1, rgb=False, masks_out=None, keyframe_step=None):
                 write_labels(os.path.join(d, os.path.basename(p)), m, palette)
         records.append({"name": seq.name, "n_frames": F, "n_objects": n_obj, "objects": objects})
     return records
+
+
+# ---- video denoising (F27) -------------------------------------------------------------------------------------------
+# The video-denoising protocol of DVDnet / FastDVDnet (Tassano et al.) on DAVIS-2017 test-dev, frames only:
+#
+#     res = evaluate_denoise(RAFT(None, args).load("raft-things.npz"), "datasets/DAVIS", sigma=20)
+#
+# Noise: additive Gaussian noise of sigma grey levels on every frame of <root>/ImageSets/2017/test-dev.txt's sequences,
+# seeded per frame from numpy's PCG64 with (crc32(sequence name), frame index), z drawn as [H,W,3] in RGB order, and the
+# noisy frame clip(rint(clean + sigma z), 0, 255) as uint8 -- unlike the published protocol, which feeds unclipped float
+# frames, so the numbers are close to published tables but not directly comparable.  The merge uses the true sigma; the
+# flow runs at the frames' own size, 20 iterations, 'sintel' padding (PROTOCOLS["davis"]).  Metrics: PSNR and SSIM of the
+# uint8 output against the clean frame (rb_frame_metrics), per-frame PSNR averaged within a sequence, then over the
+# sequences; the noisy input's alongside.
+Clip = namedtuple("Clip", "name frames")
+
+
+def davis_frames(root, split="test-dev"):
+    """The sequences of <root>/ImageSets/2017/<split>.txt, each Clip(name, frame paths) in sorted order -- frames only,
+    no annotations.  A missing list or directory, or a sequence of fewer than two frames, raises (FileNotFoundError /
+    ValueError) naming it."""
+    root = os.fspath(root)
+    lst = os.path.join(root, "ImageSets", "2017", f"{split}.txt")
+    if not os.path.isfile(lst):
+        raise FileNotFoundError(f"DAVIS: no sequence list {lst}")
+    with open(lst) as f:
+        names = [line.strip() for line in f if line.strip()]
+    if not names:
+        raise ValueError(f"DAVIS: {lst} lists no sequence")
+    clips = []
+    for name in names:
+        fdir = os.path.join(root, "JPEGImages", "480p", name)
+        if not os.path.isdir(fdir):
+            raise FileNotFoundError(f"DAVIS: sequence {name}: no directory {fdir}")
+        frames = sorted(f for f in os.listdir(fdir) if f.endswith(".jpg"))
+        if len(frames) < 2:
+            raise ValueError(f"DAVIS: sequence {name} has {len(frames)} frames; denoising needs two at least")
+        clips.append(Clip(name, [os.path.join(fdir, f) for f in frames]))
+    return clips
+
+
+def noisy_frame(clean, name, index, sigma):
+    """The protocol's noisy copy of frame `index` of sequence `name`: clean [H,W,3] uint8 in RGB order plus sigma z, z
+    standard normal [H,W,3] from PCG64 seeded with (crc32(name), index), rounded half to even and clipped to uint8."""
+    import zlib
+    rng = np.random.Generator(np.random.PCG64([zlib.crc32(name.encode()), int(index)]))
+    z = rng.standard_normal(clean.shape)
+    return np.clip(np.rint(clean.astype(np.float64) + float(sigma) * z), 0, 255).astype(np.uint8)
+
+
+def psnr_ssim(stats, H, W):
+    """Per-frame (PSNR, SSIM) [n] fp64 of rb_frame_metrics' [n,2] {sse, ssim}: PSNR = 10 log10(255^2 3HW / sse), inf
+    when sse = 0."""
+    s = np.asarray(stats, np.float64)
+    with np.errstate(divide="ignore"):
+        psnr = 10.0 * np.log10(255.0 ** 2 * 3 * H * W / s[:, 0])
+    return psnr, s[:, 1]
+
+
+def denoise_clip(engine, frames, sigma, window=None, batch=8):
+    """RaftEngine.denoise's bits for frames [F,Hs,Ws,3] uint8 (the engine's channel order, a CUDA tensor) with the flows
+    of interp_schedule(F, batch) passes kept on the GPU, so a long sequence needs no single pass over all its pairs.
+    Returns (frames [F,Hs,Ws,3] uint8, support [F,Hs,Ws] uint8) CUDA tensors."""
+    from .denoise import DEFAULT_WINDOW, check_window, merge_frames
+    from .inpaint import inpaint_rows
+    from .video import interp_schedule
+    F = len(frames)
+    window = check_window(DEFAULT_WINDOW if window is None else window, "DAVIS")
+    fws, bws = [], []
+    for ps in interp_schedule(F, batch):
+        fw, bw, _, _ = engine.forward_sequence_bidirectional(frames[ps.frames], check=False)
+        n = sum(k is not None for k in ps.pairs)
+        fws.append(fw[:n].clone())
+        bws.append(bw[:n].clone())
+    with torch.cuda.device(engine.device):
+        return merge_frames(frames, torch.cat(fws), torch.cat(bws), inpaint_rows(F, window), sigma, engine.flow_scale)
+
+
+def evaluate_denoise(model, root, sigma, window=None, batch=8, iters=None):
+    """Video denoising of a loaded networks.RAFT.RAFT model on a DAVIS-2017 tree's test-dev frames (the protocol above).
+    A model with input_size, a sigma that is not a number > 0 ("auto" included: the protocol knows its noise) or a bad
+    window raise ValueError before any frame is read.  Returns {"dataset", "split", "sigma", "iters", "pad_mode",
+    "window", "PSNR", "SSIM", "noisy_PSNR", "noisy_SSIM", "n_sequences", "sequences": [per-sequence records]}; the same
+    for every batch."""
+    from networks.utils import frame_metrics
+    from .denoise import DEFAULT_WINDOW, check_sigma, check_window
+    from .evaluate import PROTOCOLS, _engine, _imread
+    if getattr(model, "input_size", None) is not None:
+        raise ValueError("evaluate_denoise: frames run at their own size; build the model without input_size")
+    if isinstance(sigma, str):
+        raise ValueError(f"evaluate_denoise: the protocol adds noise of a known level: sigma must be a number > 0 "
+                         f"(got {sigma!r})")
+    sigma = check_sigma(sigma, "evaluate_denoise")
+    window = check_window(DEFAULT_WINDOW if window is None else window, "evaluate_denoise")
+    if int(batch) < 1:
+        raise ValueError(f"evaluate_denoise: batch must be >= 1 (got {batch})")
+    if model._params is None:
+        raise RuntimeError("RAFT.load(<npz>) must be called before evaluate_denoise")
+    clips = davis_frames(root)  # every directory checked up front
+    n_iters, pad_mode = PROTOCOLS["davis"]
+    n_iters = n_iters if iters is None else int(iters)
+    engine = _engine(model, n_iters, pad_mode)
+    dev = engine.device
+    records = []
+    for clip in clips:
+        clean = np.stack([_imread(p, True) for p in clip.frames])
+        noisy = np.stack([noisy_frame(c, clip.name, i, sigma) for i, c in enumerate(clean)])
+        if not model.upstream:  # the engine's channel order
+            clean, noisy = clean[..., ::-1], noisy[..., ::-1]
+        F, H, W, _ = clean.shape
+        with torch.cuda.device(dev):
+            gt = torch.from_numpy(np.ascontiguousarray(clean)).to(dev)
+            inp = torch.from_numpy(np.ascontiguousarray(noisy)).to(dev)
+            out, support = denoise_clip(engine, inp, sigma, window, int(batch))
+            p_out, s_out = psnr_ssim(frame_metrics(out, gt).cpu().numpy(), H, W)
+            p_in, s_in = psnr_ssim(frame_metrics(inp, gt).cpu().numpy(), H, W)
+            mean_support = float(support.double().mean().item())
+        records.append({"name": clip.name, "n_frames": F, "PSNR": float(p_out.mean()), "SSIM": float(s_out.mean()),
+                        "noisy_PSNR": float(p_in.mean()), "noisy_SSIM": float(s_in.mean()), "support": mean_support})
+    mean = lambda k: float(np.mean([r[k] for r in records]))  # noqa: E731
+    return {"dataset": "davis", "split": "test-dev", "sigma": sigma, "iters": n_iters, "pad_mode": pad_mode,
+            "window": window, "PSNR": mean("PSNR"), "SSIM": mean("SSIM"), "noisy_PSNR": mean("noisy_PSNR"),
+            "noisy_SSIM": mean("noisy_SSIM"), "n_sequences": len(records), "sequences": records}
+
+
+def denoise_summary(res):
+    """The summary line of evaluate_denoise's result."""
+    return (f"Validation DAVIS-2017 denoising (test-dev, sigma {res['sigma']:g}): PSNR: {res['PSNR']:.4f}, SSIM: "
+            f"{res['SSIM']:.4f} (noisy: PSNR: {res['noisy_PSNR']:.4f}, SSIM: {res['noisy_SSIM']:.4f})")

@@ -687,6 +687,35 @@ class RaftEngine:
             return fill_frames(frames.to(self.device), hole, fw, bw, rows, self.flow_scale)
 
     @torch.no_grad()
+    def denoise(self, frames: torch.Tensor, sigma, window=None, cuts=None):
+        """Video denoising of [F,Hs,Ws,3] uint8 frames (sizes and input_size as for forward()): sigma the noise's
+        standard deviation in grey levels, or "auto" (raft_b200.denoise.estimate_sigma on the first frames; an estimate
+        of 0 returns the frames unchanged without a flow pass).  One forward_sequence_bidirectional(check=False) pass and
+        one rb_denoise_merge launch over raft_b200.inpaint.inpaint_rows(F, window, cuts) (window default
+        raft_b200.denoise.DEFAULT_WINDOW frames each way; no side crosses a cut): each pixel merged with its patch matches
+        in frame t and in every frame the chained flows reach through the forward-backward test.  Returns fresh (frames
+        [F,Hs,Ws,3] uint8, support [F,Hs,Ws] uint8: the matched frames per pixel) CUDA tensors at the frames' own size.
+        Non-uint8 frames, a bad sigma, window or cuts raise ValueError before the pass."""
+        from .denoise import DEFAULT_WINDOW, check_sigma, check_window, estimate_sigma, merge_frames
+        from .inpaint import inpaint_rows
+        from .video import check_cuts
+        F = _sequence_length(frames) + 1
+        if frames.dtype != torch.uint8:
+            raise ValueError(f"raft_b200: denoise writes bytes: the frames must be uint8 (got {frames.dtype})")
+        sigma = check_sigma(sigma, "raft_b200")
+        window = check_window(DEFAULT_WINDOW if window is None else window, "raft_b200")
+        rows = inpaint_rows(F, window, check_cuts(() if cuts is None else cuts, F, "raft_b200"))
+        with torch.cuda.device(self.device):
+            on_dev = frames.to(self.device)
+            if sigma == "auto":
+                sigma = estimate_sigma(on_dev)
+            if sigma == 0:
+                return merge_frames(on_dev, None, None, rows, 0, self.flow_scale)
+        flow_fw, flow_bw, _, _ = self.forward_sequence_bidirectional(frames, check=False)
+        with torch.cuda.device(self.device):
+            return merge_frames(on_dev, flow_fw, flow_bw, rows, sigma, self.flow_scale)
+
+    @torch.no_grad()
     def interpolate(self, left: torch.Tensor, right: torch.Tensor, ts, native: bool = False) -> torch.Tensor:
         """Frames at times ts (each in [0, 1]; 0 = left, 1 = right) between B frame pairs: one bidirectional pass (as
         forward_bidirectional(check=False), from a graph of its own), then eagerly on the same stream, for as many times

@@ -48,7 +48,12 @@ each pass's flows completed inside the holes on the GPU (rb_masked_fill), every 
 see behind its holes (rb_inpaint_propagate) once the pairs it may reach have run, and the rest filled spatially; written
 as out/frame_<i:06d>.png.
 
-Scene cuts (scene_cut=<threshold in [0, 1]>, video_interpolate, video_stabilize, video_inpaint and warm-started video): each pass's
+video_denoise(model, "frames/", "out/", sigma=20) removes additive noise: the same sweep, every frame merged with its
+patch matches in the neighbouring frames the chained flows reach consistently (rb_denoise_merge) once the pairs it may
+reach have run; written as out/frame_<i:06d>.png.
+
+Scene cuts (scene_cut=<threshold in [0, 1]>, video_interpolate, video_stabilize, video_inpaint, video_denoise and
+warm-started video): each pass's
 decoded frames are copied to the GPU once and scored there (networks.utils.scene_cut_scores: one minus the intersection
 of consecutive frames' colour histograms); a pair whose score exceeds the threshold is a cut.  Frame-rate conversion
 copies the nearer input frame instead of blending two shots (cut_copy(), split_cut_items()), warm-started flow restarts
@@ -1319,3 +1324,102 @@ def video_inpaint(model, frames, out, masks, window=None, dilate=None, labels=No
     print(f"inpaint: pixels filled from both sides {counts[1]}, from one side {counts[2]}, spatially {counts[3]}")
     print(f"scene cuts: {len(cuts)}" + (" at pairs " + " ".join(str(k) for k in cuts) if cuts else ""))
     return names, {"counts": counts[1:].tolist(), "cuts": cuts}
+
+
+def video_denoise(model, frames, out, sigma, window=None, batch=8, workers=4, scene_cut=None):
+    """Video denoising of a clip of any length with a loaded networks.RAFT.RAFT model, in one sweep: the frames (a
+    directory's sorted *.png / *.jpg, or a list of paths, all of one size) with additive noise of standard deviation
+    sigma grey levels removed (sigma="auto": estimated from frames 0 .. 7, raft_b200.denoise.estimate_sigma), written as
+    <out>/frame_<i:06d>.png, equal byte for byte to RAFT.denoise on the whole clip for every batch and workers value.
+
+    Passes come from interp_schedule(): forward_sequence_bidirectional(check=False) on batch + 1 frames.  A window of the
+    clip stays on the GPU: the uploaded frames and the flows of the frames from t - window to the newest.  Frame t is
+    merged (rb_denoise_merge) and written once the pairs up to min(t + window, F - 1) have run, and the frames no later
+    frame reaches are dropped, so memory is bounded by the window, not the clip: 3 Hs Ws bytes (the frame) plus 16 Hn Wn
+    (the two flows) per kept frame, at most 2 window + batch + 2 of them -- about 13.3 MB per frame for 1080x1920 frames
+    and 432x1024 flows (by arithmetic), 0.21 GB at window 3, batch 8.  scene_cut (a threshold in [0, 1]) scores each
+    pass's frames on the GPU (networks.utils.scene_cut_scores); no side crosses a cut pair.  Prints the sigma used, the
+    mean support (matched frames per pixel) and the cuts.  Frames go in RGB with model.upstream and BGR otherwise, like
+    the CLI; the files are BGR.  Returns (paths, info), info a dict of "sigma", "support" (the mean) and "cuts"."""
+    import cv2
+    from networks.utils import scene_cut_scores
+    from .denoise import DEFAULT_WINDOW, ESTIMATE_FRAMES, check_sigma, check_window, estimate_sigma, merge_frames
+    from .inpaint import inpaint_rows
+
+    paths = list_frames(frames)
+    F = len(paths)
+    sigma = check_sigma(sigma, "video_denoise")
+    window = check_window(DEFAULT_WINDOW if window is None else window, "video_denoise")
+    thr = None if scene_cut is None else check_scene_cut(scene_cut)
+    batch, workers = int(batch), _workers(workers)
+    passes = interp_schedule(F, batch)
+    out = os.fspath(out)
+    os.makedirs(out, exist_ok=True)
+    engine = model.engine()
+    rgb = bool(model.upstream)
+    dev = engine.device
+    if sigma == "auto":
+        with torch.cuda.device(dev):
+            sigma = estimate_sigma(torch.from_numpy(np.stack([_imread(p, rgb) for p in paths[:ESTIMATE_FRAMES]])).to(dev))
+    cap = min(F, 2 * window + batch + 2)  # frames kept on the GPU
+    names = [os.path.join(out, f"frame_{i:06d}.png") for i in range(F)]
+    total, lock = [0], threading.Lock()
+    cuts, on_dev, store = [], None, None
+    base = have = done = 0  # store row 0 is frame base; frames base .. base + have - 1 are kept; frames < done written
+
+    def write(slot, first, n):  # writer thread: the merged frames of one pass, once its copies have landed
+        if slot is None:
+            return
+        slot.event.synchronize()
+        for r in range(n):
+            img = slot.frames[r].numpy()
+            if not cv2.imwrite(names[first + r], cv2.cvtColor(img, cv2.COLOR_RGB2BGR) if rgb else img):
+                raise OSError(f"cannot write {names[first + r]}")
+        s = int(slot.support[:n].numpy().sum(dtype=np.int64))
+        with lock:
+            total[0] += s
+
+    with _Pipeline(paths, passes, rgb, batch, workers, dev) as pipe:
+        for j, ps, imgs, src in pipe:
+            Hs, Ws = src.shape[1:3]
+            if on_dev is None:
+                on_dev = torch.empty(src.shape, dtype=torch.uint8, device=dev)
+            on_dev.copy_(src, non_blocking=True)
+            if thr is not None:
+                cuts += pass_cuts(ps.pairs, scene_cut_scores(on_dev).cpu(), thr)
+            flow_fw, flow_bw, _, _ = engine.forward_sequence_bidirectional(on_dev, check=False)
+            n = sum(k is not None for k in ps.pairs)
+            first = ps.frames[0]
+            if store is None:
+                Hn, Wn = flow_fw.shape[1:3]
+                store = dict(frames=torch.empty(cap, Hs, Ws, 3, dtype=torch.uint8, device=dev),
+                             fw=torch.empty(cap, Hn, Wn, 2, dtype=torch.float32, device=dev),
+                             bw=torch.empty(cap, Hn, Wn, 2, dtype=torch.float32, device=dev))
+            new = list(range(base + have, first + n + 1))  # the pass's frames not kept yet
+            if have + len(new) > cap:  # drop the frames no frame still to be written reaches
+                drop = max(done - window, base) - base
+                for t in store.values():
+                    t[:have - drop].copy_(t[drop:have].clone())
+                base, have = base + drop, have - drop
+            store["frames"][have:have + len(new)].copy_(on_dev[new[0] - first:new[-1] - first + 1])
+            have += len(new)
+            store["fw"][first - base:first - base + n].copy_(flow_fw[:n])
+            store["bw"][first - base:first - base + n].copy_(flow_bw[:n])
+            ran = first + n  # pairs 0 .. ran - 1 have run
+            last = done
+            while last < F and min(last + window, F - 1) <= ran:
+                last += 1
+            res = None
+            if last > done:
+                rows = inpaint_rows(F, window, sorted(cuts))[done:last].copy()
+                rows[:, 0] -= base
+                res = merge_frames(store["frames"][:have], store["fw"][:have - 1], store["bw"][:have - 1], rows, sigma,
+                                   engine.flow_scale)
+            pipe.emit(partial(write, first=done, n=last - done), cap, frames=None if res is None else res[0],
+                      support=None if res is None else res[1])
+            done = last
+    cuts = sorted(cuts)
+    mean = total[0] / (F * Hs * Ws)
+    print(f"denoise: sigma {sigma:.4g}, mean support {mean:.3f} frames")
+    print(f"scene cuts: {len(cuts)}" + (" at pairs " + " ".join(str(k) for k in cuts) if cuts else ""))
+    return names, {"sigma": float(sigma), "support": mean, "cuts": cuts}
