@@ -563,6 +563,70 @@ int rb_denoise_merge(const uint8_t* frames, int F, int Hs, int Ws, const float* 
                      uint8_t* out, uint8_t* support, void* stream);
 int rb_noise_sums(const uint8_t* frames, int N, int H, int W, int64_t* sums, void* stream);
 
+/* ---- F29: temporal consistency -- the per-pixel temporal term of a processed frame (Bonneel et al. 2015) ----------
+ * rb_tcons_terms: frame I_t, prev_frame I_(t-1), processed P_t, prev_out O_(t-1): [Hs,Ws,3] uint8; flow_fw, flow_bw
+ * [Hn,Wn,2] fp32 the pair (t-1, t) (flow_fw frame t-1 -> t, flow_bw t -> t-1); strength lambda.  Outputs c [Hs,Ws] fp32,
+ * r [Hs,Ws,3] fp32 and status [Hs,Ws] uint8.  Per pixel p = (x, y), every fp32 operation rounded on its own:
+ *   step: p0 = (fl32((x + 0.5) Wn/Ws - 0.5), likewise y) in fp64, clamped into the grid (fb_sample.cuh's px_remap);
+ *     one step of rb_track_points' step backward: f = s * the bilinear sample of flow_bw at p0, q = p0 + f; it fails
+ *     when q leaves the grid or the F5 test against s * flow_fw at q fails (status 1).  o = (fl32((q + 0.5) Ws/Wn -
+ *     0.5), likewise y) in fp64, clamped into the frame -- rb_denoise_merge's first backward step, bit for bit.
+ *   check: I^, O^ the bilinear samples (bilerp_at / bilerp1) of I_(t-1), O_(t-1) at o; d = (0 + e_0^2 + e_1^2 + e_2^2) / 3
+ *     with e_ch = I_t(p) - I^; x = d / fl32(RB_TCONS_KAPPA^2); w = (1 - x)^2 when x < 1 (status 0), else 0 (status 2).
+ *   terms: c = fl32(lambda w) + RB_TCONS_EPS; r = fl32(lambda w) (O^ - P_t(p)) per channel where status is 0, else +0.
+ * prev_frame = NULL means no previous frame (frame 0, or the first frame after a scene cut): status 3, c = RB_TCONS_EPS,
+ * r = 0, and only the outputs are touched.  One thread per pixel; no allocation.  Null pointers, Hs/Ws/Hn/Wn <= 0, a
+ * frame of >= 2^31 pixels, flow_scale <= 0 or non-finite, negative or non-finite alphas and strength <= 0 or non-finite
+ * -> RB_ERR_* before any CUDA call.  RB_TCONS_KAPPA is in grey levels, chosen on the synthetic clip of
+ * tests/test_temporal.py; it is not tuned on real footage.
+ * ---- F30: the screened Poisson solve of the correction D = O_t - P_t ----
+ * rb_screened_poisson: c [H,W] fp32 (> 0), r [H,W,3] fp32; D [H,W,3] fp32 (not aliasing r) approximates per channel
+ *   (c_p + n_p) D_p - sum_(q in N(p)) D_q = r_p,  N(p) the in-image 4-neighbours and n_p their count (Neumann boundary).
+ * Method (tests/tcons_oracle.py restates it bit for bit):
+ *   levels   level l+1 halves level l with ceil down to 1 x 1 (rb_masked_fill's pyramid); a coarse pixel's children are
+ *            (2i,2j), (2i,2j+1), (2i+1,2j), (2i+1,2j+1) (this order) inside level l; c_(l+1) = 0 + the children's c in
+ *            order.  Every level keeps the unit 4-neighbour coupling (rediscretised, not Galerkin).
+ *   stencil  s = f + e_up + e_down + e_left + e_right (+0 for a neighbour outside the level), n = 0 + 1 per in-level
+ *            neighbour in the same order; residual s - (n e + c e); sweep e = s / (c + n).
+ *   V-cycle  V(f) from e = 0 on level 0: on each level RB_TCONS_SWEEPS red-black Gauss-Seidel sweeps (red, x + y even,
+ *            first), the next level's f = 0 + the residuals of the children in order and its e = 0, down to 1 x 1 (the
+ *            same sweeps there); up: each pixel adds the cell-centred bilinear value of the coarser e (weights 1/4, 3/4
+ *            per axis, taps clamped, ((wxa e_aa + wxb e_ab) wya) + ((wxa e_ba + wxb e_bb) wyb)), then the sweeps.
+ *   solve    flexible preconditioned conjugate gradients, per channel, from D = 0: res = r, z = V(res), p = z,
+ *            rho = <res, z>; then RB_TCONS_ITERS times: q = A p, alpha = fl32(rho / <p, q>) (0 unless <p, q> > 0),
+ *            D += alpha p, res' = res - alpha q, d = res' - res, res = res'; and except after the last: z = V(res),
+ *            beta = fl32(<z, d> / rho) (0 unless rho > 0), rho = <res, z>, p = z + beta p.  A p = -(the residual of p
+ *            with f = 0).
+ *   dots     <a, b> per channel in fp64 of the exact products: blocks of 1024 pixels, thread t adds pixels t + 256 k,
+ *            k = 0..3, in order from 0 (0 past the end), then the tree s[t] += s[t + h], h = 128, ..., 1; the block
+ *            partials likewise by one block (thread t: partials t + 256 k in order, then the tree).
+ * r = 0 gives D = 0 bit for bit.  Deterministic: no atomics and a fixed sequence of launches and device copies, 61 L + 12
+ * of them at the constants below for L levels (744 for 1080 x 1920, L = 12); no allocation (workspace:
+ * rb_screened_poisson_workspace_bytes, about 17 H W floats).  Null pointers, H/W <= 0, H*W >= 2^31, any overlap of D, c, r and
+ * the workspace (except c with r, both read only) and a workspace that is too small -> RB_ERR_* before any CUDA call.
+ * ---- F31: the warping error E_warp of a video aligned with the frames (Lai et al., ECCV 2018) ----
+ * rb_warp_error: video [F,Hs,Ws,3] uint8 (F >= 2); flow_fw, flow_bw [F-1,Hn,Wn,2] fp32 of the original frames.  Per pixel
+ * p of frame k < F-1: one forward step (flow_fw[k] pulls, flow_bw[k] tests; F29's map and step, mirrored); where it
+ * passes, e = 0 + sum_ch (V_k(p) - V^_(k+1)(o))^2 in fp32, V^ the bilinear sample.  sums [F-1,2] fp64 = (sum e, count)
+ * per pair: blocks of 4096 pixels (thread t: pixels t + 256 k, k = 0..15, in order), the fixed tree, then one block
+ * per pair adds its partials in a fixed order (workspace: rb_warp_error_workspace_bytes).  The host forms E_pair =
+ * sum e / (255^2 count).  Null pointers, F < 2, F - 1 > 65535, Hs/Ws/Hn/Wn <= 0, a frame of >= 2^31 pixels, bad
+ * flow_scale or alphas and a workspace that is too small -> RB_ERR_* before any CUDA call. */
+#define RB_TCONS_KAPPA 20.0f
+#define RB_TCONS_EPS 1e-4f
+#define RB_TCONS_ITERS 6
+#define RB_TCONS_SWEEPS 2
+int rb_tcons_terms(const uint8_t* frame, const uint8_t* prev_frame, const uint8_t* processed, const uint8_t* prev_out,
+                   int Hs, int Ws, const float* flow_fw, const float* flow_bw, int Hn, int Wn, float flow_scale,
+                   float alpha1, float alpha2, float strength, float* c, float* r, uint8_t* status, void* stream);
+int rb_screened_poisson_workspace_bytes(int H, int W, size_t* bytes);
+int rb_screened_poisson(const float* c, const float* r, int H, int W, float* D, void* workspace, size_t workspace_bytes,
+                        void* stream);
+int rb_warp_error_workspace_bytes(int F, int Hs, int Ws, size_t* bytes);
+int rb_warp_error(const uint8_t* video, int F, int Hs, int Ws, const float* flow_fw, const float* flow_bw, int Hn,
+                  int Wn, float flow_scale, float alpha1, float alpha2, double* sums, void* workspace,
+                  size_t workspace_bytes, void* stream);
+
 /* ---- F6: frame interpolation -- flow_utils.py:166-274 reverse_flow_avg_skip_static, batched, and the frame blend -----
  * rb_flow_reverse: per sample of flow01 [B,H,W,2] fp32, bit for bit with the reference under numpy >= 2:
  *  1. static(p) = every channel c has d_c < 10, d_c = uint8(bg - im0) (img_u8 = 1: wraps, like numpy's uint8) or

@@ -26,13 +26,6 @@ struct DenoiseGeom {
   double rxn, ryn, rxs, rys;  // Wn / Ws, Hn / Hs, Ws / Wn, Hs / Hn
 };
 
-// x' = fl32((x + 0.5) r - 0.5) in fp64, each operation rounded on its own, clamped into [0, n - 1] (the pixel-centre map
-// of rb_inpaint_propagate)
-__device__ __forceinline__ float dn_remap(double x, double r, int n) {
-  const float v = __double2float_rn(__dsub_rn(__dmul_rn(__dadd_rn(x, 0.5), r), 0.5));
-  return fminf(fmaxf(v, 0.f), (float)(n - 1));
-}
-
 struct MergeAcc {
   float s[3];  // sum of w * centre colour per channel
   float w;     // sum of w
@@ -109,7 +102,7 @@ __device__ __forceinline__ int denoise_side(const uint8_t* __restrict__ frames, 
     if (!inside_frame(q.x, q.y, Hn, Wn)) break;
     if (fb_inconsistent(f, sample_flow(test, Wn, bilerp_at(q.x, q.y, Hn, Wn), s), a1, a2)) break;
     p = q;
-    const Bilerp b = bilerp_at(dn_remap(p.x, g.rxs, Ws), dn_remap(p.y, g.rys, Hs), Hs, Ws);
+    const Bilerp b = bilerp_at(px_remap(p.x, g.rxs, Ws), px_remap(p.y, g.rys, Hs), Hs, Ws);
     merge_frame(frames + (size_t)(t + dir * step) * ns * 3, Hs, Ws, b, ref, two_var, den, acc);
   }
   return step - 1;
@@ -152,7 +145,7 @@ __global__ void __launch_bounds__(kDenoiseThreads) denoise_merge_kernel(
     }
     MergeAcc acc = {{0.f, 0.f, 0.f}, 0.f};
     merge_frame(img, Hs, Ws, bilerp_at((float)x, (float)y, Hs, Ws), ref, two_var, den, acc);
-    const float2 p = make_float2(dn_remap(x, g.rxn, Wn), dn_remap(y, g.ryn, Hn));
+    const float2 p = make_float2(px_remap(x, g.rxn, Wn), px_remap(y, g.ryn, Hn));
     const int wf = min(min(max(nf, 0), RB_DENOISE_MAX_WINDOW), F - 1 - t);
     const int wb = min(min(max(nb, 0), RB_DENOISE_MAX_WINDOW), t);
     const int df = denoise_side(frames, fw, bw, t, 1, wf, p, Hs, Ws, Hn, Wn, g, s, a1, a2, ref, two_var, den, acc);

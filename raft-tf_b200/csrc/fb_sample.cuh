@@ -44,6 +44,13 @@ __device__ __forceinline__ float2 sample_flow(const float2* __restrict__ img, in
                      __fmul_rn(s, bilerp1(b, v00.y, v01.y, v10.y, v11.y)));
 }
 
+// x' = fl32((x + 0.5) r - 0.5) in fp64, each operation rounded on its own, clamped into [0, n - 1]: the pixel-centre map
+// between the network grid and a frame's own pixels (r = n_to / n_from)
+__device__ __forceinline__ float px_remap(double x, double r, int n) {
+  const float v = __double2float_rn(__dsub_rn(__dmul_rn(__dadd_rn(x, 0.5), r), 0.5));
+  return fminf(fmaxf(v, 0.f), (float)(n - 1));
+}
+
 // Whether q = p + f lies inside [0, W-1] x [0, H-1]; written so that a NaN coordinate counts as outside.
 __device__ __forceinline__ bool inside_frame(float qx, float qy, int H, int W) {
   return qx >= 0.f && qx <= (float)(W - 1) && qy >= 0.f && qy <= (float)(H - 1);

@@ -127,6 +127,16 @@ printed:
 
     python infer_raft.py --path noisy/ --out clean/ --denoise 20 --load raft-things.npz [--batch 8]
 
+--path ORIG --consistent PROC_DIR --consistent-strength L makes per-frame processed frames (PROC_DIR: as many as ORIG,
+the same size) temporally consistent, guided by the flow of the original frames (Bonneel et al. 2015;
+raft_b200.video.video_consistent); frames after a --scene-cut restart from the processed frame.  E_warp of the
+originals, the processed frames and the output, and the per-pixel status counts are printed:
+
+    python infer_raft.py --path orig/ --consistent styled/ --consistent-strength 0.1 --out stable/ --load raft-things.npz
+
+--path ORIG --warp-error VIDEO_DIR prints Lai et al.'s warping error of VIDEO_DIR under the flow of ORIG
+(raft_b200.video.video_warp_error) and writes the per-pair values to <--out>/warp_error.json.
+
 -m val --dataset davis --denoise SIGMA scores it on DAVIS-2017 test-dev (raft_b200.davis.evaluate_denoise): seeded
 Gaussian noise of SIGMA added to every frame, the flow at the frames' own size with 20 iterations, PSNR and SSIM of the
 output and of the noisy input printed (``Validation DAVIS-2017 denoising (test-dev, sigma S): ...``) and written to
@@ -299,6 +309,17 @@ def parser():
     p.add_argument('--denoise-window', type=int, default=None, metavar='N',
                    help='extension, with --denoise: the frames each side may look ahead or back (default 3, at most '
                         '16; not tuned)')
+    p.add_argument('--consistent', default=None, metavar='PROC_DIR',
+                   help="extension, with --path: make the per-frame processed frames of PROC_DIR (as many as --path, "
+                        "the same size) temporally consistent, guided by the flow of the --path frames (needs "
+                        "--consistent-strength); writes <--out>/frame_<i:06d>.png")
+    p.add_argument('--consistent-strength', type=float, default=None, metavar='L',
+                   help='extension, with --consistent: the strength lambda > 0 (no default); detail finer than about '
+                        '2 pi / sqrt(L) pixels keeps the processed frames\' gradients')
+    p.add_argument('--warp-error', default=None, metavar='VIDEO_DIR',
+                   help="extension, with --path: Lai et al.'s warping error E_warp of the frames of VIDEO_DIR (as many "
+                        "as --path, the same size) under the flow of the --path frames; with --out also writes "
+                        "<--out>/warp_error.json")
     p.add_argument('--upstream', action='store_true',
                    help='extension: weights converted from an official princeton-vl RAFT .pth (raft_b200.convert): RGB '
                         'frames and the upstream numerics (RAFT(..., upstream=True))')
@@ -308,9 +329,63 @@ def parser():
     return p
 
 
+def _temporal_refusals(p, args, flag, what):
+    """The refusals shared by --consistent and --warp-error."""
+    if args.path is None or args.mode != 'test':
+        p.error(f'{flag} works on a frame directory: it needs --path DIR (and no -m val)')
+    for other, given in (('--consistent', flag != '--consistent' and args.consistent is not None),
+                         ('--warp-error', flag != '--warp-error' and args.warp_error is not None),
+                         ('--denoise', args.denoise is not None), ('--inpaint', args.inpaint is not None),
+                         ('--stabilize', args.stabilize is not None), ('--stabilize-fill', args.stabilize_fill),
+                         ('--propagate', args.propagate is not None), ('--track', args.track is not None),
+                         ('--track-grid', args.track_grid is not None), ('--interpolate', args.interpolate),
+                         ('--fps', args.fps), ('--input-fps', args.input_fps), ('--warm-start', args.warm_start),
+                         ('--bidirectional', args.bidirectional), ('--native-flow', args.native_flow),
+                         ('--native-frames', args.native_frames), ('--flo', args.flo), ('--npy', args.npy),
+                         ('--keyframe-step', args.keyframe_step is not None)):
+        if given:
+            p.error(f'{flag} {what}: it cannot be combined with {other}')
+    if args.scene_cut is not None and not 0.0 <= args.scene_cut <= 1.0:
+        p.error(f'--scene-cut: {args.scene_cut} is not a threshold in [0, 1]')
+    if args.flow_size is not None and args.keep_size:
+        p.error('--flow-size sets the size frames are resized to; --keep-size runs them at their own size')
+    if args.batch < 1 or args.workers < 0:
+        p.error('--path needs --batch >= 1 and --workers >= 0')
+    from raft_b200.video import list_frames
+    other = args.consistent if flag == '--consistent' else args.warp_error
+    try:
+        a, b = list_frames(args.path), list_frames(other)
+    except (OSError, ValueError) as e:
+        p.error(f'{flag}: {e}')
+    if len(a) != len(b):
+        p.error(f'{flag}: {other} holds {len(b)} frames, --path {len(a)}: the frames must be aligned')
+    if len(a) < 2:
+        p.error(f'{flag}: a sequence needs two frames at least')
+    import cv2
+    sa, sb = cv2.imread(a[0]), cv2.imread(b[0])
+    if sa is None or sb is None or sa.shape != sb.shape:
+        p.error(f'{flag}: {b[0]} and {a[0]} differ in size (or cannot be read): the frames must be aligned')
+
+
 def main(argv=None):
     p = parser()
     args = p.parse_args(argv)
+    if args.consistent_strength is not None and args.consistent is None:
+        p.error('--consistent-strength goes with --consistent')
+    if args.consistent is not None:
+        L = args.consistent_strength
+        if L is None:
+            p.error('--consistent needs --consistent-strength L (no default)')
+        from raft_b200.temporal import check_strength
+        try:
+            check_strength(L)
+        except ValueError:
+            p.error(f'--consistent-strength: L must be a finite number > 0 (got {L})')
+        _temporal_refusals(p, args, '--consistent', 'writes consistent frames')
+        return run_consistent(args, L)
+    if args.warp_error is not None:
+        _temporal_refusals(p, args, '--warp-error', 'scores a video')
+        return run_warp_error(args)
     if args.denoise is not None:
         sigma = args.denoise
         if sigma != 'auto':
@@ -754,6 +829,34 @@ def run_denoise(args, sigma):
     files, _ = video_denoise(model, args.path, args.out, sigma, window=args.denoise_window, batch=args.batch,
                              workers=args.workers, scene_cut=args.scene_cut)
     print(f"{len(files)} denoised frames written under {args.out}")
+    return 0
+
+
+def run_consistent(args, strength):
+    """--path --consistent PROC_DIR: raft_b200.video.video_consistent, the flow of the --path frames at 432x1024 (or
+    --flow-size, or their own size with --keep-size), the frames written at their own size."""
+    from raft_b200.video import video_consistent
+    model = _video_model(args)
+    files, _ = video_consistent(model, args.path, args.consistent, args.out, strength, batch=args.batch,
+                                workers=args.workers, scene_cut=args.scene_cut)
+    print(f"{len(files)} consistent frames written under {args.out}")
+    return 0
+
+
+def run_warp_error(args):
+    """--path --warp-error VIDEO_DIR: raft_b200.video.video_warp_error; the summary line on stdout, the per-pair values
+    in <--out>/warp_error.json."""
+    from raft_b200.video import video_warp_error
+    model = _video_model(args)
+    info = video_warp_error(model, args.path, args.warp_error, batch=args.batch, workers=args.workers,
+                            scene_cut=args.scene_cut)
+    import json
+    for v in ("original", "input"):  # excluded pairs (NaN) as null
+        info[v]["E_pair"] = [None if e != e else e for e in info[v]["E_pair"]]
+        info[v]["E_warp"] = None if info[v]["E_warp"] != info[v]["E_warp"] else info[v]["E_warp"]
+    os.makedirs(args.out, exist_ok=True)
+    with open(os.path.join(args.out, "warp_error.json"), "w") as f:
+        json.dump(info, f, indent=1)
     return 0
 
 

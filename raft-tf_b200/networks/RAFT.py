@@ -232,6 +232,22 @@ class RAFT(object):
         return self.engine().denoise(_as_tensor(frames), sigma, window=window, cuts=cuts)
 
     @torch.no_grad()
+    def consistent(self, frames, processed, strength, cuts=None):
+        """Extension (temporal consistency): per-frame processed video made temporally consistent, guided by the flow of
+        the original frames (Bonneel et al., SIGGRAPH Asia 2015).  frames, processed: [F,Hs,Ws,3] uint8 (sources as for
+        ``forward``); strength > 0 (raft_b200.temporal.cutoff_wavelength gives the detail scale that keeps P's
+        gradients); cuts scene-cut pairs where the output restarts from P.  Returns fresh (frames [F,Hs,Ws,3] uint8,
+        status [F,Hs,Ws] uint8) CUDA tensors (RaftEngine.consistent)."""
+        return self.engine().consistent(_as_tensor(frames), _as_tensor(processed), strength, cuts=cuts)
+
+    @torch.no_grad()
+    def warp_error(self, frames, video, cuts=None):
+        """Extension (temporal consistency): Lai et al.'s warping error of video, [F,Hs,Ws,3] uint8 frames aligned with
+        frames, under the frames' own flow: (E_warp, E_pair [F-1] float64, NaN for cut pairs and pairs with no
+        consistent pixel) (RaftEngine.warp_error)."""
+        return self.engine().warp_error(_as_tensor(frames), _as_tensor(video), cuts=cuts)
+
+    @torch.no_grad()
     def interpolate_sequence(self, frames, t=0.5, uint8=False, bgr=False, native=False):
         """Extension (frame-rate up-conversion): the frames at time t (a float, or a sequence of times, each in [0, 1])
         between every pair of consecutive frames of [T+1,H,W,3] frames, from one ``forward_sequence_bidirectional`` pass.

@@ -868,3 +868,101 @@ def warp_frames_fill(frames, ext_fw, ext_bw, net_hw, margin, A, rows, flow_scale
                                                        capi.ptr(table), n, capi.ptr(colour), capi.ptr(status),
                                                        capi.stream()))
     return colour, status
+
+
+def _frame_u8(what, name, x, shape=None, dev=None):
+    if not (isinstance(x, torch.Tensor) and x.is_cuda and x.dim() == 3 and x.shape[-1] == 3 and x.dtype == torch.uint8
+            and (shape is None or tuple(x.shape) == tuple(shape)) and (dev is None or x.device == dev)):
+        raise ValueError(f"{what}: {name} must be an [Hs,Ws,3] uint8 CUDA tensor"
+                         + ("" if shape is None else f" of shape {list(shape)} on {dev}") + f" (got "
+                         f"{getattr(x, 'shape', None)} {getattr(x, 'dtype', type(x))})")
+    return x.contiguous()
+
+
+def tcons_terms(frame, prev_frame, processed, prev_out, flow_fw, flow_bw, strength, flow_scale=1.0, alpha1=0.01,
+                alpha2=0.5):
+    """Extension (temporal consistency): frame t's temporal term (rb_tcons_terms).  frame, prev_frame (the originals
+    I_t, I_(t-1)), processed (P_t) and prev_out (O_(t-1)): [Hs,Ws,3] uint8 CUDA tensors; flow_fw, flow_bw [Hn,Wn,2]
+    float32 the pair (t-1, t); strength > 0.  Each pixel takes one backward step through the flows with the
+    forward-backward test of fb_consistency, and the originals' colour difference at its target weighs the pull toward
+    the previous output (Tukey's biweight, cut-off raft_b200.temporal.KAPPA).  prev_frame None: no previous frame
+    (prev_out and the flows are ignored).  Returns fresh (c [Hs,Ws] float32, r [Hs,Ws,3] float32, status [Hs,Ws]
+    uint8: 0 used, 1 step failed, 2 rejected by the colour check, 3 no previous frame).  Bad arguments raise
+    ValueError."""
+    from raft_b200.temporal import check_strength
+    P = _frame_u8("tcons_terms", "processed", processed)
+    dev, (Hs, Ws) = P.device, P.shape[:2]
+    strength = check_strength(strength, "tcons_terms")
+    c = torch.empty(Hs, Ws, dtype=torch.float32, device=dev)
+    r = torch.empty(Hs, Ws, 3, dtype=torch.float32, device=dev)
+    status = torch.empty(Hs, Ws, dtype=torch.uint8, device=dev)
+    if prev_frame is None:
+        ptrs, Hn, Wn = (None, None, P, None, None, None), 1, 1
+    else:
+        I = _frame_u8("tcons_terms", "frame", frame, P.shape, dev)
+        Ip = _frame_u8("tcons_terms", "prev_frame", prev_frame, P.shape, dev)
+        Op = _frame_u8("tcons_terms", "prev_out", prev_out, P.shape, dev)
+        if not all(isinstance(f, torch.Tensor) and f.dim() == 3 for f in (flow_fw, flow_bw)):
+            raise ValueError("tcons_terms: flow_fw and flow_bw must be [Hn,Wn,2] float32 CUDA tensors")
+        _, Hn, Wn = _flow_pair("tcons_terms", flow_fw[None], flow_bw[None])
+        if flow_fw.device != dev:
+            raise ValueError(f"tcons_terms: the flows must be on {dev}")
+        ptrs = (I, Ip, P, Op, flow_fw.contiguous(), flow_bw.contiguous())
+    with torch.cuda.device(dev):
+        capi.check(capi.lib.rb_tcons_terms(*(None if t is None else capi.ptr(t) for t in ptrs[:4]), Hs, Ws,
+                                           *(None if t is None else capi.ptr(t) for t in ptrs[4:]), Hn, Wn,
+                                           float(flow_scale), float(alpha1), float(alpha2), strength, capi.ptr(c),
+                                           capi.ptr(r), capi.ptr(status), capi.stream()))
+    return c, r, status
+
+
+def screened_poisson(c, r, workspace=None):
+    """Extension (temporal consistency): the correction D [H,W,3] float32 that solves (c_p + n_p) D_p - sum of the
+    in-image 4-neighbours' D = r_p per channel (rb_screened_poisson: flexible conjugate gradients preconditioned by a
+    multigrid V-cycle of red-black Gauss-Seidel, include/raft_b200.h F30).  c [H,W] float32 > 0 and r [H,W,3] float32
+    CUDA tensors; workspace an optional uint8 CUDA buffer of at least rb_screened_poisson_workspace_bytes.  r = 0 gives
+    D = 0 bit for bit.  Bad shapes or dtypes raise ValueError."""
+    if not (isinstance(c, torch.Tensor) and c.is_cuda and c.dim() == 2 and c.dtype == torch.float32):
+        raise ValueError(f"screened_poisson: c must be an [H,W] float32 CUDA tensor (got {getattr(c, 'shape', None)} "
+                         f"{getattr(c, 'dtype', type(c))})")
+    H, W = c.shape
+    if not (isinstance(r, torch.Tensor) and tuple(r.shape) == (H, W, 3) and r.dtype == torch.float32
+            and r.device == c.device):
+        raise ValueError(f"screened_poisson: r must be an [H,W,3] = {[H, W, 3]} float32 tensor on {c.device}")
+    dev = c.device
+    cc, rr = c.contiguous(), r.contiguous()
+    D = torch.empty(H, W, 3, dtype=torch.float32, device=dev)
+    with torch.cuda.device(dev):
+        nbytes = capi.size_query(capi.lib.rb_screened_poisson_workspace_bytes, H, W)
+        if workspace is None or workspace.numel() < nbytes or workspace.device != dev:
+            workspace = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+        capi.check(capi.lib.rb_screened_poisson(capi.ptr(cc), capi.ptr(rr), H, W, capi.ptr(D), capi.ptr(workspace),
+                                                workspace.numel(), capi.stream()))
+    return D
+
+
+def warp_error(video, flow_fw, flow_bw, flow_scale=1.0, alpha1=0.01, alpha2=0.5):
+    """Extension (temporal consistency): Lai et al.'s warping-error sums (rb_warp_error) of [F,Hs,Ws,3] uint8 CUDA
+    frames V aligned with the frames that flow_fw, flow_bw [F-1,Hn,Wn,2] float32 were computed on: per pair k, the sum
+    over the pixels of frame k whose forward step passes the forward-backward test of sum_c (V_k(p) - V_(k+1)(o))^2 in
+    grey levels, and their count.  Returns a fresh [F-1,2] float64 CUDA tensor (raft_b200.temporal.pair_errors forms
+    E_warp).  Bad shapes raise ValueError."""
+    if not (isinstance(video, torch.Tensor) and video.is_cuda and video.dim() == 4 and video.shape[-1] == 3
+            and video.dtype == torch.uint8 and video.shape[0] >= 2):
+        raise ValueError(f"warp_error: video must be an [F,Hs,Ws,3] uint8 CUDA tensor with F >= 2 (got "
+                         f"{getattr(video, 'shape', None)} {getattr(video, 'dtype', type(video))})")
+    F, Hs, Ws, _ = video.shape
+    dev = video.device
+    T, Hn, Wn = _flow_pair("warp_error", flow_fw, flow_bw)
+    if T != F - 1 or flow_fw.device != dev:
+        raise ValueError(f"warp_error: {F} frames need [F-1,Hn,Wn,2] = [{F - 1},Hn,Wn,2] flows on {dev} (got "
+                         f"{tuple(flow_fw.shape)})")
+    v, fw, bw = video.contiguous(), flow_fw.contiguous(), flow_bw.contiguous()
+    sums = torch.empty(F - 1, 2, dtype=torch.float64, device=dev)
+    with torch.cuda.device(dev):
+        nbytes = capi.size_query(capi.lib.rb_warp_error_workspace_bytes, F, Hs, Ws)
+        ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+        capi.check(capi.lib.rb_warp_error(capi.ptr(v), F, Hs, Ws, capi.ptr(fw), capi.ptr(bw), Hn, Wn, float(flow_scale),
+                                          float(alpha1), float(alpha2), capi.ptr(sums), capi.ptr(ws), nbytes,
+                                          capi.stream()))
+    return sums

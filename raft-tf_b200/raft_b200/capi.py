@@ -89,6 +89,11 @@ SIGNATURES = {
                                         _vp]),
     "rb_denoise_merge": (_i, [_vp, _i, _i, _i, _vp, _vp, _i, _i, _f, _f, _f, _vp, _i, _f, _vp, _vp, _vp]),
     "rb_noise_sums": (_i, [_vp, _i, _i, _i, _vp, _vp]),
+    "rb_tcons_terms": (_i, [_vp, _vp, _vp, _vp, _i, _i, _vp, _vp, _i, _i, _f, _f, _f, _f, _vp, _vp, _vp, _vp]),
+    "rb_screened_poisson_workspace_bytes": (_i, [_i, _i, _psz]),
+    "rb_screened_poisson": (_i, [_vp, _vp, _i, _i, _vp, _vp, _sz, _vp]),
+    "rb_warp_error_workspace_bytes": (_i, [_i, _i, _i, _psz]),
+    "rb_warp_error": (_i, [_vp, _i, _i, _i, _vp, _vp, _i, _i, _f, _f, _f, _vp, _vp, _sz, _vp]),
     "rb_flow_reverse_workspace_bytes": (_i, [_i, _i, _i, _psz]),
     "rb_flow_reverse": (_i, [_vp, _vp, _vp, _i, _i, _f, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _vp, _sz, _vp]),
     "rb_frame_synthesize": (_i, [_vp, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _f, _vp, _i, _i, _i, _vp]),

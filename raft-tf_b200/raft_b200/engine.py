@@ -715,6 +715,62 @@ class RaftEngine:
         with torch.cuda.device(self.device):
             return merge_frames(on_dev, flow_fw, flow_bw, rows, sigma, self.flow_scale)
 
+    def _consistent_args(self, frames, other, name, cuts, what):
+        F = _sequence_length(frames) + 1
+        if frames.dtype != torch.uint8:
+            raise ValueError(f"raft_b200: {what} compares bytes: the frames must be uint8 (got {frames.dtype})")
+        o = torch.as_tensor(other)
+        if not (o.dtype == torch.uint8 and tuple(o.shape) == tuple(frames.shape)):
+            raise ValueError(f"raft_b200: the {name} must be [F,Hs,Ws,3] = {list(frames.shape)} uint8 frames aligned "
+                             f"with the frames (got {list(o.shape)} {o.dtype})")
+        from .video import check_cuts
+        return F, o, check_cuts(() if cuts is None else cuts, F, "raft_b200")
+
+    @torch.no_grad()
+    def consistent(self, frames: torch.Tensor, processed, strength, cuts=None):
+        """Blind video temporal consistency (Bonneel et al., SIGGRAPH Asia 2015) of processed, [F,Hs,Ws,3] uint8 frames
+        made from the [F,Hs,Ws,3] uint8 frames one at a time (sizes and input_size as for forward()).  One
+        forward_sequence_bidirectional(check=False) pass on the originals, then the frames in order on the stream, with
+        no host synchronisation per frame: frame 0 and the first frame after each scene-cut pair of cuts are P byte for
+        byte; every other frame is raft_b200.temporal.consistent_frame (rb_tcons_terms, rb_screened_poisson, the
+        rounding) against the previous output.  strength (lambda > 0) trades the pull toward the previous output
+        against P's gradients.  Returns fresh (frames [F,Hs,Ws,3] uint8, status [F,Hs,Ws] uint8: 0 the temporal term
+        is used, 1 the step failed, 2 the colour check rejected it, 3 no previous frame) CUDA tensors.  Non-uint8
+        frames, processed frames of another shape, a bad strength or cuts raise ValueError before the pass."""
+        from .temporal import check_strength, consistent_frame
+        F, P, cuts = self._consistent_args(frames, processed, "processed frames", cuts, "consistent")
+        strength = check_strength(strength, "raft_b200")
+        flow_fw, flow_bw, _, _ = self.forward_sequence_bidirectional(frames, check=False)
+        with torch.cuda.device(self.device):
+            I, P = frames.to(self.device), P.to(self.device)
+            out, status = torch.empty_like(P), torch.empty(P.shape[:3], dtype=torch.uint8, device=self.device)
+            Hs, Ws = P.shape[1:3]
+            ws = torch.empty(capi.size_query(capi.lib.rb_screened_poisson_workspace_bytes, Hs, Ws), dtype=torch.uint8,
+                             device=self.device)  # one solver workspace for every frame
+            for t in range(F):
+                first = t == 0 or (t - 1) in cuts
+                k = max(t - 1, 0)
+                out[t], status[t] = consistent_frame(I[t], None if first else I[t - 1], P[t], out[k], flow_fw[k],
+                                                     flow_bw[k], strength, self.flow_scale, ws)
+            return out, status
+
+    @torch.no_grad()
+    def warp_error(self, frames: torch.Tensor, video, cuts=None):
+        """Lai et al.'s (ECCV 2018) warping error of video, [F,Hs,Ws,3] uint8 frames aligned with the [F,Hs,Ws,3] uint8
+        frames (sizes and input_size as for forward()), under the frames' own flow: one
+        forward_sequence_bidirectional(check=False) pass and one rb_warp_error launch pair.  Returns (E_warp, E_pair):
+        E_pair [F-1] float64 per pair (NaN for a scene-cut pair of cuts and a pair with no consistent pixel), E_warp
+        their mean over the other pairs (raft_b200.temporal.pair_errors), in [0, 1].  Bad arguments raise ValueError
+        before the pass."""
+        from networks.utils import warp_error
+        from .temporal import pair_errors
+        F, V, cuts = self._consistent_args(frames, video, "video", cuts, "warp_error")
+        flow_fw, flow_bw, _, _ = self.forward_sequence_bidirectional(frames, check=False)
+        with torch.cuda.device(self.device):
+            sums = warp_error(V.to(self.device), flow_fw, flow_bw, self.flow_scale, FB_ALPHA1, FB_ALPHA2)
+        e_warp, e_pair, _ = pair_errors(sums.cpu().numpy(), cuts)
+        return e_warp, e_pair
+
     @torch.no_grad()
     def interpolate(self, left: torch.Tensor, right: torch.Tensor, ts, native: bool = False) -> torch.Tensor:
         """Frames at times ts (each in [0, 1]; 0 = left, 1 = right) between B frame pairs: one bidirectional pass (as

@@ -259,10 +259,14 @@ class _Pipeline:
     used in turn (allocated on first use with `rows` rows, default the output's own) and records one event behind them
     and the pass's work; write(slot) then runs on a writer thread (workers = 0: inline) and calls slot.event.synchronize()
     before it reads the slot (slot None: the pass had no outputs).  A slot is refilled only once its event has completed
-    and its writers have returned, so a writer's exception reaches the caller there or when the pipeline exits."""
+    and its writers have returned, so a writer's exception reaches the caller there or when the pipeline exits.
 
-    def __init__(self, paths, passes, rgb, batch, workers, device):
+    extra (a list of paths aligned with paths, each of paths[0]'s size) is decoded alongside by the same threads into a
+    second pinned buffer of each input slot; pipe.extra holds the current pass's rows of it."""
+
+    def __init__(self, paths, passes, rgb, batch, workers, device, extra=None):
         self.paths, self.passes, self.rgb, self.T, self.workers, self.device = paths, passes, rgb, batch, workers, device
+        self.extra_paths, self.extra = extra, None
         self.depth = max(1, -(-workers // batch))  # passes decoded ahead of the one the GPU is given
         self.ins = self.outs = None
         self.loose = []  # the writes of passes without outputs
@@ -288,10 +292,15 @@ class _Pipeline:
                 if pool is not None:
                     pool.shutdown(wait=True, cancel_futures=True)
 
-    def _submit(self, j):
+    def _load(self, paths, i):
+        if paths is None:
+            return None
         if self.decoders is None:
-            return [(i, lambda i=i: _imread(self.paths[i], self.rgb)) for i in self.passes[j].frames]
-        return [(i, self.decoders.submit(_imread, self.paths[i], self.rgb).result) for i in self.passes[j].frames]
+            return lambda: _imread(paths[i], self.rgb)
+        return self.decoders.submit(_imread, paths[i], self.rgb).result
+
+    def _submit(self, j):
+        return [(i, self._load(self.paths, i), self._load(self.extra_paths, i)) for i in self.passes[j].frames]
 
     def __iter__(self):
         paths, depth, shape = self.paths, self.depth, None
@@ -300,8 +309,8 @@ class _Pipeline:
             loads = ahead.pop(0)
             if j + depth < len(self.passes):
                 ahead.append(self._submit(j + depth))
-            imgs = []
-            for i, load in loads:
+            imgs, extra = [], []
+            for i, load, xload in loads:
                 img = load()
                 if shape is None:
                     shape = img.shape
@@ -309,13 +318,25 @@ class _Pipeline:
                     raise ValueError(f"video: {paths[i]} is a {img.shape[0]}x{img.shape[1]} frame, {paths[0]} is "
                                      f"{shape[0]}x{shape[1]}: every frame needs one size")
                 imgs.append(img)
+                if xload is not None:
+                    x = xload()
+                    if x.shape != shape:
+                        raise ValueError(f"video: {self.extra_paths[i]} is a {x.shape[0]}x{x.shape[1]} frame, "
+                                         f"{paths[0]} is {shape[0]}x{shape[1]}: the frames must be aligned")
+                    extra.append(x)
             if self.ins is None:
-                self.ins = [_Slot(frames=((self.T + 1,) + shape, torch.uint8)) for _ in range(2)]
+                rows = ((self.T + 1,) + shape, torch.uint8)
+                self.ins = [_Slot(frames=rows, **({} if self.extra_paths is None else {"extra": rows}))
+                            for _ in range(2)]
             self.j, self.slot = j, self.ins[j % 2]
             self.slot.wait()
             frames = self.slot.frames[:len(imgs)]
             for r, img in enumerate(imgs):
                 frames[r].numpy()[...] = img
+            if self.extra_paths is not None:
+                self.extra = self.slot.extra[:len(extra)]
+                for r, x in enumerate(extra):
+                    self.extra[r].numpy()[...] = x
             yield j, ps, imgs, frames
 
     def emit(self, write, rows=None, **outputs):
@@ -1423,3 +1444,136 @@ def video_denoise(model, frames, out, sigma, window=None, batch=8, workers=4, sc
     print(f"denoise: sigma {sigma:.4g}, mean support {mean:.3f} frames")
     print(f"scene cuts: {len(cuts)}" + (" at pairs " + " ".join(str(k) for k in cuts) if cuts else ""))
     return names, {"sigma": float(sigma), "support": mean, "cuts": cuts}
+
+
+def _aligned(frames, other, what):
+    """The frame paths of frames and of other, which must hold as many frames; anything else raises ValueError."""
+    paths, opaths = list_frames(frames), list_frames(other)
+    if len(opaths) != len(paths):
+        raise ValueError(f"{what}: {len(opaths)} frames in {other!r} for {len(paths)} original frames: the frames must "
+                         f"be aligned with the originals")
+    if len(paths) < 2:
+        raise ValueError(f"{what}: a sequence needs two frames at least (got {len(paths)})")
+    return paths, opaths
+
+
+def _temporal_sweep(model, frames, other, what, batch, workers, scene_cut, strength=None, out=None):
+    """The one sweep behind video_consistent (strength given) and video_warp_error: per pass the originals and the other
+    frames, one forward_sequence_bidirectional(check=False), and each frame whose pair ran in order; the per-pair
+    warping-error sums of the originals, of other and (with strength) of the output stay on the GPU until the end."""
+    import cv2
+    from networks.utils import scene_cut_scores, warp_error
+    from .engine import FB_ALPHA1, FB_ALPHA2
+    from .temporal import check_strength, consistent_frame
+
+    paths, opaths = _aligned(frames, other, what)
+    F = len(paths)
+    if strength is not None:
+        strength = check_strength(strength, what)
+    thr = None if scene_cut is None else check_scene_cut(scene_cut)
+    batch, workers = int(batch), _workers(workers)
+    passes = interp_schedule(F, batch)
+    names = None
+    if out is not None:
+        out = os.fspath(out)
+        os.makedirs(out, exist_ok=True)
+        names = [os.path.join(out, f"frame_{i:06d}.png") for i in range(F)]
+    engine = model.engine()
+    rgb = bool(model.upstream)
+    dev = engine.device
+    cuts = []
+    I_dev = P_dev = None
+    prev_out = None  # O of the frame before the pass's next frame
+    sums = counts = None
+
+    def write(slot, first, n):  # writer thread: the output frames of one pass, once its copies have landed
+        if slot is None:
+            return
+        slot.event.synchronize()
+        for r in range(n):
+            img = slot.frames[r].numpy()
+            if not cv2.imwrite(names[first + r], cv2.cvtColor(img, cv2.COLOR_RGB2BGR) if rgb else img):
+                raise OSError(f"cannot write {names[first + r]}")
+
+    with _Pipeline(paths, passes, rgb, batch, workers, dev, extra=opaths) as pipe:
+        for j, ps, imgs, src in pipe:
+            if I_dev is None:
+                I_dev = torch.empty(src.shape, dtype=torch.uint8, device=dev)
+                P_dev = torch.empty(src.shape, dtype=torch.uint8, device=dev)
+                sums = torch.zeros(3, F - 1, 2, dtype=torch.float64, device=dev)
+                counts = torch.zeros(4, dtype=torch.int64, device=dev)
+            I_dev.copy_(src, non_blocking=True)
+            P_dev.copy_(pipe.extra, non_blocking=True)
+            n = sum(k is not None for k in ps.pairs)
+            first = ps.frames[0]
+            if thr is not None:
+                cuts += pass_cuts(ps.pairs, scene_cut_scores(I_dev).cpu(), thr)
+            fw, bw, _, _ = engine.forward_sequence_bidirectional(I_dev, check=False)
+            fw, bw = fw[:n], bw[:n]
+            sums[0, first:first + n] = warp_error(I_dev[:n + 1], fw, bw, engine.flow_scale, FB_ALPHA1, FB_ALPHA2)
+            sums[1, first:first + n] = warp_error(P_dev[:n + 1], fw, bw, engine.flow_scale, FB_ALPHA1, FB_ALPHA2)
+            res = None
+            if strength is not None:
+                rows = list(range(0 if first == 0 else 1, n + 1))  # the pass's frames whose pair has run
+                O = torch.empty((n + 1,) + tuple(src.shape[1:]), dtype=torch.uint8, device=dev)
+                if first > 0:
+                    O[0] = prev_out
+                for r in rows:
+                    t = first + r
+                    restart = t == 0 or (t - 1) in cuts
+                    O[r], st = consistent_frame(I_dev[r], None if restart else I_dev[r - 1], P_dev[r], O[max(r - 1, 0)],
+                                                fw[max(r - 1, 0)], bw[max(r - 1, 0)], strength, engine.flow_scale)
+                    counts += torch.bincount(st.reshape(-1), minlength=4)
+                sums[2, first:first + n] = warp_error(O, fw, bw, engine.flow_scale, FB_ALPHA1, FB_ALPHA2)
+                prev_out = O[n].clone()
+                res = O[rows[0]:]
+            pipe.emit(partial(write, first=first + (0 if first == 0 else 1), n=0 if res is None else len(res)),
+                      frames=res)
+    from .temporal import pair_errors
+    cuts = sorted(cuts)
+    s = sums.cpu().numpy()
+    info = {"cuts": cuts}
+    for k, name in enumerate(("original", "input", "output")[:3 if strength is not None else 2]):
+        e, per, excluded = pair_errors(s[k], cuts)
+        info[name] = {"E_warp": e, "E_pair": per.tolist(), "excluded": excluded}
+    if strength is not None:
+        info["status"] = counts.cpu().tolist()
+    return names, info
+
+
+def video_consistent(model, frames, processed, out, strength, batch=8, workers=4, scene_cut=None):
+    """Temporal consistency of a processed clip of any length with a loaded networks.RAFT.RAFT model, in one sweep:
+    processed (a directory's sorted *.png / *.jpg, or a list of paths) holds per-frame processed versions of frames,
+    as many and of the same size.  Every output frame is written as <out>/frame_<i:06d>.png, equal byte for byte to
+    RAFT.consistent on the whole clip (with the cuts found here) for every batch and workers value.
+
+    Passes come from interp_schedule(): the pass's originals and processed frames, both decoded by the pipeline's
+    workers, and one forward_sequence_bidirectional(check=False).  Frames are corrected in order
+    (raft_b200.temporal.consistent_frame); only the pass's frames and the output of the frame before it stay on the GPU.
+    scene_cut (a threshold in [0, 1]) scores each pass's originals on the GPU; the frame after a cut pair restarts from
+    P.  Prints E_warp of the originals, of the processed frames and of the output, all from the sweep's flows, the
+    status counts and the cuts.  Frames go in RGB with model.upstream and BGR otherwise, like the CLI; the files are BGR.
+    Returns (paths, info), info a dict of "cuts", "status" (counts of statuses 0-3) and per video ("original", "input",
+    "output") its "E_warp", "E_pair" (NaN: excluded) and "excluded" pairs."""
+    names, info = _temporal_sweep(model, frames, processed, "video_consistent", batch, workers, scene_cut,
+                                  strength=strength, out=out)
+    print("consistent: E_warp original {:.6g}, processed {:.6g}, output {:.6g}".format(
+        info["original"]["E_warp"], info["input"]["E_warp"], info["output"]["E_warp"]))
+    print("status: used {} / step failed {} / rejected {} / no previous frame {}".format(*info["status"]))
+    print(f"scene cuts: {len(info['cuts'])}" + (" at pairs " + " ".join(str(k) for k in info["cuts"])
+                                                if info["cuts"] else ""))
+    return names, info
+
+
+def video_warp_error(model, frames, video, batch=8, workers=4, scene_cut=None):
+    """Lai et al.'s warping error of video (a directory or list of frames aligned with frames: as many, the same size)
+    under the flow of frames, in one sweep like video_consistent's without the solve: the same values as
+    RAFT.warp_error on the whole clip (with the cuts found here).  Prints E_warp of video and of the originals and the
+    cuts.  Returns info: "cuts" and per video ("original", "input") its "E_warp", "E_pair" and "excluded" pairs."""
+    _, info = _temporal_sweep(model, frames, video, "video_warp_error", batch, workers, scene_cut)
+    print("warp error: E_warp {:.6g} (original frames {:.6g}) over {} pairs, {} excluded".format(
+        info["input"]["E_warp"], info["original"]["E_warp"], len(info["input"]["E_pair"]),
+        len(info["input"]["excluded"])))
+    print(f"scene cuts: {len(info['cuts'])}" + (" at pairs " + " ".join(str(k) for k in info["cuts"])
+                                                if info["cuts"] else ""))
+    return info
