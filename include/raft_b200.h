@@ -115,6 +115,16 @@ int rb_debug_conv_last(int* block_n, int* bw_log2, int* grid, int* stages, int* 
 /* wgmma per product of that conv: 3 (split operands) or 1 (the single-pass kernel of RB_MATH_TC_FP16); RB_ERR_BAD_ARG if
  * no conv has been launched on this thread. */
 int rb_debug_conv_last_passes(void);
+/* Test hook: the halo A operand of the tensor-core conv (one activation box of (box rows + kh - 1) rows per channel chunk
+ * and kx, feeding all kh vertical taps).  mode -1: no conv uses it; 0 (default): the update-block convs that request it;
+ * 1: every stride-1 conv with kh > 1 (rb_conv2d included).  Results are the same bits either way.  Anything else ->
+ * RB_ERR_BAD_ARG. */
+int rb_debug_conv_halo(int mode);
+/* Launch log of the tensor-core convs on this thread since the last rb_debug_conv_override() call (the first 64):
+ * rec[10] of launch i = {block_n, bw_log2, grid, stages (B ring depth with the halo), total_tiles, halo box rows (0: one A
+ * box per tap), kh, kw, 64-channel chunks multiplied per tile, wgmma per product}.  Returns the number of launches logged,
+ * or RB_ERR_BAD_ARG if i is not one of them. */
+int rb_debug_conv_log(int i, int* rec);
 
 /* ---- A4: coords_grid(batch, ht, wd)  networks/utils.py:4-11 ----------------------------------
  * coords[b,y,x,0] = x, coords[b,y,x,1] = y. */

@@ -215,6 +215,10 @@ struct ConvParams {
   // tensor-core back end: 1 = single pass, fp16(a) * fp16(b) from the hi planes only (RB_MATH_TC_FP16; set by launch_conv,
   // never by the correlation build).  Read on the host only; last, so the kernels' view of the fields above is unchanged.
   int single_pass;
+  // tensor-core back end, kh > 1 stride-1 convs: 1 = load one activation halo of (box rows + kh - 1) rows per (channel
+  // chunk, kx) and feed all kh vertical taps from it (conv_tc.cu).  Same MMA operands in the same order, so the same bits;
+  // set by update.cu for the 3x3 and 5x1 convs of the update block.  Read on the host only.
+  int halo;
 };
 __host__ __device__ inline int conv_sx(const ConvParams& p) { return p.sx > 0 ? p.sx : 1; }
 __host__ __device__ inline int conv_sy(const ConvParams& p) { return p.sy > 0 ? p.sy : 1; }

@@ -35,6 +35,30 @@ constexpr int kSlabCols = 32;              // epilogue staging: 64 rows x 32 fp3
 constexpr int kSlabPitch = kSlabCols + 4;  // floats per staged row: 16-byte aligned rows, rows spread over the banks
 constexpr int kStagingBytes = 2 * 64 * kSlabPitch * 4;
 constexpr int kMaxSmem = 227 * 1024;       // opt-in shared memory per block on sm_90
+// operand rings: everything but the alignment slack, the epilogue staging, the barriers and the split-K partials
+constexpr int kRingBytes = kMaxSmem - 1024 /*align slack*/ - kStagingBytes - 256 /*barriers*/ - 1024 /*split-K partials*/;
+constexpr int kSmemOverhead = 1024 + kStagingBytes + 256 + 1024;
+
+// Halo A operand (ConvParams::halo, kh > 1): the A ring holds kHaloSlots slots of one (BH + kh - 1) x BW box (hi | lo)
+// per (channel chunk, kx); the B ring holds one weight tile (hi | lo) per (chunk, kx, ky), as before.  Tap ky of the box is
+// the rows [ky BW, ky BW + 128): a ky BW x 128-byte offset, a whole number of 1024-byte SW128 atoms for BW >= 8, so the
+// wgmma descriptor is the canonical one at that address.  Two slots let the producer load the next group's halo while
+// the consumers work through the current one (with one, the producer would wait for a release that needs its own load).
+constexpr int kHaloSlots = 2;
+// B ring depth next to the A ring: 0 when the two slots do not leave room for two B stages (the conv then keeps one
+// A box per tap)
+constexpr int halo_b_stages(int block_n, int planes, int halo_rows) {
+  return (kRingBytes - kHaloSlots * planes * halo_rows * 128) / (planes * block_n * 128) < 2 ? 0
+         : (kRingBytes - kHaloSlots * planes * halo_rows * 128) / (planes * block_n * 128) > 6
+             ? 6
+             : (kRingBytes - kHaloSlots * planes * halo_rows * 128) / (planes * block_n * 128);
+}
+// the geometries choose_geom picks for the update block at 55 x 128 (3x3 and 5x1 on 8 x 16 boxes), the 2 x 64 / 4 x 32
+// boxes, and the widest tile
+static_assert(halo_b_stages(128, 2, 10 * 16) == 3 && halo_b_stages(128, 2, 12 * 16) == 3, "3x3 / 5x1 halo at N = 128");
+static_assert(halo_b_stages(96, 2, 10 * 16) == 5 && halo_b_stages(96, 2, 12 * 16) == 4, "3x3 / 5x1 halo at N = 96");
+static_assert(halo_b_stages(128, 2, 4 * 64) == 2 && halo_b_stages(128, 2, 8 * 32) == 2, "2x64 3x3 / 4x32 5x1 halo at N = 128");
+static_assert(halo_b_stages(128, 2, 3 * 128) == 0, "a 1x128 3x3 halo does not fit beside two N = 128 stages");
 
 // PERSISTENT kernel: each CTA walks tiles t = blockIdx.x, blockIdx.x + gridDim.x, ... (n-tile fastest, so CTAs that
 // run side by side share the same activation tile in L2).  The smem ring and its mbarrier phases simply continue across
@@ -45,9 +69,8 @@ struct TcCfg {
   static constexpr int kPlanes = SINGLE ? 1 : 2;          // hi (| lo) per operand
   static constexpr int kBOff = kPlanes * kATileBytes;      // B_hi inside a stage: A_hi | A_lo | B_hi | B_lo, or A_hi | B_hi
   static constexpr int kStageBytes = kPlanes * (kATileBytes + kBTileBytes);
-  static constexpr int kRingBytes = kMaxSmem - 1024 /*align slack*/ - kStagingBytes - 256 /*barriers*/ - 1024 /*split-K partials*/;
   static constexpr int kStages = kRingBytes / kStageBytes > 6 ? 6 : kRingBytes / kStageBytes;
-  static constexpr int kSmemBytes = kStages * kStageBytes + 1024 + kStagingBytes + 256 + 1024;
+  static constexpr int kSmemBytes = kStages * kStageBytes + kSmemOverhead;
   static constexpr int kSlab = BLOCK_N < kSlabCols ? BLOCK_N : kSlabCols;  // columns staged at a time
   static constexpr int kAcc = BLOCK_N / 2;  // fp32 accumulator registers per thread and accumulator
 };
@@ -57,7 +80,9 @@ __device__ __forceinline__ void consumer_bar_sync(int id) { asm volatile("bar.sy
 // EXTRAS: phase timestamps (p.dbg) and fused instance-norm statistics (p.stat_part) -- a separate instantiation, so that
 // the kernel the update block runs carries none of their registers.
 // SINGLE: the single-pass variant (tmA_lo / tmB_lo are not read).
-template <int BLOCK_N, bool EXTRAS, bool SINGLE>
+// HALO: the halo A operand (g.halo_rows > 0) -- a separate instantiation, so that the one-box-per-tap kernel of every
+// other conv carries none of its ring bookkeeping.
+template <int BLOCK_N, bool EXTRAS, bool SINGLE, bool HALO>
 __global__ void __launch_bounds__(kTcThreads, 1)
 conv_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant__ CUtensorMap tmA_lo,
                const __grid_constant__ CUtensorMap tmB_hi, const __grid_constant__ CUtensorMap tmB_lo,
@@ -65,11 +90,21 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
   using Cfg = TcCfg<BLOCK_N, SINGLE>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  float* staging = reinterpret_cast<float*>(smem + STAGES * Cfg::kStageBytes);
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + STAGES * Cfg::kStageBytes + kStagingBytes);
+  // STAGES: depth of the B ring (one A | B stage per k-iteration without the halo).  Layout: [A slots] B ring | staging |
+  // barriers | split-K partials.
+  constexpr bool halo = HALO;
+  const int a_plane = halo ? g.halo_rows * 128 : kATileBytes;  // A_lo behind A_hi
+  const int a_slot_bytes = Cfg::kPlanes * a_plane;
+  const int b_stage_bytes = halo ? Cfg::kPlanes * Cfg::kBTileBytes : Cfg::kStageBytes;
+  const int b_off = halo ? 0 : Cfg::kBOff;  // B_hi inside a stage
+  uint8_t* bring = smem + (halo ? kHaloSlots * a_slot_bytes : 0);
+  float* staging = reinterpret_cast<float*>(smem + g.ring_bytes);
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + g.ring_bytes + kStagingBytes);
   uint64_t* empty_bar = full_bar + STAGES;
-  uint64_t* red_bar = empty_bar + STAGES;  // split-K: the peer's partial sums have arrived (128 pixel arrivals)
-  float2* red_buf = reinterpret_cast<float2*>(smem + STAGES * Cfg::kStageBytes + kStagingBytes + 256);  // [128 pixels] ch 0, 1
+  uint64_t* a_full = empty_bar + STAGES;   // halo: A slot loaded / released by both consumer warpgroups
+  uint64_t* a_empty = a_full + kHaloSlots;
+  uint64_t* red_bar = a_empty + kHaloSlots;  // split-K: the peer's partial sums have arrived (128 pixel arrivals)
+  float2* red_buf = reinterpret_cast<float2*>(smem + g.ring_bytes + kStagingBytes + 256);  // [128 pixels] ch 0, 1
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   long long* dbg = (EXTRAS && p.dbg) ? p.dbg + (size_t)blockIdx.x * 8 : nullptr;
@@ -95,6 +130,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
       prefetch_tmap(&tmA_hi); prefetch_tmap(&tmA_lo); prefetch_tmap(&tmB_hi); prefetch_tmap(&tmB_lo);
     }
     for (int s = 0; s < STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 2); }  // one arrival per consumer warpgroup
+    for (int s = 0; s < kHaloSlots; ++s) { mbar_init(&a_full[s], 1); mbar_init(&a_empty[s], 2); }
     mbar_init(red_bar, 128);
     fence_barrier_init();
     fence_proxy_async();
@@ -115,6 +151,8 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
       const int ph = conv_pad_y(p), pw = conv_pad_x(p), csx = conv_sx(p), csy = conv_sy(p);
       int s = 0;          // ring slot and its phase; both continue across tiles.  No integer division in this loop:
       uint32_t phase = 0;  // the k-iteration -> (chunk, kx, ky) mapping is advanced incrementally.
+      int as = 0;            // halo: A slot and its phase, likewise
+      uint32_t a_phase = 0;
       bool waited = false;
       for (int tile = first; tile < g.total_tiles; tile += stride) {
         const int mt = tile / g.n_tiles, nt = tile - mt * g.n_tiles;
@@ -141,10 +179,17 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
           if constexpr (!SINGLE) tma_load_4d(&tmA_lo, &full_bar[slot], st + kATileBytes, c0, xs + k.kx, ys + k.ky, b);
         };
         auto load_b = [&](const KIter& k, int slot) {
-          uint8_t* st = smem + slot * Cfg::kStageBytes;
+          uint8_t* st = bring + slot * b_stage_bytes + b_off;
           const int kcol = (k.ky * p.kw + k.kx) * p.cin_pad + k.ck * kChunkK;
-          tma_load_3d(&tmB_hi, &full_bar[slot], st + Cfg::kBOff, kcol, n0, wb);
-          if constexpr (!SINGLE) tma_load_3d(&tmB_lo, &full_bar[slot], st + Cfg::kBOff + Cfg::kBTileBytes, kcol, n0, wb);
+          tma_load_3d(&tmB_hi, &full_bar[slot], st, kcol, n0, wb);
+          if constexpr (!SINGLE) tma_load_3d(&tmB_lo, &full_bar[slot], st + Cfg::kBTileBytes, kcol, n0, wb);
+        };
+        // halo: the (BH + kh - 1) x BW box of all kh taps of (chunk, kx), from input row ys (TMA zero fill = SAME padding)
+        auto load_halo = [&](const KIter& k, int slot) {
+          uint8_t* st = smem + slot * a_slot_bytes;
+          const int c0 = p.in_choff + k.ck * kChunkK;
+          tma_load_4d(&tmA_hi, &a_full[slot], st, c0, xs + k.kx, ys, b);
+          if constexpr (!SINGLE) tma_load_4d(&tmA_lo, &a_full[slot], st + a_plane, c0, xs + k.kx, ys, b);
         };
         KIter k = {krank * chunks, 0, 0, conv_chunk(p, krank * chunks)};
         int it0 = 0;
@@ -152,30 +197,54 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
           // first tile of the kernel: weight tiles of the first ring stages, then wait for the predecessor kernel, then
           // the activation tiles of the same stages (the ring is empty here: slots 0.., phase 0)
           // (not when the B operand is itself an activation produced by an earlier kernel: corr build, w_per_batch)
+          // (halo: the B stages only; the halo boxes follow in the loop below)
           const int pre = p.w_per_batch ? 0 : (kiters < STAGES ? kiters : STAGES);
           KIter kb = k;
           for (int it = 0; it < pre; ++it) {
-            mbar_arrive_expect_tx(&full_bar[it], Cfg::kStageBytes);
+            mbar_arrive_expect_tx(&full_bar[it], b_stage_bytes);
             load_b(kb, it);
             k_next(kb);
           }
           asm volatile("griddepcontrol.wait;" ::: "memory");
           if (dbg) dbg[2] = gtime_ns();
-          for (int it = 0; it < pre; ++it) {
-            load_a(k, s);
-            k_next(k);
-            if (++s == STAGES) { s = 0; phase ^= 1; }
+          if (!halo) {
+            for (int it = 0; it < pre; ++it) {
+              load_a(k, s);
+              k_next(k);
+              if (++s == STAGES) { s = 0; phase ^= 1; }
+            }
           }
           it0 = pre;
           waited = true;
         }
-        for (int it = it0; it < kiters; ++it) {
-          mbar_wait(&empty_bar[s], phase ^ 1);
-          mbar_arrive_expect_tx(&full_bar[s], Cfg::kStageBytes);
-          load_a(k, s);
-          load_b(k, s);
-          k_next(k);
-          if (++s == STAGES) { s = 0; phase ^= 1; }
+        if constexpr (halo) {
+          // per (chunk, kx): one halo box into the A ring, then the kh weight tiles into the B ring (those of the first
+          // it0 k-iterations are already in flight)
+          for (int it = 0; it < kiters; ++it) {
+            if (k.ky == 0) {
+              mbar_wait(&a_empty[as], a_phase ^ 1);
+              mbar_arrive_expect_tx(&a_full[as], a_slot_bytes);
+              load_halo(k, as);
+            }
+            if (it >= it0) {
+              mbar_wait(&empty_bar[s], phase ^ 1);
+              mbar_arrive_expect_tx(&full_bar[s], b_stage_bytes);
+              load_b(k, s);
+            }
+            const bool group_end = k.ky == p.kh - 1;
+            k_next(k);
+            if (++s == STAGES) { s = 0; phase ^= 1; }
+            if (group_end && ++as == kHaloSlots) { as = 0; a_phase ^= 1; }
+          }
+        } else {
+          for (int it = it0; it < kiters; ++it) {
+            mbar_wait(&empty_bar[s], phase ^ 1);
+            mbar_arrive_expect_tx(&full_bar[s], Cfg::kStageBytes);
+            load_a(k, s);
+            load_b(k, s);
+            k_next(k);
+            if (++s == STAGES) { s = 0; phase ^= 1; }
+          }
         }
       }
     }
@@ -204,17 +273,22 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
     float hh[kNumAcc][Cfg::kAcc], xx[kNumAcc][SINGLE ? 1 : Cfg::kAcc];  // SINGLE: no cross-term accumulators
     int s = 0, pend = -1, li = 0;
     uint32_t phase = 0;
+    int as = 0, apend = -1, ky = 0;  // halo: A slot, the slot to hand back after the next wgmma_wait<1>, tap row
+    uint32_t a_phase = 0;
     // k-iterations [it0, it1) into (H, X); the wgmma group of a stage stays in flight while the next stage is issued, the
     // stage before it is handed back to the producer
     auto mma_range = [&](float* H, float* X, int it0, int it1) {
       for (int it = it0; it < it1; ++it) {
+        if (halo && ky == 0) mbar_wait(&a_full[as], a_phase);
         mbar_wait(&full_bar[s], phase);
         if (dbg && li == 0 && it == 0 && t == 0) dbg[3] = gtime_ns();
-        const uint32_t st = smem_u32(smem + s * Cfg::kStageBytes);
-        const uint64_t a_hi = wgmma_desc_sw128(st + cw * 64 * 128);
-        const uint64_t a_lo = wgmma_desc_sw128(st + kATileBytes + cw * 64 * 128);
-        const uint64_t b_hi = wgmma_desc_sw128(st + Cfg::kBOff);
-        const uint64_t b_lo = wgmma_desc_sw128(st + Cfg::kBOff + Cfg::kBTileBytes);
+        const uint32_t st = smem_u32(bring + s * b_stage_bytes);
+        // halo: tap row ky starts ky box rows into the slot
+        const uint32_t sa = halo ? smem_u32(smem + as * a_slot_bytes) + ((uint32_t)ky << g.bw_log2) * 128u : st;
+        const uint64_t a_hi = wgmma_desc_sw128(sa + cw * 64 * 128);
+        const uint64_t a_lo = wgmma_desc_sw128(sa + a_plane + cw * 64 * 128);
+        const uint64_t b_hi = wgmma_desc_sw128(st + b_off);
+        const uint64_t b_lo = wgmma_desc_sw128(st + b_off + Cfg::kBTileBytes);
         wgmma_fence();
 #pragma unroll
         for (int k = 0; k < kChunkK / 16; ++k) {
@@ -228,8 +302,15 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
         wgmma_commit();
         wgmma_wait<1>();
         if (pend >= 0 && t == 0) mbar_arrive(&empty_bar[pend]);
+        if (apend >= 0 && t == 0) mbar_arrive(&a_empty[apend]);
+        apend = -1;
         pend = s;
         if (++s == STAGES) { s = 0; phase ^= 1; }
+        if (halo && ++ky == p.kh) {  // the group's last tap: its slot goes back once this wgmma group has completed
+          ky = 0;
+          apend = as;
+          if (++as == kHaloSlots) { as = 0; a_phase ^= 1; }
+        }
       }
     };
     for (int tile = first; tile < g.total_tiles; tile += stride, ++li) {
@@ -260,7 +341,9 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
           if constexpr (!SINGLE) fence_operand(xx[a][i]);
         }
       if (t == 0) mbar_arrive(&empty_bar[pend]);
+      if (apend >= 0 && t == 0) mbar_arrive(&a_empty[apend]);
       pend = -1;
+      apend = -1;
       if (li == 0) {
         asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
         if (dbg && t == 0 && cw == 0) dbg[4] = gtime_ns();
@@ -444,6 +527,12 @@ struct ConvRecord {
 };
 static thread_local ConvOverride g_override = {0, 0, 0, 0};
 static thread_local ConvRecord g_record = {0, 0, 0, 0, 0, 0, 0, 0};
+// Test hook (rb_debug_conv_halo): -1 = no conv uses the halo A operand, 0 = as ConvParams::halo says, 1 = every conv
+// that can.  And the launch log of rb_debug_conv_log: the first kLogLen launches since the last rb_debug_conv_override().
+static thread_local int g_halo_mode = 0;
+constexpr int kLogLen = 64, kLogFields = 10;
+static thread_local int g_log[kLogLen][kLogFields];
+static thread_local int g_log_n = 0;
 
 // Ring depth of a launch: the test hook may lower it, but never below 2 -- a consumer hands a stage back only after it has
 // issued the next one (wgmma_wait<1>), so a one-stage ring deadlocks any conv with two k-iterations.
@@ -453,7 +542,12 @@ static int ring_stages(int max_stages) {
   return req < 2 ? 2 : req > max_stages ? max_stages : req;
 }
 
-static TileGeom choose_geom(int h, int w) {
+// halo_kh > 1: a conv with the halo A operand.  Every geometry streams the same weight tiles per pixel tile, and the
+// classic rule (fewest tiles) picks one-row boxes, whose halo is as large as the kh per-tap boxes it replaces; so these
+// convs take the box with the fewest rows streamed per (chunk, kx) over the whole image: the tiles times the
+// (BH + kh - 1) x BW halo plus kh weight tiles of up to 128 rows.  At 55 x 128 that is 8 x 16 (56 tiles against 55) for
+// 3x3 and 5x1 alike.
+static TileGeom choose_geom(int h, int w, int halo_kh = 0) {
   TileGeom best{};
   if (g_override.bw_log2 > 0) {
     const int bwl = g_override.bw_log2, bw = 1 << bwl, bh = kTileM >> bwl;
@@ -466,6 +560,7 @@ static TileGeom choose_geom(int h, int w) {
     int bw = 1 << bwl, bh = kTileM >> bwl;
     if (bw > w && bwl > 3) continue;  // keep the box inside the row when possible
     long tiles = (long)((w + bw - 1) / bw) * ((h + bh - 1) / bh);
+    if (halo_kh > 1) tiles *= (long)((bh + halo_kh - 1) << bwl) + halo_kh * 128;  // rows streamed per (chunk, kx)
     if (best_tiles < 0 || tiles < best_tiles) {
       best_tiles = tiles;
       best.bw_log2 = bwl; best.bh_log2 = 7 - bwl;
@@ -533,30 +628,52 @@ static int launch_cfg(const ConvParams& p_in, TileGeom g, const CUtensorMap* map
   if (!cluster2 && p.cta_limit > 0 && p.cta_limit < units) units = p.cta_limit;  // leave SMs to a concurrent conv (update.cu)
   if (max_ctas > 0 && max_ctas < units) units = max_ctas;
   const dim3 grid((g.total_tiles < units ? g.total_tiles : units) * (cluster2 ? 2 : 1));
-  const int stages = ring_stages(Cfg::kStages);
+  // halo: a B ring beside the kHaloSlots A slots; a forced ring depth applies to the B ring (the A ring stays at two)
+  const int stages = ring_stages(g.halo_rows ? halo_b_stages(BLOCK_N, Cfg::kPlanes, g.halo_rows) : Cfg::kStages);
+  g.ring_bytes = g.halo_rows ? kHaloSlots * Cfg::kPlanes * g.halo_rows * 128 + stages * Cfg::kPlanes * Cfg::kBTileBytes
+                             : stages * Cfg::kStageBytes;
+  const int smem = g.halo_rows ? g.ring_bytes + kSmemOverhead : Cfg::kSmemBytes;
   // Programmatic dependent launch: the dependent conv's prologue and its first weight tiles overlap the tail of this one.
   // Both EXTRAS instantiations get their shared-memory limit at the first launch of either.
-  constexpr auto plain = conv_tc_kernel<BLOCK_N, false, SINGLE>;
-  constexpr auto extras = conv_tc_kernel<BLOCK_N, true, SINGLE>;
+  constexpr auto plain = conv_tc_kernel<BLOCK_N, false, SINGLE, false>;
+  constexpr auto extras = conv_tc_kernel<BLOCK_N, true, SINGLE, false>;
+  constexpr auto plain_halo = conv_tc_kernel<BLOCK_N, false, SINGLE, true>;
+  constexpr auto extras_halo = conv_tc_kernel<BLOCK_N, true, SINGLE, true>;
   const int cluster = cluster2 ? 2 : 1;
-  if (p.dbg || p.stat_part)
-    rc = launch_pdl<extras, plain>(grid, dim3(kTcThreads), Cfg::kSmemBytes, cluster, s, maps[0], maps[1], maps[2], maps[3], p, g,
-                                   stages);
-  else
-    rc = launch_pdl<plain, extras>(grid, dim3(kTcThreads), Cfg::kSmemBytes, cluster, s, maps[0], maps[1], maps[2], maps[3], p, g,
-                                   stages);
+  if (!g.halo_rows) {
+    if (p.dbg || p.stat_part)
+      rc = launch_pdl<extras, plain>(grid, dim3(kTcThreads), smem, cluster, s, maps[0], maps[1], maps[2], maps[3], p, g, stages);
+    else
+      rc = launch_pdl<plain, extras>(grid, dim3(kTcThreads), smem, cluster, s, maps[0], maps[1], maps[2], maps[3], p, g, stages);
+  } else {
+    // the halo layouts take up to the whole ring budget: the limit is raised to it, for both instantiations, at the first
+    // launch of either
+    if ((rc = set_max_dyn_smem<plain_halo>(dev, kMaxSmem)) || (rc = set_max_dyn_smem<extras_halo>(dev, kMaxSmem))) return rc;
+    if (p.dbg || p.stat_part)
+      rc = launch_pdl<extras_halo>(grid, dim3(kTcThreads), smem, cluster, s, maps[0], maps[1], maps[2], maps[3], p, g, stages);
+    else
+      rc = launch_pdl<plain_halo>(grid, dim3(kTcThreads), smem, cluster, s, maps[0], maps[1], maps[2], maps[3], p, g, stages);
+  }
   if (rc) return rc;
   RB_CHECK_LAUNCH("conv_tc_kernel");
   g_record.block_n = BLOCK_N; g_record.bw_log2 = g.bw_log2; g_record.grid = (int)grid.x; g_record.stages = stages;
   g_record.total_tiles = g.total_tiles; g_record.launched = 1; g_record.passes = SINGLE ? 1 : 3;
   if (p.stat_part) ++g_record.fused_stats;
+  if (g_log_n < kLogLen) {
+    const int rec[kLogFields] = {BLOCK_N, g.bw_log2, (int)grid.x, stages, g.total_tiles, g.halo_rows, p.kh, p.kw,
+                                 conv_chunks(p), SINGLE ? 1 : 3};
+    memcpy(g_log[g_log_n++], rec, sizeof(rec));
+  }
   return RB_OK;
 }
 
 int launch_conv_tc(const ConvParams& p, cudaStream_t s) {
   RB_REQUIRE(p.cin_pad % kChunkK == 0 && p.in_stride % 8 == 0 && p.in_choff % 8 == 0, RB_ERR_BAD_SHAPE,
              "conv_tc: channel padding (cin_pad=%d stride=%d off=%d)", p.cin_pad, p.in_stride, p.in_choff);
-  const TileGeom g = choose_geom(p.h, p.w);
+  // the halo A operand: stride-1 convs over the default view with a vertical filter extent (not the split-K pair)
+  const bool want_halo = (g_halo_mode > 0 || (g_halo_mode == 0 && p.halo)) && p.kh > 1 && conv_default_view(p) &&
+                         !p.w_per_batch && !p.split_k;
+  TileGeom g = choose_geom(p.h, p.w, want_halo ? p.kh : 0);
   const long m_tiles = (long)p.B * g.tiles_x * g.tiles_y;
   int dev = 0, rc_dev;
   if ((rc_dev = current_device(&dev))) return rc_dev;
@@ -564,6 +681,11 @@ int launch_conv_tc(const ConvParams& p, cudaStream_t s) {
   int bn = choose_block_n(p.cout, m_tiles, p.cta_limit > 0 && p.cta_limit < num_sms ? p.cta_limit : num_sms);
   if (g_override.block_n > 0 && bn != 16) bn = g_override.block_n;  // the 16-wide (split-K) convs keep theirs
   const bool single = p.single_pass != 0;
+  g.halo_rows = 0;
+  if (want_halo) {  // one A box per tap when the halo box is too tall for TMA or the two slots leave no room for the B ring
+    const int box_h = (1 << g.bh_log2) + p.kh - 1, rows = box_h << g.bw_log2;
+    if (box_h <= 256 && halo_b_stages(bn, single ? 1 : 2, rows) >= 2) g.halo_rows = rows;
+  }
   CUtensorMap maps[4];
   {
     // the input view (common.cuh): strided convs traverse it with TMA element strides -- a box of bw*sx x bh*sy input
@@ -574,7 +696,8 @@ int launch_conv_tc(const ConvParams& p, cudaStream_t s) {
                (unsigned long long)rowpitch);
     uint64_t dims[4] = {(uint64_t)(p.in_cext > 0 ? p.in_cext : p.in_stride), (uint64_t)iw, (uint64_t)ih, (uint64_t)p.B};
     uint64_t str[3] = {(uint64_t)p.in_stride * 2, rowpitch * 2, rowpitch * 2 * ih};
-    uint32_t box[4] = {(uint32_t)kChunkK, (1u << g.bw_log2) * sx, (1u << g.bh_log2) * sy, 1};
+    const uint32_t box_h = g.halo_rows ? (uint32_t)(g.halo_rows >> g.bw_log2) : (1u << g.bh_log2) * sy;
+    uint32_t box[4] = {(uint32_t)kChunkK, (1u << g.bw_log2) * sx, box_h, 1};
     uint32_t es[4] = {1, (uint32_t)sx, (uint32_t)sy, 1};
     int rc;
     if ((rc = cached_tmap(&maps[0], p.in_hi, 4, dims, str, box, tc::TMAP_F16_SW128, es))) return rc;
@@ -639,7 +762,22 @@ extern "C" int rb_debug_conv_override(int block_n, int bw_log2, int max_ctas, in
              "rb_debug_conv_override: stages %d not 0 or in [2,%d]", stages, ring_max);
   g_override = {block_n, bw_log2, max_ctas, stages};
   g_record.fused_stats = 0;
+  g_log_n = 0;
   return RB_OK;
+}
+
+extern "C" int rb_debug_conv_halo(int mode) {
+  using namespace rb;
+  RB_REQUIRE(mode >= -1 && mode <= 1, RB_ERR_BAD_ARG, "rb_debug_conv_halo: mode %d not in {-1, 0, 1}", mode);
+  g_halo_mode = mode;
+  return RB_OK;
+}
+
+extern "C" int rb_debug_conv_log(int i, int* rec) {
+  using namespace rb;
+  RB_REQUIRE(i >= 0 && i < g_log_n && rec, RB_ERR_BAD_ARG, "rb_debug_conv_log: launch %d of %d logged", i, g_log_n);
+  memcpy(rec, g_log[i], sizeof(g_log[i]));
+  return g_log_n;
 }
 
 extern "C" int rb_debug_conv_last(int* block_n, int* bw_log2, int* grid, int* stages, int* total_tiles) {

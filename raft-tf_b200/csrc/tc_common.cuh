@@ -165,6 +165,8 @@ struct TileGeom {
   int n_tiles;           // cout tiles
   int m_tiles;           // B * tiles_x * tiles_y pixel tiles
   int total_tiles;       // work items: m_tiles * n_tiles
+  int halo_rows;         // > 0: rows of the activation halo box (A ring of kHaloSlots slots); 0: one A box per tap
+  int ring_bytes;        // shared memory of the operand rings (staging and barriers follow)
 };
 
 // per-thread cache of encoded tensor maps (conv_tc.cu)

@@ -397,6 +397,7 @@ static int update_step(const Variant& v, const void* blob, void* wsp, float* coo
     {
       ConvParams p = base_params(v, L.conv[P_CONVF2], blob, W.f1, v.f1, B, h, w);
       set_act(p, ACT_RELU, W.cf, v.cf, v.cor);
+      p.halo = 1;
       // convf2 runs beside convc1 / convc2 of the main stream: a small CTA budget keeps it off the SMs they need
       // (batch 1: the other convs use 55-110 of the 132 SMs)
       p.cta_limit = (long)B * h * w <= 16384 ? 38 : 0;
@@ -414,6 +415,7 @@ static int update_step(const Variant& v, const void* blob, void* wsp, float* coo
     if ((rc = launch_conv_dbg(p, s))) return rc;
     p = base_params(v, L.conv[P_CONVC2], blob, W.c1, v.c1, B, h, w);
     set_act(p, ACT_RELU, W.cf, v.cf, 0);
+    p.halo = 1;
     if ((rc = launch_conv_dbg(p, s))) return rc;
   } else {
     ConvParams p = base_params(v, L.conv[P_CONVC1], blob, W.corr, v.corr_pad, B, h, w);
@@ -424,6 +426,7 @@ static int update_step(const Variant& v, const void* blob, void* wsp, float* coo
   {
     ConvParams p = base_params(v, L.conv[P_MOTION], blob, W.cf, v.cf, B, h, w);
     set_act(p, ACT_RELU, W.hx, v.hx, xoff);
+    p.halo = 1;
     p.d1_hi = W.qx.hi; p.d1_lo = W.qx.lo; p.d1_stride = v.hx; p.d1_choff = xoff;
     if (math_mode_tc() && (p.cout & 15) == 14 && p.cout + 2 <= p.cout_pad && foff == xoff + p.cout) {
       // things: 126 channels + the 2 flow channels right behind them = one full 16-channel group -> the tensor-core
@@ -441,11 +444,13 @@ static int update_step(const Variant& v, const void* blob, void* wsp, float* coo
     hoist_inp(v, W, pass * 2 + 0, p);
     p.epi = EPI_ZR; p.f0 = W.Z; p.f1 = W.H;
     p.d0_hi = W.qx.hi; p.d0_lo = W.qx.lo; p.d0_stride = v.hx; p.d0_choff = 0;
+    p.halo = 1;  // the 5x1 (and raft-small's 3x3) convs; a 1x5 conv has no vertical taps to share
     if ((rc = launch_conv_dbg(p, s))) return rc;
     p = base_params(v, L.conv[q], blob, W.qx, v.hx, B, h, w);
     hoist_inp(v, W, pass * 2 + 1, p);
     p.epi = EPI_Q; p.f0 = W.Z; p.f1 = W.H;
     p.d0_hi = W.hx.hi; p.d0_lo = W.hx.lo; p.d0_stride = v.hx; p.d0_choff = 0;
+    p.halo = 1;
     if ((rc = launch_conv_dbg(p, s))) return rc;
   }
   // ---- flow head (model_utils.py:131-135) + coords1 += delta (RAFT.py:102) ----
@@ -455,13 +460,14 @@ static int update_step(const Variant& v, const void* blob, void* wsp, float* coo
   {
     ConvParams p = base_params(v, L.conv[P_FH1], blob, W.hx, v.hx, B, h, w);
     set_act(p, ACT_RELU, W.fh, v.fh, 0);
+    p.halo = 1;
     if ((rc = launch_conv_dbg(p, s))) return rc;
     p = base_params(v, L.conv[P_FH2], blob, W.fh, v.fh, B, h, w);
     p.epi = EPI_DELTA; p.f1 = coords1; p.f2 = delta_out;
     // 36 k-iterations on 55 CTAs at batch 1 while 77 SMs idle: two CTAs per pixel tile, half of the channel chunks each
     // (conv_tc.cu, split-K over a cluster when the tiles fit one wave of CTA pairs; the same two-halves sum on one CTA
     // otherwise, so batched and per-sample runs stay bit-identical).
-    p.split_k = 1;
+    p.split_k = 1;  // keeps one A box per tap: the split-K pair does not take the halo (conv_tc.cu)
     if ((rc = launch_conv_dbg(p, s))) return rc;
   }
   // ---- mask head (model_utils.py:180-183); only the last iteration's mask is ever consumed ----

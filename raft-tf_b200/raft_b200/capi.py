@@ -34,6 +34,8 @@ SIGNATURES = {
     "rb_debug_conv_override": (_i, [_i, _i, _i, _i]),
     "rb_debug_conv_last": (_i, [_pi, _pi, _pi, _pi, _pi]),
     "rb_debug_conv_last_passes": (_i, []),
+    "rb_debug_conv_halo": (_i, [_i]),
+    "rb_debug_conv_log": (_i, [_i, _pi]),
     "rb_coords_grid": (_i, [_vp, _i, _i, _i, _vp]),
     "rb_coords_init": (_i, [_vp, _vp, _i, _i, _i, _vp]),
     "rb_coords_to_flow": (_i, [_vp, _vp, _i, _i, _i, _vp]),
