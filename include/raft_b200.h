@@ -760,6 +760,57 @@ int rb_frame_synthesize_items_resized(const void* frames0, const void* frames1, 
                                       const float* item_t, int n_items, void* out, int out_u8, int bgr, int B,
                                       void* stream);
 
+/* ---- F32: a camera shutter for frame-rate conversion -- each output frame the mean of sub-frames over its exposure --
+ * Times are in input frames (input frame i sits at time i).  Output frame n of a conversion from rate `in` to rate `out`
+ * sits at s = n in/out; with shutter angle A in (0, 360] its exposure is [s - e/2, s + e/2], e = (A/360) in/out, and with
+ * `density` D >= 1 samples per input-frame interval it is sampled at m = max(1, ceil(D e)) times
+ * u_j = s - e/2 + (j + 1/2) e/m (the midpoint rule), each clamped into the frames [a, b] of the shot holding s (a scene
+ * cut is a shot boundary; a frame inside a cut pair k belongs to the shot of raft_b200.video.cut_copy).  A non-integer
+ * u_j is the item (k, t) = (floor(u_j), fl32(u_j - k)) -- rb_frame_synthesize_items' (or _items_resized') fp32 value --
+ * and an integer u_j is input frame u_j as prepared (the blend's value at t = 0 exactly).  The output frame is acc / m,
+ * acc the fp32 sum from +0.0 of the m values in sample order, each add rounded on its own, quantised as rb_frame_metrics
+ * does: min(max(rintf(fl32(255 v)), 0), 255), NaN -> 0.  m = 1 is the conversion without a shutter byte for byte.
+ * (Brooks & Barron, CVPR 2019: interpolate, then average; it is how Nah et al., CVPR 2017, made the GoPro blur.)
+ *
+ * rb_frame_expose_items runs a table of rows, each one output frame's run of samples, copied into the kernel parameters
+ * like rb_frame_synthesize_items' items (no copy, no allocation, no atomics, CUDA-graph capturable):
+ *   entries[i]  = (slot, sample, t): slot >= 0 is the blend of frames[sample] and frames[sample + 1] at t with slot
+ *                 `slot` of flow_t0, flow_t1 [n_slots,H,W,2] and empty0, empty1 [n_slots,H,W] (rb_flow_reverse_items'
+ *                 outputs for the steps s t and s (1 - t)); slot = RB_EXPOSE_FRAME is input frame `sample` itself;
+ *   rows[r]     = (first, count, m, acc, out, flags): entries first .. first + count - 1 in order.  flags
+ *                 RB_EXPOSE_OPEN starts the sum from +0.0, else from acc[acc]; RB_EXPOSE_CLOSE writes the quantised
+ *                 acc / m to out[out] (bgr = 1: channels reversed), else stores the sum in acc[acc].
+ * So a frame's samples may be split over calls (and over passes of a video): the fp32 sum carries through acc, and the
+ * bytes do not depend on where the calls split.  One thread per (row, pixel) adds its row's entries in order.
+ * frames [B+1,Hp,Wp,3] fp32 padded, read at the crop (top, left) + H x W as in rb_frame_synthesize_pairs; acc
+ * [n_acc,H,W,3] fp32; out [n_out,H,W,3] uint8.  Null pointers (the flows and masks may be null when n_slots = 0, acc
+ * when no row reads or stores it, out when none closes), n_entries < 1 or > RB_INTERP_MAX_STEPS, n_rows < 1 or > n_entries, bgr not 0 / 1, bad shapes or
+ * crop, a row's entries outside the table or count < 1, m < 1 or > 2^24, unknown flags, an acc or out index outside
+ * [0, n_acc) / [0, n_out), two rows of the call on one acc or out index, a slot outside [-1, n_slots), a sample outside
+ * [0, B) (a blend) or [0, B] (a frame) and a t outside [0, 1] (or NaN) -> RB_ERR_* before any CUDA call.
+ * rb_frame_expose_items_resized is the same at the frames' own Hs x Ws from flows at H x W (F16's blend, and frames as
+ * there: uint8 with frames_u8 = 1, read as np.float32(u) / 255, or fp32 as they are); frames [B+1,Hs,Ws,3] unpadded, acc
+ * [n_acc,Hs,Ws,3], out [n_out,Hs,Ws,3]. */
+#define RB_EXPOSE_FRAME (-1)
+#define RB_EXPOSE_OPEN 1
+#define RB_EXPOSE_CLOSE 2
+typedef struct {
+  int32_t slot, sample;
+  float t;
+} rb_expose_entry;
+typedef struct {
+  int32_t first, count, m, acc, out, flags;
+} rb_expose_row;
+int rb_frame_expose_items(const float* frames, int Hp, int Wp, int top, int left, const float* flow_t0,
+                          const float* flow_t1, const uint8_t* empty0, const uint8_t* empty1, int n_slots,
+                          const rb_expose_entry* entries, int n_entries, const rb_expose_row* rows, int n_rows,
+                          float* acc, int n_acc, uint8_t* out, int n_out, int bgr, int B, int H, int W, void* stream);
+int rb_frame_expose_items_resized(const void* frames, int frames_u8, int Hs, int Ws, const float* flow_t0,
+                                  const float* flow_t1, const uint8_t* empty0, const uint8_t* empty1, int H, int W,
+                                  int n_slots, const rb_expose_entry* entries, int n_entries, const rb_expose_row* rows,
+                                  int n_rows, float* acc, int n_acc, uint8_t* out, int n_out, int bgr, int B,
+                                  void* stream);
+
 /* ---- F9: end-point-error metrics (upstream RAFT's evaluate.py validate_sintel / validate_kitti) ---------------------
  * flow, gt: [B,H,W,2] fp32; valid: [B,H,W] uint8, nonzero = the pixel counts (NULL: every pixel counts).  Per pixel,
  * every operation rounded on its own (no FMA contraction), so the values equal upstream's torch expressions bit for bit:

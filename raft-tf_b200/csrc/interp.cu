@@ -269,13 +269,16 @@ struct RawU8 {
   }
 };
 
+// One pixel's three channels, in the frames' channel order
+struct Rgb {
+  float c[3];
+};
+
 // The blend of one output pixel (x, y) of an H x W frame: both frames sampled at p + F_k (clamped to the frame; NaN ->
-// 0) with the bilinear arithmetic of rb_flow_fb_check, blended by (1-t, t) with empty targets weighted 0; written to
-// out[p] as fp32, or quantised to uint8 (with bgr: channels reversed).
+// 0) with the bilinear arithmetic of rb_flow_fb_check, blended by (1-t, t) with empty targets weighted 0.
 template <class Frame>
-__device__ __forceinline__ void synthesize_px(const Frame& i0, const Frame& i1, int x, int y, int H, int W, float2 F0,
-                                              float2 F1, bool empty0, bool empty1, float t, void* out, size_t p,
-                                              int out_u8, int bgr) {
+__device__ __forceinline__ Rgb synthesize_px(const Frame& i0, const Frame& i1, int x, int y, int H, int W, float2 F0,
+                                             float2 F1, bool empty0, bool empty1, float t) {
   const float s = __fsub_rn(1.f, t);
   float w0 = empty0 ? 0.f : s, w1 = empty1 ? 0.f : t;
   if (w0 == 0.f && w1 == 0.f) w0 = s, w1 = t;
@@ -296,14 +299,43 @@ __device__ __forceinline__ void synthesize_px(const Frame& i0, const Frame& i1, 
     }
   }
   const float den = __fadd_rn(w0, w1);
+  Rgb o;
+  for (int c = 0; c < 3; ++c) o.c[c] = __fdiv_rn(__fadd_rn(__fmul_rn(w0, v[0][c]), __fmul_rn(w1, v[1][c])), den);
+  return o;
+}
+
+// out[p] as fp32, or quantised to uint8 (with bgr: channels reversed)
+__device__ __forceinline__ void store_px(const Rgb& o, void* out, size_t p, int out_u8, int bgr) {
   for (int c = 0; c < 3; ++c) {
-    const float o = __fdiv_rn(__fadd_rn(__fmul_rn(w0, v[0][c]), __fmul_rn(w1, v[1][c])), den);
     const int oc = bgr ? 2 - c : c;
     if (out_u8)
-      static_cast<uint8_t*>(out)[p * 3 + oc] = quantise(o);
+      static_cast<uint8_t*>(out)[p * 3 + oc] = quantise(o.c[c]);
     else
-      static_cast<float*>(out)[p * 3 + oc] = o;
+      static_cast<float*>(out)[p * 3 + oc] = o.c[c];
   }
+}
+
+// The inputs of the resized blend at output pixel (x, y) of Hs x Ws for reversal sample smp of the H x W flows:
+// rb_flow_resize's flow there (resize_f32_px of the low-resolution flow, then u *= su, v *= sv) and the empty mask of
+// the network pixel `near` whose area holds the pixel's centre, read through the read-only path.
+__device__ __forceinline__ void resized_px(const float* __restrict__ f0, const float* __restrict__ f1,
+                                           const uint8_t* __restrict__ e0, const uint8_t* __restrict__ e1, size_t smp,
+                                           size_t near, int H, int W, int Hs, int Ws, int y, int x, int mode, float su,
+                                           float sv, float2& F0, float2& F1, bool& m0, bool& m1) {
+  const size_t lhw = (size_t)H * W;
+  float a[2], c[2];
+  resize_f32_px<2>(f0 + smp * lhw * 2, H, W, Hs, Ws, y, x, mode, a);
+  resize_f32_px<2>(f1 + smp * lhw * 2, H, W, Hs, Ws, y, x, mode, c);
+  F0 = make_float2(__fmul_rn(a[0], su), __fmul_rn(a[1], sv));
+  F1 = make_float2(__fmul_rn(c[0], su), __fmul_rn(c[1], sv));
+  m0 = __ldg(e0 + smp * lhw + near) != 0;
+  m1 = __ldg(e1 + smp * lhw + near) != 0;
+}
+
+// the network pixel whose area holds the centre of output pixel (x, y): (((2x+1) W) div (2 Ws), ((2y+1) H) div (2 Hs))
+__device__ __forceinline__ size_t near_px(int x, int y, int H, int W, int Hs, int Ws) {
+  return (size_t)(((2 * (uint64_t)y + 1) * (uint64_t)H) / (2 * (uint64_t)Hs)) * W +
+         (size_t)(((2 * (uint64_t)x + 1) * (uint64_t)W) / (2 * (uint64_t)Ws));
 }
 
 // One thread per output pixel, blockIdx.y striding over the (time, sample) pairs (32-bit pixel indices; a pair is
@@ -326,7 +358,7 @@ __global__ void __launch_bounds__(256) frame_synthesize_kernel(const float* __re
     const size_t p = (size_t)smp * hw + q;
     const size_t crop = ((size_t)b * Hp + top) * Wp * 3 + (size_t)left * 3;
     const CropF32 i0{frames0 + crop, (size_t)Wp * 3}, i1{frames1 + crop, (size_t)Wp * 3};
-    synthesize_px(i0, i1, x, y, H, W, f0[p], f1[p], e0[p] != 0, e1[p] != 0, times.v[j], out, p, out_u8, bgr);
+    store_px(synthesize_px(i0, i1, x, y, H, W, f0[p], f1[p], e0[p] != 0, e1[p] != 0, times.v[j]), out, p, out_u8, bgr);
   }
 }
 
@@ -349,30 +381,136 @@ __global__ void __launch_bounds__(256) frame_synthesize_resized_kernel(
   const uint32_t hw = (uint32_t)Hs * (uint32_t)Ws;
   if (q >= hw) return;
   const int x = (int)(q % (uint32_t)Ws), y = (int)(q / (uint32_t)Ws);
-  const size_t lhw = (size_t)H * W;
-  const size_t near = (size_t)(((2 * (uint64_t)y + 1) * (uint64_t)H) / (2 * (uint64_t)Hs)) * W +
-                      (size_t)(((2 * (uint64_t)x + 1) * (uint64_t)W) / (2 * (uint64_t)Ws));
+  const size_t near = near_px(x, y, H, W, Hs, Ws);
   const size_t frame = (size_t)hw * 3;
   for (uint32_t smp = blockIdx.y; smp < (uint32_t)n_t * B; smp += gridDim.y) {
     const uint32_t j = smp / (uint32_t)B;
     const int b = times.items ? times.row[j] : (int)(smp % B);
     const size_t p = (size_t)smp * hw + q;
-    float a[2], c[2];
-    resize_f32_px<2>(f0 + (size_t)smp * lhw * 2, H, W, Hs, Ws, y, x, mode, a);
-    resize_f32_px<2>(f1 + (size_t)smp * lhw * 2, H, W, Hs, Ws, y, x, mode, c);
-    const float2 F0 = make_float2(__fmul_rn(a[0], su), __fmul_rn(a[1], sv));
-    const float2 F1 = make_float2(__fmul_rn(c[0], su), __fmul_rn(c[1], sv));
-    const bool m0 = __ldg(e0 + (size_t)smp * lhw + near) != 0, m1 = __ldg(e1 + (size_t)smp * lhw + near) != 0;
+    float2 F0, F1;
+    bool m0, m1;
+    resized_px(f0, f1, e0, e1, smp, near, H, W, Hs, Ws, y, x, mode, su, sv, F0, F1, m0, m1);
     if (U8) {
       const RawU8 i0{static_cast<const uint8_t*>(frames0) + b * frame, (size_t)Ws * 3, lut};
       const RawU8 i1{static_cast<const uint8_t*>(frames1) + b * frame, (size_t)Ws * 3, lut};
-      synthesize_px(i0, i1, x, y, Hs, Ws, F0, F1, m0, m1, times.v[j], out, p, out_u8, bgr);
+      store_px(synthesize_px(i0, i1, x, y, Hs, Ws, F0, F1, m0, m1, times.v[j]), out, p, out_u8, bgr);
     } else {
       const CropF32 i0{static_cast<const float*>(frames0) + b * frame, (size_t)Ws * 3};
       const CropF32 i1{static_cast<const float*>(frames1) + b * frame, (size_t)Ws * 3};
-      synthesize_px(i0, i1, x, y, Hs, Ws, F0, F1, m0, m1, times.v[j], out, p, out_u8, bgr);
+      store_px(synthesize_px(i0, i1, x, y, Hs, Ws, F0, F1, m0, m1, times.v[j]), out, p, out_u8, bgr);
     }
   }
+}
+
+// F32's table (rb_expose_entry / rb_expose_row), by value in the kernel parameters like Steps
+struct Expose {
+  rb_expose_entry e[kMaxSteps];
+  rb_expose_row r[kMaxSteps];
+};
+
+// A row's running sum at one pixel: +0.0 when the row opens, else its accumulator
+__device__ __forceinline__ Rgb expose_start(const rb_expose_row& r, const float* acc, size_t hw, uint32_t q) {
+  Rgb a;
+  for (int c = 0; c < 3; ++c)
+    a.c[c] = (r.flags & RB_EXPOSE_OPEN) ? 0.f : acc[((size_t)r.acc * hw + q) * 3 + c];
+  return a;
+}
+
+__device__ __forceinline__ void expose_add(Rgb& a, const Rgb& v) {
+  for (int c = 0; c < 3; ++c) a.c[c] = __fadd_rn(a.c[c], v.c[c]);
+}
+
+// A row's sum after its entries: closed, the quantised mean acc / m (bgr: channels reversed); else kept in acc
+__device__ __forceinline__ void expose_finish(const rb_expose_row& r, Rgb a, float* acc, uint8_t* out, size_t hw,
+                                              uint32_t q, int bgr) {
+  if (r.flags & RB_EXPOSE_CLOSE) {
+    const float m = (float)r.m;
+    for (int c = 0; c < 3; ++c) a.c[c] = __fdiv_rn(a.c[c], m);
+    store_px(a, out, (size_t)r.out * hw + q, 1, bgr);
+  } else {
+    for (int c = 0; c < 3; ++c) acc[((size_t)r.acc * hw + q) * 3 + c] = a.c[c];
+  }
+}
+
+// One thread per (row, pixel), blockIdx.y the row: the row's entries in order, each the blend of its pair at its t
+// (synthesize_px on the crops of frames[sample], frames[sample + 1] with the slot's flows and masks) or its input frame.
+__global__ void __launch_bounds__(256) frame_expose_kernel(const float* __restrict__ frames, int Hp, int Wp, int top,
+                                                           int left, const float2* __restrict__ f0,
+                                                           const float2* __restrict__ f1,
+                                                           const uint8_t* __restrict__ e0,
+                                                           const uint8_t* __restrict__ e1, Expose tab, float* acc,
+                                                           uint8_t* out, int bgr, int H, int W) {
+  const uint32_t q = blockIdx.x * blockDim.x + threadIdx.x;
+  const uint32_t hw = (uint32_t)H * W;
+  if (q >= hw) return;
+  const int x = (int)(q % W), y = (int)(q / W);
+  const rb_expose_row& r = tab.r[blockIdx.y];
+  Rgb a = expose_start(r, acc, hw, q);
+  for (int i = r.first; i < r.first + r.count; ++i) {
+    const rb_expose_entry& en = tab.e[i];
+    const CropF32 i0{frames + ((size_t)en.sample * Hp + top) * Wp * 3 + (size_t)left * 3, (size_t)Wp * 3};
+    Rgb v;
+    if (en.slot < 0) {
+      for (int c = 0; c < 3; ++c) v.c[c] = i0(y, x, c);
+    } else {
+      const CropF32 i1{i0.img + (size_t)Hp * Wp * 3, i0.row};
+      const size_t p = (size_t)en.slot * hw + q;
+      v = synthesize_px(i0, i1, x, y, H, W, f0[p], f1[p], e0[p] != 0, e1[p] != 0, en.t);
+    }
+    expose_add(a, v);
+  }
+  expose_finish(r, a, acc, out, hw, q, bgr);
+}
+
+// frame_expose_kernel at the frames' own Hs x Ws from flows and masks at H x W (resized_px, as
+// frame_synthesize_resized_kernel); uint8 frames are read as bytes and scaled by the table of the 256 quotients.
+template <bool U8>
+__global__ void __launch_bounds__(256) frame_expose_resized_kernel(const void* __restrict__ frames, int Hs, int Ws,
+                                                                   const float* __restrict__ f0,
+                                                                   const float* __restrict__ f1,
+                                                                   const uint8_t* __restrict__ e0,
+                                                                   const uint8_t* __restrict__ e1, int H, int W,
+                                                                   int mode, float su, float sv, Expose tab, float* acc,
+                                                                   uint8_t* out, int bgr) {
+  __shared__ float lut[256];
+  if (U8) {
+    for (int i = threadIdx.x; i < 256; i += blockDim.x) lut[i] = __fdiv_rn((float)i, 255.0f);
+    __syncthreads();
+  }
+  const uint32_t q = blockIdx.x * blockDim.x + threadIdx.x;
+  const uint32_t hw = (uint32_t)Hs * (uint32_t)Ws;
+  if (q >= hw) return;
+  const int x = (int)(q % (uint32_t)Ws), y = (int)(q / (uint32_t)Ws);
+  const size_t near = near_px(x, y, H, W, Hs, Ws);
+  const size_t frame = (size_t)hw * 3;
+  const rb_expose_row& r = tab.r[blockIdx.y];
+  Rgb a = expose_start(r, acc, hw, q);
+  for (int i = r.first; i < r.first + r.count; ++i) {
+    const rb_expose_entry& en = tab.e[i];
+    Rgb v;
+    float2 F0 = make_float2(0.f, 0.f), F1 = F0;
+    bool m0 = false, m1 = false;
+    if (en.slot >= 0) resized_px(f0, f1, e0, e1, (size_t)en.slot, near, H, W, Hs, Ws, y, x, mode, su, sv, F0, F1, m0, m1);
+    if (U8) {
+      const RawU8 i0{static_cast<const uint8_t*>(frames) + en.sample * frame, (size_t)Ws * 3, lut};
+      if (en.slot < 0) {
+        for (int c = 0; c < 3; ++c) v.c[c] = i0(y, x, c);
+      } else {
+        const RawU8 i1{i0.img + frame, i0.row, lut};
+        v = synthesize_px(i0, i1, x, y, Hs, Ws, F0, F1, m0, m1, en.t);
+      }
+    } else {
+      const CropF32 i0{static_cast<const float*>(frames) + en.sample * frame, (size_t)Ws * 3};
+      if (en.slot < 0) {
+        for (int c = 0; c < 3; ++c) v.c[c] = i0(y, x, c);
+      } else {
+        const CropF32 i1{i0.img + frame, i0.row};
+        v = synthesize_px(i0, i1, x, y, Hs, Ws, F0, F1, m0, m1, en.t);
+      }
+    }
+    expose_add(a, v);
+  }
+  expose_finish(r, a, acc, out, hw, q, bgr);
 }
 
 }  // namespace
@@ -685,4 +823,111 @@ extern "C" int rb_frame_synthesize_items_resized(const void* frames0, const void
   }
   return synthesize_resized_run("rb_frame_synthesize_items_resized", frames0, frames1, frames_u8, Hs, Ws, flow_t0,
                                 flow_t1, empty0, empty1, H, W, times, n_items, out, out_u8, bgr, B, stream);
+}
+
+namespace {
+
+// The checks of F32's tables, shared by both expose entries: every entry and row as include/raft_b200.h states, then
+// the table packed into the kernel parameters.  Needs acc / out non-null only when a row reads or stores / closes.
+int expose_table(const char* fn, const rb_expose_entry* entries, int n_entries, const rb_expose_row* rows, int n_rows,
+                 int n_slots, int B, const float* acc, int n_acc, const uint8_t* out, int n_out, int bgr, Expose* tab) {
+  RB_REQUIRE(entries && rows, RB_ERR_BAD_ARG, "%s: null pointer", fn);
+  RB_REQUIRE(n_entries > 0 && n_entries <= kMaxSteps, RB_ERR_BAD_ARG, "%s: %d entries (1..%d)", fn, n_entries,
+             kMaxSteps);
+  RB_REQUIRE(n_rows > 0 && n_rows <= n_entries, RB_ERR_BAD_ARG, "%s: %d rows (1..%d entries)", fn, n_rows, n_entries);
+  RB_REQUIRE(bgr == 0 || bgr == 1, RB_ERR_BAD_ARG, "%s: bgr must be 0 or 1 (got %d)", fn, bgr);
+  RB_REQUIRE(B > 0, RB_ERR_BAD_SHAPE, "%s: B = %d pairs", fn, B);
+  for (int i = 0; i < n_entries; ++i) {
+    const rb_expose_entry& e = entries[i];
+    RB_REQUIRE(e.slot >= RB_EXPOSE_FRAME && e.slot < n_slots, RB_ERR_BAD_ARG, "%s: entry %d: slot %d outside [-1, %d)",
+               fn, i, e.slot, n_slots);
+    const int hi = e.slot < 0 ? B : B - 1;
+    RB_REQUIRE(e.sample >= 0 && e.sample <= hi, RB_ERR_BAD_ARG, "%s: entry %d: sample %d outside [0, %d]", fn, i,
+               e.sample, hi);
+    RB_REQUIRE(e.slot < 0 || (e.t >= 0.f && e.t <= 1.f), RB_ERR_BAD_ARG, "%s: entry %d: t must be in [0, 1] (got %g)",
+               fn, i, (double)e.t);
+    tab->e[i] = e;
+  }
+  bool reads_acc = false, closes = false;
+  for (int r = 0; r < n_rows; ++r) {
+    const rb_expose_row& w = rows[r];
+    RB_REQUIRE(w.count >= 1 && w.first >= 0 && w.first <= n_entries - w.count, RB_ERR_BAD_ARG,
+               "%s: row %d: entries %d + %d outside the %d of the table", fn, r, w.first, w.count, n_entries);
+    RB_REQUIRE(w.m >= 1 && w.m <= (1 << 24), RB_ERR_BAD_ARG, "%s: row %d: m = %d samples (1..2^24)", fn, r, w.m);
+    RB_REQUIRE((w.flags & ~(RB_EXPOSE_OPEN | RB_EXPOSE_CLOSE)) == 0, RB_ERR_BAD_ARG, "%s: row %d: flags %d", fn, r,
+               w.flags);
+    const bool uses_acc = w.flags != (RB_EXPOSE_OPEN | RB_EXPOSE_CLOSE), close = (w.flags & RB_EXPOSE_CLOSE) != 0;
+    RB_REQUIRE(!uses_acc || (w.acc >= 0 && w.acc < n_acc), RB_ERR_BAD_ARG, "%s: row %d: acc %d outside [0, %d)", fn, r,
+               w.acc, n_acc);
+    RB_REQUIRE(!close || (w.out >= 0 && w.out < n_out), RB_ERR_BAD_ARG, "%s: row %d: out %d outside [0, %d)", fn, r,
+               w.out, n_out);
+    for (int o = 0; o < r; ++o) {  // rows run concurrently: none may touch another's accumulator or output frame
+      const rb_expose_row& v = rows[o];
+      RB_REQUIRE(!(uses_acc && v.flags != (RB_EXPOSE_OPEN | RB_EXPOSE_CLOSE) && v.acc == w.acc), RB_ERR_BAD_ARG,
+                 "%s: rows %d and %d share acc %d", fn, o, r, w.acc);
+      RB_REQUIRE(!(close && (v.flags & RB_EXPOSE_CLOSE) && v.out == w.out), RB_ERR_BAD_ARG,
+                 "%s: rows %d and %d share out %d", fn, o, r, w.out);
+    }
+    reads_acc = reads_acc || uses_acc;
+    closes = closes || close;
+    tab->r[r] = w;
+  }
+  RB_REQUIRE((!reads_acc || acc) && (!closes || out), RB_ERR_BAD_ARG, "%s: null acc or out", fn);
+  return RB_OK;
+}
+
+}  // namespace
+
+extern "C" int rb_frame_expose_items(const float* frames, int Hp, int Wp, int top, int left, const float* flow_t0,
+                                     const float* flow_t1, const uint8_t* empty0, const uint8_t* empty1, int n_slots,
+                                     const rb_expose_entry* entries, int n_entries, const rb_expose_row* rows,
+                                     int n_rows, float* acc, int n_acc, uint8_t* out, int n_out, int bgr, int B, int H,
+                                     int W, void* stream) {
+  const char* fn = "rb_frame_expose_items";
+  RB_REQUIRE(frames && (n_slots == 0 || (flow_t0 && flow_t1 && empty0 && empty1)), RB_ERR_BAD_ARG, "%s: null pointer",
+             fn);
+  Expose tab;
+  const int rc = expose_table(fn, entries, n_entries, rows, n_rows, n_slots, B, acc, n_acc, out, n_out, bgr, &tab);
+  if (rc != RB_OK) return rc;
+  RB_REQUIRE(H > 0 && W > 0, RB_ERR_BAD_SHAPE, "%s: bad shape H=%d W=%d", fn, H, W);
+  RB_REQUIRE(top >= 0 && left >= 0 && top + H <= Hp && left + W <= Wp, RB_ERR_BAD_SHAPE,
+             "%s: crop (%d, %d) + %dx%d outside the %dx%d frames", fn, top, left, H, W, Hp, Wp);
+  const size_t hw = (size_t)H * W;
+  RB_REQUIRE(hw < (size_t(1) << 32), RB_ERR_BAD_SHAPE, "%s: %zu pixels per frame exceed 32-bit indices", fn, hw);
+  const dim3 grid((unsigned)((hw + 255) / 256), (unsigned)n_rows);
+  frame_expose_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(
+      frames, Hp, Wp, top, left, reinterpret_cast<const float2*>(flow_t0), reinterpret_cast<const float2*>(flow_t1),
+      empty0, empty1, tab, acc, out, bgr, H, W);
+  RB_CHECK_LAUNCH("frame_expose_kernel");
+  return RB_OK;
+}
+
+extern "C" int rb_frame_expose_items_resized(const void* frames, int frames_u8, int Hs, int Ws, const float* flow_t0,
+                                             const float* flow_t1, const uint8_t* empty0, const uint8_t* empty1, int H,
+                                             int W, int n_slots, const rb_expose_entry* entries, int n_entries,
+                                             const rb_expose_row* rows, int n_rows, float* acc, int n_acc,
+                                             uint8_t* out, int n_out, int bgr, int B, void* stream) {
+  const char* fn = "rb_frame_expose_items_resized";
+  RB_REQUIRE(frames && (n_slots == 0 || (flow_t0 && flow_t1 && empty0 && empty1)), RB_ERR_BAD_ARG, "%s: null pointer",
+             fn);
+  RB_REQUIRE(frames_u8 == 0 || frames_u8 == 1, RB_ERR_BAD_ARG, "%s: frames_u8 must be 0 or 1 (got %d)", fn, frames_u8);
+  Expose tab;
+  const int rc = expose_table(fn, entries, n_entries, rows, n_rows, n_slots, B, acc, n_acc, out, n_out, bgr, &tab);
+  if (rc != RB_OK) return rc;
+  RB_REQUIRE(H > 0 && W > 0 && Hs > 0 && Ws > 0, RB_ERR_BAD_SHAPE, "%s: bad shape H=%d W=%d Hs=%d Ws=%d", fn, H, W, Hs,
+             Ws);
+  const size_t hw = (size_t)Hs * Ws;
+  RB_REQUIRE(hw < (size_t(1) << 32), RB_ERR_BAD_SHAPE, "%s: %zu pixels per frame exceed 32-bit indices", fn, hw);
+  const dim3 grid((unsigned)((hw + 255) / 256), (unsigned)n_rows);
+  const int mode = float_mode(H, W, Hs, Ws);
+  const float su = flow_scale_u(W, Ws), sv = flow_scale_v(H, Hs);
+  const cudaStream_t st = (cudaStream_t)stream;
+  if (frames_u8)
+    frame_expose_resized_kernel<true><<<grid, 256, 0, st>>>(frames, Hs, Ws, flow_t0, flow_t1, empty0, empty1, H, W, mode,
+                                                            su, sv, tab, acc, out, bgr);
+  else
+    frame_expose_resized_kernel<false><<<grid, 256, 0, st>>>(frames, Hs, Ws, flow_t0, flow_t1, empty0, empty1, H, W,
+                                                             mode, su, sv, tab, acc, out, bgr);
+  RB_CHECK_LAUNCH("frame_expose_resized_kernel");
+  return RB_OK;
 }

@@ -35,6 +35,14 @@ Sintel: ``<out>/<dstype>/<scene>/frameNNNN.flo``; KITTI (no --warm-start): ``<ou
 im2 of every triplet in <data>/tri_testlist.txt is interpolated from im1 and im3 at t = 0.5 (20 iterations, like the
 reference), and the mean PSNR and SSIM of the 8-bit frames against im2 are printed (``Validation Vimeo-90K: PSNR: ...,
 SSIM: ...``) and written with the per-triplet records to ``<--out>/val_vimeo.json`` (no --split test, no --warm-start).
+--dataset gopro scores the --shutter conversion's motion blur on GOPRO_Large_all (raft_b200.gopro): every --stride S
+(8) frame of each 240 fps sequence is an input, converted at its own rate and size with shutter 360 M / S and density S
+(--blur-frames M, 7), each blurred frame scored against np.rint of the mean of its M true frames, the sharp input's
+scores beside it; ``Validation GoPro motion blur (...)`` and ``<--out>/val_gopro.json`` (--split test: <data>/test,
+otherwise <data>/train):
+
+    python infer_raft.py -m val --dataset gopro --data datasets/GOPRO_Large_all --split test --load raft-things.npz
+
 --dataset tapvid scores point tracking on TAP-Vid instead (raft_b200.tapvid):
 
     python infer_raft.py -m val --dataset tapvid --data tapvid_davis.pkl --load raft-things.npz [--query-mode strided]
@@ -62,6 +70,12 @@ the frame interpolated at time s - floor(s) between frames floor(s) and floor(s)
 ``<--out>/frame_<n:06d>.png`` (raft_b200.video):
 
     python infer_raft.py --path film/ --out tv/ --input-fps 24 --fps 60 --load raft-things.npz [--batch 8]
+
+--shutter ANGLE (with --input-fps/--fps) gives the conversion a camera shutter of ANGLE degrees in (0, 360]: every
+output frame is the mean of frames interpolated across its exposure, --shutter-density D (default 16) samples per input
+frame interval, and OUT may be at most IN, so 60p -> 24p does not strobe (raft_b200.video.shutter_schedule):
+
+    python infer_raft.py --path clip60/ --out clip24/ --input-fps 60 --fps 24 --shutter 180 --load raft-things.npz
 
 --scene-cut THRESH (with --path and --interpolate, --input-fps/--fps or --warm-start) scores every consecutive pair on the
 GPU (one minus the intersection of the frames' colour histograms, in [0, 1]); a pair above THRESH is a scene cut.  There
@@ -207,10 +221,14 @@ def parser():
     p.add_argument('--small', action='store_true')
     p.add_argument('--iters', type=int, default=None,
                    help='extension: GRU iterations (test mode: 20 like the reference; -m val: the protocol\'s 32 / 24)')
-    p.add_argument('--dataset', default=None, choices=['sintel', 'kitti', 'vimeo', 'tapvid', 'davis'],
+    p.add_argument('--dataset', default=None, choices=['sintel', 'kitti', 'vimeo', 'tapvid', 'davis', 'gopro'],
                    help='-m val: which dataset --data holds (Sintel / KITTI-2015 training sets: flow; Vimeo-90K '
                         'triplets: frame interpolation; TAP-Vid .pkl file or directory of .pkl shards: point tracking; '
-                        'DAVIS-2017 tree: label propagation)')
+                        'DAVIS-2017 tree: label propagation; GOPRO_Large_all tree: motion blur of a shutter)')
+    p.add_argument('--stride', type=int, default=None, metavar='S',
+                   help='-m val --dataset gopro: every S-th 240 fps frame is an input (default 8)')
+    p.add_argument('--blur-frames', type=int, default=None, metavar='M',
+                   help='-m val --dataset gopro: the true frames averaged per blurred frame, odd and <= S (default 7)')
     p.add_argument('--query-mode', default=None, choices=['first', 'strided'],
                    help="-m val --dataset tapvid: TAP-Vid's query mode (default first: each track from its first visible "
                         "frame; strided: from every 5th frame, tracked forward and backward)")
@@ -240,6 +258,12 @@ def parser():
     p.add_argument('--fps', default=None, metavar='OUT',
                    help='extension, with --path and --input-fps: convert the frames to OUT frames per second (above IN), '
                         'written as <--out>/frame_<n:06d>.png')
+    p.add_argument('--shutter', type=float, default=None, metavar='ANGLE',
+                   help='extension, with --path --input-fps/--fps: a camera shutter of ANGLE degrees in (0, 360]: every '
+                        'output frame is the mean of interpolated sub-frames over its exposure, and OUT may be at most '
+                        'IN (down-conversion)')
+    p.add_argument('--shutter-density', type=int, default=None, metavar='D',
+                   help='extension, with --shutter: samples per input-frame interval (default 16)')
     p.add_argument('--scene-cut', type=float, default=None, metavar='THRESH',
                    help='extension, with --path and one of --interpolate, --input-fps/--fps, --warm-start, '
                         '--stabilize or two or more --propagate maps: a threshold in [0, 1] on the colour-histogram '
@@ -370,6 +394,15 @@ def _temporal_refusals(p, args, flag, what):
 def main(argv=None):
     p = parser()
     args = p.parse_args(argv)
+    if args.shutter_density is not None and args.shutter is None:
+        p.error('--shutter-density goes with --shutter')
+    if args.shutter is not None:
+        if args.fps is None or args.input_fps is None or args.path is None or args.mode != 'test':
+            p.error('--shutter exposes the frames of a frame-rate conversion: it needs --path DIR --input-fps IN --fps OUT')
+        if not 0.0 < args.shutter <= 360.0:
+            p.error(f'--shutter: ANGLE must be in (0, 360] degrees (got {args.shutter})')
+        if args.shutter_density is not None and args.shutter_density < 1:
+            p.error(f'--shutter-density: D must be >= 1 (got {args.shutter_density})')
     if args.consistent_strength is not None and args.consistent is None:
         p.error('--consistent-strength goes with --consistent')
     if args.consistent is not None:
@@ -564,7 +597,7 @@ def main(argv=None):
             if given:
                 p.error(f'--fps writes the frames of one output rate: it cannot be combined with {flag}')
         fps = (_rate(p, '--input-fps', args.input_fps), _rate(p, '--fps', args.fps))
-        if fps[1] <= fps[0]:
+        if fps[1] <= fps[0] and args.shutter is None:
             p.error(f'--fps {args.fps} must exceed --input-fps {args.input_fps}: frame-rate conversion goes up only')
     if args.native_frames:
         if args.keep_size:
@@ -613,6 +646,20 @@ def main(argv=None):
                     'scores the val split)')
         if args.dataset == 'davis' and args.warm_start:
             p.error('--warm-start warm-starts flow validation; DAVIS propagates labels through cold flows')
+    if (args.stride is not None or args.blur_frames is not None) and (args.mode != 'val' or args.dataset != 'gopro'):
+        p.error('--stride and --blur-frames go with -m val --dataset gopro')
+    if args.mode == 'val' and args.dataset == 'gopro':
+        if args.warm_start:
+            p.error('--warm-start warm-starts flow validation; the GoPro protocol runs cold bidirectional flows')
+        from raft_b200.gopro import DEFAULT_BLUR_FRAMES, DEFAULT_STRIDE, check_window
+        try:
+            check_window(DEFAULT_STRIDE if args.stride is None else args.stride,
+                         DEFAULT_BLUR_FRAMES if args.blur_frames is None else args.blur_frames)
+        except ValueError:
+            p.error(f'--stride {args.stride} --blur-frames {args.blur_frames}: S must be >= 1 and M odd with '
+                    '1 <= M <= S')
+        if args.batch < 1:
+            p.error('--batch must be >= 1')
     if args.query_mode is not None and (args.mode != 'val' or args.dataset != 'tapvid'):
         p.error('--query-mode goes with -m val --dataset tapvid')
     if args.keyframe_step is not None:
@@ -621,7 +668,7 @@ def main(argv=None):
         if args.keyframe_step < 1:
             p.error(f'--keyframe-step: the step must be >= 1 (got {args.keyframe_step})')
     if args.mode == 'val':
-        return validate(args)
+        return validate_gopro(args) if args.dataset == 'gopro' else validate(args)
     if args.mode != 'test':
         print(f"mode '{args.mode}' has no implementation in the reference either (infer_raft.py:71-95); nothing to do")
         return 0
@@ -724,7 +771,9 @@ def run_video_interpolate(args, fps=None):
     from raft_b200.video import video_interpolate
     model = _video_model(args)
     files = video_interpolate(model, args.path, args.out, args.interpolate, batch=args.batch, workers=args.workers,
-                              fps=fps, scene_cut=args.scene_cut, native=args.native_frames)
+                              fps=fps, scene_cut=args.scene_cut, native=args.native_frames,
+                              **({} if args.shutter is None else {"shutter": args.shutter,
+                                                                  "density": args.shutter_density or 16}))
     if args.scene_cut is not None:
         files = _print_cuts(*files)
     print(f"{len(files)} frames written under {args.out}")
@@ -915,6 +964,24 @@ def validate(args):
         print(line)
     os.makedirs(args.out, exist_ok=True)
     with open(os.path.join(args.out, f"val_{args.dataset}.json"), "w") as f:
+        json.dump(res, f, indent=1)
+    return 0
+
+
+def validate_gopro(args):
+    """-m val --dataset gopro: raft_b200.gopro.evaluate on --data at the frames' own size (20 iterations), the summary
+    line on stdout and everything in <--out>/val_gopro.json.  --split test scores <data>/test, the default <data>/train."""
+    import json
+    from networks import RAFT
+    from raft_b200.gopro import DEFAULT_BLUR_FRAMES, DEFAULT_STRIDE, evaluate, summary_line
+    model = RAFT.RAFT(None, args, iters=20 if args.iters is None else args.iters, upstream=args.upstream,
+                      mixed_precision=args.mixed_precision).load(args.load)
+    res = evaluate(model, args.data, "test" if args.split == "test" else "train",
+                   DEFAULT_STRIDE if args.stride is None else args.stride,
+                   DEFAULT_BLUR_FRAMES if args.blur_frames is None else args.blur_frames, batch=args.batch)
+    print(summary_line(res))
+    os.makedirs(args.out, exist_ok=True)
+    with open(os.path.join(args.out, "val_gopro.json"), "w") as f:
         json.dump(res, f, indent=1)
     return 0
 

@@ -272,6 +272,18 @@ class RAFT(object):
         return self.engine().interpolate_sequence_at(_as_tensor(frames), items, uint8=uint8, bgr=bgr, native=native)
 
     @torch.no_grad()
+    def motion_blur(self, frames, shutter, fps=None, density=16, cuts=None, native=False):
+        """Extension (frame-rate conversion with a camera shutter): [F,H,W,3] frames (dtypes and sources as for
+        ``forward``) converted from fps[0] to fps[1] -- any ratio, down-conversion included; fps=None keeps the rate and
+        only adds the blur -- each output frame the mean of interpolated sub-frames over an exposure of `shutter` degrees
+        (0, 360] centred on its time, `density` samples per input-frame interval, clamped into the clip and into the shots
+        between the scene-cut pairs `cuts` (Brooks & Barron, CVPR 2019).  One ``forward_sequence_bidirectional`` pass.
+        Returns a fresh [floor((F - 1) fps[1] / fps[0]) + 1,H,W,3] uint8 tensor in the frames' channel order; native as
+        for ``interpolate``.  Bad arguments raise ValueError (RaftEngine.motion_blur)."""
+        return self.engine().motion_blur(_as_tensor(frames), shutter, fps=fps, density=density, cuts=cuts,
+                                         native=native)
+
+    @torch.no_grad()
     def interpolate(self, input_left, input_right, t=0.5, native=False):
         """Extension (the reference computes the flow for frame interpolation and projects it to time t with
         flow_utils.py:166 on the CPU): the frames at time t between left (t = 0) and right (t = 1).  One bidirectional

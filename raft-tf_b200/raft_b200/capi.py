@@ -110,6 +110,10 @@ SIGNATURES = {
                                                _i, _vp]),
     "rb_frame_synthesize_items_resized": (_i, [_vp, _vp, _i, _i, _i, _vp, _vp, _vp, _vp, _i, _i, _vp, _vp, _i, _vp, _i,
                                                _i, _i, _vp]),
+    "rb_frame_expose_items": (_i, [_vp, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _i, _vp, _i, _vp, _i, _vp, _i, _vp, _i, _i,
+                                   _i, _i, _i, _vp]),
+    "rb_frame_expose_items_resized": (_i, [_vp, _i, _i, _i, _vp, _vp, _vp, _vp, _i, _i, _i, _vp, _i, _vp, _i, _vp, _i,
+                                           _vp, _i, _i, _i, _vp]),
     "rb_flow_metrics_workspace_bytes": (_i, [_i, _i, _i, _psz]),
     "rb_flow_metrics": (_i, [_vp, _f, _vp, _vp, _i, _i, _i, _vp, _vp, _vp, _sz, _vp]),
     "rb_frame_metrics_workspace_bytes": (_i, [_i, _i, _i, _psz]),
@@ -134,6 +138,18 @@ SIGNATURES = {
     "rb_encoder_workspace_bytes": (_i, [_i, _i, _i, _i, _psz]),
     "rb_encoder_forward": (_i, [_i, _i, _vp, _vp, _vp, _i, _i, _i, _i, _vp, _sz, _vp]),
 }
+# F32's table rows (include/raft_b200.h)
+RB_EXPOSE_FRAME, RB_EXPOSE_OPEN, RB_EXPOSE_CLOSE = -1, 1, 2
+
+
+class ExposeEntry(C.Structure):  # rb_expose_entry
+    _fields_ = [("slot", C.c_int32), ("sample", C.c_int32), ("t", C.c_float)]
+
+
+class ExposeRow(C.Structure):  # rb_expose_row
+    _fields_ = [(f, C.c_int32) for f in ("first", "count", "m", "acc", "out", "flags")]
+
+
 for _name, (_res, _args) in SIGNATURES.items():
     _fn = getattr(lib, _name)  # AttributeError here = the library does not export a declared symbol
     _fn.restype = _res

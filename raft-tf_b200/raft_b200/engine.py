@@ -142,6 +142,9 @@ class RaftEngine:
         self._capture_stream = None  # CUDA-graph capture stream on this engine's device (run())
         self._cnet_pending = False
         self._range_checked = False  # first forward of this weight set: fp16-range check of the split path's inputs
+        # motion_blur / expose: two fp32 accumulators [2,H,W,3]; an output frame whose samples span calls carries its sum
+        # in one of them, expose_slot the one the next call reads
+        self.expose_acc, self.expose_slot = None, 0
 
     # ---- buffers -------------------------------------------------------------------------------
     def _ensure(self, B: int, H: int, W: int, u8: bool = False, mode: int = FORWARD):
@@ -829,6 +832,101 @@ class RaftEngine:
         return self._synthesize(self.flow_up[:T], self.flow_bw, self.images[:T], self.images[1:], ts, uint8, bgr, ks,
                                 raw=raw)
 
+    @torch.no_grad()
+    def motion_blur(self, frames: torch.Tensor, shutter, fps=None, density: int = 16, cuts=None,
+                    native: bool = False) -> torch.Tensor:
+        """Frame-rate conversion with a camera shutter (F32): [F,H,W,3] frames converted from rate fps[0] to fps[1] (any
+        ratio; fps=None keeps the rate and only blurs), every output frame the mean of m interpolated sub-frames over its
+        exposure of shutter degrees, density samples per input-frame interval (raft_b200.video.shutter_schedule() states
+        the times, the clamping into the clip and into shots at the scene-cut pairs cuts).  One
+        forward_sequence_bidirectional(check=False) pass, then expose()'s chunks.  Returns fresh [N_out,H,W,3] uint8 in
+        the frames' channel order, N_out = floor((F - 1) fps[1] / fps[0]) + 1; native as for interpolate ([N_out,Hs,Ws,3]).
+        m = 1 is interpolate_sequence_at(uint8=True) at the output times byte for byte.  Bad arguments raise ValueError
+        before the pass."""
+        from .video import exposure, shutter_schedule
+        T = _sequence_length(frames)
+        try:
+            fin, fout = (1, 1) if fps is None else fps
+        except (TypeError, ValueError):
+            raise ValueError(f"raft_b200: fps must be None or (input_fps, output_fps) (got {fps!r})") from None
+        (ps,) = shutter_schedule(T + 1, fin, fout, shutter, density, T, () if cuts is None else cuts)
+        return self.expose(frames, ps.samples, exposure(fin, fout, shutter, density)[1], ps.opens, ps.closes,
+                           native=native)
+
+    @torch.no_grad()
+    def expose(self, frames: torch.Tensor, samples, m: int, opens, closes, bgr: bool = False,
+               native: bool = False) -> torch.Tensor:
+        """One pass of motion_blur on [T+1,H,W,3] frames: one forward_sequence_bidirectional(check=False) pass, then the
+        samples (n, i, t) in order (raft_b200.video.ShutterPass with frame indices of these frames: pair i at t, or frame
+        i with t None) of output frames of m samples each.  A frame of opens starts its sum at its first sample here; any
+        other continues the sum an earlier call left in the engine's accumulator.  A frame of closes ends at its last
+        sample here; any other leaves its sum for the next call.  Returns fresh [len(closes),H,W,3] uint8 in closes'
+        order (bgr: channels reversed); native as for interpolate.  The sums carried between calls live in this engine,
+        so while a frame is left open no other motion_blur or expose call may run on the engine: it would overwrite the
+        carried sum (video_interpolate(shutter=) owns its model's engine for the whole sweep)."""
+        self._run_sequence(frames)
+        T = self._shape[0]
+        raw = self.raw if native and self.input_size is not None else None
+        with torch.cuda.device(self.device):
+            return self._expose(self.flow_up[:T], self.flow_bw, samples, m, opens, closes, bgr, raw)
+
+    def _expose(self, flow_fw, flow_bw, samples, m, opens, closes, bgr, raw):
+        """expose()'s work after the pass, in chunks of at most RB_INTERP_MAX_STEPS samples whose items keep the reversal
+        workspace within REVERSE_WS_BOUND: rb_flow_reverse_items of the chunk's items, then one rb_frame_expose_items
+        (_resized with raw) launch.  A frame split by a chunk or pass boundary reads its sum from accumulator
+        expose_slot and a frame left open stores it in the other, which the next chunk then reads."""
+        T, H, W = self._shape[:3]
+        lib, ptr = capi.lib, capi.ptr
+        size = (H, W) if raw is None else self.src_hw
+        out = torch.empty((len(closes),) + size + (3,), dtype=torch.uint8, device=self.device)
+        if self.expose_acc is None or tuple(self.expose_acc.shape[1:3]) != size:
+            self.expose_acc = torch.zeros((2,) + size + (3,), dtype=torch.float32, device=self.device)
+        chunk = RB_INTERP_MAX_STEPS
+        while chunk > 1 and capi.size_query(lib.rb_flow_reverse_multi_workspace_bytes, chunk, 1, H, W) > REVERSE_WS_BOUND:
+            chunk = max(1, chunk // 2)
+        first, last = {}, {}
+        for g, (n, _, _) in enumerate(samples):
+            first.setdefault(n, g)
+            last[n] = g
+        opens, out_row = set(opens), {n: r for r, n in enumerate(closes)}
+        st = capi.stream()
+        for c0 in range(0, len(samples), chunk):
+            part = samples[c0:c0 + chunk]
+            items = [(i, t) for _, i, t in part if t is not None]
+            if items:
+                self._reverse(flow_fw, flow_bw, [t for _, t in items], [i for i, _ in items])
+            entries = (capi.ExposeEntry * len(part))()
+            spans, slot = [], 0  # spans: [n, first entry, count] per output frame of the chunk
+            for e, (n, i, t) in enumerate(part):
+                entries[e] = capi.ExposeEntry(capi.RB_EXPOSE_FRAME, i, 0.0) if t is None else capi.ExposeEntry(slot, i, t)
+                slot += t is not None
+                if spans and spans[-1][0] == n:
+                    spans[-1][2] += 1
+                else:
+                    spans.append([n, e, 1])
+            rows = (capi.ExposeRow * len(spans))()
+            carry = self.expose_slot
+            for r, (n, e, count) in enumerate(spans):
+                opened = n in opens and first[n] == c0 + e
+                closed = n in out_row and last[n] == c0 + e + count - 1
+                acc = self.expose_slot
+                if not closed and not (not opened and r == 0):  # left open for the next chunk: the other accumulator
+                    acc = carry = 1 - self.expose_slot
+                flags = capi.RB_EXPOSE_OPEN * opened | capi.RB_EXPOSE_CLOSE * closed
+                rows[r] = capi.ExposeRow(e, count, m, acc, out_row.get(n, 0), flags)
+            self.expose_slot = carry
+            flows = ((ptr(self.flow_t[0]), ptr(self.flow_t[1]), ptr(self.empty_t[0, 0]), ptr(self.empty_t[0, 1]))
+                     if items else (None,) * 4)
+            table = (slot, entries, len(part), rows, len(spans), ptr(self.expose_acc), 2, ptr(out), len(closes), int(bgr),
+                     T)
+            if raw is None:
+                capi.check(lib.rb_frame_expose_items(ptr(self.images), self.Hp, self.Wp, self.pad[0], self.pad[2], *flows,
+                                                     *table, H, W, st))
+            else:
+                capi.check(lib.rb_frame_expose_items_resized(ptr(raw), int(raw.dtype == torch.uint8), *size, *flows, H,
+                                                             W, *table, st))
+        return out
+
     def _native_frames(self, native, rows0, rows1):
         """The raw frames a native blend reads, rows rows0 and rows1 of the staging buffer at the frames' own size, or
         None: without native, and without input_size, where the network already runs at the frames' own size (and fp32
@@ -864,13 +962,10 @@ class RaftEngine:
         B = self._shape[0]
         self._reverse_and_blend(self.flow_up[:B], self.flow_up[B:], self.images[:B], self.images[B:], [t], out[None])
 
-    def _reverse_and_blend(self, flow_fw, flow_bw, frames0, frames1, ts, out, uint8=False, bgr=False, samples=None,
-                           raw=None):
-        """One chunk: the reversal of flow_fw by s t and of flow_bw by s (1 - t) for the n = len(ts) times, then the blend
-        into out -- rb_flow_reverse_multi and rb_frame_synthesize_pairs on all B pairs into out [n,B,H,W,3], or with
-        samples rb_flow_reverse_items and rb_frame_synthesize_items on pair samples[i] at ts[i] into out [n,H,W,3].  With
-        raw = (frames0, frames1) at the frames' own Hs x Ws, the *_resized blends of those into out [n,(B,)Hs,Ws,3].  The
-        reversal buffers are (re)allocated for the n B (n) samples."""
+    def _reverse(self, flow_fw, flow_bw, ts, samples=None):
+        """The reversals of one chunk of n = len(ts) times: flow_fw by s t and flow_bw by s (1 - t) (s = flow_scale) into
+        flow_t[0 | 1] and empty_t[:, 0 | 1], by rb_flow_reverse_multi on all B pairs, or with samples by
+        rb_flow_reverse_items on pair samples[i].  The reversal buffers are (re)allocated for the n B (n) samples."""
         B, H, W = self._shape[:3]
         n, s, d = len(ts), self.flow_scale, self.device
         per_t = B if samples is None else 1
@@ -891,6 +986,18 @@ class RaftEngine:
             else:
                 capi.check(lib.rb_flow_reverse_items(ptr(flow), B, _ints(samples), _floats(steps), n, *bufs, H, W,
                                                      ptr(self.rev_ws), self.rev_ws_bytes, st))
+
+    def _reverse_and_blend(self, flow_fw, flow_bw, frames0, frames1, ts, out, uint8=False, bgr=False, samples=None,
+                           raw=None):
+        """One chunk: the reversal of flow_fw by s t and of flow_bw by s (1 - t) for the n = len(ts) times, then the blend
+        into out -- rb_flow_reverse_multi and rb_frame_synthesize_pairs on all B pairs into out [n,B,H,W,3], or with
+        samples rb_flow_reverse_items and rb_frame_synthesize_items on pair samples[i] at ts[i] into out [n,H,W,3].  With
+        raw = (frames0, frames1) at the frames' own Hs x Ws, the *_resized blends of those into out [n,(B,)Hs,Ws,3]."""
+        B, H, W = self._shape[:3]
+        n = len(ts)
+        lib, ptr = capi.lib, capi.ptr
+        st = capi.stream()
+        self._reverse(flow_fw, flow_bw, ts, samples)
         if raw is not None:
             Hs, Ws = self.src_hw
             frames = (ptr(raw[0]), ptr(raw[1]), int(raw[0].dtype == torch.uint8), Hs, Ws, ptr(self.flow_t[0]),

@@ -98,6 +98,32 @@ def write_vimeo_tree(root: str, sizes, seed: int = 4000, shift: int = 4):
     return entries
 
 
+def write_highfps_tree(root: str, split: str, sequences, H: int, W: int, seed: int = 6000, speed=(1, 0)):
+    """A dataset in GOPRO_Large_all's layout under root: <root>/<split>/<name>/<i:06d>.png for each (name, n_frames) of
+    sequences, 8-bit crops of one smooth seeded texture that pans by speed = (dx, dy) whole pixels per frame, as a
+    240 fps camera would see it.  Returns {name: [F,H,W,3] uint8 BGR frames as written}."""
+    import os
+
+    import cv2
+    rng = np.random.default_rng(seed)
+    out = {}
+    for name, n in sequences:
+        dx, dy = speed
+        m = 2 + max(abs(dx), abs(dy)) * n
+        base = rng.random((H + 2 * m, W + 2 * m, 3), dtype=np.float32)
+        base = 0.6 * _blur(base, 3.0) + 0.4 * _blur(base, 1.0)
+        base = np.round(255 * (base - base.min()) / max(float(base.max() - base.min()), 1e-6)).astype(np.uint8)
+        d = os.path.join(root, split, name)
+        os.makedirs(d, exist_ok=True)
+        frames = []
+        for i in range(n):
+            y0, x0 = m + i * dy, m + i * dx
+            frames.append(base[y0:y0 + H, x0:x0 + W])
+            cv2.imwrite(os.path.join(d, f"{i:06d}.png"), frames[-1])
+        out[name] = np.stack(frames)
+    return out
+
+
 # PASCAL VOC's first colours, as DAVIS's annotations use them
 DAVIS_PALETTE = np.array([[0, 0, 0], [128, 0, 0], [0, 128, 0], [128, 128, 0], [0, 0, 128], [128, 0, 128],
                           [0, 128, 128], [128, 128, 128], [64, 0, 0], [192, 0, 0], [64, 128, 0], [192, 128, 0],

@@ -62,6 +62,7 @@ its chain (cold_start()) and stabilization restarts the camera path.  Without a 
 from __future__ import annotations
 
 import glob
+import math
 import os
 import threading
 from collections import namedtuple
@@ -80,6 +81,10 @@ Pass = namedtuple("Pass", "carry frames pairs")
 # one interpolate_sequence_at call of frame-rate conversion (fps_schedule()): the frames and pairs of its Pass, the output
 # frames it interpolates as (n, k, t) (output index, pair, time) and the input frames it copies as (n, i)
 FpsPass = namedtuple("FpsPass", "frames pairs items copies")
+# one pass of frame-rate conversion with a shutter (shutter_schedule()): the frames and pairs of its Pass, its samples in
+# run order as (n, i, t) -- output frame n's blend of pair i at time t, or with t None input frame i -- and the output
+# frames whose first / last sample it runs
+ShutterPass = namedtuple("ShutterPass", "frames pairs samples opens closes")
 
 
 def list_frames(frames):
@@ -174,6 +179,74 @@ def fps_schedule(n_frames, input_fps, output_fps, batch):
         else:
             items[k // T].append((n, k, float(s - k)))
     return [FpsPass(p.frames, p.pairs, i, c) for p, i, c in zip(passes, items, copies)]
+
+
+def check_shutter(shutter):
+    """A shutter angle in degrees as a Fraction in (0, 360] (parse_rate()'s parsing: a float by its shortest repr).  360 is
+    an exposure as long as the output frame interval, 180 half of it.  Anything else raises ValueError."""
+    try:
+        a = Fraction(repr(shutter)) if isinstance(shutter, float) else Fraction(shutter)
+    except (TypeError, ValueError, ZeroDivisionError, OverflowError):
+        a = None
+    if isinstance(shutter, bool) or a is None or not 0 < a <= 360:
+        raise ValueError(f"video: the shutter angle must be a number of degrees in (0, 360] (got {shutter!r})")
+    return a
+
+
+def check_density(density):
+    """The samples per input-frame interval of a shutter as an int >= 1.  Anything else raises ValueError."""
+    try:
+        ok = not isinstance(density, bool) and int(density) == density and density >= 1
+    except (TypeError, ValueError, OverflowError):
+        ok = False
+    if not ok:
+        raise ValueError(f"video: the shutter density must be an integer >= 1 (got {density!r})")
+    return int(density)
+
+
+def exposure(input_fps, output_fps, shutter, density):
+    """The exposure of one output frame in input frames and its sample count: (e, m) = ((shutter / 360) input_fps /
+    output_fps as a Fraction, max(1, ceil(density e)))."""
+    e = check_shutter(shutter) / 360 * parse_rate(input_fps) / parse_rate(output_fps)
+    return e, max(1, math.ceil(check_density(density) * e))
+
+
+def shot_range(i, last, cuts):
+    """The first and last frame of the shot holding frame i: a cut pair k ends a shot at frame k."""
+    return (max([c + 1 for c in cuts if c < i], default=0), min([c for c in cuts if c >= i], default=last))
+
+
+def shutter_schedule(n_frames, input_fps, output_fps, shutter, density, batch, cuts=()):
+    """The passes of video_interpolate(fps=(input_fps, output_fps), shutter=, density=) over n_frames frames:
+    interp_schedule()'s passes, each with the samples it runs.  Output frame n sits at s = n input_fps / output_fps, n = 0
+    .. floor((n_frames - 1) output_fps / input_fps), at any rate ratio (down-conversion and equal rates included).  Its
+    exposure [s - e/2, s + e/2] holds m samples (exposure()), u_j = s - e/2 + (j + 1/2) e / m, exact in Fractions, each
+    clamped into the frames [a, b] of the shot holding s (shot_range(); inside a cut pair k, the shot of cut_copy(k, t)).
+    An integer u_j is input frame u_j, run by the pass that holds pair min(u_j, n_frames - 2); any other is the item
+    (k, t) = (floor(u_j), float(u_j - k)) of the pass that holds pair k.  A frame's samples run in order, so they may
+    span passes.  Returns a list of ShutterPass(frames, pairs, samples, opens, closes): samples (n, i, t) with global
+    frame indices in run order (t None: input frame i, else pair i at t), opens / closes the output frames whose first /
+    last sample the pass runs.  cuts: the scene-cut pairs (check_cuts())."""
+    fin, fout = parse_rate(input_fps), parse_rate(output_fps)
+    e, m = exposure(fin, fout, shutter, density)
+    passes = interp_schedule(n_frames, batch)
+    T, last = int(batch), int(n_frames) - 1
+    cuts = check_cuts(cuts, n_frames, "shutter_schedule")
+    samples, opens, closes = [[] for _ in passes], [[] for _ in passes], [[] for _ in passes]
+    for n in range(last * fout // fin + 1):
+        s = n * fin / fout
+        k = math.floor(s)
+        a, b = shot_range(cut_copy(k, s - k) if k in cuts and s != k else k, last, cuts)
+        for j in range(m):
+            u = min(max(s - e / 2 + (j + Fraction(1, 2)) * e / m, Fraction(a)), Fraction(b))
+            i = math.floor(u)
+            p = min(i, last - 1) // T if u == i else i // T
+            samples[p].append((n, i, None if u == i else float(u - i)))
+            if j == 0:
+                opens[p].append(n)
+            if j == m - 1:
+                closes[p].append(n)
+    return [ShutterPass(p.frames, p.pairs, sm, o, c) for p, sm, o, c in zip(passes, samples, opens, closes)]
 
 
 def check_scene_cut(scene_cut):
@@ -445,7 +518,8 @@ def video(model, frames, out, batch=8, workers=4, warm_start=False, flo=None, np
     return written if thr is None else (written, cuts)
 
 
-def video_interpolate(model, frames, out, ts=None, batch=8, workers=4, fps=None, scene_cut=None, native=False):
+def video_interpolate(model, frames, out, ts=None, batch=8, workers=4, fps=None, scene_cut=None, native=False,
+                      shutter=None, density=16):
     """Frame-rate up-conversion with a loaded networks.RAFT.RAFT model of the frames (a directory's sorted *.png / *.jpg,
     or a list of paths, all of one size), written as one numbered sequence <out>/frame_<n:06d>.png.  Give exactly one of:
 
@@ -471,6 +545,13 @@ def video_interpolate(model, frames, out, ts=None, batch=8, workers=4, fps=None,
     scene_cut.  Every frame of a cut pair at time t is then a copy of the nearer input frame (cut_copy(): k for t <= 0.5,
     else k + 1), written like the input frames; only the other pairs' frames are interpolated, and a pass with none of
     them makes no engine call.  The other files are the bytes of the run without scene_cut.
+
+    shutter (degrees in (0, 360], with fps; any rate ratio, down-conversion included) gives the conversion a camera
+    shutter: every output frame is the mean of the sub-frames over its exposure, density samples per input-frame
+    interval (shutter_schedule(), RaftEngine.expose), in one sweep of interp_schedule()'s passes.  The fp32 sums of the
+    output frames whose exposure spans two passes stay on the GPU between them, so the files do not depend on batch or
+    workers: they are the frames of model.motion_blur on the whole clip, byte for byte (BGR).  With scene_cut a first
+    sweep decodes and scores every pair (no flow), so the exposures are clamped at every cut before any is summed.
     Returns the written paths in output order; with scene_cut the tuple (paths, cuts), cuts the increasing cut pairs."""
     import cv2
     from networks.utils import scene_cut_scores
@@ -480,6 +561,10 @@ def video_interpolate(model, frames, out, ts=None, batch=8, workers=4, fps=None,
         raise ValueError("video_interpolate: give the times ts or the rates fps = (input_fps, output_fps), exactly one")
     batch, workers = int(batch), _workers(workers)
     thr = None if scene_cut is None else check_scene_cut(scene_cut)
+    if shutter is not None:
+        if fps is None:
+            raise ValueError("video_interpolate: a shutter needs the rates fps = (input_fps, output_fps)")
+        return _video_shutter(model, paths, out, fps, shutter, density, batch, workers, thr, native)
     last = len(paths) - 1
     if fps is None:
         ts = check_times(ts)
@@ -548,6 +633,58 @@ def video_interpolate(model, frames, out, ts=None, batch=8, workers=4, fps=None,
                 copies = ps.copies + cut_copies
             copies = [(n, imgs[i - first]) for n, i in copies]
             pipe.emit(partial(write, made=made, copies=copies), rows, frames=res)
+    paths = [name(n) for n in range(n_out)]
+    return paths if thr is None else (paths, cuts)
+
+
+def _video_shutter(model, paths, out, fps, shutter, density, batch, workers, thr, native):
+    """video_interpolate(fps=, shutter=, density=) after its argument checks: the optional scoring sweep, then one sweep of
+    shutter_schedule()'s passes, each one RaftEngine.expose call whose closed frames are written."""
+    import cv2
+    from networks.utils import scene_cut_scores
+
+    try:
+        fin, fout = fps
+    except (TypeError, ValueError):
+        raise ValueError(f"video_interpolate: fps must be (input_fps, output_fps) (got {fps!r})") from None
+    _, m = exposure(fin, fout, shutter, density)
+    n_out = (len(paths) - 1) * parse_rate(fout) // parse_rate(fin) + 1
+    out = os.fspath(out)
+    os.makedirs(out, exist_ok=True)
+    engine = model.engine()
+    rgb, dev = bool(model.upstream), engine.device
+
+    def name(n):
+        return os.path.join(out, f"frame_{n:06d}.png")
+
+    def write(slot, made):  # writer thread: the frames one pass closed, once its copies have landed
+        if slot is None:
+            return
+        slot.event.synchronize()
+        for n, r in made:
+            if not cv2.imwrite(name(n), slot.frames[r].numpy()):
+                raise OSError(f"cannot write {name(n)}")
+
+    cuts = []
+    if thr is not None:  # every cut is known before any exposure is summed
+        on_dev = None
+        with _Pipeline(paths, interp_schedule(len(paths), batch), rgb, batch, workers, dev) as pipe:
+            for _, ps, _, src in pipe:
+                if on_dev is None:
+                    on_dev = torch.empty(src.shape, dtype=torch.uint8, device=dev)
+                on_dev.copy_(src, non_blocking=True)
+                cuts += pass_cuts(ps.pairs, scene_cut_scores(on_dev).cpu(), thr)
+                pipe.emit(lambda slot: None)
+    passes = shutter_schedule(len(paths), fin, fout, shutter, density, batch, cuts)
+    rows = max(1, max(len(p.closes) for p in passes))
+    with _Pipeline(paths, passes, rgb, batch, workers, dev) as pipe:
+        for _, ps, _, src in pipe:
+            first = ps.frames[0]
+            res = None
+            if ps.samples:
+                res = engine.expose(src, [(n, i - first, t) for n, i, t in ps.samples], m, ps.opens, ps.closes,
+                                    bgr=rgb, native=native)
+            pipe.emit(partial(write, made=[(n, r) for r, n in enumerate(ps.closes)]), rows, frames=res)
     paths = [name(n) for n in range(n_out)]
     return paths if thr is None else (paths, cuts)
 
