@@ -811,6 +811,65 @@ int rb_frame_expose_items_resized(const void* frames, int frames_u8, int Hs, int
                                   int n_rows, float* acc, int n_acc, uint8_t* out, int n_out, int bgr, int B,
                                   void* stream);
 
+/* ---- F34: camera homography -- a robust homography fit of each frame pair's camera motion to its flow --------------
+ * flow [B,Hn,Wn,2] fp32 and occ [B,Hn,Wn] uint8 of B fields (forward or backward) whose frames are Hs x Ws; sim_params
+ * [B,4] fp64 and sim_flags [B] uint8, rb_global_motion's outputs for the same fields.  Points as in F22: network pixel
+ * (i, j) is p = ((j+0.5) Ws/Wn - 0.5, (i+0.5) Hs/Hn - 0.5) - ((Ws-1)/2, (Hs-1)/2) and its target q = p + flow_scale
+ * (u Ws/Wn, v Hs/Hn), both divided by L = max(Ws, Hs) / 2: (x, y) and (qx, qy).  The model H = [[h1, h2, h3], [h4, h5,
+ * h6], [h7, h8, 1]] maps (x, y) to pi(H (x, y, 1)), pi(X, Y, z) = (X/z, Y/z).  Each point gives the DLT rows
+ * a_x = (x, y, 1, 0, 0, 0, -x qx, -y qx) with right-hand side qx and a_y = (0, 0, 0, x, y, 1, -x qy, -y qy) with qy.
+ * Each of `rounds` rounds forms the 45 fp64 sums (RB_HOMOGRAPHY_SUMS, in this order) S = sum w, the upper triangle of
+ * sum w (a_x a_x^T + a_y a_y^T) row by row ((0,0), (0,1), ..., (0,7), (1,1), ..., (7,7)), and the 8 entries of
+ * sum w (a_x qx + a_y qy), and solves the 8 x 8 system by Cholesky in fp64 in thread 0 of the pair's block, in a fixed
+ * order.  A pixel counts where occ == 0 and its flow is finite, with w = 1 / (1 + (r / cauchy_c)^2) / z^2: r = |q -
+ * pi(H p)| under the previous round's H in network pixels (x scaled by Wn/Ws, y by Hn/Hs, as F22), z = h7 x + h8 y + 1
+ * (the iteratively reweighted DLT); z <= 0 or a non-finite residual gives w = 0.  Round 0's previous H is the
+ * similarity [[a, -b, tx/L], [b, a, ty/L], [0, 0, 1]].  The reciprocals of z and of the Cauchy term are the hardware's
+ * approximate reciprocal refined by two Newton steps (within an ulp).  Outputs H [B,9] fp64 row-major in the normalised
+ * coordinates (h33 = 1) and flags [B] uint8: 0 homography; 1 singular in some round (S = 0, a Cholesky pivot <= 1e-12 x
+ * its diagonal entry, or a non-finite solution), the field keeps the initial similarity from then on; 2 the similarity
+ * was flagged unreliable, H is the identity.  sums (nullable) [B,45] fp64, the last round's.  Reduction as F22: fixed
+ * 4096-pixel chunks (a shuffle tree per warp, then the warps in order) into the workspace
+ * (rb_homography_motion_workspace_bytes), then one per-pair launch that adds the chunks in order, so a field's bits
+ * depend neither on B nor on its place in the batch; no allocation, no atomics.  Null pointers (sums excepted),
+ * B/Hn/Wn/Hs/Ws <= 0, B > 65535, flow_scale or cauchy_c <= 0 or non-finite, rounds outside [1,
+ * RB_HOMOGRAPHY_MAX_ROUNDS] and a workspace that is too small -> RB_ERR_* before any CUDA call.
+ * ---- F35: motion evidence and segmentation ----
+ * rb_motion_evidence: T frame pairs of F = T + 1 frames; flow_fw, flow_bw [T,Hn,Wn,2] fp32 (flow_fw[k] frame k -> k+1,
+ * flow_bw[k] k+1 -> k), occ_fw, occ_bw [T,Hn,Wn] uint8; H [2T,9] and flags [2T] F34's fit of the 2T fields as one batch,
+ * the forward fields first; cuts (nullable) [T] uint8, non-zero for a scene-cut pair.  evidence [F,Hn,Wn,2] fp32 = (N, C)
+ * per frame and network pixel: from +0, the forward field of pair t, then the backward field of pair t - 1, each where
+ * occ == 0, the flow is finite, the field's flag <= 1 and the pair is not a cut, adds e = r^2 / (r^2 + tau^2) to N and 1
+ * to C.  r is F34's residual under the field's H in network pixels, in fp64 with every operation rounded on its own
+ * (cv2's pixel centre, (p * (1/L)), X = (h1 x + h2 y) + h3, X / z, ((X/z - qx) L) Wn/Ws ...), r^2 = dx^2 + dy^2 rounded
+ * once to fp32; e = 1 where z <= 0 or r^2 is not finite.  e >= 0.5 exactly when r >= tau.  One thread per network pixel.
+ * rb_motion_segment: evidence [F,Hn,Wn,2] as above; flow_fw, flow_bw [F-1,Hn,Wn,2]; rows [n_rows,3] int32 in device
+ * memory, row r = (t, nf, nb) (raft_b200.inpaint.inpaint_rows' table).  Per frame pixel (x, y) of row r: p0 =
+ * rb_denoise_merge's pixel-centre map; (num, den) = the bilinear sample (fb_sample.cuh's bilerp_at / bilerp1) of
+ * (N, C) of frame t at p0; the forward side then takes up to min(nf, F-1-t) steps of rb_denoise_merge's chain, stopping
+ * at the first step that leaves the grid or fails the F5 test, and each passing step adds the bilinear samples of the
+ * frame reached at the position reached; the backward side mirrors it (up to min(nb, t) steps).  Order: frame t, the
+ * forward steps, the backward steps.  mask [n_rows,Hs,Ws] uint8 = 1 where den > 0 and 2 num >= den, else 0; status
+ * [n_rows,Hs,Ws] uint8 = 0, or 1 where den = 0 (no evidence).  A row whose t lies outside [0, F) is absent (mask 0,
+ * status 1); nf / nb are clamped into [0, RB_MOTION_SEG_MAX_WINDOW] and the clip.  Every fp32 operation is rounded on
+ * its own; no atomics, no allocation.  Null pointers (cuts excepted; the flows of rb_motion_segment may be null when
+ * F = 1), non-positive shapes, a frame of >= 2^31 pixels, flow_scale or tau <= 0 or non-finite and negative or
+ * non-finite alphas -> RB_ERR_* before any CUDA call. */
+#define RB_HOMOGRAPHY_SUMS 45
+#define RB_HOMOGRAPHY_MAX_ROUNDS 32
+#define RB_MOTION_SEG_TAU 1.0f
+#define RB_MOTION_SEG_MAX_WINDOW 16
+int rb_homography_motion_workspace_bytes(int B, int Hn, int Wn, size_t* bytes);
+int rb_homography_motion(const float* flow, const uint8_t* occ, int B, int Hn, int Wn, int Hs, int Ws, float flow_scale,
+                         const double* sim_params, const uint8_t* sim_flags, int rounds, double cauchy_c, double* H,
+                         uint8_t* flags, double* sums, void* workspace, size_t workspace_bytes, void* stream);
+int rb_motion_evidence(const float* flow_fw, const float* flow_bw, const uint8_t* occ_fw, const uint8_t* occ_bw,
+                       const double* H, const uint8_t* flags, const uint8_t* cuts, int T, int Hn, int Wn, int Hs, int Ws,
+                       float flow_scale, float tau, float* evidence, void* stream);
+int rb_motion_segment(const float* evidence, int F, int Hn, int Wn, const float* flow_fw, const float* flow_bw, int Hs,
+                      int Ws, float flow_scale, float alpha1, float alpha2, const int32_t* rows, int n_rows,
+                      uint8_t* mask, uint8_t* status, void* stream);
+
 /* ---- F9: end-point-error metrics (upstream RAFT's evaluate.py validate_sintel / validate_kitti) ---------------------
  * flow, gt: [B,H,W,2] fp32; valid: [B,H,W] uint8, nonzero = the pixel counts (NULL: every pixel counts).  Per pixel,
  * every operation rounded on its own (no FMA contraction), so the values equal upstream's torch expressions bit for bit:

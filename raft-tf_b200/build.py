@@ -9,7 +9,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 SOURCES = ["capi.cu", "corr.cu", "conv_simt.cu", "conv_tc.cu", "conv_api.cu", "gemm_tc.cu", "update.cu", "upsample.cu",
            "encoder.cu", "frames.cu", "consistency.cu", "interp.cu", "resize.cu", "metrics.cu", "warm.cu",
            "flowviz.cu", "scenecut.cu", "track.cu", "propagate.cu", "stabilize.cu",
-           "inpaint.cu", "stabfill.cu", "denoise.cu", "temporal.cu"]
+           "inpaint.cu", "stabfill.cu", "denoise.cu", "temporal.cu", "motionseg.cu"]
 LIB = os.path.join(HERE, "lib", "libraft_b200.so")
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 

@@ -141,6 +141,19 @@ printed:
 
     python infer_raft.py --path noisy/ --out clean/ --denoise 20 --load raft-things.npz [--batch 8]
 
+--path DIR --segment-motion writes <--out>/mask_<i:06d>.png, 1 where a pixel moves on its own rather than with the
+camera: each pair's camera homography is fitted robustly to its flow, each pixel's residual r (network pixels) gives
+evidence r^2 / (r^2 + tau^2), and the evidence is averaged along the flow, at most --segment-window N (default 3)
+frames each way, never across a --scene-cut and only while the forward-backward test holds (raft_b200.video.
+video_segment_motion).  --segment-tau PX sets tau (default 1 network pixel; not tuned).  The masks are palette PNGs
+that --inpaint reads as they are; <--out>/homographies.npy holds the forward pairs' homographies in the frames' pixels:
+
+    python infer_raft.py --path frames/ --out masks/ --segment-motion --load raft-things.npz [--batch 8]
+
+-m val --dataset davis --segment-motion scores it on DAVIS-2016's val sequences, unsupervised (raft_b200.davis.
+evaluate_motion): the flow at the frames' own size with 20 iterations, the union of the object labels as ground truth,
+J&F printed (``Validation DAVIS-2016 motion segmentation (val): ...``) and written to ``<--out>/val_davis_motion.json``.
+
 --path ORIG --consistent PROC_DIR --consistent-strength L makes per-frame processed frames (PROC_DIR: as many as ORIG,
 the same size) temporally consistent, guided by the flow of the original frames (Bonneel et al. 2015;
 raft_b200.video.video_consistent); frames after a --scene-cut restart from the processed frame.  E_warp of the
@@ -333,6 +346,16 @@ def parser():
     p.add_argument('--denoise-window', type=int, default=None, metavar='N',
                    help='extension, with --denoise: the frames each side may look ahead or back (default 3, at most '
                         '16; not tuned)')
+    p.add_argument('--segment-motion', action='store_true',
+                   help="extension, with --path: write <--out>/mask_<i:06d>.png, 1 where a pixel moves on its own "
+                        "rather than with the camera, and <--out>/homographies.npy.  With -m val --dataset davis: "
+                        "score it on DAVIS-2016 val (unsupervised)")
+    p.add_argument('--segment-window', type=int, default=None, metavar='N',
+                   help='extension, with --segment-motion: the frames each side may look ahead or back (default 3, at '
+                        'most 16; not tuned)')
+    p.add_argument('--segment-tau', type=float, default=None, metavar='PX',
+                   help='extension, with --segment-motion: the residual in network pixels at which a field votes 1/2 '
+                        'for motion (default 1; not tuned)')
     p.add_argument('--consistent', default=None, metavar='PROC_DIR',
                    help="extension, with --path: make the per-frame processed frames of PROC_DIR (as many as --path, "
                         "the same size) temporally consistent, guided by the flow of the --path frames (needs "
@@ -419,6 +442,10 @@ def main(argv=None):
     if args.warp_error is not None:
         _temporal_refusals(p, args, '--warp-error', 'scores a video')
         return run_warp_error(args)
+    if args.segment_motion:
+        return _segment_motion(p, args)
+    if args.segment_window is not None or args.segment_tau is not None:
+        p.error('--segment-window and --segment-tau go with --segment-motion')
     if args.denoise is not None:
         sigma = args.denoise
         if sigma != 'auto':
@@ -878,6 +905,78 @@ def run_denoise(args, sigma):
     files, _ = video_denoise(model, args.path, args.out, sigma, window=args.denoise_window, batch=args.batch,
                              workers=args.workers, scene_cut=args.scene_cut)
     print(f"{len(files)} denoised frames written under {args.out}")
+    return 0
+
+
+def _segment_motion(p, args):
+    """--segment-motion: the checks, then -m val --dataset davis (validate_motion) or --path (run_segment_motion)."""
+    from raft_b200.motionseg import MAX_WINDOW, check_tau
+    if args.segment_window is not None and not 0 <= args.segment_window <= MAX_WINDOW:
+        p.error(f'--segment-window: N must be in [0, {MAX_WINDOW}] (got {args.segment_window})')
+    if args.segment_tau is not None:
+        try:
+            check_tau(args.segment_tau)
+        except ValueError:
+            p.error(f'--segment-tau: PX must be a finite number > 0 (got {args.segment_tau})')
+    others = (('--denoise', args.denoise is not None), ('--inpaint', args.inpaint is not None),
+              ('--stabilize', args.stabilize is not None), ('--stabilize-fill', args.stabilize_fill),
+              ('--propagate', args.propagate is not None), ('--track', args.track is not None),
+              ('--track-grid', args.track_grid is not None), ('--interpolate', args.interpolate),
+              ('--fps', args.fps), ('--input-fps', args.input_fps), ('--warm-start', args.warm_start),
+              ('--bidirectional', args.bidirectional), ('--native-flow', args.native_flow),
+              ('--native-frames', args.native_frames), ('--flo', args.flo), ('--npy', args.npy),
+              ('--keyframe-step', args.keyframe_step is not None), ('--consistent', args.consistent is not None),
+              ('--warp-error', args.warp_error is not None))
+    if args.mode == 'val':
+        if args.dataset != 'davis':
+            p.error('-m val --segment-motion scores motion segmentation on DAVIS-2016 val: it needs --dataset davis')
+        if args.split == 'test':
+            p.error('--split test writes a flow submission; -m val --segment-motion scores the val sequences')
+        for other, given in others + (('--scene-cut', args.scene_cut is not None), ('--path', args.path is not None)):
+            if given:
+                p.error(f'-m val --segment-motion cannot be combined with {other}')
+        if not args.data:
+            p.error('-m val needs --data <dataset root>')
+        return validate_motion(args)
+    if args.path is None or args.mode != 'test':
+        p.error('--segment-motion segments a frame directory: it needs --path DIR (or -m val --dataset davis)')
+    for other, given in others:
+        if given:
+            p.error(f'--segment-motion writes masks: it cannot be combined with {other}')
+    if args.scene_cut is not None and not 0.0 <= args.scene_cut <= 1.0:
+        p.error(f'--scene-cut: {args.scene_cut} is not a threshold in [0, 1]')
+    if args.flow_size is not None and args.keep_size:
+        p.error('--flow-size sets the size frames are resized to; --keep-size runs them at their own size')
+    if args.batch < 1 or args.workers < 0:
+        p.error('--path needs --batch >= 1 and --workers >= 0')
+    return run_segment_motion(args)
+
+
+def run_segment_motion(args):
+    """--path --segment-motion: raft_b200.video.video_segment_motion over the frames of --path, the flow at 432x1024 (or
+    --flow-size) like test mode (or the frames' own size with --keep-size), the masks written at the frames' own size."""
+    from raft_b200.video import video_segment_motion
+    model = _video_model(args)
+    files, _ = video_segment_motion(model, args.path, args.out, window=args.segment_window, tau=args.segment_tau,
+                                    batch=args.batch, workers=args.workers, scene_cut=args.scene_cut)
+    print(f"{len(files)} motion masks written under {args.out}")
+    return 0
+
+
+def validate_motion(args):
+    """-m val --dataset davis --segment-motion: raft_b200.davis.evaluate_motion on --data, the summary line on stdout,
+    the per-sequence records in <--out>/val_davis_motion.json, the masks in DAVIS's results layout under
+    <--out>/davis_motion."""
+    import json
+    from networks import RAFT
+    from raft_b200.davis import evaluate_motion, motion_summary
+    model = RAFT.RAFT(None, args, upstream=args.upstream, mixed_precision=args.mixed_precision).load(args.load)
+    res = evaluate_motion(model, args.data, window=args.segment_window, tau=args.segment_tau, batch=args.batch,
+                          iters=args.iters, masks_out=os.path.join(args.out, 'davis_motion'))
+    print(motion_summary(res))
+    os.makedirs(args.out, exist_ok=True)
+    with open(os.path.join(args.out, "val_davis_motion.json"), "w") as f:
+        json.dump(res, f, indent=1)
     return 0
 
 

@@ -232,6 +232,18 @@ class RAFT(object):
         return self.engine().denoise(_as_tensor(frames), sigma, window=window, cuts=cuts)
 
     @torch.no_grad()
+    def segment_motion(self, frames, window=None, tau=None, cuts=None):
+        """Extension (motion segmentation): the pixels of [F,Hs,Ws,3] uint8 frames (sources as for ``forward``) whose
+        motion departs from the camera's.  One ``forward_sequence_bidirectional`` pass with the occlusion check; each
+        pair's camera homography fitted robustly to both of its flows; per pixel the evidence r^2 / (r^2 + tau^2) of
+        its residual r (network pixels, default raft_b200.motionseg.TAU), summed over its own frame and the frames its
+        chain reaches through the forward-backward test, up to `window` frames each way (default DEFAULT_WINDOW), never
+        across a scene-cut pair of cuts (RaftEngine.segment_motion).  Returns fresh (masks [F,Hs,Ws] uint8 in {0, 1},
+        status [F,Hs,Ws] uint8, homographies [F-1,3,3] fp64 in the frames' own pixels).  A bad window, tau or cuts
+        raise ValueError before the pass."""
+        return self.engine().segment_motion(_as_tensor(frames), window=window, tau=tau, cuts=cuts)
+
+    @torch.no_grad()
     def consistent(self, frames, processed, strength, cuts=None):
         """Extension (temporal consistency): per-frame processed video made temporally consistent, guided by the flow of
         the original frames (Bonneel et al., SIGGRAPH Asia 2015).  frames, processed: [F,Hs,Ws,3] uint8 (sources as for

@@ -578,6 +578,125 @@ def global_motion(flow_fw, occ_fw, frame_hw, flow_scale=1.0, rounds=None, cauchy
     return out + (sums,) if return_sums else out
 
 
+def homography_motion(flow_fw, occ_fw, frame_hw, params, reliable, flow_scale=1.0, rounds=None, cauchy_c=None,
+                      return_sums=False):
+    """Extension (motion segmentation): the camera homography of B fields fitted robustly to their flows on the GPU
+    (rb_homography_motion, include/raft_b200.h F34), started from global_motion's similarities.  flow_fw [B,Hn,Wn,2]
+    fp32 CUDA fields (forward or backward), occ_fw [B,Hn,Wn] uint8 their forward-backward masks, frame_hw = (Hs, Ws);
+    params [B,4] fp64 and reliable [B] bool are global_motion's.  `rounds` iteratively reweighted DLT rounds with Cauchy
+    scale cauchy_c network pixels (defaults: raft_b200.motionseg's ROUNDS, CAUCHY).  Returns fresh (H [B,3,3] fp64 in
+    the normalised centred coordinates of F34, flags [B] uint8: 0 fitted, 1 singular (the similarity kept), 2 the
+    similarity was unreliable (the identity)); with return_sums also the last round's [B,45] fp64 sums.  Wrong shapes or
+    dtypes raise ValueError."""
+    from raft_b200.motionseg import CAUCHY, ROUNDS, SUMS
+    if not (isinstance(flow_fw, torch.Tensor) and flow_fw.is_cuda and flow_fw.dim() == 4 and flow_fw.shape[-1] == 2
+            and flow_fw.dtype == torch.float32):
+        raise ValueError(f"homography_motion: flow_fw must be a [B,Hn,Wn,2] float32 CUDA tensor (got "
+                         f"{getattr(flow_fw, 'shape', None)} {getattr(flow_fw, 'dtype', type(flow_fw))})")
+    B, Hn, Wn, _ = flow_fw.shape
+    dev = flow_fw.device
+    if not (isinstance(occ_fw, torch.Tensor) and tuple(occ_fw.shape) == (B, Hn, Wn) and occ_fw.dtype == torch.uint8
+            and occ_fw.device == dev):
+        raise ValueError(f"homography_motion: occ_fw must be a [B,Hn,Wn] = {[B, Hn, Wn]} uint8 tensor on {dev}")
+    if not (isinstance(params, torch.Tensor) and tuple(params.shape) == (B, 4) and params.dtype == torch.float64
+            and params.device == dev and isinstance(reliable, torch.Tensor) and tuple(reliable.shape) == (B,)
+            and reliable.dtype == torch.bool and reliable.device == dev):
+        raise ValueError(f"homography_motion: params and reliable must be global_motion's [B,4] float64 and [B] bool "
+                         f"tensors on {dev}")
+    try:
+        Hs, Ws = (int(v) for v in frame_hw)
+    except (TypeError, ValueError):
+        raise ValueError(f"homography_motion: frame_hw must be (Hs, Ws) (got {frame_hw!r})") from None
+    if Hs < 1 or Ws < 1:
+        raise ValueError(f"homography_motion: frame_hw must be positive (got {frame_hw!r})")
+    rounds = ROUNDS if rounds is None else int(rounds)
+    cauchy_c = CAUCHY if cauchy_c is None else float(cauchy_c)
+    f, o, p = flow_fw.contiguous(), occ_fw.contiguous(), params.contiguous()
+    sim_flags = (~reliable).to(torch.uint8)
+    H = torch.empty(B, 3, 3, dtype=torch.float64, device=dev)
+    flags = torch.empty(B, dtype=torch.uint8, device=dev)
+    sums = torch.empty(B, SUMS, dtype=torch.float64, device=dev) if return_sums else None
+    with torch.cuda.device(dev):
+        nbytes = capi.size_query(capi.lib.rb_homography_motion_workspace_bytes, B, Hn, Wn)
+        ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+        capi.check(capi.lib.rb_homography_motion(capi.ptr(f), capi.ptr(o), B, Hn, Wn, Hs, Ws, float(flow_scale),
+                                                 capi.ptr(p), capi.ptr(sim_flags), rounds, cauchy_c, capi.ptr(H),
+                                                 capi.ptr(flags), capi.ptr(sums), capi.ptr(ws), nbytes, capi.stream()))
+    return (H, flags, sums) if return_sums else (H, flags)
+
+
+def motion_evidence(flow_fw, flow_bw, occ_fw, occ_bw, H, flags, frame_hw, cuts=None, flow_scale=1.0, tau=None):
+    """Extension (motion segmentation): the per-frame evidence of motion that departs from the camera's
+    (rb_motion_evidence, F35).  flow_fw, flow_bw [T,Hn,Wn,2] float32 consecutive flows and occ_fw, occ_bw [T,Hn,Wn] uint8
+    their masks; H [2T,3,3] fp64 and flags [2T] uint8 homography_motion's fit of the 2T fields cat(flow_fw, flow_bw);
+    frame_hw = (Hs, Ws); cuts None or a [T] uint8 CUDA tensor, non-zero for a scene-cut pair; tau in network pixels
+    (default raft_b200.motionseg.TAU).  Returns a fresh [T+1,Hn,Wn,2] float32 tensor of (N, C): the sum of
+    r^2 / (r^2 + tau^2) over the frame's usable fields and their count.  Bad arguments raise ValueError."""
+    from raft_b200.motionseg import TAU, check_tau
+    T, Hn, Wn = _flow_pair("motion_evidence", flow_fw, flow_bw)
+    dev = flow_fw.device
+    for name, t in (("occ_fw", occ_fw), ("occ_bw", occ_bw)):
+        if not (isinstance(t, torch.Tensor) and tuple(t.shape) == (T, Hn, Wn) and t.dtype == torch.uint8
+                and t.device == dev):
+            raise ValueError(f"motion_evidence: {name} must be a [T,Hn,Wn] = {[T, Hn, Wn]} uint8 tensor on {dev}")
+    if not (isinstance(H, torch.Tensor) and tuple(H.shape) == (2 * T, 3, 3) and H.dtype == torch.float64
+            and H.device == dev and isinstance(flags, torch.Tensor) and tuple(flags.shape) == (2 * T,)
+            and flags.dtype == torch.uint8 and flags.device == dev):
+        raise ValueError(f"motion_evidence: H and flags must be [2T,3,3] = {[2 * T, 3, 3]} float64 and [2T] uint8 "
+                         f"tensors on {dev}")
+    if cuts is not None and not (isinstance(cuts, torch.Tensor) and tuple(cuts.shape) == (T,)
+                                 and cuts.dtype == torch.uint8 and cuts.device == dev):
+        raise ValueError(f"motion_evidence: cuts must be None or a [T] = [{T}] uint8 tensor on {dev}")
+    try:
+        Hs, Ws = (int(v) for v in frame_hw)
+    except (TypeError, ValueError):
+        raise ValueError(f"motion_evidence: frame_hw must be (Hs, Ws) (got {frame_hw!r})") from None
+    tau = check_tau(TAU if tau is None else tau, "motion_evidence")
+    fw, bw, of, ob = flow_fw.contiguous(), flow_bw.contiguous(), occ_fw.contiguous(), occ_bw.contiguous()
+    h, fl, c = H.contiguous(), flags.contiguous(), None if cuts is None else cuts.contiguous()
+    ev = torch.empty(T + 1, Hn, Wn, 2, dtype=torch.float32, device=dev)
+    with torch.cuda.device(dev):
+        capi.check(capi.lib.rb_motion_evidence(capi.ptr(fw), capi.ptr(bw), capi.ptr(of), capi.ptr(ob), capi.ptr(h),
+                                               capi.ptr(fl), capi.ptr(c), T, Hn, Wn, Hs, Ws, float(flow_scale),
+                                               float(tau), capi.ptr(ev), capi.stream()))
+    return ev
+
+
+def motion_segment(evidence, flow_fw, flow_bw, frame_hw, rows, flow_scale=1.0, alpha1=0.01, alpha2=0.5):
+    """Extension (motion segmentation): the binary moving-object masks of F frames at their own size frame_hw = (Hs, Ws)
+    (rb_motion_segment, F35).  evidence [F,Hn,Wn,2] float32 (motion_evidence's); flow_fw, flow_bw [F-1,Hn,Wn,2] float32
+    consecutive flows; rows [n,3] integer table (t, nf, nb) (raft_b200.motionseg.segment_rows).  Each pixel adds the
+    evidence of its own frame and of every frame its chain reaches through the forward-backward test of fb_consistency.
+    Returns fresh (mask [n,Hs,Ws] uint8 0 / 1, status [n,Hs,Ws] uint8: 1 where no evidence reached the pixel).  Bad
+    shapes or a bad table raise ValueError."""
+    if not (isinstance(evidence, torch.Tensor) and evidence.is_cuda and evidence.dim() == 4 and evidence.shape[-1] == 2
+            and evidence.dtype == torch.float32):
+        raise ValueError(f"motion_segment: evidence must be an [F,Hn,Wn,2] float32 CUDA tensor (got "
+                         f"{getattr(evidence, 'shape', None)} {getattr(evidence, 'dtype', type(evidence))})")
+    F, Hn, Wn, _ = evidence.shape
+    dev = evidence.device
+    T, fh, fwd = _flow_pair("motion_segment", flow_fw, flow_bw)
+    if (T, fh, fwd) != (F - 1, Hn, Wn) or flow_fw.device != dev:
+        raise ValueError(f"motion_segment: {F} evidence maps need [F-1,Hn,Wn,2] = [{F - 1},{Hn},{Wn},2] flows on {dev} "
+                         f"(got {tuple(flow_fw.shape)})")
+    try:
+        Hs, Ws = (int(v) for v in frame_hw)
+    except (TypeError, ValueError):
+        raise ValueError(f"motion_segment: frame_hw must be (Hs, Ws) (got {frame_hw!r})") from None
+    if Hs < 1 or Ws < 1:
+        raise ValueError(f"motion_segment: frame_hw must be positive (got {frame_hw!r})")
+    table = _rows_table("motion_segment", rows, F, dev)
+    n = table.shape[0]
+    ev, fw, bw = evidence.contiguous(), flow_fw.contiguous(), flow_bw.contiguous()
+    mask = torch.empty(n, Hs, Ws, dtype=torch.uint8, device=dev)
+    status = torch.empty(n, Hs, Ws, dtype=torch.uint8, device=dev)
+    with torch.cuda.device(dev):
+        capi.check(capi.lib.rb_motion_segment(capi.ptr(ev), F, Hn, Wn, capi.ptr(fw), capi.ptr(bw), Hs, Ws,
+                                              float(flow_scale), float(alpha1), float(alpha2), capi.ptr(table), n,
+                                              capi.ptr(mask), capi.ptr(status), capi.stream()))
+    return mask, status
+
+
 def warp_frames(frames, A):
     """Extension (video stabilization): every frame of [F,H,W,C] uint8 CUDA frames (C in 1..4, any channel order) warped
     by its [2,3] matrix of A [F,2,3] (fp64, host or device), which maps an output pixel (x, y) to its source position in

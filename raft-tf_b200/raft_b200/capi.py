@@ -94,6 +94,10 @@ SIGNATURES = {
     "rb_tcons_terms": (_i, [_vp, _vp, _vp, _vp, _i, _i, _vp, _vp, _i, _i, _f, _f, _f, _f, _vp, _vp, _vp, _vp]),
     "rb_screened_poisson_workspace_bytes": (_i, [_i, _i, _psz]),
     "rb_screened_poisson": (_i, [_vp, _vp, _i, _i, _vp, _vp, _sz, _vp]),
+    "rb_homography_motion_workspace_bytes": (_i, [_i, _i, _i, _psz]),
+    "rb_homography_motion": (_i, [_vp, _vp, _i, _i, _i, _i, _i, _f, _vp, _vp, _i, _d, _vp, _vp, _vp, _vp, _sz, _vp]),
+    "rb_motion_evidence": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _f, _f, _vp, _vp]),
+    "rb_motion_segment": (_i, [_vp, _i, _i, _i, _vp, _vp, _i, _i, _f, _f, _f, _vp, _i, _vp, _vp, _vp]),
     "rb_warp_error_workspace_bytes": (_i, [_i, _i, _i, _psz]),
     "rb_warp_error": (_i, [_vp, _i, _i, _i, _vp, _vp, _i, _i, _f, _f, _f, _vp, _vp, _sz, _vp]),
     "rb_flow_reverse_workspace_bytes": (_i, [_i, _i, _i, _psz]),

@@ -55,12 +55,12 @@ Sequence = namedtuple("Sequence", "name frames annotations")
 
 
 # ---- reading ---------------------------------------------------------------------------------------------------------
-def davis_sequences(root, split="val"):
-    """The sequences of <root>/ImageSets/2017/<split>.txt, each Sequence(name, frame paths, annotation paths) in sorted
-    order.  A missing list, directory or annotation, an extra annotation, or a sequence of fewer than two frames raises
-    (FileNotFoundError / ValueError) naming it."""
+def davis_sequences(root, split="val", year="2017"):
+    """The sequences of <root>/ImageSets/<year>/<split>.txt, each Sequence(name, frame paths, annotation paths) in sorted
+    order (year "2016": DAVIS-2016's list, which ships in the DAVIS-2017 tree).  A missing list, directory or annotation,
+    an extra annotation, or a sequence of fewer than two frames raises (FileNotFoundError / ValueError) naming it."""
     root = os.fspath(root)
-    lst = os.path.join(root, "ImageSets", "2017", f"{split}.txt")
+    lst = os.path.join(root, "ImageSets", year, f"{split}.txt")
     if not os.path.isfile(lst):
         raise FileNotFoundError(f"DAVIS: no sequence list {lst}")
     with open(lst) as f:
@@ -352,3 +352,117 @@ def denoise_summary(res):
     """The summary line of evaluate_denoise's result."""
     return (f"Validation DAVIS-2017 denoising (test-dev, sigma {res['sigma']:g}): PSNR: {res['PSNR']:.4f}, SSIM: "
             f"{res['SSIM']:.4f} (noisy: PSNR: {res['noisy_PSNR']:.4f}, SSIM: {res['noisy_SSIM']:.4f})")
+
+
+# ---- motion segmentation (F34 / F35) ---------------------------------------------------------------------------------
+# DAVIS-2016's unsupervised protocol for RaftEngine.segment_motion:
+#
+#     res = evaluate_motion(RAFT(None, args).load("raft-things.npz"), "datasets/DAVIS")
+#
+# Data: the sequences of <root>/ImageSets/2016/val.txt (the 20 DAVIS-2016 val sequences, listed in the DAVIS-2017 tree),
+# frames JPEGImages/480p, checked up front as davis_sequences does.  The flow runs at the frames' own size, 20
+# iterations, 'sintel' padding (PROTOCOLS["davis"]).  Ground truth: the union of the non-zero labels of Annotations/480p,
+# the void label 255 counted as background, scored as one object with rb_label_metrics, frame_scores and db_statistics
+# on frames 1 .. F-2.
+#
+# Two caveats before comparing with published tables: the union of the DAVIS-2017 labels stands in for DAVIS-2016's
+# binary masks (they are drawn from the same annotations but may differ at object boundaries), and the scored-frame rule
+# above is the DAVIS-2017 evaluator's; diff it against the official DAVIS-2016 toolkit first.
+def segment_clip(engine, frames, window=None, tau=None, batch=8):
+    """RaftEngine.segment_motion's masks for frames [F,Hs,Ws,3] uint8 (the engine's channel order, a CUDA tensor) from
+    interp_schedule(F, batch) passes: each pass's 2n fields fitted as one batch and its evidence launched; the frame two
+    passes share sums its two halves (each launch starts from +0, so the bits are one launch's).  Returns (masks
+    [F,Hs,Ws] uint8, status [F,Hs,Ws] uint8) CUDA tensors, the same for every batch."""
+    from networks.utils import motion_evidence
+    from .motionseg import DEFAULT_WINDOW, TAU, check_tau, check_window, fit_fields, segment_frames, segment_rows
+    from .video import interp_schedule
+    F = len(frames)
+    window = check_window(DEFAULT_WINDOW if window is None else window, "DAVIS")
+    tau = check_tau(TAU if tau is None else tau, "DAVIS")
+    hw = tuple(frames.shape[1:3])
+    fws, bws, evs = [], [], []
+    for ps in interp_schedule(F, batch):
+        fw, bw, ofw, obw = engine.forward_sequence_bidirectional(frames[ps.frames], check=True)
+        n = sum(k is not None for k in ps.pairs)
+        fw, bw, ofw, obw = fw[:n], bw[:n], ofw[:n], obw[:n]
+        with torch.cuda.device(engine.device):
+            H, flags = fit_fields(torch.cat([fw, bw]), torch.cat([ofw, obw]), hw, engine.flow_scale)
+            ev = motion_evidence(fw, bw, ofw, obw, H, flags, hw, None, engine.flow_scale, tau)
+        if evs:
+            evs[-1][-1].add_(ev[0])
+            ev = ev[1:]
+        fws.append(fw.clone())
+        bws.append(bw.clone())
+        evs.append(ev)
+    with torch.cuda.device(engine.device):
+        return segment_frames(torch.cat(evs), torch.cat(fws), torch.cat(bws), hw, segment_rows(F, window),
+                              engine.flow_scale)
+
+
+def evaluate_motion(model, root, window=None, tau=None, batch=8, iters=None, masks_out=None):
+    """Motion segmentation of a loaded networks.RAFT.RAFT model on a DAVIS tree's DAVIS-2016 val sequences (the protocol
+    above).  A model with input_size, a bad window or tau raise ValueError before any frame is read.  With masks_out the
+    masks of every frame are written in DAVIS's results layout, <masks_out>/<seq>/<stem>.png (labels 0 / 1, palette of
+    the sequence's first annotation).  Returns aggregate_davis' dict plus "dataset", "split", "iters", "pad_mode",
+    "window" and "tau"; the same for every batch."""
+    from networks.utils import davis_bound_pix, label_metrics
+    from .evaluate import PROTOCOLS, _engine, _imread
+    from .motionseg import DEFAULT_WINDOW, TAU, check_tau, check_window
+    from .video import read_labels, write_labels
+    if getattr(model, "input_size", None) is not None:
+        raise ValueError("evaluate_motion: frames run at their own size; build the model without input_size")
+    window = check_window(DEFAULT_WINDOW if window is None else window, "evaluate_motion")
+    tau = check_tau(TAU if tau is None else tau, "evaluate_motion")
+    if int(batch) < 1:
+        raise ValueError(f"evaluate_motion: batch must be >= 1 (got {batch})")
+    if model._params is None:
+        raise RuntimeError("RAFT.load(<npz>) must be called before evaluate_motion")
+    seqs = davis_sequences(root, "val", year="2016")  # every file checked up front
+    n_iters, pad_mode = PROTOCOLS["davis"]
+    n_iters = n_iters if iters is None else int(iters)
+    engine = _engine(model, n_iters, pad_mode)
+    dev = engine.device
+    records = []
+    for seq in seqs:
+        frames = np.stack([_imread(p, bool(model.upstream)) for p in seq.frames])
+        annos = []
+        for p in seq.annotations:
+            lab, pal = read_labels(p)
+            annos.append(lab)
+            if len(annos) == 1:
+                palette = pal
+        gt = np.stack(annos)
+        if gt.shape[1:] != frames.shape[1:3]:
+            raise ValueError(f"DAVIS: sequence {seq.name}: annotations of {gt.shape[1]}x{gt.shape[2]}, frames of "
+                             f"{frames.shape[1]}x{frames.shape[2]}")
+        gt = ((gt != 0) & (gt != 255)).astype(np.uint8)
+        F, H, W = gt.shape
+        scored = list(range(1, F - 1))
+        with torch.cuda.device(dev):
+            pred, _ = segment_clip(engine, torch.from_numpy(frames).to(dev), window, tau, int(batch))
+            obj = dict(zip(SUMMARY[1:], (float("nan"),) * 6))
+            if scored:
+                idx = torch.tensor(scored, device=dev)
+                counts = label_metrics(pred[idx], torch.from_numpy(gt[scored]).to(dev), 1,
+                                       davis_bound_pix(H, W)).cpu().numpy()
+                J, Fm = frame_scores(counts)
+                jm, jr, jd = db_statistics(J[0])
+                fm, fr, fd = db_statistics(Fm[0])
+                obj = {"J-Mean": jm, "J-Recall": jr, "J-Decay": jd, "F-Mean": fm, "F-Recall": fr, "F-Decay": fd}
+            host = pred.cpu().numpy()
+        if masks_out is not None:
+            d = os.path.join(os.fspath(masks_out), seq.name)
+            os.makedirs(d, exist_ok=True)
+            for p, m in zip(seq.annotations, host):
+                write_labels(os.path.join(d, os.path.basename(p)), m, palette)
+        records.append({"name": seq.name, "n_frames": F, "n_objects": 1, "moving": float(host.mean()),
+                        "objects": [obj]})
+    res = aggregate_davis(records)
+    return {"dataset": "davis", "split": "val", "protocol": "DAVIS-2016 unsupervised", "iters": n_iters,
+            "pad_mode": pad_mode, "window": window, "tau": tau, **res}
+
+
+def motion_summary(res):
+    """The summary line of evaluate_motion's result."""
+    return (f"Validation DAVIS-2016 motion segmentation (val): J&F: {res['J&F-Mean']:.4f}, J: {res['J-Mean']:.4f}, "
+            f"F: {res['F-Mean']:.4f}")

@@ -718,6 +718,38 @@ class RaftEngine:
         with torch.cuda.device(self.device):
             return merge_frames(on_dev, flow_fw, flow_bw, rows, sigma, self.flow_scale)
 
+    @torch.no_grad()
+    def segment_motion(self, frames: torch.Tensor, window=None, tau=None, cuts=None):
+        """Motion segmentation of [F,Hs,Ws,3] uint8 frames (F >= 2; sizes and input_size as for forward()): the pixels
+        whose motion departs from the camera's.  One forward_sequence_bidirectional(check=True) pass; global_motion and
+        one rb_homography_motion on the 2T fields (forward then backward) as one batch; one rb_motion_evidence launch
+        (tau in network pixels, default raft_b200.motionseg.TAU; scene-cut pairs of cuts contribute nothing); one
+        rb_motion_segment launch over raft_b200.motionseg.segment_rows(F, window, cuts) (window default DEFAULT_WINDOW
+        frames each way; no chain crosses a cut).  Returns fresh (masks [F,Hs,Ws] uint8 in {0, 1}, status [F,Hs,Ws]
+        uint8: 1 where no evidence reached the pixel, homographies [F-1,3,3] fp64 host array: the forward pairs' H in
+        the frames' own pixels, h33 = 1).  Non-uint8 frames, a bad window, tau or cuts raise ValueError before the
+        pass."""
+        from networks.utils import motion_evidence
+        from .motionseg import (DEFAULT_WINDOW, TAU, check_tau, check_window, cut_flags, fit_fields, segment_frames,
+                                segment_rows, to_pixels)
+        from .video import check_cuts
+        F = _sequence_length(frames) + 1
+        if frames.dtype != torch.uint8:
+            raise ValueError(f"raft_b200: segment_motion reads bytes: the frames must be uint8 (got {frames.dtype})")
+        window = check_window(DEFAULT_WINDOW if window is None else window, "raft_b200")
+        tau = check_tau(TAU if tau is None else tau, "raft_b200")
+        cuts = check_cuts(() if cuts is None else cuts, F, "raft_b200")
+        rows = segment_rows(F, window, cuts)
+        hw = tuple(frames.shape[1:3])
+        flow_fw, flow_bw, occ_fw, occ_bw = self.forward_sequence_bidirectional(frames, check=True)
+        T = F - 1
+        with torch.cuda.device(self.device):
+            H, flags = fit_fields(torch.cat([flow_fw, flow_bw]), torch.cat([occ_fw, occ_bw]), hw, self.flow_scale)
+            ev = motion_evidence(flow_fw, flow_bw, occ_fw, occ_bw, H, flags, hw, cut_flags(cuts, range(T), self.device),
+                                 self.flow_scale, tau)
+            mask, status = segment_frames(ev, flow_fw, flow_bw, hw, rows, self.flow_scale)
+            return mask, status, to_pixels(H[:T].cpu().numpy(), hw)
+
     def _consistent_args(self, frames, other, name, cuts, what):
         F = _sequence_length(frames) + 1
         if frames.dtype != torch.uint8:

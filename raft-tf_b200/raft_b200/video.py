@@ -1583,6 +1583,121 @@ def video_denoise(model, frames, out, sigma, window=None, batch=8, workers=4, sc
     return names, {"sigma": float(sigma), "support": mean, "cuts": cuts}
 
 
+MASK_PALETTE = [[0, 0, 0], [128, 0, 0]]  # background, moving: DAVIS's colours for labels 0 and 1
+
+
+def video_segment_motion(model, frames, out, window=None, tau=None, batch=8, workers=4, scene_cut=None):
+    """Motion segmentation of a clip of any length with a loaded networks.RAFT.RAFT model, in one sweep: the frames (a
+    directory's sorted *.png / *.jpg, or a list of paths, all of one size) segmented into the pixels that move on their
+    own (1) and the rest (0), written as palette PNGs <out>/mask_<i:06d>.png (write_labels; --inpaint reads them as they
+    are) and the forward pairs' homographies in the frames' own pixels as <out>/homographies.npy [F-1,3,3] fp64, equal
+    byte for byte to RAFT.segment_motion on the whole clip for every batch and workers value.
+
+    Passes come from interp_schedule(): forward_sequence_bidirectional(check=True) on batch + 1 frames, the pass's 2n
+    fields fitted as one batch (global_motion, rb_homography_motion: a field's bits do not depend on the batch) and one
+    rb_motion_evidence launch on them.  The frame two passes share gets its forward field from the later pass and its
+    backward field from the earlier one: its (N, C) is the sum of the two launches' rows, the same bits as one launch,
+    since each launch starts from +0 and fp32 addition commutes.  A window of the clip stays on the GPU: the evidence
+    and the flows of the frames from t - window to the newest.  Frame t is segmented (rb_motion_segment) and written
+    once the evidence of frames up to min(t + window, F - 1) is complete, and the frames no later frame reaches are
+    dropped, so memory is bounded by the window, not the clip: 24 Hn Wn bytes per kept frame (evidence and two flows),
+    at most 2 window + batch + 2 of them.  scene_cut (a threshold in [0, 1]) scores each pass's frames on the GPU
+    (networks.utils.scene_cut_scores); a cut pair adds no evidence and no chain crosses it.  Prints the pairs with an
+    unreliable similarity (a field flagged 2) and with a singular fit (a field flagged 1), the mean moving fraction and
+    the cuts.  Returns (paths, info), info a dict of "unreliable", "fallback", "moving" and "cuts"."""
+    from networks.utils import motion_evidence, scene_cut_scores
+    from .motionseg import (DEFAULT_WINDOW, SINGULAR, TAU, UNRELIABLE, check_tau, check_window, cut_flags, fit_fields,
+                            segment_frames, segment_rows, to_pixels)
+
+    paths = list_frames(frames)
+    F = len(paths)
+    if F < 2:
+        raise ValueError(f"video_segment_motion: motion needs at least 2 frames (got {F})")
+    window = check_window(DEFAULT_WINDOW if window is None else window, "video_segment_motion")
+    tau = check_tau(TAU if tau is None else tau, "video_segment_motion")
+    thr = None if scene_cut is None else check_scene_cut(scene_cut)
+    batch, workers = int(batch), _workers(workers)
+    passes = interp_schedule(F, batch)
+    out = os.fspath(out)
+    os.makedirs(out, exist_ok=True)
+    engine = model.engine()
+    rgb = bool(model.upstream)
+    dev = engine.device
+    cap = min(F, 2 * window + batch + 2)  # frames kept on the GPU
+    names = [os.path.join(out, f"mask_{i:06d}.png") for i in range(F)]
+    moving, lock = [0], threading.Lock()
+    homs, field_flags = np.zeros((F - 1, 3, 3)), np.zeros((2, F - 1), np.uint8)
+    cuts, on_dev, store = [], None, None
+    base = have = done = 0  # store row 0 is frame base; frames base .. base + have - 1 are kept; frames < done written
+
+    def write(slot, first, n):  # writer thread: the masks of one pass, once its copies have landed
+        if slot is None:
+            return
+        slot.event.synchronize()
+        for r in range(n):
+            write_labels(names[first + r], slot.mask[r].numpy(), MASK_PALETTE)
+        s = int(slot.mask[:n].numpy().sum(dtype=np.int64))
+        with lock:
+            moving[0] += s
+
+    with _Pipeline(paths, passes, rgb, batch, workers, dev) as pipe:
+        for j, ps, imgs, src in pipe:
+            Hs, Ws = src.shape[1:3]
+            if on_dev is None:
+                on_dev = torch.empty(src.shape, dtype=torch.uint8, device=dev)
+            on_dev.copy_(src, non_blocking=True)
+            if thr is not None:
+                cuts += pass_cuts(ps.pairs, scene_cut_scores(on_dev).cpu(), thr)
+            flow_fw, flow_bw, occ_fw, occ_bw = engine.forward_sequence_bidirectional(on_dev, check=True)
+            n = sum(k is not None for k in ps.pairs)
+            first = ps.frames[0]
+            if store is None:
+                Hn, Wn = flow_fw.shape[1:3]
+                store = dict(ev=torch.empty(cap, Hn, Wn, 2, dtype=torch.float32, device=dev),
+                             fw=torch.empty(cap, Hn, Wn, 2, dtype=torch.float32, device=dev),
+                             bw=torch.empty(cap, Hn, Wn, 2, dtype=torch.float32, device=dev))
+            fw, bw, ofw, obw = flow_fw[:n], flow_bw[:n], occ_fw[:n], occ_bw[:n]
+            H, flags = fit_fields(torch.cat([fw, bw]), torch.cat([ofw, obw]), (Hs, Ws), engine.flow_scale)
+            ev = motion_evidence(fw, bw, ofw, obw, H, flags, (Hs, Ws), cut_flags(cuts, range(first, first + n), dev),
+                                 engine.flow_scale, tau)
+            homs[first:first + n] = to_pixels(H[:n].cpu().numpy(), (Hs, Ws))
+            field_flags[:, first:first + n] = flags.cpu().numpy().reshape(2, n)
+            new = list(range(base + have, first + n + 1))  # the pass's frames not kept yet
+            if have + len(new) > cap:  # drop the frames no frame still to be written reaches
+                drop = max(done - window, base) - base
+                for t in store.values():
+                    t[:have - drop].copy_(t[drop:have].clone())
+                base, have = base + drop, have - drop
+            k0 = new[0] - first  # 1 when frame `first` holds the previous pass's half of its evidence
+            if k0:
+                store["ev"][first - base].add_(ev[0])
+            store["ev"][have:have + len(new)].copy_(ev[k0:])
+            have += len(new)
+            store["fw"][first - base:first - base + n].copy_(fw)
+            store["bw"][first - base:first - base + n].copy_(bw)
+            ran = first + n  # pairs 0 .. ran - 1 have run: the evidence of frames < ran is complete (all at the end)
+            last = done
+            while last < F and (ran == F - 1 or min(last + window, F - 1) < ran):
+                last += 1
+            res = None
+            if last > done:
+                rows = segment_rows(F, window, sorted(cuts))[done:last].copy()
+                rows[:, 0] -= base
+                res = segment_frames(store["ev"][:have], store["fw"][:have - 1], store["bw"][:have - 1], (Hs, Ws),
+                                     rows, engine.flow_scale)
+            pipe.emit(partial(write, first=done, n=last - done), cap, mask=None if res is None else res[0])
+            done = last
+    cuts = sorted(cuts)
+    np.save(os.path.join(out, "homographies.npy"), homs)
+    unreliable = int((field_flags == UNRELIABLE).any(0).sum())
+    fallback = int((field_flags == SINGULAR).any(0).sum())
+    frac = moving[0] / (F * Hs * Ws)
+    print(f"segment motion: {unreliable} pairs with an unreliable similarity, {fallback} with a singular homography "
+          f"fit, moving fraction {frac:.4f}")
+    print(f"scene cuts: {len(cuts)}" + (" at pairs " + " ".join(str(k) for k in cuts) if cuts else ""))
+    return names, {"unreliable": unreliable, "fallback": fallback, "moving": frac, "cuts": cuts}
+
+
 def _aligned(frames, other, what):
     """The frame paths of frames and of other, which must hold as many frames; anything else raises ValueError."""
     paths, opaths = list_frames(frames), list_frames(other)
