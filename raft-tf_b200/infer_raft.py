@@ -1038,8 +1038,9 @@ def _flow_size(args):
 
 
 def _print_cuts(files, cuts):
-    """--scene-cut: the number of cut pairs and their indices (pair k: frame k -> k + 1); returns files."""
-    print(f"scene cuts: {len(cuts)}" + (" at pairs " + " ".join(str(k) for k in cuts) if cuts else ""))
+    """--scene-cut: the number of cut pairs and their indices (raft_b200.video.print_cuts); returns files."""
+    from raft_b200.video import print_cuts
+    print_cuts(cuts)
     return files
 
 

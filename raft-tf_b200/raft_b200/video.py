@@ -18,10 +18,14 @@ batch new frames, so every frame is decoded, uploaded and encoded once.  A short
 frame; its extra rows are idle and their flows discarded, so one pair of CUDA graphs serves the whole video.  warm_start
 runs T = 1 carry passes, each started from forward_interpolate of the previous pass's flow_low (upstream's warm start).
 
-Pipeline (_Pipeline, shared by video, video_interpolate and video_track): worker threads decode the frames of the next
-passes (cv2 releases the GIL) into two pinned slots used in turn, each refilled only after the event behind its pass has
-completed; each pass's outputs (colour images and flows, interpolated frames, track rows) are copied to two pinned output
-slots and encoded and written by writer threads.  The files are the same bytes for every workers value.
+Pipeline (_Pipeline, shared by every sweep here): worker threads decode the frames of the next passes (cv2 releases the
+GIL) into two pinned slots used in turn, each refilled only after the event behind its pass has completed; each pass's
+outputs (colour images and flows, interpolated frames, track rows, label maps, filled frames) are copied to two pinned
+output slots and encoded and written by writer threads (_FrameWriter for frames).  The files are the same bytes for
+every workers value.  A sweep whose GPU work reads the frames from device memory copies each pass to one reused device
+buffer (_Upload), and scores that copy for scene cuts.  The windowed sweeps (video_stabilize(fill=True), video_inpaint,
+video_denoise, video_segment_motion) keep a sliding window of frames and flows on the GPU (_Window): frame t is finished
+once the data up to frame min(t + window, F - 1) is complete, and frames no later frame reaches are dropped.
 
 video_track(model, "frames/", "out/", queries=[[0, 120.0, 64.5], ...]) tracks points through the clip (grid=STEP: a point
 at every STEP-th pixel of one frame): interp_schedule()'s passes of forward_sequence_bidirectional, each followed by one
@@ -267,6 +271,12 @@ def pass_cuts(pairs, scores, thr):
     return [k for r, k in enumerate(pairs) if k is not None and float(scores[r]) > thr]
 
 
+def print_cuts(cuts):
+    """Prints the number of scene-cut pairs and their indices (pair k: frame k -> k + 1), as the sweeps and the CLI
+    report them."""
+    print(f"scene cuts: {len(cuts)}" + (" at pairs " + " ".join(str(k) for k in cuts) if cuts else ""))
+
+
 def cut_copy(k, t):
     """The input frame that stands in for the frame at time t of pair k when the pair is a scene cut: the nearer one, k
     for t <= 0.5 and k + 1 after it (blending two shots would give a ghosted cross-dissolve)."""
@@ -435,6 +445,119 @@ class _Pipeline:
             (self.loose if o is None else o.futures).append(self.writers.submit(write, o))
 
 
+class _Upload:
+    """A device copy of each pass's pinned rows, in one buffer allocated on the first pass (later passes may be
+    shorter), and the pass's scene cuts scored on that copy."""
+
+    def __init__(self, device):
+        self.device, self.buf = device, None
+
+    def __call__(self, src, pairs, thr=None):
+        """Copies src to the buffer.  Returns (the device rows, the cut pairs of the pass with the pair indices pairs:
+        pass_cuts of networks.utils.scene_cut_scores on the device rows with a threshold thr, else [])."""
+        from networks.utils import scene_cut_scores
+        if self.buf is None:
+            self.buf = torch.empty(src.shape, dtype=src.dtype, device=self.device)
+        rows = self.buf[:len(src)]
+        rows.copy_(src, non_blocking=True)
+        return rows, ([] if thr is None else pass_cuts(pairs, scene_cut_scores(rows).cpu(), thr))
+
+
+class _FrameWriter:
+    """The write callback of a pass's finished frames (_Pipeline.emit, bound to first and n): slot.frames[r] written
+    as names[first + r] for r < n, BGR (converted when rgb), then with tally total += tally(slot, n) (0 before any
+    slot; the sums of the writer threads, taken under a lock)."""
+
+    def __init__(self, names, rgb, tally=None):
+        self.names, self.rgb, self.tally, self.total = names, rgb, tally, 0
+        self.lock = threading.Lock()
+
+    def __call__(self, slot, first, n):
+        import cv2
+        if slot is None:
+            return
+        slot.event.synchronize()
+        for r in range(n):
+            img = slot.frames[r].numpy()
+            if not cv2.imwrite(self.names[first + r], cv2.cvtColor(img, cv2.COLOR_RGB2BGR) if self.rgb else img):
+                raise OSError(f"cannot write {self.names[first + r]}")
+        if self.tally is not None:
+            c = self.tally(slot, n)
+            with self.lock:
+                self.total = self.total + c
+
+
+class _Window:
+    """The frames a windowed sweep (video_stabilize(fill=True), video_inpaint, video_denoise, video_segment_motion)
+    keeps on the GPU over interp_schedule(F, batch)'s passes.  Frame t is finished once the sweep's data is complete up
+    to frame min(t + window, F - 1), and reaches back to frame t - window, so at most cap = min(F, 2 window + batch + 2)
+    frames are kept.  Row r of a frame store holds frame base + r, row r of a pair store (flows) pair base + r; frames
+    base .. base + have - 1 are kept and the frames before done are finished.
+
+        win = _Window(F, window, batch, device)
+        for each pass, on the frames first .. first + n:
+            s = win.alloc(frames=((Hs, Ws, 3), torch.uint8), fw=((Hn, Wn, 2), torch.float32), ...)  # allocates once
+            new = win.admit(first + n)  # the store rows of the pass's frames not kept yet
+            ...                         # those frames into s[name][new], the pass's pairs from row win.row(first) on
+            t0, m, rows = win.finish(complete, table)  # frames t0 .. t0 + m - 1 are due: their table rows, rebased
+            ...                         # the sweep's kernel on win.kept(name), win.kept_pairs(name) and rows
+
+    It does no GPU work beyond allocating the stores and shifting their rows when frames are dropped."""
+
+    def __init__(self, F, window, batch, device):
+        self.F, self.window, self.device = int(F), int(window), device
+        self.cap = min(self.F, 2 * self.window + int(batch) + 2)
+        self.base = self.have = self.done = 0
+        self.store = None
+
+    def alloc(self, **rows):
+        """On the first call, allocates store[name] with cap rows of each name=(row shape, dtype); later calls do
+        nothing.  Returns the stores."""
+        if self.store is None:
+            self.store = {name: torch.empty(self.cap, *shape, dtype=dtype, device=self.device)
+                          for name, (shape, dtype) in rows.items()}
+        return self.store
+
+    def admit(self, last):
+        """Keeps the frames up to `last`: returns the store rows of those not kept yet.  When they would not fit, the
+        frames no frame still to be finished reaches (those before done - window) are dropped first; if they still
+        do not fit, RuntimeError."""
+        new = last + 1 - self.base - self.have
+        if self.have + new > self.cap:
+            drop = max(self.done - self.window, self.base) - self.base
+            if self.have - drop + new > self.cap:
+                raise RuntimeError(f"video: frames {self.base + self.have} .. {last} do not fit beside the frames a "
+                                   f"window of {self.window} keeps ({self.cap} at most)")
+            for t in self.store.values():
+                t[:self.have - drop].copy_(t[drop:self.have].clone())
+            self.base, self.have = self.base + drop, self.have - drop
+        self.have += new
+        return slice(self.have - new, self.have)
+
+    def row(self, t):
+        """The store row of frame (or pair) t."""
+        return t - self.base
+
+    def kept(self, name):
+        """The rows of frame store `name` that hold the kept frames."""
+        return self.store[name][:self.have]
+
+    def kept_pairs(self, name):
+        """The rows of pair store `name` that hold the pairs between the kept frames."""
+        return self.store[name][:self.have - 1]
+
+    def finish(self, complete, table):
+        """Finishes the frames from done on, in order, while min(t + window, F - 1) <= complete (the last frame whose
+        inputs are complete).  Returns (t0, m, table[t0:t0 + m] with column 0, the frame, as its store row)."""
+        t0 = last = self.done
+        while last < self.F and min(last + self.window, self.F - 1) <= complete:
+            last += 1
+        rows = table[t0:last].copy()
+        rows[:, 0] -= self.base
+        self.done = last
+        return t0, last - t0, rows
+
+
 def video(model, frames, out, batch=8, workers=4, warm_start=False, flo=None, npy=None, native_flow=False,
           scene_cut=None):
     """The flow between every pair of consecutive frames of a loaded networks.RAFT.RAFT model, written as
@@ -554,7 +677,6 @@ def video_interpolate(model, frames, out, ts=None, batch=8, workers=4, fps=None,
     sweep decodes and scores every pair (no flow), so the exposures are clamped at every cut before any is summed.
     Returns the written paths in output order; with scene_cut the tuple (paths, cuts), cuts the increasing cut pairs."""
     import cv2
-    from networks.utils import scene_cut_scores
 
     paths = list_frames(frames)
     if (ts is None) == (fps is None):
@@ -603,16 +725,13 @@ def video_interpolate(model, frames, out, ts=None, batch=8, workers=4, fps=None,
             if not cv2.imwrite(name(n), slot.frames[r].numpy()):
                 raise OSError(f"cannot write {name(n)}")
 
-    on_dev, cuts = None, []  # scene_cut: the pass's frames on the GPU
+    upload, cuts = _Upload(dev), []
     with _Pipeline(paths, passes, rgb, batch, workers, dev) as pipe:
         for j, ps, imgs, src in pipe:
             first = ps.frames[0]  # frame i is row i - first of the pass
-            cut = ()
+            cut = []
             if thr is not None:  # score the pass on the GPU; the engine then reads the frames from there too
-                if on_dev is None:
-                    on_dev = torch.empty(src.shape, dtype=torch.uint8, device=dev)
-                on_dev.copy_(src, non_blocking=True)
-                src, cut = on_dev, pass_cuts(ps.pairs, scene_cut_scores(on_dev).cpu(), thr)
+                src, cut = upload(src, ps.pairs, thr)
                 cuts += cut
             res = None
             if fps is None:  # row j T + r: pair r of the pass at ts[j]
@@ -641,7 +760,6 @@ def _video_shutter(model, paths, out, fps, shutter, density, batch, workers, thr
     """video_interpolate(fps=, shutter=, density=) after its argument checks: the optional scoring sweep, then one sweep of
     shutter_schedule()'s passes, each one RaftEngine.expose call whose closed frames are written."""
     import cv2
-    from networks.utils import scene_cut_scores
 
     try:
         fin, fout = fps
@@ -667,13 +785,10 @@ def _video_shutter(model, paths, out, fps, shutter, density, batch, workers, thr
 
     cuts = []
     if thr is not None:  # every cut is known before any exposure is summed
-        on_dev = None
+        upload = _Upload(dev)
         with _Pipeline(paths, interp_schedule(len(paths), batch), rgb, batch, workers, dev) as pipe:
             for _, ps, _, src in pipe:
-                if on_dev is None:
-                    on_dev = torch.empty(src.shape, dtype=torch.uint8, device=dev)
-                on_dev.copy_(src, non_blocking=True)
-                cuts += pass_cuts(ps.pairs, scene_cut_scores(on_dev).cpu(), thr)
+                cuts += upload(src, ps.pairs, thr)[1]
                 pipe.emit(lambda slot: None)
     passes = shutter_schedule(len(paths), fin, fout, shutter, density, batch, cuts)
     rows = max(1, max(len(p.closes) for p in passes))
@@ -1104,8 +1219,6 @@ def video_propagate(model, frames, out, labels, frame=0, batch=8, workers=4, sce
     reverse sweep scores its own passes), and no frame takes labels from a keyframe across a cut pair: the files are
     RAFT.propagate(..., cuts=<the cuts found>)'s, status 3 (label 0) where no keyframe reaches a frame.  It then returns
     (paths, last status, cuts), cuts the increasing cut pairs."""
-    from networks.utils import scene_cut_scores
-
     paths = list_frames(frames)
     F = len(paths)
     K, keys_np, palette = _read_keys(labels, frame, F, "video_propagate")
@@ -1137,18 +1250,15 @@ def video_propagate(model, frames, out, labels, frame=0, batch=8, workers=4, sce
 
     def run(sweep_passes, step):
         nonlocal last
-        on_dev = None
+        upload = _Upload(dev)
         with _Pipeline(paths, sweep_passes, rgb, batch, workers, dev) as pipe:
             for j, ps, imgs, src in pipe:
                 if j == 0 and tuple(src.shape[1:3]) != keys_np.shape[1:]:
                     raise ValueError(f"video_propagate: the key is {keys_np.shape[1]}x{keys_np.shape[2]}, the frames "
                                      f"{src.shape[1]}x{src.shape[2]}")
                 if thr is not None:  # score the pass on the GPU; the engine then reads the frames from there too
-                    if on_dev is None:
-                        on_dev = torch.empty(src.shape, dtype=torch.uint8, device=dev)
-                    on_dev.copy_(src, non_blocking=True)
-                    src = on_dev
-                    cuts.extend(pass_cuts(ps.pairs, scene_cut_scores(on_dev).cpu(), thr))
+                    src, cut = upload(src, ps.pairs, thr)
+                    cuts.extend(cut)
                     cuts.sort()
                 flow_fw, flow_bw, _, _ = engine.forward_sequence_bidirectional(src, check=False)
                 chunks = step(ps, flow_fw, flow_bw)
@@ -1197,8 +1307,7 @@ def video_stabilize(model, frames, out, sigma, batch=8, workers=4, scene_cut=Non
     fill_warp over inpaint_rows(F, window, cuts)) and written once the pairs up to min(t + window, F - 1) have run.  It
     also prints the pixel counts of status 1 / 2 / 3, and info gains "counts" (pixels filled from both sides, one side,
     spatially) and "margin" ((my, mx) network pixels)."""
-    import cv2
-    from networks.utils import global_motion, scene_cut_scores, warp_frames
+    from networks.utils import global_motion, warp_frames
     from .inpaint import DEFAULT_WINDOW, check_window
     from .stabilize import DEFAULT_MAX_ZOOM, camera_transforms, check_max_zoom, check_sigma
 
@@ -1228,16 +1337,13 @@ def video_stabilize(model, frames, out, sigma, batch=8, workers=4, scene_cut=Non
             motions[k] = slot.params[r].numpy()
             reliable[k] = bool(slot.reliable[r])
 
-    on_dev, cuts = None, []
+    upload, cuts = _Upload(dev), []
     with _Pipeline(paths, passes, rgb, batch, workers, dev) as pipe:
         for j, ps, imgs, src in pipe:
             hw = tuple(src.shape[1:3])
             if thr is not None:  # score the pass on the GPU; the engine then reads the frames from there too
-                if on_dev is None:
-                    on_dev = torch.empty(src.shape, dtype=torch.uint8, device=dev)
-                on_dev.copy_(src, non_blocking=True)
-                src = on_dev
-                cuts += pass_cuts(ps.pairs, scene_cut_scores(on_dev).cpu(), thr)
+                src, cut = upload(src, ps.pairs, thr)
+                cuts += cut
             flow_fw, _, occ_fw, _ = engine.forward_sequence_bidirectional(src, check=True)
             params, _, rel = global_motion(flow_fw, occ_fw, hw, flow_scale=engine.flow_scale)
             pipe.emit(partial(keep, pairs=[(r, k) for r, k in enumerate(ps.pairs) if k is not None]), batch,
@@ -1246,111 +1352,73 @@ def video_stabilize(model, frames, out, sigma, batch=8, workers=4, scene_cut=Non
     transforms, zooms, capped = camera_transforms(motions, hw, sigma, cuts, max_zoom)
     np.save(os.path.join(out, "transforms.npy"), transforms)
 
-    def name(i):
-        return os.path.join(out, f"frame_{i:06d}.png")
-
-    def write(slot, first, n):  # writer thread: the warped frames of one chunk
-        slot.event.synchronize()
-        for r in range(n):
-            img = slot.frames[r].numpy()
-            if not cv2.imwrite(name(first + r), cv2.cvtColor(img, cv2.COLOR_RGB2BGR) if rgb else img):
-                raise OSError(f"cannot write {name(first + r)}")
-
+    names = [os.path.join(out, f"frame_{i:06d}.png") for i in range(F)]
     A = torch.from_numpy(transforms).to(dev)
     if fill:
         counts, margin = _stabilize_fill_sweep(engine, paths, passes, rgb, batch, workers, hw, motions, transforms, A,
-                                               sorted(cuts), window, name)
+                                               sorted(cuts), window, names)
     else:
         chunks = [Pass(False, list(range(i, min(i + batch, F))), []) for i in range(0, F, batch)]
+        write, upload = _FrameWriter(names, rgb), _Upload(dev)
         with _Pipeline(paths, chunks, rgb, batch, workers, dev) as pipe:
-            on_dev = None
             for j, ps, imgs, src in pipe:
-                if on_dev is None:
-                    on_dev = torch.empty(src.shape, dtype=torch.uint8, device=dev)
                 n, first = len(ps.frames), ps.frames[0]
-                on_dev[:n].copy_(src, non_blocking=True)
-                res = warp_frames(on_dev[:n], A[first:first + n])
+                res = warp_frames(upload(src, ps.pairs)[0], A[first:first + n])
                 pipe.emit(partial(write, first=first, n=n), batch, frames=res)
     unreliable = [k for k in np.flatnonzero(~reliable).tolist() if k not in cuts]
     print("stabilize: zoom per shot " + " ".join(f"{z:.4f}" for z in zooms)
           + (f" (shots {' '.join(map(str, capped))} capped at {max_zoom:g})" if capped else ""))
-    print(f"scene cuts: {len(cuts)}" + (" at pairs " + " ".join(str(k) for k in cuts) if cuts else ""))
+    print_cuts(cuts)
     print(f"unreliable pairs (identity motion): {len(unreliable)}")
     info = {"zooms": zooms, "capped": capped, "cuts": cuts, "unreliable": unreliable}
     if fill:
         print(f"stabilize fill: pixels filled from both sides {counts[1]}, from one side {counts[2]}, spatially "
               f"{counts[3]}")
         info.update(counts=counts[1:].tolist(), margin=margin)
-    return [name(i) for i in range(F)], info
+    return names, info
 
 
-def _stabilize_fill_sweep(engine, paths, passes, rgb, batch, workers, hw, motions, transforms, A, cuts, window, name):
-    """video_stabilize's fill sweep: writes every frame, full-frame stabilized, with name(i).  Returns (counts [4] int64
+def _status_counts(slot, n):
+    """The [4] int64 pixel counts of each status in the first n rows of slot.status (a _FrameWriter tally)."""
+    return np.bincount(slot.status[:n].numpy().reshape(-1), minlength=4)[:4]
+
+
+def _stabilize_fill_sweep(engine, paths, passes, rgb, batch, workers, hw, motions, transforms, A, cuts, window, names):
+    """video_stabilize's fill sweep: writes every frame, full-frame stabilized, as names[i].  Returns (counts [4] int64
     of each status, margin)."""
-    import cv2
     from networks.utils import extend_flows
     from .inpaint import inpaint_rows
     from .stabilize import fill_margin, fill_warp
     F, dev = len(paths), engine.device
-    cap = min(F, 2 * window + batch + 2)  # frames kept on the GPU
-    rows_all = inpaint_rows(F, window, cuts)
-    counts, lock = np.zeros(4, np.int64), threading.Lock()
-    on_dev = store = net_hw = margin = None
-    base = have = done = 0  # store row 0 is frame base; frames base .. base + have - 1 are kept; frames < done written
-
-    def write(slot, first, n):  # writer thread: the filled frames of one pass, once its copies have landed
-        if slot is None:
-            return
-        slot.event.synchronize()
-        for r in range(n):
-            img = slot.frames[r].numpy()
-            if not cv2.imwrite(name(first + r), cv2.cvtColor(img, cv2.COLOR_RGB2BGR) if rgb else img):
-                raise OSError(f"cannot write {name(first + r)}")
-        c = np.bincount(slot.status[:n].numpy().reshape(-1), minlength=4)[:4]
-        with lock:
-            counts[:] += c
-
+    win, upload, write = _Window(F, window, batch, dev), _Upload(dev), _FrameWriter(names, rgb, _status_counts)
+    table = inpaint_rows(F, window, cuts)
+    margin = None
     with _Pipeline(paths, passes, rgb, batch, workers, dev) as pipe:
         for j, ps, imgs, src in pipe:
-            if on_dev is None:
-                on_dev = torch.empty(src.shape, dtype=torch.uint8, device=dev)
-            on_dev.copy_(src, non_blocking=True)
-            flow_fw, flow_bw, _, _ = engine.forward_sequence_bidirectional(on_dev, check=False)
+            src, _ = upload(src, ps.pairs)
+            flow_fw, flow_bw, _, _ = engine.forward_sequence_bidirectional(src, check=False)
             n = sum(k is not None for k in ps.pairs)
             first = ps.frames[0]
-            if store is None:
+            if margin is None:
                 net_hw = tuple(flow_fw.shape[1:3])
                 margin = fill_margin(transforms, hw, net_hw)
-                Hc, Wc = net_hw[0] + 2 * margin[0], net_hw[1] + 2 * margin[1]
-                store = dict(frames=torch.empty(cap, *hw, 3, dtype=torch.uint8, device=dev),
-                             fw=torch.empty(cap, Hc, Wc, 2, dtype=torch.float32, device=dev),
-                             bw=torch.empty(cap, Hc, Wc, 2, dtype=torch.float32, device=dev))
-            new = list(range(base + have, first + n + 1))  # the pass's frames not kept yet
-            if have + len(new) > cap:  # drop the frames no frame still to be written reaches
-                drop = max(done - window, base) - base
-                for t in store.values():
-                    t[:have - drop].copy_(t[drop:have].clone())
-                base, have = base + drop, have - drop
-            store["frames"][have:have + len(new)].copy_(on_dev[new[0] - first:new[-1] - first + 1])
-            have += len(new)
+                canvas = (net_hw[0] + 2 * margin[0], net_hw[1] + 2 * margin[1], 2)
+            s = win.alloc(frames=(hw + (3,), torch.uint8), fw=(canvas, torch.float32), bw=(canvas, torch.float32))
+            new = win.admit(first + n)
+            r = win.row(first)
+            s["frames"][new].copy_(src[new.start - r:n + 1])
             # copies out of the engine's views, which the next pass overwrites
             fw, bw = extend_flows(flow_fw[:n], flow_bw[:n], motions[first:first + n], hw, margin, engine.flow_scale)
-            store["fw"][first - base:first - base + n].copy_(fw)
-            store["bw"][first - base:first - base + n].copy_(bw)
-            ran = first + n  # pairs 0 .. ran - 1 have run
-            last = done
-            while last < F and min(last + window, F - 1) <= ran:
-                last += 1
+            s["fw"][r:r + n].copy_(fw)
+            s["bw"][r:r + n].copy_(bw)
+            t0, m, rows = win.finish(first + n, table)  # pairs 0 .. first + n - 1 have run
             res = None
-            if last > done:
-                rows = rows_all[done:last].copy()
-                rows[:, 0] -= base
-                res = fill_warp(store["frames"][:have], store["fw"][:have - 1], store["bw"][:have - 1], net_hw, margin,
-                                A[done:last], rows, engine.flow_scale)
-            pipe.emit(partial(write, first=done, n=last - done), cap, frames=None if res is None else res[0],
+            if m:
+                res = fill_warp(win.kept("frames"), win.kept_pairs("fw"), win.kept_pairs("bw"), net_hw, margin,
+                                A[t0:t0 + m], rows, engine.flow_scale)
+            pipe.emit(partial(write, first=t0, n=m), win.cap, frames=None if res is None else res[0],
                       status=None if res is None else res[1])
-            done = last
-    return counts, margin
+    return write.total, margin
 
 
 def list_masks(masks, F, what="video_inpaint"):
@@ -1387,8 +1455,7 @@ def video_inpaint(model, frames, out, masks, window=None, dilate=None, labels=No
     crosses a cut pair.  Prints the pixel counts of status 1 / 2 / 3 and the cuts.  Frames go in RGB with model.upstream
     and BGR otherwise, like the CLI; the files are BGR.  Returns (paths, info), info a dict of "counts" (pixels filled
     from both sides, one side, spatially) and "cuts"."""
-    import cv2
-    from networks.utils import inpaint_masks, scene_cut_scores
+    from networks.utils import inpaint_masks
     from .inpaint import (DEFAULT_DILATE, DEFAULT_WINDOW, check_dilate, check_window, complete_flows, fill_frames,
                           inpaint_rows, selection_table)
 
@@ -1406,81 +1473,47 @@ def video_inpaint(model, frames, out, masks, window=None, dilate=None, labels=No
     engine = model.engine()
     rgb = bool(model.upstream)
     dev = engine.device
-    cap = min(F, 2 * window + batch + 2)  # frames kept on the GPU
     names = [os.path.join(out, f"frame_{i:06d}.png") for i in range(F)]
-    counts, lock = np.zeros(4, np.int64), threading.Lock()
-    cuts, on_dev, store = [], None, None
-    base = have = done = 0  # store row 0 is frame base; frames base .. base + have - 1 are kept; frames < done written
-
-    def write(slot, first, n):  # writer thread: the filled frames of one pass, once its copies have landed
-        if slot is None:
-            return
-        slot.event.synchronize()
-        for r in range(n):
-            img = slot.frames[r].numpy()
-            if not cv2.imwrite(names[first + r], cv2.cvtColor(img, cv2.COLOR_RGB2BGR) if rgb else img):
-                raise OSError(f"cannot write {names[first + r]}")
-        c = np.bincount(slot.status[:n].numpy().reshape(-1), minlength=4)[:4]
-        with lock:
-            counts[:] += c
-
+    win, upload, write = _Window(F, window, batch, dev), _Upload(dev), _FrameWriter(names, rgb, _status_counts)
+    cuts = []
     with _Pipeline(paths, passes, rgb, batch, workers, dev) as pipe:
         for j, ps, imgs, src in pipe:
             Hs, Ws = src.shape[1:3]
-            if on_dev is None:
-                on_dev = torch.empty(src.shape, dtype=torch.uint8, device=dev)
-            on_dev.copy_(src, non_blocking=True)
-            if thr is not None:
-                cuts += pass_cuts(ps.pairs, scene_cut_scores(on_dev).cpu(), thr)
-            flow_fw, flow_bw, _, _ = engine.forward_sequence_bidirectional(on_dev, check=False)
+            src, cut = upload(src, ps.pairs, thr)
+            cuts += cut
+            flow_fw, flow_bw, _, _ = engine.forward_sequence_bidirectional(src, check=False)
             n = sum(k is not None for k in ps.pairs)
             first = ps.frames[0]
-            if store is None:
-                Hn, Wn = flow_fw.shape[1:3]
-                store = dict(frames=torch.empty(cap, Hs, Ws, 3, dtype=torch.uint8, device=dev),
-                             hole=torch.empty(cap, Hs, Ws, dtype=torch.uint8, device=dev),
-                             hole_net=torch.empty(cap, Hn, Wn, dtype=torch.uint8, device=dev),
-                             fw=torch.empty(cap, Hn, Wn, 2, dtype=torch.float32, device=dev),
-                             bw=torch.empty(cap, Hn, Wn, 2, dtype=torch.float32, device=dev))
-            new = list(range(base + have, first + n + 1))  # the pass's frames not kept yet
-            if have + len(new) > cap:  # drop the frames no frame still to be written reaches
-                drop = max(done - window, base) - base
-                for t in store.values():
-                    t[:have - drop].copy_(t[drop:have].clone())
-                base, have = base + drop, have - drop
+            Hn, Wn = flow_fw.shape[1:3]
+            s = win.alloc(frames=((Hs, Ws, 3), torch.uint8), hole=((Hs, Ws), torch.uint8),
+                          hole_net=((Hn, Wn), torch.uint8), fw=((Hn, Wn, 2), torch.float32),
+                          bw=((Hn, Wn, 2), torch.float32))
+            new = win.admit(first + n)
+            r = win.row(first)
             lab = []
-            for i in new:
-                m, _ = read_labels(mask_paths[i])
-                if m.shape != (Hs, Ws):
-                    raise ValueError(f"video_inpaint: {mask_paths[i]} is {m.shape[0]}x{m.shape[1]}, the frames "
+            for i in range(first + new.start - r, first + n + 1):
+                mask, _ = read_labels(mask_paths[i])
+                if mask.shape != (Hs, Ws):
+                    raise ValueError(f"video_inpaint: {mask_paths[i]} is {mask.shape[0]}x{mask.shape[1]}, the frames "
                                      f"{Hs}x{Ws}")
-                lab.append(m)
-            r0 = have
-            rows_new = slice(r0, r0 + len(new))
-            store["frames"][rows_new].copy_(on_dev[new[0] - first:new[-1] - first + 1])
+                lab.append(mask)
+            s["frames"][new].copy_(src[new.start - r:n + 1])
             h, hn = inpaint_masks(torch.from_numpy(np.stack(lab)).to(dev), (Hn, Wn), dilate, labels)
-            store["hole"][rows_new].copy_(h)
-            store["hole_net"][rows_new].copy_(hn)
-            have += len(new)
-            fw, bw = complete_flows(flow_fw[:n], flow_bw[:n], store["hole_net"][first - base:first - base + n + 1])
-            store["fw"][first - base:first - base + n].copy_(fw)
-            store["bw"][first - base:first - base + n].copy_(bw)
-            ran = first + n  # pairs 0 .. ran - 1 have run
-            last = done
-            while last < F and min(last + window, F - 1) <= ran:
-                last += 1
+            s["hole"][new].copy_(h)
+            s["hole_net"][new].copy_(hn)
+            fw, bw = complete_flows(flow_fw[:n], flow_bw[:n], s["hole_net"][r:r + n + 1])
+            s["fw"][r:r + n].copy_(fw)
+            s["bw"][r:r + n].copy_(bw)
+            t0, m, rows = win.finish(first + n, inpaint_rows(F, window, sorted(cuts)))  # pairs .. first + n - 1 ran
             res = None
-            if last > done:
-                rows = inpaint_rows(F, window, sorted(cuts))[done:last].copy()
-                rows[:, 0] -= base
-                res = fill_frames(store["frames"][:have], store["hole"][:have], store["fw"][:have - 1],
-                                  store["bw"][:have - 1], rows, engine.flow_scale)
-            pipe.emit(partial(write, first=done, n=last - done), cap, frames=None if res is None else res[0],
+            if m:
+                res = fill_frames(win.kept("frames"), win.kept("hole"), win.kept_pairs("fw"), win.kept_pairs("bw"),
+                                  rows, engine.flow_scale)
+            pipe.emit(partial(write, first=t0, n=m), win.cap, frames=None if res is None else res[0],
                       status=None if res is None else res[1])
-            done = last
-    cuts = sorted(cuts)
+    cuts, counts = sorted(cuts), write.total
     print(f"inpaint: pixels filled from both sides {counts[1]}, from one side {counts[2]}, spatially {counts[3]}")
-    print(f"scene cuts: {len(cuts)}" + (" at pairs " + " ".join(str(k) for k in cuts) if cuts else ""))
+    print_cuts(cuts)
     return names, {"counts": counts[1:].tolist(), "cuts": cuts}
 
 
@@ -1499,8 +1532,6 @@ def video_denoise(model, frames, out, sigma, window=None, batch=8, workers=4, sc
     pass's frames on the GPU (networks.utils.scene_cut_scores); no side crosses a cut pair.  Prints the sigma used, the
     mean support (matched frames per pixel) and the cuts.  Frames go in RGB with model.upstream and BGR otherwise, like
     the CLI; the files are BGR.  Returns (paths, info), info a dict of "sigma", "support" (the mean) and "cuts"."""
-    import cv2
-    from networks.utils import scene_cut_scores
     from .denoise import DEFAULT_WINDOW, ESTIMATE_FRAMES, check_sigma, check_window, estimate_sigma, merge_frames
     from .inpaint import inpaint_rows
 
@@ -1519,67 +1550,37 @@ def video_denoise(model, frames, out, sigma, window=None, batch=8, workers=4, sc
     if sigma == "auto":
         with torch.cuda.device(dev):
             sigma = estimate_sigma(torch.from_numpy(np.stack([_imread(p, rgb) for p in paths[:ESTIMATE_FRAMES]])).to(dev))
-    cap = min(F, 2 * window + batch + 2)  # frames kept on the GPU
     names = [os.path.join(out, f"frame_{i:06d}.png") for i in range(F)]
-    total, lock = [0], threading.Lock()
-    cuts, on_dev, store = [], None, None
-    base = have = done = 0  # store row 0 is frame base; frames base .. base + have - 1 are kept; frames < done written
-
-    def write(slot, first, n):  # writer thread: the merged frames of one pass, once its copies have landed
-        if slot is None:
-            return
-        slot.event.synchronize()
-        for r in range(n):
-            img = slot.frames[r].numpy()
-            if not cv2.imwrite(names[first + r], cv2.cvtColor(img, cv2.COLOR_RGB2BGR) if rgb else img):
-                raise OSError(f"cannot write {names[first + r]}")
-        s = int(slot.support[:n].numpy().sum(dtype=np.int64))
-        with lock:
-            total[0] += s
-
+    win, upload = _Window(F, window, batch, dev), _Upload(dev)
+    write = _FrameWriter(names, rgb, lambda slot, n: int(slot.support[:n].numpy().sum(dtype=np.int64)))
+    cuts = []
     with _Pipeline(paths, passes, rgb, batch, workers, dev) as pipe:
         for j, ps, imgs, src in pipe:
             Hs, Ws = src.shape[1:3]
-            if on_dev is None:
-                on_dev = torch.empty(src.shape, dtype=torch.uint8, device=dev)
-            on_dev.copy_(src, non_blocking=True)
-            if thr is not None:
-                cuts += pass_cuts(ps.pairs, scene_cut_scores(on_dev).cpu(), thr)
-            flow_fw, flow_bw, _, _ = engine.forward_sequence_bidirectional(on_dev, check=False)
+            src, cut = upload(src, ps.pairs, thr)
+            cuts += cut
+            flow_fw, flow_bw, _, _ = engine.forward_sequence_bidirectional(src, check=False)
             n = sum(k is not None for k in ps.pairs)
             first = ps.frames[0]
-            if store is None:
-                Hn, Wn = flow_fw.shape[1:3]
-                store = dict(frames=torch.empty(cap, Hs, Ws, 3, dtype=torch.uint8, device=dev),
-                             fw=torch.empty(cap, Hn, Wn, 2, dtype=torch.float32, device=dev),
-                             bw=torch.empty(cap, Hn, Wn, 2, dtype=torch.float32, device=dev))
-            new = list(range(base + have, first + n + 1))  # the pass's frames not kept yet
-            if have + len(new) > cap:  # drop the frames no frame still to be written reaches
-                drop = max(done - window, base) - base
-                for t in store.values():
-                    t[:have - drop].copy_(t[drop:have].clone())
-                base, have = base + drop, have - drop
-            store["frames"][have:have + len(new)].copy_(on_dev[new[0] - first:new[-1] - first + 1])
-            have += len(new)
-            store["fw"][first - base:first - base + n].copy_(flow_fw[:n])
-            store["bw"][first - base:first - base + n].copy_(flow_bw[:n])
-            ran = first + n  # pairs 0 .. ran - 1 have run
-            last = done
-            while last < F and min(last + window, F - 1) <= ran:
-                last += 1
+            Hn, Wn = flow_fw.shape[1:3]
+            s = win.alloc(frames=((Hs, Ws, 3), torch.uint8), fw=((Hn, Wn, 2), torch.float32),
+                          bw=((Hn, Wn, 2), torch.float32))
+            new = win.admit(first + n)
+            r = win.row(first)
+            s["frames"][new].copy_(src[new.start - r:n + 1])
+            s["fw"][r:r + n].copy_(flow_fw[:n])
+            s["bw"][r:r + n].copy_(flow_bw[:n])
+            t0, m, rows = win.finish(first + n, inpaint_rows(F, window, sorted(cuts)))  # pairs .. first + n - 1 ran
             res = None
-            if last > done:
-                rows = inpaint_rows(F, window, sorted(cuts))[done:last].copy()
-                rows[:, 0] -= base
-                res = merge_frames(store["frames"][:have], store["fw"][:have - 1], store["bw"][:have - 1], rows, sigma,
+            if m:
+                res = merge_frames(win.kept("frames"), win.kept_pairs("fw"), win.kept_pairs("bw"), rows, sigma,
                                    engine.flow_scale)
-            pipe.emit(partial(write, first=done, n=last - done), cap, frames=None if res is None else res[0],
+            pipe.emit(partial(write, first=t0, n=m), win.cap, frames=None if res is None else res[0],
                       support=None if res is None else res[1])
-            done = last
     cuts = sorted(cuts)
-    mean = total[0] / (F * Hs * Ws)
+    mean = write.total / (F * Hs * Ws)
     print(f"denoise: sigma {sigma:.4g}, mean support {mean:.3f} frames")
-    print(f"scene cuts: {len(cuts)}" + (" at pairs " + " ".join(str(k) for k in cuts) if cuts else ""))
+    print_cuts(cuts)
     return names, {"sigma": float(sigma), "support": mean, "cuts": cuts}
 
 
@@ -1605,7 +1606,7 @@ def video_segment_motion(model, frames, out, window=None, tau=None, batch=8, wor
     (networks.utils.scene_cut_scores); a cut pair adds no evidence and no chain crosses it.  Prints the pairs with an
     unreliable similarity (a field flagged 2) and with a singular fit (a field flagged 1), the mean moving fraction and
     the cuts.  Returns (paths, info), info a dict of "unreliable", "fallback", "moving" and "cuts"."""
-    from networks.utils import motion_evidence, scene_cut_scores
+    from networks.utils import motion_evidence
     from .motionseg import (DEFAULT_WINDOW, SINGULAR, TAU, UNRELIABLE, check_tau, check_window, cut_flags, fit_fields,
                             segment_frames, segment_rows, to_pixels)
 
@@ -1623,12 +1624,10 @@ def video_segment_motion(model, frames, out, window=None, tau=None, batch=8, wor
     engine = model.engine()
     rgb = bool(model.upstream)
     dev = engine.device
-    cap = min(F, 2 * window + batch + 2)  # frames kept on the GPU
     names = [os.path.join(out, f"mask_{i:06d}.png") for i in range(F)]
     moving, lock = [0], threading.Lock()
     homs, field_flags = np.zeros((F - 1, 3, 3)), np.zeros((2, F - 1), np.uint8)
-    cuts, on_dev, store = [], None, None
-    base = have = done = 0  # store row 0 is frame base; frames base .. base + have - 1 are kept; frames < done written
+    win, upload, cuts = _Window(F, window, batch, dev), _Upload(dev), []
 
     def write(slot, first, n):  # writer thread: the masks of one pass, once its copies have landed
         if slot is None:
@@ -1643,50 +1642,35 @@ def video_segment_motion(model, frames, out, window=None, tau=None, batch=8, wor
     with _Pipeline(paths, passes, rgb, batch, workers, dev) as pipe:
         for j, ps, imgs, src in pipe:
             Hs, Ws = src.shape[1:3]
-            if on_dev is None:
-                on_dev = torch.empty(src.shape, dtype=torch.uint8, device=dev)
-            on_dev.copy_(src, non_blocking=True)
-            if thr is not None:
-                cuts += pass_cuts(ps.pairs, scene_cut_scores(on_dev).cpu(), thr)
-            flow_fw, flow_bw, occ_fw, occ_bw = engine.forward_sequence_bidirectional(on_dev, check=True)
+            src, cut = upload(src, ps.pairs, thr)
+            cuts += cut
+            flow_fw, flow_bw, occ_fw, occ_bw = engine.forward_sequence_bidirectional(src, check=True)
             n = sum(k is not None for k in ps.pairs)
             first = ps.frames[0]
-            if store is None:
-                Hn, Wn = flow_fw.shape[1:3]
-                store = dict(ev=torch.empty(cap, Hn, Wn, 2, dtype=torch.float32, device=dev),
-                             fw=torch.empty(cap, Hn, Wn, 2, dtype=torch.float32, device=dev),
-                             bw=torch.empty(cap, Hn, Wn, 2, dtype=torch.float32, device=dev))
+            Hn, Wn = flow_fw.shape[1:3]
+            s = win.alloc(ev=((Hn, Wn, 2), torch.float32), fw=((Hn, Wn, 2), torch.float32),
+                          bw=((Hn, Wn, 2), torch.float32))
             fw, bw, ofw, obw = flow_fw[:n], flow_bw[:n], occ_fw[:n], occ_bw[:n]
             H, flags = fit_fields(torch.cat([fw, bw]), torch.cat([ofw, obw]), (Hs, Ws), engine.flow_scale)
             ev = motion_evidence(fw, bw, ofw, obw, H, flags, (Hs, Ws), cut_flags(cuts, range(first, first + n), dev),
                                  engine.flow_scale, tau)
             homs[first:first + n] = to_pixels(H[:n].cpu().numpy(), (Hs, Ws))
             field_flags[:, first:first + n] = flags.cpu().numpy().reshape(2, n)
-            new = list(range(base + have, first + n + 1))  # the pass's frames not kept yet
-            if have + len(new) > cap:  # drop the frames no frame still to be written reaches
-                drop = max(done - window, base) - base
-                for t in store.values():
-                    t[:have - drop].copy_(t[drop:have].clone())
-                base, have = base + drop, have - drop
-            k0 = new[0] - first  # 1 when frame `first` holds the previous pass's half of its evidence
+            new = win.admit(first + n)
+            r = win.row(first)
+            k0 = new.start - r  # 1 when frame `first` holds the previous pass's half of its evidence
             if k0:
-                store["ev"][first - base].add_(ev[0])
-            store["ev"][have:have + len(new)].copy_(ev[k0:])
-            have += len(new)
-            store["fw"][first - base:first - base + n].copy_(fw)
-            store["bw"][first - base:first - base + n].copy_(bw)
+                s["ev"][r].add_(ev[0])
+            s["ev"][new].copy_(ev[k0:])
+            s["fw"][r:r + n].copy_(fw)
+            s["bw"][r:r + n].copy_(bw)
             ran = first + n  # pairs 0 .. ran - 1 have run: the evidence of frames < ran is complete (all at the end)
-            last = done
-            while last < F and (ran == F - 1 or min(last + window, F - 1) < ran):
-                last += 1
+            t0, m, rows = win.finish(F - 1 if ran == F - 1 else ran - 1, segment_rows(F, window, sorted(cuts)))
             res = None
-            if last > done:
-                rows = segment_rows(F, window, sorted(cuts))[done:last].copy()
-                rows[:, 0] -= base
-                res = segment_frames(store["ev"][:have], store["fw"][:have - 1], store["bw"][:have - 1], (Hs, Ws),
-                                     rows, engine.flow_scale)
-            pipe.emit(partial(write, first=done, n=last - done), cap, mask=None if res is None else res[0])
-            done = last
+            if m:
+                res = segment_frames(win.kept("ev"), win.kept_pairs("fw"), win.kept_pairs("bw"), (Hs, Ws), rows,
+                                     engine.flow_scale)
+            pipe.emit(partial(write, first=t0, n=m), win.cap, mask=None if res is None else res[0])
     cuts = sorted(cuts)
     np.save(os.path.join(out, "homographies.npy"), homs)
     unreliable = int((field_flags == UNRELIABLE).any(0).sum())
@@ -1694,7 +1678,7 @@ def video_segment_motion(model, frames, out, window=None, tau=None, batch=8, wor
     frac = moving[0] / (F * Hs * Ws)
     print(f"segment motion: {unreliable} pairs with an unreliable similarity, {fallback} with a singular homography "
           f"fit, moving fraction {frac:.4f}")
-    print(f"scene cuts: {len(cuts)}" + (" at pairs " + " ".join(str(k) for k in cuts) if cuts else ""))
+    print_cuts(cuts)
     return names, {"unreliable": unreliable, "fallback": fallback, "moving": frac, "cuts": cuts}
 
 
@@ -1713,8 +1697,7 @@ def _temporal_sweep(model, frames, other, what, batch, workers, scene_cut, stren
     """The one sweep behind video_consistent (strength given) and video_warp_error: per pass the originals and the other
     frames, one forward_sequence_bidirectional(check=False), and each frame whose pair ran in order; the per-pair
     warping-error sums of the originals, of other and (with strength) of the output stay on the GPU until the end."""
-    import cv2
-    from networks.utils import scene_cut_scores, warp_error
+    from networks.utils import warp_error
     from .engine import FB_ALPHA1, FB_ALPHA2
     from .temporal import check_strength, consistent_frame
 
@@ -1734,32 +1717,17 @@ def _temporal_sweep(model, frames, other, what, batch, workers, scene_cut, stren
     rgb = bool(model.upstream)
     dev = engine.device
     cuts = []
-    I_dev = P_dev = None
     prev_out = None  # O of the frame before the pass's next frame
-    sums = counts = None
-
-    def write(slot, first, n):  # writer thread: the output frames of one pass, once its copies have landed
-        if slot is None:
-            return
-        slot.event.synchronize()
-        for r in range(n):
-            img = slot.frames[r].numpy()
-            if not cv2.imwrite(names[first + r], cv2.cvtColor(img, cv2.COLOR_RGB2BGR) if rgb else img):
-                raise OSError(f"cannot write {names[first + r]}")
-
+    upload_I, upload_P, write = _Upload(dev), _Upload(dev), _FrameWriter(names, rgb)
+    sums = torch.zeros(3, F - 1, 2, dtype=torch.float64, device=dev)
+    counts = torch.zeros(4, dtype=torch.int64, device=dev)
     with _Pipeline(paths, passes, rgb, batch, workers, dev, extra=opaths) as pipe:
         for j, ps, imgs, src in pipe:
-            if I_dev is None:
-                I_dev = torch.empty(src.shape, dtype=torch.uint8, device=dev)
-                P_dev = torch.empty(src.shape, dtype=torch.uint8, device=dev)
-                sums = torch.zeros(3, F - 1, 2, dtype=torch.float64, device=dev)
-                counts = torch.zeros(4, dtype=torch.int64, device=dev)
-            I_dev.copy_(src, non_blocking=True)
-            P_dev.copy_(pipe.extra, non_blocking=True)
+            I_dev, cut = upload_I(src, ps.pairs, thr)
+            P_dev, _ = upload_P(pipe.extra, ps.pairs)
+            cuts += cut
             n = sum(k is not None for k in ps.pairs)
             first = ps.frames[0]
-            if thr is not None:
-                cuts += pass_cuts(ps.pairs, scene_cut_scores(I_dev).cpu(), thr)
             fw, bw, _, _ = engine.forward_sequence_bidirectional(I_dev, check=False)
             fw, bw = fw[:n], bw[:n]
             sums[0, first:first + n] = warp_error(I_dev[:n + 1], fw, bw, engine.flow_scale, FB_ALPHA1, FB_ALPHA2)
@@ -1812,8 +1780,7 @@ def video_consistent(model, frames, processed, out, strength, batch=8, workers=4
     print("consistent: E_warp original {:.6g}, processed {:.6g}, output {:.6g}".format(
         info["original"]["E_warp"], info["input"]["E_warp"], info["output"]["E_warp"]))
     print("status: used {} / step failed {} / rejected {} / no previous frame {}".format(*info["status"]))
-    print(f"scene cuts: {len(info['cuts'])}" + (" at pairs " + " ".join(str(k) for k in info["cuts"])
-                                                if info["cuts"] else ""))
+    print_cuts(info["cuts"])
     return names, info
 
 
@@ -1826,6 +1793,5 @@ def video_warp_error(model, frames, video, batch=8, workers=4, scene_cut=None):
     print("warp error: E_warp {:.6g} (original frames {:.6g}) over {} pairs, {} excluded".format(
         info["input"]["E_warp"], info["original"]["E_warp"], len(info["input"]["E_pair"]),
         len(info["input"]["excluded"])))
-    print(f"scene cuts: {len(info['cuts'])}" + (" at pairs " + " ".join(str(k) for k in info["cuts"])
-                                                if info["cuts"] else ""))
+    print_cuts(info["cuts"])
     return info
