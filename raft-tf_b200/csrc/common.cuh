@@ -260,6 +260,11 @@ __device__ __forceinline__ float tanh_f(float x) {  // 1 - 2/(1+e^{2x}); exact l
   return fmaf(-2.0f, rcp_fast(1.0f + ex2_fast(2.8853900817779268f * x)), 1.0f);
 }
 
+// A frame value in [0, 1] as the byte the CLI writes, np.clip(np.rint(fl32(255 * x)), 0, 255): ties to even;
+// fmaxf(NaN, 0) = 0, so a NaN becomes 0.  The interpolation blends write uint8 frames with it, and rb_frame_metrics
+// quantises fp32 predictions with it.
+__device__ __forceinline__ uint8_t quantise(float x) { return (uint8_t)fminf(fmaxf(rintf(__fmul_rn(255.f, x)), 0.f), 255.f); }
+
 // 32-byte global accesses as two 128-bit halves.  The tensor-core epilogues have one pixel per thread, so every lane of a
 // warp-wide access touches a different 32-byte sector: 16 consecutive bytes per instruction keep the number of LSU
 // transactions of the epilogue at one per sector half.  32-byte aligned.

@@ -5,8 +5,6 @@
 // their int64 atomics are exact in any order.
 #include <math.h>
 
-#include <algorithm>
-
 #include "common.cuh"
 #include "fb_sample.cuh"
 
@@ -21,10 +19,6 @@ constexpr int kTaps = kSamp + 1;            // 6 x 6 taps
 constexpr int kSide = 2 * kSearch + 1;
 constexpr int kPw = 2 * kPatch + 1;
 constexpr float kPatchVals = (float)(kPw * kPw * 3);  // 27: d is the mean over the patch's values
-
-struct DenoiseGeom {
-  double rxn, ryn, rxs, rys;  // Wn / Ws, Hn / Hs, Ws / Wn, Hs / Hn
-};
 
 struct MergeAcc {
   float s[3];  // sum of w * centre colour per channel
@@ -83,24 +77,20 @@ __device__ __forceinline__ void merge_frame(const uint8_t* __restrict__ img, int
     }
 }
 
-// One side of pixel p (network position p0) of frame t: up to n steps of rb_track_points' step (dir = +1: pull with fw,
-// test against bw; -1: the mirror); every step that stays on the grid and passes the F5 test is a match, merged at its
-// position mapped back to frame pixels.  Returns the number of matched frames.
+// One side of pixel p (network position p0) of frame t: up to n chain steps (dir = +1 forward, -1 backward); every step
+// that stays on the grid and passes the F5 test is a match, merged at its position mapped back to frame pixels.
+// Returns the number of matched frames.
 __device__ __forceinline__ int denoise_side(const uint8_t* __restrict__ frames, const float2* __restrict__ fw,
                                             const float2* __restrict__ bw, int t, int dir, int n, float2 p, int Hs,
-                                            int Ws, int Hn, int Wn, const DenoiseGeom& g, float s, float a1, float a2,
+                                            int Ws, int Hn, int Wn, const NetGeom& g, float s, float a1, float a2,
                                             const float (&ref)[kPw][kPw][3], float two_var, float den,
                                             MergeAcc& acc) {
   const size_t nn = (size_t)Hn * Wn, ns = (size_t)Hs * Ws;
   int step = 1;
   for (; step <= n; ++step) {
-    const size_t k = (size_t)(dir > 0 ? t + step - 1 : t - step) * nn;
-    const float2* pull = (dir > 0 ? fw : bw) + k;
-    const float2* test = (dir > 0 ? bw : fw) + k;
-    const float2 f = sample_flow(pull, Wn, bilerp_at(p.x, p.y, Hn, Wn), s);
-    const float2 q = make_float2(__fadd_rn(p.x, f.x), __fadd_rn(p.y, f.y));
-    if (!inside_frame(q.x, q.y, Hn, Wn)) break;
-    if (fb_inconsistent(f, sample_flow(test, Wn, bilerp_at(q.x, q.y, Hn, Wn), s), a1, a2)) break;
+    const ChainLink l = chain_link(fw, bw, nn, t, dir, step);
+    float2 q;
+    if (chain_step(l.pull, l.test, Hn, Wn, s, a1, a2, p, q)) break;
     p = q;
     const Bilerp b = bilerp_at(px_remap(p.x, g.rxs, Ws), px_remap(p.y, g.rys, Hs), Hs, Ws);
     merge_frame(frames + (size_t)(t + dir * step) * ns * 3, Hs, Ws, b, ref, two_var, den, acc);
@@ -111,7 +101,7 @@ __device__ __forceinline__ int denoise_side(const uint8_t* __restrict__ frames, 
 // One thread per frame pixel, blockIdx.y over the rows (striding); row r = (t, nf, nb).
 __global__ void __launch_bounds__(kDenoiseThreads) denoise_merge_kernel(
     const uint8_t* __restrict__ frames, int F, int Hs, int Ws, const float2* __restrict__ fw,
-    const float2* __restrict__ bw, int Hn, int Wn, DenoiseGeom g, float s, float a1, float a2,
+    const float2* __restrict__ bw, int Hn, int Wn, NetGeom g, float s, float a1, float a2,
     const int32_t* __restrict__ rows, int n_rows, float sigma, uint8_t* __restrict__ out,
     uint8_t* __restrict__ support) {
   // the weight's constants, each operation rounded on its own: 2 sigma^2 and (H sigma)^2
@@ -202,29 +192,16 @@ extern "C" int rb_denoise_merge(const uint8_t* frames, int F, int Hs, int Ws, co
                                 const float* flow_bw, int Hn, int Wn, float flow_scale, float alpha1, float alpha2,
                                 const int32_t* rows, int n_rows, float sigma, uint8_t* out, uint8_t* support,
                                 void* stream) {
-  RB_REQUIRE(frames && rows && out && support && (F < 2 || (flow_fw && flow_bw)), RB_ERR_BAD_ARG,
-             "rb_denoise_merge: null pointer");
-  RB_REQUIRE(F > 0 && Hs > 0 && Ws > 0 && Hn > 0 && Wn > 0 && n_rows > 0, RB_ERR_BAD_SHAPE,
-             "rb_denoise_merge: bad shape F=%d Hs=%d Ws=%d Hn=%d Wn=%d n_rows=%d", F, Hs, Ws, Hn, Wn, n_rows);
-  RB_REQUIRE((size_t)Hs * Ws < (size_t(1) << 31), RB_ERR_BAD_SHAPE,
-             "rb_denoise_merge: %dx%d pixels per frame exceed one grid", Hs, Ws);
-  RB_REQUIRE(flow_scale > 0.f && isfinite(flow_scale), RB_ERR_BAD_ARG,
-             "rb_denoise_merge: flow_scale must be finite and > 0 (got %g)", (double)flow_scale);
-  RB_REQUIRE(alpha1 >= 0.f && isfinite(alpha1) && alpha2 >= 0.f && isfinite(alpha2), RB_ERR_BAD_ARG,
-             "rb_denoise_merge: alpha1, alpha2 must be finite and >= 0 (got %g, %g)", (double)alpha1, (double)alpha2);
+  const char* fn = "rb_denoise_merge";
+  if (int rc = check_rows_entry(fn, frames && rows && out && support, flow_fw, flow_bw, F, Hs, Ws, Hn, Wn, n_rows))
+    return rc;
+  if (int rc = check_rows_step(fn, Hs, Ws, flow_scale, alpha1, alpha2)) return rc;
   RB_REQUIRE(sigma > 0.f && isfinite(sigma), RB_ERR_BAD_ARG,
              "rb_denoise_merge: sigma must be finite and > 0 (got %g)", (double)sigma);
   RB_REQUIRE(out != frames, RB_ERR_BAD_ARG, "rb_denoise_merge: out must not alias frames");
-  DenoiseGeom g;
-  g.rxn = (double)Wn / (double)Ws;
-  g.ryn = (double)Hn / (double)Hs;
-  g.rxs = (double)Ws / (double)Wn;
-  g.rys = (double)Hs / (double)Hn;
-  const size_t ns = (size_t)Hs * Ws;
-  const dim3 grid((unsigned)((ns + kDenoiseThreads - 1) / kDenoiseThreads), (unsigned)std::min(n_rows, 65535));
-  denoise_merge_kernel<<<grid, kDenoiseThreads, 0, (cudaStream_t)stream>>>(
-      frames, F, Hs, Ws, reinterpret_cast<const float2*>(flow_fw), reinterpret_cast<const float2*>(flow_bw), Hn, Wn, g,
-      flow_scale, alpha1, alpha2, rows, n_rows, sigma, out, support);
+  denoise_merge_kernel<<<rows_grid(Hs, Ws, kDenoiseThreads, n_rows), kDenoiseThreads, 0, (cudaStream_t)stream>>>(
+      frames, F, Hs, Ws, reinterpret_cast<const float2*>(flow_fw), reinterpret_cast<const float2*>(flow_bw), Hn, Wn,
+      net_geom(Hs, Ws, Hn, Wn), flow_scale, alpha1, alpha2, rows, n_rows, sigma, out, support);
   RB_CHECK_LAUNCH("denoise_merge_kernel");
   return RB_OK;
 }

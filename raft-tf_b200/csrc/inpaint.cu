@@ -411,46 +411,26 @@ __global__ void __launch_bounds__(256) inpaint_grid_kernel(const uint8_t* __rest
   hole_net[(size_t)blockIdx.y * nn + q] = out;
 }
 
-struct InpaintGeom {
-  double rxn, ryn, rxs, rys;  // Wn / Ws, Hn / Hs, Ws / Wn, Hs / Hn
-};
-
-// x' = fl32((x + 0.5) r - 0.5) in fp64, each operation rounded on its own, clamped into [0, n - 1] (track_queries /
-// tracks_to_frames).
-__device__ __forceinline__ float remap(double x, double r, int n) {
-  const float v = __double2float_rn(__dsub_rn(__dmul_rn(__dadd_rn(x, 0.5), r), 0.5));
-  return fminf(fmaxf(v, 0.f), (float)(n - 1));
-}
-
-// One side of hole pixel p (network position p0) of frame t: up to n steps of rb_track_points' step (dir = +1: pull
-// with fw, test against bw; -1: the mirror), each followed by the visibility test of the position's four taps in the
-// frame reached.  Returns the distance (0: not found) and the colour.
+// One side of hole pixel p (network position p0) of frame t: up to n chain steps (dir = +1 forward, -1 backward), each
+// followed by the visibility test of the position's four taps in the frame reached.  Returns the distance (0: not
+// found) and the colour.
 __device__ __forceinline__ int inpaint_side(const uint8_t* __restrict__ frames, const uint8_t* __restrict__ hole,
                                             const float2* __restrict__ fw, const float2* __restrict__ bw, int t, int dir,
-                                            int n, float2 p, int Hs, int Ws, int Hn, int Wn, const InpaintGeom& g,
+                                            int n, float2 p, int Hs, int Ws, int Hn, int Wn, const NetGeom& g,
                                             float s, float a1, float a2, float* col) {
   const size_t nn = (size_t)Hn * Wn, ns = (size_t)Hs * Ws;
   for (int step = 1; step <= n; ++step) {
-    const size_t k = (size_t)(dir > 0 ? t + step - 1 : t - step) * nn;
-    const float2* pull = (dir > 0 ? fw : bw) + k;
-    const float2* test = (dir > 0 ? bw : fw) + k;
-    const float2 f = sample_flow(pull, Wn, bilerp_at(p.x, p.y, Hn, Wn), s);
-    const float2 q = make_float2(__fadd_rn(p.x, f.x), __fadd_rn(p.y, f.y));
-    if (!inside_frame(q.x, q.y, Hn, Wn)) return 0;
-    if (fb_inconsistent(f, sample_flow(test, Wn, bilerp_at(q.x, q.y, Hn, Wn), s), a1, a2)) return 0;
+    const ChainLink l = chain_link(fw, bw, nn, t, dir, step);
+    float2 q;
+    if (chain_step(l.pull, l.test, Hn, Wn, s, a1, a2, p, q)) return 0;
     p = q;
     const int fr = t + dir * step;
-    const Bilerp b = bilerp_at(remap(p.x, g.rxs, Ws), remap(p.y, g.rys, Hs), Hs, Ws);
+    const Bilerp b = bilerp_at(px_remap(p.x, g.rxs, Ws), px_remap(p.y, g.rys, Hs), Hs, Ws);
     const uint8_t* h = hole + (size_t)fr * ns;
     if (h[(size_t)b.y0 * Ws + b.x0] | h[(size_t)b.y0 * Ws + b.x1] | h[(size_t)b.y1 * Ws + b.x0] |
         h[(size_t)b.y1 * Ws + b.x1])
       continue;
-    const uint8_t* img = frames + (size_t)fr * ns * 3;
-    const size_t i00 = ((size_t)b.y0 * Ws + b.x0) * 3, i01 = ((size_t)b.y0 * Ws + b.x1) * 3;
-    const size_t i10 = ((size_t)b.y1 * Ws + b.x0) * 3, i11 = ((size_t)b.y1 * Ws + b.x1) * 3;
-#pragma unroll
-    for (int c = 0; c < 3; ++c)
-      col[c] = bilerp1(b, (float)img[i00 + c], (float)img[i01 + c], (float)img[i10 + c], (float)img[i11 + c]);
+    sample_rgb(frames + (size_t)fr * ns * 3, Ws, b, col);
     return step;
   }
   return 0;
@@ -459,7 +439,7 @@ __device__ __forceinline__ int inpaint_side(const uint8_t* __restrict__ frames, 
 // One thread per frame pixel, blockIdx.y over the rows (striding); row r = (t, nf, nb).
 __global__ void __launch_bounds__(256) inpaint_propagate_kernel(
     const uint8_t* __restrict__ frames, const uint8_t* __restrict__ hole, int F, int Hs, int Ws,
-    const float2* __restrict__ fw, const float2* __restrict__ bw, int Hn, int Wn, InpaintGeom g, float s, float a1,
+    const float2* __restrict__ fw, const float2* __restrict__ bw, int Hn, int Wn, NetGeom g, float s, float a1,
     float a2, const int32_t* __restrict__ rows, int n_rows, float* __restrict__ colour, uint8_t* __restrict__ status) {
   const size_t ns = (size_t)Hs * Ws;
   const size_t q = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -482,25 +462,12 @@ __global__ void __launch_bounds__(256) inpaint_propagate_kernel(
       *st = 0;
       continue;
     }
-    const float2 p = make_float2(remap(x, g.rxn, Wn), remap(y, g.ryn, Hn));
+    const float2 p = make_float2(px_remap(x, g.rxn, Wn), px_remap(y, g.ryn, Hn));
     float cf[3], cb[3];
     const int df = inpaint_side(frames, hole, fw, bw, t, 1, min(max(nf, 0), F - 1 - t), p, Hs, Ws, Hn, Wn, g, s, a1,
                                 a2, cf);
     const int db = inpaint_side(frames, hole, fw, bw, t, -1, min(max(nb, 0), t), p, Hs, Ws, Hn, Wn, g, s, a1, a2, cb);
-    if (df && db) {
-      const float wf = (float)db, wb = (float)df, den = (float)(df + db);
-#pragma unroll
-      for (int c = 0; c < 3; ++c) out[c] = __fdiv_rn(__fadd_rn(__fmul_rn(wf, cf[c]), __fmul_rn(wb, cb[c])), den);
-      *st = 1;
-    } else if (df || db) {
-#pragma unroll
-      for (int c = 0; c < 3; ++c) out[c] = df ? cf[c] : cb[c];
-      *st = 2;
-    } else {
-#pragma unroll
-      for (int c = 0; c < 3; ++c) out[c] = 0.f;
-      *st = 3;
-    }
+    blend_sides(df, cf, db, cb, out, st);
   }
 }
 
@@ -655,27 +622,14 @@ extern "C" int rb_inpaint_propagate(const uint8_t* frames, const uint8_t* hole, 
                                     const float* flow_fw, const float* flow_bw, int Hn, int Wn, float flow_scale,
                                     float alpha1, float alpha2, const int32_t* rows, int n_rows, float* colour,
                                     uint8_t* status, void* stream) {
-  RB_REQUIRE(frames && hole && rows && colour && status && (F < 2 || (flow_fw && flow_bw)), RB_ERR_BAD_ARG,
-             "rb_inpaint_propagate: null pointer");
-  RB_REQUIRE(F > 0 && Hs > 0 && Ws > 0 && Hn > 0 && Wn > 0 && n_rows > 0, RB_ERR_BAD_SHAPE,
-             "rb_inpaint_propagate: bad shape F=%d Hs=%d Ws=%d Hn=%d Wn=%d n_rows=%d", F, Hs, Ws, Hn, Wn, n_rows);
-  RB_REQUIRE((size_t)Hs * Ws < (size_t(1) << 31), RB_ERR_BAD_SHAPE,
-             "rb_inpaint_propagate: %dx%d pixels per frame exceed one grid", Hs, Ws);
-  RB_REQUIRE(flow_scale > 0.f && isfinite(flow_scale), RB_ERR_BAD_ARG,
-             "rb_inpaint_propagate: flow_scale must be finite and > 0 (got %g)", (double)flow_scale);
-  RB_REQUIRE(alpha1 >= 0.f && isfinite(alpha1) && alpha2 >= 0.f && isfinite(alpha2), RB_ERR_BAD_ARG,
-             "rb_inpaint_propagate: alpha1, alpha2 must be finite and >= 0 (got %g, %g)", (double)alpha1,
-             (double)alpha2);
-  InpaintGeom g;
-  g.rxn = (double)Wn / (double)Ws;
-  g.ryn = (double)Hn / (double)Hs;
-  g.rxs = (double)Ws / (double)Wn;
-  g.rys = (double)Hs / (double)Hn;
-  const size_t ns = (size_t)Hs * Ws;
-  const dim3 grid((unsigned)((ns + 255) / 256), (unsigned)std::min(n_rows, 65535));
-  inpaint_propagate_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(
+  const char* fn = "rb_inpaint_propagate";
+  if (int rc = check_rows_entry(fn, frames && hole && rows && colour && status, flow_fw, flow_bw, F, Hs, Ws, Hn, Wn,
+                                n_rows))
+    return rc;
+  if (int rc = check_rows_step(fn, Hs, Ws, flow_scale, alpha1, alpha2)) return rc;
+  inpaint_propagate_kernel<<<rows_grid(Hs, Ws, 256, n_rows), 256, 0, (cudaStream_t)stream>>>(
       frames, hole, F, Hs, Ws, reinterpret_cast<const float2*>(flow_fw), reinterpret_cast<const float2*>(flow_bw), Hn,
-      Wn, g, flow_scale, alpha1, alpha2, rows, n_rows, colour, status);
+      Wn, net_geom(Hs, Ws, Hn, Wn), flow_scale, alpha1, alpha2, rows, n_rows, colour, status);
   RB_CHECK_LAUNCH("inpaint_propagate_kernel");
   return RB_OK;
 }

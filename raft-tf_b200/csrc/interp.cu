@@ -249,9 +249,6 @@ __global__ void __launch_bounds__(256) erode5_kernel(const uint8_t* __restrict__
   out[i] = m;
 }
 
-// the CLI's np.clip(np.rint(fl32(255 * x)), 0, 255), as rb_frame_metrics quantises: ties to even; fmaxf(NaN, 0) = 0
-__device__ __forceinline__ uint8_t quantise(float x) { return (uint8_t)fminf(fmaxf(rintf(__fmul_rn(255.f, x)), 0.f), 255.f); }
-
 // One frame of a blend as fp32 values: pixel (y, x), channel c of frame `img`, rows `row` values apart.  CropF32 reads
 // fp32 frames (the engine's padded images from the crop's first pixel, or raw frames); RawU8 reads uint8 frames and
 // scales them as rb_frames_prepare does (np.float32(u) / 255, from a table of the 256 quotients).
@@ -330,12 +327,6 @@ __device__ __forceinline__ void resized_px(const float* __restrict__ f0, const f
   F1 = make_float2(__fmul_rn(c[0], su), __fmul_rn(c[1], sv));
   m0 = __ldg(e0 + smp * lhw + near) != 0;
   m1 = __ldg(e1 + smp * lhw + near) != 0;
-}
-
-// the network pixel whose area holds the centre of output pixel (x, y): (((2x+1) W) div (2 Ws), ((2y+1) H) div (2 Hs))
-__device__ __forceinline__ size_t near_px(int x, int y, int H, int W, int Hs, int Ws) {
-  return (size_t)(((2 * (uint64_t)y + 1) * (uint64_t)H) / (2 * (uint64_t)Hs)) * W +
-         (size_t)(((2 * (uint64_t)x + 1) * (uint64_t)W) / (2 * (uint64_t)Ws));
 }
 
 // One thread per output pixel, blockIdx.y striding over the (time, sample) pairs (32-bit pixel indices; a pair is

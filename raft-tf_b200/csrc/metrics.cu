@@ -109,11 +109,6 @@ struct Gauss11 {
   double w[kFmR + 1];  // w[k] = weight of offsets +-k
 };
 
-__device__ __forceinline__ uint8_t quantise(float x) {
-  // the CLI's np.clip(np.rint(fl32(255 * x)), 0, 255): ties to even; fmaxf(NaN, 0) = 0, so a NaN becomes 0
-  return (uint8_t)fminf(fmaxf(rintf(__fmul_rn(255.f, x)), 0.f), 255.f);
-}
-
 __global__ void __launch_bounds__(kMetricsThreads) frame_metrics_tile_kernel(
     const void* __restrict__ pred, int pred_is_u8, const uint8_t* __restrict__ gt, int H, int W, int tiles_x,
     Gauss11 g, double* __restrict__ partials) {

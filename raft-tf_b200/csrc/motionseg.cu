@@ -250,11 +250,12 @@ __device__ __forceinline__ float2 sample_ev(const float2* __restrict__ ev, int W
   return make_float2(bilerp1(b, v00.x, v01.x, v10.x, v11.x), bilerp1(b, v00.y, v01.y, v10.y, v11.y));
 }
 
-// One thread per frame pixel, blockIdx.y over the rows (striding); row r = (t, nf, nb).  The chain is rb_denoise_merge's.
+// One thread per frame pixel, blockIdx.y over the rows (striding); row r = (t, nf, nb).  Each side chains steps until
+// one leaves the grid or fails the F5 test, as rb_denoise_merge's sides do.
 __global__ void __launch_bounds__(kSegThreads) motion_segment_kernel(const float2* __restrict__ ev, int F, int Hn, int Wn,
                                                                      const float2* __restrict__ fw,
                                                                      const float2* __restrict__ bw, int Hs, int Ws,
-                                                                     double rxn, double ryn, float s, float a1, float a2,
+                                                                     NetGeom g, float s, float a1, float a2,
                                                                      const int32_t* __restrict__ rows, int n_rows,
                                                                      uint8_t* __restrict__ mask,
                                                                      uint8_t* __restrict__ status) {
@@ -270,7 +271,7 @@ __global__ void __launch_bounds__(kSegThreads) motion_segment_kernel(const float
       status[o] = 1;
       continue;
     }
-    const float2 p0 = make_float2(px_remap(x, rxn, Wn), px_remap(y, ryn, Hn));
+    const float2 p0 = make_float2(px_remap(x, g.rxn, Wn), px_remap(y, g.ryn, Hn));
     float2 acc = sample_ev(ev + (size_t)t * nn, Wn, bilerp_at(p0.x, p0.y, Hn, Wn));
 #pragma unroll 1
     for (int dir = 1; dir >= -1; dir -= 2) {
@@ -278,13 +279,9 @@ __global__ void __launch_bounds__(kSegThreads) motion_segment_kernel(const float
                             : min(min(max(nb, 0), RB_MOTION_SEG_MAX_WINDOW), t);
       float2 p = p0;
       for (int step = 1; step <= n; ++step) {
-        const size_t k = (size_t)(dir > 0 ? t + step - 1 : t - step) * nn;
-        const float2* pull = (dir > 0 ? fw : bw) + k;
-        const float2* test = (dir > 0 ? bw : fw) + k;
-        const float2 f = sample_flow(pull, Wn, bilerp_at(p.x, p.y, Hn, Wn), s);
-        const float2 qq = make_float2(__fadd_rn(p.x, f.x), __fadd_rn(p.y, f.y));
-        if (!inside_frame(qq.x, qq.y, Hn, Wn)) break;
-        if (fb_inconsistent(f, sample_flow(test, Wn, bilerp_at(qq.x, qq.y, Hn, Wn), s), a1, a2)) break;
+        const ChainLink l = chain_link(fw, bw, nn, t, dir, step);
+        float2 qq;
+        if (chain_step(l.pull, l.test, Hn, Wn, s, a1, a2, p, qq)) break;
         p = qq;
         const float2 e = sample_ev(ev + (size_t)(t + dir * step) * nn, Wn, bilerp_at(p.x, p.y, Hn, Wn));
         acc = make_float2(__fadd_rn(acc.x, e.x), __fadd_rn(acc.y, e.y));
@@ -386,22 +383,14 @@ extern "C" int rb_motion_evidence(const float* flow_fw, const float* flow_bw, co
 extern "C" int rb_motion_segment(const float* evidence, int F, int Hn, int Wn, const float* flow_fw,
                                  const float* flow_bw, int Hs, int Ws, float flow_scale, float alpha1, float alpha2,
                                  const int32_t* rows, int n_rows, uint8_t* mask, uint8_t* status, void* stream) {
-  RB_REQUIRE(evidence && rows && mask && status && (F < 2 || (flow_fw && flow_bw)), RB_ERR_BAD_ARG,
-             "rb_motion_segment: null pointer");
-  RB_REQUIRE(F > 0 && Hs > 0 && Ws > 0 && Hn > 0 && Wn > 0 && n_rows > 0, RB_ERR_BAD_SHAPE,
-             "rb_motion_segment: bad shape F=%d Hs=%d Ws=%d Hn=%d Wn=%d n_rows=%d", F, Hs, Ws, Hn, Wn, n_rows);
-  RB_REQUIRE((size_t)Hs * Ws < (size_t(1) << 31), RB_ERR_BAD_SHAPE,
-             "rb_motion_segment: %dx%d pixels per frame exceed one grid", Hs, Ws);
-  RB_REQUIRE(flow_scale > 0.f && isfinite(flow_scale), RB_ERR_BAD_ARG,
-             "rb_motion_segment: flow_scale must be finite and > 0 (got %g)", (double)flow_scale);
-  RB_REQUIRE(alpha1 >= 0.f && isfinite(alpha1) && alpha2 >= 0.f && isfinite(alpha2), RB_ERR_BAD_ARG,
-             "rb_motion_segment: alpha1, alpha2 must be finite and >= 0 (got %g, %g)", (double)alpha1, (double)alpha2);
-  const size_t ns = (size_t)Hs * Ws;
-  const dim3 grid((unsigned)((ns + kSegThreads - 1) / kSegThreads), (unsigned)std::min(n_rows, 65535));
-  motion_segment_kernel<<<grid, kSegThreads, 0, (cudaStream_t)stream>>>(
+  const char* fn = "rb_motion_segment";
+  if (int rc = check_rows_entry(fn, evidence && rows && mask && status, flow_fw, flow_bw, F, Hs, Ws, Hn, Wn, n_rows))
+    return rc;
+  if (int rc = check_rows_step(fn, Hs, Ws, flow_scale, alpha1, alpha2)) return rc;
+  motion_segment_kernel<<<rows_grid(Hs, Ws, kSegThreads, n_rows), kSegThreads, 0, (cudaStream_t)stream>>>(
       reinterpret_cast<const float2*>(evidence), F, Hn, Wn, reinterpret_cast<const float2*>(flow_fw),
-      reinterpret_cast<const float2*>(flow_bw), Hs, Ws, (double)Wn / (double)Ws, (double)Hn / (double)Hs, flow_scale,
-      alpha1, alpha2, rows, n_rows, mask, status);
+      reinterpret_cast<const float2*>(flow_bw), Hs, Ws, net_geom(Hs, Ws, Hn, Wn), flow_scale, alpha1, alpha2, rows,
+      n_rows, mask, status);
   RB_CHECK_LAUNCH("motion_segment_kernel");
   return RB_OK;
 }

@@ -101,12 +101,6 @@ __device__ __forceinline__ uint8_t vote(const uint8_t* l, const float* w) {
   return best;
 }
 
-// The network pixel holding the centre of output pixel (x, y) (rb_frame_synthesize_*_resized's `nearest`).
-__device__ __forceinline__ size_t near_pixel(int x, int y, int H, int W, int Hs, int Ws) {
-  return (size_t)(((2 * (uint64_t)y + 1) * (uint64_t)H) / (2 * (uint64_t)Hs)) * W +
-         (size_t)(((2 * (uint64_t)x + 1) * (uint64_t)W) / (2 * (uint64_t)Ws));
-}
-
 // The keyframe's labels at each output pixel p of Hs x Ws, row blockIdx.y (striding): side_taps of the row and the vote of
 // its four taps.
 __global__ void __launch_bounds__(256) labels_propagate_kernel(const float* __restrict__ acc,
@@ -120,7 +114,7 @@ __global__ void __launch_bounds__(256) labels_propagate_kernel(const float* __re
   if (q >= hw) return;
   const int x = (int)(q % (uint32_t)Ws), y = (int)(q / (uint32_t)Ws);
   const size_t lhw = (size_t)H * W;
-  const size_t near = near_pixel(x, y, H, W, Hs, Ws);
+  const size_t near = near_px(x, y, H, W, Hs, Ws);
   for (uint32_t r = blockIdx.y; r < (uint32_t)n; r += gridDim.y) {
     const SideTaps t = side_taps(acc + (size_t)r * lhw * 2, status + (size_t)r * lhw, H, W, key, Hs, Ws, mode, su, sv,
                                  x, y, near);
@@ -145,7 +139,7 @@ __global__ void __launch_bounds__(256) labels_propagate_keys_kernel(
   if (q >= hw) return;
   const int x = (int)(q % (uint32_t)Ws), y = (int)(q / (uint32_t)Ws);
   const size_t lhw = (size_t)H * W;
-  const size_t near = near_pixel(x, y, H, W, Hs, Ws);
+  const size_t near = near_px(x, y, H, W, Hs, Ws);
   for (uint32_t r = blockIdx.y; r < (uint32_t)n; r += gridDim.y) {
     const int4 row = __ldg(rows + r);
     const bool has_a = row.x >= 0 && row.x < m, has_b = row.y >= 0 && row.y < m;

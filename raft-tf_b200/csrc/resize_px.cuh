@@ -84,6 +84,13 @@ __host__ __device__ inline int float_mode(int H, int W, int Ho, int Wo) {
   return (H == Ho && W == Wo) ? RS_COPY : (H == 1 || W == 1) ? RS_OPENCV : RS_IPP;
 }
 
+// The H x W network pixel whose area holds the centre of Hs x Ws output pixel (x, y): (((2x+1) W) div (2 Ws),
+// ((2y+1) H) div (2 Hs)), as a raster index
+__device__ __forceinline__ size_t near_px(int x, int y, int H, int W, int Hs, int Ws) {
+  return (size_t)(((2 * (uint64_t)y + 1) * (uint64_t)H) / (2 * (uint64_t)Hs)) * W +
+         (size_t)(((2 * (uint64_t)x + 1) * (uint64_t)W) / (2 * (uint64_t)Ws));
+}
+
 // resize_flow's factors u *= dW / float(W_), v *= dH / float(H_): the float64 quotient rounded to fp32 (numpy >= 2,
 // float32 array)
 inline float flow_scale_u(int W, int Wo) { return (float)((double)Wo / (double)W); }

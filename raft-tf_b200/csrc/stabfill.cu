@@ -59,40 +59,32 @@ __global__ void __launch_bounds__(256) flow_extend_kernel(const float2* __restri
   }
 }
 
+// The frames' ratios to the network grid, and the Hc x Wc canvas of the extended flows: the grid with my / mx network
+// pixels added on each side.
 struct FillGeom {
-  double rxn, ryn, rxs, rys;  // Wn / Ws, Hn / Hs, Ws / Wn, Hs / Hn
+  NetGeom r;
   int Hs, Ws, Hc, Wc, my, mx;
 };
 
-// One side of a source outside frame t at canvas position p: up to n steps of rb_track_points' step on the extended
-// flows (dir = +1: pull with fw, test against bw; -1: the mirror), stopping when the position leaves the canvas or fails
-// the forward-backward test; found at the first frame t + dir n whose own pixels hold the position, unclamped.  Returns
-// the distance (0: not found) and the colour.
+// One side of a source outside frame t at canvas position p: up to n chain steps on the extended flows (dir = +1
+// forward, -1 backward), stopping when the position leaves the canvas or fails the forward-backward test; found at the
+// first frame t + dir n whose own pixels hold the position, unclamped.  Returns the distance (0: not found) and the
+// colour.
 __device__ __forceinline__ int fill_side(const uint8_t* __restrict__ frames, const float2* __restrict__ fw,
                                          const float2* __restrict__ bw, int t, int dir, int n, float2 p,
                                          const FillGeom& g, float s, float a1, float a2, float* col) {
   const size_t nc = (size_t)g.Hc * g.Wc, ns = (size_t)g.Hs * g.Ws;
   if (!inside_frame(p.x, p.y, g.Hc, g.Wc)) return 0;
   for (int step = 1; step <= n; ++step) {
-    const size_t k = (size_t)(dir > 0 ? t + step - 1 : t - step) * nc;
-    const float2* pull = (dir > 0 ? fw : bw) + k;
-    const float2* test = (dir > 0 ? bw : fw) + k;
-    const float2 f = sample_flow(pull, g.Wc, bilerp_at(p.x, p.y, g.Hc, g.Wc), s);
-    const float2 q = make_float2(__fadd_rn(p.x, f.x), __fadd_rn(p.y, f.y));
-    if (!inside_frame(q.x, q.y, g.Hc, g.Wc)) return 0;
-    if (fb_inconsistent(f, sample_flow(test, g.Wc, bilerp_at(q.x, q.y, g.Hc, g.Wc), s), a1, a2)) return 0;
+    const ChainLink l = chain_link(fw, bw, nc, t, dir, step);
+    float2 q;
+    if (chain_step(l.pull, l.test, g.Hc, g.Wc, s, a1, a2, p, q)) return 0;
     p = q;
     // canvas -> network (exact in fp64) -> frame pixels by the pixel-centre rule, unclamped
-    const float ox = __double2float_rn(__dsub_rn(__dmul_rn(__dadd_rn(__dsub_rn((double)p.x, g.mx), 0.5), g.rxs), 0.5));
-    const float oy = __double2float_rn(__dsub_rn(__dmul_rn(__dadd_rn(__dsub_rn((double)p.y, g.my), 0.5), g.rys), 0.5));
+    const float ox = __double2float_rn(px_map(__dsub_rn((double)p.x, g.mx), g.r.rxs));
+    const float oy = __double2float_rn(px_map(__dsub_rn((double)p.y, g.my), g.r.rys));
     if (!inside_frame(ox, oy, g.Hs, g.Ws)) continue;
-    const Bilerp b = bilerp_at(ox, oy, g.Hs, g.Ws);
-    const uint8_t* img = frames + (size_t)(t + dir * step) * ns * 3;
-    const size_t i00 = ((size_t)b.y0 * g.Ws + b.x0) * 3, i01 = ((size_t)b.y0 * g.Ws + b.x1) * 3;
-    const size_t i10 = ((size_t)b.y1 * g.Ws + b.x0) * 3, i11 = ((size_t)b.y1 * g.Ws + b.x1) * 3;
-#pragma unroll
-    for (int c = 0; c < 3; ++c)
-      col[c] = bilerp1(b, (float)img[i00 + c], (float)img[i01 + c], (float)img[i10 + c], (float)img[i11 + c]);
+    sample_rgb(frames + (size_t)(t + dir * step) * ns * 3, g.Ws, bilerp_at(ox, oy, g.Hs, g.Ws), col);
     return step;
   }
   return 0;
@@ -124,36 +116,17 @@ __global__ void __launch_bounds__(256) frames_warp_affine_fill_kernel(
     const float fx = __double2float_rn(sx), fy = __double2float_rn(sy);
     if (inside_frame(fx, fy, Hs, Ws) || isnan(fx) || isnan(fy)) {  // rb_frames_warp_affine's value before rounding
       const Bilerp bl = bilerp_at(fminf(fmaxf(fx, 0.f), (float)(Ws - 1)), fminf(fmaxf(fy, 0.f), (float)(Hs - 1)), Hs, Ws);
-      const uint8_t* img = frames + (size_t)t * ns * 3;
-      const size_t i00 = ((size_t)bl.y0 * Ws + bl.x0) * 3, i01 = ((size_t)bl.y0 * Ws + bl.x1) * 3;
-      const size_t i10 = ((size_t)bl.y1 * Ws + bl.x0) * 3, i11 = ((size_t)bl.y1 * Ws + bl.x1) * 3;
-#pragma unroll
-      for (int c = 0; c < 3; ++c)
-        out[c] = bilerp1(bl, (float)img[i00 + c], (float)img[i01 + c], (float)img[i10 + c], (float)img[i11 + c]);
+      sample_rgb(frames + (size_t)t * ns * 3, Ws, bl, out);
       *st = 0;
       continue;
     }
     // the source on the canvas: the pixel-centre rule to the network grid (unclamped), shifted by the margin
-    const float2 p = make_float2(
-        __double2float_rn(__dadd_rn(__dsub_rn(__dmul_rn(__dadd_rn(sx, 0.5), g.rxn), 0.5), (double)g.mx)),
-        __double2float_rn(__dadd_rn(__dsub_rn(__dmul_rn(__dadd_rn(sy, 0.5), g.ryn), 0.5), (double)g.my)));
+    const float2 p = make_float2(__double2float_rn(__dadd_rn(px_map(sx, g.r.rxn), (double)g.mx)),
+                                 __double2float_rn(__dadd_rn(px_map(sy, g.r.ryn), (double)g.my)));
     float cf[3], cb[3];
     const int df = fill_side(frames, fw, bw, t, 1, min(max(nf, 0), F - 1 - t), p, g, s, a1, a2, cf);
     const int db = fill_side(frames, fw, bw, t, -1, min(max(nb, 0), t), p, g, s, a1, a2, cb);
-    if (df && db) {
-      const float wf = (float)db, wb = (float)df, den = (float)(df + db);
-#pragma unroll
-      for (int c = 0; c < 3; ++c) out[c] = __fdiv_rn(__fadd_rn(__fmul_rn(wf, cf[c]), __fmul_rn(wb, cb[c])), den);
-      *st = 1;
-    } else if (df || db) {
-#pragma unroll
-      for (int c = 0; c < 3; ++c) out[c] = df ? cf[c] : cb[c];
-      *st = 2;
-    } else {
-#pragma unroll
-      for (int c = 0; c < 3; ++c) out[c] = 0.f;
-      *st = 3;
-    }
+    blend_sides(df, cf, db, cb, out, st);
   }
 }
 
@@ -215,10 +188,9 @@ extern "C" int rb_frames_warp_affine_fill(const uint8_t* frames, int F, int Hs, 
                                           const float* ext_bw, int Hn, int Wn, int my, int mx, float flow_scale,
                                           float alpha1, float alpha2, const double* A, const int32_t* rows, int n_rows,
                                           float* colour, uint8_t* status, void* stream) {
-  RB_REQUIRE(frames && A && rows && colour && status && (F < 2 || (ext_fw && ext_bw)), RB_ERR_BAD_ARG,
-             "rb_frames_warp_affine_fill: null pointer");
-  RB_REQUIRE(F > 0 && Hs > 0 && Ws > 0 && Hn > 0 && Wn > 0 && n_rows > 0, RB_ERR_BAD_SHAPE,
-             "rb_frames_warp_affine_fill: bad shape F=%d Hs=%d Ws=%d Hn=%d Wn=%d n_rows=%d", F, Hs, Ws, Hn, Wn, n_rows);
+  const char* fn = "rb_frames_warp_affine_fill";
+  if (int rc = check_rows_entry(fn, frames && A && rows && colour && status, ext_fw, ext_bw, F, Hs, Ws, Hn, Wn, n_rows))
+    return rc;
   RB_REQUIRE(my >= 0 && mx >= 0, RB_ERR_BAD_SHAPE, "rb_frames_warp_affine_fill: margins must be >= 0 (got my=%d mx=%d)",
              my, mx);
   const int64_t Hc = (int64_t)Hn + 2 * (int64_t)my, Wc = (int64_t)Wn + 2 * (int64_t)mx;
@@ -226,25 +198,9 @@ extern "C" int rb_frames_warp_affine_fill(const uint8_t* frames, int F, int Hs, 
                  Wc < (1 << 24) && Hc * Wc < (int64_t(1) << 31),
              RB_ERR_BAD_SHAPE, "rb_frames_warp_affine_fill: %dx%d frames or %lldx%lld canvases exceed one grid", Hs, Ws,
              (long long)Hc, (long long)Wc);
-  RB_REQUIRE(flow_scale > 0.f && isfinite(flow_scale), RB_ERR_BAD_ARG,
-             "rb_frames_warp_affine_fill: flow_scale must be finite and > 0 (got %g)", (double)flow_scale);
-  RB_REQUIRE(alpha1 >= 0.f && isfinite(alpha1) && alpha2 >= 0.f && isfinite(alpha2), RB_ERR_BAD_ARG,
-             "rb_frames_warp_affine_fill: alpha1, alpha2 must be finite and >= 0 (got %g, %g)", (double)alpha1,
-             (double)alpha2);
-  FillGeom g;
-  g.rxn = (double)Wn / (double)Ws;
-  g.ryn = (double)Hn / (double)Hs;
-  g.rxs = (double)Ws / (double)Wn;
-  g.rys = (double)Hs / (double)Hn;
-  g.Hs = Hs;
-  g.Ws = Ws;
-  g.Hc = (int)Hc;
-  g.Wc = (int)Wc;
-  g.my = my;
-  g.mx = mx;
-  const size_t ns = (size_t)Hs * Ws;
-  const dim3 grid((unsigned)((ns + 255) / 256), (unsigned)std::min(n_rows, 65535));
-  frames_warp_affine_fill_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(
+  if (int rc = check_rows_step(fn, Hs, Ws, flow_scale, alpha1, alpha2)) return rc;
+  const FillGeom g = {net_geom(Hs, Ws, Hn, Wn), Hs, Ws, (int)Hc, (int)Wc, my, mx};
+  frames_warp_affine_fill_kernel<<<rows_grid(Hs, Ws, 256, n_rows), 256, 0, (cudaStream_t)stream>>>(
       frames, F, reinterpret_cast<const float2*>(ext_fw), reinterpret_cast<const float2*>(ext_bw), g, flow_scale, alpha1,
       alpha2, A, rows, n_rows, colour, status);
   RB_CHECK_LAUNCH("frames_warp_affine_fill_kernel");

@@ -20,19 +20,6 @@ constexpr int kDotChunk = kTconsThreads * kDotPerThread;  // pixels per block of
 constexpr int kWarpPerThread = 16;
 constexpr int kWarpChunk = kTconsThreads * kWarpPerThread;  // pixels per block of the warping error
 
-struct TconsGeom {
-  double rxn, ryn, rxs, rys;  // Wn / Ws, Hn / Hs, Ws / Wn, Hs / Hn
-};
-
-TconsGeom tcons_geom(int Hs, int Ws, int Hn, int Wn) {
-  TconsGeom g;
-  g.rxn = (double)Wn / (double)Ws;
-  g.ryn = (double)Hn / (double)Hs;
-  g.rxs = (double)Ws / (double)Wn;
-  g.rys = (double)Hs / (double)Hn;
-  return g;
-}
-
 // Fixed-shape tree over the block: s[t] += s[t + h] for h = 128, 64, ..., 1.
 __device__ __forceinline__ double tc_block_sum(double v, double* s) {
   const int t = threadIdx.x;
@@ -48,31 +35,23 @@ __device__ __forceinline__ double tc_block_sum(double v, double* s) {
   return r;
 }
 
-// One step of pixel (x, y) of a frame through pull (tested against test) on the network grid, mapped back to the frame:
-// true and the bilinear taps of o when the step stays on the grid and passes the F5 test.
+// One chain step of pixel (x, y) of a frame through pull (tested against test) on the network grid, mapped back to the
+// frame: true and the bilinear taps of the target when the step stays on the grid and passes the F5 test.
 __device__ __forceinline__ bool tc_step(const float2* __restrict__ pull, const float2* __restrict__ test, int x, int y,
-                                        int Hs, int Ws, int Hn, int Wn, const TconsGeom& g, float s, float a1, float a2,
+                                        int Hs, int Ws, int Hn, int Wn, const NetGeom& g, float s, float a1, float a2,
                                         Bilerp& b) {
   const float2 p = make_float2(px_remap(x, g.rxn, Wn), px_remap(y, g.ryn, Hn));
-  const float2 f = sample_flow(pull, Wn, bilerp_at(p.x, p.y, Hn, Wn), s);
-  const float2 q = make_float2(__fadd_rn(p.x, f.x), __fadd_rn(p.y, f.y));
-  if (!inside_frame(q.x, q.y, Hn, Wn)) return false;
-  if (fb_inconsistent(f, sample_flow(test, Wn, bilerp_at(q.x, q.y, Hn, Wn), s), a1, a2)) return false;
+  float2 q;
+  if (chain_step(pull, test, Hn, Wn, s, a1, a2, p, q)) return false;
   b = bilerp_at(px_remap(q.x, g.rxs, Ws), px_remap(q.y, g.rys, Hs), Hs, Ws);
   return true;
-}
-
-__device__ __forceinline__ float tc_sample(const uint8_t* __restrict__ img, int Ws, const Bilerp& b, int ch) {
-  const size_t r0 = (size_t)b.y0 * Ws, r1 = (size_t)b.y1 * Ws;
-  return bilerp1(b, (float)img[(r0 + b.x0) * 3 + ch], (float)img[(r0 + b.x1) * 3 + ch], (float)img[(r1 + b.x0) * 3 + ch],
-                 (float)img[(r1 + b.x1) * 3 + ch]);
 }
 
 // ---- F29 ----
 __global__ void __launch_bounds__(kTconsThreads) tcons_terms_kernel(
     const uint8_t* __restrict__ It, const uint8_t* __restrict__ Ip, const uint8_t* __restrict__ Pt,
     const uint8_t* __restrict__ Op, const float2* __restrict__ fw, const float2* __restrict__ bw, int Hs, int Ws,
-    int Hn, int Wn, TconsGeom g, float s, float a1, float a2, float lam, float* __restrict__ c,
+    int Hn, int Wn, NetGeom g, float s, float a1, float a2, float lam, float* __restrict__ c,
     float* __restrict__ r, uint8_t* __restrict__ status) {
   const size_t ns = (size_t)Hs * Ws;
   const size_t q = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -89,7 +68,7 @@ __global__ void __launch_bounds__(kTconsThreads) tcons_terms_kernel(
     float d = 0.f;
 #pragma unroll
     for (int ch = 0; ch < 3; ++ch) {
-      const float e = __fsub_rn((float)It[q * 3 + ch], tc_sample(Ip, Ws, b, ch));
+      const float e = __fsub_rn((float)It[q * 3 + ch], sample_rgb1(Ip, Ws, b, ch));
       d = __fadd_rn(d, __fmul_rn(e, e));
     }
     d = __fdiv_rn(d, 3.f);
@@ -100,7 +79,7 @@ __global__ void __launch_bounds__(kTconsThreads) tcons_terms_kernel(
       w = __fmul_rn(om, om);
       st = 0;
 #pragma unroll
-      for (int ch = 0; ch < 3; ++ch) ro[ch] = __fsub_rn(tc_sample(Op, Ws, b, ch), (float)Pt[q * 3 + ch]);
+      for (int ch = 0; ch < 3; ++ch) ro[ch] = __fsub_rn(sample_rgb1(Op, Ws, b, ch), (float)Pt[q * 3 + ch]);
     } else {
       st = 2;
     }
@@ -352,7 +331,7 @@ __global__ void __launch_bounds__(kTconsThreads) tc_update_p_kernel(const double
 // grid (chunks, pairs); thread t takes pixels chunk_start + k * 256 + t, k = 0..15 in order
 __global__ void __launch_bounds__(kTconsThreads) warp_error_chunk_kernel(
     const uint8_t* __restrict__ video, int Hs, int Ws, const float2* __restrict__ fw, const float2* __restrict__ bw,
-    int Hn, int Wn, TconsGeom g, float s, float a1, float a2, double* __restrict__ partials) {
+    int Hn, int Wn, NetGeom g, float s, float a1, float a2, double* __restrict__ partials) {
   __shared__ double red[kTconsThreads];
   const int k = blockIdx.y;
   const size_t ns = (size_t)Hs * Ws, nn = (size_t)Hn * Wn;
@@ -369,7 +348,7 @@ __global__ void __launch_bounds__(kTconsThreads) warp_error_chunk_kernel(
     float e = 0.f;
 #pragma unroll
     for (int ch = 0; ch < 3; ++ch) {
-      const float d = __fsub_rn((float)a[q * 3 + ch], tc_sample(b, Ws, bl, ch));
+      const float d = __fsub_rn((float)a[q * 3 + ch], sample_rgb1(b, Ws, bl, ch));
       e = __fadd_rn(e, __fmul_rn(d, d));
     }
     sum = __dadd_rn(sum, (double)e);
@@ -517,7 +496,7 @@ extern "C" int rb_tcons_terms(const uint8_t* frame, const uint8_t* prev_frame, c
   const size_t ns = (size_t)Hs * Ws;
   tcons_terms_kernel<<<tc_blocks(ns), kTconsThreads, 0, (cudaStream_t)stream>>>(
       frame, prev_frame, processed, prev_out, reinterpret_cast<const float2*>(flow_fw),
-      reinterpret_cast<const float2*>(flow_bw), Hs, Ws, Hn, Wn, tcons_geom(Hs, Ws, Hn, Wn), flow_scale, alpha1, alpha2,
+      reinterpret_cast<const float2*>(flow_bw), Hs, Ws, Hn, Wn, net_geom(Hs, Ws, Hn, Wn), flow_scale, alpha1, alpha2,
       strength, c, r, status);
   RB_CHECK_LAUNCH("tcons_terms_kernel");
   return RB_OK;
@@ -608,7 +587,7 @@ extern "C" int rb_warp_error(const uint8_t* video, int F, int Hs, int Ws, const 
   double* part = (double*)workspace;
   warp_error_chunk_kernel<<<dim3((unsigned)chunks, (unsigned)(F - 1)), kTconsThreads, 0, st>>>(
       video, Hs, Ws, reinterpret_cast<const float2*>(flow_fw), reinterpret_cast<const float2*>(flow_bw), Hn, Wn,
-      tcons_geom(Hs, Ws, Hn, Wn), flow_scale, alpha1, alpha2, part);
+      net_geom(Hs, Ws, Hn, Wn), flow_scale, alpha1, alpha2, part);
   warp_error_pair_kernel<<<F - 1, kTconsThreads, 0, st>>>(part, (int)chunks, sums);
   RB_CHECK_LAUNCH("warp_error_kernels");
   return RB_OK;

@@ -36,21 +36,10 @@ __global__ void __launch_bounds__(128) track_points_kernel(const float2* __restr
       st = 0;
     } else if (j > 0 && st <= 1) {  // step j-1 -> j; status 2 (and a carried 3) stay as they are
       const size_t k = (size_t)(j - 1) * npix;
-      if (!inside_frame(p.x, p.y, H, W)) {  // only a query position outside the frame gets here
-        p = make_float2(nan, nan);
-        st = 2;
-      } else {
-        const float2 f = sample_flow(flow_fw + k, W, bilerp_at(p.x, p.y, H, W), s);
-        const float2 q = make_float2(__fadd_rn(p.x, f.x), __fadd_rn(p.y, f.y));
-        if (!inside_frame(q.x, q.y, H, W)) {
-          p = make_float2(nan, nan);
-          st = 2;
-        } else {
-          const float2 b = sample_flow(flow_bw + k, W, bilerp_at(q.x, q.y, H, W), s);
-          st = fb_inconsistent(f, b, a1, a2);
-          p = q;
-        }
-      }
+      float2 q;
+      // only a query position outside the frame fails the first test
+      st = inside_frame(p.x, p.y, H, W) ? chain_step(flow_fw + k, flow_bw + k, H, W, s, a1, a2, p, q) : 2;
+      p = st == 2 ? make_float2(nan, nan) : q;
     }
     tracks[(size_t)j * N + i] = p;
     status[(size_t)j * N + i] = st;
@@ -85,21 +74,10 @@ __global__ void __launch_bounds__(128) track_points_backward_kernel(
       st = 0;
     } else if (j < n_steps && st <= 1) {  // step j+1 -> j; status 2 (and a carried 3) stay as they are
       const size_t k = (size_t)j * npix;
-      if (!inside_frame(p.x, p.y, H, W)) {  // only a query position outside the frame gets here
-        p = make_float2(nan, nan);
-        st = 2;
-      } else {
-        const float2 f = sample_flow(flow_bw + k, W, bilerp_at(p.x, p.y, H, W), s);
-        const float2 q = make_float2(__fadd_rn(p.x, f.x), __fadd_rn(p.y, f.y));
-        if (!inside_frame(q.x, q.y, H, W)) {
-          p = make_float2(nan, nan);
-          st = 2;
-        } else {
-          const float2 b = sample_flow(flow_fw + k, W, bilerp_at(q.x, q.y, H, W), s);
-          st = fb_inconsistent(f, b, a1, a2);
-          p = q;
-        }
-      }
+      float2 q;
+      // only a query position outside the frame fails the first test
+      st = inside_frame(p.x, p.y, H, W) ? chain_step(flow_bw + k, flow_fw + k, H, W, s, a1, a2, p, q) : 2;
+      p = st == 2 ? make_float2(nan, nan) : q;
     }
     tracks[(size_t)j * N + i] = p;
     status[(size_t)j * N + i] = st;

@@ -797,14 +797,7 @@ def inpaint_propagate(frames, hole, flow_fw, flow_bw, rows, flow_scale=1.0, alph
     if T != F - 1 or flow_fw.device != dev:
         raise ValueError(f"inpaint_propagate: {F} frames need [F-1,Hn,Wn,2] = [{F - 1},Hn,Wn,2] flows on {dev} (got "
                          f"{tuple(flow_fw.shape)})")
-    table = torch.as_tensor(rows).cpu()
-    if not (table.dim() == 2 and table.shape[0] >= 1 and table.shape[1] == 3 and not table.is_floating_point()
-            and not table.is_complex()):
-        raise ValueError(f"inpaint_propagate: rows must be an [n,3] integer table (got {list(table.shape)} {table.dtype})")
-    t, nf, nb = table.to(torch.int64).unbind(1)
-    if not (((t >= 0) & (t < F) & (nf >= 0) & (t + nf <= F - 1) & (nb >= 0) & (nb <= t)).all()):
-        raise ValueError(f"inpaint_propagate: each row (t, nf, nb) needs t in [0, {F}), 0 <= nf <= F-1-t and 0 <= nb <= t")
-    table = table.to(device=dev, dtype=torch.int32).contiguous()
+    table = _rows_table("inpaint_propagate", rows, F, dev)
     n = table.shape[0]
     f, h, fw, bw = frames.contiguous(), hole.contiguous(), flow_fw.contiguous(), flow_bw.contiguous()
     colour = torch.empty(n, Hs, Ws, 3, dtype=torch.float32, device=dev)
